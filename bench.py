@@ -3,20 +3,22 @@
 batches of the BASELINE.json configurations.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
-                    [--config c2|c3|c4|c5|c2small|c3small|c4small] [--dist uniform|zipf]
+                    [--config c2|c3|c4|c5|c2small|c3small|c4small] [--dist uniform|zipf] [--dump-outputs DIR]
 
 Default = BASELINE.json configs[1] (C2: DeepFM, 26 tables x 1M rows, emb_dim 32, batch 65536 per GPU); c3 =
 xDeepFM / CIN (128,128), emb_dim 16, batch 32768; c4 = DIN, 100k items, T=50, emb_dim 64, batch 8192; c5 =
-DeepFM, 26 x 100M-row tables row-sharded over 8 GPUs (12.5M rows per table per GPU at any world size),
-emb_dim 128, batch 32768 per GPU.
+DeepFM, 26 tables row-sharded over the GPUs (4M rows per table per GPU at any world size: 53 GB of tables per
+80 GB GPU), emb_dim 128, batch 32768 per GPU.
 
 Prints ONE JSON line (see the task contract): `value` = device-timed whole-job samples/s with the batch
 already resident in HBM; `e2e` = the same step through the public API (`Model.fit(host arrays)`) including the
 pinned-H2D copy of the inputs and the D2H read of the loss; `roofline` = the dominant kernel group against the
 measured peaks in MEASURED_PEAKS.json (ALGORITHMIC bytes / flops of SURVEY.md section 8(d) over CUDA-event
 time); `cpu_baseline` = the CPU oracle (torch-CPU restatement of the reference math) on a bounded sample.
-`--impl reference` times the reference's CPU path: real TensorFlow + /root/reference's deepctr if importable
-(it is not in this image), else the oracle port - on the SAME config, steps and warm-up.
+`--impl reference` times the reference's CPU path: real TensorFlow + the reference's deepctr package if importable,
+else the oracle port - on the SAME config, steps and warm-up.
+`--dump-outputs DIR` writes what the last timed step computed (see dump_outputs) as .npy files; the inputs and the
+initial weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -49,10 +51,10 @@ CONFIGS = {
                vocab=100001, dim=64, maxlen=50, batch=8192, hidden=HID, att=(80, 40), n_sparse=2, n_dense=1),
     "c4small": dict(kind="din", workload="DIN (small): 5k items, seq_len=50, emb_dim=64, batch=1024",
                     vocab=5001, dim=64, maxlen=50, batch=1024, hidden=HID, att=(80, 40), n_sparse=2, n_dense=1),
-    # BASELINE.json configs[4]: V = 100M rows per table over 8 GPUs = 12.5M rows per table per GPU (weak)
-    "c5": dict(kind="deepfm", workload="DeepFM synthetic Criteo: 26 tables x 100M rows row-sharded over 8 GPUs "
-                                       "(12.5M rows per table per GPU), emb_dim=128, batch=32768 per GPU, 13 dense",
-               n_sparse=26, n_dense=13, vocab_per_gpu=12500000, dim=128, batch=32768, hidden=HID),
+    # BASELINE.json configs[4]: 4M rows per table per GPU (weak scaling): 26 x 4M x 128 x 4 B = 53 GB of an 80 GB H100
+    "c5": dict(kind="deepfm", workload="DeepFM synthetic Criteo: 26 tables x 4M rows per GPU, row-sharded, "
+                                       "emb_dim=128, batch=32768 per GPU, 13 dense",
+               n_sparse=26, n_dense=13, vocab_per_gpu=4000000, dim=128, batch=32768, hidden=HID),
     "c5small": dict(kind="deepfm", workload="C5-shaped (small): 26 tables x 200k rows per GPU, emb_dim=128, batch=8192 per GPU",
                     n_sparse=26, n_dense=13, vocab_per_gpu=200000, dim=128, batch=8192, hidden=HID),
 }
@@ -83,6 +85,18 @@ def feature_columns(cfg, FC=None):
     cols = [FC.SparseFeat("C%d" % (i + 1), cfg["vocab"], cfg["dim"]) for i in range(cfg["n_sparse"])]
     cols += [FC.DenseFeat("I%d" % (i + 1), 1) for i in range(cfg["n_dense"])]
     return cols
+
+
+def seed_initializers(model, seed=2020):
+    """Keras semantics leave some initializers unseeded (a fresh seed from the OS on every run, e.g. the final Dense
+    kernel of DeepFM); give each of them a seed derived from its weight's name, so that every run of the benchmark
+    starts from the same weights."""
+    import copy
+    import zlib
+    for w in model.weights:
+        if w.data is None and w.host_value is None and getattr(w.initializer, "seed", 0) is None:
+            w.initializer = copy.copy(w.initializer)
+            w.initializer.seed = (seed + zlib.crc32(w.name.encode())) & 0x7FFFFFFF
 
 
 def build_model(cfg, M=None, act=None):
@@ -191,7 +205,7 @@ def algorithmic(cfg):
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -229,7 +243,8 @@ def measured_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "which": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "which": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s - ceilings, not measurements
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "which": "H100 SXM data sheet"}
 
 
 def timed_alone(fn, reps=5, flush=None):
@@ -441,16 +456,16 @@ def run_cpu(cfg, steps, warmup, batch, dist):
 
 
 def run_tensorflow(cfg, steps, warmup, batch, dist):
-    """The real thing, when it can be imported: TensorFlow + the UNMODIFIED reference package (baseline/_ref or
-    /root/reference) - model.train_on_batch on the same synthetic batches, SGD, l2 = 0, all host cores.
-    Returns None when TensorFlow / the reference cannot be imported (this image: always)."""
+    """The real thing, when it can be imported: TensorFlow + the UNMODIFIED reference package (installed, or
+    under baseline/_ref) - model.train_on_batch on the same synthetic batches, SGD, l2 = 0, all host cores.
+    Returns None when TensorFlow / the reference cannot be imported."""
     try:
         import tensorflow as tf                                   # noqa: F401
     except Exception:
         return None
-    for p in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
-        if os.path.isdir(os.path.join(p, "deepctr")) and p not in sys.path:
-            sys.path.insert(0, p)
+    p = os.path.join(ROOT, "baseline", "_ref")
+    if os.path.isdir(os.path.join(p, "deepctr")) and p not in sys.path:
+        sys.path.insert(0, p)
     try:
         from deepctr import models as RM, feature_column as RFC
     except Exception:
@@ -477,6 +492,33 @@ def run_tensorflow(cfg, steps, warmup, batch, dist):
 
 
 # ------------------------------------------------------------------------------------------------
+DUMP_BUDGET = 64 << 20       # bytes
+DUMP_TABLE_ROWS = 4096       # sampled rows per embedding table
+
+
+def dump_outputs(model, loss, out_dir):
+    """What a caller of the timed training step receives after its last call: the summed loss of the batch and the
+    weights the step updated, as float32 .npy files (one per weight, '/' in names replaced by '.').  Weights of at
+    most DUMP_TABLE_ROWS rows are written whole; of each larger one (the embedding tables) a fixed, seeded sample
+    of rows (the same rows in every run), so that the whole dump stays under DUMP_BUDGET."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss_sum.npy"), loss.detach().float().reshape(-1).cpu().numpy())
+    weights = [w for w in model.weights if w.data is not None]
+    tables = [w for w in weights if w.data.dim() >= 1 and w.data.shape[0] > DUMP_TABLE_ROWS]
+    dense = [w for w in weights if w not in tables]
+    left = DUMP_BUDGET - sum(w.numel() * 4 for w in dense) - 4096
+    gen = torch.Generator().manual_seed(2020)
+    for w in dense:
+        np.save(os.path.join(out_dir, w.name.replace("/", ".") + ".npy"), w.data.detach().float().cpu().numpy())
+    for w in tables:
+        t = w.data.detach()
+        row_bytes = 4 * max(1, t[0].numel())
+        rows = max(1, min(t.shape[0], DUMP_TABLE_ROWS, left // max(1, len(tables)) // row_bytes))
+        idx = torch.randint(0, t.shape[0], (rows,), generator=gen).to(t.device)
+        np.save(os.path.join(out_dir, w.name.replace("/", ".") + ".npy"), t[idx].float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -490,6 +532,8 @@ def main():
     ap.add_argument("--cpu-sample-batch", type=int, default=8192)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss and the updated weights of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -542,6 +586,7 @@ def main():
         precision = "bf16x3"
     ops.set_gemm_precision(precision)
     model = build_model(cfg, act=args.din_act)
+    seed_initializers(model)
     model.compile(SGD(LR), "binary_crossentropy", embedding_update="sparse")
     host = synth_batches(cfg, N_BATCHES, rank, args.dist)
     dev = torch.device("cuda", local_rank)
@@ -570,10 +615,13 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     e0.record()
+    loss = None
     for i in range(args.steps):
-        model.train_step(*dev_batches[(warmup_done + i) % N_BATCHES])
+        loss = model.train_step(*dev_batches[(warmup_done + i) % N_BATCHES])
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0 and loss is not None:
+        dump_outputs(model, loss, args.dump_outputs)
     launches = L.launch_count() + model.replayed_launches
     graph_replays = args.steps if model._step_graphs else 0
     sampler.stop_flag = True
@@ -710,7 +758,7 @@ def main():
     if gemm_times:
         flops = sum(2.0 * m * n * k for _, m, n, k, _ in gemm_times)
         us = sum(t for *_, t in gemm_times)
-        roof_gemm = tensor_roof("gemm_planes_ws_kernel (tcgen05 cta_group::2, split-bf16)" if precision == "bf16x3"
+        roof_gemm = tensor_roof("gemm_planes_ws_kernel (wgmma, split-bf16)" if precision == "bf16x3"
                                 else "sgemm_kernel (fp32 FFMA)", flops, us, len(gemm_times),
                                 "achieved = 2*M*N*K algorithmic flops / CUDA-event launch time; bf16x3 issues 3 bf16 MMAs "
                                 "per fp32 product, so frac <= 1/3 and tensor_pipe_frac = 3 x frac",
@@ -759,7 +807,7 @@ def main():
                                        (world, "NVLink peer loads / red.add" if getattr(model.planner, "peer_mode", False)
                                         else "NCCL all-to-all")) if world > 1 else "1 gpu",
                        "l2_flush": "none: %d distinct batches cycle; per step the path touches %.2f GB of "
-                                   "randomly addressed table rows + activations, >> 126 MB L2" % (N_BATCHES, step_bytes)},
+                                   "randomly addressed table rows + activations, >> 50 MB L2" % (N_BATCHES, step_bytes)},
             "e2e": e2e, "gpu_launches": int(launches), "graph_replays": int(graph_replays), "clocks": sampler.summary(),
             "roofline": dominant, "roofline_gather_fwd": roof_gather, "roofline_scatter_bwd": roof_scatter,
             "roofline_gemm": roof_gemm, "roofline_group": roof_group, "kernel_ms_per_step": kernels, "shares": shares,

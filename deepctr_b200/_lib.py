@@ -183,7 +183,7 @@ _lib = None
 
 
 def build(verbose=False):
-    """Compile every CUDA source for sm_100a into deepctr_b200/libb2ctr.so (nvcc cross-compiles
+    """Compile every CUDA source for sm_90a into deepctr_b200/libb2ctr.so (nvcc cross-compiles
     without a GPU).  Called by __graft_entry__.build()."""
     r = subprocess.run(["make", "-C", CSRC, "-j8"], capture_output=True, text=True)
     if verbose or r.returncode != 0:

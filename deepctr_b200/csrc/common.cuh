@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for libb2ctr (sm_100a only).
+// common.cuh — shared helpers for libb2ctr (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -31,7 +31,7 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_
     b2ctr::count_launch();                                                            \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // Device counter of embedding ids outside [0, vocabulary_size) seen by the gather / scatter kernels of the
 // current device (one per device, allocated on first use, never freed).  Out-of-range ids read a ZERO row and
@@ -85,7 +85,7 @@ __device__ __forceinline__ void red_add_f1(float* p, float v) {
 }
 
 // ---- L2 eviction-priority variants (createpolicy + .L2::cache_hint).  Used by the embedding kernels:
-// the 26 dim-1 linear tables (104 MB at C2) fit in the 126 MB L2 and are marked evict_last, while the
+// the 26 dim-1 linear tables (104 MB at C2, twice the 50 MB L2) are marked evict_last, while the
 // once-touched streams (embedding rows, activations, gradients) are marked evict_first.
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   uint64_t p;

@@ -1,4 +1,4 @@
-// embed.cu — fused multi-table embedding gather / scatter-update for sm_100a.
+// embed.cu — fused multi-table embedding gather / scatter-update for sm_90a.
 //
 // Reference semantics restated here (never copied): deepctr/inputs.py:101-158 (lookup + pooling
 // dispatch), deepctr/layers/sequence.py:76-106 (SequencePoolingLayer), :155-183
@@ -9,7 +9,7 @@
 //   * 128-bit row accesses, rows never staged through L1 (ld.global.nc.L1::no_allocate);
 //   * every lane keeps up to 8 independent 16 B loads in flight (Little's law at 6.5 TB/s);
 //   * row updates are REDG.E.ADD.F32x4 (the add executes in the L2 slice, no read by the SM);
-//   * grids are whole multiples of 148 SMs.
+//   * grids are whole multiples of the 132 SMs.
 #include <stdlib.h>
 #include <cuda_bf16.h>
 #include "common.cuh"

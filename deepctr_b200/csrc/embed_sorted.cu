@@ -1,4 +1,4 @@
-// embed_sorted.cu — DETERMINISTIC fused embedding update of the Criteo-shaped fast path (sm_100a).
+// embed_sorted.cu — DETERMINISTIC fused embedding update of the Criteo-shaped fast path (sm_90a).
 //
 // north_star asks for bit-exact segment sums; SURVEY.md section 7: "backward duplicate-index accumulation needs a
 // sort + ordered segmented reduce, not float atomics".  b2ctr_embed_scatter_uniform_bwd (embed.cu) combines the

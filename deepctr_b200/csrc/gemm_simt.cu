@@ -1,7 +1,7 @@
 // gemm_simt.cu — exact-fp32 GEMM on the FFMA pipe with fused bias/activation epilogue.
 //
 // This is the B2CTR_GEMM_FP32 precision mode: bit-for-bit fp32 products and fp32 accumulation,
-// used for parity runs and as the checker of the tcgen05 split-bf16 path (gemm_tc.cu).
+// used for parity runs and as the checker of the wgmma split-bf16 path (gemm_tc.cu).
 // Replaces tf.tensordot/tf.matmul of deepctr/layers/core.py:193-195 (DNN), deepctr/layers/core.py:106
 // (LocalActivationUnit), deepctr/layers/interaction.py:414-418 (CrossNet), :754-757 (InteractingLayer).
 #include "common.cuh"

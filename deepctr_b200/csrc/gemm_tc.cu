@@ -1,22 +1,19 @@
-// gemm_tc.cu — fp32-in / fp32-out GEMM on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a.
+// gemm_tc.cu — fp32-in / fp32-out GEMM on the Hopper tensor cores (wgmma, sm_90a).
 //
-// Precision mode B2CTR_GEMM_BF16X3: every fp32 operand x is split on the fly into two bf16 values
+// Precision mode B2CTR_GEMM_BF16X3: every fp32 operand x is split into two bf16 values
 //   x = hi + lo,  hi = bf16(x),  lo = bf16(x - hi)           (|x - hi - lo| <= 2^-17 |x|)
-// and the product is accumulated in fp32 TMEM as  hi*hi + hi*lo + lo*hi  (the dropped lo*lo term is
-// <= 2^-16 relative), i.e. three kind::f16 UMMAs per K-step.  That keeps the reference's fp32 logits
-// within the 1e-4 bar (north_star) at ~1/3 of the bf16 tensor throughput instead of the FFMA pipe.
+// and the product is accumulated in fp32 registers as  hi*hi + hi*lo + lo*hi  (the dropped lo*lo term is
+// <= 2^-16 relative), i.e. three bf16 wgmma per K-step.  That keeps the reference's fp32 logits within the
+// 1e-4 bar at ~1/3 of the bf16 tensor throughput instead of the FFMA pipe.
 //
-// Kernel anatomy (one 128 x BN output tile per CTA, K split over gridDim.z):
-//   warps 0-7  : producers. Read the fp32 operand tiles straight from global memory with coalesced
-//                loads in whatever layout they are stored (row- or column-major: each thread gathers
-//                8 consecutive K values of one row), split them, and write the bf16 hi / lo planes into
-//                shared memory in the canonical K-major SWIZZLE_128B UMMA layout (16 B chunk index
-//                XOR row%8).  fence.proxy.async + mbarrier hand the stage to the MMA warp.
-//                After the main loop the same warps run the epilogue: tcgen05.ld the accumulator,
-//                alpha / bias / activation / accumulate, store fp32 C.
-//   warp 8     : one elected lane issues tcgen05.mma (SS form, cta_group::1, M=128, N=BN, K=16) x 4 K-steps
-//                x 3 split terms per stage, then tcgen05.commit to release the stage / publish the tile.
-// Stages: kStages x (A hi+lo 32 KB + B hi+lo BN*256 B).  TMEM: BN fp32 columns x 128 lanes.
+// Every kernel computes 128 x BN output tiles.  Operand tiles sit in shared memory as bf16 hi / lo planes in the
+// 128-byte-swizzled layouts wgmma reads through matrix descriptors (K-major: 16-byte chunk index XOR row % 8;
+// MN-major: 64-element atoms of 64 k-rows).  Two consumer warpgroups each own 64 rows of the tile and issue
+// wgmma.mma_async m64nBNk16 on them; the accumulator lives in their registers and the epilogue stores it from there.
+//   variant 1: the 256 threads split the fp32 operands into the stage themselves, then multiply it
+//   variant 2/3: the split is done once per operand into planes in global memory; cp.async moves them
+//   variant 4 (default): persistent, warp-specialised: TMA / cp.async / generating producer warps fill a stage ring
+//              guarded by mbarriers while the two consumer warpgroups multiply and run the epilogue
 #include <cuda.h>          // CUtensorMap + enums only: the encoder is resolved through the runtime (no libcuda link)
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -24,10 +21,9 @@
 
 namespace b2ctr {
 
-constexpr int kTM = 128;       // UMMA M (rows of the output tile, TMEM lanes)
+constexpr int kTM = 128;       // rows of the output tile: two warpgroups x 64
 constexpr int kTK = 64;        // K elements per stage = one 128-byte swizzle atom of bf16
-constexpr int kProducerWarps = 8;
-constexpr int kTcThreads = (kProducerWarps + 1) * 32;
+constexpr int kTcThreads = 256;   // variants 1-3: two warpgroups that both fill and multiply every stage
 
 struct TcArgs {
   const float* a; const float* b; float* c; const float* bias; float* ws;
@@ -62,41 +58,160 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
+// ---- warpgroup MMA (wgmma.mma_async, sm_90a) ----------------------------------------------------------------
+// Shared-memory matrix descriptor with 128-byte swizzle: start address >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 |
+// layout SWIZZLE_128B (1) << 62.
+//   K-major : rows of 128 B (64 bf16 along K), groups of 8 rows 1024 B apart (SBO); LBO unused (1).
+//   MN-major: 64-element atoms along M/N 8192 B apart (LBO), groups of 8 k-rows 1024 B apart (SBO).
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, int mn) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(mn ? 512 : 1) << 16) | (64ull << 32) | (1ull << 62);
+}
+// one K-step = 16 bf16 along K: 32 B inside the swizzled row (K-major) or 16 k-rows = 2048 B (MN-major)
+__device__ __forceinline__ uint64_t wgmma_desc_k(uint32_t base, int ks, int mn) {
+  return wgmma_desc(mn ? base + ks * 2048 : base + ks * 32, mn);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-//   start address >> 4 | LBO (ignored for swizzled K-major, set to 1) << 16 | SBO = 1024 B >> 4 << 32 |
-//   version 1 << 46 | layout SWIZZLE_128B (2) << 61
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// m64nNk16, D (fp32, registers) += A (bf16, smem) * B (bf16, smem); TA / TB: 1 = operand stored MN-major
+template <int N> struct Wgmma;
+template <> struct Wgmma<32> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
+  }
+};
+template <> struct Wgmma<64> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
+  }
+};
+template <> struct Wgmma<128> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
+  }
+};
+template <> struct Wgmma<256> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, %131, %132;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
+  }
+};
+// One 64-deep k-block of the split product for the 64 rows of the calling warpgroup: 4 K-steps x
+// (hi*hi + hi*lo + lo*hi), committed as one wgmma group.
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wg_kblock_t(float (&d)[BN / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
+                                            uint32_t b_lo) {
+#pragma unroll
+  for (int ks = 0; ks < kTK / 16; ++ks) {
+    const uint64_t dah = wgmma_desc_k(a_hi, ks, TA), dal = wgmma_desc_k(a_lo, ks, TA);
+    const uint64_t dbh = wgmma_desc_k(b_hi, ks, TB), dbl = wgmma_desc_k(b_lo, ks, TB);
+    Wgmma<BN>::template mma<TA, TB>(d, dah, dbh);
+    Wgmma<BN>::template mma<TA, TB>(d, dah, dbl);
+    Wgmma<BN>::template mma<TA, TB>(d, dal, dbh);
+  }
 }
-// MN-major, SWIZZLE_128B: the tile is a row of 64-element (128 B) atoms along M/N, each atom holding 64
-// k-rows of 128 B: LBO = atom stride (8192 B), SBO = stride between groups of 8 k-rows (1024 B).
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (512ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// stage at `st`: A hi / lo planes (kTM rows, a_plane bytes each), then B hi / lo (BN rows); the warpgroup `wg`
+// reads rows [64 wg, 64 wg + 64) of A, which start 8192 B into the plane in both layouts.
+template <int BN>
+__device__ __forceinline__ void wg_kblock(float (&d)[BN / 2], uint32_t st, int wg, int a_mn, int b_mn) {
+  constexpr uint32_t A_PLANE = kTM * 128, B_PLANE = BN * 128;
+  const uint32_t a_hi = st + wg * 8192, a_lo = a_hi + A_PLANE, b_hi = st + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
+  fence_acc(d);
+  wgmma_fence();
+  if (a_mn) {
+    if (b_mn) wg_kblock_t<BN, 1, 1>(d, a_hi, a_lo, b_hi, b_lo);
+    else wg_kblock_t<BN, 1, 0>(d, a_hi, a_lo, b_hi, b_lo);
+  } else {
+    if (b_mn) wg_kblock_t<BN, 0, 1>(d, a_hi, a_lo, b_hi, b_lo);
+    else wg_kblock_t<BN, 0, 0>(d, a_hi, a_lo, b_hi, b_lo);
+  }
+  wgmma_commit();
+  fence_acc(d);
 }
-__device__ __forceinline__ uint64_t umma_desc_any(uint32_t base, int ks, int mn) {
-  // one UMMA K-step = 16 bf16 along K: 32 B inside the swizzled row (K-major) or 16 k-rows = 2048 B (MN-major)
-  return mn ? umma_desc_mn(base + ks * 2048) : umma_desc(base + ks * 32);
+
+// Epilogue straight from the accumulator fragment of m64nBN: thread (warp w of the warpgroup, lane l) holds rows
+// row0 + 16w + l/4 (+ 8) and columns n0 + 8i + 2(l % 4) + {0, 1} in d[4i + {0, 1}] (and d[4i + {2, 3}] for the
+// row + 8).  Each group of four lanes writes 32 contiguous bytes of a row.  C = act(alpha acc [+ C] [+ bias]);
+// split-K slices go to the workspace instead (ws[z][m][n], reduced by tc_splitk_reduce_kernel).
+template <int BN, class G>
+__device__ __forceinline__ void store_acc(const G& g, const float (&d)[BN / 2], int64_t row0, int64_t n0, int64_t z) {
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const bool vec = (g.ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(g.c) & 7) == 0);
+  const bool vec_ws = g.n % 2 == 0;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t gm = row0 + w * 16 + (lane >> 2) + 8 * h;
+    if (gm >= g.m) continue;
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      const int64_t gn = n0 + 8 * i + 2 * (lane & 3);
+      if (gn >= g.n) continue;
+      const bool two = gn + 1 < g.n;
+      float v0 = g.alpha * d[4 * i + 2 * h], v1 = g.alpha * d[4 * i + 2 * h + 1];
+      if (g.splits > 1) {
+        float* wp = g.ws + (z * g.m + gm) * g.n + gn;
+        if (two && vec_ws) *reinterpret_cast<float2*>(wp) = make_float2(v0, v1);
+        else {
+          wp[0] = v0;
+          if (two) wp[1] = v1;
+        }
+        continue;
+      }
+      float* cp = g.c + gm * g.ldc + gn;
+      if (two && vec) {
+        if (g.accumulate) {
+          const float2 o = *reinterpret_cast<const float2*>(cp);
+          v0 += o.x; v1 += o.y;
+        }
+        if (g.bias) { v0 += __ldg(g.bias + gn); v1 += __ldg(g.bias + gn + 1); }
+        *reinterpret_cast<float2*>(cp) = make_float2(act_apply(v0, g.act), act_apply(v1, g.act));
+      } else {
+        if (g.accumulate) v0 += cp[0];
+        if (g.bias) v0 += g.bias[gn];
+        cp[0] = act_apply(v0, g.act);
+        if (two) {
+          if (g.accumulate) v1 += cp[1];
+          if (g.bias) v1 += g.bias[gn + 1];
+          cp[1] = act_apply(v1, g.act);
+        }
+      }
+    }
+  }
 }
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, N>>3 at bit 17, M>>4 at bit 24
-__device__ __forceinline__ uint32_t umma_idesc(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kTM >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
+
+__device__ __forceinline__ unsigned char* align1024(unsigned char* p) {
+  return reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~(uintptr_t)1023);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 lo, __nv_bfloat16 hi) {
@@ -138,182 +253,60 @@ __device__ __forceinline__ void produce_chunk(const float* __restrict__ base, in
   *reinterpret_cast<uint4*>(hi_tile + off) = make_uint4(h[0], h[1], h[2], h[3]);
   *reinterpret_cast<uint4*>(lo_tile + off) = make_uint4(l[0], l[1], l[2], l[3]);
 }
-
+// Variant 1: the 256 threads read the fp32 operand tiles straight from global memory with coalesced loads in
+// whatever layout they are stored (each thread gathers 8 consecutive K values of one row), split them into the
+// stage, then both warpgroups multiply it.  A stage is refilled once the wgmma group that read it has retired.
 template <int BN, int STAGES, bool A_KC, bool B_KC>
-__global__ void __launch_bounds__(kTcThreads, STAGES == 1 ? 3 : 1) gemm_bf16x3_kernel(const TcArgs g) {
+__global__ void __launch_bounds__(kTcThreads, STAGES == 1 ? 2 : 1) gemm_bf16x3_kernel(const TcArgs g) {
   constexpr int A_PLANE = kTM * 128;       // bytes of one bf16 plane of the A tile (128 rows x 64 k)
   constexpr int B_PLANE = BN * 128;
   constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* tiles = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                                          ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], accum_bar;
-  __shared__ uint32_t tmem_slot;
+  unsigned char* tiles = align1024(smem_raw);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int64_t m0 = (int64_t)blockIdx.y * kTM, n0 = (int64_t)blockIdx.x * BN;
   const int64_t kbeg = (int64_t)blockIdx.z * g.k_per_split;
   const int64_t kend = kbeg + g.k_per_split < g.k ? kbeg + g.k_per_split : g.k;
   const int nkb = kend > kbeg ? (int)((kend - kbeg + kTK - 1) / kTK) : 0;
+  const bool a_vec = A_KC && (g.sam % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.a) & 15) == 0);
+  const bool b_vec = B_KC && (g.sbn % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.b) & 15) == 0);
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], kProducerWarps);
-      mbar_init(&empty_bar[s], 1);
-    }
-    mbar_init(&accum_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == kProducerWarps) {  // the MMA warp owns the TMEM allocation
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(&tmem_slot)),
-                 "r"((uint32_t)(BN < 32 ? 32 : BN))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_slot;
-
-  if (warp < kProducerWarps) {
-    // ------------------------------- producers -------------------------------------------------
-    const bool a_vec = A_KC && (g.sam % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.a) & 15) == 0);
-    const bool b_vec = B_KC && (g.sbn % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.b) & 15) == 0);
-    const int tid = threadIdx.x;  // 0..255
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % STAGES;
-      mbar_wait(&empty_bar[s], ((kb / STAGES) & 1) ^ 1);
-      unsigned char* st = tiles + (size_t)s * STAGE;
-      const int64_t k0 = kbeg + (int64_t)kb * kTK;
-      // A tile: 128 rows x 8 chunks.  K-contiguous storage: chunk fastest (coalesced along k);
-      // otherwise row fastest (coalesced along m).
+  float d[BN / 2];
+#pragma unroll
+  for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int s = kb % STAGES;
+    unsigned char* st = tiles + (size_t)s * STAGE;
+    wgmma_wait<STAGES - 1>();          // the group that last read stage s (k-block kb - STAGES) has retired ...
+    __syncthreads();                   // ... in both warpgroups
+    const int64_t k0 = kbeg + (int64_t)kb * kTK;
+    // A tile: 128 rows x 8 chunks.  K-contiguous storage: chunk fastest (coalesced along k);
+    // otherwise row fastest (coalesced along m).
 #pragma unroll 4
-      for (int t = tid; t < kTM * 8; t += kProducerWarps * 32) {
-        const int r = A_KC ? t >> 3 : t % kTM;
-        const int c = A_KC ? t & 7 : t / kTM;
-        const int64_t kk = k0 + c * 8;
-        produce_chunk<A_KC>(g.a, g.sam, g.sak, m0 + r, g.m, kk, kend, a_vec && ((kk & 3) == 0), st,
-                            st + A_PLANE, r, c);
-      }
+    for (int t = tid; t < kTM * 8; t += kTcThreads) {
+      const int r = A_KC ? t >> 3 : t % kTM;
+      const int c = A_KC ? t & 7 : t / kTM;
+      const int64_t kk = k0 + c * 8;
+      produce_chunk<A_KC>(g.a, g.sam, g.sak, m0 + r, g.m, kk, kend, a_vec && ((kk & 3) == 0), st,
+                          st + A_PLANE, r, c);
+    }
 #pragma unroll 4
-      for (int t = tid; t < BN * 8; t += kProducerWarps * 32) {
-        const int r = B_KC ? t >> 3 : t % BN;
-        const int c = B_KC ? t & 7 : t / BN;
-        const int64_t kk = k0 + c * 8;
-        produce_chunk<B_KC>(g.b, g.sbn, g.sbk, n0 + r, g.n, kk, kend, b_vec && ((kk & 3) == 0),
-                            st + 2 * A_PLANE, st + 2 * A_PLANE + B_PLANE, r, c);
-      }
-      // make the generic-proxy writes visible to the tensor core (async proxy), then signal
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&full_bar[s]);
+    for (int t = tid; t < BN * 8; t += kTcThreads) {
+      const int r = B_KC ? t >> 3 : t % BN;
+      const int c = B_KC ? t & 7 : t / BN;
+      const int64_t kk = k0 + c * 8;
+      produce_chunk<B_KC>(g.b, g.sbn, g.sbk, n0 + r, g.n, kk, kend, b_vec && ((kk & 3) == 0),
+                          st + 2 * A_PLANE, st + 2 * A_PLANE + B_PLANE, r, c);
     }
-    // ------------------------------- epilogue --------------------------------------------------
-    if (nkb > 0) {
-      mbar_wait(&accum_bar, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    const int sub = warp & 3;                 // TMEM sub-partition this warp may read
-    const int half = warp >> 2;               // which half of the BN columns
-    constexpr int HALVES = BN >= 64 ? 2 : 1;
-    constexpr int COLS = BN / HALVES;         // columns per warp
-    const int64_t gm = m0 + sub * 32 + lane;
-    const bool vec_c = (g.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.c) & 15) == 0) &&
-                       (!g.bias || (reinterpret_cast<uintptr_t>(g.bias) & 15) == 0) && g.splits == 1;
-    if (half < HALVES) {
-#pragma unroll 1
-      for (int c0 = 0; c0 < COLS; c0 += 32) {
-        uint32_t r[32];
-        if (nkb > 0) {
-          const uint32_t taddr = tmem_base + ((uint32_t)(sub * 32) << 16) + (uint32_t)(half * COLS + c0);
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-              "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-              "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-              : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-                "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-                "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-                "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-              : "r"(taddr));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) r[j] = 0u;
-        }
-        if (gm < g.m) {
-          const int64_t gn0 = n0 + half * COLS + c0;
-          if (vec_c && gn0 + 32 <= g.n) {
-            float* crow = g.c + gm * g.ldc + gn0;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float4 v = make_float4(g.alpha * __uint_as_float(r[j]), g.alpha * __uint_as_float(r[j + 1]),
-                                     g.alpha * __uint_as_float(r[j + 2]), g.alpha * __uint_as_float(r[j + 3]));
-              if (g.accumulate) {
-                const float4 o = *reinterpret_cast<const float4*>(crow + j);
-                v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
-              }
-              if (g.bias) {
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(g.bias + gn0 + j));
-                v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
-              }
-              v.x = act_apply(v.x, g.act); v.y = act_apply(v.y, g.act);
-              v.z = act_apply(v.z, g.act); v.w = act_apply(v.w, g.act);
-              *reinterpret_cast<float4*>(crow + j) = v;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int64_t gn = gn0 + j;
-              if (gn < g.n) {
-                float v = g.alpha * __uint_as_float(r[j]);
-                if (g.splits > 1) {
-                  g.ws[((int64_t)blockIdx.z * g.m + gm) * g.n + gn] = v;
-                } else {
-                  if (g.accumulate) v += g.c[gm * g.ldc + gn];
-                  if (g.bias) v += g.bias[gn];
-                  g.c[gm * g.ldc + gn] = act_apply(v, g.act);
-                }
-              }
-            }
-          }
-        }
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  } else {
-    // ------------------------------- MMA issuer ------------------------------------------------
-    const uint32_t idesc = umma_idesc(BN);
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % STAGES;
-      mbar_wait(&full_bar[s], (kb / STAGES) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE);
-        const uint32_t a_hi = sa, a_lo = sa + A_PLANE, b_hi = sa + 2 * A_PLANE,
-                       b_lo = sa + 2 * A_PLANE + B_PLANE;
-#pragma unroll
-        for (int ks = 0; ks < kTK / 16; ++ks) {
-          const uint32_t ko = ks * 32;  // 16 bf16 = 32 bytes along K inside the swizzle atom
-          umma_f16(tmem_base, umma_desc(a_hi + ko), umma_desc(b_hi + ko), idesc, (kb | ks) ? 1u : 0u);
-          umma_f16(tmem_base, umma_desc(a_hi + ko), umma_desc(b_lo + ko), idesc, 1u);
-          umma_f16(tmem_base, umma_desc(a_lo + ko), umma_desc(b_hi + ko), idesc, 1u);
-        }
-        umma_commit(&empty_bar[s]);               // frees the stage once these MMAs retire
-        if (kb == nkb - 1) umma_commit(&accum_bar);  // accumulator complete
-      }
-      __syncwarp();
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    // make the generic-proxy writes visible to the tensor core (async proxy)
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    wg_kblock<BN>(d, smem_u32(st), wg, 0, 0);
   }
-  __syncthreads();
-  if (warp == kProducerWarps) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"((uint32_t)(BN < 32 ? 32 : BN))
-                 : "memory");
-  }
+  wgmma_wait<0>();
+  fence_acc(d);
+  store_acc<BN>(g, d, m0 + wg * 64, n0, blockIdx.z);
 }
 
 __global__ void tc_splitk_reduce_kernel(const TcArgs g) {
@@ -351,10 +344,8 @@ static cudaError_t launch_tc(const TcArgs& ta, bool akc, bool bkc, cudaStream_t 
 // ================================================================================================
 // Variant 2 ("planes"): the fp32 -> (hi, lo) bf16 split is done ONCE per operand by a streaming kernel
 // into K-major planes [rows_pad, k_pad] in workspace memory; the GEMM kernel then only moves bytes:
-// 8 warps cp.async 16-byte chunks of the planes into the swizzled UMMA tiles (3-stage pipeline, no
-// register staging, no conversion instructions), 1 warp issues the same 3 UMMAs per K-step.
-// ncu on variant 1 (profiles/r1_gemm_tc_3stage.txt: tensor pipe ~7 %, warps active 14 %) showed the
-// producers, not the tensor core, bound the kernel: every CTA re-converted both operand tiles.
+// the 256 threads cp.async 16-byte chunks of the planes into the swizzled stage tiles (no register staging,
+// no conversion instructions), so no CTA re-converts an operand tile another CTA also reads.
 // ================================================================================================
 struct PlaneArgs {
   // K-major planes: [rows_pad, k_pad] (k contiguous).  MN-major planes: [k_pad, rows_pad] (row index
@@ -380,8 +371,6 @@ struct PlaneArgs {
   // FOLD epilogue (CIN backward): dT0 [rows, cin_ld0] and dXk [rows, fold_ldx], both accumulated with red.add
   float* fold_dt0; float* fold_dxk; int64_t fold_ldx;
   int gen_groups;     // generating producers: 2 = two groups of 128 threads alternate stages, 1 = all 256 share every stage
-  int debug;          // B2CTR_TC_DEBUG knock-outs (WRONG RESULTS; tools/gemm_sweep.py attributes the per-tile cost with them):
-                      // 1 = no global stores in the epilogue, 2 = no tcgen05.ld, 4 = no MMAs issued, 8 = no operand loads
 };
 
 // dst planes [rows_pad, k_pad] <- src(r, k) = p[r*sr + k*sk]; zero outside [rows, k).
@@ -450,202 +439,83 @@ __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
 
-// CTAs per SM follow from the stage footprint: a single-stage 128x128 tile (65 KB) fits three times, so
-// short-K GEMMs (dgrad of the first layer: K = 256 = 4 k-blocks) overlap one CTA's epilogue with its
-// neighbours' main loops instead of idling the SM.
+// Multi-stage cp.async ring: the copies of k-block kb + STAGES - 1 are in flight while k-block kb is multiplied.
+// CTAs per SM follow from the stage footprint: a single-stage 128x128 tile (65 KB) fits twice, so short-K GEMMs
+// (dgrad of the first layer: K = 256 = 4 k-blocks) overlap one CTA's epilogue with its neighbour's main loop.
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(kTcThreads, (STAGES * (2 * kTM * 128 + 2 * BN * 128) + 1024 <= 75 * 1024) ? 3 : 1)
+__global__ void __launch_bounds__(kTcThreads, (STAGES * (2 * kTM * 128 + 2 * BN * 128) + 1024 <= 113 * 1024) ? 2 : 1)
     gemm_planes_kernel(const PlaneArgs g) {
   constexpr int A_PLANE = kTM * 128;
   constexpr int B_PLANE = BN * 128;
   constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* tiles = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                                          ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], accum_bar;
-  __shared__ uint32_t tmem_slot;
+  unsigned char* tiles = align1024(smem_raw);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, wg = tid >> 7;
   const int64_t m0 = (int64_t)blockIdx.y * kTM, n0 = (int64_t)blockIdx.x * BN;
   const int64_t kbeg = (int64_t)blockIdx.z * g.k_per_split;
   const int64_t kend = kbeg + g.k_per_split < g.k_pad ? kbeg + g.k_per_split : g.k_pad;
   const int nkb = kend > kbeg ? (int)((kend - kbeg) / kTK) : 0;
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], kProducerWarps);
-      mbar_init(&empty_bar[s], 1);
+  auto load = [&](int kb) {
+    const uint32_t st = smem_u32(tiles + (size_t)(kb % STAGES) * STAGE);
+    const int64_t k0 = kbeg + (int64_t)kb * kTK;
+#pragma unroll
+    for (int t = tid; t < kTM * 8; t += kTcThreads) {
+      uint32_t off;
+      int64_t src;
+      if (g.a_mn) {   // chunk c of k-row kk: 8 consecutive m inside atom c/8
+        const int kk = t / (kTM / 8), c = t % (kTM / 8);
+        off = (c >> 3) * 8192 + kk * 128 + (((c & 7) ^ (kk & 7)) << 4);
+        src = (k0 + kk) * g.a_pitch + m0 + c * 8;
+      } else {
+        const int r = t >> 3, c = t & 7;
+        off = r * 128 + ((c ^ (r & 7)) << 4);
+        src = (m0 + r) * g.a_pitch + k0 + c * 8;
+      }
+      cp_async16(st + off, g.a_hi + src);
+      cp_async16(st + A_PLANE + off, g.a_lo + src);
     }
-    mbar_init(&accum_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == kProducerWarps) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(&tmem_slot)),
-                 "r"((uint32_t)(BN < 32 ? 32 : BN))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_slot;
+#pragma unroll
+    for (int t = tid; t < BN * 8; t += kTcThreads) {
+      uint32_t off;
+      int64_t src;
+      if (g.b_mn) {
+        const int kk = t / (BN / 8), c = t % (BN / 8);
+        off = (c >> 3) * 8192 + kk * 128 + (((c & 7) ^ (kk & 7)) << 4);
+        src = (k0 + kk) * g.b_pitch + n0 + c * 8;
+      } else {
+        const int r = t >> 3, c = t & 7;
+        off = r * 128 + ((c ^ (r & 7)) << 4);
+        src = (n0 + r) * g.b_pitch + k0 + c * 8;
+      }
+      cp_async16(st + 2 * A_PLANE + off, g.b_hi + src);
+      cp_async16(st + 2 * A_PLANE + B_PLANE + off, g.b_lo + src);
+    }
+  };
 
-  if (warp < kProducerWarps) {
-    const int tid = threadIdx.x;
-    // software pipeline over k-blocks: issue the copies of block `kb`, then publish block kb-(STAGES-1)
-    for (int kb = 0; kb < nkb + STAGES - 1; ++kb) {
-      if (kb < nkb) {
-        const int s = kb % STAGES;
-        mbar_wait(&empty_bar[s], ((kb / STAGES) & 1) ^ 1);
-        const uint32_t st = smem_u32(tiles + (size_t)s * STAGE);
-        const int64_t k0 = kbeg + (int64_t)kb * kTK;
+  float d[BN / 2];
 #pragma unroll
-        for (int t = tid; t < kTM * 8; t += kProducerWarps * 32) {
-          uint32_t off;
-          int64_t src;
-          if (g.a_mn) {   // chunk c of k-row kk: 8 consecutive m inside atom c/8
-            const int kk = t / (kTM / 8), c = t % (kTM / 8);
-            off = (c >> 3) * 8192 + kk * 128 + (((c & 7) ^ (kk & 7)) << 4);
-            src = (k0 + kk) * g.a_pitch + m0 + c * 8;
-          } else {
-            const int r = t >> 3, c = t & 7;
-            off = r * 128 + ((c ^ (r & 7)) << 4);
-            src = (m0 + r) * g.a_pitch + k0 + c * 8;
-          }
-          cp_async16(st + off, g.a_hi + src);
-          cp_async16(st + A_PLANE + off, g.a_lo + src);
-        }
+  for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
 #pragma unroll
-        for (int t = tid; t < BN * 8; t += kProducerWarps * 32) {
-          uint32_t off;
-          int64_t src;
-          if (g.b_mn) {
-            const int kk = t / (BN / 8), c = t % (BN / 8);
-            off = (c >> 3) * 8192 + kk * 128 + (((c & 7) ^ (kk & 7)) << 4);
-            src = (k0 + kk) * g.b_pitch + n0 + c * 8;
-          } else {
-            const int r = t >> 3, c = t & 7;
-            off = r * 128 + ((c ^ (r & 7)) << 4);
-            src = (n0 + r) * g.b_pitch + k0 + c * 8;
-          }
-          cp_async16(st + 2 * A_PLANE + off, g.b_hi + src);
-          cp_async16(st + 2 * A_PLANE + B_PLANE + off, g.b_lo + src);
-        }
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-      if (kb >= STAGES - 1) {
-        const int j = kb - (STAGES - 1);
-        asm volatile("cp.async.wait_group %0;" ::"n"(STAGES - 1) : "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&full_bar[j % STAGES]);
-      }
-    }
-    // ---- epilogue (same as variant 1) ----
-    if (nkb > 0) {
-      mbar_wait(&accum_bar, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    const int sub = warp & 3;
-    const int half = warp >> 2;
-    constexpr int HALVES = BN >= 64 ? 2 : 1;
-    constexpr int COLS = BN / HALVES;
-    const int64_t gm = m0 + sub * 32 + lane;
-    const bool vec_c = (g.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.c) & 15) == 0) &&
-                       (!g.bias || (reinterpret_cast<uintptr_t>(g.bias) & 15) == 0) && g.splits == 1;
-    if (half < HALVES) {
-#pragma unroll 1
-      for (int c0 = 0; c0 < COLS; c0 += 32) {
-        uint32_t r[32];
-        if (nkb > 0) {
-          const uint32_t taddr = tmem_base + ((uint32_t)(sub * 32) << 16) + (uint32_t)(half * COLS + c0);
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-              "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-              "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-              : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-                "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-                "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-                "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-              : "r"(taddr));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) r[j] = 0u;
-        }
-        if (gm < g.m) {
-          const int64_t gn0 = n0 + half * COLS + c0;
-          if (vec_c && gn0 + 32 <= g.n) {
-            float* crow = g.c + gm * g.ldc + gn0;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float4 v = make_float4(g.alpha * __uint_as_float(r[j]), g.alpha * __uint_as_float(r[j + 1]),
-                                     g.alpha * __uint_as_float(r[j + 2]), g.alpha * __uint_as_float(r[j + 3]));
-              if (g.accumulate) {
-                const float4 o = *reinterpret_cast<const float4*>(crow + j);
-                v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
-              }
-              if (g.bias) {
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(g.bias + gn0 + j));
-                v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
-              }
-              v.x = act_apply(v.x, g.act); v.y = act_apply(v.y, g.act);
-              v.z = act_apply(v.z, g.act); v.w = act_apply(v.w, g.act);
-              *reinterpret_cast<float4*>(crow + j) = v;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int64_t gn = gn0 + j;
-              if (gn < g.n) {
-                float v = g.alpha * __uint_as_float(r[j]);
-                if (g.splits > 1) {
-                  g.ws[((int64_t)blockIdx.z * g.m + gm) * g.n + gn] = v;
-                } else {
-                  if (g.accumulate) v += g.c[gm * g.ldc + gn];
-                  if (g.bias) v += g.bias[gn];
-                  g.c[gm * g.ldc + gn] = act_apply(v, g.act);
-                }
-              }
-            }
-          }
-        }
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  } else {
-    const uint32_t idesc = umma_idesc(BN) | (g.a_mn ? (1u << 15) : 0u) | (g.b_mn ? (1u << 16) : 0u);
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % STAGES;
-      mbar_wait(&full_bar[s], (kb / STAGES) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE);
-        const uint32_t a_hi = sa, a_lo = sa + A_PLANE, b_hi = sa + 2 * A_PLANE, b_lo = sa + 2 * A_PLANE + B_PLANE;
-#pragma unroll
-        for (int ks = 0; ks < kTK / 16; ++ks) {
-          const uint64_t dah = umma_desc_any(a_hi, ks, g.a_mn), dal = umma_desc_any(a_lo, ks, g.a_mn);
-          const uint64_t dbh = umma_desc_any(b_hi, ks, g.b_mn), dbl = umma_desc_any(b_lo, ks, g.b_mn);
-          umma_f16(tmem_base, dah, dbh, idesc, (kb | ks) ? 1u : 0u);
-          umma_f16(tmem_base, dah, dbl, idesc, 1u);
-          umma_f16(tmem_base, dal, dbh, idesc, 1u);
-        }
-        umma_commit(&empty_bar[s]);
-        if (kb == nkb - 1) umma_commit(&accum_bar);
-      }
-      __syncwarp();
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  for (int s = 0; s < STAGES - 1; ++s) {
+    if (s < nkb) load(s);
+    asm volatile("cp.async.commit_group;" ::: "memory");
   }
-  __syncthreads();
-  if (warp == kProducerWarps) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"((uint32_t)(BN < 32 ? 32 : BN))
-                 : "memory");
+  for (int kb = 0; kb < nkb; ++kb) {
+    // the slot of k-block kb + STAGES - 1 was last read by k-block kb - 1, retired below
+    if (kb + STAGES - 1 < nkb) load(kb + STAGES - 1);
+    asm volatile("cp.async.commit_group;" ::: "memory");
+    asm volatile("cp.async.wait_group %0;" ::"n"(STAGES - 1) : "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    wg_kblock<BN>(d, smem_u32(tiles + (size_t)(kb % STAGES) * STAGE), wg, g.a_mn, g.b_mn);
+    wgmma_wait<0>();
+    __syncthreads();
   }
+  asm volatile("cp.async.wait_all;" ::: "memory");
+  fence_acc(d);
+  store_acc<BN>(g, d, m0 + wg * 64, n0, blockIdx.z);
 }
 
 template <int BN, int STAGES>
@@ -661,104 +531,31 @@ static cudaError_t launch_planes(const PlaneArgs& pa, cudaStream_t st) {
 
 
 // ================================================================================================
-// Variant 4: persistent, warp-specialised, optionally CTA-PAIRED (tcgen05 cta_group::2) planes GEMM.
-//
-// The split-bf16 scheme moves 2x the operand bytes of a plain bf16 GEMM for 3x its MMAs, so operand
-// delivery (L2 -> shared memory), not the tensor pipe, is what a 128x256 single-CTA tile runs out of
-// (96 KB per 64-deep k-block per SM, ~11 TB/s over 148 SMs).  A CTA pair computes a 256 x BN tile with
-// each CTA staging its own 128 rows of A and only HALF of the B tile (the pair's tensor cores read both
-// halves), i.e. 64 KB per k-block per SM at BN = 256 - which also leaves room for a 3-deep pipeline.
-//   warps 0-7  : epilogue (TMEM -> registers -> 32x32 transposition through a swizzled staging block -> global,
-//                128 contiguous bytes per row); warp & 3 = TMEM sub-partition, warp >> 2 = column half
+// Variant 4: persistent, warp-specialised planes GEMM.
+//   warps 0-7  : two consumer warpgroups.  Each waits for a full stage, issues the 12 wgmma of the k-block on
+//                its 64 rows of the tile, keeps one wgmma group in flight and hands the previous stage back to
+//                the producers; after the last k-block of a tile it runs the epilogue from its registers.
 //   producers  : TMA (default): one elected thread arms the stage barrier and issues cp.async.bulk.tensor.2d loads
-//                of the four plane slices; in a CTA pair both CTAs' loads complete on the LEADER's barrier
-//                (.cta_group::2).  GEN = 1 / 2: eight warps GENERATE the A tile in shared memory (CIN outer product /
-//                DIN attention input) while B arrives by TMA.  B2CTR_TC_TMA=0: four warps of 16-byte cp.async.
-//   last warp  : TMEM allocation; lane 0 of the LEADER CTA issues every tcgen05.mma of the pair
-// TMEM holds two BN-column accumulators: the epilogue of tile i overlaps the main loop of tile i+1.
-// Measured anatomy of a k-block (tools/gemm_sweep.py, B2CTR_TC_DEBUG knock-outs): the stage round trip alone
-// (commit -> empty -> producer -> full -> issuer, nothing loaded or multiplied) costs 0.25 us per k-block over 4 stages.
-// Persistent: grid = min(#tiles, #SMs / NCTA) clusters; tile = cluster id + j * #clusters, N-tile fastest
-// (neighbouring clusters share the A rows through L2).
+//                of the four plane slices.  GEN = 1 / 2: eight warps GENERATE the A tile in shared memory (CIN outer
+//                product / DIN attention input) while B arrives by TMA.  B2CTR_TC_TMA=0: four warps of 16-byte
+//                cp.async.
+// The producers run up to STAGES k-blocks ahead, across tile boundaries: the next tile's operands load while the
+// consumers run the epilogue of the current one.
+// Persistent: grid = min(#tiles, #SMs); tile = CTA id + j * #CTAs, N-tile fastest (neighbouring CTAs share the
+// A rows through L2).  BN <= 128: the m64n128 accumulator is 64 registers per consumer thread.
 // ================================================================================================
-constexpr int kWsEpilogueWarps = 8;
+constexpr int kWsConsumerWarps = 8;
 constexpr int kWsProducers = 4;   // warps
 
 struct WsArgs {
   PlaneArgs p;
-  int tiles_m, tiles_n;   // cluster tiles
+  int tiles_m, tiles_n;
   int64_t ntiles;
 };
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster.  Default (.release.cta)
-// semantics on purpose: a cluster-scope release drains every outstanding cp.async of the warp first, which
-// serialises the stage ring (measured: the peer CTA's producers spent >50% of their time in that arrive); the
-// data being published has already landed (cp.async.wait_group) and been proxy-fenced by the caller.
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-template <int NCTA>
-__device__ __forceinline__ void umma_f16_ws(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc,
-                                            uint32_t accumulate) {
-  if constexpr (NCTA == 1) {
-    umma_f16(tmem_d, da, db, idesc, accumulate);
-  } else {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-template <int NCTA>
-__device__ __forceinline__ void umma_commit_ws(uint64_t* bar) {
-  if constexpr (NCTA == 1) {
-    umma_commit(bar);
-  } else {   // arrives on `bar` in BOTH CTAs of the pair once the MMAs issued so far have completed
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"((uint16_t)3)
-        : "memory");
-  }
-}
-
 // ---- TMA (cp.async.bulk.tensor) producer primitives --------------------------------------------------
 // One elected thread arms the stage's mbarrier with the bytes that will land (expect_tx) and issues the
 // tiled bulk copies; the hardware writes the 128-byte-swizzled rows itself (CU_TENSOR_MAP_SWIZZLE_128B is
-// exactly the `chunk ^ (row & 7)` layout the UMMA descriptors above expect) and completes the barrier.
+// exactly the `chunk ^ (row & 7)` layout the wgmma descriptors above expect) and completes the barrier.
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -767,19 +564,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
       "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
       : "memory");
-}
-// CTA pair: the load issued by either CTA of the pair signals the LEADER's mbarrier (shared::cluster address `bar`),
-// so the MMA issuer waits on one barrier per stage and no warp has to relay "the peer's half has landed".
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, int32_t c0, int32_t c1, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
-      "l"(map), "r"(c0), "r"(c1), "r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(cta));
-  return r;
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
@@ -946,81 +730,51 @@ __device__ __forceinline__ void att_emit_half(const PlaneArgs& g, GenRegs& io, i
   if (reload) io.ok = okn;
 }
 
-
 // generated-operand kernels run 8 producer warps (two threads per generated row), the others 4
 template <bool GENERATED>
 struct WsLayout {
   static constexpr int kProducers = GENERATED ? 8 : kWsProducers;
-  static constexpr int kMmaWarp = kWsEpilogueWarps + kProducers;
-  static constexpr int kThreads = (kMmaWarp + 1) * 32;
+  static constexpr int kThreads = (kWsConsumerWarps + kProducers) * 32;
 };
 
 // GEN: 0 = both operands from memory; 1 = A generated as the CIN outer product; 2 = A generated as the DIN
 // attention input (one instantiation per generator: the code of the other one would only fill the instruction cache)
-template <int BN, int STAGES, int NCTA, bool TMA, int GEN = 0, bool FOLD = false>
+template <int BN, int STAGES, bool TMA, int GEN = 0, bool FOLD = false>
 __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     gemm_planes_ws_kernel(const __grid_constant__ WsArgs w, const __grid_constant__ CUtensorMap tm_ah,
                           const __grid_constant__ CUtensorMap tm_al, const __grid_constant__ CUtensorMap tm_bh,
                           const __grid_constant__ CUtensorMap tm_bl) {
+  static_assert(BN <= 128, "the consumer accumulator is BN / 2 registers per thread");
   const PlaneArgs& g = w.p;
-  constexpr int BNH = BN / NCTA;             // rows of the B tile staged by one CTA
   constexpr int A_PLANE = kTM * 128;
-  constexpr int B_PLANE = BNH * 128;
+  constexpr int B_PLANE = BN * 128;
   constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
-  constexpr uint32_t TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* tiles = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                                          ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t full_bar[STAGES], peer_full[STAGES], empty_bar[STAGES], acc_full[2], acc_empty[2];
-  __shared__ uint32_t tmem_slot;
-  unsigned char* epi_stage = tiles + (size_t)STAGES * STAGE;      // 8 epilogue warps x 4 KB (not in FOLD kernels)
+  unsigned char* tiles = align1024(smem_raw);
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t cta_rank = NCTA == 1 ? 0u : cluster_ctarank();
-  const int64_t cluster_id = blockIdx.x / NCTA, nclusters = gridDim.x / NCTA;
+  const int64_t cta0 = blockIdx.x, nctas = gridDim.x;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      // cp.async producers: one deferred arrival per producer thread of THIS CTA; TMA: one arrive.expect_tx
-      // CIN: the B planes arrive by TMA (1 arrive.expect_tx) + one arrival per generating thread
-      // generated A: one group of 128 threads per stage + the TMA expect_tx of the B planes
+      // cp.async producers: one deferred arrival per producer thread; TMA: one arrive.expect_tx
+      // generated A: one arrival per generating thread of the stage + the TMA expect_tx of the B planes
       mbar_init(&full_bar[s], GEN != 0 ? 1 + (g.gen_groups == 2 ? 128 : 256) : (TMA ? 1 : kWsProducers * 32));
-      mbar_init(&peer_full[s], 1);                    // leader only: the peer CTA's half of the stage landed
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&acc_full[a], 1);
-      mbar_init(&acc_empty[a], kWsEpilogueWarps * NCTA);   // used on the leader only
+      mbar_init(&empty_bar[s], kWsConsumerWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == WsLayout<GEN != 0>::kMmaWarp) {
-    if constexpr (NCTA == 1) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                   "r"(TMEM_COLS)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                   "r"(TMEM_COLS)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if constexpr (NCTA > 1) cluster_sync_all();      // peer barriers initialised before any remote arrive
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_slot;
 
   // tile -> coordinates (N tile fastest, then M, then the split-K slice)
   auto decode = [&](int64_t tile, int64_t& mt, int64_t& nt, int64_t& kbeg, int& nkb) {
     if constexpr (FOLD) {
-      // a cluster owns whole ROW BLOCKS and walks all their N tiles in turn (its epilogue accumulates across
-      // them): work item j of cluster c is (row block c + (j / tiles_n) * nclusters, N tile j % tiles_n)
-      const int64_t j = tile / nclusters;
+      // a CTA owns whole ROW BLOCKS and walks all their N tiles in turn (its epilogue accumulates across
+      // them): work item j of CTA c is (row block c + (j / tiles_n) * nctas, N tile j % tiles_n)
+      const int64_t j = tile / nctas;
       nt = j % w.tiles_n;
-      mt = tile % nclusters + (j / w.tiles_n) * nclusters;
+      mt = tile % nctas + (j / w.tiles_n) * nctas;
       kbeg = 0;
       nkb = mt < w.tiles_m ? (int)(g.k_pad / kTK) : 0;
       return;
@@ -1034,15 +788,14 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     nkb = kend > kbeg ? (int)((kend - kbeg) / kTK) : 0;
   };
 
-  constexpr int kMmaWarp = WsLayout<GEN != 0>::kMmaWarp;
-  if (GEN != 0 && warp >= kWsEpilogueWarps && warp < kMmaWarp) {
+  if (GEN != 0 && warp >= kWsConsumerWarps) {
     // ------------------------------------------------------------------------------ generating producers
     // 8 warps in TWO GROUPS of 128 threads; group g owns the stages with (stage counter & 1) == g and generates a
     // whole row (64 columns) per thread for them.  Two stages are therefore in production at any time: while one
     // group waits for its global loads (the producer is load-latency-bound: ncu source page, FMUL on the loaded
     // operands holds the stall samples), the other one multiplies / splits / stores.  B (filter / dY planes)
     // arrives by TMA, issued by thread 0 of the group that owns the stage.
-    const int tid = threadIdx.x - kWsEpilogueWarps * 32;
+    const int tid = threadIdx.x - kWsConsumerWarps * 32;
     const int grp = tid >> 7, t128 = tid & 127;
     if (t128 == 0) { tma_prefetch_desc(&tm_bh); tma_prefetch_desc(&tm_bl); }
     uint32_t it = 0;
@@ -1058,15 +811,15 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
       const int soff = (g.a_mn ? atom * 8192 : 0) + rr * 128;
       // (32-bit coordinates: rows, columns and tile counts of the generated-operand GEMMs fit 31 bits, checked on
       // the host; the state of two k-blocks stays in registers next to the prefetched operands)
-      const int ntiles = (int)w.ntiles, stride = (int)nclusters;
+      const int ntiles = (int)w.ntiles, stride = (int)nctas;
       auto dec = [&](int tile, int& m0, int& n0, int& kbeg, int& nkb) {
         int64_t mt, nt, kb64;
         decode(tile, mt, nt, kb64, nkb);
-        m0 = (int)((mt * NCTA + cta_rank) * kTM);
-        n0 = (int)(nt * BN + (int64_t)cta_rank * BNH);
+        m0 = (int)(mt * kTM);
+        n0 = (int)(nt * BN);
         kbeg = (int)kb64;
       };
-      int tile = (int)cluster_id, m0 = 0, n0 = 0, kbeg = 0, nkb = 0, kb = 0;
+      int tile = (int)cta0, m0 = 0, n0 = 0, kbeg = 0, nkb = 0, kb = 0;
       for (; tile < ntiles; tile += stride) {            // first tile with work
         dec(tile, m0, n0, kbeg, nkb);
         if (nkb > 0) break;
@@ -1112,7 +865,7 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
           const uint32_t st = smem_u32(stp);
           if (g.b_mn) {
 #pragma unroll
-            for (int j = 0; j < (BNH >= 64 ? BNH / 64 : 1); ++j) {
+            for (int j = 0; j < (BN >= 64 ? BN / 64 : 1); ++j) {
               tma_load_2d(st + 2 * A_PLANE + j * 8192, &tm_bh, n0 + 64 * j, k0, bar);
               tma_load_2d(st + 2 * A_PLANE + B_PLANE + j * 8192, &tm_bl, n0 + 64 * j, k0, bar);
             }
@@ -1135,12 +888,12 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
         tile = tile_n; m0 = m0_n; n0 = n0_n; kbeg = kbeg_n; nkb = nkb_n; kb = kb_n;
       }
     } else
-    for (int64_t tile = cluster_id; tile < w.ntiles; tile += nclusters) {
+    for (int64_t tile = cta0; tile < w.ntiles; tile += nctas) {
       int64_t mt, nt, kbeg;
       int nkb;
       decode(tile, mt, nt, kbeg, nkb);
-      const int64_t m0 = (mt * NCTA + cta_rank) * kTM;
-      const int32_t n0 = (int32_t)(nt * BN + (int64_t)cta_rank * BNH);
+      const int64_t m0 = mt * kTM;
+      const int32_t n0 = (int32_t)(nt * BN);
       for (int kb = 0; kb < nkb; ++kb, ++it) {
         const bool two = g.gen_groups == 2;
         if (two && (int)(it & 1) != grp) continue;
@@ -1154,7 +907,7 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
           const uint32_t st = smem_u32(stp);
           if (g.b_mn) {
 #pragma unroll
-            for (int j = 0; j < (BNH >= 64 ? BNH / 64 : 1); ++j) {
+            for (int j = 0; j < (BN >= 64 ? BN / 64 : 1); ++j) {
               tma_load_2d(st + 2 * A_PLANE + j * 8192, &tm_bh, n0 + 64 * j, (int32_t)k0, bar);
               tma_load_2d(st + 2 * A_PLANE + B_PLANE + j * 8192, &tm_bl, n0 + 64 * j, (int32_t)k0, bar);
             }
@@ -1189,67 +942,60 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
         mbar_arrive(&full_bar[s]);
       }
     }
-  } else if (TMA && warp >= kWsEpilogueWarps && warp < kMmaWarp) {
+  } else if (TMA && warp >= kWsConsumerWarps) {
     // ------------------------------------------------------------------------------ TMA producer
-    // warp 8, one elected lane: wait for a free stage, arm its barrier with the stage bytes, issue the bulk
-    // tensor copies of the four operand planes.  No registers, no per-element instructions, no proxy fence:
-    // data moves global -> swizzled shared memory inside the async proxy, where tcgen05.mma reads it.
-    if (warp == kWsEpilogueWarps && lane == 0) {
+    // one elected lane: wait for a free stage, arm its barrier with the stage bytes, issue the bulk tensor copies
+    // of the four operand planes.  Data moves global -> swizzled shared memory inside the async proxy, where
+    // wgmma reads it.
+    if (warp == kWsConsumerWarps && lane == 0) {
       tma_prefetch_desc(&tm_ah); tma_prefetch_desc(&tm_al); tma_prefetch_desc(&tm_bh); tma_prefetch_desc(&tm_bl);
       uint32_t it = 0;
-      for (int64_t tile = cluster_id; tile < w.ntiles; tile += nclusters) {
+      for (int64_t tile = cta0; tile < w.ntiles; tile += nctas) {
         int64_t mt, nt, kbeg;
         int nkb;
         decode(tile, mt, nt, kbeg, nkb);
-        const int32_t m0 = (int32_t)((mt * NCTA + cta_rank) * kTM);
-        const int32_t n0 = (int32_t)(nt * BN + (int64_t)cta_rank * BNH);
+        const int32_t m0 = (int32_t)(mt * kTM);
+        const int32_t n0 = (int32_t)(nt * BN);
         for (int kb = 0; kb < nkb; ++kb, ++it) {
           const int s = it % STAGES;
           mbar_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
           uint64_t* bar = &full_bar[s];
-          if (g.debug & 8) { mbar_arrive(bar); continue; }
-          // CTA pair: both CTAs' loads complete on the LEADER's barrier, armed there with the bytes of both halves
-          if (NCTA == 1 || cta_rank == 0) mbar_expect_tx(bar, (uint32_t)(NCTA * STAGE));
-          const uint32_t lbar = NCTA == 1 ? smem_u32(bar) : mapa_u32(smem_u32(bar), 0);
-          auto load = [&](uint32_t dst, const CUtensorMap* map, int32_t c0, int32_t c1) {
-            if constexpr (NCTA == 1) tma_load_2d(dst, map, c0, c1, bar);
-            else tma_load_2d_pair(dst, map, c0, c1, lbar);
-          };
+          mbar_expect_tx(bar, (uint32_t)STAGE);
           const uint32_t st = smem_u32(tiles + (size_t)s * STAGE);
           const int32_t k0 = (int32_t)(kbeg + (int64_t)kb * kTK);
           if (g.a_mn) {        // [k, m] planes: one 64(m) x 64(k) box per 64-wide atom
 #pragma unroll
             for (int j = 0; j < kTM / 64; ++j) {
-              load(st + j * 8192, &tm_ah, m0 + 64 * j, k0);
-              load(st + A_PLANE + j * 8192, &tm_al, m0 + 64 * j, k0);
+              tma_load_2d(st + j * 8192, &tm_ah, m0 + 64 * j, k0, bar);
+              tma_load_2d(st + A_PLANE + j * 8192, &tm_al, m0 + 64 * j, k0, bar);
             }
           } else {             // [m, k] planes: one 64(k) x 128(m) box
-            load(st, &tm_ah, k0, m0);
-            load(st + A_PLANE, &tm_al, k0, m0);
+            tma_load_2d(st, &tm_ah, k0, m0, bar);
+            tma_load_2d(st + A_PLANE, &tm_al, k0, m0, bar);
           }
-          if (g.b_mn) {
+          if (g.b_mn) {        // (an MN-major B tile is at least one 64-wide atom: BN >= 64)
 #pragma unroll
-            for (int j = 0; j < (BNH >= 64 ? BNH / 64 : 1); ++j) {
-              load(st + 2 * A_PLANE + j * 8192, &tm_bh, n0 + 64 * j, k0);
-              load(st + 2 * A_PLANE + B_PLANE + j * 8192, &tm_bl, n0 + 64 * j, k0);
+            for (int j = 0; j < (BN >= 64 ? BN / 64 : 1); ++j) {
+              tma_load_2d(st + 2 * A_PLANE + j * 8192, &tm_bh, n0 + 64 * j, k0, bar);
+              tma_load_2d(st + 2 * A_PLANE + B_PLANE + j * 8192, &tm_bl, n0 + 64 * j, k0, bar);
             }
           } else {
-            load(st + 2 * A_PLANE, &tm_bh, k0, n0);
-            load(st + 2 * A_PLANE + B_PLANE, &tm_bl, k0, n0);
+            tma_load_2d(st + 2 * A_PLANE, &tm_bh, k0, n0, bar);
+            tma_load_2d(st + 2 * A_PLANE + B_PLANE, &tm_bl, k0, n0, bar);
           }
         }
       }
     }
-  } else if (warp >= kWsEpilogueWarps && warp < kMmaWarp) {
+  } else if (warp >= kWsConsumerWarps) {
     // ------------------------------------------------------------------------------ producers
-    const int tid = threadIdx.x - kWsEpilogueWarps * 32;
+    const int tid = threadIdx.x - kWsConsumerWarps * 32;
     constexpr int NT = kWsProducers * 32;
-    int64_t tile = cluster_id, mt = 0, nt = 0, kbeg = 0;
+    int64_t tile = cta0, mt = 0, nt = 0, kbeg = 0;
     int nkb = 0, kb = 0;
     while (tile < w.ntiles) {            // first tile with work
       decode(tile, mt, nt, kbeg, nkb);
       if (nkb > 0) break;
-      tile += nclusters;
+      tile += nctas;
     }
     // Every producer thread hands its copies to the stage's mbarrier (cp.async.mbarrier.arrive.noinc: the
     // arrival fires when the thread's cp.asyncs have landed), so this warp never waits for data - only for a
@@ -1259,8 +1005,8 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
       mbar_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
       const uint32_t st = smem_u32(tiles + (size_t)s * STAGE);
       const int64_t k0 = kbeg + (int64_t)kb * kTK;
-      const int64_t m0 = (mt * NCTA + cta_rank) * kTM;
-      const int64_t n0 = nt * BN + (int64_t)cta_rank * BNH;
+      const int64_t m0 = mt * kTM;
+      const int64_t n0 = nt * BN;
 #pragma unroll 4
       for (int t = tid; t < kTM * 8; t += NT) {
         uint32_t off;
@@ -1278,11 +1024,11 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
         cp_async16(st + A_PLANE + off, g.a_lo + src);
       }
 #pragma unroll 4
-      for (int t = tid; t < BNH * 8; t += NT) {
+      for (int t = tid; t < BN * 8; t += NT) {
         uint32_t off;
         int64_t src;
         if (g.b_mn) {
-          const int kk = t / (BNH / 8), c = t % (BNH / 8);
+          const int kk = t / (BN / 8), c = t % (BN / 8);
           off = (c >> 3) * 8192 + kk * 128 + (((c & 7) ^ (kk & 7)) << 4);
           src = (k0 + kk) * g.b_pitch + n0 + c * 8;
         } else {
@@ -1296,302 +1042,103 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
       asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&full_bar[s])) : "memory");
       if (++kb == nkb) {               // next tile with work
         kb = 0;
-        tile += nclusters;
+        tile += nctas;
         while (tile < w.ntiles) {
           decode(tile, mt, nt, kbeg, nkb);
           if (nkb > 0) break;
-          tile += nclusters;
+          tile += nctas;
         }
       }
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
-  } else if (warp == kMmaWarp) {
-    // ------------------------------------------------------------------------------ MMA issuer
-    if (cta_rank == 0) {
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) |
-                             ((uint32_t)((kTM * NCTA) >> 4) << 24) | (g.a_mn ? (1u << 15) : 0u) |
-                             (g.b_mn ? (1u << 16) : 0u);
-      uint32_t it = 0, acc_it = 0;
-      for (int64_t tile = cluster_id; tile < w.ntiles; tile += nclusters) {
-        int64_t mt, nt, kbeg;
-        int nkb;
-        decode(tile, mt, nt, kbeg, nkb);
-        if (nkb == 0) continue;
-        const uint32_t ab = acc_it & 1;
-        mbar_wait_cluster(&acc_empty[ab], ((acc_it >> 1) & 1) ^ 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + ab * BN;
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = it % STAGES;
-          mbar_wait(&full_bar[s], (it / STAGES) & 1);
-          if constexpr (NCTA > 1 && !(TMA && GEN == 0)) mbar_wait_cluster(&peer_full[s], (it / STAGES) & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          if (lane == 0) {
-            const uint32_t sa = smem_u32(tiles + (size_t)s * STAGE);
-            const uint32_t a_hi = sa, a_lo = sa + A_PLANE, b_hi = sa + 2 * A_PLANE, b_lo = sa + 2 * A_PLANE + B_PLANE;
-#pragma unroll
-            for (int ks = 0; ks < kTK / 16; ++ks) {
-              if (g.debug & 4) break;
-              const uint64_t dah = umma_desc_any(a_hi, ks, g.a_mn), dal = umma_desc_any(a_lo, ks, g.a_mn);
-              const uint64_t dbh = umma_desc_any(b_hi, ks, g.b_mn), dbl = umma_desc_any(b_lo, ks, g.b_mn);
-              umma_f16_ws<NCTA>(tmem_d, dah, dbh, idesc, (kb | ks) ? 1u : 0u);
-              umma_f16_ws<NCTA>(tmem_d, dah, dbl, idesc, 1u);
-              umma_f16_ws<NCTA>(tmem_d, dal, dbh, idesc, 1u);
-            }
-            umma_commit_ws<NCTA>(&empty_bar[s]);
-            if (kb == nkb - 1) umma_commit_ws<NCTA>(&acc_full[ab]);
-          }
-          __syncwarp();
-        }
-        ++acc_it;
-      }
-    } else if constexpr (!(TMA && GEN == 0)) {
-      // peer CTA (cp.async / generated operands): relay "my half of stage s has landed" to the leader, which issues
-      // the MMAs of the pair.  With TMA for both operands the peer's loads signal the leader's barrier themselves.
-      uint32_t it = 0;
-      for (int64_t tile = cluster_id; tile < w.ntiles; tile += nclusters) {
-        int64_t mt, nt, kbeg;
-        int nkb;
-        decode(tile, mt, nt, kbeg, nkb);
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = it % STAGES;
-          mbar_wait(&full_bar[s], (it / STAGES) & 1);
-          if (lane == 0) mbar_arrive_cluster(&peer_full[s], 0);
-          __syncwarp();
-        }
-      }
-    }
   } else {
-    // ------------------------------------------------------------------------------ epilogue
-    // 8 warps: warp & 3 = TMEM sub-partition (32 rows), warp >> 2 = column half of the accumulator
-    const int sub = warp & 3, half = warp >> 2;
-    constexpr int HALVES = BN >= 64 ? 2 : 1;
-    constexpr int COLS = BN / HALVES;
-    const bool vec_c = (g.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.c) & 15) == 0) &&
-                       (!g.bias || (reinterpret_cast<uintptr_t>(g.bias) & 15) == 0);
-    const bool vec_ws = (g.n % 4 == 0);
-    uint32_t acc_it = 0;
-    if constexpr (FOLD) {
-      // CIN backward: the accumulator tile is dZ[r, q] (q = i*hp + j) = dY W'^T and is never stored - it is folded
-      // onto the two factors of the outer product right here:
-      //   dT0[r, i] += sum_j dZ[r, i*hp + j] * xk[r, j]          (one red.add per 32-column group)
-      //   dXk[r, j] += sum_i dZ[r, i*hp + j] * t0[r, i]          (registers across the N tiles of the row block,
-      //                                                           red.add.v4 once per row block)
-      // BN % hp == 0, so a thread's column groups keep their j-range from tile to tile.
-      constexpr int GROUPS = COLS / 32;
-      float dxk[GROUPS][32];
-      for (int64_t tile = cluster_id; tile < w.ntiles; tile += nclusters) {
-        int64_t mt, nt, kbeg;
-        int nkb;
-        decode(tile, mt, nt, kbeg, nkb);
-        if (nkb == 0) continue;
-        const uint32_t ab = acc_it & 1;
-        mbar_wait(&acc_full[ab], (acc_it >> 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int64_t gm = (mt * NCTA + cta_rank) * kTM + sub * 32 + lane;
-        const bool row_ok = gm < g.m;
-        const float* t0 = g.cin_t0 + (row_ok ? gm : 0) * g.cin_ld0;
-        const float* xk = g.cin_xk + (row_ok ? gm : 0) * g.cin_ldk;
-        if (nt == 0) {
-#pragma unroll
-          for (int gi = 0; gi < GROUPS; ++gi)
-#pragma unroll
-            for (int jx = 0; jx < 32; ++jx) dxk[gi][jx] = 0.f;
-        }
-#pragma unroll
-        for (int gi = 0; gi < GROUPS; ++gi) {
-          const int c0 = half * COLS + gi * 32;
-          const int64_t q = nt * BN + c0;
-          if (q < g.n) {                   // warp-uniform
-            uint32_t r[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(sub * 32) << 16) + ab * BN + (uint32_t)c0;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-                  "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-                  "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-                  "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                  "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            const int i = (int)(q / g.cin_hp), j0 = (int)(q - (int64_t)i * g.cin_hp);
-            if (row_ok && i < g.cin_m) {
-              const float a = __ldg(t0 + i);
-              float p = 0.f;
-#pragma unroll
-              for (int jx = 0; jx < 32; jx += 4) {
-                float4 xv = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (j0 + jx < g.cin_h) xv = __ldg(reinterpret_cast<const float4*>(xk + j0 + jx));
-                const float d0 = __uint_as_float(r[jx]), d1 = __uint_as_float(r[jx + 1]);
-                const float d2 = __uint_as_float(r[jx + 2]), d3 = __uint_as_float(r[jx + 3]);
-                if (j0 + jx + 1 >= g.cin_h) xv.y = 0.f;       // ragged h (rows padded to hp: loads stay in bounds)
-                if (j0 + jx + 2 >= g.cin_h) xv.z = 0.f;
-                if (j0 + jx + 3 >= g.cin_h) xv.w = 0.f;
-                p += d0 * xv.x + d1 * xv.y + d2 * xv.z + d3 * xv.w;
-                dxk[gi][jx] += d0 * a; dxk[gi][jx + 1] += d1 * a; dxk[gi][jx + 2] += d2 * a; dxk[gi][jx + 3] += d3 * a;
-              }
-              red_add_f1(g.fold_dt0 + gm * g.cin_ld0 + i, p);
-            }
-          }
-        }
-        if (nt == w.tiles_n - 1 && row_ok) {
-#pragma unroll
-          for (int gi = 0; gi < GROUPS; ++gi) {
-            const int j0 = (half * COLS + gi * 32) % g.cin_hp;
-            float* dst = g.fold_dxk + gm * g.fold_ldx + j0;
-#pragma unroll
-            for (int jx = 0; jx < 32; jx += 4)
-              if (j0 + jx < g.cin_h)
-                red_add_f4(dst + jx, make_float4(dxk[gi][jx], dxk[gi][jx + 1], dxk[gi][jx + 2], dxk[gi][jx + 3]));
-          }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-          if (NCTA == 1 || cta_rank == 0) mbar_arrive(&acc_empty[ab]);
-          else mbar_arrive_cluster(&acc_empty[ab], 0);
-        }
-        ++acc_it;
-      }
-    } else
-    for (int64_t tile = cluster_id; tile < w.ntiles; tile += nclusters) {
+    // ------------------------------------------------------------------------------ consumers
+    const int wg = warp >> 2;
+    uint32_t it = 0;
+    float d[BN / 2];
+    float dxk[FOLD ? BN / 2 : 1];      // FOLD: this thread's dXk partial sums, same layout as d
+    for (int64_t tile = cta0; tile < w.ntiles; tile += nctas) {
       int64_t mt, nt, kbeg;
       int nkb;
       decode(tile, mt, nt, kbeg, nkb);
-      const int64_t z = tile / ((int64_t)w.tiles_n * w.tiles_m);
-      const uint32_t ab = acc_it & 1;
-      if (nkb > 0) {
-        mbar_wait(&acc_full[ab], (acc_it >> 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-      // The accumulator arrives lane = row (tcgen05.ld 32x32b): a direct store would put the 32 lanes of every
-      // instruction in 32 different rows of C (16 bytes each, half a sector per lane - measured: ~4 us per
-      // 256 x 128 tile, the whole cost of a short-K tile).  Each warp therefore turns its 32 x 32 block through a
-      // 4 KB XOR-swizzled staging buffer and stores 8 lanes = 128 contiguous bytes per row, 4 rows per instruction.
-      const int64_t row_base = (mt * NCTA + cta_rank) * kTM + sub * 32;
-      unsigned char* stg = epi_stage + warp * 4096;
-      if (half < HALVES) {
-#pragma unroll 1
-        for (int c0 = half * COLS; c0 < (half + 1) * COLS; c0 += 32) {
-          const int64_t gn0 = nt * BN + c0;
-          if (gn0 >= g.n) break;           // warp-uniform
-          uint32_t r[32];
-          if (nkb > 0 && !(g.debug & 2)) {
-            const uint32_t taddr = tmem_base + ((uint32_t)(sub * 32) << 16) + ab * BN + (uint32_t)c0;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-                  "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-                  "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-                  "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                  "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          } else {
+      if (FOLD && nkb == 0) continue;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = 0u;
-          }
-          if (row_base >= g.m || (g.debug & 1)) continue;   // warp-uniform: the whole 32-row block is padding
-#pragma unroll
-          for (int c = 0; c < 8; ++c)      // row `lane`, 16-byte chunk c -> physical chunk c ^ (lane & 7)
-            *reinterpret_cast<uint4*>(stg + lane * 128 + ((c ^ (lane & 7)) << 4)) =
-                make_uint4(r[4 * c], r[4 * c + 1], r[4 * c + 2], r[4 * c + 3]);
+      for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
+        const int s = it % STAGES;
+        mbar_wait(&full_bar[s], (it / STAGES) & 1);
+        // cp.async producers write through the generic proxy
+        if (!TMA && GEN == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        wg_kblock<BN>(d, smem_u32(tiles + (size_t)s * STAGE), wg, g.a_mn, g.b_mn);
+        wgmma_wait<1>();                 // the group of the previous k-block has retired: release its stage
+        if (prev >= 0) {
           __syncwarp();
-          const int chunk = lane & 7;
-          const int64_t gn = gn0 + chunk * 4;
-          const bool full4 = gn + 4 <= g.n;
-          float4 bb = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (g.bias && g.splits == 1 && gn < g.n) {
-            if (full4 && vec_c) bb = __ldg(reinterpret_cast<const float4*>(g.bias + gn));
-            else {
-              bb.x = g.bias[gn];
-              if (gn + 1 < g.n) bb.y = g.bias[gn + 1];
-              if (gn + 2 < g.n) bb.z = g.bias[gn + 2];
-              if (gn + 3 < g.n) bb.w = g.bias[gn + 3];
-            }
-          }
-          const bool relu = g.act == B2CTR_ACT_RELU, other = g.act != B2CTR_ACT_NONE && !relu;
-#pragma unroll 2
-          for (int i = 0; i < 8; ++i) {
-            const int row = i * 4 + (lane >> 3);
-            const uint4 u = *reinterpret_cast<const uint4*>(stg + row * 128 + ((chunk ^ (row & 7)) << 4));
-            const int64_t gm = row_base + row;
-            if (gm >= g.m || gn >= g.n) continue;
-            float4 v = make_float4(g.alpha * __uint_as_float(u.x), g.alpha * __uint_as_float(u.y),
-                                   g.alpha * __uint_as_float(u.z), g.alpha * __uint_as_float(u.w));
-            if (g.splits > 1) {
-              float* wrow = g.ws + (z * g.m + gm) * g.n + gn;
-              if (vec_ws && full4) *reinterpret_cast<float4*>(wrow) = v;
-              else {
-                wrow[0] = v.x;
-                if (gn + 1 < g.n) wrow[1] = v.y;
-                if (gn + 2 < g.n) wrow[2] = v.z;
-                if (gn + 3 < g.n) wrow[3] = v.w;
-              }
-              continue;
-            }
-            float* crow = g.c + gm * g.ldc + gn;
-            const bool vec = vec_c && full4;
-            if (g.accumulate) {
-              if (vec) {
-                const float4 o = *reinterpret_cast<const float4*>(crow);
-                v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
-              } else {
-                v.x += crow[0];
-                if (gn + 1 < g.n) v.y += crow[1];
-                if (gn + 2 < g.n) v.z += crow[2];
-                if (gn + 3 < g.n) v.w += crow[3];
-              }
-            }
-            v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
-            if (relu) {
-              v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-            } else if (other) {
-              v.x = act_apply(v.x, g.act); v.y = act_apply(v.y, g.act);
-              v.z = act_apply(v.z, g.act); v.w = act_apply(v.w, g.act);
-            }
-            if (vec) *reinterpret_cast<float4*>(crow) = v;
-            else {
-              crow[0] = v.x;
-              if (gn + 1 < g.n) crow[1] = v.y;
-              if (gn + 2 < g.n) crow[2] = v.z;
-              if (gn + 3 < g.n) crow[3] = v.w;
-            }
-          }
-          __syncwarp();                    // the staging block is rewritten by the next column group
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
+        prev = s;
       }
-      if (nkb > 0) {      // hand the accumulator back to the MMA issuer of the pair
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+      wgmma_wait<0>();
+      fence_acc(d);
+      if (prev >= 0) {
         __syncwarp();
-        if (lane == 0) {
-          if (NCTA == 1 || cta_rank == 0) mbar_arrive(&acc_empty[ab]);
-          else mbar_arrive_cluster(&acc_empty[ab], 0);
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      const int64_t row0 = mt * kTM + wg * 64;
+      if constexpr (FOLD) {
+        // CIN backward: the accumulator tile is dZ[r, q] (q = i*hp + j) = dY W'^T and is never stored - it is folded
+        // onto the two factors of the outer product right here:
+        //   dT0[r, i] += sum_j dZ[r, i*hp + j] * xk[r, j]      (quad shuffle + one red.add per row and hp columns)
+        //   dXk[r, j] += sum_i dZ[r, i*hp + j] * t0[r, i]      (registers across the N tiles of the row block,
+        //                                                       red.add once per row block)
+        // BN % hp == 0, so a thread's columns keep their j from tile to tile.
+        if (nt == 0) {
+#pragma unroll
+          for (int j = 0; j < BN / 2; ++j) dxk[j] = 0.f;
         }
-        ++acc_it;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int64_t gm = row0 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+          const bool row_ok = gm < g.m;
+          const float* t0 = g.cin_t0 + (row_ok ? gm : 0) * g.cin_ld0;
+          const float* xk = g.cin_xk + (row_ok ? gm : 0) * g.cin_ldk;
+          float p = 0.f;
+#pragma unroll
+          for (int i = 0; i < BN / 8; ++i) {
+            const int c = 8 * i + 2 * (lane & 3);
+            const int64_t q = nt * BN + c;
+            const int ic = (int)(q / g.cin_hp), j = (int)(q - (int64_t)ic * g.cin_hp);
+            const bool ok = row_ok && ic < g.cin_m;
+            const float a = ok ? __ldg(t0 + ic) : 0.f;
+            const float x0 = ok && j < g.cin_h ? __ldg(xk + j) : 0.f;
+            const float x1 = ok && j + 1 < g.cin_h ? __ldg(xk + j + 1) : 0.f;
+            const float d0 = d[4 * i + 2 * h], d1 = d[4 * i + 2 * h + 1];
+            p += d0 * x0 + d1 * x1;
+            dxk[4 * i + 2 * h] += d0 * a;
+            dxk[4 * i + 2 * h + 1] += d1 * a;
+            if ((8 * (i + 1)) % g.cin_hp == 0) {     // last 8 columns of the hp-wide group of output i (warp-uniform)
+              p += __shfl_xor_sync(0xffffffffu, p, 1);
+              p += __shfl_xor_sync(0xffffffffu, p, 2);
+              if ((lane & 3) == 0 && ok) red_add_f1(g.fold_dt0 + gm * g.cin_ld0 + ic, p);
+              p = 0.f;
+            }
+          }
+          if (nt == w.tiles_n - 1 && row_ok) {
+            float* dst = g.fold_dxk + gm * g.fold_ldx;
+#pragma unroll
+            for (int i = 0; i < BN / 8; ++i) {
+              const int j = (8 * i + 2 * (lane & 3)) % g.cin_hp;
+              if (j < g.cin_h) red_add_f1(dst + j, dxk[4 * i + 2 * h]);
+              if (j + 1 < g.cin_h) red_add_f1(dst + j + 1, dxk[4 * i + 2 * h + 1]);
+            }
+          }
+        }
+      } else {
+        const int64_t z = tile / ((int64_t)w.tiles_n * w.tiles_m);
+        store_acc<BN>(g, d, row0, nt * BN, z);
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if constexpr (NCTA > 1) cluster_sync_all();      // no CTA leaves while its peer may still signal it
-  if (warp == WsLayout<GEN != 0>::kMmaWarp) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if constexpr (NCTA == 1)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
-}
-
-static int tc_debug() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("B2CTR_TC_DEBUG"); v = e ? atoi(e) : 0; }
-  return v;
 }
 
 struct TmaMaps {
@@ -1599,38 +1146,25 @@ struct TmaMaps {
   bool ok;
 };
 
-template <int BN, int STAGES, int NCTA, bool TMA, int GEN = 0, bool FOLD = false>
+template <int BN, int STAGES, bool TMA, int GEN = 0, bool FOLD = false>
 static cudaError_t launch_ws_impl(const WsArgs& wa, const TmaMaps& tm, cudaStream_t st) {
-  constexpr size_t smem = (size_t)STAGES * (2 * kTM * 128 + 2 * (BN / NCTA) * 128) + 1024 +
-                          (FOLD ? 0 : kWsEpilogueWarps * 4096);     // + the epilogue's transpose staging
+  constexpr size_t smem = (size_t)STAGES * (2 * kTM * 128 + 2 * BN * 128) + 1024;
   static_assert(smem + 256 <= 227 * 1024, "stage ring exceeds shared memory");
-  auto kern = gemm_planes_ws_kernel<BN, STAGES, NCTA, TMA, GEN, FOLD>;
+  auto kern = gemm_planes_ws_kernel<BN, STAGES, TMA, GEN, FOLD>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  const int64_t max_clusters = kNumSMs / NCTA;
-  int64_t nclusters = wa.ntiles < max_clusters ? wa.ntiles : max_clusters;
+  int64_t nctas = wa.ntiles < kNumSMs ? wa.ntiles : kNumSMs;
   WsArgs wcopy = wa;
-  if (FOLD) {      // clusters own row blocks: ntiles = work-item slots of the round-robin over row blocks
-    nclusters = wa.tiles_m < max_clusters ? wa.tiles_m : max_clusters;
-    wcopy.ntiles = ceil_div(wa.tiles_m, nclusters) * wa.tiles_n * nclusters;
+  if (FOLD) {      // CTAs own row blocks: ntiles = work-item slots of the round-robin over row blocks
+    nctas = wa.tiles_m < kNumSMs ? wa.tiles_m : kNumSMs;
+    wcopy.ntiles = ceil_div(wa.tiles_m, nctas) * wa.tiles_n * nctas;
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(nclusters * NCTA));
-  cfg.blockDim = dim3(WsLayout<GEN != 0>::kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = NCTA;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, wcopy, tm.ah, tm.al, tm.bh, tm.bl);
+  kern<<<(unsigned)nctas, WsLayout<GEN != 0>::kThreads, smem, st>>>(wcopy, tm.ah, tm.al, tm.bh, tm.bl);
+  return cudaGetLastError();
 }
-template <int BN, int STAGES, int NCTA>
+template <int BN, int STAGES>
 static cudaError_t launch_ws(const WsArgs& wa, const TmaMaps& tm, cudaStream_t st) {
-  return tm.ok ? launch_ws_impl<BN, STAGES, NCTA, true>(wa, tm, st) : launch_ws_impl<BN, STAGES, NCTA, false>(wa, tm, st);
+  return tm.ok ? launch_ws_impl<BN, STAGES, true>(wa, tm, st) : launch_ws_impl<BN, STAGES, false>(wa, tm, st);
 }
 
 // ---- tensor maps: cuTensorMapEncodeTiled resolved through the runtime's driver entry-point query ---------
@@ -1707,23 +1241,15 @@ static b2ctr_status_t gemm_planes(const b2ctr_gemm_t* g, void* workspace, size_t
   }
   const int splits = g->split_k > 1 ? g->split_k : 1;
   const bool ws_kernel = tc_variant(g) == 4;
-  int bn = ws_kernel ? (g->n <= 32 ? 32 : g->n <= 64 ? 64 : g->n <= 128 ? 128 : 256)
+  int bn = ws_kernel ? (g->n <= 32 ? 32 : g->n <= 64 ? 64 : 128)
                      : planes_bn(g->n, g->k / (g->split_k > 1 ? g->split_k : 1));
-  if (ws_kernel && bn == 256) {
-    // ragged N (dgrad of the first DNN layer: N = 845): 256-wide tiles pad it to 1024 (17 % of the MMAs and of the
-    // epilogue work are dead), 128-wide tiles to 896 (6 %).  Take the narrower tile when it saves > 8 % of the tile area.
-    static int tail = -1;
-    if (tail < 0) { const char* ev = getenv("B2CTR_TC_BN_TAIL"); tail = ev ? atoi(ev) : 1; }
-    const int64_t a256 = round_up(g->n, 256), a128 = round_up(g->n, 128);
-    if (tail && (a256 - a128) * 100 > 8 * a256) bn = 128;
-  }
   const int64_t kp = round_up(g->k > 0 ? g->k : 1, kTK), mp = round_up(g->m, 2 * kTM);
   unsigned char* w = (unsigned char*)workspace;
   float* ws = (float*)w;
   w += splits > 1 ? (size_t)splits * g->m * g->n * sizeof(float) : 0;
   w = (unsigned char*)(((uintptr_t)w + 255) & ~(uintptr_t)255);
   // variant 2: always K-major planes (row-contiguous sources go through a transposing split);
-  // variant 3: row-contiguous sources keep their layout (MN-major planes) and the UMMA descriptors do the
+  // variant 3: row-contiguous sources keep their layout (MN-major planes) and the wgmma descriptors do the
   // transposition - the same planes then serve every GEMM that reads the tensor (forward / dgrad / wgrad),
   // which is what caller-provided planes (g->a_planes / g->b_planes) exploit.
   const bool mn_ok = tc_variant(g) >= 3;
@@ -1781,35 +1307,24 @@ static b2ctr_status_t gemm_planes(const b2ctr_gemm_t* g, void* workspace, size_t
   pa.k_per_split = ceil_div(ceil_div(kp, splits), kTK) * kTK;
   pa.alpha = g->alpha; pa.act = g->act; pa.accumulate = g->accumulate; pa.splits = splits;
   pa.cin_on = 0; pa.cin_t0 = pa.cin_xk = nullptr; pa.cin_ld0 = pa.cin_ldk = pa.cin_rows = 0; pa.cin_m = pa.cin_h = pa.cin_hp = 0;
-  pa.fold_dt0 = pa.fold_dxk = nullptr; pa.fold_ldx = 0; pa.gen_groups = 0; pa.debug = tc_debug();
+  pa.fold_dt0 = pa.fold_dxk = nullptr; pa.fold_ldx = 0; pa.gen_groups = 0;
   cudaError_t e;
   const bool short_k = pa.k_per_split <= 4 * kTK;
   if (ws_kernel) {
     WsArgs wa;
     wa.p = pa;
-    int ncta = g->m > kTM ? 2 : 1;
-    if (b_mn && bn / ncta < 64) ncta = 1;        // an MN-major B half-tile must hold whole 64-wide atoms
-    wa.tiles_m = (int)ceil_div(g->m, (int64_t)kTM * ncta);
+    wa.tiles_m = (int)ceil_div(g->m, (int64_t)kTM);
     wa.tiles_n = (int)ceil_div(g->n, bn);
     wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n * splits;
     // TMA producers: four tiled tensor maps over the operand planes (box = one stage's slice of a plane)
     TmaMaps tm;
-    const int bnh = bn / ncta;
     tm.ok = tma_map_2d(&tm.ah, a_hi, a_pitch, a_prows, a_pitch, 64, a_mn ? 64 : kTM) &&
             tma_map_2d(&tm.al, a_lo, a_pitch, a_prows, a_pitch, 64, a_mn ? 64 : kTM) &&
-            tma_map_2d(&tm.bh, b_hi, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bnh) &&
-            tma_map_2d(&tm.bl, b_lo, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bnh);
-    if (ncta == 2) {
-      if (bn == 32) e = launch_ws<32, 5, 2>(wa, tm, st);
-      else if (bn == 64) e = launch_ws<64, 4, 2>(wa, tm, st);
-      else if (bn == 128) e = launch_ws<128, 4, 2>(wa, tm, st);
-      else e = launch_ws<256, 3, 2>(wa, tm, st);
-    } else {
-      if (bn == 32) e = launch_ws<32, 4, 1>(wa, tm, st);
-      else if (bn == 64) e = launch_ws<64, 4, 1>(wa, tm, st);
-      else if (bn == 128) e = launch_ws<128, 3, 1>(wa, tm, st);
-      else e = launch_ws<256, 2, 1>(wa, tm, st);
-    }
+            tma_map_2d(&tm.bh, b_hi, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bn) &&
+            tma_map_2d(&tm.bl, b_lo, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bn);
+    if (bn == 32) e = launch_ws<32, 5>(wa, tm, st);
+    else if (bn == 64) e = launch_ws<64, 4>(wa, tm, st);
+    else e = launch_ws<128, 3>(wa, tm, st);
   } else if (bn == 32) e = short_k ? launch_planes<32, 1>(pa, st) : launch_planes<32, 4>(pa, st);
   else if (bn == 64) e = short_k ? launch_planes<64, 1>(pa, st) : launch_planes<64, 4>(pa, st);
   else if (bn == 128) e = short_k ? launch_planes<128, 1>(pa, st) : launch_planes<128, 3>(pa, st);
@@ -1881,14 +1396,9 @@ static size_t gen_gemm_workspace_bytes(const GenSpec& sp, int mode, int64_t n, i
 }
 
 template <int GEN>
-static cudaError_t launch_gen(const WsArgs& wa, const TmaMaps& tm, int bn, int ncta, cudaStream_t st) {
-  if (ncta == 2) {
-    if (bn == 128) return launch_ws_impl<128, 4, 2, true, GEN>(wa, tm, st);
-    return launch_ws_impl<256, 3, 2, true, GEN>(wa, tm, st);
-  }
-  if (bn == 64) return launch_ws_impl<64, 4, 1, true, GEN>(wa, tm, st);
-  if (bn == 128) return launch_ws_impl<128, 3, 1, true, GEN>(wa, tm, st);
-  return launch_ws_impl<256, 2, 1, true, GEN>(wa, tm, st);
+static cudaError_t launch_gen(const WsArgs& wa, const TmaMaps& tm, int bn, cudaStream_t st) {
+  if (bn == 64) return launch_ws_impl<64, 4, true, GEN>(wa, tm, st);
+  return launch_ws_impl<128, 3, true, GEN>(wa, tm, st);
 }
 
 // mode 0: c[rows, n] = act(A B + bias), B = planes of a [kq, n] row-major matrix; mode 1: c[kq, n] = A^T dY,
@@ -1907,14 +1417,12 @@ static b2ctr_status_t gen_gemm(const GenSpec& sp, int mode, int64_t n, const voi
   pa.a_hi = pa.a_lo = nullptr; pa.a_pitch = 0;
   pa.cin_on = sp.kind; pa.cin_t0 = sp.p0; pa.cin_xk = sp.p1; pa.cin_ld0 = sp.ld0; pa.cin_ldk = sp.ld1;
   pa.cin_rows = sp.rows; pa.cin_m = sp.m; pa.cin_h = sp.h; pa.cin_hp = sp.hp;
-  pa.fold_dt0 = pa.fold_dxk = nullptr; pa.fold_ldx = 0; pa.debug = 0;
+  pa.fold_dt0 = pa.fold_dxk = nullptr; pa.fold_ldx = 0;
   {
     static int groups = -1;
     if (groups < 0) { const char* ev = getenv("B2CTR_GEN_GROUPS"); groups = ev ? atoi(ev) : 0; }
-    // measured (profiles/README.md): the CIN generator is faster with all 256 threads on every stage (C3 8.02 vs
-    // 8.32 ms), the (non-resident) attention generator with two groups alternating stages (C4 3.55 vs 3.59 ms)
-    // measured (C4, E = 64): the register-resident attention generator (B2CTR_GEN_GROUPS=1) is slower than the
-    // two-group one, 2.88 vs 2.61 ms per step
+    // the CIN generator runs all 256 threads on every stage; the attention generator two groups of 128 that
+    // alternate stages, or (B2CTR_GEN_GROUPS=1) all 256 with the keys held in registers
     pa.gen_groups = sp.kind == 1 ? 1 : (groups == 1 ? 1 : 2);
   }
   pa.b_mn = 1;      // both B operands are row-major matrices whose reduction dim is their row index
@@ -1933,12 +1441,10 @@ static b2ctr_status_t gen_gemm(const GenSpec& sp, int mode, int64_t n, const voi
   const __nv_bfloat16* bp = (const __nv_bfloat16*)planes;
   pa.b_hi = bp; pa.b_lo = bp + b_prows * cp; pa.b_pitch = cp;
   pa.k_per_split = ceil_div(ceil_div(pa.k_pad, splits), kTK) * kTK;
-  const int bn = n <= 64 ? 64 : (n <= 128 ? 128 : 256);
-  int ncta = pa.m > kTM ? 2 : 1;
-  if (bn / ncta < 64) ncta = 1;
+  const int bn = n <= 64 ? 64 : 128;
   WsArgs wa;
   wa.p = pa;
-  wa.tiles_m = (int)ceil_div(pa.m, (int64_t)kTM * ncta);
+  wa.tiles_m = (int)ceil_div(pa.m, (int64_t)kTM);
   wa.tiles_n = (int)ceil_div(n, bn);
   wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n * splits;
   TmaMaps tm;
@@ -1948,7 +1454,7 @@ static b2ctr_status_t gen_gemm(const GenSpec& sp, int mode, int64_t n, const voi
     return B2CTR_ERR_UNSUPPORTED;
   }
   tm.ah = tm.bh; tm.al = tm.bl;
-  const cudaError_t e = sp.kind == 1 ? launch_gen<1>(wa, tm, bn, ncta, st) : launch_gen<2>(wa, tm, bn, ncta, st);
+  const cudaError_t e = sp.kind == 1 ? launch_gen<1>(wa, tm, bn, st) : launch_gen<2>(wa, tm, bn, st);
   if (e != cudaSuccess) {
     set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e));
     return B2CTR_ERR_CUDA;
@@ -2005,24 +1511,21 @@ b2ctr_status_t cin_fold(const b2ctr_cin_gemm_t* g, float* dt0, float* dxk, int64
   pa.k_per_split = pa.k_pad; pa.alpha = 1.f; pa.act = 0; pa.accumulate = 0; pa.splits = 1;
   pa.cin_on = 0; pa.cin_t0 = g->t0; pa.cin_xk = g->xk; pa.cin_ld0 = g->ld0; pa.cin_ldk = g->ldk; pa.cin_rows = g->rows;
   pa.cin_m = g->m; pa.cin_h = g->h; pa.cin_hp = g->hp;
-  pa.fold_dt0 = dt0; pa.fold_dxk = dxk; pa.fold_ldx = ldx; pa.gen_groups = 0; pa.debug = 0;
+  pa.fold_dt0 = dt0; pa.fold_dxk = dxk; pa.fold_ldx = ldx; pa.gen_groups = 0;
   constexpr int bn = 128;
-  const int ncta = g->rows > kTM ? 2 : 1;
   WsArgs wa;
   wa.p = pa;
-  wa.tiles_m = (int)ceil_div(g->rows, (int64_t)kTM * ncta);
+  wa.tiles_m = (int)ceil_div(g->rows, (int64_t)kTM);
   wa.tiles_n = (int)ceil_div(kq, bn);
   wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n;
   TmaMaps tm;
-  const int bnh = bn / ncta;
   tm.ok = tma_map_2d(&tm.ah, pa.a_hi, cpn, a_prows, cpn, 64, kTM) && tma_map_2d(&tm.al, pa.a_lo, cpn, a_prows, cpn, 64, kTM) &&
-          tma_map_2d(&tm.bh, pa.b_hi, cpn, b_prows, cpn, 64, bnh) && tma_map_2d(&tm.bl, pa.b_lo, cpn, b_prows, cpn, 64, bnh);
+          tma_map_2d(&tm.bh, pa.b_hi, cpn, b_prows, cpn, 64, bn) && tma_map_2d(&tm.bl, pa.b_lo, cpn, b_prows, cpn, 64, bn);
   if (!tm.ok) {
     set_error("cin_fold: cuTensorMapEncodeTiled unavailable");
     return B2CTR_ERR_UNSUPPORTED;
   }
-  cudaError_t e = ncta == 2 ? launch_ws_impl<128, 4, 2, true, 0, true>(wa, tm, st)
-                            : launch_ws_impl<128, 3, 1, true, 0, true>(wa, tm, st);
+  cudaError_t e = launch_ws_impl<128, 3, true, 0, true>(wa, tm, st);
   if (e != cudaSuccess) {
     set_error("b2ctr_cin_fold: CUDA launch failed: %s", cudaGetErrorString(e));
     return B2CTR_ERR_CUDA;

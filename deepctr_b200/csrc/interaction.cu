@@ -1,4 +1,4 @@
-// interaction.cu — CrossNet, CIN helpers, InteractingLayer attention core (sm_100a).
+// interaction.cu — CrossNet, CIN helpers, InteractingLayer attention core (sm_90a).
 //
 // Reference math restated (never copied): deepctr/layers/interaction.py:410-424 (CrossNet),
 // :277-325 (CIN), :754-779 (InteractingLayer).  Pairwise reductions use warp shuffles; the dense
@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(256)
 // ------------------------------------------------------------------------------------------------
 // CIN.  X0(b,i,d) = x0[b*s0b + i*s0i + d*s0d], Xk likewise.  A batch chunk's outer product
 //   Z[(b,d), i*H + j] = X0(b,i,d) * Xk(b,j,d)
-// is materialised for a chunk small enough to stay in the 126 MB L2 and contracted with the filter
+// is materialised for a chunk small enough to stay in the 50 MB L2 and contracted with the filter
 // by b2ctr_gemm (tensor cores in BF16X3 mode); it never reaches HBM-sized buffers (DESIGN.md 4.3).
 // ------------------------------------------------------------------------------------------------
 struct CinView {

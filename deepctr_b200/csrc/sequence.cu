@@ -1,5 +1,5 @@
 // sequence.cu — DIN local-activation attention pieces, standalone sequence pooling / weighting,
-// Dice / BatchNormalization statistics, dropout (sm_100a).
+// Dice / BatchNormalization statistics, dropout (sm_90a).
 //
 // Reference math restated (never copied): deepctr/layers/core.py:94-108 (LocalActivationUnit input),
 // deepctr/layers/sequence.py:76-106, :155-183, :261-298, deepctr/layers/activation.py:59-64.

@@ -1,4 +1,4 @@
-"""Host-side runtime of the B200 CTR path.
+"""Host-side runtime of the H100 CTR path.
 
 What the reference gets from TensorFlow/Keras (symbolic ``Input``s, the ``Layer`` protocol, the
 functional ``Model`` with compile/fit/predict, automatic differentiation, optimizers) is provided
@@ -34,7 +34,7 @@ from . import kernels as K
 
 def device():
     if not torch.cuda.is_available():
-        raise L.B2ctrError("deepctr_b200 needs a CUDA device (B200, sm_100a): the compute path has no "
+        raise L.B2ctrError("deepctr_b200 needs a CUDA device (H100, sm_90a): the compute path has no "
                            "CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
 

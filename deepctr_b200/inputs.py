@@ -7,7 +7,7 @@ Reference functions mirrored (same names / arguments / return structure):
 ``get_varlen_pooling_list`` (:133-158), ``get_dense_input`` (:161-172), ``mergeDict`` (:175-181),
 ``get_embedding_vec_list`` (:74-86), ``get_inputs_list`` (:40-41).
 
-B200 design (DESIGN.md section 3): the builders still call ``Embedding`` once per feature, but the
+H100 design (DESIGN.md section 3): the builders still call ``Embedding`` once per feature, but the
 ``EmbeddingPlanner`` owned by the Model recognises, once per graph, every lookup whose ids are a
 model input (optionally through ``Hash``) and every ``SequencePoolingLayer`` /
 ``WeightedSequenceLayer`` chain hanging off such a lookup, lays all their outputs out as adjacent
@@ -473,7 +473,7 @@ class EmbeddingPlanner(object):
 
         Every 4-byte linear lookup costs a 64-byte DRAM granule in the gather and a read + write of one in the
         update: 20 % of the gather's and 22 % of the update's DRAM traffic at C2 (profiles/README.md).  The 26
-        tables are 104 MB - inside the 126 MB L2 - so they are moved into one arena once, and the two fused
+        tables are 104 MB - twice the 50 MB L2 - so they are moved into one arena once, and the two fused
         kernels fetch that range with the persisting property (b2ctr_uniform_gather_t.l2_window) while the
         embedding rows and activations stream.  B2CTR_L2_PERSIST=0 turns it off."""
         if getattr(self, "_arena", False) is not False:

@@ -9,7 +9,7 @@ from . import kernels as K
 from . import engine as E
 
 # precision mode used by every dense GEMM (DNN / attention MLP / projections); see DESIGN.md section 4.2.
-# Default: split-bf16 on the tcgen05 tensor cores (three bf16 MMAs per product, fp32 accumulation; relative
+# Default: split-bf16 on the wgmma tensor cores (three bf16 MMAs per product, fp32 accumulation; relative
 # error ~2^-16, inside the 1e-4 logit tolerance of the parity tests); 'fp32' selects the exact FFMA GEMM.
 GEMM_PRECISION = L.GEMM_BF16X3
 
@@ -32,7 +32,7 @@ def mark_uncapturable():
 
 
 def set_gemm_precision(mode):
-    """'fp32' (exact FFMA) or 'bf16x3' (tcgen05 split-bf16, ~2^-17 relative)."""
+    """'fp32' (exact FFMA) or 'bf16x3' (wgmma split-bf16, ~2^-17 relative)."""
     global GEMM_PRECISION
     GEMM_PRECISION = {"fp32": L.GEMM_FP32, "bf16x3": L.GEMM_BF16X3}[mode]
 
@@ -496,10 +496,10 @@ def cross_matrix(x0, xl, w, bias):
     return res
 
 
-CIN_CHUNK_BYTES = 48 << 20      # outer-product chunk kept well inside the 126 MB L2
+CIN_CHUNK_BYTES = 24 << 20      # outer-product chunk kept well inside the 50 MB L2
 
 
-CIN_FUSED = True              # generate the outer product inside the tcgen05 GEMM producer (b2ctr_cin_gemm)
+CIN_FUSED = True              # generate the outer product inside the wgmma GEMM producer (b2ctr_cin_gemm)
 CIN_FOLD = True               # ... and fold dZ = dY W^T onto the factors inside the GEMM epilogue (b2ctr_cin_fold)
 CIN_DZ_CHUNK_BYTES = 512 << 20
 
@@ -591,7 +591,7 @@ def _cin_fused(x, filters, biases, layer_size, activation, split_half):
                 E.add_grad(filters[i], K.cin_unpad_rows(dwp, m, h, hp).reshape(filters[i].shape))
             dhid = None
             if fold:
-                # dZ = dY W'^T exists only as TMEM tiles: the GEMM epilogue folds it onto T0 and X_k
+                # dZ = dY W'^T exists only as accumulator tiles: the GEMM epilogue folds it onto T0 and X_k
                 if i > 0:
                     dhid = _empty((rows, h), x2)
                     K.fill(dhid, 0.0)

@@ -1,5 +1,5 @@
 /*
- * b2ctr.h — C-ABI of libb2ctr.so: the B200 (sm_100a) CTR forward/backward hot path.
+ * b2ctr.h — C-ABI of libb2ctr.so: the H100 (sm_90a) CTR forward/backward hot path.
  *
  * The reference (shenweichen/DeepCTR, pure Python over TensorFlow) has no FFI of its own
  * (SURVEY.md §8b).  Each entry point below is what a maintainer would bind in place of the
@@ -159,8 +159,8 @@ typedef struct b2ctr_uniform_gather {
   void* x_planes;
   int64_t x_planes_cols;
   /* Optional persisting-L2 window (cudaAccessPolicyWindow attached to THIS launch): [l2_window, l2_window +
-   * l2_window_bytes) - the arena holding the dim-1 linear tables (26 x 1M x 4 B = 104 MB at C2, inside the
-   * 126 MB L2) - is fetched with the persisting property for a fraction l2_hit_ratio of its lines, everything
+   * l2_window_bytes) - the arena holding the dim-1 linear tables (26 x 1M x 4 B = 104 MB at C2; the
+   * 50 MB L2 holds part of it) - is fetched with the persisting property for a fraction l2_hit_ratio of its lines, everything
    * else streams.  Each 4-byte linear lookup otherwise costs a 64-byte DRAM granule in the gather and two in
    * the update.  Needs b2ctr_l2_persist_reserve() once per device.  NULL / 0 = off. */
   const void* l2_window;
@@ -231,7 +231,7 @@ B2CTR_API b2ctr_status_t b2ctr_init_normal(float* dst, int64_t n, float mean, fl
 /* ------------------------------------------------------------------------------------------ */
 enum { B2CTR_ACT_NONE = 0, B2CTR_ACT_RELU = 1, B2CTR_ACT_SIGMOID = 2, B2CTR_ACT_TANH = 3 };
 enum { B2CTR_GEMM_FP32 = 0,  /* exact fp32 FFMA path (CUDA cores)                              */
-       B2CTR_GEMM_BF16X3 = 1 /* tcgen05 tensor cores, 3-term split-bf16 (~2^-17 rel. error)    */ };
+       B2CTR_GEMM_BF16X3 = 1 /* wgmma tensor cores, 3-term split-bf16 (~2^-17 rel. error)      */ };
 
 typedef struct b2ctr_gemm {
   const float* a; const float* b; float* c;
@@ -387,7 +387,7 @@ B2CTR_API b2ctr_status_t b2ctr_cin_outer_bwd(const float* dz, const float* x0, i
  * filter is used in the matching padded layout W'[i*hp + j, n] (b2ctr_cin_filter_planes: bf16 hi/lo planes).
  *   mode 0:  c[rows, n]   = act(Z W' + bias)     (forward; deepctr/layers/interaction.py:291-306)
  *   mode 1:  c[m*hp, n]   = Z^T dY               (filter gradient; dY given as b2ctr_split_planes of [rows, n])
- * tcgen05 split-bf16 (BF16X3) arithmetic, TMA for the B operand, 128 producer threads generate A. */
+ * wgmma split-bf16 (BF16X3) arithmetic, TMA for the B operand, 128 producer threads generate A. */
 typedef struct b2ctr_cin_gemm {
   const float* t0; int64_t ld0;      /* [rows, ld0], columns >= m are ignored                          */
   const float* xk; int64_t ldk;      /* [rows, ldk], 16-byte aligned rows (ldk % 4 == 0)                */
@@ -422,7 +422,7 @@ B2CTR_API size_t b2ctr_att_gemm_workspace_bytes(const b2ctr_att_gemm_t* g);
 B2CTR_API b2ctr_status_t b2ctr_att_gemm(const b2ctr_att_gemm_t* g, void* workspace, size_t workspace_bytes,
                                        void* stream);
 /* CIN backward, data gradient: dZ = dY W'^T (dy_planes: b2ctr_split_planes of dY [rows, n]; w_planes as in mode 0)
- * is formed tile by tile in TMEM and FOLDED onto the two factors inside the GEMM epilogue - it is never stored:
+ * is formed tile by tile in registers and FOLDED onto the two factors inside the GEMM epilogue - it is never stored:
  *   dt0[r, i]  += sum_j dZ[r, i*hp + j] * xk[r, j]        dxk[r, j] += sum_i dZ[r, i*hp + j] * t0[r, i]
  * Both outputs are accumulated with red.add (zero them first; layer 0 passes dxk = dt0).  hp in {32, 64, 128};
  * c / ldc / bias / act / mode / split_k of the descriptor are ignored. */

@@ -4,7 +4,7 @@
 
     python profiles/summarize_launches.py profiles/r2_launches_c2.csv
 
-Durations are cold-cache and serialised (B200_PROFILING.md): compare SHARES, not absolutes."""
+Durations are cold-cache and serialised: compare SHARES, not absolutes."""
 import collections
 import csv
 import sys

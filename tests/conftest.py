@@ -10,7 +10,7 @@ for _p in (ROOT, os.path.join(ROOT, 'tests')):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -21,7 +21,7 @@ def cuda():
     return torch.device("cuda:0")
 
 
-# Model-level GPU parity runs in BOTH GEMM precisions: 'bf16x3' (the default: tcgen05 split-bf16, what bench.py
+# Model-level GPU parity runs in BOTH GEMM precisions: 'bf16x3' (the default: wgmma split-bf16, what bench.py
 # measures) and 'fp32' (exact FFMA path).  Modules opt in with:  from conftest import gemm_precision  # noqa
 @pytest.fixture(params=["bf16x3", "fp32"], autouse=False)
 def gemm_precision(request):

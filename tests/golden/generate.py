@@ -2,7 +2,7 @@
 """Generate tests/golden/*.npz by executing the REFERENCE's unmodified layer code
 (/root/reference/deepctr/layers/*.py) under the torch-backed ``tensorflow`` stand-in of
 tf_torch_shim.py.  Run in the build container (needs /root/reference); the fixtures are committed so
-the GPU box, which has no reference tree, can check both the oracle and the CUDA path against them.
+the GPU test machine, which has no reference tree, can check both the oracle and the CUDA path against them.
 
     python tests/golden/generate.py
 

@@ -237,8 +237,8 @@ def test_optimizers(cuda):
 @pytest.mark.parametrize("ta,tb", [(False, False), (False, True), (True, False), (True, True)])
 @pytest.mark.parametrize("variant", [1, 2, 3, 4])   # 1: split in the GEMM producers, 2: K-major planes,
 def test_gemm_bf16x3_tensor_core(cuda, m, n, k, ta, tb, variant):
-    """tcgen05 split-bf16 GEMM: error bound ~2^-16 relative to sum |a||b| (DESIGN.md section 4.2).
-    Variants: 3 = + MN-major planes, 4 = persistent warp-specialised CTA-pair kernel (cta_group::2)."""
+    """wgmma split-bf16 GEMM: error bound ~2^-16 relative to sum |a||b| (DESIGN.md section 4.2).
+    Variants: 3 = + MN-major planes, 4 = persistent warp-specialised kernel."""
     K, L = _kern()
     rng = np.random.RandomState(m + 3 * n + k)
     a = _r(rng, *((k, m) if ta else (m, k)))
@@ -285,7 +285,7 @@ def test_gemm_bf16x3_with_caller_planes(cuda, m, n, k, ta, tb, given, variant):
                                              (30000, 64, 128, False, True, 1), (20000, 40, 100, False, False, 1),
                                              (256, 256, 30000, True, False, 37)])
 def test_gemm_bf16x3_persistent_pair_many_tiles(cuda, m, n, k, ta, tb, sk):
-    """Variant 4 at shapes where every CTA pair walks many tiles (both TMEM accumulators, several trips
+    """Variant 4 at shapes where every CTA walks many tiles (the producers run ahead across tile boundaries, several trips
     round the stage ring): same products in the same K order as the one-tile-per-CTA kernel -> identical."""
     K, L = _kern()
     rng = np.random.RandomState(m + n + k)

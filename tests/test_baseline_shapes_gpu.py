@@ -4,7 +4,7 @@ bench configuration's).  Every step: the loss against the oracle evaluated on th
 (logits within 1e-4, north_star); on the graph-replayed step also every weight update against the oracle's
 autograd gradient.
 
-  C2  DeepFM   F=26 E=32 B=65536 (K=845 first GEMM, the <256,3,2> many-tile tcgen05 path, graph replay)
+  C2  DeepFM   F=26 E=32 B=65536 (K=845 first GEMM, the many-tile persistent wgmma path, graph replay)
   C3  xDeepFM  F=26 E=16 CIN (128,128) split_half relu, B=4096
   C4  DIN      T=50 E=64 att (80,40), B=2048: sigmoid (training step) and dice (inference statistics)
 """
