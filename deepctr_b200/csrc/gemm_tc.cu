@@ -9,7 +9,8 @@
 // Every kernel computes 128 x BN output tiles.  Operand tiles sit in shared memory as bf16 hi / lo planes in the
 // 128-byte-swizzled layouts wgmma reads through matrix descriptors (K-major: 16-byte chunk index XOR row % 8;
 // MN-major: 64-element atoms of 64 k-rows).  Two consumer warpgroups each own 64 rows of the tile and issue
-// wgmma.mma_async m64nBNk16 on them; the accumulator lives in their registers and the epilogue stores it from there.
+// wgmma.mma_async m64nBNk16 on them; the accumulator lives in their registers.  The epilogue stores it from there,
+// or (variant 4, plain outputs) stages it in shared memory and stores it with TMA.
 //   variant 1: the 256 threads split the fp32 operands into the stage themselves, then multiply it
 //   variant 2/3: the split is done once per operand into planes in global memory; cp.async moves them
 //   variant 4 (default): persistent, warp-specialised: TMA / cp.async / generating producer warps fill a stage ring
@@ -128,10 +129,17 @@ template <> struct Wgmma<256> {
   }
 };
 // One 64-deep k-block of the split product for the 64 rows of the calling warpgroup: 4 K-steps x
-// (hi*hi + hi*lo + lo*hi), committed as one wgmma group.
+// (hi*hi + hi*lo + lo*hi), committed as one wgmma group.  Stage at `st`: A hi / lo planes (kTM rows), then B hi / lo
+// (BN rows); the warpgroup `wg` reads rows [64 wg, 64 wg + 64) of A, which start 8192 B into the plane in both
+// layouts.  TA / TB (1 = MN-major) are template parameters and the accumulator is not touched between the MMAs and
+// the commit: a control-flow join or a register access there makes ptxas close the group early (it then commits an
+// empty group, and wgmma_wait<1> waits for the k-block just issued).  The caller fences the accumulator
+// (fence_acc) only after wgmma_wait<0>.
 template <int BN, int TA, int TB>
-__device__ __forceinline__ void wg_kblock_t(float (&d)[BN / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
-                                            uint32_t b_lo) {
+__device__ __forceinline__ void wg_kblock(float (&d)[BN / 2], uint32_t st, int wg) {
+  constexpr uint32_t A_PLANE = kTM * 128, B_PLANE = BN * 128;
+  const uint32_t a_hi = st + wg * 8192, a_lo = a_hi + A_PLANE, b_hi = st + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
+  wgmma_fence();
 #pragma unroll
   for (int ks = 0; ks < kTK / 16; ++ks) {
     const uint64_t dah = wgmma_desc_k(a_hi, ks, TA), dal = wgmma_desc_k(a_lo, ks, TA);
@@ -140,24 +148,20 @@ __device__ __forceinline__ void wg_kblock_t(float (&d)[BN / 2], uint32_t a_hi, u
     Wgmma<BN>::template mma<TA, TB>(d, dah, dbl);
     Wgmma<BN>::template mma<TA, TB>(d, dal, dbh);
   }
-}
-// stage at `st`: A hi / lo planes (kTM rows, a_plane bytes each), then B hi / lo (BN rows); the warpgroup `wg`
-// reads rows [64 wg, 64 wg + 64) of A, which start 8192 B into the plane in both layouts.
-template <int BN>
-__device__ __forceinline__ void wg_kblock(float (&d)[BN / 2], uint32_t st, int wg, int a_mn, int b_mn) {
-  constexpr uint32_t A_PLANE = kTM * 128, B_PLANE = BN * 128;
-  const uint32_t a_hi = st + wg * 8192, a_lo = a_hi + A_PLANE, b_hi = st + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
-  fence_acc(d);
-  wgmma_fence();
-  if (a_mn) {
-    if (b_mn) wg_kblock_t<BN, 1, 1>(d, a_hi, a_lo, b_hi, b_lo);
-    else wg_kblock_t<BN, 1, 0>(d, a_hi, a_lo, b_hi, b_lo);
-  } else {
-    if (b_mn) wg_kblock_t<BN, 0, 1>(d, a_hi, a_lo, b_hi, b_lo);
-    else wg_kblock_t<BN, 0, 0>(d, a_hi, a_lo, b_hi, b_lo);
-  }
   wgmma_commit();
-  fence_acc(d);
+}
+// Calls f(Major<a_mn>, Major<b_mn>) with the operand majorness as compile-time constants: the consumer loop is
+// instantiated per layout and the branch runs once per launch, outside every k-block.
+template <int V> struct Major { static constexpr int value = V; };
+template <class F>
+__device__ __forceinline__ void with_majorness(int a_mn, int b_mn, F&& f) {
+  if (a_mn) {
+    if (b_mn) f(Major<1>{}, Major<1>{});
+    else f(Major<1>{}, Major<0>{});
+  } else {
+    if (b_mn) f(Major<0>{}, Major<1>{});
+    else f(Major<0>{}, Major<0>{});
+  }
 }
 
 // Epilogue straight from the accumulator fragment of m64nBN: thread (warp w of the warpgroup, lane l) holds rows
@@ -302,7 +306,7 @@ __global__ void __launch_bounds__(kTcThreads, STAGES == 1 ? 2 : 1) gemm_bf16x3_k
     // make the generic-proxy writes visible to the tensor core (async proxy)
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    wg_kblock<BN>(d, smem_u32(st), wg, 0, 0);
+    wg_kblock<BN, 0, 0>(d, smem_u32(st), wg);
   }
   wgmma_wait<0>();
   fence_acc(d);
@@ -502,17 +506,19 @@ __global__ void __launch_bounds__(kTcThreads, (STAGES * (2 * kTM * 128 + 2 * BN 
     if (s < nkb) load(s);
     asm volatile("cp.async.commit_group;" ::: "memory");
   }
-  for (int kb = 0; kb < nkb; ++kb) {
-    // the slot of k-block kb + STAGES - 1 was last read by k-block kb - 1, retired below
-    if (kb + STAGES - 1 < nkb) load(kb + STAGES - 1);
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group %0;" ::"n"(STAGES - 1) : "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    wg_kblock<BN>(d, smem_u32(tiles + (size_t)(kb % STAGES) * STAGE), wg, g.a_mn, g.b_mn);
-    wgmma_wait<0>();
-    __syncthreads();
-  }
+  with_majorness(g.a_mn, g.b_mn, [&](auto ta, auto tb) {
+    for (int kb = 0; kb < nkb; ++kb) {
+      // the slot of k-block kb + STAGES - 1 was last read by k-block kb - 1, retired below
+      if (kb + STAGES - 1 < nkb) load(kb + STAGES - 1);
+      asm volatile("cp.async.commit_group;" ::: "memory");
+      asm volatile("cp.async.wait_group %0;" ::"n"(STAGES - 1) : "memory");
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      __syncthreads();
+      wg_kblock<BN, decltype(ta)::value, decltype(tb)::value>(d, smem_u32(tiles + (size_t)(kb % STAGES) * STAGE), wg);
+      wgmma_wait<0>();
+      __syncthreads();
+    }
+  });
   asm volatile("cp.async.wait_all;" ::: "memory");
   fence_acc(d);
   store_acc<BN>(g, d, m0 + wg * 64, n0, blockIdx.z);
@@ -551,7 +557,11 @@ struct WsArgs {
   PlaneArgs p;
   int tiles_m, tiles_n;
   int64_t ntiles;
+  int c_tma;          // the epilogue stores C through shared memory with TMA (store_acc_tma) instead of store_acc
 };
+// bytes of one consumer warpgroup's epilogue staging buffer: 64 rows x one 64-column half of the tile, fp32
+template <int BN>
+__host__ __device__ constexpr int ws_staging_bytes() { return 64 * (BN < 64 ? BN : 64) * 4; }
 // ---- TMA (cp.async.bulk.tensor) producer primitives --------------------------------------------------
 // One elected thread arms the stage's mbarrier with the bytes that will land (expect_tx) and issues the
 // tiled bulk copies; the hardware writes the 128-byte-swizzled rows itself (CU_TENSOR_MAP_SWIZZLE_128B is
@@ -567,6 +577,71 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int32_t c0, int32_t c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(src),
+               "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void warpgroup_sync(int wg) {   // named barrier 1 + wg: the 128 threads of one warpgroup
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+}
+
+// Epilogue through shared memory and TMA stores, for C = act(alpha acc + bias) (the same arithmetic as store_acc).
+// The warpgroup's 64 x BN tile leaves in 64-column halves: the 128 threads write a half into the warpgroup's staging
+// buffer as two 32-column x 64-row fp32 boxes in the 128-byte-swizzled layout (16-byte chunk index XOR row % 8: the
+// four rows a half-warp writes hit two bank sets instead of one), then one thread stores the boxes with
+// cp.async.bulk.tensor and the warpgroup returns to the MMAs.  The buffer is rewritten only after the previous
+// store has read it.  TMA clips the boxes at m, but along a row only in 16-byte units, so the map covers the first
+// n4 = n & ~3 columns and the last n - n4 columns of a row are stored from registers: padding columns of C past n
+// stay untouched.
+template <int BN, class G>
+__device__ __forceinline__ void store_acc_tma(const G& g, const float (&d)[BN / 2], const CUtensorMap* map,
+                                              uint32_t stg, int wg, int64_t row0, int64_t n0) {
+  constexpr int HALF = BN < 64 ? BN : 64;
+  const int t = threadIdx.x & 127, lane = t & 31, w = t >> 5;
+  const int64_t n4 = g.n & ~(int64_t)3;
+#pragma unroll
+  for (int hf = 0; hf < BN / HALF; ++hf) {
+    if (t == 0) bulk_wait_read();
+    warpgroup_sync(wg);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = w * 16 + (lane >> 2) + 8 * h;
+#pragma unroll
+      for (int i = hf * HALF / 8; i < (hf + 1) * HALF / 8; ++i) {
+        const int col = 8 * i + 2 * (lane & 3) - hf * HALF;
+        const int64_t gn = n0 + 8 * i + 2 * (lane & 3);
+        float v0 = g.alpha * d[4 * i + 2 * h], v1 = g.alpha * d[4 * i + 2 * h + 1];
+        if (g.bias) {
+          if (gn < g.n) v0 += __ldg(g.bias + gn);
+          if (gn + 1 < g.n) v1 += __ldg(g.bias + gn + 1);
+        }
+        v0 = act_apply(v0, g.act);
+        v1 = act_apply(v1, g.act);
+        const uint32_t off = (col >> 5) * 8192 + r * 128 + ((((col & 31) >> 2) ^ (r & 7)) << 4) + (col & 3) * 4;
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stg + off), "f"(v0), "f"(v1) : "memory");
+        if (gn >= n4 && gn < g.n && row0 + r < g.m) {     // (gn and n4 are even: the pair is all tail or none)
+          float* cp = g.c + (row0 + r) * g.ldc + gn;
+          cp[0] = v0;
+          if (gn + 1 < g.n) cp[1] = v1;
+        }
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    warpgroup_sync(wg);
+    if (t == 0 && row0 < g.m) {
+#pragma unroll
+      for (int b = 0; b < HALF / 32; ++b) {
+        const int64_t c0 = n0 + hf * HALF + 32 * b;
+        if (c0 < n4) tma_store_2d(map, stg + b * 8192, (int32_t)c0, (int32_t)row0);
+      }
+      bulk_commit();
+    }
+  }
 }
 
 // fp32 pair -> bf16 hi pair + bf16 lo pair (v = hi + lo up to 2^-17): two cvt.rn.bf16x2.f32 + four ALU ops
@@ -743,7 +818,7 @@ template <int BN, int STAGES, bool TMA, int GEN = 0, bool FOLD = false>
 __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     gemm_planes_ws_kernel(const __grid_constant__ WsArgs w, const __grid_constant__ CUtensorMap tm_ah,
                           const __grid_constant__ CUtensorMap tm_al, const __grid_constant__ CUtensorMap tm_bh,
-                          const __grid_constant__ CUtensorMap tm_bl) {
+                          const __grid_constant__ CUtensorMap tm_bl, const __grid_constant__ CUtensorMap tm_c) {
   static_assert(BN <= 128, "the consumer accumulator is BN / 2 registers per thread");
   const PlaneArgs& g = w.p;
   constexpr int A_PLANE = kTM * 128;
@@ -1054,102 +1129,120 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
   } else {
     // ------------------------------------------------------------------------------ consumers
     const int wg = warp >> 2;
-    uint32_t it = 0;
-    float d[BN / 2];
-    float dxk[FOLD ? BN / 2 : 1];      // FOLD: this thread's dXk partial sums, same layout as d
-    for (int64_t tile = cta0; tile < w.ntiles; tile += nctas) {
-      int64_t mt, nt, kbeg;
-      int nkb;
-      decode(tile, mt, nt, kbeg, nkb);
-      if (FOLD && nkb == 0) continue;
+    auto consume = [&](auto ta, auto tb) {
+      uint32_t it = 0;
+      float d[BN / 2];
+      [[maybe_unused]] float dxk[FOLD ? BN / 2 : 1];      // FOLD: this thread's dXk partial sums, same layout as d
+      for (int64_t tile = cta0; tile < w.ntiles; tile += nctas) {
+        int64_t mt, nt, kbeg;
+        int nkb;
+        decode(tile, mt, nt, kbeg, nkb);
+        if (FOLD && nkb == 0) continue;
 #pragma unroll
-      for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
-      int prev = -1;
-      for (int kb = 0; kb < nkb; ++kb, ++it) {
-        const int s = it % STAGES;
-        mbar_wait(&full_bar[s], (it / STAGES) & 1);
-        // cp.async producers write through the generic proxy
-        if (!TMA && GEN == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        wg_kblock<BN>(d, smem_u32(tiles + (size_t)s * STAGE), wg, g.a_mn, g.b_mn);
-        wgmma_wait<1>();                 // the group of the previous k-block has retired: release its stage
+        for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const int s = it % STAGES;
+          mbar_wait(&full_bar[s], (it / STAGES) & 1);
+          // cp.async producers write through the generic proxy
+          if (!TMA && GEN == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+          wg_kblock<BN, decltype(ta)::value, decltype(tb)::value>(d, smem_u32(tiles + (size_t)s * STAGE), wg);
+          wgmma_wait<1>();                 // the group of the previous k-block has retired: release its stage
+          if (prev >= 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          }
+          prev = s;
+        }
+        wgmma_wait<0>();
+        fence_acc(d);
         if (prev >= 0) {
           __syncwarp();
           if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
-        prev = s;
-      }
-      wgmma_wait<0>();
-      fence_acc(d);
-      if (prev >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[prev]);
-      }
-      const int64_t row0 = mt * kTM + wg * 64;
-      if constexpr (FOLD) {
-        // CIN backward: the accumulator tile is dZ[r, q] (q = i*hp + j) = dY W'^T and is never stored - it is folded
-        // onto the two factors of the outer product right here:
-        //   dT0[r, i] += sum_j dZ[r, i*hp + j] * xk[r, j]      (quad shuffle + one red.add per row and hp columns)
-        //   dXk[r, j] += sum_i dZ[r, i*hp + j] * t0[r, i]      (registers across the N tiles of the row block,
-        //                                                       red.add once per row block)
-        // BN % hp == 0, so a thread's columns keep their j from tile to tile.
-        if (nt == 0) {
+        const int64_t row0 = mt * kTM + wg * 64;
+        if constexpr (FOLD) {
+          // CIN backward: the accumulator tile is dZ[r, q] (q = i*hp + j) = dY W'^T and is never stored - it is folded
+          // onto the two factors of the outer product right here:
+          //   dT0[r, i] += sum_j dZ[r, i*hp + j] * xk[r, j]      (quad shuffle + one red.add per row and hp columns)
+          //   dXk[r, j] += sum_i dZ[r, i*hp + j] * t0[r, i]      (registers across the N tiles of the row block,
+          //                                                       red.add once per row block)
+          // BN % hp == 0, so a thread's columns keep their j from tile to tile.
+          if (nt == 0) {
 #pragma unroll
-          for (int j = 0; j < BN / 2; ++j) dxk[j] = 0.f;
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int64_t gm = row0 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
-          const bool row_ok = gm < g.m;
-          const float* t0 = g.cin_t0 + (row_ok ? gm : 0) * g.cin_ld0;
-          const float* xk = g.cin_xk + (row_ok ? gm : 0) * g.cin_ldk;
-          float p = 0.f;
-#pragma unroll
-          for (int i = 0; i < BN / 8; ++i) {
-            const int c = 8 * i + 2 * (lane & 3);
-            const int64_t q = nt * BN + c;
-            const int ic = (int)(q / g.cin_hp), j = (int)(q - (int64_t)ic * g.cin_hp);
-            const bool ok = row_ok && ic < g.cin_m;
-            const float a = ok ? __ldg(t0 + ic) : 0.f;
-            const float x0 = ok && j < g.cin_h ? __ldg(xk + j) : 0.f;
-            const float x1 = ok && j + 1 < g.cin_h ? __ldg(xk + j + 1) : 0.f;
-            const float d0 = d[4 * i + 2 * h], d1 = d[4 * i + 2 * h + 1];
-            p += d0 * x0 + d1 * x1;
-            dxk[4 * i + 2 * h] += d0 * a;
-            dxk[4 * i + 2 * h + 1] += d1 * a;
-            if ((8 * (i + 1)) % g.cin_hp == 0) {     // last 8 columns of the hp-wide group of output i (warp-uniform)
-              p += __shfl_xor_sync(0xffffffffu, p, 1);
-              p += __shfl_xor_sync(0xffffffffu, p, 2);
-              if ((lane & 3) == 0 && ok) red_add_f1(g.fold_dt0 + gm * g.cin_ld0 + ic, p);
-              p = 0.f;
-            }
+            for (int j = 0; j < BN / 2; ++j) dxk[j] = 0.f;
           }
-          if (nt == w.tiles_n - 1 && row_ok) {
-            float* dst = g.fold_dxk + gm * g.fold_ldx;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int64_t gm = row0 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+            const bool row_ok = gm < g.m;
+            const float* t0 = g.cin_t0 + (row_ok ? gm : 0) * g.cin_ld0;
+            const float* xk = g.cin_xk + (row_ok ? gm : 0) * g.cin_ldk;
+            float p = 0.f;
 #pragma unroll
             for (int i = 0; i < BN / 8; ++i) {
-              const int j = (8 * i + 2 * (lane & 3)) % g.cin_hp;
-              if (j < g.cin_h) red_add_f1(dst + j, dxk[4 * i + 2 * h]);
-              if (j + 1 < g.cin_h) red_add_f1(dst + j + 1, dxk[4 * i + 2 * h + 1]);
+              const int c = 8 * i + 2 * (lane & 3);
+              const int64_t q = nt * BN + c;
+              const int ic = (int)(q / g.cin_hp), j = (int)(q - (int64_t)ic * g.cin_hp);
+              const bool ok = row_ok && ic < g.cin_m;
+              const float a = ok ? __ldg(t0 + ic) : 0.f;
+              const float x0 = ok && j < g.cin_h ? __ldg(xk + j) : 0.f;
+              const float x1 = ok && j + 1 < g.cin_h ? __ldg(xk + j + 1) : 0.f;
+              const float d0 = d[4 * i + 2 * h], d1 = d[4 * i + 2 * h + 1];
+              p += d0 * x0 + d1 * x1;
+              dxk[4 * i + 2 * h] += d0 * a;
+              dxk[4 * i + 2 * h + 1] += d1 * a;
+              if ((8 * (i + 1)) % g.cin_hp == 0) {     // last 8 columns of the hp-wide group of output i (warp-uniform)
+                p += __shfl_xor_sync(0xffffffffu, p, 1);
+                p += __shfl_xor_sync(0xffffffffu, p, 2);
+                if ((lane & 3) == 0 && ok) red_add_f1(g.fold_dt0 + gm * g.cin_ld0 + ic, p);
+                p = 0.f;
+              }
+            }
+            if (nt == w.tiles_n - 1 && row_ok) {
+              float* dst = g.fold_dxk + gm * g.fold_ldx;
+#pragma unroll
+              for (int i = 0; i < BN / 8; ++i) {
+                const int j = (8 * i + 2 * (lane & 3)) % g.cin_hp;
+                if (j < g.cin_h) red_add_f1(dst + j, dxk[4 * i + 2 * h]);
+                if (j + 1 < g.cin_h) red_add_f1(dst + j + 1, dxk[4 * i + 2 * h + 1]);
+              }
             }
           }
+        } else if (w.c_tma) {
+          store_acc_tma<BN>(g, d, &tm_c, smem_u32(tiles + STAGES * STAGE + wg * ws_staging_bytes<BN>()), wg, row0,
+                            nt * BN);
+        } else {
+          const int64_t z = tile / ((int64_t)w.tiles_n * w.tiles_m);
+          store_acc<BN>(g, d, row0, nt * BN, z);
         }
-      } else {
-        const int64_t z = tile / ((int64_t)w.tiles_n * w.tiles_m);
-        store_acc<BN>(g, d, row0, nt * BN, z);
       }
+      if (!FOLD && w.c_tma && (threadIdx.x & 127) == 0) bulk_wait_all();   // the last stores have left the CTA
+    };
+    // only the layouts a launch can ask for: the CIN fold reads both operands K-major, the generated-A kernels read
+    // MN-major B planes, and an MN-major B tile is at least one 64-wide atom
+    if constexpr (FOLD) consume(Major<0>{}, Major<0>{});
+    else if constexpr (GEN != 0) {
+      if (g.a_mn) consume(Major<1>{}, Major<1>{});
+      else consume(Major<0>{}, Major<1>{});
+    } else if constexpr (BN < 64) {
+      if (g.a_mn) consume(Major<1>{}, Major<0>{});
+      else consume(Major<0>{}, Major<0>{});
+    } else {
+      with_majorness(g.a_mn, g.b_mn, consume);
     }
   }
 }
 
 struct TmaMaps {
-  CUtensorMap ah, al, bh, bl;
+  CUtensorMap ah, al, bh, bl, c;
   bool ok;
 };
 
 template <int BN, int STAGES, bool TMA, int GEN = 0, bool FOLD = false>
 static cudaError_t launch_ws_impl(const WsArgs& wa, const TmaMaps& tm, cudaStream_t st) {
-  constexpr size_t smem = (size_t)STAGES * (2 * kTM * 128 + 2 * BN * 128) + 1024;
-  static_assert(smem + 256 <= 227 * 1024, "stage ring exceeds shared memory");
+  constexpr size_t smem = (size_t)STAGES * (2 * kTM * 128 + 2 * BN * 128) + 2 * ws_staging_bytes<BN>() + 1024;
+  static_assert(smem + 256 <= 227 * 1024, "stage ring + epilogue staging exceed shared memory");
   auto kern = gemm_planes_ws_kernel<BN, STAGES, TMA, GEN, FOLD>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
@@ -1159,7 +1252,7 @@ static cudaError_t launch_ws_impl(const WsArgs& wa, const TmaMaps& tm, cudaStrea
     nctas = wa.tiles_m < kNumSMs ? wa.tiles_m : kNumSMs;
     wcopy.ntiles = ceil_div(wa.tiles_m, nctas) * wa.tiles_n * nctas;
   }
-  kern<<<(unsigned)nctas, WsLayout<GEN != 0>::kThreads, smem, st>>>(wcopy, tm.ah, tm.al, tm.bh, tm.bl);
+  kern<<<(unsigned)nctas, WsLayout<GEN != 0>::kThreads, smem, st>>>(wcopy, tm.ah, tm.al, tm.bh, tm.bl, tm.c);
   return cudaGetLastError();
 }
 template <int BN, int STAGES>
@@ -1201,6 +1294,23 @@ static bool tma_map_2d(CUtensorMap* m, const void* base, int64_t inner, int64_t 
   return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// C tensor map for the TMA-store epilogue (store_acc_tma): fp32 [m, n & ~3] with ldc elements between rows, box
+// 32 x 64 with 128-byte swizzle.  Only plain stores qualify: split-K slices go to the workspace, accumulate reads C,
+// and TMA needs a 16-byte aligned base and row pitch.  Returns whether wa.c_tma may be set.
+static bool tma_map_c(CUtensorMap* m, const PlaneArgs& p) {
+  EncodeTiledFn enc = tma_encoder();
+  if (!enc || p.splits > 1 || p.accumulate || !p.c || ((uintptr_t)p.c & 15) || p.ldc % 4 || p.ldc < p.n ||
+      p.n < 4 || p.m >= (1ll << 31) || p.n >= (1ll << 31))
+    return false;
+  cuuint64_t dims[2] = {(cuuint64_t)(p.n & ~(int64_t)3), (cuuint64_t)p.m};
+  cuuint64_t strides[1] = {(cuuint64_t)p.ldc * 4};
+  cuuint32_t box[2] = {32, 64};
+  cuuint32_t estr[2] = {1, 1};
+  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, p.c, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) ==
+         CUDA_SUCCESS;
 }
 
 static inline int64_t round_up(int64_t v, int64_t q) { return (v + q - 1) / q * q; }
@@ -1317,11 +1427,12 @@ static b2ctr_status_t gemm_planes(const b2ctr_gemm_t* g, void* workspace, size_t
     wa.tiles_n = (int)ceil_div(g->n, bn);
     wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n * splits;
     // TMA producers: four tiled tensor maps over the operand planes (box = one stage's slice of a plane)
-    TmaMaps tm;
+    TmaMaps tm{};
     tm.ok = tma_map_2d(&tm.ah, a_hi, a_pitch, a_prows, a_pitch, 64, a_mn ? 64 : kTM) &&
             tma_map_2d(&tm.al, a_lo, a_pitch, a_prows, a_pitch, 64, a_mn ? 64 : kTM) &&
             tma_map_2d(&tm.bh, b_hi, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bn) &&
             tma_map_2d(&tm.bl, b_lo, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bn);
+    wa.c_tma = tm.ok && tma_map_c(&tm.c, pa);
     if (bn == 32) e = launch_ws<32, 5>(wa, tm, st);
     else if (bn == 64) e = launch_ws<64, 4>(wa, tm, st);
     else e = launch_ws<128, 3>(wa, tm, st);
@@ -1447,13 +1558,14 @@ static b2ctr_status_t gen_gemm(const GenSpec& sp, int mode, int64_t n, const voi
   wa.tiles_m = (int)ceil_div(pa.m, (int64_t)kTM);
   wa.tiles_n = (int)ceil_div(n, bn);
   wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n * splits;
-  TmaMaps tm;
+  TmaMaps tm{};
   tm.ok = tma_map_2d(&tm.bh, pa.b_hi, cp, b_prows, cp, 64, 64) && tma_map_2d(&tm.bl, pa.b_lo, cp, b_prows, cp, 64, 64);
   if (!tm.ok) {
     set_error("%s: cuTensorMapEncodeTiled unavailable (the kernel loads its B operand by TMA)", what);
     return B2CTR_ERR_UNSUPPORTED;
   }
   tm.ah = tm.bh; tm.al = tm.bl;
+  wa.c_tma = tma_map_c(&tm.c, pa);
   const cudaError_t e = sp.kind == 1 ? launch_gen<1>(wa, tm, bn, st) : launch_gen<2>(wa, tm, bn, st);
   if (e != cudaSuccess) {
     set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e));
@@ -1518,13 +1630,14 @@ b2ctr_status_t cin_fold(const b2ctr_cin_gemm_t* g, float* dt0, float* dxk, int64
   wa.tiles_m = (int)ceil_div(g->rows, (int64_t)kTM);
   wa.tiles_n = (int)ceil_div(kq, bn);
   wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n;
-  TmaMaps tm;
+  TmaMaps tm{};
   tm.ok = tma_map_2d(&tm.ah, pa.a_hi, cpn, a_prows, cpn, 64, kTM) && tma_map_2d(&tm.al, pa.a_lo, cpn, a_prows, cpn, 64, kTM) &&
           tma_map_2d(&tm.bh, pa.b_hi, cpn, b_prows, cpn, 64, bn) && tma_map_2d(&tm.bl, pa.b_lo, cpn, b_prows, cpn, 64, bn);
   if (!tm.ok) {
     set_error("cin_fold: cuTensorMapEncodeTiled unavailable");
     return B2CTR_ERR_UNSUPPORTED;
   }
+  wa.c_tma = 0;      // the fold epilogue never stores the accumulator tile
   cudaError_t e = launch_ws_impl<128, 3, true, 0, true>(wa, tm, st);
   if (e != cudaSuccess) {
     set_error("b2ctr_cin_fold: CUDA launch failed: %s", cudaGetErrorString(e));
