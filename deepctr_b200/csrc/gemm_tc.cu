@@ -150,6 +150,30 @@ __device__ __forceinline__ void wg_kblock(float (&d)[BN / 2], uint32_t st, int w
   }
   wgmma_commit();
 }
+// Half a k-block (K-steps KS0, KS0 + 1) of the split product for all 128 rows of the tile, from ONE warpgroup (the
+// ping-pong consumers): 12 wgmma committed as one group, alternating between the accumulators of the two 64-row
+// halves so that consecutive MMAs do not depend on each other.  Each accumulator sees its K-steps and the three
+// products in wg_kblock's order, so the sums are bit-identical.  (Issuing one half's 12 dependent MMAs and then the
+// other's halves the tensor-pipe throughput.)
+template <int BN, int TA, int TB, int KS0>
+__device__ __forceinline__ void tile_kblock_half(float (&d0)[BN / 2], float (&d1)[BN / 2], uint32_t st) {
+  constexpr uint32_t A_PLANE = kTM * 128, B_PLANE = BN * 128;
+  const uint32_t a_hi = st, a_lo = a_hi + A_PLANE, b_hi = st + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
+  wgmma_fence();
+#pragma unroll
+  for (int ks = KS0; ks < KS0 + 2; ++ks) {
+    const uint64_t dah0 = wgmma_desc_k(a_hi, ks, TA), dal0 = wgmma_desc_k(a_lo, ks, TA);
+    const uint64_t dah1 = wgmma_desc_k(a_hi + 8192, ks, TA), dal1 = wgmma_desc_k(a_lo + 8192, ks, TA);
+    const uint64_t dbh = wgmma_desc_k(b_hi, ks, TB), dbl = wgmma_desc_k(b_lo, ks, TB);
+    Wgmma<BN>::template mma<TA, TB>(d0, dah0, dbh);
+    Wgmma<BN>::template mma<TA, TB>(d1, dah1, dbh);
+    Wgmma<BN>::template mma<TA, TB>(d0, dah0, dbl);
+    Wgmma<BN>::template mma<TA, TB>(d1, dah1, dbl);
+    Wgmma<BN>::template mma<TA, TB>(d0, dal0, dbh);
+    Wgmma<BN>::template mma<TA, TB>(d1, dal1, dbh);
+  }
+  wgmma_commit();
+}
 // Calls f(Major<a_mn>, Major<b_mn>) with the operand majorness as compile-time constants: the consumer loop is
 // instantiated per layout and the branch runs once per launch, outside every k-block.
 template <int V> struct Major { static constexpr int value = V; };
@@ -538,9 +562,15 @@ static cudaError_t launch_planes(const PlaneArgs& pa, cudaStream_t st) {
 
 // ================================================================================================
 // Variant 4: persistent, warp-specialised planes GEMM.
-//   warps 0-7  : two consumer warpgroups.  Each waits for a full stage, issues the 12 wgmma of the k-block on
-//                its 64 rows of the tile, keeps one wgmma group in flight and hands the previous stage back to
-//                the producers; after the last k-block of a tile it runs the epilogue from its registers.
+//   warps 0-7  : two consumer warpgroups.  Plain GEMMs (GEN = 0, no FOLD) run them PING-PONG: warpgroup j % 2 owns
+//                the whole j-th tile of the CTA (both 64-row halves, two accumulators) and the two alternate, so one
+//                warpgroup's epilogue runs while the other issues its MMAs.  Per k-block a warpgroup waits for the
+//                full stage, issues its 24 wgmma as two groups of 12 (K-steps 0-1, then 2-3, each alternating
+//                between the two halves' accumulators), keeps one group in flight and hands a stage back to the
+//                producers once both groups have retired.  Named barriers order the MMA phases: a warpgroup starts
+//                a tile only after the other one has issued the previous tile's last k-block.  The generated-operand and FOLD kernels stay COOPERATIVE: each warpgroup owns 64 rows of
+//                every tile and both run the epilogue together (their producers / fold leave no registers for a
+//                second accumulator).
 //   producers  : TMA (default): one elected thread arms the stage barrier and issues cp.async.bulk.tensor.2d loads
 //                of the four plane slices.  GEN = 1 / 2: eight warps GENERATE the A tile in shared memory (CIN outer
 //                product / DIN attention input) while B arrives by TMA.  B2CTR_TC_TMA=0: four warps of 16-byte
@@ -548,7 +578,8 @@ static cudaError_t launch_planes(const PlaneArgs& pa, cudaStream_t st) {
 // The producers run up to STAGES k-blocks ahead, across tile boundaries: the next tile's operands load while the
 // consumers run the epilogue of the current one.
 // Persistent: grid = min(#tiles, #SMs); tile = CTA id + j * #CTAs, N-tile fastest (neighbouring CTAs share the
-// A rows through L2).  BN <= 128: the m64n128 accumulator is 64 registers per consumer thread.
+// A rows through L2).  BN <= 128: an m64n128 accumulator is 64 registers per consumer thread; ping-pong consumers
+// hold two, so those kernels move registers from the producer warpgroup to them with setmaxnreg.
 // ================================================================================================
 constexpr int kWsConsumerWarps = 8;
 constexpr int kWsProducers = 4;   // warps
@@ -589,6 +620,15 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 __device__ __forceinline__ void warpgroup_sync(int wg) {   // named barrier 1 + wg: the 128 threads of one warpgroup
   asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
 }
+// Ping-pong order of the two consumer warpgroups' MMA phases: named barrier 3 + wg is passed when warpgroup wg waits
+// on it (128 threads) and the other warpgroup has arrived (128 threads).
+__device__ __forceinline__ void mma_order_wait(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(3 + wg) : "memory"); }
+__device__ __forceinline__ void mma_order_arrive(int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(3 + wg) : "memory"); }
+// Per-warpgroup register budgets (multiples of 8; all warps of the warpgroup execute them)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // Epilogue through shared memory and TMA stores, for C = act(alpha acc + bias) (the same arithmetic as store_acc).
 // The warpgroup's 64 x BN tile leaves in 64-column halves: the 128 threads write a half into the warpgroup's staging
@@ -598,36 +638,48 @@ __device__ __forceinline__ void warpgroup_sync(int wg) {   // named barrier 1 + 
 // store has read it.  TMA clips the boxes at m, but along a row only in 16-byte units, so the map covers the first
 // n4 = n & ~3 columns and the last n - n4 columns of a row are stored from registers: padding columns of C past n
 // stay untouched.
-template <int BN, class G>
-__device__ __forceinline__ void store_acc_tma(const G& g, const float (&d)[BN / 2], const CUtensorMap* map,
-                                              uint32_t stg, int wg, int64_t row0, int64_t n0) {
+// The activation is a template parameter (ACT < 0: g.act at run time) and the checks that are uniform over the
+// tile are taken outside the element loop, so the loop is straight-line code: with one warp per SM sub-partition
+// the epilogue is bound by instruction latency, not by shared-memory or store bandwidth.
+template <int BN, int ACT, class G>
+__device__ __forceinline__ void store_acc_tma_act(const G& g, const float (&d)[BN / 2], const CUtensorMap* map,
+                                                  uint32_t stg, int wg, int64_t row0, int64_t n0) {
   constexpr int HALF = BN < 64 ? BN : 64;
   const int t = threadIdx.x & 127, lane = t & 31, w = t >> 5;
   const int64_t n4 = g.n & ~(int64_t)3;
+  const bool tail = n0 + BN > n4;       // the tile holds columns past the map (stored from registers)
+  const float* bias = g.bias;
+  const float alpha = g.alpha;
 #pragma unroll
   for (int hf = 0; hf < BN / HALF; ++hf) {
     if (t == 0) bulk_wait_read();
     warpgroup_sync(wg);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r = w * 16 + (lane >> 2) + 8 * h;
+    for (int i = hf * HALF / 8; i < (hf + 1) * HALF / 8; ++i) {
+      const int col = 8 * i + 2 * (lane & 3) - hf * HALF;
+      const int64_t gn = n0 + 8 * i + 2 * (lane & 3);
+      const bool in0 = gn < g.n, in1 = gn + 1 < g.n;
+      float b0 = 0.f, b1 = 0.f;
+      if (bias) {
+        if (in0) b0 = __ldg(bias + gn);
+        if (in1) b1 = __ldg(bias + gn + 1);
+      }
 #pragma unroll
-      for (int i = hf * HALF / 8; i < (hf + 1) * HALF / 8; ++i) {
-        const int col = 8 * i + 2 * (lane & 3) - hf * HALF;
-        const int64_t gn = n0 + 8 * i + 2 * (lane & 3);
-        float v0 = g.alpha * d[4 * i + 2 * h], v1 = g.alpha * d[4 * i + 2 * h + 1];
-        if (g.bias) {
-          if (gn < g.n) v0 += __ldg(g.bias + gn);
-          if (gn + 1 < g.n) v1 += __ldg(g.bias + gn + 1);
+      for (int h = 0; h < 2; ++h) {
+        const int r = w * 16 + (lane >> 2) + 8 * h;
+        float v0 = __fmul_rn(alpha, d[4 * i + 2 * h]), v1 = __fmul_rn(alpha, d[4 * i + 2 * h + 1]);
+        if (bias) {
+          if (in0) v0 = __fadd_rn(v0, b0);
+          if (in1) v1 = __fadd_rn(v1, b1);
         }
-        v0 = act_apply(v0, g.act);
-        v1 = act_apply(v1, g.act);
+        v0 = act_apply(v0, ACT < 0 ? g.act : ACT);
+        v1 = act_apply(v1, ACT < 0 ? g.act : ACT);
         const uint32_t off = (col >> 5) * 8192 + r * 128 + ((((col & 31) >> 2) ^ (r & 7)) << 4) + (col & 3) * 4;
         asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stg + off), "f"(v0), "f"(v1) : "memory");
-        if (gn >= n4 && gn < g.n && row0 + r < g.m) {     // (gn and n4 are even: the pair is all tail or none)
+        if (tail && gn >= n4 && in0 && row0 + r < g.m) {     // (gn and n4 are even: the pair is all tail or none)
           float* cp = g.c + (row0 + r) * g.ldc + gn;
           cp[0] = v0;
-          if (gn + 1 < g.n) cp[1] = v1;
+          if (in1) cp[1] = v1;
         }
       }
     }
@@ -642,6 +694,13 @@ __device__ __forceinline__ void store_acc_tma(const G& g, const float (&d)[BN / 
       bulk_commit();
     }
   }
+}
+template <int BN, class G>
+__device__ __forceinline__ void store_acc_tma(const G& g, const float (&d)[BN / 2], const CUtensorMap* map,
+                                              uint32_t stg, int wg, int64_t row0, int64_t n0) {
+  if (g.act == B2CTR_ACT_NONE) store_acc_tma_act<BN, B2CTR_ACT_NONE>(g, d, map, stg, wg, row0, n0);
+  else if (g.act == B2CTR_ACT_RELU) store_acc_tma_act<BN, B2CTR_ACT_RELU>(g, d, map, stg, wg, row0, n0);
+  else store_acc_tma_act<BN, -1>(g, d, map, stg, wg, row0, n0);
 }
 
 // fp32 pair -> bf16 hi pair + bf16 lo pair (v = hi + lo up to 2^-17): two cvt.rn.bf16x2.f32 + four ALU ops
@@ -820,6 +879,7 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
                           const __grid_constant__ CUtensorMap tm_al, const __grid_constant__ CUtensorMap tm_bh,
                           const __grid_constant__ CUtensorMap tm_bl, const __grid_constant__ CUtensorMap tm_c) {
   static_assert(BN <= 128, "the consumer accumulator is BN / 2 registers per thread");
+  constexpr bool PINGPONG = GEN == 0 && !FOLD;
   const PlaneArgs& g = w.p;
   constexpr int A_PLANE = kTM * 128;
   constexpr int B_PLANE = BN * 128;
@@ -836,7 +896,8 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
       // cp.async producers: one deferred arrival per producer thread; TMA: one arrive.expect_tx
       // generated A: one arrival per generating thread of the stage + the TMA expect_tx of the B planes
       mbar_init(&full_bar[s], GEN != 0 ? 1 + (g.gen_groups == 2 ? 128 : 256) : (TMA ? 1 : kWsProducers * 32));
-      mbar_init(&empty_bar[s], kWsConsumerWarps);
+      // a stage is released by every consumer warp (cooperative) or by the four warps of the tile's owner (ping-pong)
+      mbar_init(&empty_bar[s], PINGPONG ? kWsConsumerWarps / 2 : kWsConsumerWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -1022,6 +1083,7 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     // one elected lane: wait for a free stage, arm its barrier with the stage bytes, issue the bulk tensor copies
     // of the four operand planes.  Data moves global -> swizzled shared memory inside the async proxy, where
     // wgmma reads it.
+    if constexpr (PINGPONG) setmaxnreg_dec<56>();
     if (warp == kWsConsumerWarps && lane == 0) {
       tma_prefetch_desc(&tm_ah); tma_prefetch_desc(&tm_al); tma_prefetch_desc(&tm_bh); tma_prefetch_desc(&tm_bl);
       uint32_t it = 0;
@@ -1063,6 +1125,7 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     }
   } else if (warp >= kWsConsumerWarps) {
     // ------------------------------------------------------------------------------ producers
+    if constexpr (PINGPONG) setmaxnreg_dec<56>();
     const int tid = threadIdx.x - kWsConsumerWarps * 32;
     constexpr int NT = kWsProducers * 32;
     int64_t tile = cta0, mt = 0, nt = 0, kbeg = 0;
@@ -1129,6 +1192,64 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
   } else {
     // ------------------------------------------------------------------------------ consumers
     const int wg = warp >> 2;
+    // Ping-pong: warpgroup wg owns the tiles j (of this CTA) with j % 2 == wg and issues each k-block as two groups
+    // of 12 wgmma over both 64-row halves (tile_kblock_half): every output element sees the same MMAs in the same
+    // order as in the cooperative loop.  Both warpgroups count every k-block of the CTA (`it`), so the
+    // stage ring is walked in the producers' order.  The order barrier also keeps a warpgroup from waiting on a
+    // full barrier whose previous phase the other warpgroup has not consumed yet (parity waits see only one phase).
+    auto pingpong = [&](auto ta, auto tb) {
+      constexpr int TA = decltype(ta)::value, TB = decltype(tb)::value;
+      const uint32_t stg = smem_u32(tiles + STAGES * STAGE + wg * ws_staging_bytes<BN>());
+      uint32_t it = 0;
+      float d0[BN / 2], d1[BN / 2];
+      int64_t j = 0;
+      for (int64_t tile = cta0; tile < w.ntiles; tile += nctas, ++j) {
+        int64_t mt, nt, kbeg;
+        int nkb;
+        decode(tile, mt, nt, kbeg, nkb);
+        if ((j & 1) != wg) {
+          it += nkb;
+          continue;
+        }
+        if (j > 0) mma_order_wait(wg);          // the other warpgroup has issued the last k-block of tile j - 1
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) d0[i] = d1[i] = 0.f;
+        int prev = -1;
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const int s = it % STAGES;
+          mbar_wait(&full_bar[s], (it / STAGES) & 1);
+          if (!TMA) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async wrote it
+          const uint32_t st = smem_u32(tiles + (size_t)s * STAGE);
+          tile_kblock_half<BN, TA, TB, 0>(d0, d1, st);
+          wgmma_wait<1>();                      // the previous k-block has retired: release its stage
+          if (prev >= 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          }
+          tile_kblock_half<BN, TA, TB, 2>(d0, d1, st);
+          wgmma_wait<1>();
+          prev = s;
+        }
+        if (tile + nctas < w.ntiles) mma_order_arrive(wg ^ 1);
+        wgmma_wait<0>();
+        fence_acc(d0);
+        fence_acc(d1);
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        const int64_t row0 = mt * kTM;
+        if (w.c_tma) {
+          store_acc_tma<BN>(g, d0, &tm_c, stg, wg, row0, nt * BN);
+          store_acc_tma<BN>(g, d1, &tm_c, stg, wg, row0 + 64, nt * BN);
+        } else {
+          const int64_t z = tile / ((int64_t)w.tiles_n * w.tiles_m);
+          store_acc<BN>(g, d0, row0, nt * BN, z);
+          store_acc<BN>(g, d1, row0 + 64, nt * BN, z);
+        }
+      }
+      if (w.c_tma && (threadIdx.x & 127) == 0) bulk_wait_all();   // the last stores have left the CTA
+    };
     auto consume = [&](auto ta, auto tb) {
       uint32_t it = 0;
       float d[BN / 2];
@@ -1144,8 +1265,6 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
         for (int kb = 0; kb < nkb; ++kb, ++it) {
           const int s = it % STAGES;
           mbar_wait(&full_bar[s], (it / STAGES) & 1);
-          // cp.async producers write through the generic proxy
-          if (!TMA && GEN == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
           wg_kblock<BN, decltype(ta)::value, decltype(tb)::value>(d, smem_u32(tiles + (size_t)s * STAGE), wg);
           wgmma_wait<1>();                 // the group of the previous k-block has retired: release its stage
           if (prev >= 0) {
@@ -1225,11 +1344,14 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     else if constexpr (GEN != 0) {
       if (g.a_mn) consume(Major<1>{}, Major<1>{});
       else consume(Major<0>{}, Major<1>{});
-    } else if constexpr (BN < 64) {
-      if (g.a_mn) consume(Major<1>{}, Major<0>{});
-      else consume(Major<0>{}, Major<0>{});
     } else {
-      with_majorness(g.a_mn, g.b_mn, consume);
+      setmaxnreg_inc<224>();       // two accumulators: 56 (producers) x 128 + 224 x 256 threads = 384 x 168 registers
+      if constexpr (BN < 64) {
+        if (g.a_mn) pingpong(Major<1>{}, Major<0>{});
+        else pingpong(Major<0>{}, Major<0>{});
+      } else {
+        with_majorness(g.a_mn, g.b_mn, pingpong);
+      }
     }
   }
 }
