@@ -150,6 +150,12 @@ SIGNATURES = {
     "b2ctr_interacting_fwd": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),
     "b2ctr_interacting_bwd": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32,
                                      _i32, _vp]),
+    "b2ctr_bi_interaction_fwd": (_i32, [_vp, _i64, _i32, _i32, _vp, _i64, _i64, _vp]),
+    "b2ctr_bi_interaction_bwd": (_i32, [_vp, _i64, _i32, _i32, _vp, _i64, _vp, _i64, _i64, _vp]),
+    "b2ctr_afm_fwd": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp]),
+    "b2ctr_afm_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
+    "b2ctr_afm_bwd": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64,
+                             _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
     "b2ctr_din_att_input_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),
     "b2ctr_din_att_input_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _vp]),
     "b2ctr_din_pool_fwd": (_i32, [_vp, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),

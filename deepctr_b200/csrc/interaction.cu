@@ -308,6 +308,431 @@ __global__ void __launch_bounds__(128)
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// BiInteractionPooling (deepctr/layers/interaction.py:196-201): one warp per sample, lanes over e.
+//   out[b, e] = 0.5 * ((sum_f x)^2 - sum_f x^2);   dx[b, f, e] = g[b, e] * (S[b, e] - x[b, f, e])
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+    bi_interaction_fwd_kernel(const float* __restrict__ x, int64_t ldx, int nfield, int dim, float* out,
+                              int64_t ldo, int64_t batch) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); b < batch; b += nw) {
+    const float* xr = x + b * ldx;
+    for (int e = lane; e < dim; e += 32) {
+      float s = 0.f, q = 0.f;
+      for (int f = 0; f < nfield; ++f) {
+        const float v = xr[f * dim + e];
+        s += v;
+        q += v * v;
+      }
+      out[b * ldo + e] = 0.5f * (s * s - q);
+    }
+  }
+}
+__global__ void __launch_bounds__(256)
+    bi_interaction_bwd_kernel(const float* __restrict__ x, int64_t ldx, int nfield, int dim,
+                              const float* __restrict__ g, int64_t ldg, float* dx, int64_t lddx, int64_t batch) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); b < batch; b += nw) {
+    const float* xr = x + b * ldx;
+    float* dr = dx + b * lddx;
+    for (int e = lane; e < dim; e += 32) {
+      const float ge = g[b * ldg + e];
+      float s = 0.f;
+      for (int f = 0; f < nfield; ++f) s += xr[f * dim + e];
+      for (int f = 0; f < nfield; ++f) dr[f * dim + e] = ge * (s - xr[f * dim + e]);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// AFMLayer attention pooling (deepctr/layers/interaction.py:122-141), the pairwise products generated on
+// chip.  For the P = F(F-1)/2 pairs p = (i < j) of a sample, in itertools.combinations order:
+//   prod_p = x_i * x_j  [E];  s_p = h . relu(W^T prod_p + bias);  alpha = softmax_p(s);  att = sum_p alpha_p prod_p
+// One warp per sample, one lane per pair (lanes stride the pair list), the sample's [F, E] rows staged in
+// shared memory with a padded pitch.  Neither prod [B,P,E] nor the hidden layer [B,P,A] ever exists.
+// E and A are padded to the template sizes EP (4/8/16/32) and AP (1/2/4/8/16) with zero weights: a padded
+// column of x / row of W / entry of bias and h contributes exactly 0 to every sum.
+// Forward: online softmax per lane, merged across the warp; the per-sample state (max, sum) is saved.
+// Backward: with sum_q alpha_q d alpha_q = <g, att>, ds_p = alpha_p (<g, prod_p> - <g, att>) needs one pass.
+//   Lanes handle 32 pairs per round and park (prod, d prod, d t, ds*hidden) of the round in shared memory;
+//   every output element then has ONE owner lane that adds the round's terms in a fixed order: dx[f, e] the
+//   lane (e, f mod 32/EP), dW[e, a] the lane (e*AP + a) mod 32, dbias / dh lane a.  Per-CTA weight partials
+//   are summed in a fixed order by afm_reduce_kernel: no float atomics, bit-identical from run to run.
+// ------------------------------------------------------------------------------------------------
+constexpr int kAfmWarps = 4;
+constexpr int kAfmMaxF = 64;
+constexpr int kAfmMaxE = 32;
+constexpr int kAfmMaxA = 16;
+
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// shared header of both AFM kernels: zero-padded W^T [AP][EP] (16-byte rows: float4 broadcast reads), bias [AP],
+// h [AP] and the pair list (i << 8 | j)
+template <int EP, int AP>
+__device__ __forceinline__ int afm_load_header(float* sm, const float* __restrict__ W, const float* __restrict__ bias,
+                                               const float* __restrict__ h, int F, int E, int A) {
+  float* sW = sm;
+  float* sb = sW + EP * AP;
+  float* sh = sb + AP;
+  int* spair = (int*)(sh + AP);
+  for (int k = threadIdx.x; k < EP * AP; k += blockDim.x) {
+    const int a = k / EP, e = k - a * EP;
+    sW[k] = (e < E && a < A) ? W[e * A + a] : 0.f;
+  }
+  for (int a = threadIdx.x; a < AP; a += blockDim.x) {
+    sb[a] = a < A ? bias[a] : 0.f;
+    sh[a] = a < A ? h[a] : 0.f;
+  }
+  const int P = F * (F - 1) / 2;
+  for (int p = threadIdx.x; p < P; p += blockDim.x) {
+    int i = 0, off = 0;
+    while (off + (F - 1 - i) <= p) { off += F - 1 - i; ++i; }
+    spair[p] = (i << 8) | (i + 1 + p - off);
+  }
+  return P;
+}
+template <int EP, int AP>
+__host__ __device__ constexpr int afm_header_floats() { return EP * AP + 2 * AP + kAfmMaxF * (kAfmMaxF - 1) / 2; }
+
+// <prod, W[:, a]> over the padded embedding axis (the a-loops stay rolled: unrolled, ptxas keeps all of W^T in
+// registers and spills)
+template <int EP>
+__device__ __forceinline__ float afm_dot(const float (&pr)[EP], const float* __restrict__ wa) {
+  float t = 0.f;
+#pragma unroll
+  for (int e = 0; e < EP; e += 4) {
+    const float4 w = *reinterpret_cast<const float4*>(wa + e);
+    t = fmaf(pr[e], w.x, t);
+    t = fmaf(pr[e + 1], w.y, t);
+    t = fmaf(pr[e + 2], w.z, t);
+    t = fmaf(pr[e + 3], w.w, t);
+  }
+  return t;
+}
+
+// [F, E] rows of sample b -> padded [F, EP + 1] tile (columns >= E stay zero from the initial fill)
+template <int EP>
+__device__ __forceinline__ void afm_stage_x(float* sx, const float* __restrict__ xr, int F, int E, int lane) {
+  constexpr int XP = EP + 1;
+  for (int k = lane; k < F * E; k += 32) {
+    const int f = k / E;
+    sx[f * XP + (k - f * E)] = xr[k];
+  }
+}
+
+template <int EP, int AP>
+__global__ void __launch_bounds__(kAfmWarps * 32)
+    afm_fwd_kernel(const float* __restrict__ x, int64_t ldx, int F, int E, int A, const float* __restrict__ W,
+                   const float* __restrict__ bias, const float* __restrict__ h, float* att, int64_t ldo,
+                   float* state, int64_t batch) {
+  constexpr int XP = EP + 1;
+  extern __shared__ float sm[];
+  const int P = afm_load_header<EP, AP>(sm, W, bias, h, F, E, A);
+  const float* sW = sm;
+  const float* sb = sW + EP * AP;
+  const float* sh = sb + AP;
+  const int* spair = (const int*)(sh + AP);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* sx = sm + afm_header_floats<EP, AP>() + warp * F * XP;
+  for (int k = lane; k < F * XP; k += 32) sx[k] = 0.f;
+  __syncthreads();
+  const int64_t nw = (int64_t)gridDim.x * kAfmWarps;
+  for (int64_t b = (int64_t)blockIdx.x * kAfmWarps + warp; b < batch; b += nw) {
+    afm_stage_x<EP>(sx, x + b * ldx, F, E, lane);
+    __syncwarp();
+    float m = -INFINITY, l = 0.f, acc[EP];
+#pragma unroll
+    for (int e = 0; e < EP; ++e) acc[e] = 0.f;
+    for (int p = lane; p < P; p += 32) {
+      const int ij = spair[p];
+      const float* xi = sx + (ij >> 8) * XP;
+      const float* xj = sx + (ij & 255) * XP;
+      float pr[EP];
+#pragma unroll
+      for (int e = 0; e < EP; ++e) pr[e] = xi[e] * xj[e];
+      float s = 0.f;
+#pragma unroll 1
+      for (int a = 0; a < AP; ++a) {
+        const float t = afm_dot<EP>(pr, sW + a * EP) + sb[a];
+        s = fmaf(sh[a], fmaxf(t, 0.f), s);
+      }
+      if (s > m) {
+        const float c = expf(m - s);     // m = -inf on the first pair: c = 0, acc and l are 0 anyway
+        l *= c;
+#pragma unroll
+        for (int e = 0; e < EP; ++e) acc[e] *= c;
+        m = s;
+      }
+      const float w = expf(s - m);
+      l += w;
+#pragma unroll
+      for (int e = 0; e < EP; ++e) acc[e] = fmaf(w, pr[e], acc[e]);
+    }
+    const float M = warp_max(m);
+    const float c = m == -INFINITY ? 0.f : expf(m - M);   // lanes without a pair (P < 32) contribute nothing
+    const float L = warp_sum(l * c);
+    const float inv = 1.f / L;
+    float* o = att + b * ldo;
+#pragma unroll
+    for (int e = 0; e < EP; ++e) {
+      const float v = warp_sum(acc[e] * c);
+      if (lane == e && e < E) o[e] = v * inv;
+    }
+    if (lane == 0) {
+      state[2 * b] = M;
+      state[2 * b + 1] = L;
+    }
+    __syncwarp();   // sx is restaged for the next sample
+  }
+}
+
+template <int EP, int AP>
+__host__ __device__ constexpr int afm_bwd_warp_floats(int F) {
+  return 2 * F * (EP + 1) + 2 * 32 * (EP + 1) + 2 * 32 * (AP + 1) + (EP + 1);
+}
+
+template <int EP, int AP>
+__global__ void __launch_bounds__(kAfmWarps * 32)
+    afm_bwd_kernel(const float* __restrict__ x, int64_t ldx, int F, int E, int A, const float* __restrict__ W,
+                   const float* __restrict__ bias, const float* __restrict__ h, const float* __restrict__ g,
+                   int64_t ldg, const float* __restrict__ att, int64_t lda, const float* __restrict__ state,
+                   float* dx, int64_t lddx, float* partial, int64_t batch) {
+  constexpr int XP = EP + 1;
+  constexpr int RP = AP + 1;                           // odd pitch: lane-indexed rows hit distinct banks
+  constexpr int NW = EP * AP + 2 * AP;                 // per-CTA partial: dW (padded), dbias, dh
+  constexpr int R = (EP * AP + 31) / 32;               // dW entries owned per lane
+  constexpr int G = 32 / EP;                           // lanes sharing one column e in the dx fold
+  extern __shared__ float sm[];
+  const int P = afm_load_header<EP, AP>(sm, W, bias, h, F, E, A);
+  const float* sW = sm;
+  const float* sb = sW + EP * AP;
+  const float* sh = sb + AP;
+  const int* spair = (const int*)(sh + AP);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* sx = sm + afm_header_floats<EP, AP>() + warp * afm_bwd_warp_floats<EP, AP>(F);
+  float* sdx = sx + F * XP;
+  float* rp = sdx + F * XP;      // [32][XP] prod of the round's pairs
+  float* rd = rp + 32 * XP;      // [32][XP] d prod
+  float* rt = rd + 32 * XP;      // [32][RP] d t (pre-relu hidden)
+  float* rh = rt + 32 * RP;      // [32][RP] ds * hidden
+  float* sg = rh + 32 * RP;      // [XP] incoming gradient of the sample
+  for (int k = lane; k < F * XP; k += 32) sx[k] = 0.f;
+  for (int k = lane; k < XP; k += 32) sg[k] = 0.f;
+  __syncthreads();
+  const int ecol = lane % EP, grp = lane / EP;
+  float accW[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) accW[r] = 0.f;
+  float accB = 0.f, accH = 0.f;
+  const int64_t nw = (int64_t)gridDim.x * kAfmWarps;
+  for (int64_t b = (int64_t)blockIdx.x * kAfmWarps + warp; b < batch; b += nw) {
+    afm_stage_x<EP>(sx, x + b * ldx, F, E, lane);
+    for (int k = lane; k < F * XP; k += 32) sdx[k] = 0.f;
+    float gatt = 0.f;
+    if (lane < E) {
+      const float ge = g[b * ldg + lane];
+      sg[lane] = ge;
+      gatt = ge * att[b * lda + lane];
+    }
+    gatt = warp_sum(gatt);
+    const float M = state[2 * b], invL = 1.f / state[2 * b + 1];
+    __syncwarp();
+    for (int base = 0; base < P; base += 32) {
+      const int p = base + lane;
+      float pr[EP], dpr[EP];
+      float* tl = rt + lane * RP;
+      float* hl = rh + lane * RP;
+      if (p < P) {
+        const int ij = spair[p];
+        const float* xi = sx + (ij >> 8) * XP;
+        const float* xj = sx + (ij & 255) * XP;
+#pragma unroll
+        for (int e = 0; e < EP; ++e) pr[e] = xi[e] * xj[e];
+        float s = 0.f, gp = 0.f;
+#pragma unroll 1
+        for (int a = 0; a < AP; ++a) {
+          const float t = afm_dot<EP>(pr, sW + a * EP) + sb[a];
+          tl[a] = t;                       // pre-activation, turned into its gradient below
+          s = fmaf(sh[a], fmaxf(t, 0.f), s);
+        }
+#pragma unroll
+        for (int e = 0; e < EP; ++e) gp = fmaf(sg[e], pr[e], gp);
+        const float alpha = expf(s - M) * invL;
+        const float ds = alpha * (gp - gatt);
+#pragma unroll
+        for (int e = 0; e < EP; ++e) dpr[e] = alpha * sg[e];
+#pragma unroll 1
+        for (int a = 0; a < AP; ++a) {
+          const float t = tl[a];
+          const float d = t > 0.f ? ds * sh[a] : 0.f;
+          hl[a] = ds * fmaxf(t, 0.f);
+          tl[a] = d;
+          const float* wa = sW + a * EP;
+#pragma unroll
+          for (int e = 0; e < EP; e += 4) {
+            const float4 w = *reinterpret_cast<const float4*>(wa + e);
+            dpr[e] = fmaf(w.x, d, dpr[e]);
+            dpr[e + 1] = fmaf(w.y, d, dpr[e + 1]);
+            dpr[e + 2] = fmaf(w.z, d, dpr[e + 2]);
+            dpr[e + 3] = fmaf(w.w, d, dpr[e + 3]);
+          }
+        }
+      } else {
+#pragma unroll
+        for (int e = 0; e < EP; ++e) pr[e] = dpr[e] = 0.f;
+        for (int a = 0; a < AP; ++a) tl[a] = hl[a] = 0.f;
+      }
+#pragma unroll
+      for (int e = 0; e < EP; ++e) {
+        rp[lane * XP + e] = pr[e];
+        rd[lane * XP + e] = dpr[e];
+      }
+      __syncwarp();
+      const int nq = min(32, P - base);
+      for (int q = 0; q < nq; ++q) {
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+          const int k = lane + 32 * r;
+          if (k < EP * AP) accW[r] = fmaf(rp[q * XP + k / AP], rt[q * RP + k % AP], accW[r]);
+        }
+        if (lane < AP) {
+          accB += rt[q * RP + lane];
+          accH += rh[q * RP + lane];
+        }
+        const int ij = spair[base + q];
+        const int i = ij >> 8, j = ij & 255;
+        const float d = rd[q * XP + ecol];
+        if (i % G == grp) sdx[i * XP + ecol] = fmaf(d, sx[j * XP + ecol], sdx[i * XP + ecol]);
+        if (j % G == grp) sdx[j * XP + ecol] = fmaf(d, sx[i * XP + ecol], sdx[j * XP + ecol]);
+      }
+      __syncwarp();
+    }
+    float* dr = dx + b * lddx;
+    for (int k = lane; k < F * E; k += 32) {
+      const int f = k / E;
+      dr[k] = sdx[f * XP + (k - f * E)];
+    }
+    __syncwarp();
+  }
+  // CTA partial: warps in a fixed order
+  float* wp = sx + 2 * F * XP;   // this warp's rp region (>= NW floats)
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const int k = lane + 32 * r;
+    if (k < EP * AP) wp[k] = accW[r];
+  }
+  if (lane < AP) {
+    wp[EP * AP + lane] = accB;
+    wp[EP * AP + AP + lane] = accH;
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < NW; k += blockDim.x) {
+    float s = 0.f;
+    for (int w = 0; w < kAfmWarps; ++w)
+      s += (sm + afm_header_floats<EP, AP>() + w * afm_bwd_warp_floats<EP, AP>(F) + 2 * F * XP)[k];
+    partial[(int64_t)blockIdx.x * NW + k] = s;
+  }
+}
+
+// dW[e, a], dbias[a], dh[a] = sum over the CTA partials in ascending CTA order
+__global__ void afm_reduce_kernel(const float* __restrict__ partial, int nblocks, int EP, int AP, int E, int A,
+                                  float* dW, float* dbias, float* dh) {
+  const int NW = EP * AP + 2 * AP;
+  const int n = E * A + 2 * A;
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+    int src;
+    float* dst;
+    if (t < E * A) {
+      const int e = t / A, a = t - e * A;
+      src = e * AP + a;
+      dst = dW + t;
+    } else if (t < E * A + A) {
+      src = EP * AP + (t - E * A);
+      dst = dbias + (t - E * A);
+    } else {
+      src = EP * AP + AP + (t - E * A - A);
+      dst = dh + (t - E * A - A);
+    }
+    float s = 0.f;
+    for (int c = 0; c < nblocks; ++c) s += partial[(int64_t)c * NW + src];
+    *dst = s;
+  }
+}
+
+static inline int afm_pad_e(int E) { return E <= 4 ? 4 : E <= 8 ? 8 : E <= 16 ? 16 : 32; }
+static inline int afm_pad_a(int A) { return A <= 1 ? 1 : A <= 2 ? 2 : A <= 4 ? 4 : A <= 8 ? 8 : 16; }
+static inline int afm_bwd_blocks(int64_t batch) { return grid_for(batch, kAfmWarps, 4); }
+static inline size_t afm_fwd_smem(int EP, int AP, int F) {
+  return sizeof(float) * ((size_t)EP * AP + 2 * AP + kAfmMaxF * (kAfmMaxF - 1) / 2 + (size_t)kAfmWarps * F * (EP + 1));
+}
+static inline size_t afm_bwd_smem(int EP, int AP, int F) {
+  const size_t warp = 2 * (size_t)F * (EP + 1) + 2 * 32 * (EP + 1) + 2 * 32 * (AP + 1) + (EP + 1);
+  return sizeof(float) * ((size_t)EP * AP + 2 * AP + kAfmMaxF * (kAfmMaxF - 1) / 2 + kAfmWarps * warp);
+}
+
+// host-side launch of one (EP, AP) instantiation; afm_dispatch picks it at run time
+struct AfmArgs {
+  const float* x; int64_t ldx; int F, E, A;
+  const float *W, *bias, *h;
+  const float* g; int64_t ldg;
+  float* att; int64_t lda;       // forward: output; backward: input
+  float* state;                  // forward: output; backward: input
+  float* dx; int64_t lddx;
+  float* partial;
+  int64_t batch;
+};
+struct AfmFwd {
+  template <int EP, int AP>
+  static cudaError_t run(const AfmArgs& a, cudaStream_t s) {
+    const size_t smem = afm_fwd_smem(EP, AP, a.F);
+    cudaError_t e = cudaFuncSetAttribute(afm_fwd_kernel<EP, AP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+    if (e != cudaSuccess) return e;
+    afm_fwd_kernel<EP, AP><<<grid_for(a.batch, kAfmWarps, 8), kAfmWarps * 32, smem, s>>>(
+        a.x, a.ldx, a.F, a.E, a.A, a.W, a.bias, a.h, a.att, a.lda, a.state, a.batch);
+    return cudaSuccess;
+  }
+};
+struct AfmBwd {
+  template <int EP, int AP>
+  static cudaError_t run(const AfmArgs& a, cudaStream_t s) {
+    const size_t smem = afm_bwd_smem(EP, AP, a.F);
+    cudaError_t e = cudaFuncSetAttribute(afm_bwd_kernel<EP, AP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+    if (e != cudaSuccess) return e;
+    afm_bwd_kernel<EP, AP><<<afm_bwd_blocks(a.batch), kAfmWarps * 32, smem, s>>>(
+        a.x, a.ldx, a.F, a.E, a.A, a.W, a.bias, a.h, a.g, a.ldg, a.att, a.lda, a.state, a.dx, a.lddx, a.partial,
+        a.batch);
+    return cudaSuccess;
+  }
+};
+template <class Op, int EP>
+cudaError_t afm_dispatch_a(int AP, const AfmArgs& a, cudaStream_t s) {
+  switch (AP) {
+    case 1: return Op::template run<EP, 1>(a, s);
+    case 2: return Op::template run<EP, 2>(a, s);
+    case 4: return Op::template run<EP, 4>(a, s);
+    case 8: return Op::template run<EP, 8>(a, s);
+    default: return Op::template run<EP, 16>(a, s);
+  }
+}
+template <class Op>
+cudaError_t afm_dispatch(int EP, int AP, const AfmArgs& a, cudaStream_t s) {
+  switch (EP) {
+    case 4: return afm_dispatch_a<Op, 4>(AP, a, s);
+    case 8: return afm_dispatch_a<Op, 8>(AP, a, s);
+    case 16: return afm_dispatch_a<Op, 16>(AP, a, s);
+    default: return afm_dispatch_a<Op, 32>(AP, a, s);
+  }
+}
+
 }  // namespace b2ctr
 
 using namespace b2ctr;
@@ -448,6 +873,86 @@ b2ctr_status_t b2ctr_interacting_bwd(const float* q, const float* k, const float
   interacting_bwd_kernel<<<(unsigned)batch, 128, smem, ST>>>(q, k, v, out, dout, dq, dk, dv, dres, nfield,
                                                             heads, dhead, scale);
   B2_CHECK_LAUNCH("b2ctr_interacting_bwd");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_bi_interaction_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, float* out,
+                                        int64_t ldo, int64_t batch, void* stream) {
+  B2_REQUIRE(x && out && nfield > 0 && dim > 0 && ldx >= (int64_t)nfield * dim && ldo >= dim,
+             "bi_interaction_fwd: bad arguments");
+  if (batch <= 0) return B2CTR_OK;
+  bi_interaction_fwd_kernel<<<grid_for(batch, 8, 8), 256, 0, ST>>>(x, ldx, nfield, dim, out, ldo, batch);
+  B2_CHECK_LAUNCH("b2ctr_bi_interaction_fwd");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_bi_interaction_bwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, const float* g,
+                                        int64_t ldg, float* dx, int64_t lddx, int64_t batch, void* stream) {
+  B2_REQUIRE(x && g && dx && nfield > 0 && dim > 0 && ldg >= dim, "bi_interaction_bwd: bad arguments");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && lddx >= (int64_t)nfield * dim, "bi_interaction_bwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  bi_interaction_bwd_kernel<<<grid_for(batch, 8, 8), 256, 0, ST>>>(x, ldx, nfield, dim, g, ldg, dx, lddx, batch);
+  B2_CHECK_LAUNCH("b2ctr_bi_interaction_bwd");
+  return B2CTR_OK;
+}
+
+#define AFM_REQUIRE_SHAPE(what)                                                                             \
+  B2_REQUIRE(nfield >= 2 && nfield <= kAfmMaxF && dim >= 1 && dim <= kAfmMaxE && factor >= 1 &&             \
+                 factor <= kAfmMaxA,                                                                         \
+             what ": needs 2 <= field count <= %d, 1 <= embedding_size <= %d and 1 <= attention_factor <= %d " \
+                  "(got %d, %d, %d)",                                                                        \
+             kAfmMaxF, kAfmMaxE, kAfmMaxA, nfield, dim, factor)
+
+b2ctr_status_t b2ctr_afm_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t factor,
+                             const float* W, const float* bias, const float* h, float* att, int64_t ldo,
+                             float* state, int64_t batch, void* stream) {
+  B2_REQUIRE(x && W && bias && h && att && state, "afm_fwd: NULL pointer");
+  AFM_REQUIRE_SHAPE("afm_fwd");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && ldo >= dim, "afm_fwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  AfmArgs a{x, ldx, nfield, dim, factor, W, bias, h, nullptr, 0, att, ldo, state, nullptr, 0, nullptr, batch};
+  const cudaError_t err = afm_dispatch<AfmFwd>(afm_pad_e(dim), afm_pad_a(factor), a, ST);
+  if (err != cudaSuccess) {
+    set_error("afm_fwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_afm_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_afm_bwd_workspace_bytes(int32_t dim, int32_t factor, int64_t batch) {
+  if (dim < 1 || factor < 1 || batch <= 0) return 0;
+  const int EP = afm_pad_e(dim), AP = afm_pad_a(factor);
+  return (size_t)afm_bwd_blocks(batch) * (size_t)(EP * AP + 2 * AP) * sizeof(float);
+}
+
+b2ctr_status_t b2ctr_afm_bwd(const float* g, int64_t ldg, const float* x, int64_t ldx, int32_t nfield, int32_t dim,
+                             int32_t factor, const float* W, const float* bias, const float* h, const float* state,
+                             const float* att, int64_t lda, float* dx, int64_t lddx, float* dW, float* dbias,
+                             float* dh, int64_t batch, void* workspace, size_t workspace_bytes, void* stream) {
+  B2_REQUIRE(g && x && W && bias && h && state && att && dx && dW && dbias && dh, "afm_bwd: NULL pointer");
+  AFM_REQUIRE_SHAPE("afm_bwd");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && lddx >= (int64_t)nfield * dim && ldg >= dim && lda >= dim,
+             "afm_bwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  const size_t need = b2ctr_afm_bwd_workspace_bytes(dim, factor, batch);
+  if (!workspace || workspace_bytes < need) {
+    set_error("afm_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  const int EP = afm_pad_e(dim), AP = afm_pad_a(factor);
+  float* partial = (float*)workspace;
+  AfmArgs a{x, ldx, nfield, dim, factor, W, bias, h, g, ldg, const_cast<float*>(att), lda, const_cast<float*>(state),
+            dx, lddx, partial, batch};
+  const cudaError_t err = afm_dispatch<AfmBwd>(EP, AP, a, ST);
+  if (err != cudaSuccess) {
+    set_error("afm_bwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_afm_bwd");
+  afm_reduce_kernel<<<(unsigned)ceil_div(dim * factor + 2 * factor, 128), 128, 0, ST>>>(
+      partial, afm_bwd_blocks(batch), EP, AP, dim, factor, dW, dbias, dh);
+  B2_CHECK_LAUNCH("b2ctr_afm_bwd(reduce)");
   return B2CTR_OK;
 }
 

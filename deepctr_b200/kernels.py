@@ -627,6 +627,50 @@ def interacting_bwd(q, k, v, out, dout, want_res, batch, F, H, D, scaling):
     return dq, dk, dv, dres
 
 
+def bi_interaction_fwd(x, ldx, nfield, dim, batch):
+    """[B, nfield*dim] window (pitch ldx) -> [B, dim]:  0.5 * ((sum_f x)^2 - sum_f x^2)."""
+    _require_cuda(x)
+    out = torch.empty((batch, dim), dtype=torch.float32, device=x.device)
+    _lib_call("bi_interaction_fwd", ptr(x), ldx, nfield, dim, ptr(out), dim, batch, stream())
+    return out
+
+
+def bi_interaction_bwd(x, ldx, nfield, dim, g, batch):
+    _require_cuda(x, g)
+    dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=x.device)
+    _lib_call("bi_interaction_bwd", ptr(x), ldx, nfield, dim, ptr(g), g.stride(0), ptr(dx), nfield * dim, batch,
+              stream())
+    return dx
+
+
+def afm_fwd(x, ldx, nfield, dim, W, bias, h, batch):
+    """AFM attention pooling -> (att [B, dim], softmax state [B, 2])."""
+    _require_cuda(x, W, bias, h)
+    factor = W.shape[1]
+    att = torch.empty((batch, dim), dtype=torch.float32, device=x.device)
+    state = torch.empty((batch, 2), dtype=torch.float32, device=x.device)
+    _lib_call("afm_fwd", ptr(x), ldx, nfield, dim, factor, ptr(W), ptr(bias), ptr(h), ptr(att), dim, ptr(state),
+              batch, stream())
+    return att, state
+
+
+def afm_bwd(g, x, ldx, nfield, dim, W, bias, h, state, att, batch):
+    """-> (dx [B, nfield*dim], dW [dim, factor], dbias [factor], dh [factor])."""
+    _require_cuda(g, x, W, bias, h, state, att)
+    factor = W.shape[1]
+    dev = x.device
+    dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=dev)
+    dW = torch.empty((dim, factor), dtype=torch.float32, device=dev)
+    db = torch.empty((factor,), dtype=torch.float32, device=dev)
+    dh = torch.empty((factor,), dtype=torch.float32, device=dev)
+    nbytes = L.lib().b2ctr_afm_bwd_workspace_bytes(dim, factor, batch)
+    ws = workspace(nbytes, dev)
+    _lib_call("afm_bwd", ptr(g), g.stride(0), ptr(x), ldx, nfield, dim, factor, ptr(W), ptr(bias), ptr(h),
+              ptr(state), ptr(att), att.stride(0), ptr(dx), nfield * dim, ptr(dW), ptr(db), ptr(dh), batch, ptr(ws),
+              nbytes, stream())
+    return dx, dW, db, dh
+
+
 def din_att_input_fwd(q, ldq, keys, ldk, batch, T, E):
     out = torch.empty((batch, T, 4 * E), dtype=torch.float32, device=q.device)
     _lib_call("din_att_input_fwd", ptr(q), ldq, ptr(keys), ldk, ptr(out), batch, T, E, stream())
@@ -734,7 +778,8 @@ def dropout(x, rate, seed):
 
 for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
-           "cin_expand_grad", "interacting_fwd", "interacting_bwd", "din_att_input_fwd", "din_att_input_bwd",
+           "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
+           "afm_bwd", "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
     globals()[_n] = _timed(globals()[_n])
@@ -786,7 +831,8 @@ for _n in ("shard_bucketize", "shard_fill", "shard_gather_rows", "shard_scatter_
 
 for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
-           "cin_expand_grad", "interacting_fwd", "interacting_bwd", "din_att_input_fwd", "din_att_input_bwd",
+           "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
+           "afm_bwd", "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "moving_update", "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
     globals()[_n] = _timed(globals()[_n])

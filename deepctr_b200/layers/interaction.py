@@ -1,9 +1,101 @@
 """Host mirror of deepctr/layers/interaction.py for the operators on the hot path:
-FM (:563-607), CrossNet (:344-435), CIN (:209-341), InteractingLayer (:697-790).
+AFMLayer (:39-160), BiInteractionPooling (:163-206), FM (:563-607), CrossNet (:344-435), CIN (:209-341),
+InteractingLayer (:697-790).
 Same constructor arguments, weight names, shape checks and error messages as the reference."""
 from .. import engine as E
 from .. import ops
-from ..engine import Layer, Zeros, glorot_normal, glorot_uniform, TruncatedNormal, l2
+from ..engine import Layer, Lambda, Zeros, glorot_normal, glorot_uniform, TruncatedNormal, l2
+from .normalization import Dropout
+
+# shapes the fused AFM kernels serve (include/b2ctr.h, b2ctr_afm_fwd)
+AFM_MAX_FIELDS, AFM_MAX_EMBEDDING, AFM_MAX_FACTOR = 64, 32, 16
+
+
+class AFMLayer(Layer):
+    """Attentional FM pooling, deepctr/layers/interaction.py:39-160.  Called on a list of F [B,1,E] tensors;
+    att = sum_p softmax_p(h . relu(W^T (v_i * v_j) + b)) (v_i * v_j) over the pairs i < j, then
+    out = Dropout(att) . projection_p  [B,1].  The pairwise products are generated inside the kernel
+    (b2ctr_afm_fwd / _bwd): nothing of size [B, F(F-1)/2, .] is stored."""
+
+    def __init__(self, attention_factor=4, l2_reg_w=0, dropout_rate=0, seed=1024, **kwargs):
+        self.attention_factor = attention_factor
+        self.l2_reg_w = l2_reg_w
+        self.dropout_rate = dropout_rate
+        self.seed = seed
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        if not isinstance(input_shape, list) or len(input_shape) < 2:
+            raise ValueError('A `AttentionalFM` layer should be called '
+                             'on a list of at least 2 inputs')
+        shape_set = set(tuple(s) for s in input_shape)
+        if len(shape_set) > 1:
+            raise ValueError('A `AttentionalFM` layer requires '
+                             'inputs with same shapes '
+                             'Got different shapes: %s' % (shape_set))
+        if len(input_shape[0]) != 3 or input_shape[0][1] != 1:
+            raise ValueError('A `AttentionalFM` layer requires '
+                             'inputs of a list with same shape tensor like\
+                             (None, 1, embedding_size)'
+                             'Got different shapes: %s' % (input_shape[0],))
+        embedding_size = int(input_shape[0][-1])
+        if (len(input_shape) > AFM_MAX_FIELDS or embedding_size > AFM_MAX_EMBEDDING
+                or not 1 <= int(self.attention_factor) <= AFM_MAX_FACTOR):
+            raise ValueError("AFMLayer supports up to %d inputs, embedding_size <= %d and 1 <= attention_factor <= %d "
+                             "(got %d inputs, embedding_size %d, attention_factor %r)"
+                             % (AFM_MAX_FIELDS, AFM_MAX_EMBEDDING, AFM_MAX_FACTOR, len(input_shape),
+                                embedding_size, self.attention_factor))
+        self.attention_W = self.add_weight(shape=(embedding_size, self.attention_factor),
+                                           initializer=glorot_normal(seed=self.seed),
+                                           regularizer=l2(self.l2_reg_w), name="attention_W")
+        self.attention_b = self.add_weight(shape=(self.attention_factor,), initializer=Zeros(), name="attention_b")
+        self.projection_h = self.add_weight(shape=(self.attention_factor, 1),
+                                            initializer=glorot_normal(seed=self.seed), name="projection_h")
+        self.projection_p = self.add_weight(shape=(embedding_size, 1), initializer=glorot_normal(seed=self.seed),
+                                            name="projection_p")
+        # the reference creates these two layers here: they take the next `dropout` / `lambda` names
+        self.dropout = self._track(Dropout(self.dropout_rate, seed=self.seed, name=self.name + "/dropout"))
+        self.tensordot = self._track(Lambda(lambda x: ops.dense(x[0], x[1]), name=self.name + "/tensordot"))
+        self.built = True
+
+    def call(self, inputs, training=None, **kwargs):
+        if inputs[0].data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs[0].data.dim()))
+        fields = ops.concat(inputs, axis=1)             # a zero-copy window of the fused gather's buffer
+        att = ops.afm(fields, self.attention_W, self.attention_b, self.projection_h)
+        att = self.dropout.call(att, training=training)
+        return self.tensordot.call([att, self.projection_p])
+
+    def compute_output_shape(self, input_shape):
+        if not isinstance(input_shape, list):
+            raise ValueError('A `AFMLayer` layer should be called '
+                             'on a list of inputs.')
+        return (None, 1)
+
+    def get_config(self):
+        config = {'attention_factor': self.attention_factor,
+                  'l2_reg_w': self.l2_reg_w, 'dropout_rate': self.dropout_rate, 'seed': self.seed}
+        base = Layer.get_config(self)
+        base.update(config)
+        return base
+
+
+class BiInteractionPooling(Layer):
+    """Bi-Interaction pooling of NFM, deepctr/layers/interaction.py:163-206.
+    [B,F,E] -> [B,1,E]:  0.5 * ((sum_f x)^2 - sum_f x^2)  (FM without the final sum over E)."""
+
+    def build(self, input_shape):
+        if len(input_shape) != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (len(input_shape)))
+        self.built = True
+
+    def call(self, inputs, **kwargs):
+        if inputs.data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs.data.dim()))
+        return ops.bi_interaction(inputs)
+
+    def compute_output_shape(self, input_shape):
+        return (None, 1, input_shape[-1])
 
 
 class FM(Layer):

@@ -3,5 +3,7 @@ from .xdeepfm import xDeepFM
 from .dcn import DCN
 from .autoint import AutoInt
 from .sequence import DIN
+from .nfm import NFM
+from .afm import AFM
 
-__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN"]
+__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM"]

@@ -393,6 +393,61 @@ def fm(x):
     return res
 
 
+def _fields2d(x):
+    """[B,F,E] -> (2-D [B, F*E] window, pitch): the fused gather's buffer is read in place."""
+    b, f, e = x.data.shape
+    src, ld = x.flat2d()
+    if src is None:
+        t = E.contiguous(x)
+        src, ld = t.reshape(b, f * e), f * e
+    return src, ld
+
+
+def bi_interaction(x):
+    """[B,F,E] -> [B,1,E]: 0.5 * ((sum_f x)^2 - sum_f x^2)  (BiInteractionPooling, layers/interaction.py:196-201)."""
+    b, f, e = x.data.shape
+    src, ld = _fields2d(x)
+    out = K.bi_interaction_fwd(src, ld, f, e, b)
+    res = E.Var(out.reshape(b, 1, e))
+
+    def bwd(grads):
+        g = grads[0].reshape(b, e)
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dx = K.bi_interaction_bwd(src, ld, f, e, g, b)
+        E.add_grad(x, dx.reshape(x.data.shape))
+
+    E.record([res], [x], bwd)
+    return res
+
+
+def afm(x, w, bias, h):
+    """[B,F,E] -> [B,E]: attention-weighted sum of the pairwise products v_i * v_j (AFMLayer up to its dropout,
+    layers/interaction.py:126-141).  The [B, P, E] products and the [B, P, A] attention hidden layer are generated
+    on chip in the forward and again in the backward; only a [B, 2] softmax state is kept."""
+    b, f, e = x.data.shape
+    src, ld = _fields2d(x)
+    wd, bd, hd = _wdata(w), _wdata(bias), _wdata(h)
+    att, state = K.afm_fwd(src, ld, f, e, wd, bd, hd.reshape(-1), b)
+    res = E.Var(att)
+
+    def bwd(grads):
+        g = grads[0].reshape(b, e)
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dx, dw, db, dh = K.afm_bwd(g, src, ld, f, e, wd, bd, hd.reshape(-1), state, att, b)
+        E.add_grad(x, dx.reshape(x.data.shape))
+        if w.requires_grad:
+            E.add_grad(w, dw)
+        if bias.requires_grad:
+            E.add_grad(bias, db.reshape(bd.shape))
+        if h.requires_grad:
+            E.add_grad(h, dh.reshape(hd.shape))
+
+    E.record([res], [x, w, bias, h], bwd)
+    return res
+
+
 def add_bias(x, b):
     """x + b over the last axis for a per-column (or scalar, when the last axis is 1) bias:
     Linear(use_bias=True) without a dense part, layers/utils.py:172-173.  Forward = copy + rank-1 update

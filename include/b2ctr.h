@@ -460,6 +460,37 @@ B2CTR_API b2ctr_status_t b2ctr_interacting_bwd(const float* q, const float* k, c
                                               int32_t nfield, int32_t heads, int32_t dhead,
                                               int32_t scaling, void* stream);
 
+/* BiInteractionPooling (deepctr/layers/interaction.py:163-206) on x [B, nfield, dim] (row pitch ldx, so a
+ * window of the fused gather's buffer is read in place):
+ *   out[b*ldo + e] = 0.5 * ((sum_f x[b,f,e])^2 - sum_f x[b,f,e]^2)
+ * backward: dx[b*lddx + f*dim + e] = g[b*ldg + e] * (S[b,e] - x[b,f,e]), S = sum_f x.  One warp per sample. */
+B2CTR_API b2ctr_status_t b2ctr_bi_interaction_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim,
+                                                 float* out, int64_t ldo, int64_t batch, void* stream);
+B2CTR_API b2ctr_status_t b2ctr_bi_interaction_bwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim,
+                                                 const float* g, int64_t ldg, float* dx, int64_t lddx,
+                                                 int64_t batch, void* stream);
+
+/* AFMLayer attention pooling (deepctr/layers/interaction.py:116-143 up to the dropout) on x [B, nfield, dim]
+ * (pitch ldx), W [dim, factor] (attention_W), bias [factor] (attention_b), h [factor] (projection_h):
+ *   prod_p = x_i * x_j for the P = nfield(nfield-1)/2 pairs i < j
+ *   alpha  = softmax_p(h . relu(W^T prod_p + bias));   att[b*ldo + e] = sum_p alpha_p prod_p[e]
+ *   state[2b] = max_p s_p, state[2b+1] = sum_p exp(s_p - max)   (saved for the backward)
+ * The pairwise products and the attention hidden layer are generated on chip and never written.
+ * Limits: 2 <= nfield <= 64, 1 <= dim <= 32, 1 <= factor <= 16; anything else is B2CTR_ERR_INVALID_ARG. */
+B2CTR_API b2ctr_status_t b2ctr_afm_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t factor,
+                                      const float* W, const float* bias, const float* h, float* att, int64_t ldo,
+                                      float* state, int64_t batch, void* stream);
+/* Backward from g = d att [B, dim] (pitch ldg), the forward's state and att (pitch lda):
+ *   dx [B, nfield*dim] (pitch lddx, overwritten), dW [dim, factor], dbias [factor], dh [factor] (overwritten).
+ * Weight gradients are summed per CTA into the workspace and reduced in a fixed order: no float atomics,
+ * bit-identical from run to run. */
+B2CTR_API size_t b2ctr_afm_bwd_workspace_bytes(int32_t dim, int32_t factor, int64_t batch);
+B2CTR_API b2ctr_status_t b2ctr_afm_bwd(const float* g, int64_t ldg, const float* x, int64_t ldx, int32_t nfield,
+                                      int32_t dim, int32_t factor, const float* W, const float* bias,
+                                      const float* h, const float* state, const float* att, int64_t lda,
+                                      float* dx, int64_t lddx, float* dW, float* dbias, float* dh, int64_t batch,
+                                      void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* 6. Sequence operators (DIN, pooling, Dice / BatchNormalization, dropout)                     */
 /* ------------------------------------------------------------------------------------------ */
