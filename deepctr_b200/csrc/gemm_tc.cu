@@ -6,15 +6,16 @@
 // <= 2^-16 relative), i.e. three bf16 wgmma per K-step.  That keeps the reference's fp32 logits within the
 // 1e-4 bar at ~1/3 of the bf16 tensor throughput instead of the FFMA pipe.
 //
-// Every kernel computes 128 x BN output tiles.  Operand tiles sit in shared memory as bf16 hi / lo planes in the
-// 128-byte-swizzled layouts wgmma reads through matrix descriptors (K-major: 16-byte chunk index XOR row % 8;
-// MN-major: 64-element atoms of 64 k-rows).  Two consumer warpgroups each own 64 rows of the tile and issue
-// wgmma.mma_async m64nBNk16 on them; the accumulator lives in their registers.  The epilogue stores it from there,
-// or (variant 4, plain outputs) stages it in shared memory and stores it with TMA.
-//   variant 1: the 256 threads split the fp32 operands into the stage themselves, then multiply it
-//   variant 2/3: the split is done once per operand into planes in global memory; cp.async moves them
-//   variant 4 (default): persistent, warp-specialised: TMA / cp.async / generating producer warps fill a stage ring
-//              guarded by mbarriers while the two consumer warpgroups multiply and run the epilogue
+// Every kernel computes 128 x BN output tiles.  The fp32 -> (hi, lo) split is done once per operand into bf16
+// planes in global memory (or the producer warps generate the A operand, CIN / DIN attention).  Operand tiles sit in
+// shared memory in the 128-byte-swizzled layouts wgmma reads through matrix descriptors (K-major: 16-byte chunk
+// index XOR row % 8; MN-major: 64-element atoms of 64 k-rows).  The accumulator lives in the registers of two
+// consumer warpgroups.
+//   gemm_planes_ws_kernel (variant 4, the default and the only production path): persistent, warp-specialised: TMA
+//       or generating producer warps fill a stage ring guarded by mbarriers while the two consumer warpgroups
+//       multiply and run the epilogue (plain outputs: staged in shared memory and stored with TMA).
+//   gemm_planes_kernel (variant 3): non-persistent, cp.async, register epilogue.  It issues the same wgmma in the
+//       same order per output element, so it is the reference the bit-exact tests compare variant 4 against.
 #include <cuda.h>          // CUtensorMap + enums only: the encoder is resolved through the runtime (no libcuda link)
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -24,16 +25,32 @@ namespace b2ctr {
 
 constexpr int kTM = 128;       // rows of the output tile: two warpgroups x 64
 constexpr int kTK = 64;        // K elements per stage = one 128-byte swizzle atom of bf16
-constexpr int kTcThreads = 256;   // variants 1-3: two warpgroups that both fill and multiply every stage
+constexpr int kTcThreads = 256;   // gemm_planes_kernel: two warpgroups that both fill and multiply every stage
 
-struct TcArgs {
-  const float* a; const float* b; float* c; const float* bias; float* ws;
-  int64_t m, n, k;
-  int64_t sam, sak, sbn, sbk;   // A(m,k) = a[m*sam + k*sak];  B(n,k) = b[n*sbn + k*sbk]
+struct PlaneArgs {
+  // K-major planes: [rows_pad, k_pad] (k contiguous).  MN-major planes: [k_pad, rows_pad] (row index
+  // contiguous) - the natural layout of a row-major operand whose reduction dim is its row index
+  // (wgrad: X^T, dZ^T; forward: W).  *_pitch = elements between consecutive plane rows.
+  const __nv_bfloat16* a_hi; const __nv_bfloat16* a_lo;
+  const __nv_bfloat16* b_hi; const __nv_bfloat16* b_lo;
+  int64_t a_pitch, b_pitch;
+  int a_mn, b_mn;
+  float* c; const float* bias; float* ws;
+  int64_t m, n, k_pad;
   int64_t ldc;
   int64_t k_per_split;
   float alpha;
   int act, accumulate, splits;
+  // CIN mode (cin_on): the A operand is never stored anywhere - the producer warps GENERATE its bf16 hi/lo tile
+  // in shared memory from the two factors of the outer product (deepctr/layers/interaction.py:287-297):
+  //   A[r, i*hp + j] = t0[r*ld0 + i] * xk[r*ldk + j]   (j < h, i < m; zero otherwise),  r = (sample, embedding dim)
+  // a_mn = 0: A is [rows, m*hp] (forward, M = r);  a_mn = 1: A^T, i.e. M = i*hp + j and K = r (filter gradient).
+  const float* cin_t0; const float* cin_xk;
+  int64_t cin_ld0, cin_ldk, cin_rows;
+  int cin_m, cin_h, cin_hp, cin_on;
+  // FOLD epilogue (CIN backward): dT0 [rows, cin_ld0] and dXk [rows, fold_ldx], both accumulated with red.add
+  float* fold_dt0; float* fold_dxk; int64_t fold_ldx;
+  int gen_groups;     // generating producers: 2 = two groups of 128 threads alternate stages, 1 = all 256 share every stage
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -192,8 +209,9 @@ __device__ __forceinline__ void with_majorness(int a_mn, int b_mn, F&& f) {
 // row0 + 16w + l/4 (+ 8) and columns n0 + 8i + 2(l % 4) + {0, 1} in d[4i + {0, 1}] (and d[4i + {2, 3}] for the
 // row + 8).  Each group of four lanes writes 32 contiguous bytes of a row.  C = act(alpha acc [+ C] [+ bias]);
 // split-K slices go to the workspace instead (ws[z][m][n], reduced by tc_splitk_reduce_kernel).
-template <int BN, class G>
-__device__ __forceinline__ void store_acc(const G& g, const float (&d)[BN / 2], int64_t row0, int64_t n0, int64_t z) {
+template <int BN>
+__device__ __forceinline__ void store_acc(const PlaneArgs& g, const float (&d)[BN / 2], int64_t row0, int64_t n0,
+                                          int64_t z) {
   const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
   const bool vec = (g.ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(g.c) & 7) == 0);
   const bool vec_ws = g.n % 2 == 0;
@@ -246,98 +264,7 @@ __device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 lo, __nv_bfloat16 hi
   return (uint32_t)__bfloat16_as_ushort(lo) | ((uint32_t)__bfloat16_as_ushort(hi) << 16);
 }
 
-// Gather 8 consecutive K values of row r (global k in [k0, k0+8)), split, and store both planes.
-// tile layout: row r at byte r*128, 16-byte chunk c stored at slot (c ^ (r & 7)).
-template <bool K_CONTIG>
-__device__ __forceinline__ void produce_chunk(const float* __restrict__ base, int64_t sr, int64_t sk,
-                                              int64_t row, int64_t nrows, int64_t k0, int64_t kend,
-                                              bool vec_ok, unsigned char* hi_tile, unsigned char* lo_tile,
-                                              int r, int c) {
-  float v[8];
-  if (row < nrows) {
-    const float* p = base + row * sr + k0 * sk;
-    if (K_CONTIG && vec_ok && k0 + 8 <= kend) {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(p));
-      const float4 b = __ldg(reinterpret_cast<const float4*>(p) + 1);
-      v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = (k0 + j < kend) ? __ldg(p + j * sk) : 0.f;
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = 0.f;
-  }
-  uint32_t h[4], l[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const __nv_bfloat16 h0 = __float2bfloat16_rn(v[2 * j]), h1 = __float2bfloat16_rn(v[2 * j + 1]);
-    const __nv_bfloat16 l0 = __float2bfloat16_rn(v[2 * j] - __bfloat162float(h0));
-    const __nv_bfloat16 l1 = __float2bfloat16_rn(v[2 * j + 1] - __bfloat162float(h1));
-    h[j] = pack_bf16(h0, h1);
-    l[j] = pack_bf16(l0, l1);
-  }
-  const int off = r * 128 + ((c ^ (r & 7)) << 4);
-  *reinterpret_cast<uint4*>(hi_tile + off) = make_uint4(h[0], h[1], h[2], h[3]);
-  *reinterpret_cast<uint4*>(lo_tile + off) = make_uint4(l[0], l[1], l[2], l[3]);
-}
-// Variant 1: the 256 threads read the fp32 operand tiles straight from global memory with coalesced loads in
-// whatever layout they are stored (each thread gathers 8 consecutive K values of one row), split them into the
-// stage, then both warpgroups multiply it.  A stage is refilled once the wgmma group that read it has retired.
-template <int BN, int STAGES, bool A_KC, bool B_KC>
-__global__ void __launch_bounds__(kTcThreads, STAGES == 1 ? 2 : 1) gemm_bf16x3_kernel(const TcArgs g) {
-  constexpr int A_PLANE = kTM * 128;       // bytes of one bf16 plane of the A tile (128 rows x 64 k)
-  constexpr int B_PLANE = BN * 128;
-  constexpr int STAGE = 2 * A_PLANE + 2 * B_PLANE;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* tiles = align1024(smem_raw);
-
-  const int tid = threadIdx.x, wg = tid >> 7;
-  const int64_t m0 = (int64_t)blockIdx.y * kTM, n0 = (int64_t)blockIdx.x * BN;
-  const int64_t kbeg = (int64_t)blockIdx.z * g.k_per_split;
-  const int64_t kend = kbeg + g.k_per_split < g.k ? kbeg + g.k_per_split : g.k;
-  const int nkb = kend > kbeg ? (int)((kend - kbeg + kTK - 1) / kTK) : 0;
-  const bool a_vec = A_KC && (g.sam % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.a) & 15) == 0);
-  const bool b_vec = B_KC && (g.sbn % 4 == 0) && ((reinterpret_cast<uintptr_t>(g.b) & 15) == 0);
-
-  float d[BN / 2];
-#pragma unroll
-  for (int j = 0; j < BN / 2; ++j) d[j] = 0.f;
-  for (int kb = 0; kb < nkb; ++kb) {
-    const int s = kb % STAGES;
-    unsigned char* st = tiles + (size_t)s * STAGE;
-    wgmma_wait<STAGES - 1>();          // the group that last read stage s (k-block kb - STAGES) has retired ...
-    __syncthreads();                   // ... in both warpgroups
-    const int64_t k0 = kbeg + (int64_t)kb * kTK;
-    // A tile: 128 rows x 8 chunks.  K-contiguous storage: chunk fastest (coalesced along k);
-    // otherwise row fastest (coalesced along m).
-#pragma unroll 4
-    for (int t = tid; t < kTM * 8; t += kTcThreads) {
-      const int r = A_KC ? t >> 3 : t % kTM;
-      const int c = A_KC ? t & 7 : t / kTM;
-      const int64_t kk = k0 + c * 8;
-      produce_chunk<A_KC>(g.a, g.sam, g.sak, m0 + r, g.m, kk, kend, a_vec && ((kk & 3) == 0), st,
-                          st + A_PLANE, r, c);
-    }
-#pragma unroll 4
-    for (int t = tid; t < BN * 8; t += kTcThreads) {
-      const int r = B_KC ? t >> 3 : t % BN;
-      const int c = B_KC ? t & 7 : t / BN;
-      const int64_t kk = k0 + c * 8;
-      produce_chunk<B_KC>(g.b, g.sbn, g.sbk, n0 + r, g.n, kk, kend, b_vec && ((kk & 3) == 0),
-                          st + 2 * A_PLANE, st + 2 * A_PLANE + B_PLANE, r, c);
-    }
-    // make the generic-proxy writes visible to the tensor core (async proxy)
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    wg_kblock<BN, 0, 0>(d, smem_u32(st), wg);
-  }
-  wgmma_wait<0>();
-  fence_acc(d);
-  store_acc<BN>(g, d, m0 + wg * 64, n0, blockIdx.z);
-}
-
-__global__ void tc_splitk_reduce_kernel(const TcArgs g) {
+__global__ void tc_splitk_reduce_kernel(const PlaneArgs g) {
   const int64_t total = g.m * g.n;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (int64_t)gridDim.x * blockDim.x) {
@@ -350,57 +277,13 @@ __global__ void tc_splitk_reduce_kernel(const TcArgs g) {
   }
 }
 
-template <int BN, int STAGES>
-static cudaError_t launch_tc(const TcArgs& ta, bool akc, bool bkc, cudaStream_t st) {
-  constexpr size_t smem = (size_t)STAGES * (2 * kTM * 128 + 2 * BN * 128) + 1024;
-  dim3 grid((unsigned)ceil_div(ta.n, BN), (unsigned)ceil_div(ta.m, kTM), (unsigned)ta.splits);
-#define B2_TC_LAUNCH(AK, BK)                                                                         \
-  do {                                                                                               \
-    auto kern = gemm_bf16x3_kernel<BN, STAGES, AK, BK>;                                              \
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-    if (e != cudaSuccess) return e;                                                                  \
-    kern<<<grid, kTcThreads, smem, st>>>(ta);                                                        \
-  } while (0)
-  if (akc && bkc) B2_TC_LAUNCH(true, true);
-  else if (akc && !bkc) B2_TC_LAUNCH(true, false);
-  else if (!akc && bkc) B2_TC_LAUNCH(false, true);
-  else B2_TC_LAUNCH(false, false);
-#undef B2_TC_LAUNCH
-  return cudaGetLastError();
-}
-
 // ================================================================================================
-// Variant 2 ("planes"): the fp32 -> (hi, lo) bf16 split is done ONCE per operand by a streaming kernel
-// into K-major planes [rows_pad, k_pad] in workspace memory; the GEMM kernel then only moves bytes:
-// the 256 threads cp.async 16-byte chunks of the planes into the swizzled stage tiles (no register staging,
-// no conversion instructions), so no CTA re-converts an operand tile another CTA also reads.
+// Operand planes and the non-persistent reference kernel (variant 3)
+// The fp32 -> (hi, lo) bf16 split is done ONCE per operand by a streaming kernel into planes in workspace memory,
+// so no CTA re-converts an operand tile another CTA also reads.  A row-contiguous operand keeps its layout
+// (MN-major planes, the wgmma descriptors do the transposition); only a row-contiguous B under a 32-wide N tile
+// (an MN-major tile is one 64-wide atom) goes through the transposing split into K-major planes.
 // ================================================================================================
-struct PlaneArgs {
-  // K-major planes: [rows_pad, k_pad] (k contiguous).  MN-major planes: [k_pad, rows_pad] (row index
-  // contiguous) - the natural layout of a row-major operand whose reduction dim is its row index
-  // (wgrad: X^T, dZ^T; forward: W).  *_pitch = elements between consecutive plane rows.
-  const __nv_bfloat16* a_hi; const __nv_bfloat16* a_lo;
-  const __nv_bfloat16* b_hi; const __nv_bfloat16* b_lo;
-  int64_t a_pitch, b_pitch;
-  int a_mn, b_mn;
-  float* c; const float* bias; float* ws;
-  int64_t m, n, k_pad;
-  int64_t ldc;
-  int64_t k_per_split;
-  float alpha;
-  int act, accumulate, splits;
-  // CIN mode (cin_on): the A operand is never stored anywhere - the producer warps GENERATE its bf16 hi/lo tile
-  // in shared memory from the two factors of the outer product (deepctr/layers/interaction.py:287-297):
-  //   A[r, i*hp + j] = t0[r*ld0 + i] * xk[r*ldk + j]   (j < h, i < m; zero otherwise),  r = (sample, embedding dim)
-  // a_mn = 0: A is [rows, m*hp] (forward, M = r);  a_mn = 1: A^T, i.e. M = i*hp + j and K = r (filter gradient).
-  const float* cin_t0; const float* cin_xk;
-  int64_t cin_ld0, cin_ldk, cin_rows;
-  int cin_m, cin_h, cin_hp, cin_on;
-  // FOLD epilogue (CIN backward): dT0 [rows, cin_ld0] and dXk [rows, fold_ldx], both accumulated with red.add
-  float* fold_dt0; float* fold_dxk; int64_t fold_ldx;
-  int gen_groups;     // generating producers: 2 = two groups of 128 threads alternate stages, 1 = all 256 share every stage
-};
-
 // dst planes [rows_pad, k_pad] <- src(r, k) = p[r*sr + k*sk]; zero outside [rows, k).
 // K-contiguous source: thread = (row, 8 consecutive k).
 __global__ void __launch_bounds__(256)
@@ -561,7 +444,7 @@ static cudaError_t launch_planes(const PlaneArgs& pa, cudaStream_t st) {
 
 
 // ================================================================================================
-// Variant 4: persistent, warp-specialised planes GEMM.
+// Variant 4: persistent, warp-specialised planes GEMM - the kernel every production GEMM runs.
 //   warps 0-7  : two consumer warpgroups.  Plain GEMMs (GEN = 0, no FOLD) run them PING-PONG: warpgroup j % 2 owns
 //                the whole j-th tile of the CTA (both 64-row halves, two accumulators) and the two alternate, so one
 //                warpgroup's epilogue runs while the other issues its MMAs.  Per k-block a warpgroup waits for the
@@ -571,10 +454,10 @@ static cudaError_t launch_planes(const PlaneArgs& pa, cudaStream_t st) {
 //                a tile only after the other one has issued the previous tile's last k-block.  The generated-operand and FOLD kernels stay COOPERATIVE: each warpgroup owns 64 rows of
 //                every tile and both run the epilogue together (their producers / fold leave no registers for a
 //                second accumulator).
-//   producers  : TMA (default): one elected thread arms the stage barrier and issues cp.async.bulk.tensor.2d loads
-//                of the four plane slices.  GEN = 1 / 2: eight warps GENERATE the A tile in shared memory (CIN outer
-//                product / DIN attention input) while B arrives by TMA.  B2CTR_TC_TMA=0: four warps of 16-byte
-//                cp.async.
+//   producers  : GEN = 0: one elected thread arms the stage barrier and issues cp.async.bulk.tensor.2d (TMA) loads
+//                of the four plane slices; its warpgroup gives up its registers to the ping-pong consumers.
+//                GEN = 1 / 2: eight warps GENERATE the A tile in shared memory (CIN outer product / DIN attention
+//                input) while B arrives by TMA.
 // The producers run up to STAGES k-blocks ahead, across tile boundaries: the next tile's operands load while the
 // consumers run the epilogue of the current one.
 // Persistent: grid = min(#tiles, #SMs); tile = CTA id + j * #CTAs, N-tile fastest (neighbouring CTAs share the
@@ -582,7 +465,7 @@ static cudaError_t launch_planes(const PlaneArgs& pa, cudaStream_t st) {
 // hold two, so those kernels move registers from the producer warpgroup to them with setmaxnreg.
 // ================================================================================================
 constexpr int kWsConsumerWarps = 8;
-constexpr int kWsProducers = 4;   // warps
+constexpr int kWsProducers = 4;   // warps: one issues the TMA loads, but setmaxnreg works per warpgroup
 
 struct WsArgs {
   PlaneArgs p;
@@ -641,8 +524,8 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 // The activation is a template parameter (ACT < 0: g.act at run time) and the checks that are uniform over the
 // tile are taken outside the element loop, so the loop is straight-line code: with one warp per SM sub-partition
 // the epilogue is bound by instruction latency, not by shared-memory or store bandwidth.
-template <int BN, int ACT, class G>
-__device__ __forceinline__ void store_acc_tma_act(const G& g, const float (&d)[BN / 2], const CUtensorMap* map,
+template <int BN, int ACT>
+__device__ __forceinline__ void store_acc_tma_act(const PlaneArgs& g, const float (&d)[BN / 2], const CUtensorMap* map,
                                                   uint32_t stg, int wg, int64_t row0, int64_t n0) {
   constexpr int HALF = BN < 64 ? BN : 64;
   const int t = threadIdx.x & 127, lane = t & 31, w = t >> 5;
@@ -695,8 +578,8 @@ __device__ __forceinline__ void store_acc_tma_act(const G& g, const float (&d)[B
     }
   }
 }
-template <int BN, class G>
-__device__ __forceinline__ void store_acc_tma(const G& g, const float (&d)[BN / 2], const CUtensorMap* map,
+template <int BN>
+__device__ __forceinline__ void store_acc_tma(const PlaneArgs& g, const float (&d)[BN / 2], const CUtensorMap* map,
                                               uint32_t stg, int wg, int64_t row0, int64_t n0) {
   if (g.act == B2CTR_ACT_NONE) store_acc_tma_act<BN, B2CTR_ACT_NONE>(g, d, map, stg, wg, row0, n0);
   else if (g.act == B2CTR_ACT_RELU) store_acc_tma_act<BN, B2CTR_ACT_RELU>(g, d, map, stg, wg, row0, n0);
@@ -873,7 +756,7 @@ struct WsLayout {
 
 // GEN: 0 = both operands from memory; 1 = A generated as the CIN outer product; 2 = A generated as the DIN
 // attention input (one instantiation per generator: the code of the other one would only fill the instruction cache)
-template <int BN, int STAGES, bool TMA, int GEN = 0, bool FOLD = false>
+template <int BN, int STAGES, int GEN = 0, bool FOLD = false>
 __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     gemm_planes_ws_kernel(const __grid_constant__ WsArgs w, const __grid_constant__ CUtensorMap tm_ah,
                           const __grid_constant__ CUtensorMap tm_al, const __grid_constant__ CUtensorMap tm_bh,
@@ -893,9 +776,9 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      // cp.async producers: one deferred arrival per producer thread; TMA: one arrive.expect_tx
-      // generated A: one arrival per generating thread of the stage + the TMA expect_tx of the B planes
-      mbar_init(&full_bar[s], GEN != 0 ? 1 + (g.gen_groups == 2 ? 128 : 256) : (TMA ? 1 : kWsProducers * 32));
+      // TMA: one arrive.expect_tx; generated A: one arrival per generating thread of the stage + the TMA expect_tx
+      // of the B planes
+      mbar_init(&full_bar[s], GEN != 0 ? 1 + (g.gen_groups == 2 ? 128 : 256) : 1);
       // a stage is released by every consumer warp (cooperative) or by the four warps of the tile's owner (ping-pong)
       mbar_init(&empty_bar[s], PINGPONG ? kWsConsumerWarps / 2 : kWsConsumerWarps);
     }
@@ -1078,7 +961,7 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
         mbar_arrive(&full_bar[s]);
       }
     }
-  } else if (TMA && warp >= kWsConsumerWarps) {
+  } else if (warp >= kWsConsumerWarps) {
     // ------------------------------------------------------------------------------ TMA producer
     // one elected lane: wait for a free stage, arm its barrier with the stage bytes, issue the bulk tensor copies
     // of the four operand planes.  Data moves global -> swizzled shared memory inside the async proxy, where
@@ -1123,72 +1006,6 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
         }
       }
     }
-  } else if (warp >= kWsConsumerWarps) {
-    // ------------------------------------------------------------------------------ producers
-    if constexpr (PINGPONG) setmaxnreg_dec<56>();
-    const int tid = threadIdx.x - kWsConsumerWarps * 32;
-    constexpr int NT = kWsProducers * 32;
-    int64_t tile = cta0, mt = 0, nt = 0, kbeg = 0;
-    int nkb = 0, kb = 0;
-    while (tile < w.ntiles) {            // first tile with work
-      decode(tile, mt, nt, kbeg, nkb);
-      if (nkb > 0) break;
-      tile += nctas;
-    }
-    // Every producer thread hands its copies to the stage's mbarrier (cp.async.mbarrier.arrive.noinc: the
-    // arrival fires when the thread's cp.asyncs have landed), so this warp never waits for data - only for a
-    // free stage - and all STAGES blocks are genuinely in flight.
-    for (uint32_t it = 0; tile < w.ntiles; ++it) {
-      const int s = it % STAGES;
-      mbar_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
-      const uint32_t st = smem_u32(tiles + (size_t)s * STAGE);
-      const int64_t k0 = kbeg + (int64_t)kb * kTK;
-      const int64_t m0 = mt * kTM;
-      const int64_t n0 = nt * BN;
-#pragma unroll 4
-      for (int t = tid; t < kTM * 8; t += NT) {
-        uint32_t off;
-        int64_t src;
-        if (g.a_mn) {
-          const int kk = t / (kTM / 8), c = t % (kTM / 8);
-          off = (c >> 3) * 8192 + kk * 128 + (((c & 7) ^ (kk & 7)) << 4);
-          src = (k0 + kk) * g.a_pitch + m0 + c * 8;
-        } else {
-          const int r = t >> 3, c = t & 7;
-          off = r * 128 + ((c ^ (r & 7)) << 4);
-          src = (m0 + r) * g.a_pitch + k0 + c * 8;
-        }
-        cp_async16(st + off, g.a_hi + src);
-        cp_async16(st + A_PLANE + off, g.a_lo + src);
-      }
-#pragma unroll 4
-      for (int t = tid; t < BN * 8; t += NT) {
-        uint32_t off;
-        int64_t src;
-        if (g.b_mn) {
-          const int kk = t / (BN / 8), c = t % (BN / 8);
-          off = (c >> 3) * 8192 + kk * 128 + (((c & 7) ^ (kk & 7)) << 4);
-          src = (k0 + kk) * g.b_pitch + n0 + c * 8;
-        } else {
-          const int r = t >> 3, c = t & 7;
-          off = r * 128 + ((c ^ (r & 7)) << 4);
-          src = (n0 + r) * g.b_pitch + k0 + c * 8;
-        }
-        cp_async16(st + 2 * A_PLANE + off, g.b_hi + src);
-        cp_async16(st + 2 * A_PLANE + B_PLANE + off, g.b_lo + src);
-      }
-      asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(&full_bar[s])) : "memory");
-      if (++kb == nkb) {               // next tile with work
-        kb = 0;
-        tile += nctas;
-        while (tile < w.ntiles) {
-          decode(tile, mt, nt, kbeg, nkb);
-          if (nkb > 0) break;
-          tile += nctas;
-        }
-      }
-    }
-    asm volatile("cp.async.wait_all;" ::: "memory");
   } else {
     // ------------------------------------------------------------------------------ consumers
     const int wg = warp >> 2;
@@ -1218,7 +1035,6 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
         for (int kb = 0; kb < nkb; ++kb, ++it) {
           const int s = it % STAGES;
           mbar_wait(&full_bar[s], (it / STAGES) & 1);
-          if (!TMA) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async wrote it
           const uint32_t st = smem_u32(tiles + (size_t)s * STAGE);
           tile_kblock_half<BN, TA, TB, 0>(d0, d1, st);
           wgmma_wait<1>();                      // the previous k-block has retired: release its stage
@@ -1358,14 +1174,13 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
 
 struct TmaMaps {
   CUtensorMap ah, al, bh, bl, c;
-  bool ok;
 };
 
-template <int BN, int STAGES, bool TMA, int GEN = 0, bool FOLD = false>
+template <int BN, int STAGES, int GEN = 0, bool FOLD = false>
 static cudaError_t launch_ws_impl(const WsArgs& wa, const TmaMaps& tm, cudaStream_t st) {
   constexpr size_t smem = (size_t)STAGES * (2 * kTM * 128 + 2 * BN * 128) + 2 * ws_staging_bytes<BN>() + 1024;
   static_assert(smem + 256 <= 227 * 1024, "stage ring + epilogue staging exceed shared memory");
-  auto kern = gemm_planes_ws_kernel<BN, STAGES, TMA, GEN, FOLD>;
+  auto kern = gemm_planes_ws_kernel<BN, STAGES, GEN, FOLD>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   int64_t nctas = wa.ntiles < kNumSMs ? wa.ntiles : kNumSMs;
@@ -1377,10 +1192,6 @@ static cudaError_t launch_ws_impl(const WsArgs& wa, const TmaMaps& tm, cudaStrea
   kern<<<(unsigned)nctas, WsLayout<GEN != 0>::kThreads, smem, st>>>(wcopy, tm.ah, tm.al, tm.bh, tm.bl, tm.c);
   return cudaGetLastError();
 }
-template <int BN, int STAGES>
-static cudaError_t launch_ws(const WsArgs& wa, const TmaMaps& tm, cudaStream_t st) {
-  return tm.ok ? launch_ws_impl<BN, STAGES, true>(wa, tm, st) : launch_ws_impl<BN, STAGES, false>(wa, tm, st);
-}
 
 // ---- tensor maps: cuTensorMapEncodeTiled resolved through the runtime's driver entry-point query ---------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1391,8 +1202,6 @@ static EncodeTiledFn tma_encoder() {
   static bool tried = false;
   if (!tried) {
     tried = true;
-    const char* ev = getenv("B2CTR_TC_TMA");
-    if (ev && atoi(ev) == 0) return nullptr;
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
@@ -1447,32 +1256,25 @@ static inline int planes_bn(int64_t n, int64_t k) {
   return 256;
 }
 
-static int tc_variant(const b2ctr_gemm_t* g) {
-  if (g->variant >= 1 && g->variant <= 4) return g->variant;
-  static int mode = -1;
-  if (mode < 0) {
-    const char* ev = getenv("B2CTR_TC_VARIANT");
-    mode = ev ? atoi(ev) : 4;
-  }
-  return (mode >= 1 && mode <= 4) ? mode : 4;
-}
-
 size_t gemm_bf16x3_workspace_bytes(const b2ctr_gemm_t* g) {
   size_t splitk = g->split_k > 1 ? (size_t)g->split_k * g->m * g->n * sizeof(float) : 0;
-  if (tc_variant(g) == 1) return splitk;
-  const int bn = planes_bn(g->n, g->k / (g->split_k > 1 ? g->split_k : 1));
   const int64_t kp = round_up(g->k > 0 ? g->k : 1, kTK), mp = round_up(g->m, 2 * kTM), np = round_up(g->n, 256);
   return splitk + (size_t)(mp + np) * kp * 2 * sizeof(__nv_bfloat16) + 512;
 }
 
-static b2ctr_status_t gemm_planes(const b2ctr_gemm_t* g, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+// variant 0 / 4: the persistent kernel; variant 3: the non-persistent reference kernel
+b2ctr_status_t gemm_bf16x3(const b2ctr_gemm_t* g, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  B2_REQUIRE(g->variant == 0 || g->variant == 3 || g->variant == 4, "gemm: variant must be 0, 3 or 4, got %d",
+             g->variant);
+  B2_REQUIRE(((uintptr_t)g->a_planes & 15) == 0 && ((uintptr_t)g->b_planes & 15) == 0,
+             "gemm: a_planes / b_planes must be 16-byte aligned");
   const size_t need = gemm_bf16x3_workspace_bytes(g);
   if (!workspace || workspace_bytes < need) {
     set_error("gemm(bf16x3): needs %zu workspace bytes, got %zu", need, workspace_bytes);
     return B2CTR_ERR_WORKSPACE;
   }
   const int splits = g->split_k > 1 ? g->split_k : 1;
-  const bool ws_kernel = tc_variant(g) == 4;
+  const bool ws_kernel = g->variant != 3;
   int bn = ws_kernel ? (g->n <= 32 ? 32 : g->n <= 64 ? 64 : 128)
                      : planes_bn(g->n, g->k / (g->split_k > 1 ? g->split_k : 1));
   const int64_t kp = round_up(g->k > 0 ? g->k : 1, kTK), mp = round_up(g->m, 2 * kTM);
@@ -1480,20 +1282,19 @@ static b2ctr_status_t gemm_planes(const b2ctr_gemm_t* g, void* workspace, size_t
   float* ws = (float*)w;
   w += splits > 1 ? (size_t)splits * g->m * g->n * sizeof(float) : 0;
   w = (unsigned char*)(((uintptr_t)w + 255) & ~(uintptr_t)255);
-  // variant 2: always K-major planes (row-contiguous sources go through a transposing split);
-  // variant 3: row-contiguous sources keep their layout (MN-major planes) and the wgmma descriptors do the
-  // transposition - the same planes then serve every GEMM that reads the tensor (forward / dgrad / wgrad),
-  // which is what caller-provided planes (g->a_planes / g->b_planes) exploit.
-  const bool mn_ok = tc_variant(g) >= 3;
+  // Row-contiguous sources keep their layout (MN-major planes) and the wgmma descriptors do the transposition -
+  // the same planes then serve every GEMM that reads the tensor (forward / dgrad / wgrad), which is what
+  // caller-provided planes (g->a_planes / g->b_planes) exploit.  An MN-major B tile is at least one 64-wide atom:
+  // under a 32-wide N tile a row-contiguous B goes through the transposing split into K-major planes instead.
   const bool a_kc = !g->trans_a, b_kc = g->trans_b != 0;
   const int64_t a_sr = g->trans_a ? g->k : g->m, a_sc = g->trans_a ? g->m : g->k;   // stored rows / cols
   const int64_t b_sr = g->trans_b ? g->n : g->k, b_sc = g->trans_b ? g->k : g->n;
-  const bool a_given = g->a_planes && (a_kc || mn_ok);
-  bool b_given = g->b_planes && (b_kc || (mn_ok && bn >= 64));
+  const bool a_given = g->a_planes != nullptr;
+  const bool b_given = g->b_planes && (b_kc || bn >= 64);
   if (b_given && !b_kc && planes_cols_pad(b_sc) % bn != 0) bn = planes_cols_pad(b_sc) == 64 ? 64 : 128;   // N tiles inside the pad
   const int64_t np = round_up(g->n, bn);
-  const int a_mn = a_given ? !a_kc : ((!a_kc && mn_ok) ? 1 : 0);
-  const int b_mn = b_given ? !b_kc : ((!b_kc && mn_ok && bn >= 64) ? 1 : 0);   // an MN atom is 64 elements wide
+  const int a_mn = !a_kc;
+  const int b_mn = !b_kc && bn >= 64;
   __nv_bfloat16 *a_hi, *a_lo, *b_hi, *b_lo;
   int64_t a_pitch, b_pitch;
   int64_t a_prows, b_prows;      // rows of the plane matrices as stored (TMA extents)
@@ -1515,8 +1316,7 @@ static b2ctr_status_t gemm_planes(const b2ctr_gemm_t* g, void* workspace, size_t
     a_hi = (__nv_bfloat16*)w; a_lo = a_hi + mp * kp; w = (unsigned char*)(a_lo + mp * kp);
     a_pitch = a_mn ? mp : kp; a_prows = a_mn ? kp : mp;
     if (a_kc) split_k(g->a, g->lda, g->m, g->k, mp, kp, a_hi, a_lo);
-    else if (a_mn) split_k(g->a, g->lda, g->k, g->m, kp, mp, a_hi, a_lo);
-    else split_t(g->a, g->lda, g->m, mp, a_hi, a_lo);
+    else split_k(g->a, g->lda, g->k, g->m, kp, mp, a_hi, a_lo);
     B2_CHECK_LAUNCH("b2ctr_gemm(bf16x3 split A)");
   }
   if (b_given) {
@@ -1550,14 +1350,17 @@ static b2ctr_status_t gemm_planes(const b2ctr_gemm_t* g, void* workspace, size_t
     wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n * splits;
     // TMA producers: four tiled tensor maps over the operand planes (box = one stage's slice of a plane)
     TmaMaps tm{};
-    tm.ok = tma_map_2d(&tm.ah, a_hi, a_pitch, a_prows, a_pitch, 64, a_mn ? 64 : kTM) &&
-            tma_map_2d(&tm.al, a_lo, a_pitch, a_prows, a_pitch, 64, a_mn ? 64 : kTM) &&
-            tma_map_2d(&tm.bh, b_hi, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bn) &&
-            tma_map_2d(&tm.bl, b_lo, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bn);
-    wa.c_tma = tm.ok && tma_map_c(&tm.c, pa);
-    if (bn == 32) e = launch_ws<32, 5>(wa, tm, st);
-    else if (bn == 64) e = launch_ws<64, 4>(wa, tm, st);
-    else e = launch_ws<128, 3>(wa, tm, st);
+    if (!(tma_map_2d(&tm.ah, a_hi, a_pitch, a_prows, a_pitch, 64, a_mn ? 64 : kTM) &&
+          tma_map_2d(&tm.al, a_lo, a_pitch, a_prows, a_pitch, 64, a_mn ? 64 : kTM) &&
+          tma_map_2d(&tm.bh, b_hi, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bn) &&
+          tma_map_2d(&tm.bl, b_lo, b_pitch, b_prows, b_pitch, 64, b_mn ? 64 : bn))) {
+      set_error("b2ctr_gemm(bf16x3): cuTensorMapEncodeTiled unavailable (the kernel loads its operands by TMA)");
+      return B2CTR_ERR_UNSUPPORTED;
+    }
+    wa.c_tma = tma_map_c(&tm.c, pa);
+    if (bn == 32) e = launch_ws_impl<32, 5>(wa, tm, st);
+    else if (bn == 64) e = launch_ws_impl<64, 4>(wa, tm, st);
+    else e = launch_ws_impl<128, 3>(wa, tm, st);
   } else if (bn == 32) e = short_k ? launch_planes<32, 1>(pa, st) : launch_planes<32, 4>(pa, st);
   else if (bn == 64) e = short_k ? launch_planes<64, 1>(pa, st) : launch_planes<64, 4>(pa, st);
   else if (bn == 128) e = short_k ? launch_planes<128, 1>(pa, st) : launch_planes<128, 3>(pa, st);
@@ -1568,10 +1371,7 @@ static b2ctr_status_t gemm_planes(const b2ctr_gemm_t* g, void* workspace, size_t
   }
   count_launch();
   if (splits > 1) {
-    TcArgs ta;
-    ta.c = g->c; ta.bias = g->bias; ta.ws = ws; ta.m = g->m; ta.n = g->n; ta.ldc = g->ldc;
-    ta.act = g->act; ta.accumulate = g->accumulate; ta.splits = splits;
-    tc_splitk_reduce_kernel<<<grid_for(g->m * g->n, 256, 4), 256, 0, st>>>(ta);
+    tc_splitk_reduce_kernel<<<grid_for(g->m * g->n, 256, 4), 256, 0, st>>>(pa);
     B2_CHECK_LAUNCH("b2ctr_gemm(bf16x3 splitk_reduce)");
   }
   return B2CTR_OK;
@@ -1630,8 +1430,8 @@ static size_t gen_gemm_workspace_bytes(const GenSpec& sp, int mode, int64_t n, i
 
 template <int GEN>
 static cudaError_t launch_gen(const WsArgs& wa, const TmaMaps& tm, int bn, cudaStream_t st) {
-  if (bn == 64) return launch_ws_impl<64, 4, true, GEN>(wa, tm, st);
-  return launch_ws_impl<128, 3, true, GEN>(wa, tm, st);
+  if (bn == 64) return launch_ws_impl<64, 4, GEN>(wa, tm, st);
+  return launch_ws_impl<128, 3, GEN>(wa, tm, st);
 }
 
 // mode 0: c[rows, n] = act(A B + bias), B = planes of a [kq, n] row-major matrix; mode 1: c[kq, n] = A^T dY,
@@ -1681,8 +1481,7 @@ static b2ctr_status_t gen_gemm(const GenSpec& sp, int mode, int64_t n, const voi
   wa.tiles_n = (int)ceil_div(n, bn);
   wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n * splits;
   TmaMaps tm{};
-  tm.ok = tma_map_2d(&tm.bh, pa.b_hi, cp, b_prows, cp, 64, 64) && tma_map_2d(&tm.bl, pa.b_lo, cp, b_prows, cp, 64, 64);
-  if (!tm.ok) {
+  if (!tma_map_2d(&tm.bh, pa.b_hi, cp, b_prows, cp, 64, 64) || !tma_map_2d(&tm.bl, pa.b_lo, cp, b_prows, cp, 64, 64)) {
     set_error("%s: cuTensorMapEncodeTiled unavailable (the kernel loads its B operand by TMA)", what);
     return B2CTR_ERR_UNSUPPORTED;
   }
@@ -1695,10 +1494,7 @@ static b2ctr_status_t gen_gemm(const GenSpec& sp, int mode, int64_t n, const voi
   }
   count_launch();
   if (splits > 1) {
-    TcArgs ta;
-    ta.c = c; ta.bias = bias; ta.ws = pa.ws; ta.m = pa.m; ta.n = n; ta.ldc = ldc;
-    ta.act = act; ta.accumulate = 0; ta.splits = splits;
-    tc_splitk_reduce_kernel<<<grid_for(pa.m * n, 256, 4), 256, 0, st>>>(ta);
+    tc_splitk_reduce_kernel<<<grid_for(pa.m * n, 256, 4), 256, 0, st>>>(pa);
     B2_CHECK_LAUNCH("generated-operand gemm (splitk_reduce)");
   }
   return B2CTR_OK;
@@ -1753,14 +1549,13 @@ b2ctr_status_t cin_fold(const b2ctr_cin_gemm_t* g, float* dt0, float* dxk, int64
   wa.tiles_n = (int)ceil_div(kq, bn);
   wa.ntiles = (int64_t)wa.tiles_m * wa.tiles_n;
   TmaMaps tm{};
-  tm.ok = tma_map_2d(&tm.ah, pa.a_hi, cpn, a_prows, cpn, 64, kTM) && tma_map_2d(&tm.al, pa.a_lo, cpn, a_prows, cpn, 64, kTM) &&
-          tma_map_2d(&tm.bh, pa.b_hi, cpn, b_prows, cpn, 64, bn) && tma_map_2d(&tm.bl, pa.b_lo, cpn, b_prows, cpn, 64, bn);
-  if (!tm.ok) {
+  if (!(tma_map_2d(&tm.ah, pa.a_hi, cpn, a_prows, cpn, 64, kTM) && tma_map_2d(&tm.al, pa.a_lo, cpn, a_prows, cpn, 64, kTM) &&
+        tma_map_2d(&tm.bh, pa.b_hi, cpn, b_prows, cpn, 64, bn) && tma_map_2d(&tm.bl, pa.b_lo, cpn, b_prows, cpn, 64, bn))) {
     set_error("cin_fold: cuTensorMapEncodeTiled unavailable");
     return B2CTR_ERR_UNSUPPORTED;
   }
   wa.c_tma = 0;      // the fold epilogue never stores the accumulator tile
-  cudaError_t e = launch_ws_impl<128, 3, true, 0, true>(wa, tm, st);
+  cudaError_t e = launch_ws_impl<128, 3, 0, true>(wa, tm, st);
   if (e != cudaSuccess) {
     set_error("b2ctr_cin_fold: CUDA launch failed: %s", cudaGetErrorString(e));
     return B2CTR_ERR_CUDA;
@@ -1799,53 +1594,6 @@ b2ctr_status_t split_planes(const float* src, int64_t ld, int64_t rows, int64_t 
   split_planes_kernel<<<grid_for(rp * (cp / 8), 256, 8), 256, 0, st>>>(src, ld, rows, cols, rp, cp, hi, hi + rp * cp,
                                                                       vec);
   B2_CHECK_LAUNCH("b2ctr_split_planes");
-  return B2CTR_OK;
-}
-
-b2ctr_status_t gemm_bf16x3(const b2ctr_gemm_t* g, void* workspace, size_t workspace_bytes,
-                           cudaStream_t st) {
-  if (tc_variant(g) >= 2) return gemm_planes(g, workspace, workspace_bytes, st);
-  TcArgs ta;
-  ta.a = g->a; ta.b = g->b; ta.c = g->c; ta.bias = g->bias; ta.ws = (float*)workspace;
-  ta.m = g->m; ta.n = g->n; ta.k = g->k;
-  ta.sam = g->trans_a ? 1 : g->lda;  ta.sak = g->trans_a ? g->lda : 1;
-  ta.sbn = g->trans_b ? g->ldb : 1;  ta.sbk = g->trans_b ? 1 : g->ldb;
-  ta.ldc = g->ldc; ta.alpha = g->alpha; ta.act = g->act; ta.accumulate = g->accumulate;
-  ta.splits = g->split_k > 1 ? g->split_k : 1;
-  if (ta.splits > 1) {
-    const size_t need = gemm_bf16x3_workspace_bytes(g);
-    if (!workspace || workspace_bytes < need) {
-      set_error("gemm(bf16x3): split_k=%d needs %zu workspace bytes, got %zu", ta.splits, need, workspace_bytes);
-      return B2CTR_ERR_WORKSPACE;
-    }
-  }
-  ta.k_per_split = ceil_div(ceil_div(g->k, ta.splits), kTK) * kTK;
-  const bool akc = !g->trans_a;   // A stored [M,K]: K contiguous
-  const bool bkc = g->trans_b != 0;  // B stored [N,K]: K contiguous
-  cudaError_t e;
-  static int stages_mode = -1;
-  if (stages_mode < 0) {
-    const char* ev = getenv("B2CTR_TC_STAGES");
-    stages_mode = ev ? atoi(ev) : 1;
-  }
-  if (stages_mode == 1) {        // single stage, 3 CTAs per SM: neighbours hide each other's load latency
-    if (g->n <= 32) e = launch_tc<32, 1>(ta, akc, bkc, st);
-    else if (g->n <= 64) e = launch_tc<64, 1>(ta, akc, bkc, st);
-    else e = launch_tc<128, 1>(ta, akc, bkc, st);
-  } else {                       // deep intra-CTA pipeline, 1 CTA per SM
-    if (g->n <= 32) e = launch_tc<32, 4>(ta, akc, bkc, st);
-    else if (g->n <= 64) e = launch_tc<64, 4>(ta, akc, bkc, st);
-    else e = launch_tc<128, 3>(ta, akc, bkc, st);
-  }
-  if (e != cudaSuccess) {
-    set_error("b2ctr_gemm(bf16x3): CUDA launch failed: %s", cudaGetErrorString(e));
-    return B2CTR_ERR_CUDA;
-  }
-  count_launch();
-  if (ta.splits > 1) {
-    tc_splitk_reduce_kernel<<<grid_for(g->m * g->n, 256, 4), 256, 0, st>>>(ta);
-    B2_CHECK_LAUNCH("b2ctr_gemm(bf16x3 splitk_reduce)");
-  }
   return B2CTR_OK;
 }
 

@@ -15,6 +15,7 @@ its Keras protocol (deepctr_b200/layers/) have a runtime:
 
 All arithmetic is done by libb2ctr.so through ``kernels.py``; nothing here computes with torch.
 """
+import gc
 import inspect
 import threading
 from collections import OrderedDict
@@ -1033,7 +1034,6 @@ class Model(object):
     def close(self):
         """Release what must not outlive the process group: captured step graphs (they hold NCCL kernels) and
         the CUDA-IPC mappings of the other ranks' table shards.  Call before dist.destroy_process_group()."""
-        import gc
         self._step_graphs = {}
         self._graph_pool = None
         planner = getattr(self, "planner", None)
@@ -1181,6 +1181,10 @@ class Model(object):
         it0 = self.optimizer.iterations
         n0 = L.launch_count()
         graph = torch.cuda.CUDAGraph()
+        # No garbage collection while the stream captures: a collection can run the destructors of unrelated dead
+        # CUDA objects (graphs, pinned host buffers, events), and some of them make CUDA calls a capture forbids.
+        gc_enabled = gc.isenabled()
+        gc.disable()
         try:
             with torch.cuda.graph(graph, pool=self._graph_pool, capture_error_mode="thread_local"):
                 loss_sum, pred, batch = self._loss_step_impl(feed, labels, True)
@@ -1195,6 +1199,9 @@ class Model(object):
             for w in self.weights:             # nothing ran on the device; drop the half-built python state
                 w.grad = None
             return None
+        finally:
+            if gc_enabled:
+                gc.enable()
         self.optimizer.iterations = it0        # capturing does not execute the step
         if ops.UNCAPTURABLE != self._uncapturable0:
             self.step_graph = "off"

@@ -14,8 +14,8 @@ from . import engine as E
 GEMM_PRECISION = L.GEMM_BF16X3
 
 
-# BF16X3: split every GEMM operand into bf16 planes once per step and reuse them (needs MN-major operands,
-# i.e. tc variant 3)
+# BF16X3: split every GEMM operand into bf16 planes once per step and reuse them (the GEMM reads a row-major
+# operand whose reduction dim is its row index as MN-major planes, so one split serves forward, dgrad and wgrad)
 PLANE_REUSE = True
 # the fused embedding gather also writes the planes of the first DNN operand (saves re-reading X to split it)
 GATHER_PLANES = False    # measured: -11 us/step but +60 us inside the gather kernel itself; opt-in

@@ -245,7 +245,7 @@ typedef struct b2ctr_gemm {
   int32_t precision;       /* B2CTR_GEMM_*                                                     */
   int32_t split_k;         /* >1: split the K loop over this many CTAs (needs workspace)       */
   float alpha;             /* scales op(A)@op(B)                                               */
-  int32_t variant;         /* BF16X3 only: 0 default, 1 in-kernel split, 2 K-major planes, 3 + MN-major */
+  int32_t variant;         /* BF16X3 only: 0 default (persistent), 3 non-persistent reference kernel, 4 persistent */
   const void* a_planes;    /* optional: b2ctr_split_planes() of the STORED a / b matrix.  Lets one split */
   const void* b_planes;    /* serve every GEMM that reads the tensor (forward, dgrad, wgrad); BF16X3 only */
 } b2ctr_gemm_t;

@@ -235,10 +235,10 @@ def test_optimizers(cuda):
 @pytest.mark.parametrize("m,n,k", [(128, 128, 64), (1, 1, 1), (257, 256, 845), (130, 64, 128), (1000, 1, 64),
                                    (64, 300, 7), (4096, 256, 848), (300, 40, 200)])
 @pytest.mark.parametrize("ta,tb", [(False, False), (False, True), (True, False), (True, True)])
-@pytest.mark.parametrize("variant", [1, 2, 3, 4])   # 1: split in the GEMM producers, 2: K-major planes,
+@pytest.mark.parametrize("variant", [3, 4])
 def test_gemm_bf16x3_tensor_core(cuda, m, n, k, ta, tb, variant):
     """wgmma split-bf16 GEMM: error bound ~2^-16 relative to sum |a||b| (DESIGN.md section 4.2).
-    Variants: 3 = + MN-major planes, 4 = persistent warp-specialised kernel."""
+    Variants: 3 = non-persistent reference kernel, 4 = persistent warp-specialised kernel."""
     K, L = _kern()
     rng = np.random.RandomState(m + 3 * n + k)
     a = _r(rng, *((k, m) if ta else (m, k)))
@@ -303,7 +303,7 @@ def test_gemm_bf16x3_persistent_pair_many_tiles(cuda, m, n, k, ta, tb, sk):
     torch.testing.assert_close(got, ref, rtol=2e-4, atol=2e-3 * max(1.0, (k / 256.0) ** 0.5))
 
 
-@pytest.mark.parametrize("variant", [1, 2, 3, 4])
+@pytest.mark.parametrize("variant", [3, 4])
 def test_gemm_bf16x3_splitk_accumulate(cuda, variant):
     K, L = _kern()
     rng = np.random.RandomState(77)
@@ -321,6 +321,32 @@ def test_gemm_bf16x3_splitk_accumulate(cuda, variant):
     c2 = c0.to(cuda)
     K.gemm(xd, dy, c=c2, trans_a=True, accumulate=True, split_k=8, alpha=0.5, m=m, n=n, k=k)
     torch.testing.assert_close(c.cpu(), c2.cpu(), rtol=1e-4, atol=2e-3)
+
+
+@pytest.mark.parametrize("variant", [1, 2, 5])
+def test_gemm_bf16x3_rejects_unknown_variant(cuda, variant):
+    """only 0 (default), 3 and 4 select a kernel; anything else is an argument error and launches nothing"""
+    K, L = _kern()
+    a, b = torch.ones((256, 64), device=cuda), torch.ones((64, 128), device=cuda)
+    n0 = L.launch_count()
+    with pytest.raises(ValueError, match="variant"):
+        K.gemm(a, b, precision=L.GEMM_BF16X3, variant=variant)
+    assert L.launch_count() == n0
+
+
+@pytest.mark.parametrize("given", ["a", "b"])
+def test_gemm_bf16x3_rejects_misaligned_planes(cuda, given):
+    """caller planes must be 16-byte aligned (TMA and cp.async read them in 16-byte units): a view 8 bytes into an
+    allocation is an argument error and launches nothing"""
+    K, L = _kern()
+    a, b = torch.ones((256, 64), device=cuda), torch.ones((64, 128), device=cuda)
+    planes = K.split_planes(a if given == "a" else b)
+    buf = torch.zeros(planes.numel() + 8, dtype=torch.uint8, device=cuda)
+    buf[8:].copy_(planes)
+    n0 = L.launch_count()
+    with pytest.raises(ValueError, match="aligned"):
+        K.gemm(a, b, precision=L.GEMM_BF16X3, **{given + "_planes": buf[8:]})
+    assert L.launch_count() == n0
 
 
 @pytest.mark.parametrize("m,n", [(512, 256), (256, 128), (1024, 64)])

@@ -16,6 +16,8 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "deepctr_b200", "libb2ctr.so")
 KTK_MMAS = 12          # wgmma per k-block: 64 / 16 K-steps x 3 products
+# gemm_planes_ws_kernel<BN, STAGES, GEN, FOLD>
+WS = re.compile(r"gemm_planes_ws_kernelILi(\d+)ELi(\d+)ELi(\d+)ELb([01])E")
 
 
 def _cuobjdump():
@@ -71,7 +73,10 @@ def _groups(instrs):
 
 def test_ws_kernels_overlap_consecutive_kblocks(sass):
     ws = _kernels(sass, "gemm_planes_ws_kernel")
-    assert len(ws) >= 8, sorted(sass)       # plain (TMA / cp.async, BN 32/64/128), CIN, attention, fold
+    # (BN, GEN, FOLD): plain BN 32 / 64 / 128, CIN (GEN 1) and attention (GEN 2) BN 64 / 128, and the CIN fold
+    got = sorted((int(WS.search(n).group(1)), int(WS.search(n).group(3)), WS.search(n).group(4) == "1") for n in ws)
+    assert got == sorted([(32, 0, False), (64, 0, False), (128, 0, False), (64, 1, False), (128, 1, False),
+                          (64, 2, False), (128, 2, False), (128, 0, True)]), sorted(ws)
     for name, instrs in ws.items():
         n_mma, n_close, n_empty, waits = _groups(instrs)
         assert n_empty == 0, "%s: %d empty wgmma groups" % (name, n_empty)
@@ -81,7 +86,7 @@ def test_ws_kernels_overlap_consecutive_kblocks(sass):
         assert not bad, "%s: a k-block's group is followed by %s" % (name, bad[0])
 
 
-@pytest.mark.parametrize("stem", ["gemm_planes_kernel", "gemm_bf16x3_kernel"])
+@pytest.mark.parametrize("stem", ["gemm_planes_kernel"])
 def test_other_wgmma_kernels_commit_one_group_per_kblock(sass, stem):
     ks = _kernels(sass, stem)
     assert ks, stem

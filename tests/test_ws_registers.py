@@ -9,10 +9,7 @@ import subprocess
 
 import pytest
 
-from test_sass_pipeline import LIB, _cuobjdump
-
-# gemm_planes_ws_kernel<BN, STAGES, TMA, GEN, FOLD>
-WS = re.compile(r"gemm_planes_ws_kernelILi(\d+)ELi(\d+)ELb([01])ELi(\d+)ELb([01])E")
+from test_sass_pipeline import LIB, WS, _cuobjdump
 
 
 def test_plain_ws_kernels_use_no_stack():
@@ -29,13 +26,11 @@ def test_plain_ws_kernels_use_no_stack():
             name = m.group(1)
             continue
         k = WS.search(name or "")
-        if k and k.group(4) == "0" and k.group(5) == "0":
+        if k and k.group(3) == "0" and k.group(4) == "0":
             res = dict(re.findall(r"(\w+(?:\[\d+\])?):(\d+)", line))
             if res:
                 plain[name] = res
                 name = None
-    # BN 32 / 64 / 128, each with the TMA and the cp.async producers
-    assert {(WS.search(n).group(1), WS.search(n).group(3)) for n in plain} >= \
-        {(bn, tma) for bn in ("32", "64", "128") for tma in "01"}, sorted(plain)
+    assert sorted(int(WS.search(n).group(1)) for n in plain) == [32, 64, 128], sorted(plain)
     bad = {n: (r["STACK"], r["LOCAL"]) for n, r in plain.items() if r["STACK"] != "0" or r["LOCAL"] != "0"}
     assert not bad, bad

@@ -1,6 +1,6 @@
 """Per-shape timing of the split-bf16 wgmma GEMM (CUDA events, caller-provided planes as ops.dense passes
 them) for the C2 DeepFM layer shapes: forward / dgrad / wgrad of 845->256->128->64 at batch 65536.
-usage: python tools/gemm_bench.py [variants...]   (default: 3 4)"""
+usage: python tools/gemm_bench.py [variants...]   (default: 3 4; 3 = non-persistent reference, 4 = persistent)"""
 import sys
 
 import torch
