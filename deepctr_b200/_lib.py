@@ -156,6 +156,14 @@ SIGNATURES = {
     "b2ctr_afm_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
     "b2ctr_afm_bwd": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64,
                              _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
+    "b2ctr_senet_fwd": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _i64, _vp, _i64, _vp]),
+    "b2ctr_senet_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
+    "b2ctr_senet_bwd": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64,
+                               _vp, _sz, _vp]),
+    "b2ctr_bilinear_fwd": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _i64, _vp]),
+    "b2ctr_bilinear_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
+    "b2ctr_bilinear_bwd": (_i32, [_vp, _i64, _i64, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _vp, _i64,
+                                  _vp, _sz, _vp]),
     "b2ctr_din_att_input_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),
     "b2ctr_din_att_input_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _vp]),
     "b2ctr_din_pool_fwd": (_i32, [_vp, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),

@@ -1,8 +1,10 @@
 // interaction.cu — CrossNet, CIN helpers, InteractingLayer attention core (sm_90a).
 //
 // Reference math restated (never copied): deepctr/layers/interaction.py:410-424 (CrossNet),
-// :277-325 (CIN), :754-779 (InteractingLayer).  Pairwise reductions use warp shuffles; the dense
+// :277-325 (CIN), :754-779 (InteractingLayer), :1113-1126 (SENETLayer), :1190-1209 (BilinearInteraction).  Pairwise reductions use warp shuffles; the dense
 // contractions (CIN feature-map contraction, Q/K/V projections, CrossNet-matrix) go through b2ctr_gemm.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace b2ctr {
@@ -733,6 +735,449 @@ cudaError_t afm_dispatch(int EP, int AP, const AfmArgs& a, cudaStream_t s) {
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// SENETLayer (deepctr/layers/interaction.py:1113-1126): one warp per sample, x [F, E] read in place.
+//   Z = mean_e x;  A1 = relu(Z W1) [R];  A2 = relu(A1 W2) [F];  V = x * A2[:, None]
+// Backward, with d2 = relu'(A2) . <dV_f, x_f>,  d1 = relu'(A1) . (W2 d2),  dZ = W1 d1:
+//   dx = dV * A2 + dZ / E;   dW1 = Z^T d1,  dW2 = A1^T d2   (relu' is 0 at 0, as in TF)
+// The weight gradients are summed per CTA in shared memory: the warps of a CTA take samples in lockstep rounds,
+// park (Z, A1, d1, d2) of their sample, and every entry of dW1 / dW2 has ONE owner thread that adds the round's
+// samples in warp order.  senet_reduce_kernel then sums the CTA partials in CTA order: bit-identical runs.
+// ------------------------------------------------------------------------------------------------
+constexpr int kSenetWarps = 8;
+constexpr int kSenetMaxF = 64;
+constexpr int kSenetVec = 6 * kSenetMaxF;     // per-warp vectors: z, a1, a2, d1, d2, dz
+
+__global__ void __launch_bounds__(kSenetWarps * 32)
+    senet_fwd_kernel(const float* __restrict__ x, int64_t ldx, int F, int E, int R, const float* __restrict__ W1,
+                     const float* __restrict__ W2, float* v, int64_t ldv, float* saved, int64_t batch) {
+  __shared__ float sm[kSenetWarps * kSenetVec];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* sz = sm + warp * kSenetVec;
+  float* sa1 = sz + kSenetMaxF;
+  float* sa2 = sa1 + kSenetMaxF;
+  const float inv_e = 1.f / (float)E;
+  const int64_t nw = (int64_t)gridDim.x * kSenetWarps;
+  for (int64_t b = (int64_t)blockIdx.x * kSenetWarps + warp; b < batch; b += nw) {
+    const float* xr = x + b * ldx;
+    for (int f = 0; f < F; ++f) {
+      float s = 0.f;
+      for (int e = lane; e < E; e += 32) s += xr[f * E + e];
+      s = warp_sum(s);
+      if (lane == 0) sz[f] = s * inv_e;
+    }
+    __syncwarp();
+    float* sv = saved + b * (R + F);
+    for (int r = lane; r < R; r += 32) {
+      float t = 0.f;
+      for (int f = 0; f < F; ++f) t = fmaf(sz[f], W1[f * R + r], t);
+      t = fmaxf(t, 0.f);
+      sa1[r] = t;
+      sv[r] = t;
+    }
+    __syncwarp();
+    for (int f = lane; f < F; f += 32) {
+      float t = 0.f;
+      for (int r = 0; r < R; ++r) t = fmaf(sa1[r], W2[r * F + f], t);
+      t = fmaxf(t, 0.f);
+      sa2[f] = t;
+      sv[R + f] = t;
+    }
+    __syncwarp();
+    float* vr = v + b * ldv;
+    for (int k = lane; k < F * E; k += 32) vr[k] = xr[k] * sa2[k / E];
+    __syncwarp();   // the vectors are rewritten for the next sample
+  }
+}
+
+__global__ void __launch_bounds__(kSenetWarps * 32)
+    senet_bwd_kernel(const float* __restrict__ g, int64_t ldg, const float* __restrict__ x, int64_t ldx, int F, int E,
+                     int R, const float* __restrict__ W1, const float* __restrict__ W2,
+                     const float* __restrict__ saved, float* dx, int64_t lddx, float* partial, int64_t batch) {
+  __shared__ float sm[kSenetWarps * kSenetVec + 2 * kSenetMaxF * kSenetMaxF];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* sz = sm + warp * kSenetVec;
+  float* sa1 = sz + kSenetMaxF;
+  float* sa2 = sa1 + kSenetMaxF;
+  float* sd1 = sa2 + kSenetMaxF;
+  float* sd2 = sd1 + kSenetMaxF;
+  float* sdz = sd2 + kSenetMaxF;
+  float* acc = sm + kSenetWarps * kSenetVec;     // [F*R] dW1, then [R*F] dW2; entry k owned by thread k % blockDim
+  const int nacc = 2 * F * R;
+  for (int k = threadIdx.x; k < nacc; k += blockDim.x) acc[k] = 0.f;
+  const float inv_e = 1.f / (float)E;
+  const int64_t step = (int64_t)gridDim.x * kSenetWarps;
+  for (int64_t b0 = (int64_t)blockIdx.x * kSenetWarps; b0 < batch; b0 += step) {
+    const int64_t b = b0 + warp;
+    if (b < batch) {
+      const float* xr = x + b * ldx;
+      const float* gr = g + b * ldg;
+      const float* sv = saved + b * (R + F);
+      for (int f = 0; f < F; ++f) {
+        float s = 0.f, d = 0.f;
+        for (int e = lane; e < E; e += 32) {
+          const float xv = xr[f * E + e];
+          s += xv;
+          d = fmaf(gr[f * E + e], xv, d);
+        }
+        s = warp_sum(s);
+        d = warp_sum(d);
+        if (lane == 0) {
+          const float a2 = sv[R + f];
+          sz[f] = s * inv_e;
+          sa2[f] = a2;
+          sd2[f] = a2 > 0.f ? d : 0.f;
+        }
+      }
+      __syncwarp();
+      for (int r = lane; r < R; r += 32) {
+        float t = 0.f;
+        for (int f = 0; f < F; ++f) t = fmaf(sd2[f], W2[r * F + f], t);
+        const float a1 = sv[r];
+        sa1[r] = a1;
+        sd1[r] = a1 > 0.f ? t : 0.f;
+      }
+      __syncwarp();
+      for (int f = lane; f < F; f += 32) {
+        float t = 0.f;
+        for (int r = 0; r < R; ++r) t = fmaf(sd1[r], W1[f * R + r], t);
+        sdz[f] = t * inv_e;
+      }
+      __syncwarp();
+      float* dr = dx + b * lddx;
+      for (int k = lane; k < F * E; k += 32) {
+        const int f = k / E;
+        dr[k] = fmaf(gr[k], sa2[f], sdz[f]);
+      }
+    } else {
+      for (int k = lane; k < kSenetMaxF; k += 32) sz[k] = sa1[k] = sd1[k] = sd2[k] = 0.f;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < nacc; k += blockDim.x) {
+      float a = acc[k];
+      if (k < F * R) {
+        const int f = k / R, r = k - f * R;
+        for (int w = 0; w < kSenetWarps; ++w) a = fmaf(sm[w * kSenetVec + f], sm[w * kSenetVec + 3 * kSenetMaxF + r], a);
+      } else {
+        const int q = k - F * R, r = q / F, f = q - r * F;
+        for (int w = 0; w < kSenetWarps; ++w)
+          a = fmaf(sm[w * kSenetVec + kSenetMaxF + r], sm[w * kSenetVec + 4 * kSenetMaxF + f], a);
+      }
+      acc[k] = a;
+    }
+    __syncthreads();
+  }
+  for (int k = threadIdx.x; k < nacc; k += blockDim.x) partial[(int64_t)blockIdx.x * nacc + k] = acc[k];
+}
+
+// out[k] = sum over the n CTA partials (pitch `pitch`) in ascending order
+__global__ void ordered_sum_kernel(const float* __restrict__ partial, int64_t pitch, int n, int64_t count, float* out) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < count; k += (int64_t)gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int c = 0; c < n; ++c) s += partial[(int64_t)c * pitch + k];
+    out[k] = s;
+  }
+}
+
+static inline int senet_bwd_blocks(int64_t batch) { return grid_for(batch, kSenetWarps, 4); }
+
+// ------------------------------------------------------------------------------------------------
+// BilinearInteraction (deepctr/layers/interaction.py:1190-1209).  For the P = F(F-1)/2 pairs p = (i < j) in
+// itertools.combinations order, with W_k(p) one of the stacked [E, E] weights (k = 0 'all', i 'each', p
+// 'interaction'):
+//   out_p = (x_i W_k) * x_j  [E]
+// written to out[b*ldo + col0 + p*pitch + o]: a window of a wider buffer (the DNN input) is written in place.
+// Backward from g_p (same addressing):
+//   dx_i += W_k (g_p * x_j),   dx_j += g_p * (x_i W_k),   dW_k += x_i^T (g_p * x_j)
+// Every kernel is a register-tiled [TS, EP] x [EP, EP] product on shared-memory tiles: 256 threads, each owning
+// 4 samples x 4 columns, E padded with zeros to EP in {4, 8, 16, 32, 64} (TS = 4096 / EP samples per tile).
+// * bilinear_fwd_kernel: CTA (pair, sample tile).  The pair index runs fastest so the CTAs that share a
+//   sample tile find it in L2.
+// * bilinear_dx_kernel: CTA (field, sample tile); the field's F-1 pairs are added in ascending partner order
+//   into registers: one owner per (b, f, e), no atomics.
+// * bilinear_dw_kernel: CTA (pair, batch chunk) -> partial[chunk][pair][E][E]; bilinear_dw_reduce_kernel adds,
+//   for each weight, its pairs in ascending order and each pair's chunks in ascending order.
+// ------------------------------------------------------------------------------------------------
+constexpr int kBiThreads = 256;
+constexpr int kBiMaxF = 64;
+constexpr int kBiMaxE = 64;
+constexpr int kBiDwSub = 64;      // samples staged per round of bilinear_dw_kernel
+
+__host__ __device__ __forceinline__ int bi_pair_index(int F, int i, int j) { return i * (2 * F - i - 1) / 2 + (j - i - 1); }
+__host__ __device__ __forceinline__ int bi_weight_index(int type, int i, int p) { return type == 0 ? 0 : type == 1 ? i : p; }
+__device__ __forceinline__ void bi_pair_of(int F, int p, int& i, int& j) {
+  int off = 0;
+  i = 0;
+  while (off + (F - 1 - i) <= p) { off += F - 1 - i; ++i; }
+  j = i + 1 + p - off;
+}
+
+// M[r][c] = W[r][c] (or W[c][r] when trans), zero outside [E, E]
+template <int EP>
+__device__ __forceinline__ void bi_stage_w(float* M, const float* __restrict__ W, int E, bool trans) {
+  for (int k = threadIdx.x; k < EP * EP; k += blockDim.x) {
+    const int r = k / EP, c = k - r * EP;
+    M[k] = (r < E && c < E) ? (trans ? W[c * E + r] : W[r * E + c]) : 0.f;
+  }
+}
+
+// acc[r][c] += sum_k AT[k][s0 + r] * M[k][o0 + c]
+template <int EP>
+__device__ __forceinline__ void bi_tile_mm(const float* AT, int apitch, const float* M, int s0, int o0,
+                                           float (&acc)[4][4]) {
+#pragma unroll 4
+  for (int k = 0; k < EP; ++k) {
+    const float4 a = *reinterpret_cast<const float4*>(AT + k * apitch + s0);
+    const float4 m = *reinterpret_cast<const float4*>(M + k * EP + o0);
+    const float av[4] = {a.x, a.y, a.z, a.w}, mv[4] = {m.x, m.y, m.z, m.w};
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int c = 0; c < 4; ++c) acc[r][c] = fmaf(av[r], mv[c], acc[r][c]);
+  }
+}
+
+template <int EP>
+__host__ __device__ constexpr int bi_ts() { return 4096 / EP; }
+template <int EP>
+__host__ __device__ constexpr int bi_apitch() { return bi_ts<EP>() + 4; }
+template <int EP>
+__host__ __device__ constexpr int bi_smem_floats() { return EP * bi_apitch<EP>() + EP * EP; }
+
+struct BiArgs {
+  const float* x; int64_t ldx;
+  int F, E, type;
+  const float* W;
+  float* out; int64_t ldo, col0, pitch;      // forward output / backward gradient window
+  float* dx; int64_t lddx;
+  float* partial; int nchunk;
+  int64_t batch;
+};
+
+template <int EP>
+__global__ void __launch_bounds__(kBiThreads) bilinear_fwd_kernel(const BiArgs a) {
+  constexpr int TS = bi_ts<EP>(), AP = bi_apitch<EP>(), NOG = EP / 4;
+  extern __shared__ __align__(16) float sm[];
+  float* AT = sm;
+  float* M = sm + EP * AP;
+  const int F = a.F, E = a.E, p = blockIdx.x;
+  int i, j;
+  bi_pair_of(F, p, i, j);
+  bi_stage_w<EP>(M, a.W + (int64_t)bi_weight_index(a.type, i, p) * E * E, E, false);
+  const int o0 = (threadIdx.x % NOG) * 4, s0 = (threadIdx.x / NOG) * 4;
+  const int64_t ntiles = (a.batch + TS - 1) / TS;
+  for (int64_t t = blockIdx.y; t < ntiles; t += gridDim.y) {
+    const int64_t b0 = t * TS;
+    const int ns = (int)min((int64_t)TS, a.batch - b0);
+    for (int k = threadIdx.x; k < TS * EP; k += blockDim.x) {
+      const int s = k / EP, e = k - s * EP;
+      AT[e * AP + s] = (s < ns && e < E) ? a.x[(b0 + s) * a.ldx + i * E + e] : 0.f;
+    }
+    __syncthreads();
+    float acc[4][4] = {};
+    bi_tile_mm<EP>(AT, AP, M, s0, o0, acc);
+    if (o0 < E) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        if (s0 + r >= ns) break;
+        const int64_t b = b0 + s0 + r;
+        const float* xj = a.x + b * a.ldx + j * E + o0;
+        float* o = a.out + b * a.ldo + a.col0 + (int64_t)p * a.pitch + o0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (o0 + c < E) o[c] = acc[r][c] * xj[c];
+      }
+    }
+    __syncthreads();   // AT is restaged for the next tile
+  }
+}
+
+template <int EP>
+__global__ void __launch_bounds__(kBiThreads) bilinear_dx_kernel(const BiArgs a) {
+  constexpr int TS = bi_ts<EP>(), AP = bi_apitch<EP>(), NOG = EP / 4;
+  extern __shared__ __align__(16) float sm[];
+  float* AT = sm;
+  float* M = sm + EP * AP;
+  const int F = a.F, E = a.E, f = blockIdx.x;
+  const int o0 = (threadIdx.x % NOG) * 4, s0 = (threadIdx.x / NOG) * 4;
+  const int64_t ntiles = (a.batch + TS - 1) / TS;
+  for (int64_t t = blockIdx.y; t < ntiles; t += gridDim.y) {
+    const int64_t b0 = t * TS;
+    const int ns = (int)min((int64_t)TS, a.batch - b0);
+    float dacc[4][4] = {};
+    for (int q = 0; q < F; ++q) {
+      if (q == f) continue;
+      const bool second = q < f;            // pair (q, f): f is the second field
+      const int i = second ? q : f, j = second ? f : q;
+      const int p = bi_pair_index(F, i, j);
+      bi_stage_w<EP>(M, a.W + (int64_t)bi_weight_index(a.type, i, p) * E * E, E, !second);
+      for (int k = threadIdx.x; k < TS * EP; k += blockDim.x) {
+        const int s = k / EP, e = k - s * EP;
+        float v = 0.f;
+        if (s < ns && e < E) {
+          const int64_t b = b0 + s;
+          v = a.x[b * a.ldx + q * E + e];
+          if (!second) v *= a.out[b * a.ldo + a.col0 + (int64_t)p * a.pitch + e];
+        }
+        AT[e * AP + s] = v;
+      }
+      __syncthreads();
+      float acc[4][4] = {};
+      bi_tile_mm<EP>(AT, AP, M, s0, o0, acc);
+      if (second) {
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          if (s0 + r >= ns) break;
+          const float* gp = a.out + (b0 + s0 + r) * a.ldo + a.col0 + (int64_t)p * a.pitch + o0;
+#pragma unroll
+          for (int c = 0; c < 4; ++c)
+            if (o0 + c < E) dacc[r][c] = fmaf(gp[c], acc[r][c], dacc[r][c]);
+        }
+      } else {
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int c = 0; c < 4; ++c) dacc[r][c] += acc[r][c];
+      }
+      __syncthreads();   // AT and M are restaged for the next partner
+    }
+    if (o0 < E) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        if (s0 + r >= ns) break;
+        float* d = a.dx + (b0 + s0 + r) * a.lddx + f * E + o0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (o0 + c < E) d[c] = dacc[r][c];
+      }
+    }
+  }
+}
+
+template <int EP>
+__host__ __device__ constexpr int bi_dw_smem_floats() {
+  return 2 * kBiDwSub * EP > (kBiThreads / ((EP / 4) * (EP / 4))) * EP * EP ? 2 * kBiDwSub * EP
+                                                                          : (kBiThreads / ((EP / 4) * (EP / 4))) * EP * EP;
+}
+
+template <int EP>
+__global__ void __launch_bounds__(kBiThreads) bilinear_dw_kernel(const BiArgs a) {
+  constexpr int NOG = EP / 4, NT = NOG * NOG, G = kBiThreads / NT;
+  extern __shared__ __align__(16) float sm[];
+  float* XS = sm;                          // [kBiDwSub][EP]: x_i
+  float* TT = sm + kBiDwSub * EP;          // [kBiDwSub][EP]: g_p * x_j
+  const int F = a.F, E = a.E, p = blockIdx.x, c = blockIdx.y;
+  int i, j;
+  bi_pair_of(F, p, i, j);
+  const int tl = threadIdx.x % NT, grp = threadIdx.x / NT;
+  const int e0 = (tl / NOG) * 4, o0 = (tl % NOG) * 4;
+  const int64_t per = (a.batch + a.nchunk - 1) / a.nchunk;
+  const int64_t lo = (int64_t)c * per, hi = min(a.batch, lo + per);
+  float acc[4][4] = {};
+  for (int64_t b0 = lo; b0 < hi; b0 += kBiDwSub) {
+    const int ns = (int)min((int64_t)kBiDwSub, hi - b0);
+    for (int k = threadIdx.x; k < kBiDwSub * EP; k += blockDim.x) {
+      const int s = k / EP, e = k - s * EP;
+      float xv = 0.f, tv = 0.f;
+      if (s < ns && e < E) {
+        const int64_t b = b0 + s;
+        xv = a.x[b * a.ldx + i * E + e];
+        tv = a.out[b * a.ldo + a.col0 + (int64_t)p * a.pitch + e] * a.x[b * a.ldx + j * E + e];
+      }
+      XS[k] = xv;
+      TT[k] = tv;
+    }
+    __syncthreads();
+    for (int s = grp; s < ns; s += G) {
+      const float4 xv = *reinterpret_cast<const float4*>(XS + s * EP + e0);
+      const float4 tv = *reinterpret_cast<const float4*>(TT + s * EP + o0);
+      const float av[4] = {xv.x, xv.y, xv.z, xv.w}, mv[4] = {tv.x, tv.y, tv.z, tv.w};
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[r][q] = fmaf(av[r], mv[q], acc[r][q]);
+    }
+    __syncthreads();
+  }
+  // sample groups in a fixed order
+  float* red = sm;                         // [G][EP*EP]
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) red[grp * EP * EP + (e0 + r) * EP + o0 + q] = acc[r][q];
+  __syncthreads();
+  float* dst = a.partial + ((int64_t)c * (F * (F - 1) / 2) + p) * E * E;
+  for (int k = threadIdx.x; k < E * E; k += blockDim.x) {
+    const int e = k / E, o = k - e * E;
+    float s = 0.f;
+    for (int g = 0; g < G; ++g) s += red[g * EP * EP + e * EP + o];
+    dst[k] = s;
+  }
+}
+
+// dW[k][e][o] = sum over the pairs of weight k (ascending) of the sum over their chunk partials (ascending)
+__global__ void bilinear_dw_reduce_kernel(const float* __restrict__ partial, int F, int E, int type, int nchunk,
+                                          float* dW, int64_t count) {
+  const int P = F * (F - 1) / 2;
+  const int ee = E * E;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < count; t += (int64_t)gridDim.x * blockDim.x) {
+    const int k = (int)(t / ee), q = (int)(t - (int64_t)k * ee);
+    const int plo = type == 0 ? 0 : type == 1 ? bi_pair_index(F, k, k + 1) : k;
+    const int phi = type == 0 ? P : type == 1 ? bi_pair_index(F, k, F - 1) + 1 : k + 1;
+    float s = 0.f;
+    for (int p = plo; p < phi; ++p)
+      for (int c = 0; c < nchunk; ++c) s += partial[((int64_t)c * P + p) * ee + q];
+    dW[t] = s;
+  }
+}
+
+static inline int bi_pad_e(int E) { return E <= 4 ? 4 : E <= 8 ? 8 : E <= 16 ? 16 : E <= 32 ? 32 : 64; }
+static inline int bi_num_weights(int type, int F) { return type == 0 ? 1 : type == 1 ? F - 1 : F * (F - 1) / 2; }
+// batch chunks of the weight-gradient pass: about 8 CTAs per SM over all pairs, at least 64 samples a chunk
+static inline int bi_dw_chunks(int F, int64_t batch) {
+  const int64_t P = (int64_t)F * (F - 1) / 2;
+  const int64_t want = ceil_div((int64_t)kNumSMs * 8, P);
+  const int64_t most = ceil_div(batch, kBiDwSub);
+  return (int)std::max<int64_t>(1, std::min(want, most));
+}
+static inline unsigned bi_tile_grid(int64_t batch, int TS) { return (unsigned)std::min<int64_t>(ceil_div(batch, TS), 65535); }
+
+struct BiFwd {
+  template <int EP>
+  static cudaError_t run(const BiArgs& a, cudaStream_t s) {
+    const size_t smem = sizeof(float) * bi_smem_floats<EP>();
+    const dim3 grid(a.F * (a.F - 1) / 2, bi_tile_grid(a.batch, bi_ts<EP>()));
+    bilinear_fwd_kernel<EP><<<grid, kBiThreads, smem, s>>>(a);
+    return cudaSuccess;
+  }
+};
+struct BiBwd {
+  template <int EP>
+  static cudaError_t run(const BiArgs& a, cudaStream_t s) {
+    if (a.dx) {
+      const size_t smem = sizeof(float) * bi_smem_floats<EP>();
+      bilinear_dx_kernel<EP><<<dim3(a.F, bi_tile_grid(a.batch, bi_ts<EP>())), kBiThreads, smem, s>>>(a);
+      const cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) return e;
+    }
+    if (a.partial) {
+      const size_t smem = sizeof(float) * bi_dw_smem_floats<EP>();   // <= 32 KB for every EP
+      bilinear_dw_kernel<EP><<<dim3(a.F * (a.F - 1) / 2, a.nchunk), kBiThreads, smem, s>>>(a);
+    }
+    return cudaSuccess;
+  }
+};
+template <class Op>
+cudaError_t bi_dispatch(int EP, const BiArgs& a, cudaStream_t s) {
+  switch (EP) {
+    case 4: return Op::template run<4>(a, s);
+    case 8: return Op::template run<8>(a, s);
+    case 16: return Op::template run<16>(a, s);
+    case 32: return Op::template run<32>(a, s);
+    default: return Op::template run<64>(a, s);
+  }
+}
+
 }  // namespace b2ctr
 
 using namespace b2ctr;
@@ -953,6 +1398,122 @@ b2ctr_status_t b2ctr_afm_bwd(const float* g, int64_t ldg, const float* x, int64_
   afm_reduce_kernel<<<(unsigned)ceil_div(dim * factor + 2 * factor, 128), 128, 0, ST>>>(
       partial, afm_bwd_blocks(batch), EP, AP, dim, factor, dW, dbias, dh);
   B2_CHECK_LAUNCH("b2ctr_afm_bwd(reduce)");
+  return B2CTR_OK;
+}
+
+#define SENET_REQUIRE_SHAPE(what)                                                                         \
+  B2_REQUIRE(nfield >= 2 && nfield <= kSenetMaxF && dim >= 1 && reduce >= 1 && reduce <= kSenetMaxF,       \
+             what ": needs 2 <= field count <= %d, embedding_size >= 1 and 1 <= reduction size <= %d "        \
+                  "(got %d, %d, %d)",                                                                      \
+             kSenetMaxF, kSenetMaxF, nfield, dim, reduce)
+
+b2ctr_status_t b2ctr_senet_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t reduce,
+                               const float* W1, const float* W2, float* v, int64_t ldv, float* saved, int64_t batch,
+                               void* stream) {
+  B2_REQUIRE(x && W1 && W2 && v && saved, "senet_fwd: NULL pointer");
+  SENET_REQUIRE_SHAPE("senet_fwd");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && ldv >= (int64_t)nfield * dim, "senet_fwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  senet_fwd_kernel<<<grid_for(batch, kSenetWarps, 8), kSenetWarps * 32, 0, ST>>>(x, ldx, nfield, dim, reduce, W1, W2,
+                                                                                v, ldv, saved, batch);
+  B2_CHECK_LAUNCH("b2ctr_senet_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_senet_bwd_workspace_bytes(int32_t nfield, int32_t reduce, int64_t batch) {
+  if (nfield < 1 || reduce < 1 || batch <= 0) return 0;
+  return (size_t)senet_bwd_blocks(batch) * 2 * (size_t)nfield * reduce * sizeof(float);
+}
+
+b2ctr_status_t b2ctr_senet_bwd(const float* g, int64_t ldg, const float* x, int64_t ldx, int32_t nfield, int32_t dim,
+                               int32_t reduce, const float* W1, const float* W2, const float* saved, float* dx,
+                               int64_t lddx, float* dW1, float* dW2, int64_t batch, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  B2_REQUIRE(g && x && W1 && W2 && saved && dx && dW1 && dW2, "senet_bwd: NULL pointer");
+  SENET_REQUIRE_SHAPE("senet_bwd");
+  const int64_t w = (int64_t)nfield * dim;
+  B2_REQUIRE(ldg >= w && ldx >= w && lddx >= w, "senet_bwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  const size_t need = b2ctr_senet_bwd_workspace_bytes(nfield, reduce, batch);
+  if (!workspace || workspace_bytes < need) {
+    set_error("senet_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  float* partial = (float*)workspace;
+  const int nb = senet_bwd_blocks(batch);
+  senet_bwd_kernel<<<nb, kSenetWarps * 32, 0, ST>>>(g, ldg, x, ldx, nfield, dim, reduce, W1, W2, saved, dx, lddx,
+                                                   partial, batch);
+  B2_CHECK_LAUNCH("b2ctr_senet_bwd");
+  const int64_t fr = (int64_t)nfield * reduce;
+  ordered_sum_kernel<<<(unsigned)ceil_div(fr, 128), 128, 0, ST>>>(partial, 2 * fr, nb, fr, dW1);
+  ordered_sum_kernel<<<(unsigned)ceil_div(fr, 128), 128, 0, ST>>>(partial + fr, 2 * fr, nb, fr, dW2);
+  B2_CHECK_LAUNCH("b2ctr_senet_bwd(reduce)");
+  return B2CTR_OK;
+}
+
+#define BILINEAR_REQUIRE_SHAPE(what)                                                                          \
+  B2_REQUIRE(nfield >= 2 && nfield <= kBiMaxF && dim >= 1 && dim <= kBiMaxE && type >= 0 && type <= 2,        \
+             what ": needs 2 <= field count <= %d, 1 <= embedding_size <= %d and type 0 / 1 / 2 "               \
+                  "(got %d, %d, %d)",                                                                         \
+             kBiMaxF, kBiMaxE, nfield, dim, type)
+#define BILINEAR_REQUIRE_WINDOW(what, ld, col0, pitch)                                                        \
+  B2_REQUIRE(col0 >= 0 && pitch >= dim &&                                                                     \
+                 ld >= col0 + (int64_t)(nfield * (nfield - 1) / 2 - 1) * pitch + dim,                         \
+             what ": the pair window (col0 %lld, pitch %lld) does not fit a row of %lld",                     \
+             (long long)col0, (long long)pitch, (long long)ld)
+
+b2ctr_status_t b2ctr_bilinear_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t type,
+                                  const float* W, float* out, int64_t ldo, int64_t col0, int64_t pitch, int64_t batch,
+                                  void* stream) {
+  B2_REQUIRE(x && W && out, "bilinear_fwd: NULL pointer");
+  BILINEAR_REQUIRE_SHAPE("bilinear_fwd");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim, "bilinear_fwd: ldx too small");
+  BILINEAR_REQUIRE_WINDOW("bilinear_fwd", ldo, col0, pitch);
+  if (batch <= 0) return B2CTR_OK;
+  BiArgs a{x, ldx, nfield, dim, type, W, out, ldo, col0, pitch, nullptr, 0, nullptr, 0, batch};
+  const cudaError_t err = bi_dispatch<BiFwd>(bi_pad_e(dim), a, ST);
+  if (err != cudaSuccess) {
+    set_error("bilinear_fwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_bilinear_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_bilinear_bwd_workspace_bytes(int32_t nfield, int32_t dim, int64_t batch) {
+  if (nfield < 2 || dim < 1 || batch <= 0) return 0;
+  return (size_t)bi_dw_chunks(nfield, batch) * (size_t)(nfield * (nfield - 1) / 2) * dim * dim * sizeof(float);
+}
+
+b2ctr_status_t b2ctr_bilinear_bwd(const float* g, int64_t ldg, int64_t gcol0, int64_t gpitch, const float* x,
+                                  int64_t ldx, int32_t nfield, int32_t dim, int32_t type, const float* W, float* dx,
+                                  int64_t lddx, float* dW, int64_t batch, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  B2_REQUIRE(g && x && W && (dx || dW), "bilinear_bwd: NULL pointer, or nothing to compute");
+  BILINEAR_REQUIRE_SHAPE("bilinear_bwd");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && (!dx || lddx >= (int64_t)nfield * dim), "bilinear_bwd: ld too small");
+  BILINEAR_REQUIRE_WINDOW("bilinear_bwd", ldg, gcol0, gpitch);
+  if (batch <= 0) return B2CTR_OK;
+  const size_t need = dW ? b2ctr_bilinear_bwd_workspace_bytes(nfield, dim, batch) : 0;
+  if (dW && (!workspace || workspace_bytes < need)) {
+    set_error("bilinear_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  const int nchunk = bi_dw_chunks(nfield, batch);
+  BiArgs a{x, ldx, nfield, dim, type, W, const_cast<float*>(g), ldg, gcol0, gpitch, dx, lddx,
+           dW ? (float*)workspace : nullptr, nchunk, batch};
+  const cudaError_t err = bi_dispatch<BiBwd>(bi_pad_e(dim), a, ST);
+  if (err != cudaSuccess) {
+    set_error("bilinear_bwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_bilinear_bwd");
+  if (dW) {
+    const int64_t count = (int64_t)bi_num_weights(type, nfield) * dim * dim;
+    bilinear_dw_reduce_kernel<<<grid_for(count, 256, 8), 256, 0, ST>>>((const float*)workspace, nfield, dim, type,
+                                                                     nchunk, dW, count);
+    B2_CHECK_LAUNCH("b2ctr_bilinear_bwd(reduce)");
+  }
   return B2CTR_OK;
 }
 

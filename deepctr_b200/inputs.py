@@ -352,6 +352,7 @@ class EmbeddingPlanner(object):
         self.main_ld = (self.main_width + self.tail_reserve + 3) // 4 * 4
         self.lin_ld = max(1, (self.lin_width + 3) // 4 * 4)
         self.fast = self._fast_eligible()
+        self.dnn_places = _plan_dnn_input(model, consumers, out_ids)
 
     # ---- configuration ---------------------------------------------------------------------------
     def tables(self):
@@ -837,10 +838,16 @@ class EmbeddingPlanner(object):
             self.lin_hint = True
         return None
 
+    def dnn_input_place(self, layer):
+        """(DnnInputPlacement, index) when ``layer`` writes its output into the first DNN layer's input."""
+        return self.dnn_places.get(id(layer))
+
     def append_dense(self, emb_flat, dense_flat):
         """combined_dnn_input: place the dense features behind the embeddings in the main buffer so the
         DNN input is a zero-copy window.  Returns the window or None."""
         from . import ops
+        if emb_flat.base is not None and isinstance(emb_flat.base.owner, DnnInputPlacement):
+            return emb_flat.base.owner.append_dense(emb_flat, dense_flat)
         if (emb_flat.base is None or emb_flat.base.owner is not self or emb_flat.ncols == -1
                 or emb_flat.base.ncols != self.main_width or emb_flat.base.data is None
                 or emb_flat.base.data.shape[1] != self.main_ld):
@@ -864,6 +871,124 @@ class EmbeddingPlanner(object):
             if is_pack and self.fast and len(self.main) == self.fast_n:
                 self.tail_hint = (dense_flat.col0, nd)
         return ops._window(base, 0, self.main_width + nd, (b, self.main_width + nd))
+
+
+class DnnInputPlacement(object):
+    """n BilinearInteraction layers whose [B,P,E] outputs reach the DNN only as Flatten(Concat(outputs, -1))
+    (FiBiNET, deepctr/models/fibinet.py:58), possibly followed by combined_dnn_input's dense columns.  The layers
+    write their pairs straight into one [B, ld] buffer, ld = round_up(n*P*E + n_dense, 4): pair p of layer k at
+    columns p*n*E + k*E, which is exactly the layout of the concatenation.  The Concat is then a zero-copy window,
+    combined_dnn_input copies only the dense columns behind it, and the first Dense reads the buffer in place; its
+    data gradient is adopted as the buffer's gradient and each layer's backward reads its strided part."""
+
+    def __init__(self, n, P, E, ndense):
+        self.n, self.P, self.E, self.ndense = n, P, E, ndense
+        self.width = n * P * E
+        self.ld = (self.width + ndense + 3) // 4 * 4
+        self.buf = None                 # this step's buffer Var, dropped once the backward has consumed it
+        self.outs = [None] * n
+
+    def _release(self):
+        """Forget this step's buffer (5.46 GB at C2), so that it is freed with the step's last reference and never
+        coexists with the next step's."""
+        self.buf = None
+        self.outs = [None] * self.n
+
+    def out_view(self, k, b, device):
+        """Where layer k writes its [B,P,E] output this step (a new buffer when a step starts)."""
+        if self.buf is None or self.outs[k] is not None or self.buf.data.shape[0] != b:
+            self._release()
+            t = torch.empty((b, self.ld), dtype=torch.float32, device=device)
+            self.buf = E.Var(t, ncols=self.width, owner=self, name="__dnn_input__")
+            self.outs = [None] * self.n
+        t = self.buf.data
+        return t.as_strided((b, self.P, self.E), (self.ld, self.n * self.E, 1), t.storage_offset() + k * self.E)
+
+    def placed(self, k, var):
+        var.owner = self
+        self.outs[k] = var
+
+    def placed_concat(self, xs, axis):
+        """ops.concat of the n placed outputs along the last axis: the window [0, n*P*E) of the buffer."""
+        from . import ops
+        if (self.buf is None or axis not in (-1, 2) or len(xs) != self.n
+                or any(a is not b for a, b in zip(xs, self.outs))):
+            return None
+        base, b, n, E_ = self.buf, self.buf.data.shape[0], self.n, self.E
+
+        def bwd(grads):
+            g = grads[0]
+            for k, v in enumerate(xs):
+                E.add_grad(v, g.as_strided((b, self.P, E_), (g.stride(0), n * E_, 1), g.storage_offset() + k * E_))
+            self._release()             # only the tape still holds the buffer; it goes when the backward ends
+
+        E.record([base], xs, bwd)
+        return ops._window(base, 0, self.width, (b, self.P, n * E_))
+
+    def append_dense(self, emb_flat, dense_flat):
+        from . import ops
+        nd = dense_flat.data.shape[1]
+        if (emb_flat.col0 != 0 or emb_flat.ncols != self.width or self.width + nd > self.ld
+                or dense_flat.requires_grad):
+            return None
+        src, ld = dense_flat.flat2d()
+        if src is None:
+            return None
+        base = emb_flat.base
+        b = base.data.shape[0]
+        K.copy2d(src, ld, base.data, self.ld, b, nd, dst_off=self.width)
+        base.ncols = self.width + nd
+        return ops._window(base, 0, self.width + nd, (b, self.width + nd))
+
+
+# FiBiNET's bilinear outputs written in place into the DNN input; False keeps every layer's own output buffer
+# (same results, used by the tests to compare the two)
+DNN_INPUT_PLACEMENT = True
+
+
+def _plan_dnn_input(model, consumers, out_ids):
+    """{id(BilinearInteraction layer): (DnnInputPlacement, index)}, decided once from the model's graph."""
+    if not DNN_INPUT_PLACEMENT:
+        return {}
+    from .layers.core import DNN
+    from .layers.interaction import BilinearInteraction
+    from .layers.utils import Concat, NoMask, _CombinedDNNInput
+    calls = defaultdict(int)
+    for node in model._order:
+        calls[id(node.layer)] += 1
+    places = {}
+    for node in model._order:
+        if not isinstance(node.layer, Concat) or node.layer.axis not in (-1, 2):
+            continue
+        srcs = E._flatten(node.inputs)
+        layers = [t.node.layer for t in srcs]
+        if (len(srcs) < 2 or not all(isinstance(l, BilinearInteraction) for l in layers)
+                or len(set(id(l) for l in layers)) != len(layers) or any(calls[id(l)] != 1 for l in layers)
+                or any(len(consumers[id(t)]) != 1 or id(t) in out_ids for t in srcs)
+                or len(set(tuple(t.shape) for t in srcs)) != 1):
+            continue
+        # then only Flatten / NoMask (combined_dnn_input wraps the flattened concat in both) up to the DNN input
+        flat, fc = node.outputs[0], None
+        while True:
+            fc = consumers[id(flat)]
+            if len(fc) != 1 or id(flat) in out_ids or not isinstance(fc[0].layer, (E.Flatten, NoMask)):
+                break
+            flat = fc[0].outputs[0]
+        if flat is node.outputs[0] or len(fc) != 1 or id(flat) in out_ids or len(flat.shape) != 2:
+            continue
+        ndense = 0
+        if isinstance(fc[0].layer, _CombinedDNNInput):
+            ins = E._flatten(fc[0].inputs)
+            if ins[0] is not flat:
+                continue
+            ndense = int(np.prod(ins[1].shape[1:]))
+        elif not isinstance(fc[0].layer, DNN):
+            continue
+        _, P, Ed = srcs[0].shape
+        pl = DnnInputPlacement(len(srcs), int(P), int(Ed), ndense)
+        for k, l in enumerate(layers):
+            places[id(l)] = (pl, k)
+    return places
 
 
 # ================================================================================================

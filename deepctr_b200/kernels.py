@@ -671,6 +671,61 @@ def afm_bwd(g, x, ldx, nfield, dim, W, bias, h, state, att, batch):
     return dx, dW, db, dh
 
 
+def senet_fwd(x, ldx, nfield, dim, W1, W2, batch):
+    """SENETLayer on a [B, nfield*dim] window (pitch ldx) -> (V [B, nfield*dim], saved (A1, A2) [B, R + nfield])."""
+    _require_cuda(x, W1, W2)
+    reduce = W1.shape[1]
+    v = torch.empty((batch, nfield * dim), dtype=torch.float32, device=x.device)
+    saved = torch.empty((batch, reduce + nfield), dtype=torch.float32, device=x.device)
+    _lib_call("senet_fwd", ptr(x), ldx, nfield, dim, reduce, ptr(W1), ptr(W2), ptr(v), nfield * dim, ptr(saved),
+              batch, stream())
+    return v, saved
+
+
+def senet_bwd(g, x, ldx, nfield, dim, W1, W2, saved, batch):
+    """-> (dx [B, nfield*dim], dW1 [nfield, R], dW2 [R, nfield])."""
+    _require_cuda(g, x, W1, W2, saved)
+    reduce = W1.shape[1]
+    dev = x.device
+    dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=dev)
+    dW1 = torch.empty((nfield, reduce), dtype=torch.float32, device=dev)
+    dW2 = torch.empty((reduce, nfield), dtype=torch.float32, device=dev)
+    nbytes = L.lib().b2ctr_senet_bwd_workspace_bytes(nfield, reduce, batch)
+    ws = workspace(nbytes, dev)
+    _lib_call("senet_bwd", ptr(g), g.stride(0), ptr(x), ldx, nfield, dim, reduce, ptr(W1), ptr(W2), ptr(saved),
+              ptr(dx), nfield * dim, ptr(dW1), ptr(dW2), batch, ptr(ws), nbytes, stream())
+    return dx, dW1, dW2
+
+
+BILINEAR_TYPES = {"all": 0, "each": 1, "interaction": 2}
+
+
+def bilinear_fwd(x, ldx, nfield, dim, btype, W, batch, out=None, col0=0, pitch=None):
+    """BilinearInteraction on a [B, nfield*dim] window (pitch ldx) with the stacked weights W [nW, dim, dim].
+    Pair p goes to columns [col0 + p*pitch, +dim) of ``out`` [B, ld] (default: a new [B, P*dim])."""
+    _require_cuda(x, W)
+    P = nfield * (nfield - 1) // 2
+    if out is None:
+        out = torch.empty((batch, P * dim), dtype=torch.float32, device=x.device)
+    pitch = dim if pitch is None else pitch
+    _lib_call("bilinear_fwd", ptr(x), ldx, nfield, dim, BILINEAR_TYPES[btype], ptr(W), ptr(out), out.stride(0), col0,
+              pitch, batch, stream())
+    return out
+
+
+def bilinear_bwd(g, ldg, gcol0, gpitch, x, ldx, nfield, dim, btype, W, batch, want_dx=True, want_dw=True):
+    """g: the data pointer of the gradient buffer addressed like the forward's output -> (dx [B, nfield*dim], dW)."""
+    _require_cuda(g, x, W)
+    dev = x.device
+    dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=dev) if want_dx else None
+    dW = torch.empty(tuple(W.shape), dtype=torch.float32, device=dev) if want_dw else None
+    nbytes = L.lib().b2ctr_bilinear_bwd_workspace_bytes(nfield, dim, batch) if want_dw else 0
+    ws = workspace(nbytes, dev) if want_dw else None
+    _lib_call("bilinear_bwd", ptr(g), ldg, gcol0, gpitch, ptr(x), ldx, nfield, dim, BILINEAR_TYPES[btype], ptr(W),
+              ptr(dx), nfield * dim, ptr(dW), batch, ptr(ws), nbytes, stream())
+    return dx, dW
+
+
 def din_att_input_fwd(q, ldq, keys, ldk, batch, T, E):
     out = torch.empty((batch, T, 4 * E), dtype=torch.float32, device=q.device)
     _lib_call("din_att_input_fwd", ptr(q), ldq, ptr(keys), ldk, ptr(out), batch, T, E, stream())
@@ -779,7 +834,7 @@ def dropout(x, rate, seed):
 for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
            "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
-           "afm_bwd", "din_att_input_fwd", "din_att_input_bwd",
+           "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
     globals()[_n] = _timed(globals()[_n])
@@ -832,7 +887,7 @@ for _n in ("shard_bucketize", "shard_fill", "shard_gather_rows", "shard_scatter_
 for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
            "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
-           "afm_bwd", "din_att_input_fwd", "din_att_input_bwd",
+           "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "moving_update", "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
     globals()[_n] = _timed(globals()[_n])

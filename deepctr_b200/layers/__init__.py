@@ -2,7 +2,8 @@
 from ..engine import Layer, Dense, Flatten, Concatenate, Add, Lambda, Input
 from .activation import Dice, Activation, activation_layer
 from .core import DNN, LocalActivationUnit, PredictionLayer
-from .interaction import AFMLayer, BiInteractionPooling, FM, CrossNet, CIN, InteractingLayer
+from .interaction import (AFMLayer, BiInteractionPooling, BilinearInteraction, FM, CrossNet, CIN, InteractingLayer,
+                          SENETLayer)
 from .normalization import BatchNormalization, Dropout
 from .sequence import SequencePoolingLayer, WeightedSequenceLayer, AttentionSequencePoolingLayer
 from .utils import (NoMask, Hash, Linear, Concat, _Add, concat_func, add_func, combined_dnn_input,
@@ -11,6 +12,7 @@ from .utils import (NoMask, Hash, Linear, Concat, _Add, concat_func, add_func, c
 custom_objects = {
     'DNN': DNN, 'PredictionLayer': PredictionLayer, 'LocalActivationUnit': LocalActivationUnit,
     'AFMLayer': AFMLayer, 'BiInteractionPooling': BiInteractionPooling,
+    'SENETLayer': SENETLayer, 'BilinearInteraction': BilinearInteraction,
     'FM': FM, 'CrossNet': CrossNet, 'CIN': CIN, 'InteractingLayer': InteractingLayer,
     'SequencePoolingLayer': SequencePoolingLayer, 'WeightedSequenceLayer': WeightedSequenceLayer,
     'AttentionSequencePoolingLayer': AttentionSequencePoolingLayer, 'Dice': Dice, 'Hash': Hash,

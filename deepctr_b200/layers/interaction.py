@@ -1,7 +1,11 @@
 """Host mirror of deepctr/layers/interaction.py for the operators on the hot path:
 AFMLayer (:39-160), BiInteractionPooling (:163-206), FM (:563-607), CrossNet (:344-435), CIN (:209-341),
-InteractingLayer (:697-790).
+InteractingLayer (:697-790), SENETLayer (:1067-1139), BilinearInteraction (:1142-1221).
 Same constructor arguments, weight names, shape checks and error messages as the reference."""
+import itertools
+
+import torch
+
 from .. import engine as E
 from .. import ops
 from ..engine import Layer, Lambda, Zeros, glorot_normal, glorot_uniform, TruncatedNormal, l2
@@ -9,6 +13,8 @@ from .normalization import Dropout
 
 # shapes the fused AFM kernels serve (include/b2ctr.h, b2ctr_afm_fwd)
 AFM_MAX_FIELDS, AFM_MAX_EMBEDDING, AFM_MAX_FACTOR = 64, 32, 16
+# shapes the SENET / bilinear kernels serve (include/b2ctr.h, b2ctr_senet_fwd, b2ctr_bilinear_fwd)
+SENET_MAX_FIELDS, BILINEAR_MAX_FIELDS, BILINEAR_MAX_EMBEDDING = 64, 64, 64
 
 
 class AFMLayer(Layer):
@@ -281,6 +287,133 @@ class InteractingLayer(Layer):
     def get_config(self):
         config = {'att_embedding_size': self.att_embedding_size, 'head_num': self.head_num,
                   'use_res': self.use_res, 'seed': self.seed}
+        base = Layer.get_config(self)
+        base.update(config)
+        return base
+
+
+class SENETLayer(Layer):
+    """SENET of FiBiNET, deepctr/layers/interaction.py:1067-1139.  Called on a list of F [B,1,E] tensors; returns F
+    [B,1,E] windows of V = x * relu(relu(mean_e(x) W_1) W_2)[:, :, None] (b2ctr_senet_fwd / _bwd: the input is read
+    in place, only V and the [B, R + F] excitation are written)."""
+
+    def __init__(self, reduction_ratio=3, seed=1024, **kwargs):
+        self.reduction_ratio = reduction_ratio
+        self.seed = seed
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        if not isinstance(input_shape, list) or len(input_shape) < 2:
+            raise ValueError('A `AttentionalFM` layer should be called '
+                             'on a list of at least 2 inputs')
+        self.filed_size = len(input_shape)
+        self.embedding_size = input_shape[0][-1]
+        reduction_size = max(1, self.filed_size // self.reduction_ratio)
+        if self.filed_size > SENET_MAX_FIELDS or not 1 <= reduction_size <= SENET_MAX_FIELDS:
+            raise ValueError("SENETLayer supports up to %d inputs and a reduction size of 1 to %d "
+                             "(got %d inputs, reduction size %r)"
+                             % (SENET_MAX_FIELDS, SENET_MAX_FIELDS, self.filed_size, reduction_size))
+        self.W_1 = self.add_weight(shape=(self.filed_size, reduction_size), initializer=glorot_normal(seed=self.seed),
+                                   name="W_1")
+        self.W_2 = self.add_weight(shape=(reduction_size, self.filed_size), initializer=glorot_normal(seed=self.seed),
+                                   name="W_2")
+        # the reference creates this layer here: it takes the next `lambda` name
+        self.tensordot = self._track(Lambda(lambda x: ops.dense(x[0], x[1]), name=self.name + "/tensordot"))
+        self.built = True
+
+    def call(self, inputs, training=None, **kwargs):
+        if inputs[0].data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs[0].data.dim()))
+        x = ops.concat(inputs, axis=1)           # a zero-copy window of the fused gather's buffer
+        b, f, e = x.data.shape
+        v = ops.senet(x, self.W_1, self.W_2)
+        return [ops._window(v, i * e, e, (b, 1, e)) for i in range(f)]
+
+    def compute_output_shape(self, input_shape):
+        return input_shape
+
+    def compute_mask(self, inputs, mask=None):
+        return [None] * self.filed_size
+
+    def get_config(self):
+        config = {'reduction_ratio': self.reduction_ratio, 'seed': self.seed}
+        base = Layer.get_config(self)
+        base.update(config)
+        return base
+
+
+class BilinearInteraction(Layer):
+    """Bilinear interaction of FiBiNET, deepctr/layers/interaction.py:1142-1221.  Called on a list of F [B,1,E]
+    tensors; output [B, P, E] with row p = (i < j) equal to (v_i W) * v_j, W one weight ('all'), one per first field
+    ('each') or one per pair ('interaction').  The weights keep the reference's names and order but their data are
+    views of one stacked [nW, E, E] buffer, which is what b2ctr_bilinear_fwd / _bwd take.  When the model's graph
+    lets it (inputs.DnnInputPlacement), the pairs are written straight into the first DNN layer's input."""
+
+    def __init__(self, bilinear_type="interaction", seed=1024, **kwargs):
+        self.bilinear_type = bilinear_type
+        self.seed = seed
+        self._stack = None
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        if not isinstance(input_shape, list) or len(input_shape) < 2:
+            raise ValueError('A `AttentionalFM` layer should be called '
+                             'on a list of at least 2 inputs')
+        embedding_size = int(input_shape[0][-1])
+        if len(input_shape) > BILINEAR_MAX_FIELDS or embedding_size > BILINEAR_MAX_EMBEDDING:
+            raise ValueError("BilinearInteraction supports up to %d inputs and embedding_size <= %d "
+                             "(got %d inputs, embedding_size %d)"
+                             % (BILINEAR_MAX_FIELDS, BILINEAR_MAX_EMBEDDING, len(input_shape), embedding_size))
+        shape = (embedding_size, embedding_size)
+        if self.bilinear_type == "all":
+            self.W = self.add_weight(shape=shape, initializer=glorot_normal(seed=self.seed), name="bilinear_weight")
+        elif self.bilinear_type == "each":
+            self.W_list = [self.add_weight(shape=shape, initializer=glorot_normal(seed=self.seed),
+                                           name="bilinear_weight" + str(i)) for i in range(len(input_shape) - 1)]
+        elif self.bilinear_type == "interaction":
+            self.W_list = [self.add_weight(shape=shape, initializer=glorot_normal(seed=self.seed),
+                                           name="bilinear_weight" + str(i) + '_' + str(j))
+                           for i, j in itertools.combinations(range(len(input_shape)), 2)]
+        else:
+            raise NotImplementedError
+        self.built = True
+
+    def _weights_stacked(self):
+        """The weights' device data as views of one [nW, E, E] buffer (built on the first call)."""
+        ws = [self.W] if self.bilinear_type == "all" else self.W_list
+        st = self._stack
+        if st is None or ws[0].data is None or ws[0].data.data_ptr() != st.data_ptr() or ws[-1].data is None \
+                or ws[-1].data.data_ptr() != st[-1].data_ptr():
+            st = torch.stack([w.materialize() for w in ws])
+            for k, w in enumerate(ws):
+                w.data = st[k]
+            self._stack = st
+        return ws, st
+
+    def call(self, inputs, **kwargs):
+        if inputs[0].data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs[0].data.dim()))
+        if self.bilinear_type not in ("all", "each", "interaction"):
+            raise NotImplementedError
+        x = ops.concat(inputs, axis=1)
+        ws, st = self._weights_stacked()
+        planner = getattr(self, "_planner", None)
+        place = planner.dnn_input_place(self) if planner is not None else None
+        if place is None:
+            return ops.bilinear_interaction(x, ws, st, self.bilinear_type)
+        pl, k = place
+        b, f, e = x.data.shape
+        out = ops.bilinear_interaction(x, ws, st, self.bilinear_type, out=pl.out_view(k, b, x.data.device))
+        pl.placed(k, out)
+        return out
+
+    def compute_output_shape(self, input_shape):
+        filed_size = len(input_shape)
+        embedding_size = input_shape[0][-1]
+        return (None, filed_size * (filed_size - 1) // 2, embedding_size)
+
+    def get_config(self):
+        config = {'bilinear_type': self.bilinear_type, 'seed': self.seed}
         base = Layer.get_config(self)
         base.update(config)
         return base

@@ -5,5 +5,6 @@ from .autoint import AutoInt
 from .sequence import DIN
 from .nfm import NFM
 from .afm import AFM
+from .fibinet import FiBiNET
 
-__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM"]
+__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET"]

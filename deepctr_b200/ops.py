@@ -214,6 +214,11 @@ def concat(xs, axis=-1):
     xs = list(xs)
     if len(xs) == 1:
         return xs[0]
+    placed = getattr(xs[0].owner, "placed_concat", None)
+    if placed is not None:             # outputs written side by side into one buffer (inputs.DnnInputPlacement)
+        res = placed(xs, axis)
+        if res is not None:
+            return res
     shapes = [tuple(v.shape) for v in xs]
     ax, flat_ok = _flat_concat_ok(shapes, axis)
     out_shape = list(shapes[0])
@@ -445,6 +450,61 @@ def afm(x, w, bias, h):
             E.add_grad(h, dh.reshape(hd.shape))
 
     E.record([res], [x, w, bias, h], bwd)
+    return res
+
+
+def senet(x, w1, w2):
+    """[B,F,E] -> V [B,F,E]: x reweighted by relu(relu(mean_e(x) W1) W2) (SENETLayer, layers/interaction.py:1119-1124).
+    x is read in place; only V and the [B, R + F] excitation (A1, A2) are written."""
+    b, f, e = x.data.shape
+    src, ld = _fields2d(x)
+    w1d, w2d = _wdata(w1), _wdata(w2)
+    v, saved = K.senet_fwd(src, ld, f, e, w1d, w2d, b)
+    res = E.Var(v)                       # [B, F*E]: the layer hands out per-field windows of it
+
+    def bwd(grads):
+        g = grads[0]
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dx, dw1, dw2 = K.senet_bwd(g.reshape(b, f * e), src, ld, f, e, w1d, w2d, saved, b)
+        E.add_grad(x, dx.reshape(x.data.shape))
+        if w1.requires_grad:
+            E.add_grad(w1, dw1)
+        if w2.requires_grad:
+            E.add_grad(w2, dw2)
+
+    E.record([res], [x, w1, w2], bwd)
+    return res
+
+
+def bilinear_interaction(x, weights, stack, btype, out=None):
+    """[B,F,E] -> [B,P,E]: (v_i W_k) * v_j for the pairs i < j (BilinearInteraction, layers/interaction.py:1196-1208).
+    ``stack`` [nW,E,E] holds the data of ``weights`` (each weight's data is a view of it); the gradient comes back
+    as one stacked buffer handed to each weight as a view.  ``out``: a strided [B,P,E] view of a wider buffer to
+    write the pairs into (the DNN input, see inputs.DnnInputPlacement); default a new [B,P,E] tensor."""
+    b, f, e = x.data.shape
+    P = f * (f - 1) // 2
+    src, ld = _fields2d(x)
+    if out is None:
+        out = K.bilinear_fwd(src, ld, f, e, btype, stack, b).reshape(b, P, e)
+    else:
+        K.bilinear_fwd(src, ld, f, e, btype, stack, b, out=out, col0=0, pitch=out.stride(1))
+    res = E.Var(out)
+
+    def bwd(grads):
+        g = grads[0].reshape(b, P, e)
+        if g.stride(2) != 1 or g.stride(1) < e:
+            g = g.contiguous()
+        want_dw = any(w.requires_grad for w in weights)
+        dx, dw = K.bilinear_bwd(g, g.stride(0), 0, g.stride(1), src, ld, f, e, btype, stack, b,
+                                want_dx=x.requires_grad, want_dw=want_dw)
+        if dx is not None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        for k, w in enumerate(weights):
+            if w.requires_grad:
+                E.add_grad(w, dw[k])
+
+    E.record([res], [x] + list(weights), bwd)
     return res
 
 

@@ -491,6 +491,43 @@ B2CTR_API b2ctr_status_t b2ctr_afm_bwd(const float* g, int64_t ldg, const float*
                                       float* dx, int64_t lddx, float* dW, float* dbias, float* dh, int64_t batch,
                                       void* workspace, size_t workspace_bytes, void* stream);
 
+/* SENETLayer (deepctr/layers/interaction.py:1067-1139) on x [B, nfield, dim] (row pitch ldx), W1 [nfield, reduce],
+ * W2 [reduce, nfield]:
+ *   Z = mean_e x;  A1 = relu(Z W1);  A2 = relu(A1 W2);  v[b*ldv + f*dim + e] = x[b,f,e] * A2[b,f]
+ *   saved [B, reduce + nfield] = (A1, A2), kept for the backward.
+ * Limits: 2 <= nfield <= 64, 1 <= reduce <= 64; anything else is B2CTR_ERR_INVALID_ARG. */
+B2CTR_API b2ctr_status_t b2ctr_senet_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t reduce,
+                                        const float* W1, const float* W2, float* v, int64_t ldv, float* saved,
+                                        int64_t batch, void* stream);
+/* Backward from g = dV (pitch ldg): dx = g * A2 + dZ / dim (pitch lddx, overwritten), dW1, dW2 (overwritten).
+ * The gradient of relu at 0 is 0.  Weight gradients go through per-CTA partials in the workspace, summed in a
+ * fixed order: bit-identical from run to run. */
+B2CTR_API size_t b2ctr_senet_bwd_workspace_bytes(int32_t nfield, int32_t reduce, int64_t batch);
+B2CTR_API b2ctr_status_t b2ctr_senet_bwd(const float* g, int64_t ldg, const float* x, int64_t ldx, int32_t nfield,
+                                        int32_t dim, int32_t reduce, const float* W1, const float* W2,
+                                        const float* saved, float* dx, int64_t lddx, float* dW1, float* dW2,
+                                        int64_t batch, void* workspace, size_t workspace_bytes, void* stream);
+
+/* BilinearInteraction (deepctr/layers/interaction.py:1142-1221) on x [B, nfield, dim] (row pitch ldx) and the
+ * stacked weights W [nW, dim, dim]: type 0 'all' (nW = 1), 1 'each' (nW = nfield - 1, W_i for the pairs (i, j)),
+ * 2 'interaction' (nW = P, one per pair).  For the P = nfield(nfield-1)/2 pairs p = (i < j) in
+ * itertools.combinations order:
+ *   out[b*ldo + col0 + p*pitch + o] = (x_i W_k)[o] * x_j[o]
+ * so the output can be a window of a wider buffer (the first DNN layer's input); nothing else is written.
+ * Limits: 2 <= nfield <= 64, 1 <= dim <= 64, pitch >= dim. */
+B2CTR_API b2ctr_status_t b2ctr_bilinear_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t type,
+                                           const float* W, float* out, int64_t ldo, int64_t col0, int64_t pitch,
+                                           int64_t batch, void* stream);
+/* Backward from g, addressed like the forward's output (ldg, gcol0, gpitch), read in place:
+ *   dx [B, nfield*dim] (pitch lddx, overwritten; may be NULL), dW [nW, dim, dim] (overwritten; may be NULL).
+ * Every dx element has one owner that adds its pairs in a fixed order; dW goes through ordered partials in the
+ * workspace.  No float atomics: bit-identical from run to run. */
+B2CTR_API size_t b2ctr_bilinear_bwd_workspace_bytes(int32_t nfield, int32_t dim, int64_t batch);
+B2CTR_API b2ctr_status_t b2ctr_bilinear_bwd(const float* g, int64_t ldg, int64_t gcol0, int64_t gpitch,
+                                           const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t type,
+                                           const float* W, float* dx, int64_t lddx, float* dW, int64_t batch,
+                                           void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* 6. Sequence operators (DIN, pooling, Dice / BatchNormalization, dropout)                     */
 /* ------------------------------------------------------------------------------------------ */

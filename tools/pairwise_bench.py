@@ -1,16 +1,19 @@
 #!/usr/bin/env python
-"""NFM / AFM on the C2 synthetic set (26 tables x 1M rows, emb_dim 32, batch 65536, uniform ids; NFM also gets the
-13 dense features, AFM takes none: its builder refuses DenseFeat) and the fused pairwise kernels at that shape.
+"""NFM / AFM / FiBiNET on the C2 synthetic set (26 tables x 1M rows, emb_dim 32, batch 65536, uniform ids; NFM and
+FiBiNET also get the 13 dense features, AFM takes none: its builder refuses DenseFeat) and the pairwise kernels at
+that shape.
 
-    python tools/pairwise_bench.py [--steps 20] [--warmup 5] [--reps 50]
+    python tools/pairwise_bench.py [--steps 20] [--warmup 5] [--reps 50] [--models NFM,AFM,FiBiNET]
 
 Prints one JSON line per measurement:
   * the hardware context (card, power limit, max SM clock), read in the same run;
   * the training step (graph-replayed once warm) of NFM (256, 128, 64) and AFM (attention_factor 8): device time
     from CUDA events and samples/s;
-  * forward and backward of b2ctr_afm_* and b2ctr_bi_interaction_*: median over --reps launches, with the FFMA bound
-    (132 SMs x 128 FP32 lanes x 2 flop x max SM clock) and the HBM bound (3.35 TB/s, H100 SXM data sheet) of the
-    flops and bytes their shapes imply.
+  * forward and backward of b2ctr_afm_*, b2ctr_bi_interaction_*, b2ctr_senet_* and b2ctr_bilinear_* (each type):
+    median over --reps launches, with the FFMA bound (132 SMs x 128 FP32 lanes x 2 flop x max SM clock) and the HBM
+    bound (3.35 TB/s, H100 SXM data sheet) of the flops and bytes their shapes imply;
+  * FiBiNET's first DNN layer alone: the split of its [65536, 20816] operand into bf16 planes and the three
+    20813 -> 256 GEMMs (forward, data gradient, weight gradient), so the step can be broken down.
 """
 import argparse
 import json
@@ -53,6 +56,9 @@ def step_time(builder, steps, warmup):
     E.clear_session()
     if builder == "NFM":
         model = M.NFM(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding=0)
+    elif builder == "FiBiNET":
+        model = M.FiBiNET(cols, cols, bilinear_type="interaction", dnn_hidden_units=(256, 128, 64), l2_reg_linear=0,
+                          l2_reg_embedding=0)
     else:
         model = M.AFM(cols, cols, attention_factor=8, l2_reg_linear=0, l2_reg_embedding=0, l2_reg_att=0)
     bench.seed_initializers(model)
@@ -136,20 +142,100 @@ def kernels(reps, hw):
     return out
 
 
+def _report(name, shape, reps, fn, flops, nbytes, ffma_peak):
+    med, lo, hi = median_us(fn, reps)
+    return {"what": "kernel", "kernel": name, "shape": shape, "reps": reps, "median_us": med, "min_us": lo,
+            "max_us": hi, "flops": flops, "bytes": nbytes, "hbm_bound_us": nbytes / HBM_BYTES_PER_S * 1e6,
+            "ffma_bound_us": flops / ffma_peak * 1e6 if ffma_peak else None}
+
+
+def fibinet_kernels(reps, hw):
+    """SENET and the bilinear kernels at C2 (26 fields, E = 32, B = 65536), the pairs written into the [B, 20816]
+    DNN input as FiBiNET places them; then the split and the GEMMs of the 20813 -> 256 first layer."""
+    import torch
+    from deepctr_b200 import _lib as L, kernels as K, ops
+    B, F, E, nd, R = 65536, 26, 32, 13, 8
+    P = F * (F - 1) // 2
+    dev = torch.device("cuda", 0)
+    g = torch.Generator(device=dev).manual_seed(2)
+    clk = hw.get("max_sm_clock_mhz") or None
+    ffma_peak = 132 * 128 * 2 * clk * 1e6 if clk else None
+    ldx = F * E + nd + 3
+    buf = torch.randn((B, ldx), device=dev, generator=g) * 0.1
+    xw = buf[:, :F * E]
+    W1 = torch.randn((F, R), device=dev, generator=g) * 0.3
+    W2 = torch.randn((R, F), device=dev, generator=g) * 0.3
+    kd = 2 * P * E + nd
+    ld = (kd + 3) // 4 * 4
+    dnn_in = torch.randn((B, ld), device=dev, generator=g) * 0.1       # also the bilinear outputs' gradient
+    shape = dict(B=B, F=F, E=E, P=P, ldx=ldx, ld_out=ld)
+    x_bytes, v_bytes = B * F * E * 4, B * F * E * 4
+    v, saved = K.senet_fwd(xw, ldx, F, E, W1, W2, B)
+    out = [_report("senet_fwd", shape, reps, lambda: K.senet_fwd(xw, ldx, F, E, W1, W2, B),
+                   B * (F * E * 2 + 4 * F * R), x_bytes + v_bytes + B * (R + F) * 4, ffma_peak),
+           _report("senet_bwd", shape, reps, lambda: K.senet_bwd(v, xw, ldx, F, E, W1, W2, saved, B),
+                   B * (F * E * 6 + 8 * F * R), 3 * x_bytes + B * (R + F) * 4, ffma_peak)]
+    pair_bytes = B * P * E * 4
+    for t in ("all", "each", "interaction"):
+        nw = 1 if t == "all" else F - 1 if t == "each" else P
+        W = torch.randn((nw, E, E), device=dev, generator=g) / E ** 0.5
+        # forward: (v_i W) per pair 2E^2 + the product E; backward: dx (2 x 2E^2 + E), dW (2E^2 + E) per pair
+        out.append(_report("bilinear_fwd_" + t, shape, reps,
+                           lambda: K.bilinear_fwd(xw, ldx, F, E, t, W, B, out=dnn_in, col0=0, pitch=2 * E),
+                           B * P * (2 * E * E + E), x_bytes + pair_bytes, ffma_peak))
+        gv = dnn_in[:, E:]
+        out.append(_report("bilinear_bwd_" + t, shape, reps,
+                           lambda: K.bilinear_bwd(gv, ld, 0, 2 * E, xw, ldx, F, E, t, W, B),
+                           B * P * (6 * E * E + 3 * E), 2 * x_bytes + 3 * pair_bytes, ffma_peak))
+        del W
+    # the first DNN layer 20813 -> 256 on the placed buffer, timed alone
+    n = 256
+    x2 = dnn_in[:, :kd]
+    w = torch.randn((kd, n), device=dev, generator=g) / kd ** 0.5
+    dz = torch.randn((B, n), device=dev, generator=g) / B
+    xp, wp, dzp = K.split_planes(x2), K.split_planes(w), K.split_planes(dz)
+    gshape = dict(m=B, k=kd, n=n, ld=ld)
+    bf = L.GEMM_BF16X3
+    dxbuf = torch.empty((B, ld), device=dev)
+    gemm_flops = 2 * B * kd * n
+    out.append(_report("split_planes_dnn_input", gshape, reps, lambda: K.split_planes(x2), 0,
+                       B * kd * 4 + B * kd * 4, ffma_peak))
+    out.append(_report("gemm_fwd_20813x256", gshape, reps,
+                       lambda: K.gemm(x2, w, act=L.ACT_RELU, precision=bf, m=B, n=n, k=kd, a_planes=xp, b_planes=wp),
+                       gemm_flops, B * kd * 4 + B * n * 4, None))
+    out.append(_report("gemm_dgrad_20813x256", gshape, reps,
+                       lambda: K.gemm(dz, w, c=dxbuf[:, :kd], trans_b=True, precision=bf, m=B, n=kd, k=n,
+                                      a_planes=dzp, b_planes=wp),
+                       gemm_flops, B * kd * 4 + B * n * 4, None))
+    out.append(_report("gemm_wgrad_20813x256", gshape, reps,
+                       lambda: K.gemm(x2, dz, trans_a=True, precision=bf, split_k=ops._split_k(kd, n, B), m=kd, n=n,
+                                      k=B, a_planes=xp, b_planes=dzp),
+                       gemm_flops, B * kd * 4 + B * n * 4, None))
+    del buf, dnn_in, xp, dxbuf
+    torch.cuda.empty_cache()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--reps", type=int, default=50)
+    ap.add_argument("--models", default="NFM,AFM,FiBiNET")
     args = ap.parse_args()
+    models = args.models.split(",")
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("pairwise_bench.py needs a CUDA device")
     hw = hardware()
     print(json.dumps(dict(what="hardware", **hw)), flush=True)
-    for r in kernels(args.reps, hw):
-        print(json.dumps(r), flush=True)
-    for builder in ("NFM", "AFM"):
+    if "NFM" in models or "AFM" in models:
+        for r in kernels(args.reps, hw):
+            print(json.dumps(r), flush=True)
+    if "FiBiNET" in models:
+        for r in fibinet_kernels(args.reps, hw):
+            print(json.dumps(r), flush=True)
+    for builder in models:
         print(json.dumps(step_time(builder, args.steps, args.warmup)), flush=True)
 
 
