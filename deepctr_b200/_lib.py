@@ -48,9 +48,7 @@ class UniformGather(C.Structure):
                 ("ldx", C.c_int64), ("dense_ld", C.c_int64), ("x_cols", C.c_int64),
                 ("nfeat", C.c_int32),
                 ("ndense", C.c_int32), ("fm_mask", C.c_uint64 * 2), ("flags", C.c_int32), ("world", C.c_int32),
-                ("peer_tables", C.c_void_p), ("peer_lin_tables", C.c_void_p),
-                ("x_planes", C.c_void_p), ("x_planes_cols", C.c_int64),
-                ("l2_window", C.c_void_p), ("l2_window_bytes", C.c_int64), ("l2_hit_ratio", C.c_float)]
+                ("peer_tables", C.c_void_p), ("peer_lin_tables", C.c_void_p)]
 
 
 class Gemm(C.Structure):
@@ -100,8 +98,6 @@ SIGNATURES = {
     "b2ctr_init_normal": (_i32, [_vp, _i64, _f32, _f32, _u64, _vp]),
     "b2ctr_gemm_workspace_bytes": (_sz, [C.POINTER(Gemm)]),
     "b2ctr_enable_peer_access": (_i32, [_i32]),
-    "b2ctr_l2_persist_reserve": (_i32, [_i64, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
-    "b2ctr_set_l2_fetch_granularity": (_i32, [_i32]),
     "b2ctr_host_pack": (_i32, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64), _i32, _vp, _i32]),
     "b2ctr_gemm": (_i32, [C.POINTER(Gemm), _vp, _sz, _vp]),
     "b2ctr_planes_bytes": (_sz, [_i64, _i64]),

@@ -30,7 +30,7 @@ unsigned long long* oob_counter() {
 }  // namespace b2ctr
 
 extern "C" {
-int32_t b2ctr_abi_version(void) { return 1; }
+int32_t b2ctr_abi_version(void) { return 2; }
 b2ctr_status_t b2ctr_embed_oob_count(int64_t* count, int32_t reset, void* stream) {
   B2_REQUIRE(count, "embed_oob_count: NULL count");
   unsigned long long* d = b2ctr::oob_counter();
@@ -52,36 +52,6 @@ b2ctr_status_t b2ctr_embed_oob_count(int64_t* count, int32_t reset, void* stream
 const char* b2ctr_last_error(void) { return b2ctr::g_err; }
 int64_t b2ctr_launch_count(void) { return (int64_t)b2ctr::g_launches.load(); }
 void b2ctr_reset_launch_count(void) { b2ctr::g_launches.store(0); }
-b2ctr_status_t b2ctr_set_l2_fetch_granularity(int32_t bytes) {
-  // cudaLimitMaxL2FetchGranularity is a hint (32 / 64 / 128): with random 4-byte and 128-byte row reads the
-  // default 64 B granule doubles the DRAM traffic of every dim-1 (linear-term) lookup
-  cudaError_t e = cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)bytes);
-  if (e != cudaSuccess) {
-    b2ctr::set_error("set_l2_fetch_granularity(%d): %s", bytes, cudaGetErrorString(e));
-    cudaGetLastError();
-    return B2CTR_ERR_CUDA;
-  }
-  return B2CTR_OK;
-}
-b2ctr_status_t b2ctr_l2_persist_reserve(int64_t bytes, int64_t* granted, int64_t* max_window) {
-  int dev = 0, max_persist = 0, max_win = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, dev);
-  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&max_win, cudaDevAttrMaxAccessPolicyWindowSize, dev);
-  size_t want = bytes < 0 ? 0 : (size_t)bytes;
-  if (want > (size_t)max_persist) want = (size_t)max_persist;
-  if (e == cudaSuccess) e = cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want);
-  size_t got = 0;
-  if (e == cudaSuccess) e = cudaDeviceGetLimit(&got, cudaLimitPersistingL2CacheSize);
-  if (e != cudaSuccess) {
-    b2ctr::set_error("l2_persist_reserve(%lld): %s", (long long)bytes, cudaGetErrorString(e));
-    cudaGetLastError();
-    return B2CTR_ERR_CUDA;
-  }
-  if (granted) *granted = (int64_t)got;
-  if (max_window) *max_window = (int64_t)max_win;
-  return B2CTR_OK;
-}
 b2ctr_status_t b2ctr_enable_peer_access(int32_t peer_device) {
   cudaError_t e = cudaDeviceEnablePeerAccess(peer_device, 0);
   if (e == cudaErrorPeerAccessAlreadyEnabled) {

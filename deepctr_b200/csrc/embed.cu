@@ -10,8 +10,6 @@
 //   * every lane keeps up to 8 independent 16 B loads in flight (Little's law at 6.5 TB/s);
 //   * row updates are REDG.E.ADD.F32x4 (the add executes in the L2 slice, no read by the SM);
 //   * grids are whole multiples of the 132 SMs.
-#include <stdlib.h>
-#include <cuda_bf16.h>
 #include "common.cuh"
 
 namespace b2ctr {
@@ -411,35 +409,13 @@ struct UniParams {
   int32_t dim;
   int32_t idx_dtype;
   int32_t has_lin;
-  int32_t l2_hints;
   int32_t store_grads;
   // row-sharded tables over peer mappings (world = 2^wshift shards): device arrays [nfeat * world]
   float* const* peer_tab;
   float* const* peer_lin;
   int32_t world;
   int32_t wshift;
-  // optional bf16 hi/lo planes of x (first DNN GEMM operand): row pitch xp_pitch elements, columns
-  // [0, xp_pitch) are written (zero beyond the data)
-  __nv_bfloat16* xp_hi;
-  __nv_bfloat16* xp_lo;
-  int64_t xp_pitch;
 };
-
-__device__ __forceinline__ void store_planes4(const UniParams& p, int64_t off, float4 v) {
-  const __nv_bfloat16 h0 = __float2bfloat16_rn(v.x), h1 = __float2bfloat16_rn(v.y);
-  const __nv_bfloat16 h2 = __float2bfloat16_rn(v.z), h3 = __float2bfloat16_rn(v.w);
-  const __nv_bfloat16 l0 = __float2bfloat16_rn(v.x - __bfloat162float(h0));
-  const __nv_bfloat16 l1 = __float2bfloat16_rn(v.y - __bfloat162float(h1));
-  const __nv_bfloat16 l2 = __float2bfloat16_rn(v.z - __bfloat162float(h2));
-  const __nv_bfloat16 l3 = __float2bfloat16_rn(v.w - __bfloat162float(h3));
-  uint2 h, l;
-  h.x = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-  h.y = (uint32_t)__bfloat16_as_ushort(h2) | ((uint32_t)__bfloat16_as_ushort(h3) << 16);
-  l.x = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-  l.y = (uint32_t)__bfloat16_as_ushort(l2) | ((uint32_t)__bfloat16_as_ushort(l3) << 16);
-  *reinterpret_cast<uint2*>(p.xp_hi + off) = h;
-  *reinterpret_cast<uint2*>(p.xp_lo + off) = l;
-}
 
 // peer (NVLink) accesses: no read-only / L2-policy qualifiers - the line lives in the owner's L2
 __device__ __forceinline__ float4 ld_peer_f4(const float* p) {
@@ -476,15 +452,14 @@ __device__ __forceinline__ int64_t uni_id(const UniParams& p, int f, int64_t b) 
 // Latency hiding (ncu, profiles/r1_embed_before.txt: 40 % DRAM, 35 % warps active): the id -> row -> store
 // chain is broken by prefetching the NEXT sample's ids before the current rows are requested, and the
 // register budget is capped at 64 (4 CTAs = 32 warps per SM).
-template <int LPR, bool SHARD, bool PLANES>
-__global__ void __launch_bounds__(256, (SHARD || PLANES) ? 3 : 4)
+template <int LPR, bool SHARD>
+__global__ void __launch_bounds__(256, SHARD ? 3 : 4)
     gather_uniform_fwd_kernel(const __grid_constant__ UniParams p, int64_t batch) {
   constexpr int RPI = 32 / LPR;
   constexpr int U = 7;   // 7 x RPI(4) = 28 >= 26 Criteo fields in one pass at dim 32
   const int lane = threadIdx.x & 31;
   const int slot = lane / LPR, chunk = lane % LPR;
   const int F = p.nfeat, dim = p.dim;
-  const bool hints = p.l2_hints != 0;
   const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -521,8 +496,7 @@ __global__ void __launch_bounds__(256, (SHARD || PLANES) ? 3 : 4)
           } else if (SHARD) {
             v[u] = ld_peer_f4(shard_row(p.peer_tab, p, f, id, dim) + chunk * 4);
           } else {
-            const float* src = p.table[f] + id * dim + chunk * 4;
-            v[u] = hints ? ldg_stream_f4_pol(src, pol_stream) : ldg_stream_f4(src);
+            v[u] = ldg_stream_f4_pol(p.table[f] + id * dim + chunk * 4, pol_stream);
           }
         }
       }
@@ -530,9 +504,7 @@ __global__ void __launch_bounds__(256, (SHARD || PLANES) ? 3 : 4)
       for (int u = 0; u < U; ++u) {
         const int f = f0 + u * RPI + slot;
         if (f < F) {
-          if (hints) stg_stream_f4_pol(xrow + (int64_t)f * dim + chunk * 4, v[u], pol_stream);
-          else stg_stream_f4(xrow + (int64_t)f * dim + chunk * 4, v[u]);
-          if (PLANES) store_planes4(p, b * p.xp_pitch + (int64_t)f * dim + chunk * 4, v[u]);
+          stg_stream_f4_pol(xrow + (int64_t)f * dim + chunk * 4, v[u], pol_stream);
           if ((p.fm_mask >> f) & 1ull) {
             s.x += v[u].x; s.y += v[u].y; s.z += v[u].z; s.w += v[u].w;
             q += v[u].x * v[u].x + v[u].y * v[u].y + v[u].z * v[u].z + v[u].w * v[u].w;
@@ -563,8 +535,8 @@ __global__ void __launch_bounds__(256, (SHARD || PLANES) ? 3 : 4)
           if (ok0) l += ld_peer_f1(shard_row(p.peer_lin, p, lane, id0, 1));
           if (ok1) l += ld_peer_f1(shard_row(p.peer_lin, p, lane + 32, id1, 1));
         } else {
-          if (ok0) l += hints ? ldg_f1_pol(p.lin[lane] + id0, pol_keep) : p.lin[lane][id0];
-          if (ok1) l += hints ? ldg_f1_pol(p.lin[lane + 32] + id1, pol_keep) : p.lin[lane + 32][id1];
+          if (ok0) l += ldg_f1_pol(p.lin[lane] + id0, pol_keep);
+          if (ok1) l += ldg_f1_pol(p.lin[lane + 32] + id1, pol_keep);
         }
       }
       l = warp_sum(l);
@@ -575,15 +547,6 @@ __global__ void __launch_bounds__(256, (SHARD || PLANES) ? 3 : 4)
     for (int64_t c = c0 + lane; c < p.x_cols; c += 32) {
       const int j = (int)(c - c0);
       xrow[c] = j < p.ndense ? p.dense[b * p.dense_ld + j] : 0.f;
-    }
-    if (PLANES) {
-      for (int64_t c = c0 + lane; c < p.xp_pitch; c += 32) {
-        const int j = (int)(c - c0);
-        const float v = j < p.ndense ? p.dense[b * p.dense_ld + j] : 0.f;
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        p.xp_hi[b * p.xp_pitch + c] = h;
-        p.xp_lo[b * p.xp_pitch + c] = __float2bfloat16_rn(v - __bfloat162float(h));
-      }
     }
     id0 = nid0;
     id1 = nid1;
@@ -602,7 +565,6 @@ __global__ void __launch_bounds__(256, SHARD ? 2 : 3)
   const int lane = threadIdx.x & 31;
   const int slot = lane / LPR, chunk = lane % LPR;
   const int F = p.nfeat, dim = p.dim;
-  const bool hints = p.l2_hints != 0;
   const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
   const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
   int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -651,7 +613,7 @@ __global__ void __launch_bounds__(256, SHARD ? 2 : 3)
         xv[u] = g[u];
         if (f < F) {
           const int64_t off = (int64_t)f * dim + chunk * 4;
-          if (dxrow) g[u] = hints ? ldg_stream_f4_pol(dxrow + off, pol_stream) : ldg_stream_f4(dxrow + off);
+          if (dxrow) g[u] = ldg_stream_f4_pol(dxrow + off, pol_stream);
           if (dfm && ((p.fm_mask >> f) & 1ull)) xv[u] = *reinterpret_cast<const float4*>(xrow + off);  // L1 hit
         }
       }
@@ -673,8 +635,7 @@ __global__ void __launch_bounds__(256, SHARD ? 2 : 3)
           r.x *= scale; r.y *= scale; r.z *= scale; r.w *= scale;
           if (SHARD) red_peer_f4(shard_row(p.peer_tab, p, f, id, dim) + chunk * 4, r);
           else if (p.store_grads) stg_stream_f4(p.table[f] + id * dim + chunk * 4, r);
-          else if (hints) red_add_f4_pol(p.table[f] + id * dim + chunk * 4, r, pol_stream);
-          else red_add_f4(p.table[f] + id * dim + chunk * 4, r);
+          else red_add_f4_pol(p.table[f] + id * dim + chunk * 4, r, pol_stream);
         }
       }
     }
@@ -689,8 +650,8 @@ __global__ void __launch_bounds__(256, SHARD ? 2 : 3)
         if (ok0) p.lin[lane][id0] = gl;
         if (ok1) p.lin[lane + 32][id1] = gl;
       } else {
-        if (ok0) { if (hints) red_add_f1_pol(p.lin[lane] + id0, gl, pol_keep); else red_add_f1(p.lin[lane] + id0, gl); }
-        if (ok1) { if (hints) red_add_f1_pol(p.lin[lane + 32] + id1, gl, pol_keep); else red_add_f1(p.lin[lane + 32] + id1, gl); }
+        if (ok0) red_add_f1_pol(p.lin[lane] + id0, gl, pol_keep);
+        if (ok1) red_add_f1_pol(p.lin[lane + 32] + id1, gl, pol_keep);
       }
     }
     id0 = nid0;
@@ -803,31 +764,6 @@ static b2ctr_status_t validate_feats(const b2ctr_feature_t* feats, int32_t nfeat
     }                                                                                    \
   } while (0)
 
-// <<<grid, 256, 0, st>>> with an optional persisting-L2 access-policy window as a launch attribute (it
-// becomes a kernel-node attribute when the step is captured into a CUDA graph)
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_uni(void (*kern)(KArgs...), int grid, cudaStream_t st, const b2ctr_uniform_gather_t* g,
-                              Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(256);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  cfg.attrs = attr;
-  cfg.numAttrs = 0;
-  if (g->l2_window && g->l2_window_bytes > 0) {
-    attr[0].id = cudaLaunchAttributeAccessPolicyWindow;
-    attr[0].val.accessPolicyWindow.base_ptr = const_cast<void*>(g->l2_window);
-    attr[0].val.accessPolicyWindow.num_bytes = (size_t)g->l2_window_bytes;
-    attr[0].val.accessPolicyWindow.hitRatio = g->l2_hit_ratio > 0.f ? (g->l2_hit_ratio < 1.f ? g->l2_hit_ratio : 1.f) : 1.f;
-    attr[0].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    attr[0].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    cfg.numAttrs = 1;
-  }
-  return cudaLaunchKernelEx(&cfg, kern, args...);
-}
-
 static b2ctr_status_t fill_uni(const b2ctr_uniform_gather_t* g, UniParams* p) {
   B2_REQUIRE(g && g->feats && g->x, "uniform gather: NULL descriptor / feats / x");
   B2_REQUIRE(g->nfeat > 0 && g->nfeat <= kUniMaxFeat, "uniform gather: nfeat must be in [1,%d]",
@@ -854,8 +790,6 @@ static b2ctr_status_t fill_uni(const b2ctr_uniform_gather_t* g, UniParams* p) {
     B2_REQUIRE(g->world > 1 || !g->lin_tables || p->lin[f], "uniform gather: lin_tables[%d] is NULL", f);
   }
   p->oob = oob_counter();
-  p->xp_hi = p->xp_lo = nullptr;
-  p->xp_pitch = 0;
   p->world = g->world > 1 ? g->world : 1;
   p->wshift = 0;
   p->peer_tab = g->peer_tables;
@@ -880,9 +814,6 @@ static b2ctr_status_t fill_uni(const b2ctr_uniform_gather_t* g, UniParams* p) {
   p->dim = dim;
   p->idx_dtype = g->feats[0].idx_dtype;
   p->has_lin = g->world > 1 ? (g->peer_lin_tables != nullptr) : (g->lin_tables != nullptr);
-  static int hints = -1;
-  if (hints < 0) { const char* ev = getenv("B2CTR_L2_HINTS"); hints = ev ? atoi(ev) : 1; }
-  p->l2_hints = (g->l2_window && g->l2_window_bytes > 0) ? 0 : hints;   // the window replaces the per-load hints
   p->store_grads = (g->flags & B2CTR_UNIFORM_STORE_GRADS) ? 1 : 0;
   return B2CTR_OK;
 }
@@ -933,12 +864,12 @@ b2ctr_status_t b2ctr_embed_scatter_add(const b2ctr_feature_t* feats, int32_t nfe
 
 #define B2_DISPATCH_LPR1(KERNEL, SH, dim, ...)                                 \
   switch ((dim) / 4) {                                                         \
-    case 1: le = launch_uni(KERNEL<1, SH>, grid, st, g, __VA_ARGS__); break;   \
-    case 2: le = launch_uni(KERNEL<2, SH>, grid, st, g, __VA_ARGS__); break;   \
-    case 4: le = launch_uni(KERNEL<4, SH>, grid, st, g, __VA_ARGS__); break;   \
-    case 8: le = launch_uni(KERNEL<8, SH>, grid, st, g, __VA_ARGS__); break;   \
-    case 16: le = launch_uni(KERNEL<16, SH>, grid, st, g, __VA_ARGS__); break; \
-    default: le = launch_uni(KERNEL<32, SH>, grid, st, g, __VA_ARGS__); break; \
+    case 1: KERNEL<1, SH><<<grid, 256, 0, st>>>(__VA_ARGS__); break;           \
+    case 2: KERNEL<2, SH><<<grid, 256, 0, st>>>(__VA_ARGS__); break;           \
+    case 4: KERNEL<4, SH><<<grid, 256, 0, st>>>(__VA_ARGS__); break;           \
+    case 8: KERNEL<8, SH><<<grid, 256, 0, st>>>(__VA_ARGS__); break;           \
+    case 16: KERNEL<16, SH><<<grid, 256, 0, st>>>(__VA_ARGS__); break;         \
+    default: KERNEL<32, SH><<<grid, 256, 0, st>>>(__VA_ARGS__); break;         \
   }
 #define B2_DISPATCH_LPR(KERNEL, dim, ...)                                      \
   if (p.world > 1) { B2_DISPATCH_LPR1(KERNEL, true, dim, __VA_ARGS__) }        \
@@ -950,46 +881,9 @@ b2ctr_status_t b2ctr_embed_gather_uniform_fwd(const b2ctr_uniform_gather_t* g, i
   b2ctr_status_t s = fill_uni(g, &p);
   if (s != B2CTR_OK) return s;
   if (batch <= 0) return B2CTR_OK;
-  if (g->x_planes) {
-    B2_REQUIRE(batch % 256 == 0, "uniform gather: x_planes needs a batch that is a multiple of 256 (got %lld)",
-               (long long)batch);
-    B2_REQUIRE(g->x_planes_cols >= (int64_t)g->nfeat * p.dim + g->ndense && g->x_planes_cols <= p.x_cols,
-               "uniform gather: x_planes_cols out of range");
-    B2_REQUIRE(aligned16(g->x_planes), "uniform gather: x_planes must be 16-byte aligned");
-    p.xp_pitch = planes_cols_pad(g->x_planes_cols);
-    p.xp_hi = (__nv_bfloat16*)g->x_planes;
-    p.xp_lo = p.xp_hi + planes_rows_pad(batch) * p.xp_pitch;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = grid_for(batch, 8, 8);
-#define B2_GATHER_CASE(LPRV)                                                                         \
-  case LPRV:                                                                                         \
-    if (p.world > 1) {                                                                               \
-      if (p.xp_hi) le = launch_uni(gather_uniform_fwd_kernel<LPRV, true, true>, grid, st, g, p, batch);      \
-      else le = launch_uni(gather_uniform_fwd_kernel<LPRV, true, false>, grid, st, g, p, batch);             \
-    } else {                                                                                         \
-      if (p.xp_hi) le = launch_uni(gather_uniform_fwd_kernel<LPRV, false, true>, grid, st, g, p, batch);     \
-      else le = launch_uni(gather_uniform_fwd_kernel<LPRV, false, false>, grid, st, g, p, batch);            \
-    }                                                                                                \
-    break;
-  cudaError_t le = cudaSuccess;
-  switch (p.dim / 4) {
-    B2_GATHER_CASE(1) B2_GATHER_CASE(2) B2_GATHER_CASE(4) B2_GATHER_CASE(8) B2_GATHER_CASE(16)
-    default:
-      if (p.world > 1) {
-        if (p.xp_hi) le = launch_uni(gather_uniform_fwd_kernel<32, true, true>, grid, st, g, p, batch);
-        else le = launch_uni(gather_uniform_fwd_kernel<32, true, false>, grid, st, g, p, batch);
-      } else {
-        if (p.xp_hi) le = launch_uni(gather_uniform_fwd_kernel<32, false, true>, grid, st, g, p, batch);
-        else le = launch_uni(gather_uniform_fwd_kernel<32, false, false>, grid, st, g, p, batch);
-      }
-  }
-#undef B2_GATHER_CASE
-  if (le != cudaSuccess) {
-    set_error("b2ctr_embed_gather_uniform_fwd: launch failed: %s", cudaGetErrorString(le));
-    cudaGetLastError();
-    return B2CTR_ERR_CUDA;
-  }
+  B2_DISPATCH_LPR(gather_uniform_fwd_kernel, p.dim, p, batch);
   B2_CHECK_LAUNCH("b2ctr_embed_gather_uniform_fwd");
   return B2CTR_OK;
 }
@@ -1004,13 +898,7 @@ b2ctr_status_t b2ctr_embed_scatter_uniform_bwd(const b2ctr_uniform_gather_t* g, 
   if (batch <= 0) return B2CTR_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = grid_for(batch, 8, 8);
-  cudaError_t le = cudaSuccess;
   B2_DISPATCH_LPR(scatter_uniform_bwd_kernel, p.dim, p, dx, dfm, dlinear, scale, lin_scale, batch);
-  if (le != cudaSuccess) {
-    set_error("b2ctr_embed_scatter_uniform_bwd: launch failed: %s", cudaGetErrorString(le));
-    cudaGetLastError();
-    return B2CTR_ERR_CUDA;
-  }
   B2_CHECK_LAUNCH("b2ctr_embed_scatter_uniform_bwd");
   return B2CTR_OK;
 }

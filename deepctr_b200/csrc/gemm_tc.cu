@@ -18,7 +18,6 @@
 //       same order per output element, so it is the reference the bit-exact tests compare variant 4 against.
 #include <cuda.h>          // CUtensorMap + enums only: the encoder is resolved through the runtime (no libcuda link)
 #include <cuda_bf16.h>
-#include <stdlib.h>
 #include "common.cuh"
 
 namespace b2ctr {
@@ -50,7 +49,6 @@ struct PlaneArgs {
   int cin_m, cin_h, cin_hp, cin_on;
   // FOLD epilogue (CIN backward): dT0 [rows, cin_ld0] and dXk [rows, fold_ldx], both accumulated with red.add
   float* fold_dt0; float* fold_dxk; int64_t fold_ldx;
-  int gen_groups;     // generating producers: 2 = two groups of 128 threads alternate stages, 1 = all 256 share every stage
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -607,11 +605,9 @@ __device__ __forceinline__ void store_chunk(const float (&v)[8], unsigned char* 
 // into bf16 hi/lo and stored as four 16-byte chunks [c0, c0+4) of the 128-byte-swizzled row `rr`.
 // Two steps, so that the producer loop can issue the global loads of k-block kb + 1 before it multiplies / splits /
 // stores k-block kb.
-struct GenRegs {       // one register image for both generators (only one of them runs in a launch)
-  float4 x[8];         // CIN: 32 values of X_k;  attention: 32 key values
-  float a;             // CIN: T0[r, i]
-  const float* q;      // attention: the row's query values
-  bool ok;             // attention: row inside the matrix
+struct GenRegs {
+  float4 x[8];         // 32 values of X_k
+  float a;             // T0[r, i]
 };
 __device__ __forceinline__ void cin_load_half(const PlaneArgs& g, int64_t r, int q0, GenRegs& o) {
   const bool row_ok = r < g.cin_rows;
@@ -692,60 +688,6 @@ __device__ __noinline__ void att_generate_half(const PlaneArgs& g, int64_t r, in
     store_chunk(v, hi_row, lo_row, ((c0 + c) ^ (rr & 7)) << 4);
   }
 }
-// Attention input with the thread's 32 key values RESIDENT in registers (64 % E == 0, E >= 32: a thread's e-range
-// is the same in every k-block).  A forward tile (4E / 64 k-blocks over the same rows) then loads its keys once - and
-// the keys of the NEXT tile (or, kernel gradient, of the next k-block's rows) are loaded into the same registers as
-// soon as the last use of each pair has issued: the loads stay in flight across the stage hand-over.  The query
-// values come from L1 (a CTA's 128 rows belong to 3-4 samples).
-__device__ __forceinline__ void att_locate(const PlaneArgs& g, int64_t r, int e0, const float*& q, const float*& k,
-                                           bool& ok) {
-  const int T = g.cin_m, E = g.cin_h;
-  ok = r < g.cin_rows;
-  const uint32_t bu = ok ? (uint32_t)r / (uint32_t)T : 0u;
-  const int t = ok ? (int)((uint32_t)r - bu * (uint32_t)T) : 0;
-  q = g.cin_t0 + (int64_t)bu * g.cin_ld0 + e0;
-  k = g.cin_xk + (int64_t)bu * g.cin_ldk + (int64_t)t * E + e0;
-}
-__device__ __forceinline__ void att_load_keys(const PlaneArgs& g, int64_t r, int col0, GenRegs& o) {
-  const int E = g.cin_h;
-  const float* k;
-  att_locate(g, r, col0 - (col0 / E) * E, o.q, k, o.ok);
-#pragma unroll
-  for (int c = 0; c < 8; ++c)
-    o.x[c] = o.ok ? __ldg(reinterpret_cast<const float4*>(k) + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-}
-__device__ __forceinline__ void att_emit_half(const PlaneArgs& g, GenRegs& io, int col0, unsigned char* hi_row,
-                                              unsigned char* lo_row, int rr, int c0, bool reload, int64_t r_next) {
-  const int E = g.cin_h;
-  const int seg = col0 / E;
-  const float* q = io.q;
-  const bool ok = io.ok;
-  const float* kn = nullptr;
-  bool okn = false;
-  if (reload) att_locate(g, r_next, col0 - seg * E, io.q, kn, okn);
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    const float4 k0 = io.x[2 * c], k1 = io.x[2 * c + 1];
-    float4 q0 = make_float4(0.f, 0.f, 0.f, 0.f), q1 = q0;
-    if (ok && seg != 1 && seg < 4) {
-      q0 = __ldg(reinterpret_cast<const float4*>(q) + 2 * c);
-      q1 = __ldg(reinterpret_cast<const float4*>(q) + 2 * c + 1);
-    }
-    if (reload) {
-      io.x[2 * c] = okn ? __ldg(reinterpret_cast<const float4*>(kn) + 2 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
-      io.x[2 * c + 1] = okn ? __ldg(reinterpret_cast<const float4*>(kn) + 2 * c + 1) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    const float qa[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-    const float ka[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
-    float v[8];
-#pragma unroll
-    for (int jx = 0; jx < 8; ++jx)
-      v[jx] = seg == 0 ? qa[jx] : seg == 1 ? ka[jx] : seg == 2 ? __fsub_rn(qa[jx], ka[jx])
-            : seg == 3 ? __fmul_rn(qa[jx], ka[jx]) : 0.f;       // seg >= 4: columns of the M padding (kernel gradient)
-    store_chunk(v, hi_row, lo_row, ((c0 + c) ^ (rr & 7)) << 4);
-  }
-  if (reload) io.ok = okn;
-}
 
 // generated-operand kernels run 8 producer warps (two threads per generated row), the others 4
 template <bool GENERATED>
@@ -778,7 +720,7 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     for (int s = 0; s < STAGES; ++s) {
       // TMA: one arrive.expect_tx; generated A: one arrival per generating thread of the stage + the TMA expect_tx
       // of the B planes
-      mbar_init(&full_bar[s], GEN != 0 ? 1 + (g.gen_groups == 2 ? 128 : 256) : 1);
+      mbar_init(&full_bar[s], GEN == 1 ? 1 + 256 : GEN == 2 ? 1 + 128 : 1);
       // a stage is released by every consumer warp (cooperative) or by the four warps of the tile's owner (ping-pong)
       mbar_init(&empty_bar[s], PINGPONG ? kWsConsumerWarps / 2 : kWsConsumerWarps);
     }
@@ -818,13 +760,12 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
     const int grp = tid >> 7, t128 = tid & 127;
     if (t128 == 0) { tma_prefetch_desc(&tm_bh); tma_prefetch_desc(&tm_bl); }
     uint32_t it = 0;
-    const bool att_res = GEN == 2 && g.cin_h >= 32 && 64 % g.cin_h == 0;
-    if (GEN == 1 || (att_res && g.gen_groups == 1)) {
-      // 256 threads per stage (two per generated row), software-pipelined over the FLATTENED sequence of k-blocks
-      // of all the tiles of this CTA: the operands of the next k-block (the next tile's first one included) are
-      // requested while the current one is multiplied / split / stored, and stay in flight across the stage
+    if constexpr (GEN == 1) {
+      // CIN: 256 threads per stage (two per generated row), software-pipelined over the FLATTENED sequence of
+      // k-blocks of all the tiles of this CTA: the operands of the next k-block (the next tile's first one included)
+      // are requested while the current one is multiplied / split / stored, and stay in flight across the stage
       // hand-over.  The generator was load-latency-bound (ncu source page: the stall samples sit on the first use
-      // of the loaded operands); with K = 4E = 256 the attention GEMM has only 4 k-blocks per tile.
+      // of the loaded operands).
       const int half = tid & 1;
       const int atom = tid >> 7, rr = g.a_mn ? (tid & 127) >> 1 : tid >> 1;
       const int soff = (g.a_mn ? atom * 8192 : 0) + rr * 128;
@@ -847,15 +788,12 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
       auto row_of = [&](int m0_, int k0_) { return g.a_mn ? k0_ + rr : m0_ + rr; };
       auto col_of = [&](int m0_, int k0_) { return g.a_mn ? m0_ + atom * 64 + half * 32 : k0_ + half * 32; };
       GenRegs gr;
-      if (tile < ntiles) {
-        if constexpr (GEN == 1) cin_load_half(g, row_of(m0, kbeg), col_of(m0, kbeg), gr);     // (k_of(kbeg, 0, .) == kbeg)
-        else att_load_keys(g, row_of(m0, kbeg), col_of(m0, kbeg), gr);
-      }
+      if (tile < ntiles) cin_load_half(g, row_of(m0, kbeg), col_of(m0, kbeg), gr);     // (k_of(kbeg, 0, .) == kbeg)
       // CIN forward, hp = nj * 64: the k-blocks of a tile are walked j-block-major (all i for the first 64 columns of
       // X_k, then all i for the next 64 ...).  A thread's 32 values of X_k are then the same for m consecutive
       // k-blocks and stay in registers; only T0[r, i] is fetched per k-block.  (The B planes are fetched at the same
       // k0, and the order of the K accumulation is free.)
-      const int nj = (GEN == 1 && !g.a_mn && g.splits == 1 && g.cin_hp >= 128) ? g.cin_hp / kTK : 1;
+      const int nj = (!g.a_mn && g.splits == 1 && g.cin_hp >= 128) ? g.cin_hp / kTK : 1;
       auto k_of = [&](int kbeg_, int kb_, int nkb_) {
         if (nj == 1) return kbeg_ + kb_ * kTK;
         const int ni = nkb_ / nj;                      // = m (k_pad = m * hp)
@@ -893,14 +831,9 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
             tma_load_2d(st + 2 * A_PLANE + B_PLANE, &tm_bl, k0, n0, bar);
           }
         }
-        if constexpr (GEN == 1) {
-          const int r = row_of(m0, k0), r_n = row_of(m0_n, k0_n), q = col_of(m0, k0), q_n = col_of(m0_n, k0_n);
-          cin_emit_half(g, gr, q, stp + soff, stp + A_PLANE + soff, rr, half * 4, has_next, r_n, q_n,
-                        has_next && (r_n != r || q_n % g.cin_hp != q % g.cin_hp));
-        } else {
-          const int r = row_of(m0, k0), r_n = row_of(m0_n, k0_n);
-          att_emit_half(g, gr, col_of(m0, k0), stp + soff, stp + A_PLANE + soff, rr, half * 4, has_next && r_n != r, r_n);
-        }
+        const int r = row_of(m0, k0), r_n = row_of(m0_n, k0_n), q = col_of(m0, k0), q_n = col_of(m0_n, k0_n);
+        cin_emit_half(g, gr, q, stp + soff, stp + A_PLANE + soff, rr, half * 4, has_next, r_n, q_n,
+                      has_next && (r_n != r || q_n % g.cin_hp != q % g.cin_hp));
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         mbar_arrive(&full_bar[s]);
         ++it;
@@ -914,13 +847,12 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
       const int64_t m0 = mt * kTM;
       const int32_t n0 = (int32_t)(nt * BN);
       for (int kb = 0; kb < nkb; ++kb, ++it) {
-        const bool two = g.gen_groups == 2;
-        if (two && (int)(it & 1) != grp) continue;
+        if ((int)(it & 1) != grp) continue;
         const int s = it % STAGES;
         mbar_wait(&empty_bar[s], ((it / STAGES) & 1) ^ 1);
         unsigned char* stp = tiles + (size_t)s * STAGE;
         const int64_t k0 = kbeg + (int64_t)kb * kTK;
-        if (two ? t128 == 0 : tid == 0) {
+        if (t128 == 0) {
           uint64_t* bar = &full_bar[s];
           mbar_expect_tx(bar, (uint32_t)(2 * B_PLANE));
           const uint32_t st = smem_u32(stp);
@@ -935,27 +867,15 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
             tma_load_2d(st + 2 * A_PLANE + B_PLANE, &tm_bl, (int32_t)k0, n0, bar);
           }
         }
-        if (two) {
-          if (g.a_mn) {      // A^T: M = q (two 64-wide atoms), K = r: thread -> (atom, k-row)
-            const int atom = t128 >> 6, rr = t128 & 63;
-            unsigned char* row = stp + atom * 8192 + rr * 128;
-            att_generate_half(g, k0 + rr, (int)(m0 + atom * 64), row, row + A_PLANE, rr, 0);
-            att_generate_half(g, k0 + rr, (int)(m0 + atom * 64 + 32), row, row + A_PLANE, rr, 4);
-          } else {           // A: M = r, K = q: thread -> row
-            unsigned char* row = stp + t128 * 128;
-            att_generate_half(g, m0 + t128, (int)k0, row, row + A_PLANE, t128, 0);
-            att_generate_half(g, m0 + t128, (int)(k0 + 32), row, row + A_PLANE, t128, 4);
-          }
-        } else {
-          const int half = tid & 1;           // two threads per generated row: 32 of its 64 columns each
-          if (g.a_mn) {
-            const int atom = tid >> 7, rr = (tid & 127) >> 1;
-            att_generate_half(g, k0 + rr, (int)(m0 + atom * 64 + half * 32), stp + atom * 8192 + rr * 128,
-                          stp + A_PLANE + atom * 8192 + rr * 128, rr, half * 4);
-          } else {
-            const int rr = tid >> 1;
-            att_generate_half(g, m0 + rr, (int)(k0 + half * 32), stp + rr * 128, stp + A_PLANE + rr * 128, rr, half * 4);
-          }
+        if (g.a_mn) {      // A^T: M = q (two 64-wide atoms), K = r: thread -> (atom, k-row)
+          const int atom = t128 >> 6, rr = t128 & 63;
+          unsigned char* row = stp + atom * 8192 + rr * 128;
+          att_generate_half(g, k0 + rr, (int)(m0 + atom * 64), row, row + A_PLANE, rr, 0);
+          att_generate_half(g, k0 + rr, (int)(m0 + atom * 64 + 32), row, row + A_PLANE, rr, 4);
+        } else {           // A: M = r, K = q: thread -> row
+          unsigned char* row = stp + t128 * 128;
+          att_generate_half(g, m0 + t128, (int)k0, row, row + A_PLANE, t128, 0);
+          att_generate_half(g, m0 + t128, (int)(k0 + 32), row, row + A_PLANE, t128, 4);
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         mbar_arrive(&full_bar[s]);
@@ -1339,7 +1259,7 @@ b2ctr_status_t gemm_bf16x3(const b2ctr_gemm_t* g, void* workspace, size_t worksp
   pa.k_per_split = ceil_div(ceil_div(kp, splits), kTK) * kTK;
   pa.alpha = g->alpha; pa.act = g->act; pa.accumulate = g->accumulate; pa.splits = splits;
   pa.cin_on = 0; pa.cin_t0 = pa.cin_xk = nullptr; pa.cin_ld0 = pa.cin_ldk = pa.cin_rows = 0; pa.cin_m = pa.cin_h = pa.cin_hp = 0;
-  pa.fold_dt0 = pa.fold_dxk = nullptr; pa.fold_ldx = 0; pa.gen_groups = 0;
+  pa.fold_dt0 = pa.fold_dxk = nullptr; pa.fold_ldx = 0;
   cudaError_t e;
   const bool short_k = pa.k_per_split <= 4 * kTK;
   if (ws_kernel) {
@@ -1451,13 +1371,6 @@ static b2ctr_status_t gen_gemm(const GenSpec& sp, int mode, int64_t n, const voi
   pa.cin_on = sp.kind; pa.cin_t0 = sp.p0; pa.cin_xk = sp.p1; pa.cin_ld0 = sp.ld0; pa.cin_ldk = sp.ld1;
   pa.cin_rows = sp.rows; pa.cin_m = sp.m; pa.cin_h = sp.h; pa.cin_hp = sp.hp;
   pa.fold_dt0 = pa.fold_dxk = nullptr; pa.fold_ldx = 0;
-  {
-    static int groups = -1;
-    if (groups < 0) { const char* ev = getenv("B2CTR_GEN_GROUPS"); groups = ev ? atoi(ev) : 0; }
-    // the CIN generator runs all 256 threads on every stage; the attention generator two groups of 128 that
-    // alternate stages, or (B2CTR_GEN_GROUPS=1) all 256 with the keys held in registers
-    pa.gen_groups = sp.kind == 1 ? 1 : (groups == 1 ? 1 : 2);
-  }
   pa.b_mn = 1;      // both B operands are row-major matrices whose reduction dim is their row index
   pa.c = c; pa.bias = bias; pa.ws = (float*)workspace; pa.ldc = ldc;
   pa.alpha = 1.f; pa.act = act; pa.accumulate = 0; pa.splits = splits;
@@ -1541,7 +1454,7 @@ b2ctr_status_t cin_fold(const b2ctr_cin_gemm_t* g, float* dt0, float* dxk, int64
   pa.k_per_split = pa.k_pad; pa.alpha = 1.f; pa.act = 0; pa.accumulate = 0; pa.splits = 1;
   pa.cin_on = 0; pa.cin_t0 = g->t0; pa.cin_xk = g->xk; pa.cin_ld0 = g->ld0; pa.cin_ldk = g->ldk; pa.cin_rows = g->rows;
   pa.cin_m = g->m; pa.cin_h = g->h; pa.cin_hp = g->hp;
-  pa.fold_dt0 = dt0; pa.fold_dxk = dxk; pa.fold_ldx = ldx; pa.gen_groups = 0;
+  pa.fold_dt0 = dt0; pa.fold_dxk = dxk; pa.fold_ldx = ldx;
   constexpr int bn = 128;
   WsArgs wa;
   wa.p = pa;

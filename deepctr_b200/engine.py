@@ -44,13 +44,12 @@ class Var(object):
     """Runtime tensor.  ``data`` has the logical shape; when ``base`` is set, ``data`` is a strided
     window [col0, col0+ncols) of ``base.data`` (a [B, ld] buffer) and gradients are routed there."""
     __slots__ = ("data", "grad", "requires_grad", "mask", "base", "col0", "ncols", "owner", "name",
-                 "vshape", "planes", "xplanes")
+                 "vshape", "planes")
 
     def __init__(self, data, requires_grad=False, mask=None, base=None, col0=0, ncols=0, owner=None,
                  name=None, vshape=None):
         self.data = data
         self.planes = None      # (key, bf16 hi/lo planes) cache of ops.dense in BF16X3 mode
-        self.xplanes = None     # (ncols, planes) of the leading ncols columns, emitted by the fused gather
         self.vshape = vshape    # logical shape of a VIRTUAL var (data is None: fused away this step)
         self.grad = None
         self.requires_grad = requires_grad

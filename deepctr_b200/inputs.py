@@ -469,44 +469,6 @@ class EmbeddingPlanner(object):
             self.peers = (emb, lin, token)
         return self.peers
 
-    def _linear_arena(self):
-        """One contiguous buffer for the dim-1 (linear-term) tables + a persisting-L2 window over it.
-
-        Every 4-byte linear lookup costs a 64-byte DRAM granule in the gather and a read + write of one in the
-        update: 20 % of the gather's and 22 % of the update's DRAM traffic at C2 (profiles/README.md).  The 26
-        tables are 104 MB - twice the 50 MB L2 - so they are moved into one arena once, and the two fused
-        kernels fetch that range with the persisting property (b2ctr_uniform_gather_t.l2_window) while the
-        embedding rows and activations stream.  B2CTR_L2_PERSIST=0 turns it off."""
-        if getattr(self, "_arena", False) is not False:
-            return self._arena
-        import os
-        self._arena = None
-        if os.environ.get("B2CTR_L2_PERSIST", "0") != "1" or getattr(self, "sharded", False):
-            return None
-        ws, seen = [], set()
-        for s_ in self.lin:
-            w = s_.emb.embeddings
-            if id(w) not in seen:
-                seen.add(id(w))
-                ws.append(w)
-        sizes = [(w.numel() + 63) // 64 * 64 for w in ws]
-        total = sum(sizes)
-        if total * 4 < (16 << 20) or torch.cuda.is_current_stream_capturing():
-            return None                       # small tables live in L2 anyway
-        granted, max_window = K.l2_persist_reserve(total * 4)
-        if granted <= 0 or max_window <= 0:
-            return None
-        arena = torch.empty((total,), dtype=torch.float32, device=ws[0].materialize().device)
-        off = 0
-        for w, n in zip(ws, sizes):
-            view = arena[off:off + w.numel()].view(w.shape_)
-            view.copy_(w.materialize())        # a memcpy, once
-            w.data = view
-            off += n
-        nbytes = min(total * 4, max_window)
-        self._arena = (arena, (arena.data_ptr(), nbytes, min(1.0, granted / float(nbytes))))
-        return self._arena
-
     def _fast_eligible(self):
         m = self.main
         if not m or len(m) > 64:
@@ -611,24 +573,10 @@ class EmbeddingPlanner(object):
                     fm = torch.empty((batch,), dtype=torch.float32, device=dev)
                     for f in range(c0 // d, (c0 + nc) // d):
                         fm_mask |= 1 << f
-            arena = self._linear_arena() if (lin_fused and lin_tabs is not None and peer is None
-                                             and getattr(self, "route", None) is None) else None
-            if arena is not None:     # (the tables were re-homed into the arena: take their new addresses)
-                lin_tabs = [s.emb.embeddings.materialize().reshape(-1) for s in self.lin]
             plan = K.UniformPlan(feats, lin_tabs, dense, x, linear, fm, fm_mask)
-            plan.set_window(arena[1] if arena is not None else None)
             plan.g.x_cols = self.main_ld if only_fast else self.fast_n * fast_slots[0].dim
             if peer is not None:
                 plan.set_peers(self.dist.world, peer[0].table, peer[1].table if peer[1] is not None else None)
-            from . import ops as _ops
-            if (only_fast and self.tail_done is not None and batch % 256 == 0 and batch >= 256
-                    and _ops.GEMM_PRECISION == L.GEMM_BF16X3 and _ops.PLANE_REUSE and _ops.GATHER_PLANES):
-                # the DNN reads x[:, :F*E+nd] as its first GEMM operand: emit its bf16 hi/lo planes here
-                kd = self.main_width + self.tail_done[1]
-                xp = torch.empty((L.lib().b2ctr_planes_bytes(batch, kd),), dtype=torch.uint8, device=dev)
-                plan.g.x_planes = xp.data_ptr()
-                plan.g.x_planes_cols = kd
-                bufs["main"].xplanes = (kd, xp)
             K.embed_gather_uniform_fwd(plan, batch)
             if fm is not None:
                 self.fm_result = (self.fm_hint, E.Var(fm.reshape(batch, 1)))
@@ -766,9 +714,6 @@ class EmbeddingPlanner(object):
                                           None if dlin is None else dlin.reshape(-1).contiguous(),
                                           1 if adagrad else 0, o.lr, o.lr, 1e-7, acc, lacc, batch)
                     return self._backward_generic(feed, bufs, generic, opt, batch)
-                arena = getattr(self, "_arena", None)
-                if arena and lin_tabs is not None and all(sc < 0 for _, sc in lt):
-                    bplan.set_window(arena[1])        # fused SGD on the linear tables inside the arena
                 K.embed_scatter_uniform_bwd(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
                                             None if dlin is None else dlin.reshape(-1).contiguous(),
                                             scale, lin_scale, batch)

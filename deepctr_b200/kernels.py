@@ -129,11 +129,6 @@ class UniformPlan(object):
         self.g.fm_mask[0] = fm_mask & 0xFFFFFFFFFFFFFFFF
         self.g.fm_mask[1] = 0
 
-    def set_window(self, window):
-        """(base pointer, bytes, hit ratio) of the persisting-L2 window (the linear-table arena) or None."""
-        if window is not None:
-            self.g.l2_window, self.g.l2_window_bytes, self.g.l2_hit_ratio = window
-
     def set_peers(self, world, peer_tables, peer_lin_tables):
         """Row-sharded tables addressed through peer mappings (parallel.PeerTables.table device arrays)."""
         self.peer_refs = (peer_tables, peer_lin_tables)
@@ -142,31 +137,7 @@ class UniformPlan(object):
         self.g.peer_lin_tables = peer_lin_tables.data_ptr() if peer_lin_tables is not None else None
 
 
-_l2_granule_done = set()
-
-
-def _l2_fetch_hint():
-    """Once per device: DRAM -> L2 fetch granule for the random-row embedding traffic (B2CTR_L2_FETCH=32|64|128,
-    0 = leave the driver default)."""
-    dev = torch.cuda.current_device()
-    if dev in _l2_granule_done:
-        return
-    _l2_granule_done.add(dev)
-    import os
-    want = int(os.environ.get("B2CTR_L2_FETCH", "0"))
-    if want:
-        L.check(L.lib().b2ctr_set_l2_fetch_granularity(want), "set_l2_fetch_granularity")
-
-
-def l2_persist_reserve(nbytes):
-    """-> (granted set-aside bytes, max access-policy window bytes) on the current device."""
-    got, win = C.c_int64(0), C.c_int64(0)
-    L.check(L.lib().b2ctr_l2_persist_reserve(int(nbytes), C.byref(got), C.byref(win)), "l2_persist_reserve")
-    return int(got.value), int(win.value)
-
-
 def embed_gather_uniform_fwd(plan, batch):
-    _l2_fetch_hint()
     L.check(L.lib().b2ctr_embed_gather_uniform_fwd(C.byref(plan.g), batch, stream()),
             "embed_gather_uniform_fwd")
 

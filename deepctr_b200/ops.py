@@ -14,13 +14,6 @@ from . import engine as E
 GEMM_PRECISION = L.GEMM_BF16X3
 
 
-# BF16X3: split every GEMM operand into bf16 planes once per step and reuse them (the GEMM reads a row-major
-# operand whose reduction dim is its row index as MN-major planes, so one split serves forward, dgrad and wgrad)
-PLANE_REUSE = True
-# the fused embedding gather also writes the planes of the first DNN operand (saves re-reading X to split it)
-GATHER_PLANES = False    # measured: -11 us/step but +60 us inside the gather kernel itself; opt-in
-
-
 # bumped by ops whose kernels take per-step by-value state (dropout seeds) or that need the host (string
 # hashing): a model that ran one of them is never replayed as a CUDA graph (engine.Model._graph_eligible)
 UNCAPTURABLE = 0
@@ -70,11 +63,6 @@ def _as2d(x):
 def _planes_of(var, t2):
     """bf16 hi/lo planes of a Var's 2-D view, split once per step and shared by every GEMM that reads it
     (forward of each consumer + the wgrad GEMMs)."""
-    base = var.base
-    if (base is not None and base.xplanes is not None and var.col0 == 0 and base.data is not None
-            and base.xplanes[0] == t2.shape[1] and t2.data_ptr() == base.data.data_ptr()
-            and t2.stride(0) == base.data.stride(0)):
-        return base.xplanes[1]       # the fused gather already wrote the planes of this window
     key = (t2.data_ptr(), tuple(t2.shape), t2.stride(0))
     if var.planes is None or var.planes[0] != key:
         var.planes = (key, K.split_planes(t2))
@@ -93,7 +81,7 @@ def dense(x, w, b=None, activation=None):
     # BF16X3: operands are split into bf16 planes once and the planes are reused by forward/dgrad/wgrad
     # skinny layers (the final [*, 1] projection) are GEMVs: exact-fp32 FFMA path, no tensor-core staging
     prec = GEMM_PRECISION if min(n, kdim) >= 16 else L.GEMM_FP32
-    reuse = prec == L.GEMM_BF16X3 and PLANE_REUSE and m >= 128
+    reuse = prec == L.GEMM_BF16X3 and m >= 128
     xp = _planes_of(x, x2) if reuse else None
     wp = K.split_planes(wd) if reuse else None
     y = K.gemm(x2, wd, bias=bd, act=fused_act, precision=prec, m=m, n=n, k=kdim, a_planes=xp, b_planes=wp)
@@ -616,17 +604,21 @@ def cross_matrix(x0, xl, w, bias):
 CIN_CHUNK_BYTES = 24 << 20      # outer-product chunk kept well inside the 50 MB L2
 
 
-CIN_FUSED = True              # generate the outer product inside the wgmma GEMM producer (b2ctr_cin_gemm)
-CIN_FOLD = True               # ... and fold dZ = dY W^T onto the factors inside the GEMM epilogue (b2ctr_cin_fold)
+CIN_FOLD = True               # fused CIN: fold dZ = dY W^T onto the factors inside the GEMM epilogue (b2ctr_cin_fold)
 CIN_DZ_CHUNK_BYTES = 512 << 20
 
 
-def cin(x, filters, biases, layer_size, activation, split_half):
+def cin_fusable(x, layer_size, split_half):
+    """The outer product can be generated inside the wgmma GEMM producer (b2ctr_cin_gemm)."""
     B, m, D = x.shape
+    hid = [n // 2 if split_half else n for n in layer_size[:-1]]
+    return (GEMM_PRECISION == L.GEMM_BF16X3 and B * D >= 256 and D in (4, 8, 16, 32, 64, 128)
+            and min(layer_size) >= 8 and all(n % 4 == 0 for n in layer_size) and all(h % 4 == 0 for h in hid))
+
+
+def cin(x, filters, biases, layer_size, activation, split_half):
     with K.profile_tag("cin"):
-        hid = [n // 2 if split_half else n for n in layer_size[:-1]]
-        if (CIN_FUSED and GEMM_PRECISION == L.GEMM_BF16X3 and B * D >= 256 and D in (4, 8, 16, 32, 64, 128)
-                and min(layer_size) >= 8 and all(n % 4 == 0 for n in layer_size) and all(h % 4 == 0 for h in hid)):
+        if cin_fusable(x, layer_size, split_half):
             return _cin_fused(x, filters, biases, layer_size, activation, split_half)
         return _cin(x, filters, biases, layer_size, activation, split_half)
 
@@ -888,12 +880,10 @@ def din_att_input(query, keys):
     return res
 
 
-DIN_FUSED = True     # generate [q, k, q-k, q*k] inside the first attention GEMM (b2ctr_att_gemm)
-
-
 def din_att_fusable(query, keys, n_out):
+    """[q, k, q-k, q*k] can be generated inside the first attention GEMM (b2ctr_att_gemm)."""
     B, T, Edim = keys.shape
-    return (DIN_FUSED and GEMM_PRECISION == L.GEMM_BF16X3 and Edim % 8 == 0 and B * T >= 256 and n_out >= 8
+    return (GEMM_PRECISION == L.GEMM_BF16X3 and Edim % 8 == 0 and B * T >= 256 and n_out >= 8
             and n_out % 4 == 0)
 
 

@@ -52,11 +52,6 @@ B2CTR_API void b2ctr_reset_launch_count(void);
  * persistent pool of `threads` helper threads (0 = pick from the core count, 1 = inline memcpy).  Replaces the
  * per-feature numpy -> tensor conversion of Keras' data adapter behind model.fit(model_input, y)
  * (reference examples/run_classification_criteo.py:48); the caller uploads dst with one cudaMemcpyAsync. */
-/* Hint for the current device: largest DRAM -> L2 fetch granule (32, 64 or 128 bytes;
- * cudaLimitMaxL2FetchGranularity).  The embedding path is dominated by random row reads, 32 keeps a 4-byte
- * linear-term lookup from dragging a second sector in. */
-B2CTR_API b2ctr_status_t b2ctr_set_l2_fetch_granularity(int32_t bytes);
-
 /* One process per GPU: let kernels of the current device dereference memory of `peer_device` that was
  * mapped through CUDA IPC (cudaDeviceEnablePeerAccess; already-enabled is not an error). */
 B2CTR_API b2ctr_status_t b2ctr_enable_peer_access(int32_t peer_device);
@@ -152,20 +147,6 @@ typedef struct b2ctr_uniform_gather {
    * ignored.  Gathers are plain peer loads, the backward update is red.add at the owner's L2. */
   float* const* peer_tables;
   float* const* peer_lin_tables; /* [nfeat * world] or NULL */
-  /* gather_uniform_fwd only: also emit the bf16 hi/lo operand planes (b2ctr_split_planes layout) of
-   * x[:, 0:x_planes_cols] - the A operand of the first DNN GEMM - so that X is not read again to split it.
-   * Buffer of b2ctr_planes_bytes(batch, x_planes_cols) bytes; batch must be a multiple of 256 and
-   * F*dim + ndense <= x_planes_cols <= x_cols.  NULL = off. */
-  void* x_planes;
-  int64_t x_planes_cols;
-  /* Optional persisting-L2 window (cudaAccessPolicyWindow attached to THIS launch): [l2_window, l2_window +
-   * l2_window_bytes) - the arena holding the dim-1 linear tables (26 x 1M x 4 B = 104 MB at C2; the
-   * 50 MB L2 holds part of it) - is fetched with the persisting property for a fraction l2_hit_ratio of its lines, everything
-   * else streams.  Each 4-byte linear lookup otherwise costs a 64-byte DRAM granule in the gather and two in
-   * the update.  Needs b2ctr_l2_persist_reserve() once per device.  NULL / 0 = off. */
-  const void* l2_window;
-  int64_t l2_window_bytes;
-  float l2_hit_ratio;
 } b2ctr_uniform_gather_t;
 /* scatter_uniform_bwd: every (sample, feature) id is distinct (the ids are positions in a private row
  * buffer, as on the row-sharded path): write scale*g instead of accumulating, no zero-fill needed. */
@@ -173,11 +154,6 @@ typedef struct b2ctr_uniform_gather {
 
 B2CTR_API b2ctr_status_t b2ctr_embed_gather_uniform_fwd(const b2ctr_uniform_gather_t* g,
                                                        int64_t batch, void* stream);
-
-/* Set aside up to `bytes` of the current device's L2 for persisting accesses (cudaLimitPersistingL2CacheSize,
- * clamped to the device maximum).  *granted = the set-aside size, *max_window = the largest access-policy
- * window the device accepts.  bytes = 0 releases the set-aside. */
-B2CTR_API b2ctr_status_t b2ctr_l2_persist_reserve(int64_t bytes, int64_t* granted, int64_t* max_window);
 
 /* Backward of the above fused with the row update:
  *   g_row(b,f) = dx[b, f*dim:(f+1)*dim] + dfm[b] * (S_b - x[b, f*dim:...])   (FM Jacobian, App. A.6)

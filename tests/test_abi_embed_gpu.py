@@ -243,38 +243,6 @@ def test_invalid_arguments_raise_value_error(cuda):
         K.embed_gather_fwd([f], 2)
 
 
-def test_uniform_gather_emits_operand_planes(cuda):
-    """x_planes of b2ctr_uniform_gather_t: the gather writes the bf16 hi/lo planes of x[:, :F*E+nd] exactly as
-    b2ctr_split_planes would produce them from the x it just wrote (same rounding, same zero padding)."""
-    from deepctr_b200 import kernels as K, _lib as L
-    rng = np.random.RandomState(4)
-    B, F, E, nd, V = 512, 26, 32, 13, 1000
-    ld = (F * E + nd + 3) // 4 * 4
-    tabs = [torch.tensor(rng.normal(size=(V, E)).astype(np.float32), device=cuda) for _ in range(F)]
-    ids = torch.tensor(rng.randint(0, V, (B, F)).astype(np.int32), device=cuda)
-    dense = torch.tensor(rng.rand(B, nd).astype(np.float32), device=cuda)
-    x = torch.empty((B, ld), device=cuda)
-    feats = [K.make_feature(tabs[f], ids[:, f], x, out_col=f * E, out_ld=ld) for f in range(F)]
-    plan = K.UniformPlan(feats, None, dense, x, None, None, 0)
-    kd = F * E + nd
-    nbytes = L.lib().b2ctr_planes_bytes(B, kd)
-    xp = torch.full((nbytes,), 0x5A, dtype=torch.uint8, device=cuda)
-    plan.g.x_planes = xp.data_ptr()
-    plan.g.x_planes_cols = kd
-    K.embed_gather_uniform_fwd(plan, B)
-    want = K.split_planes(x[:, :kd])
-    pad = 256                                            # trailing slack of the buffer is not written by either
-    assert torch.equal(xp[:nbytes - pad], want[:nbytes - pad])
-    # batch not a multiple of 256 is rejected (padding rows would stay uninitialised)
-    x2 = torch.empty((300, ld), device=cuda)
-    feats2 = [K.make_feature(tabs[f], ids[:300, f], x2, out_col=f * E, out_ld=ld) for f in range(F)]
-    plan2 = K.UniformPlan(feats2, None, dense[:300], x2, None, None, 0)
-    plan2.g.x_planes = xp.data_ptr()
-    plan2.g.x_planes_cols = kd
-    with pytest.raises(ValueError):
-        K.embed_gather_uniform_fwd(plan2, 300)
-
-
 # ---- ids outside [0, vocab): zero rows, no out-of-bounds access in either direction, counted ----------
 def test_out_of_range_ids_generic(cuda):
     K, L = _kern()

@@ -12,7 +12,7 @@ def _declared():
     return sorted(set(re.findall(r"B2CTR_API\s+[\w\s\*]+?\b(b2ctr_\w+)\s*\(", src)))
 
 
-def test_header_symbols_are_exported_and_bound():
+def test_abi_v2_symbols_are_exported_and_bound():
     from deepctr_b200 import _lib as L
     names = _declared()
     assert len(names) >= 20
@@ -21,16 +21,16 @@ def test_header_symbols_are_exported_and_bound():
         assert hasattr(handle, n), "libb2ctr.so does not export %s" % n
         assert n in L.SIGNATURES, "_lib.SIGNATURES lacks %s" % n
     assert set(L.SIGNATURES) == set(names)
-    assert handle.b2ctr_abi_version() == 1
+    assert handle.b2ctr_abi_version() == 2
     assert handle.b2ctr_last_error() is not None
 
 
-def test_struct_layouts_match_header():
+def test_abi_v2_struct_layouts_match_header():
     from deepctr_b200 import _lib as L
     assert ctypes.sizeof(L.Feature) == 112
     assert L.Feature.src_table.offset == 96
     assert ctypes.sizeof(L.Gemm) == 128
-    assert ctypes.sizeof(L.UniformGather) == 160
+    assert ctypes.sizeof(L.UniformGather) == 120
 
 
 def test_kernels_refuse_cpu_tensors():

@@ -384,15 +384,15 @@ def test_dropout_mask_is_consistent_between_forward_and_backward(cuda):
     (300, 26, 16, (128, 128), True, "relu"),     # the C3 layer sizes: K' = 832 / 1664, 2-CTA tiles, ragged last row tile
 ])
 @pytest.mark.parametrize("fold", [True, False])
-def test_cin_generated_outer_product(cuda, B, F, E_, layer_size, split_half, act, fold):
+def test_cin_fused_generated_outer_product(cuda, B, F, E_, layer_size, split_half, act, fold):
     """b2ctr_cin_gemm: the outer product is generated inside the tensor-core GEMM producer (forward and filter
     gradient); checked against the oracle's literal op sequence, all gradients."""
     from deepctr_b200.layers import CIN
     from deepctr_b200 import ops, _lib as L
     ops.set_gemm_precision("bf16x3")
-    assert ops.CIN_FUSED
     rng = np.random.RandomState(21)
     x = rng.normal(0, 0.5, size=(B, F, E_)).astype(np.float32)
+    assert ops.cin_fusable(x, layer_size, split_half)
     layer = CIN(layer_size, act, split_half, seed=3)
     layer.build((None, F, E_))
     for w in layer.weights:
