@@ -77,6 +77,18 @@ class AttGemm(C.Structure):
                 ("act", C.c_int32), ("mode", C.c_int32), ("split_k", C.c_int32)]
 
 
+class Mha(C.Structure):
+    """b2ctr_mha_t"""
+    _fields_ = [("q", C.c_void_p), ("ldq", C.c_int64), ("k", C.c_void_p), ("ldk", C.c_int64),
+                ("v", C.c_void_p), ("ldv", C.c_int64), ("res", C.c_void_p), ("ldr", C.c_int64),
+                ("out", C.c_void_p), ("ldo", C.c_int64), ("stats", C.c_void_p),
+                ("qlen", C.c_void_p), ("klen", C.c_void_p), ("qmask", C.c_void_p), ("kmask", C.c_void_p),
+                ("batch", C.c_int64), ("T", C.c_int32), ("heads", C.c_int32), ("d", C.c_int32),
+                ("scale", C.c_float), ("blinding", C.c_int32), ("dropout_rate", C.c_float), ("seed", C.c_uint64),
+                ("dout", C.c_void_p), ("lddo", C.c_int64), ("dq", C.c_void_p), ("lddq", C.c_int64),
+                ("dk", C.c_void_p), ("lddk", C.c_int64), ("dv", C.c_void_p), ("lddv", C.c_int64)]
+
+
 _vp, _i32, _i64, _f32, _sz, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t, C.c_uint64
 
 # name -> (restype, argtypes).  Must list every symbol of include/b2ctr.h (tests check this).
@@ -177,6 +189,12 @@ SIGNATURES = {
     "b2ctr_dice_bwd_workspace_bytes": (_sz, [_i64, _i64]),
     "b2ctr_dice_bwd": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _f32, _i32, _vp, _sz, _vp]),
     "b2ctr_dropout": (_i32, [_vp, _vp, _i64, _f32, _u64, _vp]),
+    "b2ctr_mha_fwd": (_i32, [C.POINTER(Mha), _vp]),
+    "b2ctr_mha_bwd": (_i32, [C.POINTER(Mha), _vp]),
+    "b2ctr_layernorm_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _i32, _f32, _vp]),
+    "b2ctr_layernorm_bwd_workspace_bytes": (_sz, [_i64, _i32]),
+    "b2ctr_layernorm_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _i64, _i32, _vp,
+                                   _sz, _vp]),
     "b2ctr_shard_bucketize": (_i32, [C.POINTER(Feature), _i32, _i64, _i32, _vp, _vp, _vp]),
     "b2ctr_shard_fill": (_i32, [C.POINTER(Feature), _i32, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
     "b2ctr_shard_gather_rows": (_i32, [C.POINTER(_vp), C.POINTER(_vp), _i32, _i32, _vp, _i64, _vp, _vp, _vp]),

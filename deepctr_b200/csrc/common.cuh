@@ -135,6 +135,14 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// counter-based hash behind b2ctr_dropout's keep test: element i survives iff
+// mix32(seed * 0x9E3779B97F4A7C15 + i) >= rate * 2^32 (also used by the attention kernels' dropout)
+__device__ __forceinline__ uint32_t mix32(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ULL;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebULL;
+  return (uint32_t)((z ^ (z >> 31)) >> 32);
+}
+
 __device__ __forceinline__ int64_t load_idx(const void* p, int64_t off, int dtype) {
   return dtype == B2CTR_IDX_I64 ? reinterpret_cast<const int64_t*>(p)[off]
                                 : (int64_t) reinterpret_cast<const int32_t*>(p)[off];

@@ -367,12 +367,7 @@ __global__ void bn_bwd2_kernel(const float* __restrict__ x, const float* __restr
   }
 }
 
-// dropout: keep with prob 1-rate (counter-based hash of (seed, index)), scale by 1/(1-rate)
-__device__ __forceinline__ uint32_t mix32(uint64_t z) {
-  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ULL;
-  z = (z ^ (z >> 27)) * 0x94d049bb133111ebULL;
-  return (uint32_t)((z ^ (z >> 31)) >> 32);
-}
+// dropout: keep with prob 1-rate (counter-based hash of (seed, index), mix32 in common.cuh), scale by 1/(1-rate)
 __global__ void dropout_kernel(const float* __restrict__ x, float* y, int64_t n, float rate, uint64_t seed) {
   const float keep_scale = 1.f / (1.f - rate);
   const uint32_t thr = (uint32_t)(rate * 4294967296.0);

@@ -443,6 +443,14 @@ class Weight(Var):
 # ================================================================================================
 # symbolic graph (Keras functional API)
 # ================================================================================================
+class TensorShape(tuple):
+    """Static shape of a KTensor: a tuple that also answers TensorFlow's ``as_list()`` (the reference's builders
+    call ``tensor.get_shape().as_list()``, e.g. deepctr/models/sequence/bst.py:86)."""
+
+    def as_list(self):
+        return list(self)
+
+
 class KTensor(object):
     """Symbolic tensor produced by ``Input`` or by calling a Layer on symbolic tensors."""
     _count = 0
@@ -456,7 +464,7 @@ class KTensor(object):
         self.name = name or "tensor_%d" % KTensor._count
 
     def get_shape(self):
-        return self.shape
+        return TensorShape(self.shape)
 
     def __repr__(self):
         return "<KTensor %s shape=%s dtype=%s>" % (self.name, self.shape, self.dtype)

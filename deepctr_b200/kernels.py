@@ -802,6 +802,72 @@ def dropout(x, rate, seed):
     return y
 
 
+def _mha_desc(q, ldq, k, ldk, v, ldv, batch, T, heads, d, scale, blinding, rate, seed, stats, qlen, klen, qmask,
+              kmask):
+    a = L.Mha()
+    a.q, a.ldq, a.k, a.ldk, a.v, a.ldv = q.data_ptr(), ldq, k.data_ptr(), ldk, v.data_ptr(), ldv
+    a.stats = stats.data_ptr()
+    a.qlen, a.klen = (qlen.data_ptr() if qlen is not None else None), (klen.data_ptr() if klen is not None else None)
+    a.qmask = qmask.data_ptr() if qmask is not None else None
+    a.kmask = kmask.data_ptr() if kmask is not None else None
+    a.batch, a.T, a.heads, a.d = batch, T, heads, d
+    a.scale, a.blinding, a.dropout_rate, a.seed = scale, int(blinding), rate, seed & 0xFFFFFFFFFFFFFFFF
+    return a
+
+
+def mha_fwd(q, ldq, k, ldk, v, ldv, batch, T, heads, d, scale, blinding=False, rate=0.0, seed=0, res=None, ldr=0,
+            qlen=None, klen=None, qmask=None, kmask=None):
+    """Masked multi-head attention over rows b*T + t of q / k / v (row pitches ld*) -> (out [B*T, heads*d],
+    softmax statistics [B, heads, T, 2]).  Validity from int32 lengths [B] or uint8 masks [B, T]."""
+    _require_cuda(q, k, v, res)
+    out = torch.empty((batch * T, heads * d), dtype=torch.float32, device=q.device)
+    stats = torch.empty((batch, heads, T, 2), dtype=torch.float32, device=q.device)
+    a = _mha_desc(q, ldq, k, ldk, v, ldv, batch, T, heads, d, scale, blinding, rate, seed, stats, qlen, klen, qmask,
+                  kmask)
+    a.res, a.ldr = (res.data_ptr() if res is not None else None), ldr
+    a.out, a.ldo = out.data_ptr(), heads * d
+    L.check(L.lib().b2ctr_mha_fwd(C.byref(a), stream()), "mha_fwd")
+    return out, stats
+
+
+def mha_bwd(dout, lddo, q, ldq, k, ldk, v, ldv, stats, batch, T, heads, d, scale, blinding=False, rate=0.0, seed=0,
+            qlen=None, klen=None, qmask=None, kmask=None):
+    """-> (dq, dk, dv), each [B*T, heads*d]."""
+    _require_cuda(dout, q, k, v, stats)
+    w = heads * d
+    dq, dk, dv = (torch.empty((batch * T, w), dtype=torch.float32, device=q.device) for _ in range(3))
+    a = _mha_desc(q, ldq, k, ldk, v, ldv, batch, T, heads, d, scale, blinding, rate, seed, stats, qlen, klen, qmask,
+                  kmask)
+    a.dout, a.lddo = dout.data_ptr(), lddo
+    a.dq, a.lddq, a.dk, a.lddk, a.dv, a.lddv = dq.data_ptr(), w, dk.data_ptr(), w, dv.data_ptr(), w
+    L.check(L.lib().b2ctr_mha_bwd(C.byref(a), stream()), "mha_bwd")
+    return dq, dk, dv
+
+
+def layernorm_fwd(a, lda, b, ldb, gamma, beta, rows, n, eps):
+    """LayerNormalization of a (+ b) over rows of n columns -> (y [rows, n], stats (mean, rstd) [rows, 2])."""
+    _require_cuda(a, b, gamma, beta)
+    y = torch.empty((rows, n), dtype=torch.float32, device=a.device)
+    stats = torch.empty((rows, 2), dtype=torch.float32, device=a.device)
+    _lib_call("layernorm_fwd", ptr(a), lda, ptr(b), ldb, ptr(gamma), ptr(beta), ptr(y), n, ptr(stats), rows, n, eps,
+              stream())
+    return y, stats
+
+
+def layernorm_bwd(a, lda, b, ldb, gamma, stats, dy, rows, n, want_dgamma=True, want_dbeta=True):
+    """-> (dx [rows, n], dgamma [n] | None, dbeta [n] | None)."""
+    _require_cuda(a, b, gamma, stats, dy)
+    dev = a.device
+    dx = torch.empty((rows, n), dtype=torch.float32, device=dev)
+    dgamma = torch.empty((n,), dtype=torch.float32, device=dev) if want_dgamma else None
+    dbeta = torch.empty((n,), dtype=torch.float32, device=dev) if want_dbeta else None
+    nbytes = L.lib().b2ctr_layernorm_bwd_workspace_bytes(rows, n)
+    ws = workspace(nbytes, dev)
+    _lib_call("layernorm_bwd", ptr(a), lda, ptr(b), ldb, ptr(gamma), ptr(stats), ptr(dy), dy.stride(0), ptr(dx), n,
+              ptr(dgamma), ptr(dbeta), rows, n, ptr(ws), nbytes, stream())
+    return dx, dgamma, dbeta
+
+
 for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
            "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
@@ -861,4 +927,8 @@ for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filte
            "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "moving_update", "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
+    globals()[_n] = _timed(globals()[_n])
+
+
+for _n in ("mha_fwd", "mha_bwd", "layernorm_fwd", "layernorm_bwd"):
     globals()[_n] = _timed(globals()[_n])

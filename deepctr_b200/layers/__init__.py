@@ -4,8 +4,9 @@ from .activation import Dice, Activation, activation_layer
 from .core import DNN, LocalActivationUnit, PredictionLayer
 from .interaction import (AFMLayer, BiInteractionPooling, BilinearInteraction, FM, CrossNet, CIN, InteractingLayer,
                           SENETLayer)
-from .normalization import BatchNormalization, Dropout
-from .sequence import SequencePoolingLayer, WeightedSequenceLayer, AttentionSequencePoolingLayer
+from .normalization import BatchNormalization, Dropout, LayerNormalization
+from .sequence import (SequencePoolingLayer, WeightedSequenceLayer, AttentionSequencePoolingLayer, Transformer,
+                       PositionEncoding)
 from .utils import (NoMask, Hash, Linear, Concat, _Add, concat_func, add_func, combined_dnn_input,
                     reduce_sum, reduce_mean, reduce_max, div, softmax)
 
@@ -17,4 +18,5 @@ custom_objects = {
     'SequencePoolingLayer': SequencePoolingLayer, 'WeightedSequenceLayer': WeightedSequenceLayer,
     'AttentionSequencePoolingLayer': AttentionSequencePoolingLayer, 'Dice': Dice, 'Hash': Hash,
     'Linear': Linear, 'Concat': Concat, 'NoMask': NoMask, '_Add': _Add,
+    'Transformer': Transformer, 'PositionEncoding': PositionEncoding, 'LayerNormalization': LayerNormalization,
 }

@@ -1,1 +1,2 @@
 from .din import DIN
+from .bst import BST

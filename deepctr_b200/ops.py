@@ -335,6 +335,23 @@ def add_n(xs):
     return res
 
 
+def add(x, y):
+    """x + y for two tensors of the same shape (the Transformer's ``result += fw2``, layers/sequence.py:626)."""
+    if tuple(x.shape) != tuple(y.shape):
+        raise ValueError("add: shapes differ: %s vs %s" % (tuple(x.shape), tuple(y.shape)))
+    res = E.Var(K.add_n([E.contiguous(x), E.contiguous(y)]))
+
+    def bwd(grads):
+        # x and y receive the same tensor: add_grad may adopt it as x.grad and later accumulate into it in place.
+        # In the Transformer y (fw2) is produced after x and its backward runs next, before anything else adds
+        # to x, so y has consumed the shared tensor by then.
+        E.add_grad(x, grads[0])
+        E.add_grad(y, grads[0])
+
+    E.record([res], [x, y], bwd)
+    return res
+
+
 def rowsum(x):
     """sum over all non-batch axes -> [B,1]  (Linear mode 0/2, layers/utils.py:160-171)."""
     src, ld = x.flat2d()
@@ -496,20 +513,21 @@ def bilinear_interaction(x, weights, stack, btype, out=None):
     return res
 
 
-def add_bias(x, b):
-    """x + b over the last axis for a per-column (or scalar, when the last axis is 1) bias:
-    Linear(use_bias=True) without a dense part, layers/utils.py:172-173.  Forward = copy + rank-1 update
-    ones[B,1] @ b[1,n] through the skinny GEMM kernel; backward = pass-through and a column sum."""
+def add_bias(x, b, scale=1.0, per_sample=False):
+    """x + scale * b over the last axis for a per-column (or scalar, when the last axis is 1) bias:
+    Linear(use_bias=True) without a dense part, layers/utils.py:172-173.  ``per_sample``: b spans every non-batch
+    axis (PositionEncoding's x + sqrt(E) P[t] over the [B, T*E] view, layers/sequence.py:683-689).  Forward = copy
+    + rank-1 update ones[B,1] @ b[1,n] through the skinny GEMM kernel; backward = pass-through and a column sum."""
     xt = E.contiguous(x)
-    x2 = xt.reshape(-1, xt.shape[-1])
+    x2 = xt.reshape(xt.shape[0], -1) if per_sample else xt.reshape(-1, xt.shape[-1])
     m, n = x2.shape
     bd = b.materialize() if isinstance(b, E.Weight) else b.data
     if bd.numel() != n:
         raise ValueError("add_bias: bias has %d elements, last axis has %d" % (bd.numel(), n))
     y = K.add_n([x2])                                     # copy
     ones = K.fill(torch.empty((m, 1), dtype=torch.float32, device=y.device), 1.0)
-    K.gemm(ones, bd.reshape(1, n), c=y, accumulate=True, m=m, n=n, k=1)
-    out = E.Var(y.reshape(x.data.shape))
+    K.gemm(ones, bd.reshape(1, n), c=y, accumulate=True, alpha=scale, m=m, n=n, k=1)
+    out = E.Var(y.reshape(x.data.shape), mask=x.mask if per_sample else None)
 
     def bwd(grads):
         dy = grads[0]
@@ -520,6 +538,8 @@ def add_bias(x, b):
             if not dy2.is_contiguous():
                 dy2 = dy2.contiguous()
             _, db = K.bias_act_bwd(dy2, None, L.ACT_NONE, want_dz=False, want_dbias=True)
+            if scale != 1.0:
+                db = K.add_n([db], scales=[scale], out=db)
             E.add_grad(b, db.reshape(bd.shape))
 
     E.record([out], [x, b], bwd)
@@ -1075,6 +1095,92 @@ def batchnorm(x, gamma, beta, moving_mean, moving_var, eps, training, momentum=0
 
     E.record([res], [x, gamma, beta], bwd)
     return res
+
+
+def mha(q, k, v, heads, scale, blinding=False, rate=0.0, seed=0, res=None, qlen=None, klen=None, qmask=None,
+        kmask=None):
+    """Masked multi-head scaled-dot-product attention of the reference's Transformer (layers/sequence.py:544-617)
+    on [B, T, heads*d] projections, read in place through their row pitches; ``res`` (added in the epilogue) is
+    the residual.  Validity from int32 lengths (Vars [B, 1]) or uint8 [B, T] masks.  Only [B, heads, T, 2]
+    softmax statistics are kept for the backward, which recomputes the probabilities."""
+    B, T, W = q.shape
+    d = W // heads
+    for name, x in (("k", k), ("v", v), ("res", res)):
+        if x is not None and tuple(x.shape) != (B, T, W):
+            raise ValueError("mha: %s has shape %s, the queries %s" % (name, tuple(x.shape), (B, T, W)))
+    for name, x, want in (("qlen", qlen, B), ("klen", klen, B)):
+        if x is not None and x.data.numel() != want:
+            raise ValueError("mha: %s has %d entries for a batch of %d" % (name, x.data.numel(), want))
+    for name, x in (("qmask", qmask), ("kmask", kmask)):
+        if x is not None and tuple(x.shape) != (B, T):
+            raise ValueError("mha: %s has shape %s, expected %s" % (name, tuple(x.shape), (B, T)))
+    if rate:
+        mark_uncapturable()
+    q2, ldq = _as2d(q)
+    k2, ldk = _as2d(k)
+    v2, ldv = _as2d(v)
+    r2, ldr = _as2d(res) if res is not None else (None, 0)
+    ql = _len_i32(qlen) if qlen is not None else None
+    kl = _len_i32(klen) if klen is not None else None
+    kw = dict(blinding=blinding, rate=rate, seed=seed, qlen=ql, klen=kl, qmask=qmask, kmask=kmask)
+    out, stats = K.mha_fwd(q2, ldq, k2, ldk, v2, ldv, B, T, heads, d, scale, res=r2, ldr=ldr, **kw)
+    o = E.Var(out.reshape(B, T, W))
+
+    def bwd(grads):
+        g = grads[0].reshape(B * T, W)
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dq, dk, dv = K.mha_bwd(g, W, q2, ldq, k2, ldk, v2, ldv, stats, B, T, heads, d, scale, **kw)
+        E.add_grad(q, dq.reshape(q.shape))
+        E.add_grad(k, dk.reshape(k.shape))
+        E.add_grad(v, dv.reshape(v.shape))
+        if res is not None:
+            E.add_grad(res, g.reshape(res.shape))
+
+    E.record([o], [q, k, v, res], bwd)
+    return o
+
+
+def layernorm(a, gamma, beta, eps, b=None):
+    """LayerNormalization over the last axis of a (+ b) (layers/normalization.py:34-43); the sum of the two
+    summands is formed inside the kernel, and both receive the same gradient."""
+    shape = a.shape
+    n = shape[-1]
+    a2, lda = _as2d(a)
+    b2, ldb = _as2d(b) if b is not None else (None, 0)
+    rows = a2.shape[0]
+    gd = _wdata(gamma) if gamma is not None else None
+    bd = _wdata(beta) if beta is not None else None
+    y, stats = K.layernorm_fwd(a2, lda, b2, ldb, gd, bd, rows, n, eps)
+    res = E.Var(y.reshape(shape))
+
+    def bwd(grads):
+        g = grads[0].reshape(rows, n)
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dx, dgamma, dbeta = K.layernorm_bwd(a2, lda, b2, ldb, gd, stats, g, rows, n,
+                                            want_dgamma=gamma is not None and gamma.requires_grad,
+                                            want_dbeta=beta is not None and beta.requires_grad)
+        E.add_grad(a, dx.reshape(shape))
+        if b is not None:
+            # the same tensor for both summands: see ops.add on why the Transformer's tape order makes that safe
+            E.add_grad(b, dx.reshape(shape))
+        if dgamma is not None:
+            E.add_grad(gamma, dgamma.reshape(gamma.shape))
+        if dbeta is not None:
+            E.add_grad(beta, dbeta.reshape(beta.shape))
+
+    E.record([res], [a, b, gamma, beta], bwd)
+    return res
+
+
+def full_lengths(batch, T, device):
+    """int32 [B, 1] filled with T (the unmasked sequence of reduce_mean / reduce_sum over the time axis), written
+    by the fill kernel through a float32 view of the bits."""
+    import struct
+    out = torch.empty((batch, 1), dtype=torch.int32, device=device)
+    K.fill(out.view(torch.float32), struct.unpack("<f", struct.pack("<i", int(T)))[0])
+    return E.Var(out)
 
 
 def dropout(x, rate, seed):

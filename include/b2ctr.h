@@ -566,6 +566,57 @@ B2CTR_API b2ctr_status_t b2ctr_dropout(const float* x, float* y, int64_t n, floa
                                       void* stream);
 
 /* ------------------------------------------------------------------------------------------ */
+/* 6b. Transformer layer of BST (deepctr/layers/sequence.py:431-651, layers/normalization.py:18-51) */
+/* ------------------------------------------------------------------------------------------ */
+/* Masked multi-head scaled-dot-product attention over [B, T, heads*d] (sequence.py:544-617).
+ * Row r = b*T + t of Q / K / V starts at q + r*ldq (k + r*ldk, v + r*ldv); head h is columns [h*d, (h+1)*d).
+ * For every (b, h, query i):
+ *   s_j = scale * q_i . k_j;  s_j = -2^32 where key j is invalid, and on the diagonal j == i when blinding;
+ *   p_j = softmax_j(s);  P_j = p_j * valid_q(i) * keep(i, j) / (1 - dropout_rate)
+ *   out[r*ldo + h*d + c] = sum_j P_j v_j[c] (+ res[r*ldr + h*d + c] when res != NULL)
+ * (a sample whose keys are all masked gets uniform 1/T weights before the query mask, as in the reference).
+ * keep(i, j) is b2ctr_dropout's test on the element index ((h*B + b)*T + i)*T + j of the reference's
+ * head-major [heads*B, T, T] layout; dropout_rate == 0 keeps everything.
+ * Validity: t < qlen[b] (klen) when given, else qmask[b*T + t] != 0 (kmask) when given, else valid.
+ * stats [B, heads, T, 2] = (max_j s_j, sum_j exp(s_j - max)) is all the backward needs: the [B, heads, T, T]
+ * scores and probabilities never reach memory in either direction.
+ * Backward: dq / dk / dv (pitches lddq / lddk / lddv, overwritten) from dout (pitch lddo); the residual's
+ * gradient is dout itself.  One owner per element, terms added in a fixed order, no float atomics:
+ * bit-identical from run to run.  Limits: 1 <= T <= 128, 1 <= d <= 64; anything else is INVALID_ARG. */
+typedef struct b2ctr_mha {
+  const float* q; int64_t ldq;
+  const float* k; int64_t ldk;
+  const float* v; int64_t ldv;
+  const float* res; int64_t ldr;
+  float* out; int64_t ldo;
+  float* stats;
+  const int32_t* qlen; const int32_t* klen;
+  const uint8_t* qmask; const uint8_t* kmask;
+  int64_t batch; int32_t T, heads, d;
+  float scale; int32_t blinding; float dropout_rate; uint64_t seed;
+  const float* dout; int64_t lddo;               /* backward only */
+  float* dq; int64_t lddq;
+  float* dk; int64_t lddk;
+  float* dv; int64_t lddv;
+} b2ctr_mha_t;
+B2CTR_API b2ctr_status_t b2ctr_mha_fwd(const b2ctr_mha_t* a, void* stream);
+B2CTR_API b2ctr_status_t b2ctr_mha_bwd(const b2ctr_mha_t* a, void* stream);
+
+/* LayerNormalization (normalization.py:34-43) over the last axis of x = a (+ b), rows of n <= 1024 columns:
+ *   mean = avg(x), var = avg((x - mean)^2), y = (x - mean) / sqrt(var + eps) * gamma + beta
+ * gamma / beta may be NULL (scale / center off); b may be NULL.  stats [rows, 2] = (mean, 1/sqrt(var + eps)).
+ * Backward: dx (pitch lddx, overwritten; the gradient of both summands), dgamma / dbeta [n] (overwritten, may be
+ * NULL) through per-CTA partials in the workspace summed in CTA order: bit-identical from run to run. */
+B2CTR_API b2ctr_status_t b2ctr_layernorm_fwd(const float* a, int64_t lda, const float* b, int64_t ldb,
+                                            const float* gamma, const float* beta, float* y, int64_t ldy,
+                                            float* stats, int64_t rows, int32_t n, float eps, void* stream);
+B2CTR_API size_t b2ctr_layernorm_bwd_workspace_bytes(int64_t rows, int32_t n);
+B2CTR_API b2ctr_status_t b2ctr_layernorm_bwd(const float* a, int64_t lda, const float* b, int64_t ldb,
+                                            const float* gamma, const float* stats, const float* dy, int64_t lddy,
+                                            float* dx, int64_t lddx, float* dgamma, float* dbeta, int64_t rows,
+                                            int32_t n, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------ */
 /* 7. Row-sharded embedding exchange (SURVEY.md 8e; new capability, no reference counterpart)     */
 /*    row r of every table lives on rank r % world as local row r / world.                        */
 /* ------------------------------------------------------------------------------------------ */
