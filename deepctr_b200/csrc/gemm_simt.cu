@@ -536,7 +536,11 @@ b2ctr_status_t b2ctr_split_planes(const float* src, int64_t ld, int64_t rows, in
 
 b2ctr_status_t b2ctr_gemm(const b2ctr_gemm_t* g, void* workspace, size_t workspace_bytes,
                           void* stream) {
-  B2_REQUIRE(g && g->a && g->b && g->c, "gemm: NULL descriptor or matrix pointer");
+  B2_REQUIRE(g && g->c, "gemm: NULL descriptor or matrix pointer");
+  // bf16x3 with caller planes: gemm_bf16x3 checks that an fp32 operand left NULL is not one it has to split
+  const bool bf = g->precision == B2CTR_GEMM_BF16X3;
+  B2_REQUIRE((g->a || (bf && g->a_planes)) && (g->b || (bf && g->b_planes)),
+             "gemm: NULL A or B (allowed only in bf16x3 mode with the operand's planes)");
   B2_REQUIRE(g->m >= 0 && g->n >= 0 && g->k >= 0, "gemm: negative dimension");
   B2_REQUIRE(g->lda >= (g->trans_a ? g->m : g->k) && g->ldb >= (g->trans_b ? g->k : g->n) &&
                  g->ldc >= g->n,

@@ -206,7 +206,8 @@ __device__ __forceinline__ void with_majorness(int a_mn, int b_mn, F&& f) {
 // Epilogue straight from the accumulator fragment of m64nBN: thread (warp w of the warpgroup, lane l) holds rows
 // row0 + 16w + l/4 (+ 8) and columns n0 + 8i + 2(l % 4) + {0, 1} in d[4i + {0, 1}] (and d[4i + {2, 3}] for the
 // row + 8).  Each group of four lanes writes 32 contiguous bytes of a row.  C = act(alpha acc [+ C] [+ bias]);
-// split-K slices go to the workspace instead (ws[z][m][n], reduced by tc_splitk_reduce_kernel).
+// split-K slices go to the workspace instead (ws[z][m][n], reduced by tc_splitk_reduce_kernel).  The persistent
+// kernel uses it for what store_acc_tma cannot store (accumulate, unaligned C, split-K with n % 4 != 0).
 template <int BN>
 __device__ __forceinline__ void store_acc(const PlaneArgs& g, const float (&d)[BN / 2], int64_t row0, int64_t n0,
                                           int64_t z) {
@@ -273,6 +274,60 @@ __global__ void tc_splitk_reduce_kernel(const PlaneArgs g) {
     if (g.bias) v += g.bias[gn];
     g.c[gm * g.ldc + gn] = act_apply(v, g.act);
   }
+}
+// The same reduction for n % 4 == 0: a thread owns four consecutive outputs of a row, loads the slices' float4 partials
+// kReduceBatch at a time (all in flight before the first add) and adds them in ascending z from 0.f, then accumulate,
+// bias and activation, as tc_splitk_reduce_kernel does: bit-identical results.  The scalar kernel issued one load per
+// add from a loop with a run-time trip count, so at 256 x 128 x 64 slices its 32768 threads were load-latency-bound.
+constexpr int kReduceBatch = 16;
+__global__ void __launch_bounds__(128) tc_splitk_reduce4_kernel(const PlaneArgs g) {
+  const int64_t total4 = g.m * g.n / 4;
+  const float4* ws = reinterpret_cast<const float4*>(g.ws);
+  const bool vec_c = g.ldc % 4 == 0 && ((reinterpret_cast<uintptr_t>(g.c) & 15) == 0);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total4;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    float v[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int z0 = 0; z0 < g.splits; z0 += kReduceBatch) {
+      float4 p[kReduceBatch];
+#pragma unroll
+      for (int j = 0; j < kReduceBatch; ++j)
+        if (z0 + j < g.splits) p[j] = __ldcs(ws + (int64_t)(z0 + j) * total4 + i);
+#pragma unroll
+      for (int j = 0; j < kReduceBatch; ++j)
+        if (z0 + j < g.splits) {
+          v[0] += p[j].x; v[1] += p[j].y; v[2] += p[j].z; v[3] += p[j].w;
+        }
+    }
+    const int64_t gm = (4 * i) / g.n, gn = 4 * i - gm * g.n;
+    float* cp = g.c + gm * g.ldc + gn;
+    if (g.accumulate) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) v[e] += cp[e];
+    }
+    if (g.bias) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) v[e] += __ldg(g.bias + gn + e);
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e) v[e] = act_apply(v[e], g.act);
+    if (vec_c) *reinterpret_cast<float4*>(cp) = make_float4(v[0], v[1], v[2], v[3]);
+    else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) cp[e] = v[e];
+    }
+  }
+}
+// split-K reduction of a persistent-kernel launch: the float4 kernel when the workspace rows allow it, with blocks
+// small enough that the grid covers the SMs (256 x 128 is 8192 threads, 128 x 64 only 2048)
+static void splitk_reduce(const PlaneArgs& pa, cudaStream_t st) {
+  if (pa.n % 4 != 0 || ((uintptr_t)pa.ws & 15) != 0) {
+    tc_splitk_reduce_kernel<<<grid_for(pa.m * pa.n, 256, 4), 256, 0, st>>>(pa);
+    return;
+  }
+  const int64_t total4 = pa.m * pa.n / 4;
+  int tpb = 128;
+  while (tpb > 32 && ceil_div(total4, tpb) < kNumSMs) tpb /= 2;
+  tc_splitk_reduce4_kernel<<<grid_for(total4, tpb, 2048 / tpb), tpb, 0, st>>>(pa);
 }
 
 // ================================================================================================
@@ -451,7 +506,8 @@ static cudaError_t launch_planes(const PlaneArgs& pa, cudaStream_t st) {
 //                producers once both groups have retired.  Named barriers order the MMA phases: a warpgroup starts
 //                a tile only after the other one has issued the previous tile's last k-block.  The generated-operand and FOLD kernels stay COOPERATIVE: each warpgroup owns 64 rows of
 //                every tile and both run the epilogue together (their producers / fold leave no registers for a
-//                second accumulator).
+//                second accumulator).  The plain kernels run cooperatively too when a split-K launch has at most
+//                one unit per CTA (WsArgs::coop): ping-pong would leave warpgroup 1 idle.
 //   producers  : GEN = 0: one elected thread arms the stage barrier and issues cp.async.bulk.tensor.2d (TMA) loads
 //                of the four plane slices; its warpgroup gives up its registers to the ping-pong consumers.
 //                GEN = 1 / 2: eight warps GENERATE the A tile in shared memory (CIN outer product / DIN attention
@@ -469,7 +525,9 @@ struct WsArgs {
   PlaneArgs p;
   int tiles_m, tiles_n;
   int64_t ntiles;
-  int c_tma;          // the epilogue stores C through shared memory with TMA (store_acc_tma) instead of store_acc
+  int c_tma;          // the epilogue stores through shared memory with TMA (store_acc_tma) instead of store_acc:
+                      // 1 = C (2-D map), 2 = split-K slices into the workspace (3-D map)
+  int coop;           // plain kernels: the consumers run cooperatively instead of ping-pong
 };
 // bytes of one consumer warpgroup's epilogue staging buffer: 64 rows x one 64-column half of the tile, fp32
 template <int BN>
@@ -493,6 +551,11 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int32_t c0, int32_t c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(src),
                "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int32_t c0, int32_t c1, int32_t c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(map), "r"(src),
+               "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
@@ -522,14 +585,16 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 // The activation is a template parameter (ACT < 0: g.act at run time) and the checks that are uniform over the
 // tile are taken outside the element loop, so the loop is straight-line code: with one warp per SM sub-partition
 // the epilogue is bound by instruction latency, not by shared-memory or store bandwidth.
+// Split-K slices (z >= 0) leave the same way: alpha acc only, stored into slice z of the workspace through a 3-D map
+// {n, m, splits} that clips rows >= m inside the slice.  That map needs n % 4 == 0, so a slice has no tail columns.
 template <int BN, int ACT>
 __device__ __forceinline__ void store_acc_tma_act(const PlaneArgs& g, const float (&d)[BN / 2], const CUtensorMap* map,
-                                                  uint32_t stg, int wg, int64_t row0, int64_t n0) {
+                                                  uint32_t stg, int wg, int64_t row0, int64_t n0, int32_t z) {
   constexpr int HALF = BN < 64 ? BN : 64;
   const int t = threadIdx.x & 127, lane = t & 31, w = t >> 5;
   const int64_t n4 = g.n & ~(int64_t)3;
   const bool tail = n0 + BN > n4;       // the tile holds columns past the map (stored from registers)
-  const float* bias = g.bias;
+  const float* bias = z < 0 ? g.bias : nullptr;
   const float alpha = g.alpha;
 #pragma unroll
   for (int hf = 0; hf < BN / HALF; ++hf) {
@@ -570,18 +635,21 @@ __device__ __forceinline__ void store_acc_tma_act(const PlaneArgs& g, const floa
 #pragma unroll
       for (int b = 0; b < HALF / 32; ++b) {
         const int64_t c0 = n0 + hf * HALF + 32 * b;
-        if (c0 < n4) tma_store_2d(map, stg + b * 8192, (int32_t)c0, (int32_t)row0);
+        if (c0 >= n4) continue;
+        if (z < 0) tma_store_2d(map, stg + b * 8192, (int32_t)c0, (int32_t)row0);
+        else tma_store_3d(map, stg + b * 8192, (int32_t)c0, (int32_t)row0, z);
       }
       bulk_commit();
     }
   }
 }
+// z < 0: C = act(alpha acc + bias) through the 2-D C map; z >= 0: split-K slice z through the 3-D workspace map
 template <int BN>
 __device__ __forceinline__ void store_acc_tma(const PlaneArgs& g, const float (&d)[BN / 2], const CUtensorMap* map,
-                                              uint32_t stg, int wg, int64_t row0, int64_t n0) {
-  if (g.act == B2CTR_ACT_NONE) store_acc_tma_act<BN, B2CTR_ACT_NONE>(g, d, map, stg, wg, row0, n0);
-  else if (g.act == B2CTR_ACT_RELU) store_acc_tma_act<BN, B2CTR_ACT_RELU>(g, d, map, stg, wg, row0, n0);
-  else store_acc_tma_act<BN, -1>(g, d, map, stg, wg, row0, n0);
+                                              uint32_t stg, int wg, int64_t row0, int64_t n0, int32_t z) {
+  if (z >= 0 || g.act == B2CTR_ACT_NONE) store_acc_tma_act<BN, B2CTR_ACT_NONE>(g, d, map, stg, wg, row0, n0, z);
+  else if (g.act == B2CTR_ACT_RELU) store_acc_tma_act<BN, B2CTR_ACT_RELU>(g, d, map, stg, wg, row0, n0, z);
+  else store_acc_tma_act<BN, -1>(g, d, map, stg, wg, row0, n0, z);
 }
 
 // fp32 pair -> bf16 hi pair + bf16 lo pair (v = hi + lo up to 2^-17): two cvt.rn.bf16x2.f32 + four ALU ops
@@ -722,7 +790,7 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
       // of the B planes
       mbar_init(&full_bar[s], GEN == 1 ? 1 + 256 : GEN == 2 ? 1 + 128 : 1);
       // a stage is released by every consumer warp (cooperative) or by the four warps of the tile's owner (ping-pong)
-      mbar_init(&empty_bar[s], PINGPONG ? kWsConsumerWarps / 2 : kWsConsumerWarps);
+      mbar_init(&empty_bar[s], PINGPONG && !w.coop ? kWsConsumerWarps / 2 : kWsConsumerWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -975,9 +1043,15 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
           if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
         const int64_t row0 = mt * kTM;
-        if (w.c_tma) {
-          store_acc_tma<BN>(g, d0, &tm_c, stg, wg, row0, nt * BN);
-          store_acc_tma<BN>(g, d1, &tm_c, stg, wg, row0 + 64, nt * BN);
+        // (z is a constant -1 for plain outputs: a run-time z in their epilogue cost the forward and dgrad launches
+        // several microseconds each)
+        if (w.c_tma == 2) {
+          const int32_t z = (int32_t)(tile / ((int64_t)w.tiles_n * w.tiles_m));
+          store_acc_tma<BN>(g, d0, &tm_c, stg, wg, row0, nt * BN, z);
+          store_acc_tma<BN>(g, d1, &tm_c, stg, wg, row0 + 64, nt * BN, z);
+        } else if (w.c_tma) {
+          store_acc_tma<BN>(g, d0, &tm_c, stg, wg, row0, nt * BN, -1);
+          store_acc_tma<BN>(g, d1, &tm_c, stg, wg, row0 + 64, nt * BN, -1);
         } else {
           const int64_t z = tile / ((int64_t)w.tiles_n * w.tiles_m);
           store_acc<BN>(g, d0, row0, nt * BN, z);
@@ -1065,8 +1139,11 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
             }
           }
         } else if (w.c_tma) {
-          store_acc_tma<BN>(g, d, &tm_c, smem_u32(tiles + STAGES * STAGE + wg * ws_staging_bytes<BN>()), wg, row0,
-                            nt * BN);
+          const uint32_t stg = smem_u32(tiles + STAGES * STAGE + wg * ws_staging_bytes<BN>());
+          if (w.c_tma == 2)
+            store_acc_tma<BN>(g, d, &tm_c, stg, wg, row0, nt * BN, (int32_t)(tile / ((int64_t)w.tiles_n * w.tiles_m)));
+          else
+            store_acc_tma<BN>(g, d, &tm_c, stg, wg, row0, nt * BN, -1);
         } else {
           const int64_t z = tile / ((int64_t)w.tiles_n * w.tiles_m);
           store_acc<BN>(g, d, row0, nt * BN, z);
@@ -1082,11 +1159,17 @@ __global__ void __launch_bounds__(WsLayout<GEN != 0>::kThreads, 1)
       else consume(Major<0>{}, Major<1>{});
     } else {
       setmaxnreg_inc<224>();       // two accumulators: 56 (producers) x 128 + 224 x 256 threads = 384 x 168 registers
+      // w.coop (split-K launches with at most one unit per CTA): ping-pong would leave warpgroup 1 idle, so both
+      // warpgroups take 64 rows of the unit, in variant 3's order
+      auto run = [&](auto ta, auto tb) {
+        if (w.coop) consume(ta, tb);
+        else pingpong(ta, tb);
+      };
       if constexpr (BN < 64) {
-        if (g.a_mn) pingpong(Major<1>{}, Major<0>{});
-        else pingpong(Major<0>{}, Major<0>{});
+        if (g.a_mn) run(Major<1>{}, Major<0>{});
+        else run(Major<0>{}, Major<0>{});
       } else {
-        with_majorness(g.a_mn, g.b_mn, pingpong);
+        with_majorness(g.a_mn, g.b_mn, run);
       }
     }
   }
@@ -1163,6 +1246,22 @@ static bool tma_map_c(CUtensorMap* m, const PlaneArgs& p) {
              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) ==
          CUDA_SUCCESS;
 }
+// Split-K workspace map for the same epilogue: fp32 [splits, m, n] (ws[z][m][n]), box 32 x 64 x 1.  The third
+// dimension keeps TMA's row clipping at m inside each slice.  Rows must be whole 16-byte units (n % 4 == 0);
+// otherwise the slices keep the register epilogue.  Returns whether wa.c_tma may be 2.
+static bool tma_map_ws(CUtensorMap* m, const PlaneArgs& p) {
+  EncodeTiledFn enc = tma_encoder();
+  if (!enc || p.splits < 2 || !p.ws || ((uintptr_t)p.ws & 15) || p.n % 4 || p.m >= (1ll << 31) ||
+      p.n >= (1ll << 31))
+    return false;
+  cuuint64_t dims[3] = {(cuuint64_t)p.n, (cuuint64_t)p.m, (cuuint64_t)p.splits};
+  cuuint64_t strides[2] = {(cuuint64_t)p.n * 4, (cuuint64_t)(p.m * p.n) * 4};
+  cuuint32_t box[3] = {32, 64, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, p.ws, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) ==
+         CUDA_SUCCESS;
+}
 
 static inline int64_t round_up(int64_t v, int64_t q) { return (v + q - 1) / q * q; }
 // Padded extent of caller planes: rows to 256 (largest N tile of a K-major B / M tile pair), columns to 128
@@ -1211,6 +1310,9 @@ b2ctr_status_t gemm_bf16x3(const b2ctr_gemm_t* g, void* workspace, size_t worksp
   const int64_t b_sr = g->trans_b ? g->n : g->k, b_sc = g->trans_b ? g->k : g->n;
   const bool a_given = g->a_planes != nullptr;
   const bool b_given = g->b_planes && (b_kc || bn >= 64);
+  // an fp32 operand is read only when this call splits it (given planes are used whenever the tiling allows)
+  B2_REQUIRE(a_given || g->a, "gemm: NULL A without its planes");
+  B2_REQUIRE(b_given || g->b, "gemm: NULL B, and its planes are missing or unusable at N = %lld", (long long)g->n);
   if (b_given && !b_kc && planes_cols_pad(b_sc) % bn != 0) bn = planes_cols_pad(b_sc) == 64 ? 64 : 128;   // N tiles inside the pad
   const int64_t np = round_up(g->n, bn);
   const int a_mn = !a_kc;
@@ -1277,7 +1379,11 @@ b2ctr_status_t gemm_bf16x3(const b2ctr_gemm_t* g, void* workspace, size_t worksp
       set_error("b2ctr_gemm(bf16x3): cuTensorMapEncodeTiled unavailable (the kernel loads its operands by TMA)");
       return B2CTR_ERR_UNSUPPORTED;
     }
-    wa.c_tma = tma_map_c(&tm.c, pa);
+    wa.c_tma = tma_map_c(&tm.c, pa) ? 1 : tma_map_ws(&tm.c, pa) ? 2 : 0;
+    // split-K with at most one unit per CTA (256 -> 128 and 128 -> 64 wgrads: 128 and 64 units): cooperative
+    // consumers.  With more units (845 -> 256: 252 on 132 CTAs) ping-pong overlaps one unit's epilogue with the
+    // next one's MMAs.
+    wa.coop = splits > 1 && wa.ntiles <= kNumSMs;
     if (bn == 32) e = launch_ws_impl<32, 5>(wa, tm, st);
     else if (bn == 64) e = launch_ws_impl<64, 4>(wa, tm, st);
     else e = launch_ws_impl<128, 3>(wa, tm, st);
@@ -1291,7 +1397,9 @@ b2ctr_status_t gemm_bf16x3(const b2ctr_gemm_t* g, void* workspace, size_t worksp
   }
   count_launch();
   if (splits > 1) {
-    tc_splitk_reduce_kernel<<<grid_for(g->m * g->n, 256, 4), 256, 0, st>>>(pa);
+    // variant 3 keeps the scalar reduction: the reference the persistent path is compared against
+    if (ws_kernel) splitk_reduce(pa, st);
+    else tc_splitk_reduce_kernel<<<grid_for(g->m * g->n, 256, 4), 256, 0, st>>>(pa);
     B2_CHECK_LAUNCH("b2ctr_gemm(bf16x3 splitk_reduce)");
   }
   return B2CTR_OK;
@@ -1400,6 +1508,7 @@ static b2ctr_status_t gen_gemm(const GenSpec& sp, int mode, int64_t n, const voi
   }
   tm.ah = tm.bh; tm.al = tm.bl;
   wa.c_tma = tma_map_c(&tm.c, pa);
+  wa.coop = 0;
   const cudaError_t e = sp.kind == 1 ? launch_gen<1>(wa, tm, bn, st) : launch_gen<2>(wa, tm, bn, st);
   if (e != cudaSuccess) {
     set_error("%s: CUDA launch failed: %s", what, cudaGetErrorString(e));
@@ -1468,6 +1577,7 @@ b2ctr_status_t cin_fold(const b2ctr_cin_gemm_t* g, float* dt0, float* dxk, int64
     return B2CTR_ERR_UNSUPPORTED;
   }
   wa.c_tma = 0;      // the fold epilogue never stores the accumulator tile
+  wa.coop = 0;
   cudaError_t e = launch_ws_impl<128, 3, 0, true>(wa, tm, st);
   if (e != cudaSuccess) {
     set_error("b2ctr_cin_fold: CUDA launch failed: %s", cudaGetErrorString(e));

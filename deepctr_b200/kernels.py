@@ -182,28 +182,41 @@ def init_normal(dst, mean, std, seed):
 def gemm(a, b, c=None, bias=None, trans_a=False, trans_b=False, act=L.ACT_NONE, accumulate=False,
          precision=L.GEMM_FP32, split_k=1, alpha=1.0, m=None, n=None, k=None, variant=0, a_planes=None,
          b_planes=None):
-    """C[M,N] = act(alpha * op(A) @ op(B) + bias) on 2-D row-major (possibly ld-padded) tensors."""
-    _require_cuda(a, b, c, bias)
+    """C[M,N] = act(alpha * op(A) @ op(B) + bias) on 2-D row-major (possibly ld-padded) tensors.
+
+    In BF16X3 mode an fp32 operand may be None when its planes are given (m, n, k then required); the call raises
+    ValueError, before any launch, if it would have to split that operand itself."""
+    _require_cuda(a, b, c, bias, a_planes, b_planes)
+    if (a is None and a_planes is None) or (b is None and b_planes is None):
+        raise ValueError("gemm: an fp32 operand may be None only when its planes are given")
+    if (a is None or b is None) and None in (m, n, k):
+        raise ValueError("gemm: m, n and k are required when an fp32 operand is None")
     if m is None:
         m = a.shape[1] if trans_a else a.shape[0]
     if k is None:
         k = a.shape[0] if trans_a else a.shape[1]
     if n is None:
         n = b.shape[0] if trans_b else b.shape[1]
+    dev = next(t.device for t in (a, b, a_planes, b_planes) if t is not None)
     if c is None:
-        c = torch.empty((m, n), dtype=torch.float32, device=a.device)
+        c = torch.empty((m, n), dtype=torch.float32, device=dev)
     g = L.Gemm()
-    g.a, g.b, g.c = a.data_ptr(), b.data_ptr(), c.data_ptr()
+    g.a = a.data_ptr() if a is not None else None
+    g.b = b.data_ptr() if b is not None else None
+    g.c = c.data_ptr()
     g.bias = bias.data_ptr() if bias is not None else None
     g.m, g.n, g.k = m, n, k
-    g.lda, g.ldb, g.ldc = a.stride(0), b.stride(0), c.stride(0)
+    # (a missing operand gets the smallest leading dimension the C-ABI accepts; it is never read)
+    g.lda = a.stride(0) if a is not None else (m if trans_a else k)
+    g.ldb = b.stride(0) if b is not None else (k if trans_b else n)
+    g.ldc = c.stride(0)
     g.trans_a, g.trans_b = int(trans_a), int(trans_b)
     g.act, g.accumulate, g.precision, g.split_k, g.alpha = act, int(accumulate), precision, split_k, alpha
     g.variant = variant
     g.a_planes = a_planes.data_ptr() if a_planes is not None else None
     g.b_planes = b_planes.data_ptr() if b_planes is not None else None
     nbytes = L.lib().b2ctr_gemm_workspace_bytes(C.byref(g))
-    ws = workspace(nbytes, a.device)
+    ws = workspace(nbytes, dev)
     L.check(L.lib().b2ctr_gemm(C.byref(g), ptr(ws), nbytes if ws is not None else 0, stream()), "gemm")
     return c
 

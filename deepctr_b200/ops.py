@@ -98,11 +98,12 @@ def dense(x, w, b=None, activation=None):
         dzp = None
         if fused_act != L.ACT_NONE or need_db:
             if need_planes and fused_act != L.ACT_NONE and dy.stride(0) % 4 == 0 and K.planes_fusable(m, n):
-                dz, db, dzp = K.bias_act_bwd(dy, y, fused_act, want_dz=True, want_dbias=need_db, want_planes=True)
+                # the dgrad and wgrad below read only the planes (n >= 64 here): dz itself is never written
+                dz, db, dzp = K.bias_act_bwd(dy, y, fused_act, want_dz=False, want_dbias=need_db, want_planes=True)
             else:
                 dz, db = K.bias_act_bwd(dy, y, fused_act, want_dz=fused_act != L.ACT_NONE, want_dbias=need_db)
-            if dz is None:
-                dz = dy
+                if dz is None:
+                    dz = dy
         else:
             dz, db = dy, None
         if need_planes and dzp is None:

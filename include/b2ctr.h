@@ -224,6 +224,8 @@ typedef struct b2ctr_gemm {
   int32_t variant;         /* BF16X3 only: 0 default (persistent), 3 non-persistent reference kernel, 4 persistent */
   const void* a_planes;    /* optional: b2ctr_split_planes() of the STORED a / b matrix.  Lets one split */
   const void* b_planes;    /* serve every GEMM that reads the tensor (forward, dgrad, wgrad); BF16X3 only */
+                           /* a / b may then be NULL unless the call must split that operand itself    */
+                           /* (B with N <= 32 stored [K,N]): B2CTR_ERR_INVALID_ARG                    */
 } b2ctr_gemm_t;
 
 /* bf16 (hi, lo) planes of an fp32 matrix [rows, cols]: hi = bf16(x), lo = bf16(x - hi), zero padded to
