@@ -202,6 +202,8 @@ __global__ void cin_expand_grad_kernel(const float* __restrict__ dout, int64_t l
 // q/k/v/res/out: [B, F, H*D] contiguous.
 // ------------------------------------------------------------------------------------------------
 constexpr int kIntMaxF = 64;
+// F*H*D bound of both entry points: the backward stages K, V, dK and dV (4 F*H*D floats) in 48 KB of shared memory
+constexpr int kIntMaxFHD = 48 * 1024 / (4 * (int)sizeof(float));
 
 __global__ void __launch_bounds__(128)
     interacting_fwd_kernel(const float* __restrict__ q, const float* __restrict__ k,
@@ -1295,9 +1297,10 @@ b2ctr_status_t b2ctr_interacting_fwd(const float* q, const float* k, const float
   B2_REQUIRE(q && k && v && out, "interacting_fwd: NULL pointer");
   B2_REQUIRE(nfield > 0 && nfield <= kIntMaxF && heads > 0 && dhead > 0 && dhead <= 32,
              "interacting_fwd: needs field_size <= %d and att_embedding_size <= 32", kIntMaxF);
+  B2_REQUIRE((int64_t)nfield * heads * dhead <= kIntMaxFHD,
+             "interacting_fwd: field_size * head_num * att_embedding_size must be <= %d", kIntMaxFHD);
   if (batch <= 0) return B2CTR_OK;
   const size_t smem = (size_t)2 * nfield * heads * dhead * sizeof(float);
-  B2_REQUIRE(smem <= 48 * 1024, "interacting_fwd: F*H*D too large for shared memory");
   const float scale = scaling ? 1.f / sqrtf((float)dhead) : 1.f;
   interacting_fwd_kernel<<<(unsigned)batch, 128, smem, ST>>>(q, k, v, res, out, nfield, heads, dhead, scale);
   B2_CHECK_LAUNCH("b2ctr_interacting_fwd");
@@ -1311,9 +1314,10 @@ b2ctr_status_t b2ctr_interacting_bwd(const float* q, const float* k, const float
   B2_REQUIRE(q && k && v && out && dout && dq && dk && dv, "interacting_bwd: NULL pointer");
   B2_REQUIRE(nfield > 0 && nfield <= kIntMaxF && heads > 0 && dhead > 0 && dhead <= 32,
              "interacting_bwd: needs field_size <= %d and att_embedding_size <= 32", kIntMaxF);
+  B2_REQUIRE((int64_t)nfield * heads * dhead <= kIntMaxFHD,
+             "interacting_bwd: field_size * head_num * att_embedding_size must be <= %d", kIntMaxFHD);
   if (batch <= 0) return B2CTR_OK;
   const size_t smem = (size_t)4 * nfield * heads * dhead * sizeof(float);
-  B2_REQUIRE(smem <= 48 * 1024, "interacting_bwd: F*H*D too large for shared memory");
   const float scale = scaling ? 1.f / sqrtf((float)dhead) : 1.f;
   interacting_bwd_kernel<<<(unsigned)batch, 128, smem, ST>>>(q, k, v, out, dout, dq, dk, dv, dres, nfield,
                                                             heads, dhead, scale);

@@ -280,14 +280,15 @@ __global__ void dice_fwd_kernel(const float* __restrict__ x, const float* __rest
   }
 }
 // Dice backward, pass 1: g = dL/dxn = dy * x * (1-alpha) * p * (1-p);  emits
-//   dx_direct = dy * (alpha + (1-alpha) p),  g,  and per-block column partials of [g, g*xn, dy*x*(1-p)]
+//   dx_direct = dy * (alpha + (1-alpha) p),  g,  and per-block column partials of [g, g*xn, dy*x*(1-p)]:
+//   block b's row of 3n partials at partial[b*3n ...], the layout colsum_final_kernel reduces over 3n columns
 __global__ void dice_bwd1_kernel(const float* __restrict__ x, const float* __restrict__ mean,
                                  const float* __restrict__ var, const float* __restrict__ alpha,
                                  const float* __restrict__ dy, float* dx, float* g_out, float* partial,
                                  int64_t m, int64_t n, float eps) {
   const int64_t r0 = (int64_t)blockIdx.x * kStatRows;
   const int64_t r1 = r0 + kStatRows < m ? r0 + kStatRows : m;
-  const int64_t nb = gridDim.x;
+  float* prow = partial + (int64_t)blockIdx.x * 3 * n;
   for (int64_t c = threadIdx.x; c < n; c += blockDim.x) {
     const float mu = mean[c], rs = rsqrtf(var[c] + eps), al = alpha[c];
     float sg = 0.f, sgx = 0.f, sa = 0.f;
@@ -303,9 +304,9 @@ __global__ void dice_bwd1_kernel(const float* __restrict__ x, const float* __res
       sgx += g * xn;
       sa += d * xv * (1.f - p);
     }
-    partial[((int64_t)blockIdx.x) * n + c] = sg;
-    partial[(nb + blockIdx.x) * n + c] = sgx;
-    partial[(2 * nb + blockIdx.x) * n + c] = sa;
+    prow[c] = sg;
+    prow[n + c] = sgx;
+    prow[2 * n + c] = sa;
   }
 }
 // pass 2: dx += rs * (g - [training] (mean_g + xn * mean_gxn))
@@ -329,12 +330,13 @@ __global__ void dice_bwd2_kernel(const float* __restrict__ x, const float* __res
 }
 // BatchNormalization backward (training: batch statistics; inference: constants)
 //   dxn = dy * gamma;  dx = rs * (dxn - [training](mean(dxn) + xn * mean(dxn*xn)))
+// pass 1 writes block b's column partials [dy, dy*xn] as one row of 2n at partial[b*2n ...]
 __global__ void bn_bwd1_kernel(const float* __restrict__ x, const float* __restrict__ mean,
                                const float* __restrict__ var, const float* __restrict__ dy, float* partial,
                                int64_t m, int64_t n, float eps) {
   const int64_t r0 = (int64_t)blockIdx.x * kStatRows;
   const int64_t r1 = r0 + kStatRows < m ? r0 + kStatRows : m;
-  const int64_t nb = gridDim.x;
+  float* prow = partial + (int64_t)blockIdx.x * 2 * n;
   for (int64_t c = threadIdx.x; c < n; c += blockDim.x) {
     const float mu = mean[c], rs = rsqrtf(var[c] + eps);
     float sd = 0.f, sdx = 0.f;
@@ -343,8 +345,8 @@ __global__ void bn_bwd1_kernel(const float* __restrict__ x, const float* __restr
       sd += dy[i];
       sdx += dy[i] * (x[i] - mu) * rs;
     }
-    partial[((int64_t)blockIdx.x) * n + c] = sd;
-    partial[(nb + blockIdx.x) * n + c] = sdx;
+    prow[c] = sd;
+    prow[n + c] = sdx;
   }
 }
 __global__ void bn_bwd2_kernel(const float* __restrict__ x, const float* __restrict__ mean,

@@ -15,6 +15,8 @@ from .normalization import Dropout
 AFM_MAX_FIELDS, AFM_MAX_EMBEDDING, AFM_MAX_FACTOR = 64, 32, 16
 # shapes the SENET / bilinear kernels serve (include/b2ctr.h, b2ctr_senet_fwd, b2ctr_bilinear_fwd)
 SENET_MAX_FIELDS, BILINEAR_MAX_FIELDS, BILINEAR_MAX_EMBEDDING = 64, 64, 64
+# shapes the InteractingLayer attention kernels serve (include/b2ctr.h, b2ctr_interacting_fwd / _bwd)
+INTERACTING_MAX_FIELDS, INTERACTING_MAX_ATT_EMBEDDING, INTERACTING_MAX_FHD = 64, 32, 3072
 
 
 class AFMLayer(Layer):
@@ -260,6 +262,15 @@ class InteractingLayer(Layer):
             raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (len(input_shape)))
         embedding_size = int(input_shape[-1])
         n = self.att_embedding_size * self.head_num
+        fields = input_shape[1]
+        if (fields is not None and int(fields) > INTERACTING_MAX_FIELDS
+                or self.att_embedding_size > INTERACTING_MAX_ATT_EMBEDDING
+                or fields is not None and int(fields) * n > INTERACTING_MAX_FHD):
+            raise ValueError("InteractingLayer supports up to %d fields, att_embedding_size <= %d and "
+                             "fields * head_num * att_embedding_size <= %d (got %s fields, head_num %d, "
+                             "att_embedding_size %d)" % (INTERACTING_MAX_FIELDS, INTERACTING_MAX_ATT_EMBEDDING,
+                                                         INTERACTING_MAX_FHD, fields, self.head_num,
+                                                         self.att_embedding_size))
         self.W_Query = self.add_weight(name='query', shape=[embedding_size, n],
                                        initializer=TruncatedNormal(seed=self.seed))
         self.W_key = self.add_weight(name='key', shape=[embedding_size, n],

@@ -427,7 +427,10 @@ B2CTR_API b2ctr_status_t b2ctr_cin_expand_grad(const float* dout, int64_t ldo, i
                                               int32_t d, int64_t nb, void* stream);
 
 /* InteractingLayer attention core (deepctr/layers/interaction.py:760-777) on projected
- * q/k/v[/res] of shape [B, F, heads*dhead]: out = relu(softmax(q_h k_h^T [/sqrt(d)]) v_h + res). */
+ * q/k/v[/res] of shape [B, F, heads*dhead]: out = relu(softmax(q_h k_h^T [/sqrt(d)]) v_h + res).
+ * Both entry points accept the same shapes: F <= 64, dhead <= 32 and F*heads*dhead <= 3072 (the
+ * backward keeps K, V, dK and dV of one sample in 48 KB of shared memory), so a forward that runs
+ * always has a backward that runs. */
 B2CTR_API b2ctr_status_t b2ctr_interacting_fwd(const float* q, const float* k, const float* v,
                                               const float* res, float* out, int64_t batch,
                                               int32_t nfield, int32_t heads, int32_t dhead,

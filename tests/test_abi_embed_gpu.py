@@ -45,30 +45,32 @@ def test_single_lookup_bit_exact(cuda, dim, dtype):
 
 @pytest.mark.parametrize("mode", ["sum", "mean", "max"])
 @pytest.mark.parametrize("maskmode", ["length", "zero"])
-@pytest.mark.parametrize("dim", [4, 6, 32])
+@pytest.mark.parametrize("dim", [4, 6, 32, 130])
 def test_pooled_bag_bit_exact(cuda, mode, maskmode, dim):
+    """bags of 9 and of 50 positions; dim 130 takes the scalar path with several lane passes"""
     K, L = _kern()
     rng = np.random.RandomState(1)
-    B, T, V = 131, 9, 50
+    B, V = 131, 50
     host, dev = _mk_tables(rng, 1, V, dim, cuda, std=1.0)
-    lens = rng.randint(0, T + 1, size=B)
-    lens[0], lens[1] = 0, T  # empty and full bags
-    idx = rng.randint(1, V, size=(B, T))
-    for b in range(B):
-        idx[b, lens[b]:] = 0
-    idx_t = torch.tensor(idx, dtype=torch.int32)
-    seq = O.embedding_lookup(host[0], idx_t)
-    if maskmode == "length":
-        want = O.sequence_pooling(seq, mode, lengths=torch.tensor(lens))
-        mask_mode, length = L.MASK_LENGTH, torch.tensor(lens, dtype=torch.int32, device=cuda)
-    else:
-        want = O.sequence_pooling(seq, mode, mask=idx_t != 0)
-        mask_mode, length = L.MASK_ZERO_ID, None
-    out = torch.empty((B, dim), device=cuda)
-    f = K.make_feature(dev[0], idx_t.to(cuda), out, maxlen=T, pool=L.POOL_BY_NAME[mode],
-                       mask_mode=mask_mode, length=length)
-    K.embed_gather_fwd([f], B)
-    assert torch.equal(out.cpu(), want[:, 0, :]), "pooled segment results must be bit-exact"
+    for T in (9, 50):
+        lens = rng.randint(0, T + 1, size=B)
+        lens[0], lens[1] = 0, T  # empty and full bags
+        idx = rng.randint(1, V, size=(B, T))
+        for b in range(B):
+            idx[b, lens[b]:] = 0
+        idx_t = torch.tensor(idx, dtype=torch.int32)
+        seq = O.embedding_lookup(host[0], idx_t)
+        if maskmode == "length":
+            want = O.sequence_pooling(seq, mode, lengths=torch.tensor(lens))
+            mask_mode, length = L.MASK_LENGTH, torch.tensor(lens, dtype=torch.int32, device=cuda)
+        else:
+            want = O.sequence_pooling(seq, mode, mask=idx_t != 0)
+            mask_mode, length = L.MASK_ZERO_ID, None
+        out = torch.empty((B, dim), device=cuda)
+        f = K.make_feature(dev[0], idx_t.to(cuda), out, maxlen=T, pool=L.POOL_BY_NAME[mode],
+                           mask_mode=mask_mode, length=length)
+        K.embed_gather_fwd([f], B)
+        assert torch.equal(out.cpu(), want[:, 0, :]), "pooled segment results must be bit-exact (T = %d)" % T
 
 
 @pytest.mark.parametrize("norm", [True, False])
@@ -114,25 +116,191 @@ def test_sequence_emit_and_scatter(cuda):
     torch.testing.assert_close(gtab.cpu(), want, rtol=1e-5, atol=1e-6)
 
 
+NEG_PAD32 = float(np.float32(-4294967295.0))   # the softmax padding -2^32 + 1, which is -2^32 in fp32
+
+
+def _bag64(tab64, ids, valid, mode, weight_mode=None, w=None):
+    """float64 restatement of a pooled (optionally weighted) bag, sequence.py:76-106 and :155-183.  The max-pool mask
+    x - 1e9 is computed in fp32 as the reference does (every masked |x| < 32 then ties at -1e9); its gradient is 1."""
+    seq = tab64[torch.as_tensor(ids, dtype=torch.int64)]                           # [B, T, E]
+    v = torch.as_tensor(valid)
+    if weight_mode is not None:
+        w64 = torch.as_tensor(w).double()
+        if weight_mode == "softmax":
+            wt = torch.softmax(torch.where(v, w64, torch.full_like(w64, NEG_PAD32)), dim=1)
+        else:
+            wt = torch.where(v, w64, torch.zeros_like(w64))
+        seq = seq * wt[:, :, None]
+    v3 = v[:, :, None]
+    if mode == "max":
+        s32 = seq.detach().float()
+        hist = seq + (torch.where(v3, s32, s32 - 1e9).double() - seq).detach()
+        return hist.amax(dim=1)
+    out = (seq * v3).sum(dim=1)
+    if mode == "mean":
+        out = out / (v.sum(dim=1, keepdim=True).double() + 1e-8)
+    return out
+
+
 @pytest.mark.parametrize("mode", ["sum", "mean", "max"])
 def test_pooled_scatter_matches_autograd(cuda, mode):
+    """table gradient of pooled bags against float64 autograd: length and zero-id masks, a hashed feature, raw and
+    softmax position weights, and a dim that is not a multiple of 4 (the scalar path)"""
     K, L = _kern()
     rng = np.random.RandomState(4)
-    B, T, V, dim = 50, 6, 30, 8
-    host, dev = _mk_tables(rng, 1, V, dim, cuda, std=1.0)
-    lens = rng.randint(0, T + 1, size=B)
-    idx = torch.tensor(rng.randint(1, V, size=(B, T)), dtype=torch.int32)
-    tab = host[0].clone().requires_grad_(True)
-    pooled = O.sequence_pooling(O.embedding_lookup(tab, idx), mode, lengths=torch.tensor(lens))
-    g = torch.tensor(rng.normal(size=(B, dim)).astype(np.float32))
-    (pooled[:, 0, :] * g).sum().backward()
-    gtab = torch.zeros((V, dim), device=cuda)
-    # max pooling re-reads the forward rows (src_table) to find the arg-max positions
-    f = K.make_feature(gtab, idx.to(cuda), g.to(cuda), maxlen=T, pool=L.POOL_BY_NAME[mode],
-                       mask_mode=L.MASK_LENGTH, length=torch.tensor(lens, dtype=torch.int32, device=cuda),
-                       src_table=dev[0])
-    K.embed_scatter_add([f], B, 1.0)
-    torch.testing.assert_close(gtab.cpu(), tab.grad, rtol=1e-5, atol=1e-6)
+    B, T, V = 50, 6, 30
+    # (mask mode, hashed, weight mode, dim)
+    cases = [("length", False, None, 8), ("zero", False, None, 8), ("zero", True, None, 6),
+             ("length", False, "raw", 8), ("length", False, "softmax", 6), ("zero", True, "softmax", 8),
+             ("zero", False, "raw", 6)]
+    for maskmode, hashed, weight_mode, dim in cases:
+        what = "%s mask, hashed=%s, weights %s, dim %d" % (maskmode, hashed, weight_mode, dim)
+        host, dev = _mk_tables(rng, 1, V, dim, cuda, std=1.0)
+        lens = rng.randint(0, T + 1, size=B)
+        lens[0] = 0
+        if hashed:
+            raw = rng.randint(1, 10 ** 6, size=(B, T))
+            raw[rng.rand(B, T) < 0.3] = 0                       # padding ids hash to bucket 0 and are masked
+            raw[0] = 0
+            ids = O.hash_layer(raw, V, mask_zero=True)
+            idx = torch.tensor(raw, dtype=torch.int64)
+        else:
+            ids = rng.randint(0 if maskmode == "zero" else 1, V, size=(B, T))
+            ids[0] = 0
+            idx = torch.tensor(ids, dtype=torch.int32)
+        valid = np.arange(T)[None, :] < lens[:, None] if maskmode == "length" else ids != 0
+        w = rng.normal(size=(B, T)).astype(np.float32)
+        tab = host[0].double().requires_grad_(True)
+        pooled = _bag64(tab, ids, valid, mode, weight_mode, w)
+        g = torch.tensor(rng.normal(size=(B, dim)).astype(np.float32))
+        (pooled * g.double()).sum().backward()
+        gtab = torch.zeros((V, dim), device=cuda)
+        # max pooling re-reads the forward rows (src_table) to find the arg-max positions
+        f = K.make_feature(gtab, idx.to(cuda), g.to(cuda), maxlen=T, pool=L.POOL_BY_NAME[mode],
+                           mask_mode=L.MASK_LENGTH if maskmode == "length" else L.MASK_ZERO_ID,
+                           length=torch.tensor(lens, dtype=torch.int32, device=cuda) if maskmode == "length" else None,
+                           hash_mode=L.HASH_FARM_MASK_ZERO if hashed else L.HASH_NONE,
+                           weight=torch.tensor(w, device=cuda) if weight_mode else None,
+                           weight_mode={None: L.WEIGHT_NONE, "raw": L.WEIGHT_RAW, "softmax": L.WEIGHT_SOFTMAX}[weight_mode],
+                           src_table=dev[0])
+        K.embed_scatter_add([f], B, 1.0)
+        # atomics add a row's contributions in any order: fp32 tolerance against float64
+        torch.testing.assert_close(gtab.cpu().double(), tab.grad, rtol=1e-5, atol=1e-6, msg=what)
+
+
+def test_mixed_features_one_launch(cuda):
+    """~70 features of dims 3 / 8 / 64 / 130 in one gather and one scatter call (two 64-descriptor launches, the
+    sub-warp width set by the widest feature): every pool mode, hashed and plain, int32 and int64 ids, each
+    feature's ids (and lengths) a column window of one packed id buffer, weights a column window of a wider float
+    buffer, outputs at out_col of a row wider than the features.  Unweighted results are bit-exact against the
+    oracle; weighted ones and the scatter (atomics) are compared with float64."""
+    K, L = _kern()
+    rng = np.random.RandomState(21)
+    B, V, nf = 301, 23, 70
+    dims = [3, 8, 64, 130]
+    pools = ["none", "sum", "mean", "max"]
+    spec = []                                   # (dim, pool, T, hashed, int64, mask, weight)
+    for i in range(nf):
+        pool = pools[(i // 4) % 4]
+        T = 1 if (pool == "none" and i % 3 == 0) else 2 + i % 6
+        mask = "none" if pool == "none" else ("zero" if i % 3 == 0 else "length")
+        weight = None if pool == "none" else [None, "raw", "softmax"][(i // 16) % 3]
+        spec.append((dims[i % 4], pool, T, i % 3 == 0, i % 2 == 1, mask, weight))
+    # packed id buffers (int32 also holds the lengths) and the weight buffer, each feature a column window
+    n32 = n64 = 0
+    cols = []                                   # (first id column, length column or None)
+    for dim, pool, T, hashed, i64, mask, weight in spec:
+        if i64:
+            ic, n64 = n64, n64 + T
+        else:
+            ic, n32 = n32, n32 + T
+        lc = None
+        if mask == "length":
+            lc, n32 = n32, n32 + 1
+        cols.append((ic, lc))
+    ids32 = np.zeros((B, n32 + 3), dtype=np.int32)
+    ids64 = np.zeros((B, n64 + 3), dtype=np.int64)
+    wcols = sum(T for _, _, T, *_ in spec)
+    wbuf = rng.normal(size=(B, wcols + 5)).astype(np.float32)
+    widths = [T * dim if pool == "none" else dim for dim, pool, T, *_ in spec]
+    ld = sum(widths) + 7
+    per = []                                    # reference inputs per feature
+    wc = 0
+    for (dim, pool, T, hashed, i64, mask, weight), (ic, lc) in zip(spec, cols):
+        buf = ids64 if i64 else ids32
+        raw = rng.randint(1, 10 ** 6 if hashed else V, size=(B, T))
+        lens = rng.randint(0, T + 1, size=B)
+        lens[0] = 0
+        if mask == "zero":
+            raw[rng.rand(B, T) < 0.3] = 0
+            raw[0] = 0
+        buf[:, ic:ic + T] = raw
+        if lc is not None:
+            ids32[:, lc] = lens
+        ids = O.hash_layer(raw, V, mask_zero=True) if hashed else raw
+        valid = (ids != 0) if mask == "zero" else (np.arange(T)[None, :] < lens[:, None]) if mask == "length" \
+            else np.ones((B, T), dtype=bool)
+        per.append((ids, valid, wc))
+        wc += T
+    host, dev = [], []
+    for dim, *_ in spec:
+        h, d = _mk_tables(rng, 1, V, dim, cuda, std=1.0)
+        host.append(h[0])
+        dev.append(d[0])
+    i32_d, i64_d = torch.tensor(ids32, device=cuda), torch.tensor(ids64, device=cuda)
+    w_d = torch.tensor(wbuf, device=cuda)
+    out = torch.full((B, ld), -3.0, device=cuda)
+
+    def feats(tables, target, src=None):
+        fs, oc = [], 0
+        for k, ((dim, pool, T, hashed, i64, mask, weight), (ic, lc), (_, _, wc0)) in enumerate(zip(spec, cols, per)):
+            ib = i64_d if i64 else i32_d
+            fs.append(K.make_feature(
+                tables[k], ib[:, ic:ic + T], target, out_col=oc, out_ld=ld, maxlen=T,
+                pool=L.POOL_NONE if pool == "none" else L.POOL_BY_NAME[pool],
+                mask_mode={"none": L.MASK_NONE, "zero": L.MASK_ZERO_ID, "length": L.MASK_LENGTH}[mask],
+                length=i32_d[:, lc] if lc is not None else None,
+                weight=w_d[:, wc0:wc0 + T] if weight else None,
+                weight_mode={None: L.WEIGHT_NONE, "raw": L.WEIGHT_RAW, "softmax": L.WEIGHT_SOFTMAX}[weight],
+                hash_mode=L.HASH_FARM_MASK_ZERO if hashed else L.HASH_NONE,
+                src_table=src[k] if src is not None else None))
+            oc += widths[k]
+        return fs
+
+    K.embed_gather_fwd(feats(dev, out), B)
+    got = out.cpu()
+    assert torch.all(got[:, ld - 7:] == -3.0)                       # columns behind the last feature
+    gout = torch.tensor(rng.normal(size=(B, ld)).astype(np.float32))
+    tabs64 = [h.double().requires_grad_(True) for h in host]
+    loss = 0
+    oc = 0
+    for k, (dim, pool, T, hashed, i64, mask, weight) in enumerate(spec):
+        ids, valid, wc0 = per[k]
+        seg = got[:, oc:oc + widths[k]]
+        what = "feature %d (dim %d, %s, T %d, hashed %s, weights %s)" % (k, dim, pool, T, hashed, weight)
+        idt = torch.tensor(ids, dtype=torch.int64)
+        if pool == "none":
+            assert torch.equal(seg, O.embedding_lookup(host[k], idt).reshape(B, T * dim)), what
+            ref = tabs64[k][idt].reshape(B, T * dim)
+        else:
+            w = wbuf[:, wc0:wc0 + T]
+            ref = _bag64(tabs64[k], ids, valid, pool, weight, w)
+            if weight is None:
+                want = O.sequence_pooling(O.embedding_lookup(host[k], idt), pool, mask=torch.tensor(valid))
+                assert torch.equal(seg, want[:, 0, :]), what + ": unweighted pooling must be bit-exact"
+            else:
+                # a sum of at most 7 weighted rows of magnitude < 5: fp32 error well below 1e-5
+                torch.testing.assert_close(seg.double(), ref.detach(), rtol=1e-5, atol=1e-5, msg=what)
+        loss = loss + (ref * gout[:, oc:oc + widths[k]].double()).sum()
+        oc += widths[k]
+    loss.backward()
+    grads = [torch.zeros_like(d) for d in dev]
+    K.embed_scatter_add(feats(grads, gout.to(cuda), src=dev), B, 1.0)
+    # each table row receives up to B*T/V ~ 90 contributions, added by atomics in any order: normwise fp32 tolerance
+    for k, (dim, pool, T, hashed, i64, mask, weight) in enumerate(spec):
+        ref = tabs64[k].grad
+        err = float((grads[k].cpu().double() - ref).abs().max()) / float(ref.abs().max())
+        assert err < 4e-6, "scatter of feature %d (dim %d, %s, weights %s): error %.3g" % (k, dim, pool, weight, err)
 
 
 @pytest.mark.parametrize("dim", [4, 8, 16, 32, 64, 128])

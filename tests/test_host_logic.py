@@ -211,3 +211,19 @@ def test_shard_transport_choice():
     assert parallel.choose_transport(c5, 2) == "peer"      # measured: full rate
     assert parallel.choose_transport(c5, 8) == "a2a"       # measured: peer 17.6 ms, all-to-all 4.2 ms per step
     assert parallel.choose_transport(c5, 1) == "peer"
+
+
+@pytest.mark.parametrize("fields,heads,att", [(64, 2, 32), (65, 1, 8), (4, 1, 33), (64, 4, 13)])
+def test_interacting_layer_rejects_unsupported_shapes_at_build(fields, heads, att):
+    """F <= 64, att_embedding_size <= 32 and F * head_num * att_embedding_size <= 3072 (the attention backward's
+    shared memory): a shape outside is refused when the layer is built, not at the first training step"""
+    from deepctr_b200.layers import InteractingLayer
+    with pytest.raises(ValueError, match="InteractingLayer supports"):
+        InteractingLayer(att_embedding_size=att, head_num=heads).build((None, fields, 16))
+
+
+def test_interacting_layer_builds_at_the_bound():
+    from deepctr_b200.layers import InteractingLayer
+    layer = InteractingLayer(att_embedding_size=16, head_num=3)
+    layer.build((None, 64, 16))
+    assert layer.built
