@@ -1062,7 +1062,9 @@ __host__ __device__ constexpr int bi_dw_smem_floats() {
                                                                           : (kBiThreads / ((EP / 4) * (EP / 4))) * EP * EP;
 }
 
-template <int EP>
+// kPairScalar: the gradient is one scalar per (sample, pair) at out[b*ldo + col0 + p] (FEFM, b2ctr_fefm_bwd)
+// instead of an [E] vector per pair
+template <int EP, bool kPairScalar = false>
 __global__ void __launch_bounds__(kBiThreads) bilinear_dw_kernel(const BiArgs a) {
   constexpr int NOG = EP / 4, NT = NOG * NOG, G = kBiThreads / NT;
   extern __shared__ __align__(16) float sm[];
@@ -1084,7 +1086,8 @@ __global__ void __launch_bounds__(kBiThreads) bilinear_dw_kernel(const BiArgs a)
       if (s < ns && e < E) {
         const int64_t b = b0 + s;
         xv = a.x[b * a.ldx + i * E + e];
-        tv = a.out[b * a.ldo + a.col0 + (int64_t)p * a.pitch + e] * a.x[b * a.ldx + j * E + e];
+        tv = a.out[b * a.ldo + a.col0 + (kPairScalar ? (int64_t)p : (int64_t)p * a.pitch + e)] *
+             a.x[b * a.ldx + j * E + e];
       }
       XS[k] = xv;
       TT[k] = tv;
@@ -1179,6 +1182,325 @@ cudaError_t bi_dispatch(int EP, const BiArgs& a, cudaStream_t s) {
     default: return Op::template run<64>(a, s);
   }
 }
+
+// ------------------------------------------------------------------------------------------------
+// FwFMLayer (deepctr/layers/interaction.py:1395-1411): out[b] = sum_{i<j} r[i][j] <x_i, x_j>, upper triangle of the
+// [F, F] strengths only.  One warp per sample, the sample's [F, E] staged in shared memory (row pitch E+1); lane e
+// computes, for 4 first fields i0..i0+3 at a time, y_k = sum_j rt[j][i0+k] x_j[e] from one float4 of the
+// transposed, zero-padded strengths rt [F][FQ] (rt[j][i] = r[i][j] for i < j, else 0), then adds x_{i0+k}[e] y_k.
+// Backward from g [B, 1]:
+//   dx_i = g * sum_{j != i} r[min(i,j)][max(i,j)] x_j   (same loop on the symmetric rt, partners ascending)
+//   dR[i][j] = sum_b g_b <x_i, x_j> for i < j, 0 elsewhere.
+// The CTA's warps take samples in lockstep rounds; every upper-triangle entry of dR has ONE owner thread that adds
+// the round's samples in warp order into a per-CTA accumulator, written as a partial and summed over the CTAs in
+// CTA order by fwfm_dr_reduce_kernel.  No atomics: bit-identical runs.
+// ------------------------------------------------------------------------------------------------
+constexpr int kFwWarps = 8;
+constexpr int kFwMaxF = 64;
+constexpr int kFwMaxE = 64;
+
+__host__ __device__ __forceinline__ int fw_fq(int F) { return (F + 3) & ~3; }
+static inline size_t fw_fwd_smem(int F, int E) {
+  return sizeof(float) * ((size_t)F * fw_fq(F) + (size_t)kFwWarps * F * (E + 1));
+}
+static inline size_t fw_bwd_smem(int F, int E) {
+  return fw_fwd_smem(F, E) + sizeof(float) * (kFwWarps + 2 * (size_t)(F * (F - 1) / 2));
+}
+static inline int fw_bwd_blocks(int64_t batch) { return grid_for(batch, kFwWarps, 4); }
+
+// rt[j][i] = r[i][j] where i < j (sym: also r[j][i]'s mirror where i > j), 0 elsewhere and in the padding
+__device__ __forceinline__ void fw_stage_r(float* rt, const float* __restrict__ r, int F, bool sym) {
+  const int FQ = fw_fq(F);
+  for (int k = threadIdx.x; k < F * FQ; k += blockDim.x) {
+    const int j = k / FQ, i = k - j * FQ;
+    rt[k] = (i < j) ? r[i * F + j] : (sym && i > j && i < F) ? r[j * F + i] : 0.f;
+  }
+}
+
+// y[k] = sum_{j in [j0, F)} rt[j][i0+k] * sx[j][e]
+__device__ __forceinline__ void fw_rows4(const float* rt, const float* sx, int F, int XP, int i0, int j0, int e,
+                                         float (&y)[4]) {
+  const int FQ = fw_fq(F);
+  y[0] = y[1] = y[2] = y[3] = 0.f;
+  for (int j = j0; j < F; ++j) {
+    const float xj = sx[j * XP + e];
+    const float4 rr = *reinterpret_cast<const float4*>(rt + j * FQ + i0);
+    y[0] = fmaf(rr.x, xj, y[0]);
+    y[1] = fmaf(rr.y, xj, y[1]);
+    y[2] = fmaf(rr.z, xj, y[2]);
+    y[3] = fmaf(rr.w, xj, y[3]);
+  }
+}
+
+__device__ __forceinline__ void fw_stage_x(float* sx, const float* __restrict__ xr, int F, int E, int lane) {
+  const int XP = E + 1;
+  for (int k = lane; k < F * E; k += 32) {
+    const int f = k / E;
+    sx[f * XP + (k - f * E)] = xr[k];
+  }
+}
+
+__global__ void __launch_bounds__(kFwWarps * 32)
+    fwfm_fwd_kernel(const float* __restrict__ x, int64_t ldx, int F, int E, const float* __restrict__ r, float* out,
+                    int64_t ldo, int64_t batch) {
+  extern __shared__ __align__(16) float sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, XP = E + 1;
+  float* rt = sm;
+  float* sx = sm + F * fw_fq(F) + warp * F * XP;
+  fw_stage_r(rt, r, F, false);
+  __syncthreads();
+  const int64_t nw = (int64_t)gridDim.x * kFwWarps;
+  for (int64_t b = (int64_t)blockIdx.x * kFwWarps + warp; b < batch; b += nw) {
+    fw_stage_x(sx, x + b * ldx, F, E, lane);
+    __syncwarp();
+    float acc = 0.f;
+    for (int e = lane; e < E; e += 32) {
+      for (int i0 = 0; i0 < F - 1; i0 += 4) {
+        float y[4];
+        fw_rows4(rt, sx, F, XP, i0, i0 + 1, e, y);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          if (i0 + k < F) acc = fmaf(sx[(i0 + k) * XP + e], y[k], acc);
+      }
+    }
+    acc = warp_sum(acc);
+    if (lane == 0) out[b * ldo] = acc;
+    __syncwarp();   // sx is restaged for the next sample
+  }
+}
+
+__global__ void __launch_bounds__(kFwWarps * 32)
+    fwfm_bwd_kernel(const float* __restrict__ g, int64_t ldg, const float* __restrict__ x, int64_t ldx, int F, int E,
+                    const float* __restrict__ r, float* dx, int64_t lddx, float* partial, int64_t batch) {
+  extern __shared__ __align__(16) float sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, XP = E + 1;
+  const int P = F * (F - 1) / 2;
+  float* rt = sm;                                          // symmetric strengths [F][FQ]
+  float* sxs = sm + F * fw_fq(F);                          // kFwWarps x [F][XP]
+  float* sg = sxs + kFwWarps * F * XP;                     // [kFwWarps]: g of the round's samples
+  float* acc = sg + kFwWarps;                              // [P]: this CTA's dR, entry k owned by thread k % blockDim
+  int* pairs = reinterpret_cast<int*>(acc + P);            // [P]: (i << 8) | j
+  float* sx = sxs + warp * F * XP;
+  fw_stage_r(rt, r, F, true);
+  for (int i = 0, k = 0; i < F; ++i)
+    for (int j = i + 1; j < F; ++j, ++k)
+      if (k % blockDim.x == threadIdx.x) {
+        pairs[k] = (i << 8) | j;
+        acc[k] = 0.f;
+      }
+  __syncthreads();
+  const int64_t step = (int64_t)gridDim.x * kFwWarps;
+  for (int64_t b0 = (int64_t)blockIdx.x * kFwWarps; b0 < batch; b0 += step) {
+    const int64_t b = b0 + warp;
+    if (b < batch) {
+      fw_stage_x(sx, x + b * ldx, F, E, lane);
+      const float gb = g[b * ldg];
+      if (lane == 0) sg[warp] = gb;
+      __syncwarp();
+      if (dx) {
+        float* dr = dx + b * lddx;
+        for (int e = lane; e < E; e += 32) {
+          for (int i0 = 0; i0 < F; i0 += 4) {
+            float y[4];
+            fw_rows4(rt, sx, F, XP, i0, 0, e, y);
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+              if (i0 + k < F) dr[(i0 + k) * E + e] = gb * y[k];
+          }
+        }
+      }
+    }
+    if (!partial) {
+      __syncwarp();
+      continue;
+    }
+    __syncthreads();
+    const int nvalid = (int)min((int64_t)kFwWarps, batch - b0);
+    for (int k = threadIdx.x; k < P; k += blockDim.x) {
+      const int i = pairs[k] >> 8, j = pairs[k] & 255;
+      float a = acc[k];
+      for (int w = 0; w < nvalid; ++w) {
+        const float* xi = sxs + w * F * XP + i * XP;
+        const float* xj = sxs + w * F * XP + j * XP;
+        float d = 0.f;
+        for (int e = 0; e < E; ++e) d = fmaf(xi[e], xj[e], d);
+        a = fmaf(sg[w], d, a);
+      }
+      acc[k] = a;
+    }
+    __syncthreads();   // the round's samples are restaged
+  }
+  if (partial)
+    for (int k = threadIdx.x; k < P; k += blockDim.x) partial[(int64_t)blockIdx.x * P + k] = acc[k];
+}
+
+// dR[i][j] = sum over the n CTA partials (ascending) of entry p(i, j) for i < j; 0 on and below the diagonal
+__global__ void fwfm_dr_reduce_kernel(const float* __restrict__ partial, int n, int F, float* dR) {
+  const int P = F * (F - 1) / 2;
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < F * F; t += gridDim.x * blockDim.x) {
+    const int i = t / F, j = t - i * F;
+    float s = 0.f;
+    if (i < j) {
+      const int p = bi_pair_index(F, i, j);
+      for (int c = 0; c < n; ++c) s += partial[(int64_t)c * P + p];
+    }
+    dR[t] = s;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// FEFMLayer (deepctr/layers/interaction.py:1478-1491).  With S_p = W_p + W_p^T (fefm_sym_kernel, once per step)
+// for the P pairs p = (i < j) in itertools.combinations order:
+//   out[b*ldo + col0 + p] = x_i S_p x_j^T
+// Backward from g[b*ldg + gcol0 + p], read in place:
+//   dx_f = sum_{q != f} g_p(f,q) x_q S_p      (S_p symmetric: the same form for either field of the pair)
+//   dS_p = sum_b g_p x_i^T x_j,   dW_p = dS_p + dS_p^T
+// The products are the register-tiled [TS, EP] x [EP, EP] shared-memory tiles of the bilinear kernels above.
+// * fefm_fwd_kernel: CTA (first field i, sample tile).  x_i's tile is staged once; for every partner j > i the CTA
+//   stages S_p, forms the [TS, E] product and dots each row with x_j in the epilogue (a reduction over the EP/4
+//   threads of a row): no [B, E] intermediate reaches memory.  The field index runs fastest so the CTAs that
+//   share a sample tile find its x_j rows in L2.
+// * fefm_dx_kernel: CTA (field, sample tile); the rows of x_q are scaled by g_p as they are staged and the F-1
+//   partners are accumulated into the same registers in ascending order: one owner per (b, f, e), no atomics.
+// * dS: bilinear_dw_kernel<EP, true> partials per (pair, batch chunk); fefm_dw_reduce_kernel adds the chunks in
+//   ascending order, for both dS_p and its transpose.
+// ------------------------------------------------------------------------------------------------
+constexpr int kFeMaxF = 64;
+constexpr int kFeMaxE = 64;
+
+__global__ void fefm_sym_kernel(const float* __restrict__ W, int E, float* S, int64_t count) {
+  const int ee = E * E;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < count; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = t / ee;
+    const int q = (int)(t - p * ee), r = q / E, c = q - r * E;
+    S[t] = W[t] + W[p * ee + c * E + r];
+  }
+}
+
+template <int EP>
+__global__ void __launch_bounds__(kBiThreads) fefm_fwd_kernel(const BiArgs a) {
+  constexpr int TS = bi_ts<EP>(), AP = bi_apitch<EP>(), NOG = EP / 4;
+  extern __shared__ __align__(16) float sm[];
+  float* AT = sm;
+  float* M = sm + EP * AP;
+  const int F = a.F, E = a.E, i = blockIdx.x;
+  const int o0 = (threadIdx.x % NOG) * 4, s0 = (threadIdx.x / NOG) * 4;
+  const int64_t ntiles = (a.batch + TS - 1) / TS;
+  for (int64_t t = blockIdx.y; t < ntiles; t += gridDim.y) {
+    const int64_t b0 = t * TS;
+    const int ns = (int)min((int64_t)TS, a.batch - b0);
+    for (int k = threadIdx.x; k < TS * EP; k += blockDim.x) {
+      const int s = k / EP, e = k - s * EP;
+      AT[e * AP + s] = (s < ns && e < E) ? a.x[(b0 + s) * a.ldx + i * E + e] : 0.f;
+    }
+    for (int j = i + 1; j < F; ++j) {
+      const int p = bi_pair_index(F, i, j);
+      bi_stage_w<EP>(M, a.W + (int64_t)p * E * E, E, false);
+      __syncthreads();
+      float acc[4][4] = {};
+      bi_tile_mm<EP>(AT, AP, M, s0, o0, acc);
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const bool live = s0 + r < ns;
+        float v = 0.f;
+        if (live) {
+          const float* xj = a.x + (b0 + s0 + r) * a.ldx + j * E + o0;
+#pragma unroll
+          for (int c = 0; c < 4; ++c)
+            if (o0 + c < E) v = fmaf(acc[r][c], xj[c], v);
+        }
+#pragma unroll
+        for (int off = NOG / 2; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+        if (live && o0 == 0) a.out[(b0 + s0 + r) * a.ldo + a.col0 + p] = v;
+      }
+      __syncthreads();   // M is restaged for the next partner, AT for the next tile
+    }
+  }
+}
+
+template <int EP>
+__global__ void __launch_bounds__(kBiThreads) fefm_dx_kernel(const BiArgs a) {
+  constexpr int TS = bi_ts<EP>(), AP = bi_apitch<EP>(), NOG = EP / 4;
+  extern __shared__ __align__(16) float sm[];
+  float* AT = sm;
+  float* M = sm + EP * AP;
+  const int F = a.F, E = a.E, f = blockIdx.x;
+  const int o0 = (threadIdx.x % NOG) * 4, s0 = (threadIdx.x / NOG) * 4;
+  const int64_t ntiles = (a.batch + TS - 1) / TS;
+  for (int64_t t = blockIdx.y; t < ntiles; t += gridDim.y) {
+    const int64_t b0 = t * TS;
+    const int ns = (int)min((int64_t)TS, a.batch - b0);
+    float acc[4][4] = {};
+    for (int q = 0; q < F; ++q) {
+      if (q == f) continue;
+      const int p = q < f ? bi_pair_index(F, q, f) : bi_pair_index(F, f, q);
+      bi_stage_w<EP>(M, a.W + (int64_t)p * E * E, E, false);
+      for (int k = threadIdx.x; k < TS * EP; k += blockDim.x) {
+        const int s = k / EP, e = k - s * EP;
+        float v = 0.f;
+        if (s < ns && e < E) {
+          const int64_t b = b0 + s;
+          v = a.out[b * a.ldo + a.col0 + p] * a.x[b * a.ldx + q * E + e];
+        }
+        AT[e * AP + s] = v;
+      }
+      __syncthreads();
+      bi_tile_mm<EP>(AT, AP, M, s0, o0, acc);
+      __syncthreads();   // AT and M are restaged for the next partner
+    }
+    if (o0 < E) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        if (s0 + r >= ns) break;
+        float* d = a.dx + (b0 + s0 + r) * a.lddx + f * E + o0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (o0 + c < E) d[c] = acc[r][c];
+      }
+    }
+  }
+}
+
+// dW[p][e][o] = sum_c partial[c][p][e][o] + sum_c partial[c][p][o][e], chunks ascending
+__global__ void fefm_dw_reduce_kernel(const float* __restrict__ partial, int P, int E, int nchunk, float* dW,
+                                      int64_t count) {
+  const int ee = E * E;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < count; t += (int64_t)gridDim.x * blockDim.x) {
+    const int p = (int)(t / ee), q = (int)(t - (int64_t)p * ee), e = q / E, o = q - e * E;
+    float s = 0.f, st = 0.f;
+    for (int c = 0; c < nchunk; ++c) {
+      const float* part = partial + ((int64_t)c * P + p) * ee;
+      s += part[e * E + o];
+      st += part[o * E + e];
+    }
+    dW[t] = s + st;
+  }
+}
+
+struct FeFwd {
+  template <int EP>
+  static cudaError_t run(const BiArgs& a, cudaStream_t s) {
+    const size_t smem = sizeof(float) * bi_smem_floats<EP>();
+    fefm_fwd_kernel<EP><<<dim3(a.F - 1, bi_tile_grid(a.batch, bi_ts<EP>())), kBiThreads, smem, s>>>(a);
+    return cudaSuccess;
+  }
+};
+struct FeBwd {
+  template <int EP>
+  static cudaError_t run(const BiArgs& a, cudaStream_t s) {
+    if (a.dx) {
+      const size_t smem = sizeof(float) * bi_smem_floats<EP>();
+      fefm_dx_kernel<EP><<<dim3(a.F, bi_tile_grid(a.batch, bi_ts<EP>())), kBiThreads, smem, s>>>(a);
+      const cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) return e;
+    }
+    if (a.partial) {
+      const size_t smem = sizeof(float) * bi_dw_smem_floats<EP>();
+      bilinear_dw_kernel<EP, true><<<dim3(a.F * (a.F - 1) / 2, a.nchunk), kBiThreads, smem, s>>>(a);
+    }
+    return cudaSuccess;
+  }
+};
 
 }  // namespace b2ctr
 
@@ -1517,6 +1839,135 @@ b2ctr_status_t b2ctr_bilinear_bwd(const float* g, int64_t ldg, int64_t gcol0, in
     bilinear_dw_reduce_kernel<<<grid_for(count, 256, 8), 256, 0, ST>>>((const float*)workspace, nfield, dim, type,
                                                                      nchunk, dW, count);
     B2_CHECK_LAUNCH("b2ctr_bilinear_bwd(reduce)");
+  }
+  return B2CTR_OK;
+}
+
+#define FWFM_REQUIRE_SHAPE(what)                                                                       \
+  B2_REQUIRE(nfield >= 2 && nfield <= kFwMaxF && dim >= 1 && dim <= kFwMaxE,                            \
+             what ": needs 2 <= field count <= %d and 1 <= embedding_size <= %d (got %d, %d)", kFwMaxF, \
+             kFwMaxE, nfield, dim)
+
+b2ctr_status_t b2ctr_fwfm_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, const float* r, float* out,
+                              int64_t ldo, int64_t batch, void* stream) {
+  FWFM_REQUIRE_SHAPE("fwfm_fwd");
+  B2_REQUIRE(x && r && out, "fwfm_fwd: NULL pointer");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && ldo >= 1, "fwfm_fwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  // large F * E need more than the default 48 KB; the attribute belongs to the current device, so it is set per call
+  const cudaError_t err = cudaFuncSetAttribute(fwfm_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               (int)fw_fwd_smem(nfield, dim));
+  if (err != cudaSuccess) {
+    set_error("fwfm_fwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  fwfm_fwd_kernel<<<grid_for(batch, kFwWarps, 8), kFwWarps * 32, fw_fwd_smem(nfield, dim), ST>>>(
+      x, ldx, nfield, dim, r, out, ldo, batch);
+  B2_CHECK_LAUNCH("b2ctr_fwfm_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_fwfm_bwd_workspace_bytes(int32_t nfield, int64_t batch) {
+  if (nfield < 2 || batch <= 0) return 0;
+  return (size_t)fw_bwd_blocks(batch) * (size_t)(nfield * (nfield - 1) / 2) * sizeof(float);
+}
+
+b2ctr_status_t b2ctr_fwfm_bwd(const float* g, int64_t ldg, const float* x, int64_t ldx, int32_t nfield, int32_t dim,
+                              const float* r, float* dx, int64_t lddx, float* dR, int64_t batch, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+  FWFM_REQUIRE_SHAPE("fwfm_bwd");
+  B2_REQUIRE(g && x && r && (dx || dR), "fwfm_bwd: NULL pointer, or nothing to compute");
+  B2_REQUIRE(ldg >= 1 && ldx >= (int64_t)nfield * dim && (!dx || lddx >= (int64_t)nfield * dim),
+             "fwfm_bwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  const size_t need = dR ? b2ctr_fwfm_bwd_workspace_bytes(nfield, batch) : 0;
+  if (dR && (!workspace || workspace_bytes < need)) {
+    set_error("fwfm_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  const cudaError_t err = cudaFuncSetAttribute(fwfm_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               (int)fw_bwd_smem(nfield, dim));
+  if (err != cudaSuccess) {
+    set_error("fwfm_bwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  const int nb = fw_bwd_blocks(batch);
+  float* partial = dR ? (float*)workspace : nullptr;
+  fwfm_bwd_kernel<<<nb, kFwWarps * 32, fw_bwd_smem(nfield, dim), ST>>>(g, ldg, x, ldx, nfield, dim, r, dx, lddx,
+                                                                     partial, batch);
+  B2_CHECK_LAUNCH("b2ctr_fwfm_bwd");
+  if (dR) {
+    fwfm_dr_reduce_kernel<<<(unsigned)ceil_div((int64_t)nfield * nfield, 256), 256, 0, ST>>>(partial, nb, nfield, dR);
+    B2_CHECK_LAUNCH("b2ctr_fwfm_bwd(reduce)");
+  }
+  return B2CTR_OK;
+}
+
+#define FEFM_REQUIRE_SHAPE(what)                                                                       \
+  B2_REQUIRE(nfield >= 2 && nfield <= kFeMaxF && dim >= 1 && dim <= kFeMaxE,                            \
+             what ": needs 2 <= field count <= %d and 1 <= embedding_size <= %d (got %d, %d)", kFeMaxF, \
+             kFeMaxE, nfield, dim)
+
+b2ctr_status_t b2ctr_fefm_sym(const float* W, int32_t npairs, int32_t dim, float* S, void* stream) {
+  B2_REQUIRE(W && S && W != S, "fefm_sym: NULL or aliased pointer");
+  B2_REQUIRE(npairs >= 1 && dim >= 1 && dim <= kFeMaxE, "fefm_sym: needs npairs >= 1 and 1 <= dim <= %d (got %d, %d)",
+             kFeMaxE, npairs, dim);
+  const int64_t count = (int64_t)npairs * dim * dim;
+  fefm_sym_kernel<<<grid_for(count, 256, 8), 256, 0, ST>>>(W, dim, S, count);
+  B2_CHECK_LAUNCH("b2ctr_fefm_sym");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_fefm_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, const float* S, float* out,
+                              int64_t ldo, int64_t col0, int64_t batch, void* stream) {
+  FEFM_REQUIRE_SHAPE("fefm_fwd");
+  B2_REQUIRE(x && S && out, "fefm_fwd: NULL pointer");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim, "fefm_fwd: ldx too small");
+  B2_REQUIRE(col0 >= 0 && ldo >= col0 + nfield * (nfield - 1) / 2,
+             "fefm_fwd: the pair window (col0 %lld) does not fit a row of %lld", (long long)col0, (long long)ldo);
+  if (batch <= 0) return B2CTR_OK;
+  BiArgs a{x, ldx, nfield, dim, 2, S, out, ldo, col0, 1, nullptr, 0, nullptr, 0, batch};
+  const cudaError_t err = bi_dispatch<FeFwd>(bi_pad_e(dim), a, ST);
+  if (err != cudaSuccess) {
+    set_error("fefm_fwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_fefm_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_fefm_bwd_workspace_bytes(int32_t nfield, int32_t dim, int64_t batch) {
+  return b2ctr_bilinear_bwd_workspace_bytes(nfield, dim, batch);
+}
+
+b2ctr_status_t b2ctr_fefm_bwd(const float* g, int64_t ldg, int64_t gcol0, const float* x, int64_t ldx, int32_t nfield,
+                              int32_t dim, const float* S, float* dx, int64_t lddx, float* dW, int64_t batch,
+                              void* workspace, size_t workspace_bytes, void* stream) {
+  FEFM_REQUIRE_SHAPE("fefm_bwd");
+  B2_REQUIRE(g && x && S && (dx || dW), "fefm_bwd: NULL pointer, or nothing to compute");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && (!dx || lddx >= (int64_t)nfield * dim), "fefm_bwd: ld too small");
+  B2_REQUIRE(gcol0 >= 0 && ldg >= gcol0 + nfield * (nfield - 1) / 2,
+             "fefm_bwd: the pair window (col0 %lld) does not fit a row of %lld", (long long)gcol0, (long long)ldg);
+  if (batch <= 0) return B2CTR_OK;
+  const size_t need = dW ? b2ctr_fefm_bwd_workspace_bytes(nfield, dim, batch) : 0;
+  if (dW && (!workspace || workspace_bytes < need)) {
+    set_error("fefm_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  const int nchunk = bi_dw_chunks(nfield, batch);
+  BiArgs a{x, ldx, nfield, dim, 2, S, const_cast<float*>(g), ldg, gcol0, 1, dx, lddx,
+           dW ? (float*)workspace : nullptr, nchunk, batch};
+  const cudaError_t err = bi_dispatch<FeBwd>(bi_pad_e(dim), a, ST);
+  if (err != cudaSuccess) {
+    set_error("fefm_bwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_fefm_bwd");
+  if (dW) {
+    const int P = nfield * (nfield - 1) / 2;
+    const int64_t count = (int64_t)P * dim * dim;
+    fefm_dw_reduce_kernel<<<grid_for(count, 256, 8), 256, 0, ST>>>((const float*)workspace, P, dim, nchunk, dW, count);
+    B2_CHECK_LAUNCH("b2ctr_fefm_bwd(reduce)");
   }
   return B2CTR_OK;
 }

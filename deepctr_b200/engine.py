@@ -127,12 +127,13 @@ def contiguous(var):
 
 
 class _TapeNode(object):
-    __slots__ = ("outputs", "backward", "tag")
+    __slots__ = ("outputs", "backward", "tag", "keep")
 
-    def __init__(self, outputs, backward):
+    def __init__(self, outputs, backward, keep=False):
         self.outputs = outputs
         self.backward = backward
         self.tag = K.PROFILE_TAG       # bench attribution: the backward launches join the forward's group
+        self.keep = keep               # the outputs' gradients are only read: an earlier node consumes them
 
 
 class Tape(object):
@@ -142,8 +143,8 @@ class Tape(object):
         self.nodes = []
         self.ctx = {}
 
-    def record(self, outputs, backward):
-        self.nodes.append(_TapeNode(list(outputs), backward))
+    def record(self, outputs, backward, keep=False):
+        self.nodes.append(_TapeNode(list(outputs), backward, keep))
 
     def backward(self):
         _state.opt_ctx = self.ctx
@@ -157,8 +158,9 @@ class Tape(object):
                         node.backward(grads)
                 else:
                     node.backward(grads)
-                for o in node.outputs:
-                    o.grad = None   # free as we go
+                if not node.keep:
+                    for o in node.outputs:
+                        o.grad = None   # free as we go
         finally:
             _state.opt_ctx = None
         self.nodes = []
@@ -233,8 +235,10 @@ class recording(object):
         _state.tape = self.prev
 
 
-def record(outputs, inputs, backward):
-    """Register a backward closure if a tape is active and any input needs a gradient."""
+def record(outputs, inputs, backward, keep_grads=False):
+    """Register a backward closure if a tape is active and any input needs a gradient.  ``keep_grads``: the
+    closure only reads its outputs' gradients and leaves them for the node that produced those outputs (an op that
+    wrote its result into a window of another op's buffer, see ops.fefm)."""
     tape = current_tape()
     if tape is None:
         return False
@@ -242,7 +246,7 @@ def record(outputs, inputs, backward):
         return False
     for o in outputs:
         o.requires_grad = True
-    tape.record(outputs, backward)
+    tape.record(outputs, backward, keep_grads)
     return True
 
 

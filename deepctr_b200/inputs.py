@@ -349,7 +349,9 @@ class EmbeddingPlanner(object):
         for t in model.inputs:
             if t.dtype in ("float32", "float64", "float16") and len(t.shape) == 2:
                 self.tail_reserve += int(t.shape[1])
-        self.main_ld = (self.main_width + self.tail_reserve + 3) // 4 * 4
+        # DeepFEFM's FEFM scores go behind the dense columns (fefm_place): P more columns in the row pitch
+        self.fefm_places = _plan_fefm_input(model, consumers, out_ids)
+        self.main_ld = (self.main_width + self.tail_reserve + sum(self.fefm_places.values()) + 3) // 4 * 4
         self.lin_ld = max(1, (self.lin_width + 3) // 4 * 4)
         self.fast = self._fast_eligible()
         self.dnn_places = _plan_dnn_input(model, consumers, out_ids)
@@ -787,6 +789,21 @@ class EmbeddingPlanner(object):
         """(DnnInputPlacement, index) when ``layer`` writes its output into the first DNN layer's input."""
         return self.dnn_places.get(id(layer))
 
+    def fefm_place(self, layer, x):
+        """The [B, P] window of this step's main buffer, behind the dense columns, where the FEFMLayer ``layer``
+        writes its scores (ops.fefm ``out``), or None.  With the embeddings at [0, main_width) and
+        combined_dnn_input's dense columns behind them, DeepFEFM's concat([combined_dnn_input, scores]) is then the
+        zero-copy window [0, main_width + n_dense + P) of the buffer, the first Dense reads it in place and its data
+        gradient becomes the buffer's gradient, whose score columns the FEFM backward reads in place."""
+        from . import ops
+        P = self.fefm_places.get(id(layer))
+        base = x.base
+        if (P is None or base is None or base.owner is not self or base.data is None
+                or base.ncols != self.main_width or base.data.shape[1] != self.main_ld):
+            return None
+        b = base.data.shape[0]
+        return ops._window(base, self.main_width + self.tail_reserve, P, (b, P))
+
     def append_dense(self, emb_flat, dense_flat):
         """combined_dnn_input: place the dense features behind the embeddings in the main buffer so the
         DNN input is a zero-copy window.  Returns the window or None."""
@@ -886,9 +903,45 @@ class DnnInputPlacement(object):
         return ops._window(base, 0, self.width + nd, (b, self.width + nd))
 
 
-# FiBiNET's bilinear outputs written in place into the DNN input; False keeps every layer's own output buffer
-# (same results, used by the tests to compare the two)
+# FiBiNET's bilinear outputs and DeepFEFM's FEFM scores written in place into the DNN input; False keeps every
+# layer's own output buffer (same results, used by the tests to compare the two)
 DNN_INPUT_PLACEMENT = True
+
+
+def _plan_fefm_input(model, consumers, out_ids):
+    """{id(FEFMLayer): P} for DeepFEFM's DNN input concat([combined_dnn_input(...), NoMask(FEFM(x))], axis=1)
+    (deepctr/models/deepfefm.py:64-78) when that concatenation reaches only the DNN: the planner then reserves the
+    P score columns behind the dense tail of the main buffer (fefm_place).  Decided once from the model's graph;
+    every other graph plans nothing and keeps its row pitch."""
+    if not DNN_INPUT_PLACEMENT:
+        return {}
+    from .layers.core import DNN
+    from .layers.interaction import FEFMLayer
+    from .layers.utils import Concat, NoMask, _CombinedDNNInput
+    calls = defaultdict(int)
+    for node in model._order:
+        calls[id(node.layer)] += 1
+    places = {}
+    for node in model._order:
+        if not isinstance(node.layer, Concat) or node.layer.axis not in (1, -1):
+            continue
+        srcs = E._flatten(node.inputs)
+        if len(srcs) != 2 or len(srcs[0].shape) != 2 or len(srcs[1].shape) != 2:
+            continue
+        head, tail = srcs
+        if not isinstance(head.node.layer, (_CombinedDNNInput, E.Flatten)) or len(consumers[id(head)]) != 1:
+            continue
+        while isinstance(tail.node.layer, NoMask):                   # concat_func of the single FEFM output
+            tail = E._flatten(tail.node.inputs)[0]
+        fefm = tail.node.layer
+        if not isinstance(fefm, FEFMLayer) or calls[id(fefm)] != 1 or id(fefm) in places:
+            continue
+        out = node.outputs[0]
+        oc = consumers[id(out)]
+        if len(oc) != 1 or id(out) in out_ids or not isinstance(oc[0].layer, DNN):
+            continue
+        places[id(fefm)] = int(tail.shape[1])
+    return places
 
 
 def _plan_dnn_input(model, consumers, out_ids):

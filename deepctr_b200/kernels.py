@@ -710,6 +710,59 @@ def bilinear_bwd(g, ldg, gcol0, gpitch, x, ldx, nfield, dim, btype, W, batch, wa
     return dx, dW
 
 
+def fwfm_fwd(x, ldx, nfield, dim, r, batch):
+    """FwFMLayer on a [B, nfield*dim] window (pitch ldx) with the strengths r [nfield, nfield] -> [B, 1]."""
+    _require_cuda(x, r)
+    out = torch.empty((batch, 1), dtype=torch.float32, device=x.device)
+    _lib_call("fwfm_fwd", ptr(x), ldx, nfield, dim, ptr(r), ptr(out), 1, batch, stream())
+    return out
+
+
+def fwfm_bwd(g, ldg, x, ldx, nfield, dim, r, batch, want_dx=True, want_dr=True):
+    """-> (dx [B, nfield*dim] or None, dR [nfield, nfield] or None)."""
+    _require_cuda(g, x, r)
+    dev = x.device
+    dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=dev) if want_dx else None
+    dR = torch.empty((nfield, nfield), dtype=torch.float32, device=dev) if want_dr else None
+    nbytes = L.lib().b2ctr_fwfm_bwd_workspace_bytes(nfield, batch) if want_dr else 0
+    ws = workspace(nbytes, dev) if want_dr else None
+    _lib_call("fwfm_bwd", ptr(g), ldg, ptr(x), ldx, nfield, dim, ptr(r), ptr(dx), nfield * dim, ptr(dR), batch,
+              ptr(ws), nbytes, stream())
+    return dx, dR
+
+
+def fefm_sym(W):
+    """S_p = W_p + W_p^T for the stacked weights W [P, dim, dim]."""
+    _require_cuda(W)
+    S = torch.empty_like(W)
+    _lib_call("fefm_sym", ptr(W), W.shape[0], W.shape[1], ptr(S), stream())
+    return S
+
+
+def fefm_fwd(x, ldx, nfield, dim, S, batch, out=None, col0=0):
+    """FEFMLayer on a [B, nfield*dim] window (pitch ldx) with S from fefm_sym: pair p's score goes to column
+    col0 + p of ``out`` [B, ld] (default: a new [B, P])."""
+    _require_cuda(x, S, out)
+    if out is None:
+        out = torch.empty((batch, nfield * (nfield - 1) // 2), dtype=torch.float32, device=x.device)
+    _lib_call("fefm_fwd", ptr(x), ldx, nfield, dim, ptr(S), ptr(out), out.stride(0), col0, batch, stream())
+    return out
+
+
+def fefm_bwd(g, ldg, gcol0, x, ldx, nfield, dim, S, batch, want_dx=True, want_dw=True):
+    """g: the data pointer of the gradient buffer addressed like the forward's output -> (dx [B, nfield*dim] or
+    None, dW [P, dim, dim] or None)."""
+    _require_cuda(g, x, S)
+    dev = x.device
+    dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=dev) if want_dx else None
+    dW = torch.empty(tuple(S.shape), dtype=torch.float32, device=dev) if want_dw else None
+    nbytes = L.lib().b2ctr_fefm_bwd_workspace_bytes(nfield, dim, batch) if want_dw else 0
+    ws = workspace(nbytes, dev) if want_dw else None
+    _lib_call("fefm_bwd", ptr(g), ldg, gcol0, ptr(x), ldx, nfield, dim, ptr(S), ptr(dx), nfield * dim, ptr(dW), batch,
+              ptr(ws), nbytes, stream())
+    return dx, dW
+
+
 def din_att_input_fwd(q, ldq, keys, ldk, batch, T, E):
     out = torch.empty((batch, T, 4 * E), dtype=torch.float32, device=q.device)
     _lib_call("din_att_input_fwd", ptr(q), ldq, ptr(keys), ldk, ptr(out), batch, T, E, stream())
@@ -884,7 +937,8 @@ def layernorm_bwd(a, lda, b, ldb, gamma, stats, dy, rows, n, want_dgamma=True, w
 for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
            "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
-           "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "din_att_input_fwd", "din_att_input_bwd",
+           "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "fwfm_fwd", "fwfm_bwd", "fefm_sym",
+           "fefm_fwd", "fefm_bwd", "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
     globals()[_n] = _timed(globals()[_n])
@@ -937,7 +991,8 @@ for _n in ("shard_bucketize", "shard_fill", "shard_gather_rows", "shard_scatter_
 for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
            "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
-           "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "din_att_input_fwd", "din_att_input_bwd",
+           "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "fwfm_fwd", "fwfm_bwd", "fefm_sym",
+           "fefm_fwd", "fefm_bwd", "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "moving_update", "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
     globals()[_n] = _timed(globals()[_n])

@@ -3,7 +3,7 @@ from ..engine import Layer, Dense, Flatten, Concatenate, Add, Lambda, Input
 from .activation import Dice, Activation, activation_layer
 from .core import DNN, LocalActivationUnit, PredictionLayer
 from .interaction import (AFMLayer, BiInteractionPooling, BilinearInteraction, FM, CrossNet, CIN, InteractingLayer,
-                          SENETLayer)
+                          SENETLayer, FwFMLayer, FEFMLayer)
 from .normalization import BatchNormalization, Dropout, LayerNormalization
 from .sequence import (SequencePoolingLayer, WeightedSequenceLayer, AttentionSequencePoolingLayer, Transformer,
                        PositionEncoding)
@@ -14,6 +14,7 @@ custom_objects = {
     'DNN': DNN, 'PredictionLayer': PredictionLayer, 'LocalActivationUnit': LocalActivationUnit,
     'AFMLayer': AFMLayer, 'BiInteractionPooling': BiInteractionPooling,
     'SENETLayer': SENETLayer, 'BilinearInteraction': BilinearInteraction,
+    'FwFMLayer': FwFMLayer, 'FEFMLayer': FEFMLayer,
     'FM': FM, 'CrossNet': CrossNet, 'CIN': CIN, 'InteractingLayer': InteractingLayer,
     'SequencePoolingLayer': SequencePoolingLayer, 'WeightedSequenceLayer': WeightedSequenceLayer,
     'AttentionSequencePoolingLayer': AttentionSequencePoolingLayer, 'Dice': Dice, 'Hash': Hash,

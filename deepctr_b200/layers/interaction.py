@@ -1,6 +1,7 @@
 """Host mirror of deepctr/layers/interaction.py for the operators on the hot path:
 AFMLayer (:39-160), BiInteractionPooling (:163-206), FM (:563-607), CrossNet (:344-435), CIN (:209-341),
-InteractingLayer (:697-790), SENETLayer (:1067-1139), BilinearInteraction (:1142-1221).
+InteractingLayer (:697-790), SENETLayer (:1067-1139), BilinearInteraction (:1142-1221), FwFMLayer (:1350-1425),
+FEFMLayer (:1428-1499).
 Same constructor arguments, weight names, shape checks and error messages as the reference."""
 import itertools
 
@@ -15,8 +16,25 @@ from .normalization import Dropout
 AFM_MAX_FIELDS, AFM_MAX_EMBEDDING, AFM_MAX_FACTOR = 64, 32, 16
 # shapes the SENET / bilinear kernels serve (include/b2ctr.h, b2ctr_senet_fwd, b2ctr_bilinear_fwd)
 SENET_MAX_FIELDS, BILINEAR_MAX_FIELDS, BILINEAR_MAX_EMBEDDING = 64, 64, 64
+# shapes the FwFM / FEFM kernels serve (include/b2ctr.h, b2ctr_fwfm_fwd, b2ctr_fefm_fwd)
+FWFM_MAX_FIELDS, FWFM_MAX_EMBEDDING = 64, 64
+FEFM_MAX_FIELDS, FEFM_MAX_EMBEDDING = 64, 64
 # shapes the InteractingLayer attention kernels serve (include/b2ctr.h, b2ctr_interacting_fwd / _bwd)
 INTERACTING_MAX_FIELDS, INTERACTING_MAX_ATT_EMBEDDING, INTERACTING_MAX_FHD = 64, 32, 3072
+
+
+def _weights_stacked(layer, ws):
+    """(ws, stack): the weights' device data as views of one [n, E, E] buffer ``layer._stack``, rebuilt when a
+    weight's data is no longer its view (first call, set_value, loading).  The weights stay separate weights for
+    set_value, loading by name and the optimizers; the kernels take the stack."""
+    st = layer._stack
+    if st is None or ws[0].data is None or ws[0].data.data_ptr() != st.data_ptr() or ws[-1].data is None \
+            or ws[-1].data.data_ptr() != st[-1].data_ptr():
+        st = torch.stack([w.materialize() for w in ws])
+        for k, w in enumerate(ws):
+            w.data = st[k]
+        layer._stack = st
+    return ws, st
 
 
 class AFMLayer(Layer):
@@ -389,25 +407,13 @@ class BilinearInteraction(Layer):
             raise NotImplementedError
         self.built = True
 
-    def _weights_stacked(self):
-        """The weights' device data as views of one [nW, E, E] buffer (built on the first call)."""
-        ws = [self.W] if self.bilinear_type == "all" else self.W_list
-        st = self._stack
-        if st is None or ws[0].data is None or ws[0].data.data_ptr() != st.data_ptr() or ws[-1].data is None \
-                or ws[-1].data.data_ptr() != st[-1].data_ptr():
-            st = torch.stack([w.materialize() for w in ws])
-            for k, w in enumerate(ws):
-                w.data = st[k]
-            self._stack = st
-        return ws, st
-
     def call(self, inputs, **kwargs):
         if inputs[0].data.dim() != 3:
             raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs[0].data.dim()))
         if self.bilinear_type not in ("all", "each", "interaction"):
             raise NotImplementedError
         x = ops.concat(inputs, axis=1)
-        ws, st = self._weights_stacked()
+        ws, st = _weights_stacked(self, [self.W] if self.bilinear_type == "all" else self.W_list)
         planner = getattr(self, "_planner", None)
         place = planner.dnn_input_place(self) if planner is not None else None
         if place is None:
@@ -428,3 +434,98 @@ class BilinearInteraction(Layer):
         base = Layer.get_config(self)
         base.update(config)
         return base
+
+
+class FwFMLayer(Layer):
+    """Field-weighted FM, deepctr/layers/interaction.py:1350-1425.  Called on a [B, F, E] tensor; output [B, 1] =
+    sum_{i<j} r[i, j] <x_i, x_j> with the [F, F] field_pair_strengths r, of which only the upper triangle is read
+    (b2ctr_fwfm_fwd / _bwd: the input is read in place; the gradient of r is 0 on and below the diagonal)."""
+
+    def __init__(self, num_fields=4, regularizer=0.000001, **kwargs):
+        self.num_fields = num_fields
+        self.regularizer = regularizer
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        if len(input_shape) != 3:
+            raise ValueError("Unexpected inputs dimensions % d,                             expect to be 3 dimensions"
+                             % (len(input_shape)))
+        if input_shape[1] != self.num_fields:
+            raise ValueError("Mismatch in number of fields {} and                  concatenated embeddings dims {}"
+                             .format(self.num_fields, input_shape[1]))
+        embedding_size = int(input_shape[2])
+        if not 2 <= self.num_fields <= FWFM_MAX_FIELDS or not 1 <= embedding_size <= FWFM_MAX_EMBEDDING:
+            raise ValueError("FwFMLayer supports 2 to %d fields and embedding_size 1 to %d "
+                             "(got %d fields, embedding_size %d)"
+                             % (FWFM_MAX_FIELDS, FWFM_MAX_EMBEDDING, self.num_fields, embedding_size))
+        self.field_strengths = self.add_weight(name='field_pair_strengths', shape=(self.num_fields, self.num_fields),
+                                               initializer=TruncatedNormal(), regularizer=l2(self.regularizer),
+                                               trainable=True)
+        self.built = True
+
+    def call(self, inputs, **kwargs):
+        if inputs.data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs.data.dim()))
+        if inputs.data.shape[1] != self.num_fields:
+            raise ValueError("Mismatch in number of fields {} and                  concatenated embeddings dims {}"
+                             .format(self.num_fields, inputs.data.shape[1]))
+        return ops.fwfm(inputs, self.field_strengths)
+
+    def compute_output_shape(self, input_shape):
+        return (None, 1)
+
+    def get_config(self):
+        config = Layer.get_config(self).copy()
+        config.update({'num_fields': self.num_fields, 'regularizer': self.regularizer})
+        return config
+
+
+class FEFMLayer(Layer):
+    """Field-embedded FM, deepctr/layers/interaction.py:1428-1499.  Called on a [B, F, E] tensor; output [B, P] with
+    column p = (i < j) equal to x_i (W_p + W_p^T) x_j^T.  The P weights field_embeddings{i}-{j} keep the reference's
+    names and order but their data are views of one stacked [P, E, E] buffer, which is what b2ctr_fefm_sym / _fwd /
+    _bwd take.  In DeepFEFM the scores are written straight into the first DNN layer's input
+    (inputs.EmbeddingPlanner.fefm_place)."""
+
+    def __init__(self, regularizer, **kwargs):
+        self.regularizer = regularizer
+        self._stack = None
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        if len(input_shape) != 3:
+            raise ValueError("Unexpected inputs dimensions % d,                                expect to be 3 "
+                             "dimensions" % (len(input_shape)))
+        self.num_fields = int(input_shape[1])
+        embedding_size = int(input_shape[2])
+        if not 2 <= self.num_fields <= FEFM_MAX_FIELDS or not 1 <= embedding_size <= FEFM_MAX_EMBEDDING:
+            raise ValueError("FEFMLayer supports 2 to %d fields and embedding_size 1 to %d "
+                             "(got %d fields, embedding_size %d)"
+                             % (FEFM_MAX_FIELDS, FEFM_MAX_EMBEDDING, self.num_fields, embedding_size))
+        self.field_embeddings = {}
+        for fi, fj in itertools.combinations(range(self.num_fields), 2):
+            field_pair_id = str(fi) + "-" + str(fj)
+            self.field_embeddings[field_pair_id] = self.add_weight(name='field_embeddings' + field_pair_id,
+                                                                   shape=(embedding_size, embedding_size),
+                                                                   initializer=TruncatedNormal(),
+                                                                   regularizer=l2(self.regularizer),
+                                                                   trainable=True)
+        self.built = True
+
+    def call(self, inputs, **kwargs):
+        if inputs.data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs.data.dim()))
+        ws, st = _weights_stacked(self, list(self.field_embeddings.values()))
+        planner = getattr(self, "_planner", None)
+        out = planner.fefm_place(self, inputs) if planner is not None else None
+        return ops.fefm(inputs, ws, st, out=out)
+
+    def compute_output_shape(self, input_shape):
+        # the reference divides with `/` (a float); the graph here needs the integer column count
+        num_fields = int(input_shape[1])
+        return (None, (num_fields * (num_fields - 1)) // 2)
+
+    def get_config(self):
+        config = Layer.get_config(self).copy()
+        config.update({'regularizer': self.regularizer})
+        return config

@@ -6,5 +6,7 @@ from .sequence import DIN, BST
 from .nfm import NFM
 from .afm import AFM
 from .fibinet import FiBiNET
+from .fwfm import FwFM
+from .deepfefm import DeepFEFM
 
-__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST"]
+__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM"]

@@ -514,6 +514,71 @@ def bilinear_interaction(x, weights, stack, btype, out=None):
     return res
 
 
+def fwfm(x, r):
+    """[B,F,E] -> [B,1]: sum_{i<j} r[i,j] <x_i, x_j> over the upper triangle of r [F,F] (FwFMLayer,
+    layers/interaction.py:1403-1411).  x is read in place; the gradient of r is 0 on and below the diagonal."""
+    b, f, e = x.data.shape
+    src, ld = _fields2d(x)
+    rd = _wdata(r)
+    res = E.Var(K.fwfm_fwd(src, ld, f, e, rd, b))
+
+    def bwd(grads):
+        if not (x.requires_grad or r.requires_grad):
+            return
+        g = grads[0].reshape(b, 1)
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dx, dr = K.fwfm_bwd(g, g.stride(0), src, ld, f, e, rd, b, want_dx=x.requires_grad, want_dr=r.requires_grad)
+        if dx is not None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        if dr is not None:
+            E.add_grad(r, dr)
+
+    E.record([res], [x, r], bwd)
+    return res
+
+
+def fefm(x, weights, stack, out=None):
+    """[B,F,E] -> [B,P]: x_i (W_p + W_p^T) x_j^T for the pairs p = (i < j) (FEFMLayer, layers/interaction.py:1481-1491).
+    ``stack`` [P,E,E] holds the data of ``weights`` (each weight's data is a view of it); the symmetric S_p are
+    built once per call and the gradient comes back as one stacked buffer handed to each weight as a view.
+    x is read in place; no per-pair [B,E] product is written.
+
+    ``out``: a [B,P] column window (``_window``) of a wider buffer Var to write the scores into (DeepFEFM's DNN
+    input behind the gather buffer's dense columns, inputs.EmbeddingPlanner.fefm_place); it is returned.  Every
+    consumer's gradient then lands in that buffer's gradient, so the backward is keyed on the buffer: it reads the
+    score columns of its gradient in place and leaves the gradient to the buffer's own backward (the gather's
+    scatter), which runs after it.  Default: a new [B,P] tensor."""
+    b, f, e = x.data.shape
+    src, ld = _fields2d(x)
+    S = K.fefm_sym(stack)
+    if out is None:
+        res = E.Var(K.fefm_fwd(src, ld, f, e, S, b))
+        key, gcol0 = res, 0
+    else:
+        key, gcol0 = out.base, out.col0
+        K.fefm_fwd(src, ld, f, e, S, b, out=key.data, col0=gcol0)
+        res = out
+
+    def bwd(grads):
+        g = grads[0]
+        if g.dim() != 2 or g.stride(1) != 1 or g.stride(0) < g.shape[1]:
+            g = g.contiguous().reshape(b, -1)
+        want_dw = any(w.requires_grad for w in weights)
+        if not (x.requires_grad or want_dw):
+            return
+        dx, dw = K.fefm_bwd(g, g.stride(0), gcol0, src, ld, f, e, S, b, want_dx=x.requires_grad, want_dw=want_dw)
+        if dx is not None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        for k, w in enumerate(weights):
+            if w.requires_grad:
+                E.add_grad(w, dw[k])
+
+    if E.record([key], [x] + list(weights), bwd, keep_grads=out is not None):
+        res.requires_grad = True
+    return res
+
+
 def add_bias(x, b, scale=1.0, per_sample=False):
     """x + scale * b over the last axis for a per-column (or scalar, when the last axis is 1) bias:
     Linear(use_bias=True) without a dense part, layers/utils.py:172-173.  ``per_sample``: b spans every non-batch

@@ -509,6 +509,41 @@ B2CTR_API b2ctr_status_t b2ctr_bilinear_bwd(const float* g, int64_t ldg, int64_t
                                            const float* W, float* dx, int64_t lddx, float* dW, int64_t batch,
                                            void* workspace, size_t workspace_bytes, void* stream);
 
+/* FwFMLayer (deepctr/layers/interaction.py:1350-1425) on x [B, nfield, dim] (row pitch ldx) and the field-pair
+ * strengths r [nfield, nfield], of which only the upper triangle i < j is read:
+ *   out[b*ldo] = sum_{i<j} r[i][j] <x_i, x_j>
+ * Limits: 2 <= nfield <= 64, 1 <= dim <= 64; anything else is B2CTR_ERR_INVALID_ARG. */
+B2CTR_API b2ctr_status_t b2ctr_fwfm_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, const float* r,
+                                       float* out, int64_t ldo, int64_t batch, void* stream);
+/* Backward from g [B, 1] (pitch ldg):
+ *   dx_i = g * sum_{j != i} r[min(i,j)][max(i,j)] x_j   (pitch lddx, overwritten; may be NULL)
+ *   dR [nfield, nfield] (overwritten; may be NULL): sum_b g_b <x_i, x_j> for i < j, exactly 0 elsewhere.
+ * Every dx element has one owner that adds its partners in ascending order; dR goes through per-CTA partials in
+ * the workspace, summed in CTA order.  No float atomics: bit-identical from run to run. */
+B2CTR_API size_t b2ctr_fwfm_bwd_workspace_bytes(int32_t nfield, int64_t batch);
+B2CTR_API b2ctr_status_t b2ctr_fwfm_bwd(const float* g, int64_t ldg, const float* x, int64_t ldx, int32_t nfield,
+                                       int32_t dim, const float* r, float* dx, int64_t lddx, float* dR, int64_t batch,
+                                       void* workspace, size_t workspace_bytes, void* stream);
+
+/* FEFMLayer (deepctr/layers/interaction.py:1428-1499).  b2ctr_fefm_sym builds S_p = W_p + W_p^T for the npairs
+ * stacked [dim, dim] weights W (S must not alias W); the forward and backward take S.  For the
+ * P = nfield(nfield-1)/2 pairs p = (i < j) in itertools.combinations order, on x [B, nfield, dim] (row pitch ldx):
+ *   out[b*ldo + col0 + p] = x_i S_p x_j^T
+ * so the scores can be a window of a wider buffer (the first DNN layer's input); nothing else is written.
+ * Limits: 2 <= nfield <= 64, 1 <= dim <= 64. */
+B2CTR_API b2ctr_status_t b2ctr_fefm_sym(const float* W, int32_t npairs, int32_t dim, float* S, void* stream);
+B2CTR_API b2ctr_status_t b2ctr_fefm_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, const float* S,
+                                       float* out, int64_t ldo, int64_t col0, int64_t batch, void* stream);
+/* Backward from g[b*ldg + gcol0 + p], read in place:
+ *   dx_f = sum_{q != f} g_p(f,q) x_q S_p   (pitch lddx, overwritten; may be NULL)
+ *   dW_p = dS_p + dS_p^T with dS_p = sum_b g_p x_i^T x_j   ([P, dim, dim], overwritten; may be NULL)
+ * Every dx element has one owner that adds its partners in ascending order; dW goes through per-(pair, batch chunk)
+ * partials in the workspace, reduced in a fixed order.  No float atomics: bit-identical from run to run. */
+B2CTR_API size_t b2ctr_fefm_bwd_workspace_bytes(int32_t nfield, int32_t dim, int64_t batch);
+B2CTR_API b2ctr_status_t b2ctr_fefm_bwd(const float* g, int64_t ldg, int64_t gcol0, const float* x, int64_t ldx,
+                                       int32_t nfield, int32_t dim, const float* S, float* dx, int64_t lddx, float* dW,
+                                       int64_t batch, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* 6. Sequence operators (DIN, pooling, Dice / BatchNormalization, dropout)                     */
 /* ------------------------------------------------------------------------------------------ */

@@ -4,6 +4,7 @@ FiBiNET also get the 13 dense features, AFM takes none: its builder refuses Dens
 that shape.
 
     python tools/pairwise_bench.py [--steps 20] [--warmup 5] [--reps 50] [--models NFM,AFM,FiBiNET]
+    python tools/pairwise_bench.py --models FwFM,DeepFEFM
 
 Prints one JSON line per measurement:
   * the hardware context (card, power limit, max SM clock), read in the same run;
@@ -13,7 +14,9 @@ Prints one JSON line per measurement:
     median over --reps launches, with the FFMA bound (132 SMs x 128 FP32 lanes x 2 flop x max SM clock) and the HBM
     bound (3.35 TB/s, H100 SXM data sheet) of the flops and bytes their shapes imply;
   * FiBiNET's first DNN layer alone: the split of its [65536, 20816] operand into bf16 planes and the three
-    20813 -> 256 GEMMs (forward, data gradient, weight gradient), so the step can be broken down.
+    20813 -> 256 GEMMs (forward, data gradient, weight gradient), so the step can be broken down;
+  * with FwFM / DeepFEFM (not in the default set): b2ctr_fwfm_* and b2ctr_fefm_* against the same two bounds, and the
+    training steps of FwFM and DeepFEFM with their default (256, 128, 64) DNN.
 """
 import argparse
 import json
@@ -56,6 +59,10 @@ def step_time(builder, steps, warmup):
     E.clear_session()
     if builder == "NFM":
         model = M.NFM(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding=0)
+    elif builder == "FwFM":
+        model = M.FwFM(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding=0)
+    elif builder == "DeepFEFM":
+        model = M.DeepFEFM(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding_feat=0)
     elif builder == "FiBiNET":
         model = M.FiBiNET(cols, cols, bilinear_type="interaction", dnn_hidden_units=(256, 128, 64), l2_reg_linear=0,
                           l2_reg_embedding=0)
@@ -216,6 +223,46 @@ def fibinet_kernels(reps, hw):
     return out
 
 
+def fefm_kernels(reps, hw):
+    """FwFM and FEFM at C2 (26 fields, E = 32, B = 65536), x a window of the [B, 848] gather buffer and FEFM's scores
+    written at column 845 of a [B, 1172] buffer, as DeepFEFM's DNN input holds them."""
+    import torch
+    from deepctr_b200 import kernels as K
+    B, F, E, nd = 65536, 26, 32, 13
+    P = F * (F - 1) // 2
+    dev = torch.device("cuda", 0)
+    g = torch.Generator(device=dev).manual_seed(3)
+    clk = hw.get("max_sm_clock_mhz") or None
+    ffma_peak = 132 * 128 * 2 * clk * 1e6 if clk else None
+    ldx = (F * E + nd + 3) // 4 * 4
+    buf = torch.randn((B, ldx), device=dev, generator=g) * 0.1
+    xw = buf[:, :F * E]
+    x_bytes = B * F * E * 4
+    shape = dict(B=B, F=F, E=E, P=P, ldx=ldx)
+    r = torch.randn((F, F), device=dev, generator=g) * 0.3
+    gl = torch.randn((B, 1), device=dev, generator=g)
+    # FwFM: 2E flop per pair; the backward recomputes the dots for dR (2E per pair) and forms dx (2E per pair, twice)
+    out = [_report("fwfm_fwd", shape, reps, lambda: K.fwfm_fwd(xw, ldx, F, E, r, B), B * P * 2 * E,
+                   x_bytes + B * 4, ffma_peak),
+           _report("fwfm_bwd", shape, reps, lambda: K.fwfm_bwd(gl, 1, xw, ldx, F, E, r, B), B * P * 6 * E,
+                   2 * x_bytes + B * 4, ffma_peak)]
+    W = torch.randn((P, E, E), device=dev, generator=g) / E ** 0.5
+    S = K.fefm_sym(W)
+    ld, col0 = (F * E + nd + P + 3) // 4 * 4, F * E + nd
+    dnn_in = torch.randn((B, ld), device=dev, generator=g) * 0.1       # also the scores' gradient
+    shape = dict(shape, ld_out=ld, col0=col0)
+    w_bytes = P * E * E * 4
+    out.append(_report("fefm_sym", dict(P=P, E=E), reps, lambda: K.fefm_sym(W), P * E * E, 3 * w_bytes, ffma_peak))
+    # forward: x_i S_p 2E^2 + the dot 2E per pair; backward: dx 2 x (2E^2 + E), dS 2E^2 + E per pair
+    out.append(_report("fefm_fwd", shape, reps, lambda: K.fefm_fwd(xw, ldx, F, E, S, B, out=dnn_in, col0=col0),
+                       B * P * (2 * E * E + 2 * E), x_bytes + w_bytes + B * P * 4, ffma_peak))
+    out.append(_report("fefm_bwd", shape, reps, lambda: K.fefm_bwd(dnn_in, ld, col0, xw, ldx, F, E, S, B),
+                       B * P * (6 * E * E + 3 * E), 2 * x_bytes + 2 * w_bytes + B * P * 4, ffma_peak))
+    del buf, dnn_in, W, S
+    torch.cuda.empty_cache()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -234,6 +281,9 @@ def main():
             print(json.dumps(r), flush=True)
     if "FiBiNET" in models:
         for r in fibinet_kernels(args.reps, hw):
+            print(json.dumps(r), flush=True)
+    if "FwFM" in models or "DeepFEFM" in models:
+        for r in fefm_kernels(args.reps, hw):
             print(json.dumps(r), flush=True)
     for builder in models:
         print(json.dumps(step_time(builder, args.steps, args.warmup)), flush=True)
