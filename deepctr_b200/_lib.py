@@ -179,6 +179,13 @@ SIGNATURES = {
     "b2ctr_fefm_fwd": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _vp]),
     "b2ctr_fefm_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
     "b2ctr_fefm_bwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _sz, _vp]),
+    "b2ctr_pnn_inner_fwd": (_i32, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "b2ctr_pnn_inner_bwd_workspace_bytes": (_sz, [_i32, _i32, _i32, _i64]),
+    "b2ctr_pnn_inner_bwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _sz,
+                                   _vp]),
+    "b2ctr_pnn_outer_fwd": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _vp]),
+    "b2ctr_pnn_outer_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
+    "b2ctr_pnn_outer_bwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _sz, _vp]),
     "b2ctr_din_att_input_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),
     "b2ctr_din_att_input_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _vp]),
     "b2ctr_din_pool_fwd": (_i32, [_vp, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),

@@ -4,6 +4,7 @@
 // :277-325 (CIN), :754-779 (InteractingLayer), :1113-1126 (SENETLayer), :1190-1209 (BilinearInteraction).  Pairwise reductions use warp shuffles; the dense
 // contractions (CIN feature-map contraction, Q/K/V projections, CrossNet-matrix) go through b2ctr_gemm.
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -914,13 +915,17 @@ __device__ __forceinline__ void bi_pair_of(int F, int p, int& i, int& j) {
   j = i + 1 + p - off;
 }
 
-// M[r][c] = W[r][c] (or W[c][r] when trans), zero outside [E, E]
+// M[r][c] = W[r][c] (or W[c][r] when trans) for a matrix of row stride ld, zero outside [E, E]
 template <int EP>
-__device__ __forceinline__ void bi_stage_w(float* M, const float* __restrict__ W, int E, bool trans) {
+__device__ __forceinline__ void bi_stage_w(float* M, const float* __restrict__ W, int E, bool trans, int64_t ld) {
   for (int k = threadIdx.x; k < EP * EP; k += blockDim.x) {
     const int r = k / EP, c = k - r * EP;
-    M[k] = (r < E && c < E) ? (trans ? W[c * E + r] : W[r * E + c]) : 0.f;
+    M[k] = (r < E && c < E) ? (trans ? W[c * ld + r] : W[r * ld + c]) : 0.f;
   }
+}
+template <int EP>
+__device__ __forceinline__ void bi_stage_w(float* M, const float* __restrict__ W, int E, bool trans) {
+  bi_stage_w<EP>(M, W, E, trans, (int64_t)E);
 }
 
 // acc[r][c] += sum_k AT[k][s0 + r] * M[k][o0 + c]
@@ -1364,9 +1369,22 @@ __global__ void fwfm_dr_reduce_kernel(const float* __restrict__ partial, int n, 
 //   partners are accumulated into the same registers in ascending order: one owner per (b, f, e), no atomics.
 // * dS: bilinear_dw_kernel<EP, true> partials per (pair, batch chunk); fefm_dw_reduce_kernel adds the chunks in
 //   ascending order, for both dS_p and its transpose.
+// kPnn: OutterProductLayer(kernel_type='mat') (deepctr/layers/interaction.py:881-911) on the same tiles.  Its score
+// is out_p = sum_{k,l} x_j[k] K[k][p][l] x_i[l] = x_i M_p x_j^T with M_p[l][k] = K[k][p][l], not symmetric: M_p is
+// staged transposed straight from the reference's [E, P, E] kernel (row stride P*E), and the dx kernel stages
+// M_p^T for the first field of a pair (dx_i = g x_j M_p^T) and M_p for the second (dx_j = g x_i M_p).
 // ------------------------------------------------------------------------------------------------
 constexpr int kFeMaxF = 64;
 constexpr int kFeMaxE = 64;
+
+// M = M_p (FEFM: S_p, [P][E][E]; kPnn: K[:, p, :]^T, or K[:, p, :] when trans)
+template <int EP, bool kPnn>
+__device__ __forceinline__ void fe_stage_m(float* M, const float* __restrict__ W, int F, int E, int p, bool trans) {
+  if (kPnn)
+    bi_stage_w<EP>(M, W + (int64_t)p * E, E, !trans, (int64_t)(F * (F - 1) / 2) * E);
+  else
+    bi_stage_w<EP>(M, W + (int64_t)p * E * E, E, false);
+}
 
 __global__ void fefm_sym_kernel(const float* __restrict__ W, int E, float* S, int64_t count) {
   const int ee = E * E;
@@ -1377,7 +1395,7 @@ __global__ void fefm_sym_kernel(const float* __restrict__ W, int E, float* S, in
   }
 }
 
-template <int EP>
+template <int EP, bool kPnn = false>
 __global__ void __launch_bounds__(kBiThreads) fefm_fwd_kernel(const BiArgs a) {
   constexpr int TS = bi_ts<EP>(), AP = bi_apitch<EP>(), NOG = EP / 4;
   extern __shared__ __align__(16) float sm[];
@@ -1395,7 +1413,7 @@ __global__ void __launch_bounds__(kBiThreads) fefm_fwd_kernel(const BiArgs a) {
     }
     for (int j = i + 1; j < F; ++j) {
       const int p = bi_pair_index(F, i, j);
-      bi_stage_w<EP>(M, a.W + (int64_t)p * E * E, E, false);
+      fe_stage_m<EP, kPnn>(M, a.W, F, E, p, false);
       __syncthreads();
       float acc[4][4] = {};
       bi_tile_mm<EP>(AT, AP, M, s0, o0, acc);
@@ -1418,7 +1436,7 @@ __global__ void __launch_bounds__(kBiThreads) fefm_fwd_kernel(const BiArgs a) {
   }
 }
 
-template <int EP>
+template <int EP, bool kPnn = false>
 __global__ void __launch_bounds__(kBiThreads) fefm_dx_kernel(const BiArgs a) {
   constexpr int TS = bi_ts<EP>(), AP = bi_apitch<EP>(), NOG = EP / 4;
   extern __shared__ __align__(16) float sm[];
@@ -1434,7 +1452,7 @@ __global__ void __launch_bounds__(kBiThreads) fefm_dx_kernel(const BiArgs a) {
     for (int q = 0; q < F; ++q) {
       if (q == f) continue;
       const int p = q < f ? bi_pair_index(F, q, f) : bi_pair_index(F, f, q);
-      bi_stage_w<EP>(M, a.W + (int64_t)p * E * E, E, false);
+      fe_stage_m<EP, kPnn>(M, a.W, F, E, p, q > f);
       for (int k = threadIdx.x; k < TS * EP; k += blockDim.x) {
         const int s = k / EP, e = k - s * EP;
         float v = 0.f;
@@ -1477,20 +1495,35 @@ __global__ void fefm_dw_reduce_kernel(const float* __restrict__ partial, int P, 
   }
 }
 
+// pnn mat: dK[k][p][l] = sum_c partial[c][p][l][k] (bilinear_dw_kernel's x_i^T (g_p x_j)), chunks ascending; no
+// transposed second term as FEFM has
+__global__ void pnn_mat_dk_reduce_kernel(const float* __restrict__ partial, int P, int E, int nchunk, float* dK,
+                                         int64_t count) {
+  const int ee = E * E, pe = P * E;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < count; t += (int64_t)gridDim.x * blockDim.x) {
+    const int k = (int)(t / pe), q = (int)(t - (int64_t)k * pe), p = q / E, l = q - p * E;
+    float s = 0.f;
+    for (int c = 0; c < nchunk; ++c) s += partial[((int64_t)c * P + p) * ee + l * E + k];
+    dK[t] = s;
+  }
+}
+
+template <bool kPnn>
 struct FeFwd {
   template <int EP>
   static cudaError_t run(const BiArgs& a, cudaStream_t s) {
     const size_t smem = sizeof(float) * bi_smem_floats<EP>();
-    fefm_fwd_kernel<EP><<<dim3(a.F - 1, bi_tile_grid(a.batch, bi_ts<EP>())), kBiThreads, smem, s>>>(a);
+    fefm_fwd_kernel<EP, kPnn><<<dim3(a.F - 1, bi_tile_grid(a.batch, bi_ts<EP>())), kBiThreads, smem, s>>>(a);
     return cudaSuccess;
   }
 };
+template <bool kPnn>
 struct FeBwd {
   template <int EP>
   static cudaError_t run(const BiArgs& a, cudaStream_t s) {
     if (a.dx) {
       const size_t smem = sizeof(float) * bi_smem_floats<EP>();
-      fefm_dx_kernel<EP><<<dim3(a.F, bi_tile_grid(a.batch, bi_ts<EP>())), kBiThreads, smem, s>>>(a);
+      fefm_dx_kernel<EP, kPnn><<<dim3(a.F, bi_tile_grid(a.batch, bi_ts<EP>())), kBiThreads, smem, s>>>(a);
       const cudaError_t e = cudaGetLastError();
       if (e != cudaSuccess) return e;
     }
@@ -1501,6 +1534,215 @@ struct FeBwd {
     return cudaSuccess;
   }
 };
+
+// ------------------------------------------------------------------------------------------------
+// PNN's InnerProductLayer (deepctr/layers/interaction.py:655-678) and OutterProductLayer(kernel_type 'vec' / 'num')
+// (:912-919).  For the P pairs p = (i < j) in itertools.combinations order, on x [B, F, E] read in place:
+//   B2CTR_PNN_INNER        out[b*ldo + col0 + p]         = <x_i, x_j>
+//   B2CTR_PNN_ELEMENTWISE  out[b*ldo + col0 + p*E + e]   = x_i[e] x_j[e]          (reduce_sum=False)
+//   B2CTR_PNN_VEC          out[b*ldo + col0 + p]         = sum_e x_i[e] x_j[e] K[p][e]
+//   B2CTR_PNN_NUM          out[b*ldo + col0 + p]         = K[p] <x_i, x_j>
+// Both kernels are instantiated per mode.
+// * pnn_inner_fwd_kernel: one warp per sample, its [F, E] staged in shared memory (row pitch E+1, so the lanes'
+//   consecutive partners j hit distinct banks while the shared x_i is a broadcast); lane p owns pair p (or, for
+//   the elementwise form, the flattened (p, e)) and writes it, so the row is stored coalesced.  'vec' stages K
+//   once per CTA (pitch E+1) when it fits (kPnStageKMax).
+// * pnn_inner_dx_kernel: one warp per sample, sample and pair gradient staged; lane (f, e) adds its F-1 partners
+//   in ascending order, the pair index stepped rather than recomputed: dx_f[e] = sum_{q != f} g_p w_p[e] x_q[e].
+//   One owner per element, no atomics.
+// * pnn_inner_dk_kernel (vec / num): CTA (tile of kPnDkPer * 256 kernel entries, batch chunk); each thread keeps
+//   its entries' sums over the chunk in registers and writes them as a partial, and ordered_sum_kernel adds the
+//   chunks in ascending order.  Bit-identical from run to run.
+// ------------------------------------------------------------------------------------------------
+constexpr int kPnWarps = 8;
+constexpr int kPnMaxF = 64;
+constexpr int kPnMaxE = 64;
+constexpr int kPnDkPer = 8;
+
+// 'vec' forward: the kernel K [P, E] is staged once per CTA in shared memory (row pitch E+1: lane p reads row p
+// conflict-free) when it takes at most this many floats; larger kernels are read through L1
+constexpr int kPnStageKMax = 16384;
+
+static inline bool pn_stage_k(int F, int E, int mode) {
+  return mode == B2CTR_PNN_VEC && (int64_t)F * (F - 1) / 2 * (E + 1) <= kPnStageKMax;
+}
+static inline size_t pn_fwd_smem(int F, int E, int mode) {
+  const size_t P = (size_t)F * (F - 1) / 2;
+  return sizeof(int) * P + sizeof(float) * ((pn_stage_k(F, E, mode) ? P * (E + 1) : 0) +
+                                            (size_t)kPnWarps * F * (E + 1));
+}
+static inline size_t pn_dx_smem(int F, int E) {
+  return sizeof(float) * (size_t)kPnWarps * (F * (E + 1) + F * (F - 1) / 2);
+}
+
+// pairs[p] = (i << 8) | j, for the CTA
+__device__ __forceinline__ void pn_stage_pairs(int* pairs, int F) {
+  for (int i = 0, k = 0; i < F; ++i)
+    for (int j = i + 1; j < F; ++j, ++k)
+      if (k % blockDim.x == threadIdx.x) pairs[k] = (i << 8) | j;
+}
+
+template <int kMode>
+__global__ void __launch_bounds__(kPnWarps * 32)
+    pnn_inner_fwd_kernel(const float* __restrict__ x, int64_t ldx, int F, int E, const float* __restrict__ K,
+                         bool stage_k, float* out, int64_t ldo, int64_t col0, int64_t batch) {
+  extern __shared__ __align__(16) float sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, XP = E + 1, P = F * (F - 1) / 2;
+  int* pairs = reinterpret_cast<int*>(sm);
+  float* sk = sm + P;                                          // [P][XP] when stage_k
+  float* sx = sk + (stage_k ? P * XP : 0) + warp * F * XP;
+  pn_stage_pairs(pairs, F);
+  if (kMode == B2CTR_PNN_VEC && stage_k)
+    for (int k = threadIdx.x; k < P * E; k += blockDim.x) {
+      const int p = k / E;
+      sk[p * XP + (k - p * E)] = K[k];
+    }
+  __syncthreads();
+  const int64_t nw = (int64_t)gridDim.x * kPnWarps;
+  for (int64_t b = (int64_t)blockIdx.x * kPnWarps + warp; b < batch; b += nw) {
+    fw_stage_x(sx, x + b * ldx, F, E, lane);
+    __syncwarp();
+    float* o = out + b * ldo + col0;
+    if (kMode == B2CTR_PNN_ELEMENTWISE) {
+      for (int k = lane; k < P * E; k += 32) {
+        const int p = k / E, e = k - p * E, i = pairs[p] >> 8, j = pairs[p] & 255;
+        o[k] = sx[i * XP + e] * sx[j * XP + e];
+      }
+    } else {
+      for (int p = lane; p < P; p += 32) {
+        const float* xi = sx + (pairs[p] >> 8) * XP;
+        const float* xj = sx + (pairs[p] & 255) * XP;
+        float acc = 0.f;
+        if (kMode == B2CTR_PNN_VEC) {
+          if (stage_k) {
+            const float* kp = sk + p * XP;
+            for (int e = 0; e < E; ++e) acc = fmaf(xi[e] * xj[e], kp[e], acc);
+          } else {
+            const float* kp = K + (int64_t)p * E;
+            for (int e = 0; e < E; ++e) acc = fmaf(xi[e] * xj[e], __ldg(kp + e), acc);
+          }
+        } else {
+          for (int e = 0; e < E; ++e) acc = fmaf(xi[e], xj[e], acc);
+          if (kMode == B2CTR_PNN_NUM) acc *= __ldg(K + p);
+        }
+        o[p] = acc;
+      }
+    }
+    __syncwarp();   // sx is restaged for the next sample
+  }
+}
+
+// w_p[e] * x_q[e] for pair p, partner q
+template <int kMode>
+__device__ __forceinline__ float pn_dx_term(const float* gb, const float* sg, const float* __restrict__ K,
+                                            const float* sx, int XP, int E, int p, int q, int e, float acc) {
+  float w;
+  if (kMode == B2CTR_PNN_ELEMENTWISE)
+    w = gb[(int64_t)p * E + e];
+  else if (kMode == B2CTR_PNN_VEC)
+    w = sg[p] * __ldg(K + (int64_t)p * E + e);
+  else
+    w = sg[p];
+  return fmaf(w, sx[q * XP + e], acc);
+}
+
+// launch bounds with a minimum of 4 CTAs per SM: without it ptxas spills the 'vec' instantiation
+template <int kMode>
+__global__ void __launch_bounds__(kPnWarps * 32, 4)
+    pnn_inner_dx_kernel(const float* __restrict__ g, int64_t ldg, int64_t gcol0, const float* __restrict__ x,
+                        int64_t ldx, int F, int E, const float* __restrict__ K, float* dx, int64_t lddx,
+                        int64_t batch) {
+  extern __shared__ __align__(16) float sm[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, XP = E + 1, P = F * (F - 1) / 2;
+  float* sx = sm + warp * (F * XP + P);
+  float* sg = sx + F * XP;                                     // [P]: g_p (times K[p] for num)
+  const int64_t nw = (int64_t)gridDim.x * kPnWarps;
+  for (int64_t b = (int64_t)blockIdx.x * kPnWarps + warp; b < batch; b += nw) {
+    fw_stage_x(sx, x + b * ldx, F, E, lane);
+    const float* gb = g + b * ldg + gcol0;
+    if (kMode != B2CTR_PNN_ELEMENTWISE)
+      for (int p = lane; p < P; p += 32) sg[p] = kMode == B2CTR_PNN_NUM ? gb[p] * __ldg(K + p) : gb[p];
+    __syncwarp();
+    float* d = dx + b * lddx;
+    for (int k = lane; k < F * E; k += 32) {
+      const int f = k / E, e = k - f * E;
+      float acc = 0.f;
+      // partners ascending: q < f in pairs (q, f), p(q+1, f) = p(q, f) + F - q - 2; then q > f in pairs (f, q),
+      // consecutive from p(f, f+1)
+      int p = f - 1;
+      for (int q = 0; q < f; ++q) {
+        acc = pn_dx_term<kMode>(gb, sg, K, sx, XP, E, p, q, e, acc);
+        p += F - q - 2;
+      }
+      p = bi_pair_index(F, f, f + 1);
+      for (int q = f + 1; q < F; ++q, ++p) acc = pn_dx_term<kMode>(gb, sg, K, sx, XP, E, p, q, e, acc);
+      d[k] = acc;
+    }
+    __syncwarp();   // sx / sg are restaged for the next sample
+  }
+}
+
+template <class Op>
+cudaError_t pn_dispatch(int mode, Op op) {
+  switch (mode) {
+    case B2CTR_PNN_INNER: return op(std::integral_constant<int, B2CTR_PNN_INNER>());
+    case B2CTR_PNN_ELEMENTWISE: return op(std::integral_constant<int, B2CTR_PNN_ELEMENTWISE>());
+    case B2CTR_PNN_VEC: return op(std::integral_constant<int, B2CTR_PNN_VEC>());
+    default: return op(std::integral_constant<int, B2CTR_PNN_NUM>());
+  }
+}
+
+// vec: entry n = p*E + e, sum_b g_p x_i[e] x_j[e];  num: entry n = p, sum_b g_p <x_i, x_j>
+__global__ void __launch_bounds__(256)
+    pnn_inner_dk_kernel(const float* __restrict__ g, int64_t ldg, int64_t gcol0, const float* __restrict__ x,
+                        int64_t ldx, int F, int E, int vec, float* partial, int nent, int nchunk, int64_t batch) {
+  const int c = blockIdx.y;
+  const int64_t per = (batch + nchunk - 1) / nchunk;
+  const int64_t lo = (int64_t)c * per, hi = min(batch, lo + per);
+  int pp[kPnDkPer], xi[kPnDkPer], xj[kPnDkPer];
+  float acc[kPnDkPer];
+#pragma unroll
+  for (int m = 0; m < kPnDkPer; ++m) {
+    const int n = blockIdx.x * (kPnDkPer * 256) + m * 256 + threadIdx.x;
+    const int p = n < nent ? (vec ? n / E : n) : 0, e = vec && n < nent ? n - p * E : 0;
+    int i, j;
+    bi_pair_of(F, p, i, j);
+    pp[m] = n < nent ? p : -1;
+    xi[m] = i * E + e;
+    xj[m] = j * E + e;
+    acc[m] = 0.f;
+  }
+  for (int64_t b = lo; b < hi; ++b) {
+    const float* xb = x + b * ldx;
+    const float* gb = g + b * ldg + gcol0;
+#pragma unroll
+    for (int m = 0; m < kPnDkPer; ++m) {
+      if (pp[m] < 0) continue;
+      float t;
+      if (vec) {
+        t = xb[xi[m]] * xb[xj[m]];
+      } else {
+        t = 0.f;
+        for (int e = 0; e < E; ++e) t = fmaf(xb[xi[m] + e], xb[xj[m] + e], t);
+      }
+      acc[m] = fmaf(gb[pp[m]], t, acc[m]);
+    }
+  }
+#pragma unroll
+  for (int m = 0; m < kPnDkPer; ++m)
+    if (pp[m] >= 0) partial[(int64_t)c * nent + blockIdx.x * (kPnDkPer * 256) + m * 256 + threadIdx.x] = acc[m];
+}
+
+static inline int pn_dk_entries(int F, int E, int mode) {
+  const int P = F * (F - 1) / 2;
+  return mode == B2CTR_PNN_VEC ? P * E : mode == B2CTR_PNN_NUM ? P : 0;
+}
+static inline int pn_dk_tiles(int nent) { return (int)ceil_div((int64_t)nent, kPnDkPer * 256); }
+// batch chunks of the kernel-gradient pass: about 8 CTAs per SM over all entry tiles, at least 64 samples a chunk
+static inline int pn_dk_chunks(int nent, int64_t batch) {
+  const int64_t want = ceil_div((int64_t)kNumSMs * 8, pn_dk_tiles(nent));
+  return (int)std::max<int64_t>(1, std::min(want, ceil_div(batch, 64)));
+}
 
 }  // namespace b2ctr
 
@@ -1927,7 +2169,7 @@ b2ctr_status_t b2ctr_fefm_fwd(const float* x, int64_t ldx, int32_t nfield, int32
              "fefm_fwd: the pair window (col0 %lld) does not fit a row of %lld", (long long)col0, (long long)ldo);
   if (batch <= 0) return B2CTR_OK;
   BiArgs a{x, ldx, nfield, dim, 2, S, out, ldo, col0, 1, nullptr, 0, nullptr, 0, batch};
-  const cudaError_t err = bi_dispatch<FeFwd>(bi_pad_e(dim), a, ST);
+  const cudaError_t err = bi_dispatch<FeFwd<false>>(bi_pad_e(dim), a, ST);
   if (err != cudaSuccess) {
     set_error("fefm_fwd: %s", cudaGetErrorString(err));
     return B2CTR_ERR_CUDA;
@@ -1957,7 +2199,7 @@ b2ctr_status_t b2ctr_fefm_bwd(const float* g, int64_t ldg, int64_t gcol0, const 
   const int nchunk = bi_dw_chunks(nfield, batch);
   BiArgs a{x, ldx, nfield, dim, 2, S, const_cast<float*>(g), ldg, gcol0, 1, dx, lddx,
            dW ? (float*)workspace : nullptr, nchunk, batch};
-  const cudaError_t err = bi_dispatch<FeBwd>(bi_pad_e(dim), a, ST);
+  const cudaError_t err = bi_dispatch<FeBwd<false>>(bi_pad_e(dim), a, ST);
   if (err != cudaSuccess) {
     set_error("fefm_bwd: %s", cudaGetErrorString(err));
     return B2CTR_ERR_CUDA;
@@ -1968,6 +2210,159 @@ b2ctr_status_t b2ctr_fefm_bwd(const float* g, int64_t ldg, int64_t gcol0, const 
     const int64_t count = (int64_t)P * dim * dim;
     fefm_dw_reduce_kernel<<<grid_for(count, 256, 8), 256, 0, ST>>>((const float*)workspace, P, dim, nchunk, dW, count);
     B2_CHECK_LAUNCH("b2ctr_fefm_bwd(reduce)");
+  }
+  return B2CTR_OK;
+}
+
+#define PNN_REQUIRE_SHAPE(what)                                                                        \
+  B2_REQUIRE(nfield >= 2 && nfield <= kPnMaxF && dim >= 1 && dim <= kPnMaxE,                             \
+             what ": needs 2 <= field count <= %d and 1 <= embedding_size <= %d (got %d, %d)", kPnMaxF, \
+             kPnMaxE, nfield, dim)
+
+static inline int64_t pn_out_cols(int nfield, int dim, int mode) {
+  const int64_t P = (int64_t)nfield * (nfield - 1) / 2;
+  return mode == B2CTR_PNN_ELEMENTWISE ? P * dim : P;
+}
+
+b2ctr_status_t b2ctr_pnn_inner_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t mode,
+                                   const float* K, float* out, int64_t ldo, int64_t col0, int64_t batch,
+                                   void* stream) {
+  PNN_REQUIRE_SHAPE("pnn_inner_fwd");
+  B2_REQUIRE(mode >= B2CTR_PNN_INNER && mode <= B2CTR_PNN_NUM, "pnn_inner_fwd: unknown mode %d", mode);
+  B2_REQUIRE(x && out && (K || mode == B2CTR_PNN_INNER || mode == B2CTR_PNN_ELEMENTWISE),
+             "pnn_inner_fwd: NULL pointer");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim, "pnn_inner_fwd: ldx too small");
+  B2_REQUIRE(col0 >= 0 && ldo >= col0 + pn_out_cols(nfield, dim, mode),
+             "pnn_inner_fwd: the pair window (col0 %lld) does not fit a row of %lld", (long long)col0,
+             (long long)ldo);
+  if (batch <= 0) return B2CTR_OK;
+  const size_t smem = pn_fwd_smem(nfield, dim, mode);
+  const bool stage_k = pn_stage_k(nfield, dim, mode);
+  // large F * E need more than the default 48 KB; the attribute belongs to the current device, so it is set per call
+  const cudaError_t err = pn_dispatch(mode, [&](auto m) {
+    constexpr int kMode = decltype(m)::value;
+    const cudaError_t e = cudaFuncSetAttribute(pnn_inner_fwd_kernel<kMode>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    pnn_inner_fwd_kernel<kMode><<<grid_for(batch, kPnWarps, 8), kPnWarps * 32, smem, ST>>>(
+        x, ldx, nfield, dim, K, stage_k, out, ldo, col0, batch);
+    return cudaSuccess;
+  });
+  if (err != cudaSuccess) {
+    set_error("pnn_inner_fwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_pnn_inner_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_pnn_inner_bwd_workspace_bytes(int32_t nfield, int32_t dim, int32_t mode, int64_t batch) {
+  if (nfield < 2 || dim < 1 || batch <= 0) return 0;
+  const int nent = pn_dk_entries(nfield, dim, mode);
+  if (nent == 0) return 0;
+  return (size_t)pn_dk_chunks(nent, batch) * (size_t)nent * sizeof(float);
+}
+
+b2ctr_status_t b2ctr_pnn_inner_bwd(const float* g, int64_t ldg, int64_t gcol0, const float* x, int64_t ldx,
+                                   int32_t nfield, int32_t dim, int32_t mode, const float* K, float* dx,
+                                   int64_t lddx, float* dK, int64_t batch, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+  PNN_REQUIRE_SHAPE("pnn_inner_bwd");
+  B2_REQUIRE(mode >= B2CTR_PNN_INNER && mode <= B2CTR_PNN_NUM, "pnn_inner_bwd: unknown mode %d", mode);
+  const bool weighted = mode == B2CTR_PNN_VEC || mode == B2CTR_PNN_NUM;
+  B2_REQUIRE(g && x && (K || !weighted) && (dx || dK), "pnn_inner_bwd: NULL pointer, or nothing to compute");
+  B2_REQUIRE(!dK || weighted, "pnn_inner_bwd: mode %d has no kernel weight", mode);
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && (!dx || lddx >= (int64_t)nfield * dim), "pnn_inner_bwd: ld too small");
+  B2_REQUIRE(gcol0 >= 0 && ldg >= gcol0 + pn_out_cols(nfield, dim, mode),
+             "pnn_inner_bwd: the pair window (col0 %lld) does not fit a row of %lld", (long long)gcol0,
+             (long long)ldg);
+  if (batch <= 0) return B2CTR_OK;
+  const size_t need = dK ? b2ctr_pnn_inner_bwd_workspace_bytes(nfield, dim, mode, batch) : 0;
+  if (dK && (!workspace || workspace_bytes < need)) {
+    set_error("pnn_inner_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  if (dx) {
+    const size_t smem = pn_dx_smem(nfield, dim);
+    const cudaError_t err = pn_dispatch(mode, [&](auto m) {
+      constexpr int kMode = decltype(m)::value;
+      const cudaError_t e = cudaFuncSetAttribute(pnn_inner_dx_kernel<kMode>,
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e != cudaSuccess) return e;
+      pnn_inner_dx_kernel<kMode><<<grid_for(batch, kPnWarps, 8), kPnWarps * 32, smem, ST>>>(
+          g, ldg, gcol0, x, ldx, nfield, dim, K, dx, lddx, batch);
+      return cudaSuccess;
+    });
+    if (err != cudaSuccess) {
+      set_error("pnn_inner_bwd: %s", cudaGetErrorString(err));
+      return B2CTR_ERR_CUDA;
+    }
+    B2_CHECK_LAUNCH("b2ctr_pnn_inner_bwd(dx)");
+  }
+  if (dK) {
+    const int nent = pn_dk_entries(nfield, dim, mode), nchunk = pn_dk_chunks(nent, batch);
+    float* partial = (float*)workspace;
+    pnn_inner_dk_kernel<<<dim3(pn_dk_tiles(nent), nchunk), 256, 0, ST>>>(
+        g, ldg, gcol0, x, ldx, nfield, dim, mode == B2CTR_PNN_VEC, partial, nent, nchunk, batch);
+    B2_CHECK_LAUNCH("b2ctr_pnn_inner_bwd(dK)");
+    ordered_sum_kernel<<<grid_for(nent, 256, 8), 256, 0, ST>>>(partial, nent, nchunk, nent, dK);
+    B2_CHECK_LAUNCH("b2ctr_pnn_inner_bwd(reduce)");
+  }
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_pnn_outer_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, const float* K,
+                                   float* out, int64_t ldo, int64_t col0, int64_t batch, void* stream) {
+  PNN_REQUIRE_SHAPE("pnn_outer_fwd");
+  B2_REQUIRE(x && K && out, "pnn_outer_fwd: NULL pointer");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim, "pnn_outer_fwd: ldx too small");
+  B2_REQUIRE(col0 >= 0 && ldo >= col0 + nfield * (nfield - 1) / 2,
+             "pnn_outer_fwd: the pair window (col0 %lld) does not fit a row of %lld", (long long)col0, (long long)ldo);
+  if (batch <= 0) return B2CTR_OK;
+  BiArgs a{x, ldx, nfield, dim, 2, K, out, ldo, col0, 1, nullptr, 0, nullptr, 0, batch};
+  const cudaError_t err = bi_dispatch<FeFwd<true>>(bi_pad_e(dim), a, ST);
+  if (err != cudaSuccess) {
+    set_error("pnn_outer_fwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_pnn_outer_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_pnn_outer_bwd_workspace_bytes(int32_t nfield, int32_t dim, int64_t batch) {
+  return b2ctr_bilinear_bwd_workspace_bytes(nfield, dim, batch);
+}
+
+b2ctr_status_t b2ctr_pnn_outer_bwd(const float* g, int64_t ldg, int64_t gcol0, const float* x, int64_t ldx,
+                                   int32_t nfield, int32_t dim, const float* K, float* dx, int64_t lddx, float* dK,
+                                   int64_t batch, void* workspace, size_t workspace_bytes, void* stream) {
+  PNN_REQUIRE_SHAPE("pnn_outer_bwd");
+  B2_REQUIRE(g && x && K && (dx || dK), "pnn_outer_bwd: NULL pointer, or nothing to compute");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && (!dx || lddx >= (int64_t)nfield * dim), "pnn_outer_bwd: ld too small");
+  B2_REQUIRE(gcol0 >= 0 && ldg >= gcol0 + nfield * (nfield - 1) / 2,
+             "pnn_outer_bwd: the pair window (col0 %lld) does not fit a row of %lld", (long long)gcol0,
+             (long long)ldg);
+  if (batch <= 0) return B2CTR_OK;
+  const size_t need = dK ? b2ctr_pnn_outer_bwd_workspace_bytes(nfield, dim, batch) : 0;
+  if (dK && (!workspace || workspace_bytes < need)) {
+    set_error("pnn_outer_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  const int nchunk = bi_dw_chunks(nfield, batch);
+  BiArgs a{x, ldx, nfield, dim, 2, K, const_cast<float*>(g), ldg, gcol0, 1, dx, lddx,
+           dK ? (float*)workspace : nullptr, nchunk, batch};
+  const cudaError_t err = bi_dispatch<FeBwd<true>>(bi_pad_e(dim), a, ST);
+  if (err != cudaSuccess) {
+    set_error("pnn_outer_bwd: %s", cudaGetErrorString(err));
+    return B2CTR_ERR_CUDA;
+  }
+  B2_CHECK_LAUNCH("b2ctr_pnn_outer_bwd");
+  if (dK) {
+    const int P = nfield * (nfield - 1) / 2;
+    const int64_t count = (int64_t)P * dim * dim;
+    pnn_mat_dk_reduce_kernel<<<grid_for(count, 256, 8), 256, 0, ST>>>((const float*)workspace, P, dim, nchunk, dK,
+                                                                      count);
+    B2_CHECK_LAUNCH("b2ctr_pnn_outer_bwd(reduce)");
   }
   return B2CTR_OK;
 }

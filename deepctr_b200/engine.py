@@ -738,6 +738,43 @@ class Flatten(Layer):
         return (input_shape[0], n)
 
 
+class Reshape(Layer):
+    """Keras' Reshape(target_shape): the per-sample shape becomes ``target_shape`` (one entry may be -1).  A window
+    of a wider buffer stays a zero-copy view of it (PNN's linear_signal over the gather buffer)."""
+
+    def __init__(self, target_shape, **kwargs):
+        Layer.__init__(self, **kwargs)
+        self.target_shape = tuple(target_shape)
+
+    def _resolve(self, input_shape):
+        n = 1
+        for s in input_shape[1:]:
+            n *= s
+        known = 1
+        for s in self.target_shape:
+            if s != -1:
+                known *= s
+        shape = tuple(n // known if s == -1 else s for s in self.target_shape)
+        total = 1
+        for s in shape:
+            total *= s
+        if total != n or list(self.target_shape).count(-1) > 1:
+            raise ValueError("total size of new array must be unchanged, input_shape = %s, output_shape = %s"
+                             % (list(input_shape[1:]), list(self.target_shape)))
+        return shape
+
+    def call(self, inputs, **kwargs):
+        return ops.reshape(inputs, (None,) + self._resolve(tuple(inputs.data.shape)))
+
+    def compute_output_shape(self, input_shape):
+        return (input_shape[0],) + self._resolve(tuple(input_shape))
+
+    def get_config(self):
+        c = Layer.get_config(self)
+        c.update(target_shape=self.target_shape)
+        return c
+
+
 class Concatenate(Layer):
     def __init__(self, axis=-1, **kwargs):
         Layer.__init__(self, **kwargs)

@@ -351,7 +351,11 @@ class EmbeddingPlanner(object):
                 self.tail_reserve += int(t.shape[1])
         # DeepFEFM's FEFM scores go behind the dense columns (fefm_place): P more columns in the row pitch
         self.fefm_places = _plan_fefm_input(model, consumers, out_ids)
-        self.main_ld = (self.main_width + self.tail_reserve + sum(self.fefm_places.values()) + 3) // 4 * 4
+        # PNN's inner / outer products go between the embeddings and the dense columns (pnn_place): P per product
+        # more columns in the row pitch
+        self.pnn_places, self.pnn_cols = _plan_pnn_input(model, consumers, out_ids)
+        self.main_ld = (self.main_width + self.tail_reserve + sum(self.fefm_places.values()) + self.pnn_cols
+                        + 3) // 4 * 4
         self.lin_ld = max(1, (self.lin_width + 3) // 4 * 4)
         self.fast = self._fast_eligible()
         self.dnn_places = _plan_dnn_input(model, consumers, out_ids)
@@ -560,7 +564,7 @@ class EmbeddingPlanner(object):
                 lin_tabs = [s.emb.embeddings.materialize().reshape(-1) for s in self.lin] if lin_fused else None
             only_fast = len(self.main) == self.fast_n
             dense = None
-            if only_fast and self.tail_hint is not None and "__dense_pack__" in feed:
+            if only_fast and self.tail_hint is not None and "__dense_pack__" in feed and not self.pnn_cols:
                 c0, nd = self.tail_hint
                 dp = feed["__dense_pack__"].data
                 if c0 + nd <= dp.shape[1] and self.main_width + nd <= self.main_ld:
@@ -576,7 +580,10 @@ class EmbeddingPlanner(object):
                     for f in range(c0 // d, (c0 + nc) // d):
                         fm_mask |= 1 << f
             plan = K.UniformPlan(feats, lin_tabs, dense, x, linear, fm, fm_mask)
-            plan.g.x_cols = self.main_ld if only_fast else self.fast_n * fast_slots[0].dim
+            # with PNN's products placed, the gather's zero padding stops at the embeddings: the product columns
+            # behind them are written by the product kernels, the dense columns by append_dense
+            plan.g.x_cols = (self.main_ld if only_fast and not self.pnn_cols
+                             else self.fast_n * fast_slots[0].dim)
             if peer is not None:
                 plan.set_peers(self.dist.world, peer[0].table, peer[1].table if peer[1] is not None else None)
             K.embed_gather_uniform_fwd(plan, batch)
@@ -804,9 +811,27 @@ class EmbeddingPlanner(object):
         b = base.data.shape[0]
         return ops._window(base, self.main_width + self.tail_reserve, P, (b, P))
 
+    def pnn_place(self, layer, x):
+        """The [B, P] window of this step's main buffer where PNN's InnerProductLayer / OutterProductLayer ``layer``
+        writes its scores (ops.pnn_inner / ops.pnn_outer ``out``), or None.  ``x`` must be the embeddings' window
+        [0, main_width): the products then follow it in the order of PNN's concat([linear_signal, inner, outer]),
+        so that concatenation is a zero-copy window, combined_dnn_input copies only the dense columns behind it
+        (append_dense) and the first Dense reads the buffer in place.  Its data gradient becomes the buffer's
+        gradient, whose product columns the product backwards read in place."""
+        from . import ops
+        rel = self.pnn_places.get(id(layer))
+        base = x.base
+        if (rel is None or base is None or base.owner is not self or base.data is None or x.ncols == -1
+                or x.col0 != 0 or x.ncols != self.main_width or base.ncols != self.main_width
+                or base.data.shape[1] != self.main_ld):
+            return None
+        b, f, _ = x.data.shape
+        P = f * (f - 1) // 2
+        return ops._window(base, self.main_width + rel, P, (b, P))
+
     def append_dense(self, emb_flat, dense_flat):
-        """combined_dnn_input: place the dense features behind the embeddings in the main buffer so the
-        DNN input is a zero-copy window.  Returns the window or None."""
+        """combined_dnn_input: place the dense features behind the embeddings (and PNN's placed products) in the
+        main buffer so the DNN input is a zero-copy window.  Returns the window or None."""
         from . import ops
         if emb_flat.base is not None and isinstance(emb_flat.base.owner, DnnInputPlacement):
             return emb_flat.base.owner.append_dense(emb_flat, dense_flat)
@@ -814,13 +839,21 @@ class EmbeddingPlanner(object):
                 or emb_flat.base.ncols != self.main_width or emb_flat.base.data is None
                 or emb_flat.base.data.shape[1] != self.main_ld):
             return None
-        if emb_flat.col0 != 0 or emb_flat.ncols != self.main_width:
+        width = self.main_width + self.pnn_cols if self.pnn_cols else self.main_width
+        if emb_flat.col0 != 0 or emb_flat.ncols != width:
             return None
         b = emb_flat.data.shape[0]
         nd = dense_flat.data.shape[1]
-        if self.main_width + nd > self.main_ld:
+        if width + nd > self.main_ld:
             return None
         base = emb_flat.base
+        if self.pnn_cols:
+            # the fused gather would write its dense tail at main_width, over the products: always copy
+            src, ld = dense_flat.flat2d()
+            if src is None:
+                return None
+            K.copy2d(src, ld, base.data, base.data.stride(0), b, nd, dst_off=width)
+            return ops._window(base, 0, width + nd, (b, width + nd))
         is_pack = (dense_flat.base is not None and dense_flat.base.name == "__dense_pack__"
                    and dense_flat.ncols != -1)
         if is_pack and self.tail_done == (dense_flat.col0, nd):
@@ -903,8 +936,8 @@ class DnnInputPlacement(object):
         return ops._window(base, 0, self.width + nd, (b, self.width + nd))
 
 
-# FiBiNET's bilinear outputs and DeepFEFM's FEFM scores written in place into the DNN input; False keeps every
-# layer's own output buffer (same results, used by the tests to compare the two)
+# FiBiNET's bilinear outputs, DeepFEFM's FEFM scores and PNN's products written in place into the DNN input; False
+# keeps every layer's own output buffer (same results, used by the tests to compare the two)
 DNN_INPUT_PLACEMENT = True
 
 
@@ -942,6 +975,69 @@ def _plan_fefm_input(model, consumers, out_ids):
             continue
         places[id(fefm)] = int(tail.shape[1])
     return places
+
+
+def _plan_pnn_input(model, consumers, out_ids):
+    """({id(product layer): column offset behind the embeddings}, total product columns) for PNN's DNN input
+    concat([linear_signal, Flatten(InnerProductLayer(...)), OutterProductLayer(...)]) (deepctr/models/pnn.py:46-63,
+    either product or both) when that concatenation reaches the first DNN layer only through combined_dnn_input:
+    the planner then reserves the product columns between the embeddings and the dense columns of the main buffer
+    (pnn_place).  Decided once from the model's graph; every other graph plans nothing and keeps its row pitch."""
+    if not DNN_INPUT_PLACEMENT:
+        return {}, 0
+    from .layers.core import DNN
+    from .layers.interaction import InnerProductLayer, OutterProductLayer
+    from .layers.utils import Concat, NoMask, _CombinedDNNInput
+    calls = defaultdict(int)
+    for node in model._order:
+        calls[id(node.layer)] += 1
+
+    def only_use(t):
+        return len(consumers[id(t)]) == 1 and id(t) not in out_ids
+
+    for node in model._order:
+        if not isinstance(node.layer, Concat) or node.layer.axis not in (1, -1):
+            continue
+        srcs = E._flatten(node.inputs)
+        if not 2 <= len(srcs) <= 3 or any(len(t.shape) != 2 or not only_use(t) for t in srcs):
+            continue
+        if not isinstance(srcs[0].node.layer, E.Reshape):
+            continue
+        products = []
+        for t in srcs[1:]:
+            layer = t.node.layer
+            if isinstance(layer, E.Flatten):                          # Flatten(InnerProductLayer()(...))
+                inner = E._flatten(t.node.inputs)[0]
+                layer = inner.node.layer
+                if not (isinstance(layer, InnerProductLayer) and layer.reduce_sum and only_use(inner)):
+                    break
+            elif not isinstance(layer, OutterProductLayer):
+                break
+            if calls[id(layer)] != 1:
+                break
+            products.append((layer, int(t.shape[1])))
+        if len(products) != len(srcs) - 1 or len(set(id(l) for l, _ in products)) != len(products):
+            continue
+        # combined_dnn_input: NoMask + Flatten of the single deep input, then _CombinedDNNInput with the dense
+        # features or the DNN directly
+        flat = node.outputs[0]
+        while only_use(flat) and isinstance(consumers[id(flat)][0].layer, (NoMask, E.Flatten)):
+            flat = consumers[id(flat)][0].outputs[0]
+        if not only_use(flat):
+            continue
+        nxt = consumers[id(flat)][0]
+        if isinstance(nxt.layer, _CombinedDNNInput):
+            if E._flatten(nxt.inputs)[0] is not flat or not only_use(nxt.outputs[0]):
+                continue
+            nxt = consumers[id(nxt.outputs[0])][0]
+        if not isinstance(nxt.layer, DNN):
+            continue
+        places, col = {}, 0
+        for layer, w in products:
+            places[id(layer)] = col
+            col += w
+        return places, col
+    return {}, 0
 
 
 def _plan_dnn_input(model, consumers, out_ids):

@@ -763,6 +763,61 @@ def fefm_bwd(g, ldg, gcol0, x, ldx, nfield, dim, S, batch, want_dx=True, want_dw
     return dx, dW
 
 
+PNN_MODES = {"inner": 0, "elementwise": 1, "vec": 2, "num": 3}   # b2ctr.h B2CTR_PNN_*
+
+
+def pnn_inner_fwd(x, ldx, nfield, dim, mode, Kw, batch, out=None, col0=0):
+    """InnerProductLayer / OutterProductLayer('vec' | 'num') on a [B, nfield*dim] window (pitch ldx); ``mode`` a
+    PNN_MODES key, ``Kw`` the kernel (None for 'inner' / 'elementwise').  The pair scores (P*dim products for
+    'elementwise') go to columns col0.. of ``out`` [B, ld] (default: a new [B, P] or [B, P*dim])."""
+    _require_cuda(x, Kw, out)
+    m = PNN_MODES[mode]
+    if out is None:
+        P = nfield * (nfield - 1) // 2
+        out = torch.empty((batch, P * dim if mode == "elementwise" else P), dtype=torch.float32, device=x.device)
+    _lib_call("pnn_inner_fwd", ptr(x), ldx, nfield, dim, m, ptr(Kw), ptr(out), out.stride(0), col0, batch, stream())
+    return out
+
+
+def pnn_inner_bwd(g, ldg, gcol0, x, ldx, nfield, dim, mode, Kw, batch, want_dx=True, want_dk=True):
+    """g: the data pointer of the gradient buffer addressed like the forward's output -> (dx [B, nfield*dim] or
+    None, dK shaped like Kw or None)."""
+    _require_cuda(g, x, Kw)
+    dev = x.device
+    m = PNN_MODES[mode]
+    want_dk = want_dk and mode in ("vec", "num")
+    dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=dev) if want_dx else None
+    dK = torch.empty(tuple(Kw.shape), dtype=torch.float32, device=dev) if want_dk else None
+    nbytes = L.lib().b2ctr_pnn_inner_bwd_workspace_bytes(nfield, dim, m, batch) if want_dk else 0
+    ws = workspace(nbytes, dev) if want_dk else None
+    _lib_call("pnn_inner_bwd", ptr(g), ldg, gcol0, ptr(x), ldx, nfield, dim, m, ptr(Kw), ptr(dx), nfield * dim,
+              ptr(dK), batch, ptr(ws), nbytes, stream())
+    return dx, dK
+
+
+def pnn_outer_fwd(x, ldx, nfield, dim, Kw, batch, out=None, col0=0):
+    """OutterProductLayer('mat') with the kernel Kw [dim, P, dim] read in place: pair p's score goes to column
+    col0 + p of ``out`` [B, ld] (default: a new [B, P])."""
+    _require_cuda(x, Kw, out)
+    if out is None:
+        out = torch.empty((batch, nfield * (nfield - 1) // 2), dtype=torch.float32, device=x.device)
+    _lib_call("pnn_outer_fwd", ptr(x), ldx, nfield, dim, ptr(Kw), ptr(out), out.stride(0), col0, batch, stream())
+    return out
+
+
+def pnn_outer_bwd(g, ldg, gcol0, x, ldx, nfield, dim, Kw, batch, want_dx=True, want_dk=True):
+    """-> (dx [B, nfield*dim] or None, dK [dim, P, dim] or None)."""
+    _require_cuda(g, x, Kw)
+    dev = x.device
+    dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=dev) if want_dx else None
+    dK = torch.empty(tuple(Kw.shape), dtype=torch.float32, device=dev) if want_dk else None
+    nbytes = L.lib().b2ctr_pnn_outer_bwd_workspace_bytes(nfield, dim, batch) if want_dk else 0
+    ws = workspace(nbytes, dev) if want_dk else None
+    _lib_call("pnn_outer_bwd", ptr(g), ldg, gcol0, ptr(x), ldx, nfield, dim, ptr(Kw), ptr(dx), nfield * dim,
+              ptr(dK), batch, ptr(ws), nbytes, stream())
+    return dx, dK
+
+
 def din_att_input_fwd(q, ldq, keys, ldk, batch, T, E):
     out = torch.empty((batch, T, 4 * E), dtype=torch.float32, device=q.device)
     _lib_call("din_att_input_fwd", ptr(q), ldq, ptr(keys), ldk, ptr(out), batch, T, E, stream())
@@ -938,7 +993,8 @@ for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filte
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
            "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
            "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "fwfm_fwd", "fwfm_bwd", "fefm_sym",
-           "fefm_fwd", "fefm_bwd", "din_att_input_fwd", "din_att_input_bwd",
+           "fefm_fwd", "fefm_bwd", "pnn_inner_fwd", "pnn_inner_bwd", "pnn_outer_fwd", "pnn_outer_bwd",
+           "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
     globals()[_n] = _timed(globals()[_n])
@@ -992,7 +1048,8 @@ for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filte
            "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
            "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
            "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "fwfm_fwd", "fwfm_bwd", "fefm_sym",
-           "fefm_fwd", "fefm_bwd", "din_att_input_fwd", "din_att_input_bwd",
+           "fefm_fwd", "fefm_bwd", "pnn_inner_fwd", "pnn_inner_bwd", "pnn_outer_fwd", "pnn_outer_bwd",
+           "din_att_input_fwd", "din_att_input_bwd",
            "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
            "moving_update", "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
     globals()[_n] = _timed(globals()[_n])

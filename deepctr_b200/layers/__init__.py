@@ -1,9 +1,9 @@
 """deepctr.layers surface for the hot path (deepctr/layers/__init__.py:3-54 lists the reference's)."""
-from ..engine import Layer, Dense, Flatten, Concatenate, Add, Lambda, Input
+from ..engine import Layer, Dense, Flatten, Reshape, Concatenate, Add, Lambda, Input
 from .activation import Dice, Activation, activation_layer
 from .core import DNN, LocalActivationUnit, PredictionLayer
 from .interaction import (AFMLayer, BiInteractionPooling, BilinearInteraction, FM, CrossNet, CIN, InteractingLayer,
-                          SENETLayer, FwFMLayer, FEFMLayer)
+                          SENETLayer, FwFMLayer, FEFMLayer, InnerProductLayer, OutterProductLayer)
 from .normalization import BatchNormalization, Dropout, LayerNormalization
 from .sequence import (SequencePoolingLayer, WeightedSequenceLayer, AttentionSequencePoolingLayer, Transformer,
                        PositionEncoding)
@@ -15,6 +15,7 @@ custom_objects = {
     'AFMLayer': AFMLayer, 'BiInteractionPooling': BiInteractionPooling,
     'SENETLayer': SENETLayer, 'BilinearInteraction': BilinearInteraction,
     'FwFMLayer': FwFMLayer, 'FEFMLayer': FEFMLayer,
+    'InnerProductLayer': InnerProductLayer, 'OutterProductLayer': OutterProductLayer,
     'FM': FM, 'CrossNet': CrossNet, 'CIN': CIN, 'InteractingLayer': InteractingLayer,
     'SequencePoolingLayer': SequencePoolingLayer, 'WeightedSequenceLayer': WeightedSequenceLayer,
     'AttentionSequencePoolingLayer': AttentionSequencePoolingLayer, 'Dice': Dice, 'Hash': Hash,

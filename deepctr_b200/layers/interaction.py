@@ -1,7 +1,7 @@
 """Host mirror of deepctr/layers/interaction.py for the operators on the hot path:
 AFMLayer (:39-160), BiInteractionPooling (:163-206), FM (:563-607), CrossNet (:344-435), CIN (:209-341),
 InteractingLayer (:697-790), SENETLayer (:1067-1139), BilinearInteraction (:1142-1221), FwFMLayer (:1350-1425),
-FEFMLayer (:1428-1499).
+FEFMLayer (:1428-1499), InnerProductLayer (:610-695), OutterProductLayer (:793-931).
 Same constructor arguments, weight names, shape checks and error messages as the reference."""
 import itertools
 
@@ -19,6 +19,8 @@ SENET_MAX_FIELDS, BILINEAR_MAX_FIELDS, BILINEAR_MAX_EMBEDDING = 64, 64, 64
 # shapes the FwFM / FEFM kernels serve (include/b2ctr.h, b2ctr_fwfm_fwd, b2ctr_fefm_fwd)
 FWFM_MAX_FIELDS, FWFM_MAX_EMBEDDING = 64, 64
 FEFM_MAX_FIELDS, FEFM_MAX_EMBEDDING = 64, 64
+# shapes the PNN product kernels serve (include/b2ctr.h, b2ctr_pnn_inner_fwd, b2ctr_pnn_outer_fwd)
+PNN_MAX_FIELDS, PNN_MAX_EMBEDDING = 64, 64
 # shapes the InteractingLayer attention kernels serve (include/b2ctr.h, b2ctr_interacting_fwd / _bwd)
 INTERACTING_MAX_FIELDS, INTERACTING_MAX_ATT_EMBEDDING, INTERACTING_MAX_FHD = 64, 32, 3072
 
@@ -529,3 +531,115 @@ class FEFMLayer(Layer):
         config = Layer.get_config(self).copy()
         config.update({'regularizer': self.regularizer})
         return config
+
+
+def _check_product_inputs(name, input_shape):
+    """The reference's list-of-[B,1,E] checks and messages (InnerProductLayer / OutterProductLayer.build), then the
+    kernels' limits."""
+    if not isinstance(input_shape, list) or len(input_shape) < 2:
+        raise ValueError('A `%s` layer should be called '
+                         'on a list of at least 2 inputs' % name)
+    shape_set = set(tuple(s) for s in input_shape)
+    if len(shape_set) > 1:
+        raise ValueError('A `%s` layer requires '
+                         'inputs with same shapes '
+                         'Got different shapes: %s' % (name, shape_set))
+    if len(input_shape[0]) != 3 or input_shape[0][1] != 1:
+        raise ValueError('A `%s` layer requires '
+                         'inputs of a list with same shape tensor like (None,1,embedding_size)'
+                         'Got different shapes: %s' % (name, input_shape[0]))
+    num_inputs, embed_size = len(input_shape), int(input_shape[0][-1])
+    if num_inputs > PNN_MAX_FIELDS or not 1 <= embed_size <= PNN_MAX_EMBEDDING:
+        raise ValueError("%s supports 2 to %d inputs and embedding_size 1 to %d (got %d inputs, embedding_size %d)"
+                         % (name, PNN_MAX_FIELDS, PNN_MAX_EMBEDDING, num_inputs, embed_size))
+    return num_inputs, embed_size
+
+
+def _product_place(layer, x):
+    planner = getattr(layer, "_planner", None)
+    return planner.pnn_place(layer, x) if planner is not None else None
+
+
+def _product_operand(inputs):
+    if inputs[0].data.dim() != 3:
+        raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs[0].data.dim()))
+    # consecutive windows of the gather buffer concatenate to a zero-copy [B, F, E] window; anything else is one copy
+    return ops.concat(inputs, axis=1)
+
+
+class InnerProductLayer(Layer):
+    """PNN's inner products, deepctr/layers/interaction.py:610-695.  Called on a list of F [B,1,E] tensors; output
+    [B, P, 1] with row p = (i < j) equal to <v_i, v_j> (reduce_sum=True), or [B, P, E] with v_i * v_j
+    (b2ctr_pnn_inner_fwd: the gather buffer is read in place and no per-pair [B, E] product is written for the
+    inner products).  In PNN the products are written straight into the first DNN layer's input
+    (inputs.EmbeddingPlanner.pnn_place)."""
+
+    def __init__(self, reduce_sum=True, **kwargs):
+        self.reduce_sum = reduce_sum
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        _check_product_inputs("InnerProductLayer", input_shape)
+        self.built = True
+
+    def call(self, inputs, **kwargs):
+        x = _product_operand(inputs)
+        if not self.reduce_sum:
+            return ops.pnn_inner(x, "elementwise")
+        return ops.pnn_inner(x, "inner", out=_product_place(self, x))
+
+    def compute_output_shape(self, input_shape):
+        num_inputs = len(input_shape)
+        num_pairs = num_inputs * (num_inputs - 1) // 2
+        input_shape = input_shape[0]
+        return (input_shape[0], num_pairs, 1 if self.reduce_sum else input_shape[-1])
+
+    def get_config(self):
+        config = {'reduce_sum': self.reduce_sum}
+        base_config = Layer.get_config(self)
+        base_config.update(config)
+        return base_config
+
+
+class OutterProductLayer(Layer):
+    """PNN's outer products, deepctr/layers/interaction.py:793-931.  Called on a list of F [B,1,E] tensors; output
+    [B, P] with, for the pair p = (i < j), sum_{k,l} v_j[k] K[k,p,l] v_i[l] (kernel_type 'mat', K [E,P,E], on the
+    FEFM tiles: b2ctr_pnn_outer_fwd), sum_e v_i[e] v_j[e] K[p,e] ('vec', K [P,E]) or K[p] <v_i, v_j> ('num', K [P,1])
+    (b2ctr_pnn_inner_fwd).  The weight keeps the reference's name, shape and glorot_uniform(seed) initialiser."""
+
+    def __init__(self, kernel_type='mat', seed=1024, **kwargs):
+        if kernel_type not in ['mat', 'vec', 'num']:
+            raise ValueError("kernel_type must be mat,vec or num")
+        self.kernel_type = kernel_type
+        self.seed = seed
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        num_inputs, embed_size = _check_product_inputs("OutterProductLayer", input_shape)
+        num_pairs = num_inputs * (num_inputs - 1) // 2
+        if self.kernel_type == 'mat':
+            self.kernel = self.add_weight(shape=(embed_size, num_pairs, embed_size),
+                                          initializer=glorot_uniform(seed=self.seed), name='kernel')
+        elif self.kernel_type == 'vec':
+            self.kernel = self.add_weight(shape=(num_pairs, embed_size,), initializer=glorot_uniform(self.seed),
+                                          name='kernel')
+        elif self.kernel_type == 'num':
+            self.kernel = self.add_weight(shape=(num_pairs, 1), initializer=glorot_uniform(self.seed), name='kernel')
+        self.built = True
+
+    def call(self, inputs, **kwargs):
+        x = _product_operand(inputs)
+        out = _product_place(self, x)
+        if self.kernel_type == 'mat':
+            return ops.pnn_outer(x, self.kernel, out=out)
+        return ops.pnn_inner(x, self.kernel_type, self.kernel, out=out)
+
+    def compute_output_shape(self, input_shape):
+        num_inputs = len(input_shape)
+        return (None, num_inputs * (num_inputs - 1) // 2)
+
+    def get_config(self):
+        config = {'kernel_type': self.kernel_type, 'seed': self.seed}
+        base_config = Layer.get_config(self)
+        base_config.update(config)
+        return base_config

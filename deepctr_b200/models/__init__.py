@@ -8,5 +8,6 @@ from .afm import AFM
 from .fibinet import FiBiNET
 from .fwfm import FwFM
 from .deepfefm import DeepFEFM
+from .pnn import PNN
 
-__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM"]
+__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM", "PNN"]

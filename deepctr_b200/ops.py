@@ -579,6 +579,85 @@ def fefm(x, weights, stack, out=None):
     return res
 
 
+def _pair_grad(grads, b):
+    g = grads[0]
+    if g.dim() != 2 or g.stride(1) != 1 or g.stride(0) < g.shape[1]:
+        g = g.contiguous().reshape(b, -1)
+    return g
+
+
+def pnn_inner(x, mode, kernel=None, out=None):
+    """[B,F,E] -> PNN's pairwise products for the pairs p = (i < j) (b2ctr_pnn_inner_fwd): mode 'inner'
+    <x_i, x_j> as [B,P,1] (InnerProductLayer, layers/interaction.py:669-678), 'elementwise' x_i * x_j as [B,P,E]
+    (reduce_sum=False), 'vec' / 'num' the kernel-weighted inner products as [B,P] (OutterProductLayer,
+    :912-919, with ``kernel`` [P,E] / [P,1]).  x is read in place.
+
+    ``out``: a [B,P] column window (``_window``) of a wider buffer Var to write the scores into (PNN's DNN input,
+    inputs.EmbeddingPlanner.pnn_place); the result is then a window of that buffer.  Every consumer's gradient
+    lands in that buffer's gradient, so the backward is keyed on the buffer: it reads the score columns of its
+    gradient in place and leaves the gradient to the buffer's own backward (the gather's scatter), as ops.fefm."""
+    b, f, e = x.data.shape
+    P = f * (f - 1) // 2
+    src, ld = _fields2d(x)
+    kd = _wdata(kernel) if kernel is not None else None
+    shape = {"inner": (b, P, 1), "elementwise": (b, P, e)}.get(mode, (b, P))
+    if out is None:
+        res = E.Var(K.pnn_inner_fwd(src, ld, f, e, mode, kd, b).reshape(shape))
+        key, gcol0 = res, 0
+    else:
+        key, gcol0 = out.base, out.col0
+        K.pnn_inner_fwd(src, ld, f, e, mode, kd, b, out=key.data, col0=gcol0)
+        res = _window(key, gcol0, P, shape)
+    wts = [kernel] if kernel is not None else []
+
+    def bwd(grads):
+        want_dk = kernel is not None and kernel.requires_grad
+        if not (x.requires_grad or want_dk):
+            return
+        g = _pair_grad(grads, b)
+        dx, dk = K.pnn_inner_bwd(g, g.stride(0), gcol0, src, ld, f, e, mode, kd, b, want_dx=x.requires_grad,
+                                 want_dk=want_dk)
+        if dx is not None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        if dk is not None:
+            E.add_grad(kernel, dk)
+
+    if E.record([key], [x] + wts, bwd, keep_grads=out is not None):
+        res.requires_grad = True
+    return res
+
+
+def pnn_outer(x, kernel, out=None):
+    """[B,F,E] -> [B,P]: sum_{k,l} x_j[k] K[k,p,l] x_i[l] for the pairs p = (i < j) (OutterProductLayer
+    kernel_type='mat', layers/interaction.py:881-911), with the kernel [E,P,E] read in place by the FEFM tiles
+    (b2ctr_pnn_outer_fwd): no per-pair [B,E] product is written.  ``out`` as in pnn_inner."""
+    b, f, e = x.data.shape
+    src, ld = _fields2d(x)
+    kd = _wdata(kernel)
+    if out is None:
+        res = E.Var(K.pnn_outer_fwd(src, ld, f, e, kd, b))
+        key, gcol0 = res, 0
+    else:
+        key, gcol0 = out.base, out.col0
+        K.pnn_outer_fwd(src, ld, f, e, kd, b, out=key.data, col0=gcol0)
+        res = out
+
+    def bwd(grads):
+        if not (x.requires_grad or kernel.requires_grad):
+            return
+        g = _pair_grad(grads, b)
+        dx, dk = K.pnn_outer_bwd(g, g.stride(0), gcol0, src, ld, f, e, kd, b, want_dx=x.requires_grad,
+                                 want_dk=kernel.requires_grad)
+        if dx is not None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        if dk is not None:
+            E.add_grad(kernel, dk)
+
+    if E.record([key], [x, kernel], bwd, keep_grads=out is not None):
+        res.requires_grad = True
+    return res
+
+
 def add_bias(x, b, scale=1.0, per_sample=False):
     """x + scale * b over the last axis for a per-column (or scalar, when the last axis is 1) bias:
     Linear(use_bias=True) without a dense part, layers/utils.py:172-173.  ``per_sample``: b spans every non-batch

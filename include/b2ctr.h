@@ -544,6 +544,43 @@ B2CTR_API b2ctr_status_t b2ctr_fefm_bwd(const float* g, int64_t ldg, int64_t gco
                                        int32_t nfield, int32_t dim, const float* S, float* dx, int64_t lddx, float* dW,
                                        int64_t batch, void* workspace, size_t workspace_bytes, void* stream);
 
+/* PNN (deepctr/models/pnn.py).  For the P = nfield(nfield-1)/2 pairs p = (i < j) in itertools.combinations order,
+ * on x [B, nfield, dim] (row pitch ldx), written to the column window out[b*ldo + col0 + ...] of a wider buffer:
+ *   B2CTR_PNN_INNER        out[.. + p]         = <x_i, x_j>                 InnerProductLayer()
+ *   B2CTR_PNN_ELEMENTWISE  out[.. + p*dim + e] = x_i[e] x_j[e]              InnerProductLayer(reduce_sum=False)
+ *   B2CTR_PNN_VEC          out[.. + p]         = sum_e x_i[e] x_j[e] K[p][e]  OutterProductLayer('vec'), K [P, dim]
+ *   B2CTR_PNN_NUM          out[.. + p]         = K[p] <x_i, x_j>            OutterProductLayer('num'), K [P, 1]
+ * K is ignored (may be NULL) for the first two.  Limits: 2 <= nfield <= 64, 1 <= dim <= 64. */
+enum { B2CTR_PNN_INNER = 0, B2CTR_PNN_ELEMENTWISE = 1, B2CTR_PNN_VEC = 2, B2CTR_PNN_NUM = 3 };
+B2CTR_API b2ctr_status_t b2ctr_pnn_inner_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, int32_t mode,
+                                            const float* K, float* out, int64_t ldo, int64_t col0, int64_t batch,
+                                            void* stream);
+/* Backward from g[b*ldg + gcol0 + ...] (addressed like the forward's output), read in place:
+ *   dx_f[e] = sum_{q != f} g_p w_p[e] x_q[e]   (pitch lddx, overwritten; may be NULL)
+ *   dK (vec / num only; may be NULL): sum_b g_p x_i[e] x_j[e]  /  sum_b g_p <x_i, x_j>
+ * Every dx element has one owner that adds its partners in ascending order; dK goes through per-(entry tile,
+ * batch chunk) partials in the workspace, summed in chunk order.  No float atomics: bit-identical from run to run. */
+B2CTR_API size_t b2ctr_pnn_inner_bwd_workspace_bytes(int32_t nfield, int32_t dim, int32_t mode, int64_t batch);
+B2CTR_API b2ctr_status_t b2ctr_pnn_inner_bwd(const float* g, int64_t ldg, int64_t gcol0, const float* x, int64_t ldx,
+                                            int32_t nfield, int32_t dim, int32_t mode, const float* K, float* dx,
+                                            int64_t lddx, float* dK, int64_t batch, void* workspace,
+                                            size_t workspace_bytes, void* stream);
+
+/* OutterProductLayer(kernel_type='mat') with the reference's kernel K [dim, P, dim], read in place:
+ *   out[b*ldo + col0 + p] = sum_{k,l} x_j[k] K[k][p][l] x_i[l]
+ * on the FEFM kernels' register-tiled products (no [B, dim] product reaches memory).  Backward from
+ * g[b*ldg + gcol0 + p]:
+ *   dx_i = g_p x_j K[:,p,:],   dx_j = g_p K[:,p,:] x_i   (pitch lddx, overwritten; may be NULL)
+ *   dK[k][p][l] = sum_b g_p x_j[k] x_i[l]                ([dim, P, dim], overwritten; may be NULL)
+ * Same ordering guarantees as b2ctr_fefm_bwd.  Limits: 2 <= nfield <= 64, 1 <= dim <= 64. */
+B2CTR_API b2ctr_status_t b2ctr_pnn_outer_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim, const float* K,
+                                            float* out, int64_t ldo, int64_t col0, int64_t batch, void* stream);
+B2CTR_API size_t b2ctr_pnn_outer_bwd_workspace_bytes(int32_t nfield, int32_t dim, int64_t batch);
+B2CTR_API b2ctr_status_t b2ctr_pnn_outer_bwd(const float* g, int64_t ldg, int64_t gcol0, const float* x, int64_t ldx,
+                                            int32_t nfield, int32_t dim, const float* K, float* dx, int64_t lddx,
+                                            float* dK, int64_t batch, void* workspace, size_t workspace_bytes,
+                                            void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* 6. Sequence operators (DIN, pooling, Dice / BatchNormalization, dropout)                     */
 /* ------------------------------------------------------------------------------------------ */

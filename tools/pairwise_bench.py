@@ -5,6 +5,7 @@ that shape.
 
     python tools/pairwise_bench.py [--steps 20] [--warmup 5] [--reps 50] [--models NFM,AFM,FiBiNET]
     python tools/pairwise_bench.py --models FwFM,DeepFEFM
+    python tools/pairwise_bench.py --models PNN
 
 Prints one JSON line per measurement:
   * the hardware context (card, power limit, max SM clock), read in the same run;
@@ -16,7 +17,10 @@ Prints one JSON line per measurement:
   * FiBiNET's first DNN layer alone: the split of its [65536, 20816] operand into bf16 planes and the three
     20813 -> 256 GEMMs (forward, data gradient, weight gradient), so the step can be broken down;
   * with FwFM / DeepFEFM (not in the default set): b2ctr_fwfm_* and b2ctr_fefm_* against the same two bounds, and the
-    training steps of FwFM and DeepFEFM with their default (256, 128, 64) DNN.
+    training steps of FwFM and DeepFEFM with their default (256, 128, 64) DNN;
+  * with PNN (not in the default set): b2ctr_pnn_inner_* (inner, vec, num) and b2ctr_pnn_outer_* (mat) against the
+    same two bounds, and the training steps of IPNN (the default), OPNN with kernel_type 'mat' and both products,
+    with the (256, 128, 64) DNN.
 """
 import argparse
 import json
@@ -32,6 +36,10 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
+# --models PNN: the three product configurations timed
+PNN_STEPS = {"PNN-inner": dict(use_inner=True, use_outter=False),
+             "PNN-outer-mat": dict(use_inner=False, use_outter=True, kernel_type="mat"),
+             "PNN-inner-outer-mat": dict(use_inner=True, use_outter=True, kernel_type="mat")}
 
 
 def hardware():
@@ -63,6 +71,8 @@ def step_time(builder, steps, warmup):
         model = M.FwFM(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding=0)
     elif builder == "DeepFEFM":
         model = M.DeepFEFM(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding_feat=0)
+    elif builder.startswith("PNN"):
+        model = M.PNN(cols, dnn_hidden_units=(256, 128, 64), l2_reg_embedding=0, **PNN_STEPS[builder])
     elif builder == "FiBiNET":
         model = M.FiBiNET(cols, cols, bilinear_type="interaction", dnn_hidden_units=(256, 128, 64), l2_reg_linear=0,
                           l2_reg_embedding=0)
@@ -263,6 +273,50 @@ def fefm_kernels(reps, hw):
     return out
 
 
+def pnn_kernels(reps, hw):
+    """PNN's products at C2 (26 fields, E = 32, B = 65536), x a window of the [B, 848] gather buffer and the scores
+    written at column 845 of a [B, 1172] buffer."""
+    import torch
+    from deepctr_b200 import kernels as K
+    B, F, E, nd = 65536, 26, 32, 13
+    P = F * (F - 1) // 2
+    dev = torch.device("cuda", 0)
+    g = torch.Generator(device=dev).manual_seed(4)
+    clk = hw.get("max_sm_clock_mhz") or None
+    ffma_peak = 132 * 128 * 2 * clk * 1e6 if clk else None
+    ldx = (F * E + nd + 3) // 4 * 4
+    buf = torch.randn((B, ldx), device=dev, generator=g) * 0.1
+    xw = buf[:, :F * E]
+    x_bytes, s_bytes = B * F * E * 4, B * P * 4
+    ld, col0 = (F * E + nd + P + 3) // 4 * 4, F * E + nd
+    dnn_in = torch.randn((B, ld), device=dev, generator=g) * 0.1       # also the scores' gradient
+    shape = dict(B=B, F=F, E=E, P=P, ldx=ldx, ld_out=ld, col0=col0)
+    out = []
+    # inner / vec / num: 2E flop per pair forward; backward dx 2E per pair and field (twice), dK 2E (vec) per pair
+    for mode, Kw in (("inner", None), ("vec", torch.randn((P, E), device=dev, generator=g) / E ** 0.5),
+                     ("num", torch.randn((P, 1), device=dev, generator=g))):
+        k_bytes = 0 if Kw is None else Kw.numel() * 4
+        out.append(_report("pnn_inner_fwd_" + mode, shape, reps,
+                           lambda: K.pnn_inner_fwd(xw, ldx, F, E, mode, Kw, B, out=dnn_in, col0=col0),
+                           B * P * 2 * E, x_bytes + s_bytes + k_bytes, ffma_peak))
+        out.append(_report("pnn_inner_bwd_" + mode, shape, reps,
+                           lambda: K.pnn_inner_bwd(dnn_in, ld, col0, xw, ldx, F, E, mode, Kw, B),
+                           B * P * (4 * E + (2 * E if Kw is not None else 0)), 2 * x_bytes + s_bytes + 2 * k_bytes,
+                           ffma_peak))
+    Km = torch.randn((E, P, E), device=dev, generator=g) / E ** 0.5
+    k_bytes = Km.numel() * 4
+    # mat, the FEFM tiles: forward x_i M_p 2E^2 + the dot 2E per pair; backward dx 2 x (2E^2 + E), dK 2E^2 + E
+    out.append(_report("pnn_outer_fwd_mat", shape, reps,
+                       lambda: K.pnn_outer_fwd(xw, ldx, F, E, Km, B, out=dnn_in, col0=col0),
+                       B * P * (2 * E * E + 2 * E), x_bytes + k_bytes + s_bytes, ffma_peak))
+    out.append(_report("pnn_outer_bwd_mat", shape, reps,
+                       lambda: K.pnn_outer_bwd(dnn_in, ld, col0, xw, ldx, F, E, Km, B),
+                       B * P * (6 * E * E + 3 * E), 2 * x_bytes + 2 * k_bytes + s_bytes, ffma_peak))
+    del buf, dnn_in, Km
+    torch.cuda.empty_cache()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -285,6 +339,10 @@ def main():
     if "FwFM" in models or "DeepFEFM" in models:
         for r in fefm_kernels(args.reps, hw):
             print(json.dumps(r), flush=True)
+    if "PNN" in models:
+        for r in pnn_kernels(args.reps, hw):
+            print(json.dumps(r), flush=True)
+        models = [m for m in models if m != "PNN"] + list(PNN_STEPS)
     for builder in models:
         print(json.dumps(step_time(builder, args.steps, args.warmup)), flush=True)
 
