@@ -4,9 +4,11 @@
 // sort + ordered segmented reduce, not float atomics".  b2ctr_embed_scatter_uniform_bwd (embed.cu) combines the
 // gradient rows of duplicate ids with red.global.add: exact up to fp32 re-association, but in an order that
 // changes from run to run.  This path instead
-//   1. keys every (sample, feature) lookup with (feature << vbits | id)           [make_keys_kernel]
-//   2. stably radix-sorts the keys (cub::DeviceRadixSort, CUDA toolkit)          -> runs of equal (feature, id),
-//      inside a run in ascending sample order
+//   1. keys every (sample, feature) lookup with (table << vbits | id)             [make_keys_kernel]
+//      "table" is the first feature with the same table (features that share an embedding_name share one
+//      table, its linear twin and its Adagrad state): all the lookups of one row form ONE run
+//   2. stably radix-sorts the keys (cub::DeviceRadixSort, CUDA toolkit)          -> runs of equal (table, id),
+//      inside a run in ascending (sample, feature) order
 //   3. gives every run to ONE warp, which sums the run's gradient rows in that order in fp32 (no FMA
 //      contraction) and writes the row exactly once                               [apply_runs_kernel]
 // -> run-to-run bit-identical, and the natural home of optimizers that need a per-row read-modify-write of
@@ -36,7 +38,8 @@ struct SortedParams {
   int64_t ldx;
   uint64_t fm_mask;
   int32_t nfeat, dim, idx_dtype, optimizer;
-  int32_t shift;               // bits of the largest vocabulary: key = feature << shift | id
+  int32_t shift;               // bits of the largest vocabulary: key = group[feature] << shift | id
+  int8_t group[kMaxFeat];      // first feature with the same table (and lin table and accumulators)
   float lr, lin_lr, eps;
 };
 
@@ -48,7 +51,8 @@ __global__ void __launch_bounds__(256)
     const int f = (int)(n - b * p.nfeat);
     const int64_t id = load_idx(p.idx[f], b * p.idx_stride[f], p.idx_dtype);
     // ids outside the vocabulary get the key of a feature that does not exist: they sort last and are skipped
-    keys[n] = ((uint64_t)(id_in_range(id, p.vocab[f]) ? f : p.nfeat) << p.shift) | (id_in_range(id, p.vocab[f]) ? (uint64_t)id : 0ull);
+    const bool ok = id_in_range(id, p.vocab[f]);
+    keys[n] = ((uint64_t)(ok ? p.group[f] : p.nfeat) << p.shift) | (ok ? (uint64_t)id : 0ull);
     vals[n] = (uint32_t)n;
   }
 }
@@ -76,16 +80,17 @@ __global__ void __launch_bounds__(256)
   const int chunks = p.dim >> 2;
   for (int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < total; i += nw) {
     const uint64_t key = keys[i];
-    const int f = (int)(key >> p.shift);
+    const int f = (int)(key >> p.shift);                                      // the table's first feature
     if (f >= p.nfeat || (i > 0 && keys[i - 1] == key)) continue;             // invalid id / not the head of a run
     const int64_t id = (int64_t)(key & ((1ull << p.shift) - 1));
-    const bool fm_on = p.dfm != nullptr && ((p.fm_mask >> f) & 1ull);
     float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
     float gl = 0.f;
-    for (int64_t j = i; j < total && keys[j] == key; ++j) {                  // ascending sample order (stable sort)
+    for (int64_t j = i; j < total && keys[j] == key; ++j) {                  // ascending (b, f) order (stable sort)
       const int64_t b = (int64_t)(vals[j] / (uint32_t)p.nfeat);
+      const int fj = (int)(vals[j] - (uint32_t)b * (uint32_t)p.nfeat);        // this lookup's own feature
+      const bool fm_on = p.dfm != nullptr && ((p.fm_mask >> fj) & 1ull);
       if (lane < chunks) {
-        const int64_t off = b * p.ldx + (int64_t)f * p.dim + lane * 4;
+        const int64_t off = b * p.ldx + (int64_t)fj * p.dim + lane * 4;
         float4 r = p.dx ? *reinterpret_cast<const float4*>(p.dx + off) : make_float4(0.f, 0.f, 0.f, 0.f);
         if (fm_on) {
           const float gf = p.dfm[b];
@@ -189,6 +194,16 @@ b2ctr_status_t b2ctr_embed_update_sorted(const b2ctr_uniform_gather_t* g, const 
     p.lin_acc[f] = lin_acc_tables ? lin_acc_tables[f] : nullptr;
     B2_REQUIRE(optimizer == 0 || (p.acc[f] && (!p.lin[f] || !dlinear || p.lin_acc[f])),
                "embed_update_sorted: adagrad accumulator of feature %d missing", f);
+    // features that share a table are one run per row: they must share everything the run writes
+    p.group[f] = (int8_t)f;
+    for (int h = 0; h < f; ++h) {
+      if (p.table[h] != p.table[f]) continue;
+      B2_REQUIRE(p.lin[h] == p.lin[f] && p.acc[h] == p.acc[f] && p.lin_acc[h] == p.lin_acc[f],
+                 "embed_update_sorted: features %d and %d share a table but not its linear table / accumulators",
+                 h, f);
+      p.group[f] = p.group[h];
+      break;
+    }
   }
   p.x = g->x; p.dx = dx; p.dfm = dfm; p.dlinear = g->lin_tables ? dlinear : nullptr; p.ldx = g->ldx;
   p.fm_mask = g->fm_mask[0]; p.nfeat = g->nfeat; p.dim = dim; p.idx_dtype = g->feats[0].idx_dtype;

@@ -149,7 +149,7 @@ def embed_scatter_uniform_bwd(plan, dx, dfm, dlinear, scale, lin_scale, batch):
 
 
 def embed_update_sorted(plan, dx, dfm, dlinear, optimizer, lr, lin_lr, eps, acc_tables, lin_acc_tables, batch):
-    """Deterministic fused update (sort by (feature, id) + ordered segmented reduce, one write per row):
+    """Deterministic fused update (sort by (table, id) + ordered segmented reduce, one write per row):
     optimizer 0 = SGD, 1 = Keras Adagrad (lazy / sparse apply) with per-element accumulators."""
     nf = plan.g.nfeat
     dim = plan.feat_arr[0].dim

@@ -158,7 +158,8 @@ B2CTR_API b2ctr_status_t b2ctr_embed_gather_uniform_fwd(const b2ctr_uniform_gath
 /* Backward of the above fused with the row update:
  *   g_row(b,f) = dx[b, f*dim:(f+1)*dim] + dfm[b] * (S_b - x[b, f*dim:...])   (FM Jacobian, App. A.6)
  *   table_f[id] += scale * g_row ;  lin_table_f[id] += lin_scale * dlinear[b]
- * dx, dfm, dlinear may each be NULL.  ddense (if not NULL) receives dx[:, F*dim : F*dim+ndense]. */
+ * dx, dfm, dlinear may each be NULL.  The dense columns of dx are not read: their gradient is the caller's.
+ * Rows of duplicate ids are combined with red.global.add, in an order that changes from run to run. */
 B2CTR_API b2ctr_status_t b2ctr_embed_scatter_uniform_bwd(const b2ctr_uniform_gather_t* g,
                                                         const float* dx, const float* dfm,
                                                         const float* dlinear, float scale,
@@ -174,12 +175,14 @@ B2CTR_API b2ctr_status_t b2ctr_embed_scatter_uniform_bwd(const b2ctr_uniform_gat
 B2CTR_API b2ctr_status_t b2ctr_embed_oob_count(int64_t* count, int32_t reset, void* stream);
 
 /* DETERMINISTIC fused update of the Criteo-shaped fast path (same descriptor and gradients as
- * b2ctr_embed_scatter_uniform_bwd; tables whole, world <= 1): the lookups are sorted by (feature, id), the
- * gradient rows of duplicate ids are summed in ascending sample order in fp32 and every touched row is written
- * ONCE - bit-identical from run to run, and the home of row-state optimizers:
+ * b2ctr_embed_scatter_uniform_bwd; tables whole, world <= 1): the lookups are sorted by (table, id), the
+ * gradient rows of all the lookups of one row are summed in ascending (sample, feature) order in fp32 and every
+ * touched row is written ONCE - bit-identical from run to run, and the home of row-state optimizers:
  *   optimizer 0: w -= lr * g                       (row-wise SGD)
  *   optimizer 1: acc += g^2; w -= lr * g / (sqrt(acc) + eps)   (Keras Adagrad, whose sparse apply is lazy)
  * acc_tables / lin_acc_tables: host arrays [nfeat] of device pointers shaped like the tables (optimizer 1).
+ * Features may share a table (a shared embedding_name); they must then share its linear table and
+ * accumulators too, else the call fails with B2CTR_ERR_INVALID_ARG before any launch.
  * Uses cub::DeviceRadixSort from the CUDA toolkit for the key sort. */
 B2CTR_API size_t b2ctr_embed_update_sorted_workspace_bytes(int32_t nfeat, int32_t dim, int64_t batch);
 B2CTR_API b2ctr_status_t b2ctr_embed_update_sorted(const b2ctr_uniform_gather_t* g, const float* dx,
