@@ -128,6 +128,13 @@ SIGNATURES = {
     "b2ctr_mask_from_len": (_i32, [_vp, _i64, _i32, _vp, _vp]),
     "b2ctr_fm_fwd": (_i32, [_vp, _i64, _i32, _i32, _vp, _i64, _vp]),
     "b2ctr_fm_bwd": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp, _i64, _i32, _i64, _vp]),
+    "b2ctr_fm_weighted_fwd": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _vp, _i64, _vp]),
+    "b2ctr_fm_weighted_bwd": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _vp, _vp, _i64, _i32, _vp, _i64, _i64, _vp]),
+    "b2ctr_field_scale_fwd": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _vp, _i64, _i64, _vp]),
+    "b2ctr_field_scale_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp, _i64, _i32, _vp, _i64, _i64,
+                                     _vp]),
+    "b2ctr_softmax_rows_fwd": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _f32, _vp]),
+    "b2ctr_softmax_rows_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i64, _i32, _f32, _vp]),
     "b2ctr_predict_loss": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp]),
     "b2ctr_sgd_step": (_i32, [_vp, _vp, _f32, _f32, _i64, _vp]),
     "b2ctr_sgd_step_multi": (_i32, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.POINTER(C.c_float), _i32, _f32, _vp]),

@@ -216,18 +216,23 @@ __global__ void rowsum_kernel(const float* __restrict__ x, int64_t ld, float* ou
 // -------------------------------------------------------------------------------------------
 // FM (deepctr/layers/interaction.py:597-602): one warp per sample, lanes over the embedding
 // axis, fields walked sequentially; pairwise reduction over e by warp shuffles.
+// WEIGHTED: FM of (m ⊙ x) with per-sample field weights m [B, F] (IFM / DIFM), the product formed
+// in registers.  With m == 1 every multiply by m is exact, so the result is the unweighted one bit for bit.
 // -------------------------------------------------------------------------------------------
-__global__ void fm_fwd_kernel(const float* __restrict__ x, int64_t ldx, int nfield, int dim,
-                              float* out, int64_t batch) {
+template <bool WEIGHTED>
+__global__ void fm_fwd_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ m,
+                              int64_t ldm, int nfield, int dim, float* out, int64_t batch) {
   const int lane = threadIdx.x & 31;
   const int64_t nw = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); b < batch; b += nw) {
     const float* xr = x + b * ldx;
+    const float* mr = WEIGHTED ? m + b * ldm : nullptr;
     float tot = 0.f;
     for (int e = lane; e < dim; e += 32) {
       float s = 0.f, q = 0.f;
       for (int f = 0; f < nfield; ++f) {
-        const float v = xr[f * dim + e];
+        float v = xr[f * dim + e];
+        if (WEIGHTED) v *= mr[f];
         s += v;
         q += v * v;
       }
@@ -237,23 +242,146 @@ __global__ void fm_fwd_kernel(const float* __restrict__ x, int64_t ldx, int nfie
     if (lane == 0) out[b] = 0.5f * tot;
   }
 }
-__global__ void fm_bwd_kernel(const float* __restrict__ x, int64_t ldx, int nfield, int dim,
-                              const float* __restrict__ dout, float* dx, int64_t lddx, int acc,
-                              int64_t batch) {
+// dx_f = g m_f (S - m_f x_f) with S = sum_f m_f x_f (m == 1 unweighted).  WEIGHTED also writes
+// dm_f = g sum_e x_f (S - m_f x_f): per 32-column chunk a fixed shuffle tree, chunks added in order by lane 0,
+// so dm is bit-identical from run to run.
+template <bool WEIGHTED>
+__global__ void fm_bwd_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ m,
+                              int64_t ldm, int nfield, int dim, const float* __restrict__ dout, float* dx,
+                              int64_t lddx, float* dm, int64_t lddm, int acc, int64_t batch) {
   const int lane = threadIdx.x & 31;
   const int64_t nw = (int64_t)gridDim.x * (blockDim.x >> 5);
   for (int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); b < batch; b += nw) {
     const float* xr = x + b * ldx;
-    float* dr = dx + b * lddx;
+    const float* mr = WEIGHTED ? m + b * ldm : nullptr;
+    float* dr = dx ? dx + b * lddx : nullptr;
+    float* dmr = WEIGHTED && dm ? dm + b * lddm : nullptr;
     const float g = dout[b];
-    for (int e = lane; e < dim; e += 32) {
+    for (int e0 = 0; e0 < dim; e0 += 32) {
+      const int e = e0 + lane;
+      const bool on = e < dim;
       float s = 0.f;
-      for (int f = 0; f < nfield; ++f) s += xr[f * dim + e];
+      if (on)
+        for (int f = 0; f < nfield; ++f) s += WEIGHTED ? mr[f] * xr[f * dim + e] : xr[f * dim + e];
       for (int f = 0; f < nfield; ++f) {
-        const float v = g * (s - xr[f * dim + e]);
-        dr[f * dim + e] = acc ? dr[f * dim + e] + v : v;
+        if (WEIGHTED) {
+          const float mf = mr[f];
+          const float xv = on ? xr[f * dim + e] : 0.f;
+          const float r = s - mf * xv;
+          if (on && dr) {
+            const float v = g * mf * r;
+            dr[f * dim + e] = acc ? dr[f * dim + e] + v : v;
+          }
+          if (dmr) {
+            const float t = warp_sum(xv * r);
+            if (lane == 0) dmr[f] = e0 == 0 ? t : dmr[f] + t;
+          }
+        } else if (on) {
+          const float v = g * (s - xr[f * dim + e]);
+          dr[f * dim + e] = acc ? dr[f * dim + e] + v : v;
+        }
       }
     }
+    if (dmr && lane == 0)
+      for (int f = 0; f < nfield; ++f) dmr[f] *= g;
+  }
+}
+
+// -------------------------------------------------------------------------------------------
+// Field scale y[b,f,:] = x[b,f,:] * m[b,f] (the refine product of IFM / DIFM, feature_column.py:193-200,
+// ifm.py:66-67) and its backward.  One group of W lanes (W = the power of two >= min(dim, 32)) per (b, f)
+// row, lanes striding e; dm's row sum is a fixed shuffle tree inside the group (deterministic).
+// -------------------------------------------------------------------------------------------
+__device__ __forceinline__ float group_sum(float v, int width) {
+  for (int o = width >> 1; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o, width);
+  return v;
+}
+__global__ void field_scale_fwd_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ m,
+                                       int64_t ldm, int nfield, int dim, float* y, int64_t ldy, int64_t batch,
+                                       int width) {
+  const int sub = threadIdx.x & (width - 1);
+  const int64_t groups = (int64_t)gridDim.x * (blockDim.x / width);
+  const int64_t rows = batch * nfield;
+  for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / width; r < rows; r += groups) {
+    const int64_t b = r / nfield;
+    const int f = (int)(r - b * nfield);
+    const float mf = m[b * ldm + f];
+    const float* xr = x + b * ldx + (int64_t)f * dim;
+    float* yr = y + b * ldy + (int64_t)f * dim;
+    for (int e = sub; e < dim; e += width) yr[e] = xr[e] * mf;
+  }
+}
+__global__ void field_scale_bwd_kernel(const float* __restrict__ dy, int64_t lddy, const float* __restrict__ x,
+                                       int64_t ldx, const float* __restrict__ m, int64_t ldm, int nfield, int dim,
+                                       float* dx, int64_t lddx, float* dm, int64_t lddm, int acc, int64_t batch,
+                                       int width) {
+  const int sub = threadIdx.x & (width - 1);
+  const int64_t groups = (int64_t)gridDim.x * (blockDim.x / width);
+  const int64_t rows = batch * nfield;
+  // every group of a warp runs the same number of iterations (rows rounded up), so the shuffles stay converged
+  const int64_t rows_pad = (rows + 32 / width - 1) / (32 / width) * (32 / width);
+  for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / width; r < rows_pad; r += groups) {
+    const bool on = r < rows;
+    const int64_t b = on ? r / nfield : 0;
+    const int f = on ? (int)(r - b * nfield) : 0;
+    const float mf = on ? m[b * ldm + f] : 0.f;
+    const float* dyr = dy + b * lddy + (int64_t)f * dim;
+    const float* xr = x + b * ldx + (int64_t)f * dim;
+    float t = 0.f;
+    if (on)
+      for (int e = sub; e < dim; e += width) {
+        const float gv = dyr[e];
+        if (dx) {
+          float* p = dx + b * lddx + (int64_t)f * dim + e;
+          const float v = gv * mf;
+          *p = acc ? *p + v : v;
+        }
+        t += gv * xr[e];
+      }
+    t = group_sum(t, width);
+    if (on && sub == 0 && dm) dm[b * lddm + f] = t;
+  }
+}
+
+// -------------------------------------------------------------------------------------------
+// y = scale * softmax(x) along the rows of a [B, C] window (layers/utils.py softmax; IFM's F * softmax(z)).
+// One warp per row; the maximum is subtracted first.  Backward: dx = y (dy - sum_j y_j dy_j / scale).
+// -------------------------------------------------------------------------------------------
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+__global__ void softmax_rows_fwd_kernel(const float* __restrict__ x, int64_t ldx, float* y, int64_t ldy,
+                                        int64_t rows, int cols, float scale) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); r < rows; r += nw) {
+    const float* xr = x + r * ldx;
+    float* yr = y + r * ldy;
+    float mx = -INFINITY;
+    for (int c = lane; c < cols; c += 32) mx = fmaxf(mx, xr[c]);
+    mx = warp_max(mx);
+    float s = 0.f;
+    for (int c = lane; c < cols; c += 32) s += expf(xr[c] - mx);
+    s = warp_sum(s);
+    const float k = scale / s;
+    for (int c = lane; c < cols; c += 32) yr[c] = expf(xr[c] - mx) * k;
+  }
+}
+__global__ void softmax_rows_bwd_kernel(const float* __restrict__ y, int64_t ldy, const float* __restrict__ dy,
+                                        int64_t lddy, float* dx, int64_t lddx, int64_t rows, int cols,
+                                        float scale) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); r < rows; r += nw) {
+    const float* yr = y + r * ldy;
+    const float* gr = dy + r * lddy;
+    float* dr = dx + r * lddx;
+    float d = 0.f;
+    for (int c = lane; c < cols; c += 32) d += yr[c] * gr[c];
+    d = warp_sum(d) / scale;
+    for (int c = lane; c < cols; c += 32) dr[c] = yr[c] * (gr[c] - d);
   }
 }
 
@@ -527,7 +655,7 @@ b2ctr_status_t b2ctr_fm_fwd(const float* x, int64_t ldx, int32_t nfield, int32_t
                             int64_t batch, void* stream) {
   B2_REQUIRE(x && out && nfield > 0 && dim > 0 && ldx >= (int64_t)nfield * dim, "fm_fwd: bad arguments");
   if (batch <= 0) return B2CTR_OK;
-  fm_fwd_kernel<<<grid_for(batch, 8, 8), 256, 0, ST>>>(x, ldx, nfield, dim, out, batch);
+  fm_fwd_kernel<false><<<grid_for(batch, 8, 8), 256, 0, ST>>>(x, ldx, nullptr, 0, nfield, dim, out, batch);
   B2_CHECK_LAUNCH("b2ctr_fm_fwd");
   return B2CTR_OK;
 }
@@ -537,9 +665,86 @@ b2ctr_status_t b2ctr_fm_bwd(const float* x, int64_t ldx, int32_t nfield, int32_t
   B2_REQUIRE(x && dout && dx && nfield > 0 && dim > 0, "fm_bwd: bad arguments");
   B2_REQUIRE(ldx >= (int64_t)nfield * dim && lddx >= (int64_t)nfield * dim, "fm_bwd: ld too small");
   if (batch <= 0) return B2CTR_OK;
-  fm_bwd_kernel<<<grid_for(batch, 8, 8), 256, 0, ST>>>(x, ldx, nfield, dim, dout, dx, lddx, accumulate,
-                                                      batch);
+  fm_bwd_kernel<false><<<grid_for(batch, 8, 8), 256, 0, ST>>>(x, ldx, nullptr, 0, nfield, dim, dout, dx, lddx,
+                                                             nullptr, 0, accumulate, batch);
   B2_CHECK_LAUNCH("b2ctr_fm_bwd");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_fm_weighted_fwd(const float* x, int64_t ldx, const float* m, int64_t ldm, int32_t nfield,
+                                     int32_t dim, float* out, int64_t batch, void* stream) {
+  B2_REQUIRE(x && m && out && nfield > 0 && dim > 0, "fm_weighted_fwd: bad arguments");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && ldm >= nfield, "fm_weighted_fwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  fm_fwd_kernel<true><<<grid_for(batch, 8, 8), 256, 0, ST>>>(x, ldx, m, ldm, nfield, dim, out, batch);
+  B2_CHECK_LAUNCH("b2ctr_fm_weighted_fwd");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_fm_weighted_bwd(const float* x, int64_t ldx, const float* m, int64_t ldm, int32_t nfield,
+                                     int32_t dim, const float* dout, float* dx, int64_t lddx, int32_t accumulate,
+                                     float* dm, int64_t lddm, int64_t batch, void* stream) {
+  B2_REQUIRE(x && m && dout && (dx || dm) && nfield > 0 && dim > 0, "fm_weighted_bwd: bad arguments");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && ldm >= nfield && (!dx || lddx >= (int64_t)nfield * dim) &&
+                 (!dm || lddm >= nfield),
+             "fm_weighted_bwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  fm_bwd_kernel<true><<<grid_for(batch, 8, 8), 256, 0, ST>>>(x, ldx, m, ldm, nfield, dim, dout, dx, lddx, dm,
+                                                            lddm, accumulate, batch);
+  B2_CHECK_LAUNCH("b2ctr_fm_weighted_bwd");
+  return B2CTR_OK;
+}
+
+static int field_scale_width(int32_t dim) {
+  int w = 1;
+  while (w < dim && w < 32) w <<= 1;
+  return w;
+}
+
+b2ctr_status_t b2ctr_field_scale_fwd(const float* x, int64_t ldx, const float* m, int64_t ldm, int32_t nfield,
+                                     int32_t dim, float* y, int64_t ldy, int64_t batch, void* stream) {
+  B2_REQUIRE(x && m && y && nfield > 0 && dim > 0, "field_scale_fwd: bad arguments");
+  B2_REQUIRE(ldx >= (int64_t)nfield * dim && ldm >= nfield && ldy >= (int64_t)nfield * dim,
+             "field_scale_fwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  const int w = field_scale_width(dim);
+  field_scale_fwd_kernel<<<grid_for(batch * nfield, 256 / w, 8), 256, 0, ST>>>(x, ldx, m, ldm, nfield, dim, y, ldy,
+                                                                               batch, w);
+  B2_CHECK_LAUNCH("b2ctr_field_scale_fwd");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_field_scale_bwd(const float* dy, int64_t lddy, const float* x, int64_t ldx, const float* m,
+                                     int64_t ldm, int32_t nfield, int32_t dim, float* dx, int64_t lddx,
+                                     int32_t accumulate, float* dm, int64_t lddm, int64_t batch, void* stream) {
+  B2_REQUIRE(dy && x && m && (dx || dm) && nfield > 0 && dim > 0, "field_scale_bwd: bad arguments");
+  B2_REQUIRE(lddy >= (int64_t)nfield * dim && ldx >= (int64_t)nfield * dim && ldm >= nfield &&
+                 (!dx || lddx >= (int64_t)nfield * dim) && (!dm || lddm >= nfield),
+             "field_scale_bwd: ld too small");
+  if (batch <= 0) return B2CTR_OK;
+  const int w = field_scale_width(dim);
+  field_scale_bwd_kernel<<<grid_for(batch * nfield, 256 / w, 8), 256, 0, ST>>>(
+      dy, lddy, x, ldx, m, ldm, nfield, dim, dx, lddx, dm, lddm, accumulate, batch, w);
+  B2_CHECK_LAUNCH("b2ctr_field_scale_bwd");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_softmax_rows_fwd(const float* x, int64_t ldx, float* y, int64_t ldy, int64_t rows,
+                                      int32_t cols, float scale, void* stream) {
+  B2_REQUIRE(x && y && cols > 0 && ldx >= cols && ldy >= cols && scale != 0.f, "softmax_rows_fwd: bad arguments");
+  if (rows <= 0) return B2CTR_OK;
+  softmax_rows_fwd_kernel<<<grid_for(rows, 8, 8), 256, 0, ST>>>(x, ldx, y, ldy, rows, cols, scale);
+  B2_CHECK_LAUNCH("b2ctr_softmax_rows_fwd");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_softmax_rows_bwd(const float* y, int64_t ldy, const float* dy, int64_t lddy, float* dx,
+                                      int64_t lddx, int64_t rows, int32_t cols, float scale, void* stream) {
+  B2_REQUIRE(y && dy && dx && cols > 0 && ldy >= cols && lddy >= cols && lddx >= cols && scale != 0.f,
+             "softmax_rows_bwd: bad arguments");
+  if (rows <= 0) return B2CTR_OK;
+  softmax_rows_bwd_kernel<<<grid_for(rows, 8, 8), 256, 0, ST>>>(y, ldy, dy, lddy, dx, lddx, rows, cols, scale);
+  B2_CHECK_LAUNCH("b2ctr_softmax_rows_bwd");
   return B2CTR_OK;
 }
 

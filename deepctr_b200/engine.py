@@ -646,7 +646,13 @@ class Layer(object):
     def _output_dtype(self, inputs):
         return "float32"
 
+    # True on layers whose call() takes an ops.ScaledFields (the refine product kept as its factors) as it is; every
+    # other layer receives the materialised product
+    takes_scaled_fields = False
+
     def _invoke(self, vars_in, training, kwargs=None):
+        if not self.takes_scaled_fields:
+            vars_in = _map_structure(lambda v: v.product() if isinstance(v, ops.ScaledFields) else v, vars_in)
         if self._call_args is None:
             try:
                 self._call_args = set(inspect.signature(self.call).parameters)
@@ -822,7 +828,13 @@ class Lambda(Layer):
         return self.function(inputs)
 
     def compute_output_shape(self, input_shape):
-        return self._out_shape if self._out_shape is not None else input_shape
+        """``output_shape`` when given; over a list of inputs the shape of the highest-rank one (the broadcast result
+        of an elementwise lambda such as ``x[0] * expand_dims(x[1], -1)``), so that the Lambda has one output."""
+        if self._out_shape is not None:
+            return self._out_shape
+        if isinstance(input_shape, list) and input_shape and isinstance(input_shape[0], (list, tuple)):
+            return tuple(max(input_shape, key=len))
+        return input_shape
 
 
 # ================================================================================================

@@ -359,6 +359,10 @@ class EmbeddingPlanner(object):
         self.lin_ld = max(1, (self.lin_width + 3) // 4 * 4)
         self.fast = self._fast_eligible()
         self.dnn_places = _plan_dnn_input(model, consumers, out_ids)
+        # IFM / DIFM scale the linear lookups by per-sample field weights before Linear sums them: their rows are
+        # needed, so they are never fused into the gather's row-sum (lin_hint)
+        from .layers.utils import RefineWeight
+        self.lin_refined = any(isinstance(node.layer, RefineWeight) for node in model._order)
 
     # ---- configuration ---------------------------------------------------------------------------
     def tables(self):
@@ -385,6 +389,10 @@ class EmbeddingPlanner(object):
             if mode == "sparse_deterministic" or optimizer.name == "adagrad":
                 raise ValueError("the deterministic / Adagrad row-wise update covers models whose sparse features are "
                                  "single-valued columns of one embedding_dim (the Criteo shape)")
+        if self.sorted_update and self.lin and self.lin_refined:
+            raise ValueError("the deterministic / Adagrad row-wise update sums the linear lookups inside the gather, "
+                             "but this model scales them by field weights first (sparse_feat_refine_weight): use "
+                             "embedding_update='dense', or 'sparse' with the 'sgd' optimizer")
         if self.sorted_update and self.lin:
             self.lin_hint = True        # the linear tables are updated by the same sorted pass from the first step on
         tabs = list(self.tables())
@@ -418,7 +426,7 @@ class EmbeddingPlanner(object):
         self.sharded = False
         if ctx.world == 1:
             return
-        lin_ok = self.fast and self._lin_matches_fast()
+        lin_ok = self.fast and self._lin_matches_fast() and not self.lin_refined
         shardable = self.fast and (lin_ok or not self.lin)
         will_shard = set()
         if shardable:

@@ -354,6 +354,72 @@ def fm_bwd(x, nfield, dim, dout, dx=None, accumulate=False, ldx=None):
     return dx
 
 
+def fm_weighted_fwd(x, ldx, m, nfield, dim, batch):
+    """FM of m ⊙ x: x a [B, nfield*dim] window (row pitch ldx), m [B, nfield] (row pitch m.stride(0)) -> [B]."""
+    _require_cuda(x, m)
+    out = torch.empty((batch,), dtype=torch.float32, device=x.device)
+    L.check(L.lib().b2ctr_fm_weighted_fwd(ptr(x), ldx, ptr(m), m.stride(0), nfield, dim, ptr(out), batch, stream()),
+            "fm_weighted_fwd")
+    return out
+
+
+def fm_weighted_bwd(x, ldx, m, nfield, dim, dout, batch, dx=None, accumulate=False, want_dx=True, want_dm=True):
+    """(dx [B, nfield*dim] or the given window, dm [B, nfield] | None).  ``dx`` given: written with its own row pitch,
+    added to when ``accumulate``."""
+    _require_cuda(x, m, dout, dx)
+    if dx is None and want_dx:
+        dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=x.device)
+        accumulate = False
+    dm = torch.empty((batch, nfield), dtype=torch.float32, device=x.device) if want_dm else None
+    L.check(L.lib().b2ctr_fm_weighted_bwd(ptr(x), ldx, ptr(m), m.stride(0), nfield, dim, ptr(dout), ptr(dx),
+                                          dx.stride(0) if dx is not None else nfield * dim, int(accumulate), ptr(dm),
+                                          nfield, batch, stream()), "fm_weighted_bwd")
+    return dx, dm
+
+
+def field_scale_fwd(x, ldx, m, nfield, dim, batch, out=None):
+    """y[b, f*dim + e] = x[b, f*dim + e] * m[b, f] -> [B, nfield*dim] (or into ``out``, a 2-D window)."""
+    _require_cuda(x, m, out)
+    if out is None:
+        out = torch.empty((batch, nfield * dim), dtype=torch.float32, device=x.device)
+    L.check(L.lib().b2ctr_field_scale_fwd(ptr(x), ldx, ptr(m), m.stride(0), nfield, dim, ptr(out), out.stride(0),
+                                          batch, stream()), "field_scale_fwd")
+    return out
+
+
+def field_scale_bwd(dy, x, ldx, m, nfield, dim, batch, dx=None, accumulate=False, want_dx=True, want_dm=True):
+    """(dx = dy * m [B, nfield*dim] or the given window, dm = sum_e dy x [B, nfield] | None)."""
+    _require_cuda(dy, x, m, dx)
+    if dx is None and want_dx:
+        dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=x.device)
+        accumulate = False
+    dm = torch.empty((batch, nfield), dtype=torch.float32, device=x.device) if want_dm else None
+    L.check(L.lib().b2ctr_field_scale_bwd(ptr(dy), dy.stride(0), ptr(x), ldx, ptr(m), m.stride(0), nfield, dim,
+                                          ptr(dx), dx.stride(0) if dx is not None else nfield * dim, int(accumulate),
+                                          ptr(dm), nfield, batch, stream()), "field_scale_bwd")
+    return dx, dm
+
+
+def softmax_rows_fwd(x, scale=1.0):
+    """scale * softmax along the rows of a 2-D window x (row pitch x.stride(0)) -> a new [rows, cols] tensor."""
+    _require_cuda(x)
+    rows, cols = x.shape
+    y = torch.empty((rows, cols), dtype=torch.float32, device=x.device)
+    L.check(L.lib().b2ctr_softmax_rows_fwd(ptr(x), x.stride(0), ptr(y), cols, rows, cols, scale, stream()),
+            "softmax_rows_fwd")
+    return y
+
+
+def softmax_rows_bwd(y, dy, scale=1.0):
+    """dx = y * (dy - sum_j y_j dy_j / scale) for 2-D windows y, dy -> a new [rows, cols] tensor."""
+    _require_cuda(y, dy)
+    rows, cols = y.shape
+    dx = torch.empty((rows, cols), dtype=torch.float32, device=y.device)
+    L.check(L.lib().b2ctr_softmax_rows_bwd(ptr(y), y.stride(0), ptr(dy), dy.stride(0), ptr(dx), cols, rows, cols,
+                                           scale, stream()), "softmax_rows_bwd")
+    return dx
+
+
 # ---- head / loss / optimizers ---------------------------------------------------------------
 def predict_loss(logit, bias=None, labels=None, task=L.TASK_BINARY, want_grad=False):
     """Returns (pred[B], dlogit[B] | None, dbias[1] | None, loss_sum[1] | None)."""

@@ -129,7 +129,9 @@ class BiInteractionPooling(Layer):
 class FM(Layer):
     """Factorization Machine second-order term, deepctr/layers/interaction.py:563-607.
     [B,F,E] -> [B,1].  When the input is the fused gather's buffer the value comes out of the gather
-    kernel's epilogue (no extra pass over [B,F,E])."""
+    kernel's epilogue (no extra pass over [B,F,E]).  IFM / DIFM's refined input x * m reaches it as its two factors
+    (ops.ScaledFields) and runs the field-weighted FM: the product is never written."""
+    takes_scaled_fields = True
 
     def build(self, input_shape):
         if len(input_shape) != 3:
@@ -138,10 +140,10 @@ class FM(Layer):
         self.built = True
 
     def call(self, inputs, **kwargs):
-        if inputs.data.dim() != 3:
-            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs.data.dim()))
+        if len(inputs.shape) != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (len(inputs.shape)))
         planner = getattr(self, "_planner", None)
-        if planner is not None:
+        if planner is not None and not isinstance(inputs, ops.ScaledFields):
             fused = planner.lookup_fm(inputs)
             if fused is not None:
                 return fused

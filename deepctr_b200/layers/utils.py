@@ -230,10 +230,20 @@ class Linear(Layer):
 
 
 class RefineWeight(Layer):
-    """The Lambda of feature_column.py:193-195 (IFM / DIFM refine weights): x * expand_dims(w, 1)."""
+    """The Lambda of feature_column.py:193-200 (IFM / DIFM refine weights): the dim-1 linear lookups [B, 1, F_lin]
+    times expand_dims(m, 1) for m [B, F] (b2ctr_field_scale_fwd with dim 1).  F_lin must equal F: the reference
+    broadcasts when one of them is 1 and fails inside TensorFlow otherwise; here both are a ValueError at build time."""
+
+    def build(self, input_shape):
+        sparse, weight = input_shape
+        if len(weight) != 2 or int(sparse[-1]) != int(weight[-1]):
+            raise ValueError("sparse_feat_refine_weight has %s field weights but the linear part has %d sparse "
+                             "features: the two counts must be equal" % (weight[-1], int(sparse[-1])))
+        self.built = True
 
     def call(self, inputs, **kwargs):
-        raise NotImplementedError("sparse_feat_refine_weight (IFM/DIFM) is outside the hot path (SURVEY 8a a14)")
+        sparse, weight = inputs
+        return ops.field_scale(sparse, weight)
 
     def compute_output_shape(self, input_shape):
         return input_shape[0]

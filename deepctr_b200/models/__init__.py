@@ -9,5 +9,8 @@ from .fibinet import FiBiNET
 from .fwfm import FwFM
 from .deepfefm import DeepFEFM
 from .pnn import PNN
+from .ifm import IFM
+from .difm import DIFM
 
-__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM", "PNN"]
+__all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM", "PNN",
+           "IFM", "DIFM"]

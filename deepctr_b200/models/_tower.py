@@ -9,17 +9,26 @@ from ..layers.utils import add_func, combined_dnn_input, concat_func
 
 
 class Tower(object):
-    def __init__(self, input_columns, linear_columns, dnn_columns, seed, l2_linear, l2_embedding, grouped=False):
+    def __init__(self, input_columns, linear_columns, dnn_columns, seed, l2_linear, l2_embedding, grouped=False,
+                 defer_linear=False):
+        """``defer_linear``: the linear logit is not built here but by ``linear()``, after the embeddings (IFM / DIFM
+        reweight it with field weights computed from them)."""
         self.seed = seed
         self.features = build_input_features(input_columns)
         self.inputs = list(self.features.values())
-        self.linear_logit = get_linear_logit(self.features, linear_columns, seed=seed, prefix='linear',
-                                             l2_reg=l2_linear)
+        self._linear = (linear_columns, l2_linear)
+        self.linear_logit = None if defer_linear else self.linear()
         looked_up, self.dense_values = input_from_feature_columns(self.features, dnn_columns, l2_embedding, seed,
                                                                   support_group=grouped)
         self.groups = looked_up if grouped else None          # group name -> [B,1,E] tensors
         self.embeddings = [t for g in looked_up.values() for t in g] if grouped else looked_up
         self._flat = None
+
+    def linear(self, refine_weight=None):
+        """The first-order logit; ``refine_weight`` [B, F] scales the sparse lookups (sparse_feat_refine_weight)."""
+        columns, l2_reg = self._linear
+        return get_linear_logit(self.features, columns, seed=self.seed, prefix='linear', l2_reg=l2_reg,
+                                sparse_feat_refine_weight=refine_weight)
 
     def field_matrix(self, embeddings=None):
         """[B, F, E] stack of per-field embeddings (a zero-copy window of the fused gather's buffer)."""

@@ -384,7 +384,10 @@ def zeros_like_batch(x, cols=1):
 
 # ---- FM ------------------------------------------------------------------------------------------
 def fm(x):
-    """[B,F,E] -> [B,1]  (layers/interaction.py:597-602)."""
+    """[B,F,E] -> [B,1]  (layers/interaction.py:597-602).  A ``ScaledFields`` input runs the field-weighted FM on its
+    two factors (fm_weighted)."""
+    if isinstance(x, ScaledFields):
+        return fm_weighted(x.x, x.m)
     b, f, e = x.data.shape
     src, ld = x.flat2d()
     if src is None:
@@ -401,6 +404,108 @@ def fm(x):
         E.add_grad(x, dx.reshape(x.data.shape))
 
     E.record([res], [x], bwd)
+    return res
+
+
+# ---- field weights (IFM / DIFM) -------------------------------------------------------------------
+class ScaledFields(E.Var):
+    """The refine product x * expand_dims(m, -1) of IFM / DIFM (ifm.py:66-67, difm.py:74-75), kept as its two
+    factors x [B,F,E] and m [B,F]: FM consumes them directly (fm_weighted), every other layer receives the
+    materialised product (``product``, called by engine.Layer._invoke)."""
+    __slots__ = ("x", "m", "_product")
+
+    def __init__(self, x, m):
+        E.Var.__init__(self, None, requires_grad=x.requires_grad or m.requires_grad, vshape=tuple(x.shape))
+        self.x, self.m, self._product = x, m, None
+
+    def product(self):
+        if self._product is None:
+            self._product = field_scale(self.x, self.m)
+        return self._product
+
+
+def scale_fields(x, m):
+    """[B,F,E] x, [B,F] m -> x * m[:, :, None], deferred (``ScaledFields``): nothing is computed here."""
+    if len(x.shape) != 3 or tuple(m.shape) != (x.shape[0], x.shape[1]):
+        raise ValueError("scale_fields: x must be [B, F, E] and m [B, F], got %s and %s"
+                         % (tuple(x.shape), tuple(m.shape)))
+    return ScaledFields(x, m)
+
+
+def _m2d(m, b, f):
+    t = m.data
+    if t.dim() == 2 and t.shape == (b, f) and t.stride(1) == 1:
+        return t
+    return E.contiguous(m).reshape(b, f)
+
+
+def _grad_window(x, w):
+    """(2-D view to write x's gradient into, accumulate) when x is a column window of a [B, ld] buffer: its slice of
+    the buffer's gradient (added to when that exists; adopted as it, like engine.add_grad does, when x covers every
+    used column), else (None, False)."""
+    base = x.base
+    if base is None or x.ncols == -1 or base.data is None or base.data.dim() != 2:
+        return None, False
+    if base.grad is not None:
+        return base.grad[:, x.col0:x.col0 + w], True
+    used = base.ncols if base.ncols > 0 else base.data.shape[1]
+    if x.col0 == 0 and w >= used:
+        base.grad = torch.empty_like(base.data)
+        base.requires_grad = True
+        return base.grad[:, :w], False
+    return None, False
+
+
+def fm_weighted(x, m):
+    """[B,F,E] x, [B,F] m -> [B,1]: FM of m ⊙ x without writing m ⊙ x (b2ctr_fm_weighted_fwd).  x is read in place;
+    the backward writes dx straight into the gather buffer's gradient when x is a window of it."""
+    b, f, e = x.data.shape
+    src, ld = _fields2d(x)
+    md = _m2d(m, b, f)
+    res = E.Var(K.fm_weighted_fwd(src, ld, md, f, e, b).reshape(b, 1))
+
+    def bwd(grads):
+        g = grads[0].reshape(b).contiguous()
+        dxw, acc = _grad_window(x, f * e) if x.requires_grad else (None, False)
+        dx, dm = K.fm_weighted_bwd(src, ld, md, f, e, g, b, dx=dxw, accumulate=acc, want_dx=x.requires_grad,
+                                   want_dm=m.requires_grad)
+        if x.requires_grad and dxw is None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        if dm is not None:
+            E.add_grad(m, dm)
+
+    E.record([res], [x, m], bwd)
+    return res
+
+
+def field_scale(x, m):
+    """x * m over fields: x's per-sample values are F = m.shape[1] fields of dim values each ([B,F,E] for the FM
+    input, [B,1,F] with dim 1 for the linear lookups of get_linear_logit).  Materialised, same shape as x."""
+    b, f = m.shape
+    src, ld = x.flat2d()
+    if src is None:
+        src = E.contiguous(x).reshape(b, -1)
+        ld = src.stride(0)
+    w = src.shape[1]
+    if w % f:
+        raise ValueError("field_scale: %d values per sample are not %d fields" % (w, f))
+    dim = w // f
+    md = _m2d(m, b, f)
+    res = E.Var(K.field_scale_fwd(src, ld, md, f, dim, b).reshape(x.data.shape))
+
+    def bwd(grads):
+        g = grads[0].reshape(b, w)
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dxw, acc = _grad_window(x, w) if x.requires_grad else (None, False)
+        dx, dm = K.field_scale_bwd(g, src, ld, md, f, dim, b, dx=dxw, accumulate=acc, want_dx=x.requires_grad,
+                                   want_dm=m.requires_grad)
+        if x.requires_grad and dxw is None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        if dm is not None:
+            E.add_grad(m, dm)
+
+    E.record([res], [x, m], bwd)
     return res
 
 
@@ -1355,5 +1460,22 @@ def div(x, y):
     raise NotImplementedError("div is only used inside SequencePoolingLayer, which has its own kernel")
 
 
-def softmax(x, dim=-1):
-    raise NotImplementedError("softmax is only used inside attention layers, which have their own kernels")
+def softmax(x, dim=-1, scale=1.0):
+    """scale * softmax(x) along the last axis of a 2-D x (layers/utils.py:306-310; IFM's F * softmax(z, dim=1),
+    ifm.py:60) on b2ctr_softmax_rows_fwd / _bwd.  Other ranks and axes: NotImplementedError."""
+    if x.data.dim() != 2 or dim not in (-1, 1):
+        raise NotImplementedError("softmax over axis %r of a %d-D tensor: only the last axis of a 2-D tensor is "
+                                  "supported" % (dim, x.data.dim()))
+    x2, _ = _as2d(x)
+    scale = float(scale)
+    y = K.softmax_rows_fwd(x2, scale)
+    res = E.Var(y)
+
+    def bwd(grads):
+        g = grads[0].reshape(y.shape)
+        if g.stride(1) != 1:
+            g = g.contiguous()
+        E.add_grad(x, K.softmax_rows_bwd(y, g, scale))
+
+    E.record([res], [x], bwd)
+    return res

@@ -291,6 +291,39 @@ B2CTR_API b2ctr_status_t b2ctr_fm_fwd(const float* x, int64_t ldx, int32_t nfiel
 B2CTR_API b2ctr_status_t b2ctr_fm_bwd(const float* x, int64_t ldx, int32_t nfield, int32_t dim,
                                      const float* dout, float* dx, int64_t lddx, int32_t accumulate,
                                      int64_t batch, void* stream);
+/* FM of the field-weighted input m ⊙ x (IFM / DIFM: FM(refined embeddings), deepctr/models/ifm.py:66-68) without
+ * writing m ⊙ x.  x [B, nfield, dim] (row pitch ldx), m [B, nfield] (row pitch ldm):
+ *   out[b] = 1/2 sum_e [(sum_f m_bf x_bfe)^2 - sum_f m_bf^2 x_bfe^2]
+ * Backward, with S_be = sum_f m_bf x_bfe:
+ *   dx_bfe = g_b m_bf (S_be - m_bf x_bfe)       (pitch lddx; added to dx when accumulate; may be NULL)
+ *   dm_bf  = g_b sum_e x_bfe (S_be - m_bf x_bfe) (pitch lddm, overwritten; may be NULL)
+ * Same launch shape and limits as b2ctr_fm_fwd / _bwd; with m == 1 the results equal theirs bit for bit.  No float
+ * atomics: bit-identical from run to run. */
+B2CTR_API b2ctr_status_t b2ctr_fm_weighted_fwd(const float* x, int64_t ldx, const float* m, int64_t ldm,
+                                              int32_t nfield, int32_t dim, float* out, int64_t batch, void* stream);
+B2CTR_API b2ctr_status_t b2ctr_fm_weighted_bwd(const float* x, int64_t ldx, const float* m, int64_t ldm,
+                                              int32_t nfield, int32_t dim, const float* dout, float* dx, int64_t lddx,
+                                              int32_t accumulate, float* dm, int64_t lddm, int64_t batch,
+                                              void* stream);
+/* Materialised field scale (RefineWeight of get_linear_logit, feature_column.py:193-200, with dim = 1; the refine
+ * product when its consumer is not FM):  y[b, f*dim + e] = x[b, f*dim + e] * m[b, f]   (pitches ldx, ldm, ldy).
+ * Backward: dx = dy * m (pitch lddx; added when accumulate; may be NULL), dm[b, f] = sum_e dy x (pitch lddm,
+ * overwritten; may be NULL), summed in a fixed order: bit-identical from run to run. */
+B2CTR_API b2ctr_status_t b2ctr_field_scale_fwd(const float* x, int64_t ldx, const float* m, int64_t ldm,
+                                              int32_t nfield, int32_t dim, float* y, int64_t ldy, int64_t batch,
+                                              void* stream);
+B2CTR_API b2ctr_status_t b2ctr_field_scale_bwd(const float* dy, int64_t lddy, const float* x, int64_t ldx,
+                                              const float* m, int64_t ldm, int32_t nfield, int32_t dim, float* dx,
+                                              int64_t lddx, int32_t accumulate, float* dm, int64_t lddm,
+                                              int64_t batch, void* stream);
+/* y = scale * softmax(x) along the rows of a [rows, cols] window (layers/utils.py softmax on the last axis; IFM
+ * uses scale = F).  The row maximum is subtracted first.  Backward: dx = y * (dy - sum_j y_j dy_j / scale),
+ * overwritten.  scale must not be 0. */
+B2CTR_API b2ctr_status_t b2ctr_softmax_rows_fwd(const float* x, int64_t ldx, float* y, int64_t ldy, int64_t rows,
+                                               int32_t cols, float scale, void* stream);
+B2CTR_API b2ctr_status_t b2ctr_softmax_rows_bwd(const float* y, int64_t ldy, const float* dy, int64_t lddy,
+                                               float* dx, int64_t lddx, int64_t rows, int32_t cols, float scale,
+                                               void* stream);
 
 /* ------------------------------------------------------------------------------------------ */
 /* 4. Prediction head, loss, optimizers                                                         */

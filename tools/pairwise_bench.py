@@ -6,6 +6,7 @@ that shape.
     python tools/pairwise_bench.py [--steps 20] [--warmup 5] [--reps 50] [--models NFM,AFM,FiBiNET]
     python tools/pairwise_bench.py --models FwFM,DeepFEFM
     python tools/pairwise_bench.py --models PNN
+    python tools/pairwise_bench.py --models IFM,DIFM
 
 Prints one JSON line per measurement:
   * the hardware context (card, power limit, max SM clock), read in the same run;
@@ -20,7 +21,10 @@ Prints one JSON line per measurement:
     training steps of FwFM and DeepFEFM with their default (256, 128, 64) DNN;
   * with PNN (not in the default set): b2ctr_pnn_inner_* (inner, vec, num) and b2ctr_pnn_outer_* (mat) against the
     same two bounds, and the training steps of IPNN (the default), OPNN with kernel_type 'mat' and both products,
-    with the (256, 128, 64) DNN.
+    with the (256, 128, 64) DNN;
+  * with IFM / DIFM (not in the default set): b2ctr_fm_weighted_*, b2ctr_field_scale_* (E = 32 and the linear term's
+    E = 1) and b2ctr_softmax_rows_* against the HBM bound, and the training steps of IFM and DIFM (13 dense features,
+    (256, 128, 64) DNN).
 """
 import argparse
 import json
@@ -73,6 +77,8 @@ def step_time(builder, steps, warmup):
         model = M.DeepFEFM(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding_feat=0)
     elif builder.startswith("PNN"):
         model = M.PNN(cols, dnn_hidden_units=(256, 128, 64), l2_reg_embedding=0, **PNN_STEPS[builder])
+    elif builder in ("IFM", "DIFM"):
+        model = getattr(M, builder)(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding=0)
     elif builder == "FiBiNET":
         model = M.FiBiNET(cols, cols, bilinear_type="interaction", dnn_hidden_units=(256, 128, 64), l2_reg_linear=0,
                           l2_reg_embedding=0)
@@ -317,6 +323,55 @@ def pnn_kernels(reps, hw):
     return out
 
 
+def ifm_kernels(reps, hw):
+    """IFM / DIFM's field-weight kernels at C2 (26 fields, E = 32, B = 65536), x a window of the [B, 848] gather
+    buffer: the field-weighted FM (backward with and without accumulate into the buffer's gradient), the
+    materialised field scale at E = 32 (what the deferred FM avoids) and at E = 1 (the linear term), and IFM's
+    F * softmax over [B, 26]."""
+    import torch
+    from deepctr_b200 import kernels as K
+    B, F, E, nd = 65536, 26, 32, 13
+    dev = torch.device("cuda", 0)
+    g = torch.Generator(device=dev).manual_seed(5)
+    clk = hw.get("max_sm_clock_mhz") or None
+    ffma_peak = 132 * 128 * 2 * clk * 1e6 if clk else None
+    ldx = (F * E + nd + 3) // 4 * 4
+    buf = torch.randn((B, ldx), device=dev, generator=g) * 0.1
+    dbuf = torch.randn((B, ldx), device=dev, generator=g)
+    xw, dxw = buf[:, :F * E], dbuf[:, :F * E]
+    m = torch.randn((B, F), device=dev, generator=g)
+    go = torch.randn((B,), device=dev, generator=g)
+    x_bytes, m_bytes = B * F * E * 4, B * F * 4
+    shape = dict(B=B, F=F, E=E, ldx=ldx)
+    out = [_report("fm_weighted_fwd", shape, reps, lambda: K.fm_weighted_fwd(xw, ldx, m, F, E, B),
+                   B * F * E * 4, x_bytes + m_bytes + B * 4, ffma_peak),
+           _report("fm_weighted_bwd", shape, reps, lambda: K.fm_weighted_bwd(xw, ldx, m, F, E, go, B, dx=dxw),
+                   B * F * E * 8, 2 * x_bytes + 2 * m_bytes + B * 4, ffma_peak),
+           _report("fm_weighted_bwd_accumulate", shape, reps,
+                   lambda: K.fm_weighted_bwd(xw, ldx, m, F, E, go, B, dx=dxw, accumulate=True),
+                   B * F * E * 8, 3 * x_bytes + 2 * m_bytes + B * 4, ffma_peak)]
+    y = K.field_scale_fwd(xw, ldx, m, F, E, B)
+    out += [_report("field_scale_fwd", shape, reps, lambda: K.field_scale_fwd(xw, ldx, m, F, E, B, out=y),
+                    B * F * E, 2 * x_bytes + m_bytes, ffma_peak),
+            _report("field_scale_bwd", shape, reps, lambda: K.field_scale_bwd(y, xw, ldx, m, F, E, B, dx=dxw),
+                    B * F * E * 3, 3 * x_bytes + 2 * m_bytes, ffma_peak)]
+    lin = torch.randn((B, 28), device=dev, generator=g)
+    shape1 = dict(B=B, F=F, E=1, ldx=28)
+    out += [_report("field_scale_fwd_e1", shape1, reps, lambda: K.field_scale_fwd(lin, 28, m, F, 1, B),
+                    B * F, 3 * m_bytes, ffma_peak),
+            _report("field_scale_bwd_e1", shape1, reps, lambda: K.field_scale_bwd(m, lin, 28, m, F, 1, B),
+                    B * F * 3, 5 * m_bytes, ffma_peak)]
+    sm = K.softmax_rows_fwd(m, float(F))
+    shape_s = dict(B=B, C=F)
+    out += [_report("softmax_rows_fwd", shape_s, reps, lambda: K.softmax_rows_fwd(m, float(F)), B * F * 5,
+                    2 * m_bytes, ffma_peak),
+            _report("softmax_rows_bwd", shape_s, reps, lambda: K.softmax_rows_bwd(sm, m, float(F)), B * F * 4,
+                    3 * m_bytes, ffma_peak)]
+    del buf, dbuf, y
+    torch.cuda.empty_cache()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -343,6 +398,9 @@ def main():
         for r in pnn_kernels(args.reps, hw):
             print(json.dumps(r), flush=True)
         models = [m for m in models if m != "PNN"] + list(PNN_STEPS)
+    if "IFM" in models or "DIFM" in models:
+        for r in ifm_kernels(args.reps, hw):
+            print(json.dumps(r), flush=True)
     for builder in models:
         print(json.dumps(step_time(builder, args.steps, args.warmup)), flush=True)
 
