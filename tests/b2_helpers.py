@@ -1,4 +1,4 @@
-"""Shared test helpers: synthetic CTR data and model -> oracle weight extraction."""
+"""Shared test helpers: synthetic CTR data and training runs, GPU logits and tolerances, oracle weights."""
 import numpy as np
 import torch
 
@@ -12,6 +12,68 @@ def criteo_like(rng, n, n_sparse=6, n_dense=3, vocab=50, dim=8, dtype="int32"):
     x.update({"I%d" % i: rng.rand(n).astype(np.float32) for i in range(n_dense)})
     y = (rng.rand(n) < 0.3).astype(np.float32)
     return cols, x, y
+
+
+def criteo_model(builder, rng, n_dense=3, **kw):
+    """``builder`` over criteo_like's 10 sparse columns (vocabulary 50 + i, dim 8) and ``n_dense`` dense ones, with
+    l2 = 0 and seed 3, and a batch of 512 drawn from ``rng``: (model, x, y)."""
+    from deepctr_b200 import engine as E, models as M
+    cols, x, y = criteo_like(rng, 512, n_sparse=10, n_dense=n_dense)
+    E.clear_session()
+    if builder == "PNN":                      # PNN(dnn_feature_columns, ...): no linear part
+        return M.PNN(cols, l2_reg_embedding=0, seed=3, **kw), x, y
+    l2 = "l2_reg_embedding_feat" if builder == "DeepFEFM" else "l2_reg_embedding"
+    return getattr(M, builder)(cols, cols, l2_reg_linear=0, seed=3, **{l2: 0}, **kw), x, y
+
+
+def train(builder, graph, kw, placed=True, steps=6, init=None):
+    """``steps`` SGD steps of criteo_model(builder, RandomState(4), **kw), built with the DNN-input placement on or
+    off, from ``init`` or from the built model's weights: (losses, {name: weight}, replayed launches, init)."""
+    from deepctr_b200 import inputs as I
+    from deepctr_b200.engine import SGD
+    I.DNN_INPUT_PLACEMENT = placed
+    try:
+        model, x, y = criteo_model(builder, np.random.RandomState(4), **kw)
+    finally:
+        I.DNN_INPUT_PLACEMENT = True
+    if builder == "FiBiNET":
+        assert bool(model.planner.dnn_places) == placed
+    elif builder == "PNN":
+        products = kw.get("use_inner", True) or kw.get("use_outter", False)
+        assert bool(model.planner.pnn_places) == (placed and products)
+    if init is None:            # Keras leaves the Dense kernels unseeded: start every run from the same weights
+        init = [w.value() for w in model.weights]
+    else:
+        model.set_weights(init)
+    model.compile(SGD(0.05), "binary_crossentropy", embedding_update="sparse", step_graph=graph)
+    losses = [model.train_on_batch(x, y) for _ in range(steps)]
+    return losses, {w.name: w.value() for w in model.weights}, model.replayed_launches, init
+
+
+def logits(model, x):
+    """pre-activation logits of the compiled graph (what PredictionLayer receives)."""
+    from deepctr_b200 import engine as E
+    model._materialize()
+    feed = model._feed(x)
+    logit_t, head = model._head()
+    vals = model._run(feed, False, upto=head)
+    return E.contiguous(vals[id(logit_t)]).reshape(-1, 1).cpu().numpy()
+
+
+def logit_tol(want):
+    """absolute tolerance of a GPU model's logits or predictions in the current GEMM precision."""
+    from deepctr_b200 import ops, _lib as L
+    scale = max(float(np.abs(want).max()), 1e-3)
+    return (1e-4 if ops.GEMM_PRECISION == L.GEMM_BF16X3 else 2e-5) * scale
+
+
+def close(got, want, what, tol=2e-5, floor=0.0):
+    """Max error relative to max |want|, or to ``floor`` when that is larger: the magnitude of the terms whose
+    difference a kernel forms where the result cancels to about 0.  Takes numpy arrays or torch tensors."""
+    got, want = torch.as_tensor(got).double(), torch.as_tensor(want).double()
+    scale = max(float(want.abs().max()), float(floor), 1e-30)
+    err = float((got - want).abs().max()) / scale
+    assert err < tol, "%s: max error %.3e relative to max |value|" % (what, err)
 
 
 def randomize_weights(model, rng, std=0.1):

@@ -219,20 +219,19 @@ def fixtures():
 def builders():
     """The graphs the reference's bst.py SOURCE builds on this package for the model fixtures, and its defaults."""
     import generate_builders as GB
-    import test_reference_builders_dropin as D
-    import test_bst_goldens as BG
+    import golden_models as G
     from deepctr_b200 import engine as E
     out = {"signatures": {}, "defaults": {}}
     GB._FILES["BST"] = ("models/sequence/bst.py", "models.sequence.bst")
     with GB._aliased():
         build = GB._reference_builder(REF + "/deepctr", "BST")
-        for name in BG.MODEL_CASES:
-            fx = BG.Fixture(name)
-            args, kw = BG.builder_args(fx)
+        for name in G.FAMILIES["bst"].cases:
+            fx = G.FAMILIES["bst"].fixture(name)
+            args, kw = G.builder_args(fx)
             E.clear_session()
             model = build(*args, **kw)
-            BG.weight_map(fx, model)
-            out["signatures"][name] = D.signature(model)
+            G.weight_map(fx, model)
+            out["signatures"][name] = G.signature(model)
         out["defaults"]["BST"] = [[k, repr(p.default)] for k, p in inspect.signature(build).parameters.items()]
     E.clear_session()
     with open(BUILDERS_JSON, "w") as f:

@@ -26,7 +26,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.dirname(HERE))
 
 import golden_models as G  # noqa: E402
-from test_reference_builders_dropin import BUILDERS, signature, builder_args  # noqa: E402
+from golden_models import signature, builder_args  # noqa: E402
 
 _FILES = {"DeepFM": ("models/deepfm.py", "models.deepfm"), "xDeepFM": ("models/xdeepfm.py", "models.xdeepfm"),
           "DCN": ("models/dcn.py", "models.dcn"), "AutoInt": ("models/autoint.py", "models.autoint"),
@@ -97,7 +97,7 @@ def main(ref):
             model = build(*args, **kw)
             G.weight_map(fx, model)          # the reference-built graph carries the fixture's weights by name
             out["signatures"][name] = signature(model)
-        for name in BUILDERS:
+        for name in G.FAMILIES["models"].builders:
             sig = inspect.signature(_reference_builder(ref, name))
             out["defaults"][name] = [[k, repr(p.default)] for k, p in sig.parameters.items()]
     E.clear_session()

@@ -107,7 +107,7 @@ def fixtures():
 def builders():
     import golden_models as G
     import generate_builders as GB
-    from test_reference_builders_dropin import signature, builder_args
+    from golden_models import signature, builder_args
     from deepctr_b200 import engine as E
     out = {"signatures": {}, "defaults": {}}
     names = sorted(os.path.basename(p)[:-4] for p in os.listdir(MODEL_OUT) if p.endswith(".npz"))

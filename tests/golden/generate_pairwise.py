@@ -169,7 +169,7 @@ def fixtures():
 def builders():
     import golden_models as G
     import generate_builders as GB
-    from test_reference_builders_dropin import signature, builder_args
+    from golden_models import signature, builder_args
     from deepctr_b200 import engine as E
     from deepctr_b200.layers.normalization import Dropout
     out = {"signatures": {}, "defaults": {}}

@@ -1,6 +1,6 @@
-"""Shared loader for the MODEL-level golden fixtures (tests/golden/models/*.npz, produced by the
+"""Shared loader for the MODEL-level golden fixtures (tests/golden/models*/*.npz, produced by the
 reference's own feature_column.py / inputs.py / builders under the TF shim: see
-tests/golden/generate_models.py) and the two mappings a test needs:
+tests/golden/generate_*.py), the table of fixture families, and the mappings a test needs:
 
 * ``oracle_weights``  fixture weight keys -> the dict oracle/models.py takes;
 * ``assign_weights``  fixture weight keys -> the weights of a deepctr_b200 model built from the same columns.
@@ -11,19 +11,28 @@ Key convention of the fixtures: ``<top-level layer name>/<reference attribute pa
 neither the oracle nor this package materialises them.
 """
 import glob
+import itertools
 import json
 import os
+import re
 
 import numpy as np
 import torch
 
-MODELS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "models")
-CASES = sorted(os.path.basename(p)[:-4] for p in glob.glob(os.path.join(MODELS, "*.npz")))
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+MODELS = os.path.join(GOLDEN, "models")
+
+
+def _cases(models_dir):
+    return sorted(os.path.basename(p)[:-4] for p in glob.glob(os.path.join(models_dir, "*.npz")))
+
+
+CASES = _cases(MODELS)
 
 
 class Fixture(object):
-    def __init__(self, name):
-        d = np.load(os.path.join(MODELS, name + ".npz"))
+    def __init__(self, name, models_dir=MODELS):
+        d = np.load(os.path.join(models_dir, name + ".npz"))
         self.name = name
         self.meta = json.loads(str(d["meta"]))
         self.x = {k[2:]: d[k] for k in d.files if k.startswith("x_")}
@@ -75,9 +84,7 @@ def oracle_weights(fx, requires_grad=False):
     leaves = {}
 
     def t(key):
-        v = torch.tensor(fx.w[key], requires_grad=requires_grad and key in fx.g)
-        leaves[key] = v
-        return v
+        return _leaf(fx, leaves, key, requires_grad)
 
     W = {"tables": {}, "att": []}
     for name in fx.layer_names("Embedding"):
@@ -131,9 +138,10 @@ def oracle_weights(fx, requires_grad=False):
     return W, leaves
 
 
-def oracle_forward(fx, W, FC):
+def oracle_forward(fx, W):
     """(logit, prediction) of oracle/models.py for this fixture's builder + kwargs."""
     from oracle import models as OM
+    from deepctr_b200 import feature_column as FC
     kw = fx.kwargs
     x = fx.inputs()
     lin, dnn = columns(fx, "linear", FC), columns(fx, "dnn", FC)
@@ -170,20 +178,40 @@ def loss_of(fx, pred):
 _RENAMES = [("/local_att/", "/local_activation_unit/"), ("/activation_layers", "/act")]
 
 
-def build_model(fx):
-    """Build the deepctr_b200 model of this fixture (graph construction only: works without a GPU)."""
-    from deepctr_b200 import engine as E
+def builder_args(fx):
+    """(positional, keyword) arguments of the fixture's builder call."""
     from deepctr_b200 import feature_column as FC
-    from deepctr_b200 import models as M
-    E.clear_session()
     kw = dict(fx.kwargs)
     for k in ("dnn_hidden_units", "cin_layer_size", "att_hidden_size", "fm_group"):
         if k in kw:
             kw[k] = tuple(kw[k])
-    lin, dnn = columns(fx, "linear", FC), columns(fx, "dnn", FC)
-    if fx.builder == "DIN":
-        return M.DIN(dnn, ["item_id", "cate_id"], **kw)
-    return getattr(M, fx.builder)(lin, dnn, **kw)
+    dnn = columns(fx, "dnn", FC)
+    if fx.builder in ("DIN", "BST"):
+        return (dnn, ["item_id", "cate_id"]), kw
+    if fx.builder == "PNN":                  # PNN(dnn_feature_columns, **kwargs) (pnn.py:18)
+        return (dnn,), kw
+    return (columns(fx, "linear", FC), dnn), kw
+
+
+def build(fx):
+    """Build the deepctr_b200 model of this fixture (graph construction only: works without a GPU)."""
+    from deepctr_b200 import engine as E
+    from deepctr_b200 import models as M
+    args, kw = builder_args(fx)
+    E.clear_session()
+    return getattr(M, fx.builder)(*args, **kw)
+
+
+def signature(model):
+    """What reference_builders*.json records of a built graph: inputs, layers, weights, planner slots."""
+    from deepctr_b200 import engine as E
+    layers = [(type(l).__name__, l.name) for l in model.layers if not isinstance(l, E.InputLayer)]
+    weights = [(w.name, tuple(w.shape), w.trainable) for w in model.weights]
+    slots = [(s.emb.name, s.input_name, s.maxlen, s.pool, s.mask_mode, s.len_name, s.weight_name, s.weight_mode,
+              s.dim, s.buf, s.col) for s in model.planner.slots]
+    sig = {"inputs": list(model.input_names), "layers": layers, "weights": weights, "slots": slots,
+           "fast": (model.planner.fast, getattr(model.planner, "fast_n", 0))}
+    return json.loads(json.dumps(sig))      # tuples -> lists, as stored
 
 
 def weight_map(fx, model):
@@ -212,3 +240,221 @@ def assign_weights(fx, model):
     for key, w in wm.items():
         w.set_value(fx.w[key])
     return wm
+
+
+# ---- the fixture families -----------------------------------------------------------------------------
+def _leaf(fx, leaves, key, requires_grad):
+    v = torch.tensor(fx.w[key], requires_grad=requires_grad and key in fx.g)
+    leaves[key] = v
+    return v
+
+
+def _pairwise_weights(fx, requires_grad=False):
+    """oracle_weights plus the AFMLayer weights (one dict per layer, in graph order)."""
+    W, leaves = oracle_weights(fx, requires_grad)
+    W["afm"] = [{k: _leaf(fx, leaves, "%s/%s" % (name, k), requires_grad)
+                 for k in ("attention_W", "attention_b", "projection_h", "projection_p")}
+                for name in fx.layer_names("AFMLayer")]
+    return W, leaves
+
+
+def _pairwise_forward(fx, W):
+    import pairwise_oracle as PO
+    from deepctr_b200 import feature_column as FC
+    x = fx.inputs()
+    lin, dnn = columns(fx, "linear", FC), columns(fx, "dnn", FC)
+    if fx.builder == "NFM":
+        return PO.nfm(x, lin, dnn, W, task=fx.task)
+    kw = fx.kwargs
+    fm_group = kw.get("fm_group", "default_group")
+    return PO.afm_model(x, lin, dnn, W, fm_group=tuple(fm_group) if isinstance(fm_group, list) else fm_group,
+                        use_attention=kw.get("use_attention", True), task=fx.task)
+
+
+def _creation_order(name):
+    m = re.search(r"_(\d+)$", name)
+    return int(m.group(1)) if m else 0
+
+
+def _fibinet_weights(fx, requires_grad=False):
+    """oracle_weights plus the SENET weights and the two bilinear layers' weights (SENET branch first: the layer
+    created first)."""
+    W, leaves = oracle_weights(fx, requires_grad)
+    senet = fx.layer_names("SENETLayer")[0]
+    W["senet"] = (_leaf(fx, leaves, senet + "/W_1", requires_grad), _leaf(fx, leaves, senet + "/W_2", requires_grad))
+    W["bilinear"] = [[_leaf(fx, leaves, k, requires_grad) for k in fx.w if k.startswith(name + "/bilinear_weight")]
+                     for name in sorted(fx.layer_names("BilinearInteraction"), key=_creation_order)]
+    W.setdefault("dnn_kernels", [])
+    W.setdefault("dnn_biases", [])
+    return W, leaves
+
+
+def _fibinet_forward(fx, W):
+    import fibinet_oracle as FO
+    from deepctr_b200 import feature_column as FC
+    lin, dnn = columns(fx, "linear", FC), columns(fx, "dnn", FC)
+    return FO.fibinet(fx.inputs(), lin, dnn, W, bilinear_type=fx.kwargs.get("bilinear_type", "interaction"),
+                      task=fx.task)
+
+
+def _fefm_weights(fx, requires_grad=False):
+    """oracle_weights plus W['fwfm'] (each FwFMLayer's strengths, in creation order) or W['fefm'] (the FEFMLayer's
+    P matrices, in itertools.combinations order)."""
+    W, leaves = oracle_weights(fx, requires_grad)
+    W["fwfm"] = [_leaf(fx, leaves, n + "/field_pair_strengths", requires_grad) for n in fx.layer_names("FwFMLayer")]
+    for n in fx.layer_names("FEFMLayer"):
+        F = int(round((1 + np.sqrt(1 + 8 * len([k for k in fx.w if k.startswith(n + "/")]))) / 2))
+        W["fefm"] = [_leaf(fx, leaves, "%s/field_embeddings%d-%d" % (n, i, j), requires_grad)
+                     for i, j in itertools.combinations(range(F), 2)]
+    return W, leaves
+
+
+def _fefm_forward(fx, W):
+    import fefm_oracle as FO
+    from deepctr_b200 import feature_column as FC
+    lin, dnn = columns(fx, "linear", FC), columns(fx, "dnn", FC)
+    kw = fx.kwargs
+    if fx.builder == "FwFM":
+        return FO.fwfm_model(fx.inputs(), lin, dnn, W, fm_group=tuple(kw.get("fm_group", ("default_group",))),
+                             task=fx.task)
+    return FO.deepfefm(fx.inputs(), lin, dnn, W, use_fefm=kw.get("use_fefm", True),
+                       use_linear=kw.get("use_linear", True),
+                       use_fefm_embed_in_dnn=kw.get("use_fefm_embed_in_dnn", True),
+                       exclude_feature_embed_in_dnn=kw.get("exclude_feature_embed_in_dnn", False), task=fx.task)
+
+
+def _pnn_weights(fx, requires_grad=False):
+    """oracle_weights plus W['outer'], the OutterProductLayer kernel when it is on the output path."""
+    W, leaves = oracle_weights(fx, requires_grad)
+    for n in fx.layer_names("OutterProductLayer"):
+        W["outer"] = _leaf(fx, leaves, n + "/kernel", requires_grad)
+    return W, leaves
+
+
+def _pnn_forward(fx, W):
+    import pnn_oracle as PO
+    from deepctr_b200 import feature_column as FC
+    kw = fx.kwargs
+    return PO.pnn(fx.inputs(), columns(fx, "dnn", FC), W, use_inner=kw.get("use_inner", True),
+                  use_outter=kw.get("use_outter", False), kernel_type=kw.get("kernel_type", "mat"), task=fx.task)
+
+
+def _ifm_weights(fx, requires_grad=False):
+    """oracle_weights plus W['m_kernels'], the Dense(F) kernels in creation order."""
+    W, leaves = oracle_weights(fx, requires_grad)
+    W["m_kernels"] = [leaves[n + "/kernel"] if n + "/kernel" in leaves else
+                      _leaf(fx, leaves, n + "/kernel", requires_grad) for n in fx.layer_names("Dense")]
+    return W, leaves
+
+
+def _ifm_forward(fx, W):
+    import ifm_oracle as IO
+    from deepctr_b200 import feature_column as FC
+    kw = fx.kwargs
+    args = (fx.inputs(), columns(fx, "linear", FC), columns(fx, "dnn", FC), W)
+    if fx.builder == "IFM":
+        return IO.ifm(*args, task=fx.task)
+    return IO.difm(*args, att_embedding_size=kw.get("att_embedding_size", 8), att_head_num=kw.get("att_head_num", 8),
+                   att_res=kw.get("att_res", True), task=fx.task)
+
+
+def _bst_weights(fx, requires_grad=False):
+    """The dict tests/bst_oracle.py takes; every fixture weight is a leaf."""
+    leaves = {k: torch.tensor(v, requires_grad=requires_grad) for k, v in fx.w.items()}
+    tables = {k.split("/")[0][len("sparse_emb_"):]: v for k, v in leaves.items() if k.endswith("/embeddings")}
+    trs = []
+    for name in fx.layer_names("Transformer"):
+        trs.append({k[len(name) + 1:]: v for k, v in leaves.items() if k.startswith(name + "/")})
+    p = fx.layer_names("AttentionSequencePoolingLayer")[0] + "/local_att/"
+    n = len([k for k in leaves if k.startswith(p + "dnn/kernel")])
+    lau = {"dnn_kernels": [leaves["%sdnn/kernel%d" % (p, i)] for i in range(n)],
+           "dnn_biases": [leaves["%sdnn/bias%d" % (p, i)] for i in range(n)],
+           "kernel": leaves[p + "kernel"], "bias": leaves[p + "bias"]}
+    dnn = fx.layer_names("DNN")[-1]
+    m = len([k for k in leaves if k.startswith(dnn + "/kernel")])
+    W = {"tables": tables, "transformers": trs, "lau": lau,
+         "dnn_kernels": [leaves["%s/kernel%d" % (dnn, i)] for i in range(m)],
+         "dnn_biases": [leaves["%s/bias%d" % (dnn, i)] for i in range(m)],
+         "dense_kernel": leaves[fx.layer_names("Dense")[-1] + "/kernel"],
+         "global_bias": leaves[fx.layer_names("PredictionLayer")[-1] + "/global_bias"]}
+    return W, leaves
+
+
+def _bst_forward(fx, W):
+    import bst_oracle as BO
+    from deepctr_b200 import feature_column as FC
+    kw = fx.kwargs
+    return BO.bst(fx.inputs(), columns(fx, "dnn", FC), ["item_id", "cate_id"], W,
+                  transformer_num=kw.get("transformer_num", 1), att_head_num=kw.get("att_head_num", 8))
+
+
+class Family(object):
+    """One directory of model fixtures, the builders that made them and the oracle that restates them.
+
+    ``n_cases``, ``builders`` and ``tasks`` are what the fixture set holds.  The flags keep what legitimately differs
+    between families:
+
+    * ``graph_weight_order``: fixtures whose model lists its weights in graph order, which differs from the reference's
+      creation order (the graph order itself is pinned against the reference-built graph);
+    * ``placed``: the builders write their products into the DNN input in place, so the GPU fixture tests run with and
+      without that placement;
+    * ``predict_atol``: the absolute tolerance of the GPU predictions, where the family has its own.
+    """
+
+    def __init__(self, subdir, builders_json, builders, oracle_weights, oracle_forward, n_cases, tasks,
+                 graph_weight_order=(), placed=False, predict_atol=None):
+        self.models_dir = os.path.join(GOLDEN, subdir)
+        self.cases = _cases(self.models_dir)
+        self.builders_json = os.path.join(GOLDEN, builders_json)
+        self.builders = builders
+        self.oracle_weights, self.oracle_forward = oracle_weights, oracle_forward
+        self.n_cases, self.tasks = n_cases, tasks
+        self.graph_weight_order, self.placed, self.predict_atol = graph_weight_order, placed, predict_atol
+
+    def fixture(self, name):
+        return Fixture(name, self.models_dir)
+
+    def reference_builders(self):
+        with open(self.builders_json) as f:
+            return json.load(f)
+
+
+FAMILIES = {
+    "models": Family("models", "reference_builders.json", ("DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN"),
+                     oracle_weights, oracle_forward, 17, {"binary", "regression"},
+                     graph_weight_order=("autoint_2x2_res", "autoint_attonly", "dcn_crossonly", "dcn_empty_linear",
+                                         "dcn_matrix1", "dcn_vector2", "deepfm_groups_varlen")),
+    "pairwise": Family("models_pairwise", "reference_builders_pairwise.json", ("NFM", "AFM"),
+                       _pairwise_weights, _pairwise_forward, 4, {"binary"},
+                       graph_weight_order=("afm_fm_only", "afm_two_groups")),     # AFM looks up embeddings first
+    "fibinet": Family("models_fibinet", "reference_builders_fibinet.json", ("FiBiNET",),
+                      _fibinet_weights, _fibinet_forward, 5, {"binary"}, placed=True),
+    "fefm": Family("models_fefm", "reference_builders_fefm.json", ("FwFM", "DeepFEFM"),
+                   _fefm_weights, _fefm_forward, 10, {"binary", "regression"}, placed=True,
+                   # a group's FwFMLayer is built before the next group's embeddings
+                   graph_weight_order=("fwfm_two_groups",)),
+    "pnn": Family("models_pnn", "reference_builders_pnn.json", ("PNN",),
+                  _pnn_weights, _pnn_forward, 9, {"binary", "regression"}, placed=True),
+    "ifm": Family("models_ifm", "reference_builders_ifm.json", ("IFM", "DIFM"),
+                  _ifm_weights, _ifm_forward, 6, {"binary", "regression"},
+                  graph_weight_order=("difm_defaults", "difm_no_att_res", "difm_two_heads_varlen", "ifm_criteo",
+                                      "ifm_regression", "ifm_varlen")),
+    "bst": Family("models_bst", "reference_builders_bst.json", ("BST",),
+                  _bst_weights, _bst_forward, 4, {"binary"}, predict_atol=1e-5),
+}
+
+
+# ---- layer fixtures (tests/golden/<family>/*.npz) -----------------------------------------------------
+def layer_cases(subdir):
+    return _cases(os.path.join(GOLDEN, subdir))
+
+
+def load_layer(subdir, name):
+    """(meta, {key: array}) of a layer fixture; the keys keep the npz's order."""
+    d = np.load(os.path.join(GOLDEN, subdir, name + ".npz"))
+    return json.loads(str(d["meta"])), {k: d[k] for k in d.files if k != "meta"}
+
+
+def layer_weight_names(d):
+    """weight names of a layer fixture, in the layer's order (the npz keeps insertion order)."""
+    return [k[2:] for k in d if k.startswith("w_")]

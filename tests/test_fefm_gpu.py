@@ -6,24 +6,33 @@
 * the C2 shape (B = 65536, F = 26, E = 32): the input a window of the [B, 848] gather buffer, and FEFM's scores
   written behind its 845 embedding and dense columns in a [B, 1172] buffer;
 * layer fixtures of the reference's own FwFMLayer / FEFMLayer (tests/golden/fefm/);
-* model fixtures (tests/golden/models_fefm/): logits and one SGD step in both GEMM precisions;
-* a graph-replayed training step equals an eager one;
+* with the placement, the step copies no score block ;
+* model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions, placed and unplaced;
+  a graph-replayed training step equals an eager one; the placement gives the results of the unplaced graph;
 * C2-shaped DeepFEFM: the logits of the first and last 512 samples against the CPU oracle.
 """
 import numpy as np
 import pytest
 import torch
 
+import b2_helpers as H
 import golden_models as G
-import test_fefm_goldens as FG
+import model_golden_checks as C
+from model_golden_checks import placement  # noqa: F401  (the placed / unplaced parameter)
 
 pytestmark = pytest.mark.gpu
 
-
-def _close(got, want, what, tol=2e-5):
-    scale = max(float(want.abs().max()), 1e-30)
-    err = float((got.double() - want).abs().max()) / scale
-    assert err < tol, "%s: max error %.3e relative to max |value|" % (what, err)
+T = C.gpu_model_tests("fefm")
+test_model_forward_matches_reference = T.forward
+test_model_sgd_step_matches_reference_gradients = T.sgd_step
+test_graph_replayed_step_equals_eager = C.graph_replay_test([
+    pytest.param("FwFM", dict(dnn_hidden_units=(32, 16)), id="fwfm"),
+    pytest.param("DeepFEFM", dict(dnn_hidden_units=(32, 16)), id="deepfefm"),
+    pytest.param("DeepFEFM", dict(dnn_hidden_units=()), id="deepfefm_no_dnn")])
+test_placement_gives_the_unplaced_results = C.placement_test([
+    pytest.param("DeepFEFM", dict(dnn_hidden_units=(32, 16)), 1e-5, 1e-6, id="defaults"),
+    pytest.param("DeepFEFM", dict(dnn_hidden_units=(32,), use_linear=False), 1e-5, 1e-6, id="no_linear"),
+    pytest.param("DeepFEFM", dict(dnn_hidden_units=(32,), use_fefm=False), 1e-5, 1e-6, id="no_fefm_logit")])
 
 
 def _ref_fwfm(x, r):
@@ -58,9 +67,9 @@ def _check_fwfm(cuda, B, F, E, seed, tail=13):
     r64 = r.double().requires_grad_(True)
     ref = _ref_fwfm(x64, r64)
     (ref * g.double()).sum().backward()
-    _close(out, ref.detach(), "out")
-    _close(dx.reshape(B, F, E), x64.grad, "dx")
-    _close(dR, r64.grad, "dR", 1e-4)
+    H.close(out, ref.detach(), "out")
+    H.close(dx.reshape(B, F, E), x64.grad, "dx")
+    H.close(dR, r64.grad, "dR", 1e-4)
     assert not bool(torch.tril(dR).any()), "dR is 0 on and below the diagonal"
     return (g, gbuf.stride(0), xw, ldx, r, dx, dR)
 
@@ -89,9 +98,9 @@ def _check_fefm(cuda, B, F, E, seed, ldx=None, ld=None, col0=3):
     W64 = W.double().requires_grad_(True)
     ref = _ref_fefm(x64, W64)
     (ref * g[:, col0:col0 + P].double()).sum().backward()
-    _close(got, ref.detach(), "out")
-    _close(dx.reshape(B, F, E), x64.grad, "dx")
-    _close(dW, W64.grad, "dW", 1e-4)
+    H.close(got, ref.detach(), "out")
+    H.close(dx.reshape(B, F, E), x64.grad, "dx")
+    H.close(dW, W64.grad, "dW", 1e-4)
     return (g, ld, col0, xw, ldx, S, dx, dW)
 
 
@@ -140,13 +149,13 @@ def test_kernels_reject_unsupported_shapes(cuda):
                    col0=3)
 
 
-@pytest.mark.parametrize("name", FG.LAYER_CASES)
+@pytest.mark.parametrize("name", G.layer_cases("fefm"))
 def test_layer_fixture(cuda, name):
     from deepctr_b200 import kernels as K
-    meta, d = FG.load_layer(name)
+    meta, d = G.load_layer("fefm", name)
     x = torch.tensor(d["x"], device=cuda)
     B, F, Ed = x.shape
-    ws = [torch.tensor(d["w_" + k], device=cuda) for k in FG.layer_weight_names(d)]
+    ws = [torch.tensor(d["w_" + k], device=cuda) for k in G.layer_weight_names(d)]
     dout = torch.tensor(d["dout"], device=cuda).reshape(B, -1).contiguous()
     tol = dict(rtol=1e-4, atol=1e-5)
     if meta["layer"] == "FwFMLayer":
@@ -160,95 +169,8 @@ def test_layer_fixture(cuda, name):
         grads = list(dW)
     np.testing.assert_allclose(out.reshape(d["out"].shape).cpu().numpy(), d["out"], **tol)
     np.testing.assert_allclose(dx.reshape(B, F, Ed).cpu().numpy(), d["gx"], **tol)
-    for k, gk in zip(FG.layer_weight_names(d), grads):
+    for k, gk in zip(G.layer_weight_names(d), grads):
         np.testing.assert_allclose(gk.cpu().numpy(), d["g_" + k], err_msg=k, **tol)
-
-
-# ---- model level ----------------------------------------------------------------------------------
-@pytest.fixture(params=[True, False], ids=["placed", "unplaced"])
-def placement(request):
-    from deepctr_b200 import inputs as I
-    I.DNN_INPUT_PLACEMENT = request.param
-    yield request.param
-    I.DNN_INPUT_PLACEMENT = True
-
-
-def _model(fx):
-    model = FG.build(fx)
-    return model, G.assign_weights(fx, model)
-
-
-@pytest.mark.usefixtures("gemm_precision", "placement")
-@pytest.mark.parametrize("name", FG.MODEL_CASES)
-def test_model_forward_matches_reference(cuda, name):
-    from test_model_goldens_gpu import _logits, _tol
-    fx = FG.Fixture(name)
-    model, _ = _model(fx)
-    x = fx.inputs()
-    np.testing.assert_allclose(_logits(model, x), fx.logit, rtol=1e-4, atol=_tol(fx.logit))
-    np.testing.assert_allclose(model.predict(x, batch_size=len(fx.y)), fx.out, rtol=1e-4, atol=_tol(fx.out))
-
-
-@pytest.mark.usefixtures("gemm_precision", "placement")
-@pytest.mark.parametrize("name", FG.MODEL_CASES)
-def test_model_sgd_step_matches_reference_gradients(cuda, name):
-    from deepctr_b200.engine import SGD
-    fx = FG.Fixture(name)
-    model, wm = _model(fx)
-    lr = 0.5
-    model.compile(SGD(lr), "mse" if fx.task == "regression" else "binary_crossentropy", embedding_update="dense")
-    loss = model.train_on_batch(fx.inputs(), fx.y)
-    assert abs(loss - fx.loss) <= 2e-4 * max(1.0, abs(fx.loss)), (loss, fx.loss)
-    for key, w in wm.items():
-        if key not in fx.g:
-            continue
-        want = fx.g[key]
-        got = (fx.w[key] - w.value()) / lr
-        np.testing.assert_allclose(got, want, rtol=2e-3, atol=3e-4 * float(np.abs(want).max()) + 2e-6, err_msg=key)
-
-
-def _criteo_model(builder, rng, n_dense=3, n=512, dim=8, **kw):
-    from deepctr_b200 import engine as E, models as M
-    from deepctr_b200 import feature_column as FC
-    cols = [FC.SparseFeat("C%d" % i, 50 + i, dim) for i in range(10)]
-    cols += [FC.DenseFeat("I%d" % i, 1) for i in range(n_dense)]
-    E.clear_session()
-    l2 = dict(l2_reg_embedding=0) if builder == "FwFM" else dict(l2_reg_embedding_feat=0)
-    model = getattr(M, builder)(cols, cols, l2_reg_linear=0, seed=3, **dict(l2, **kw))
-    x = {"C%d" % i: rng.randint(0, 50 + i, size=n).astype(np.int32) for i in range(10)}
-    x.update({"I%d" % i: rng.rand(n).astype(np.float32) for i in range(n_dense)})
-    y = (rng.rand(n) < 0.3).astype(np.float32)
-    return model, x, y
-
-
-def _train(builder, graph, kw, steps=6, init=None, placed=True):
-    from deepctr_b200 import inputs as I
-    from deepctr_b200.engine import SGD
-    I.DNN_INPUT_PLACEMENT = placed
-    try:
-        model, x, y = _criteo_model(builder, np.random.RandomState(4), **kw)
-    finally:
-        I.DNN_INPUT_PLACEMENT = True
-    if init is None:            # Keras leaves the final Dense kernel unseeded: start every run from the same weights
-        init = [w.value() for w in model.weights]
-    else:
-        model.set_weights(init)
-    model.compile(SGD(0.05), "binary_crossentropy", embedding_update="sparse", step_graph=graph)
-    losses = [model.train_on_batch(x, y) for _ in range(steps)]
-    return losses, {w.name: w.value() for w in model.weights}, model.replayed_launches, init
-
-
-@pytest.mark.parametrize("builder,kw", [("FwFM", dict(dnn_hidden_units=(32, 16))),
-                                        ("DeepFEFM", dict(dnn_hidden_units=(32, 16))),
-                                        ("DeepFEFM", dict(dnn_hidden_units=()))],
-                         ids=["fwfm", "deepfefm", "deepfefm_no_dnn"])
-def test_graph_replayed_step_equals_eager(cuda, builder, kw):
-    l_graph, w_graph, replayed, init = _train(builder, "auto", kw)
-    l_eager, w_eager, _, _ = _train(builder, "off", kw, init=init)
-    assert replayed > 0, "the training step was never replayed as a CUDA graph"
-    np.testing.assert_allclose(l_graph, l_eager, rtol=1e-5, atol=1e-6)
-    for k, v in w_eager.items():
-        np.testing.assert_allclose(w_graph[k], v, rtol=1e-4, atol=1e-6 + 1e-4 * float(np.abs(v).max()), err_msg=k)
 
 
 def test_c2_shape_deepfefm_tail_rows_match_the_oracle(cuda):
@@ -259,7 +181,6 @@ def test_c2_shape_deepfefm_tail_rows_match_the_oracle(cuda):
     from deepctr_b200 import engine as E, models as M
     from deepctr_b200 import feature_column as FC
     from deepctr_b200.layers import DNN, FEFMLayer
-    from test_model_goldens_gpu import _logits, _tol
     B, F, Ed, nd, V = 65536, 26, 32, 13, 1 << 20
     cols = [FC.SparseFeat("C%d" % i, V, Ed) for i in range(F)] + [FC.DenseFeat("I%d" % i, 1) for i in range(nd)]
     E.clear_session()
@@ -272,7 +193,7 @@ def test_c2_shape_deepfefm_tail_rows_match_the_oracle(cuda):
     rng = np.random.RandomState(0)
     x = {"C%d" % i: rng.randint(0, V, size=B).astype(np.int32) for i in range(F)}
     x.update({"I%d" % i: rng.rand(B).astype(np.float32) for i in range(nd)})
-    full = _logits(model, x)
+    full = H.logits(model, x)
     assert np.isfinite(full).all()
 
     rows = np.r_[0:512, B - 512:B]
@@ -297,20 +218,7 @@ def test_c2_shape_deepfefm_tail_rows_match_the_oracle(cuda):
     with torch.no_grad():
         want, _ = FO.deepfefm(xs, cols, cols, W)
     want = want.numpy().reshape(-1, 1)
-    np.testing.assert_allclose(full[rows], want, rtol=1e-4, atol=_tol(want))
-
-
-@pytest.mark.parametrize("kw", [dict(dnn_hidden_units=(32, 16)), dict(dnn_hidden_units=(32,), use_linear=False),
-                                dict(dnn_hidden_units=(32,), use_fefm=False)],
-                         ids=["defaults", "no_linear", "no_fefm_logit"])
-def test_placement_gives_the_unplaced_results(cuda, kw):
-    # the same arithmetic on differently laid out operands (the unplaced DNN input is a [B, 128] tensor, the placed
-    # one a window of the [B, 132] gather buffer): six steps agree to rounding, e.g. 5e-11 on an embedding of 1e-5
-    l_p, w_p, _, init = _train("DeepFEFM", "off", kw)
-    l_u, w_u, _, _ = _train("DeepFEFM", "off", kw, init=init, placed=False)
-    np.testing.assert_allclose(l_p, l_u, rtol=1e-6, atol=0)
-    for k, v in w_u.items():
-        np.testing.assert_allclose(w_p[k], v, rtol=1e-5, atol=1e-6 * float(np.abs(v).max()), err_msg=k)
+    np.testing.assert_allclose(full[rows], want, rtol=1e-4, atol=H.logit_tol(want))
 
 
 def test_placed_step_copies_no_score_block(cuda, monkeypatch):
@@ -335,7 +243,7 @@ def test_placed_step_copies_no_score_block(cuda, monkeypatch):
     for placed in (True, False):
         I.DNN_INPUT_PLACEMENT = placed
         try:
-            model, x, y = _criteo_model("DeepFEFM", np.random.RandomState(5), dnn_hidden_units=(16,))
+            model, x, y = H.criteo_model("DeepFEFM", np.random.RandomState(5), dnn_hidden_units=(16,))
         finally:
             I.DNN_INPUT_PLACEMENT = True
         assert bool(model.planner.fefm_places) == placed

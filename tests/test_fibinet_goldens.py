@@ -1,114 +1,41 @@
 """CPU: FiBiNET and its layers (SENETLayer, BilinearInteraction) against fixtures the reference's own layer and
 builder code produced (tests/golden/generate_fibinet.py):
 
-1. the CPU restatement of tests/fibinet_oracle.py (built on oracle/) reproduces every layer output, model logit,
-   prediction, loss and gradient;
-2. the deepctr_b200 builder creates the reference's weight set and graph (names, shapes, order, planner slots), and
-   has the reference's keyword defaults;
-3. the documented shape limits of the SENET / bilinear kernels raise ValueError, an unknown bilinear_type raises
+1. the CPU restatement of tests/fibinet_oracle.py (built on oracle/) reproduces every layer output and, with the
+   checks shared by every family (model_golden_checks), every model fixture, weight set, graph and keyword default;
+2. the documented shape limits of the SENET / bilinear kernels raise ValueError, an unknown bilinear_type raises
    NotImplementedError;
-4. the DNN-input placement is planned for FiBiNET's graph, and only there.
+3. the DNN-input placement is planned for FiBiNET's graph, and only there.
 """
-import glob
-import inspect
-import json
-import os
-import re
 
 import numpy as np
 import pytest
 import torch
 
 import golden_models as G
-from test_reference_builders_dropin import signature, builder_args
+import model_golden_checks as C
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-LAYERS = os.path.join(HERE, "golden", "fibinet")
-MODELS = os.path.join(HERE, "golden", "models_fibinet")
-BUILDERS_JSON = os.path.join(HERE, "golden", "reference_builders_fibinet.json")
-LAYER_CASES = sorted(os.path.basename(p)[:-4] for p in glob.glob(os.path.join(LAYERS, "*.npz")))
-MODEL_CASES = sorted(os.path.basename(p)[:-4] for p in glob.glob(os.path.join(MODELS, "*.npz")))
-
-
-def load_layer(name):
-    d = np.load(os.path.join(LAYERS, name + ".npz"))
-    meta = json.loads(str(d["meta"]))
-    return meta, {k: d[k] for k in d.files if k != "meta"}
-
-
-def layer_weight_names(d):
-    """weight names of a layer fixture, in the layer's order (the npz keeps insertion order)."""
-    return [k[2:] for k in d if k.startswith("w_")]
-
-
-class Fixture(G.Fixture):
-    """golden_models.Fixture read from tests/golden/models_fibinet/."""
-
-    def __init__(self, name):
-        d = np.load(os.path.join(MODELS, name + ".npz"))
-        self.name = name
-        self.meta = json.loads(str(d["meta"]))
-        self.x = {k[2:]: d[k] for k in d.files if k.startswith("x_")}
-        self.y = d["y"]
-        self.w = {k[2:]: d[k] for k in d.files if k.startswith("w_")}
-        self.g = {k[2:]: d[k] for k in d.files if k.startswith("g_")}
-        self.out, self.logit, self.loss = d["out"], d["logit"], float(d["loss"])
-        self.builder, self.kwargs = self.meta["builder"], self.meta["kwargs"]
-        self.task = self.meta.get("task", "binary")
-        self.training = bool(self.meta.get("training"))
-
-
-def _creation_order(name):
-    m = re.search(r"_(\d+)$", name)
-    return int(m.group(1)) if m else 0
-
-
-def oracle_weights(fx, requires_grad=False):
-    """golden_models.oracle_weights plus the SENET weights and the two bilinear layers' weights (SENET branch
-    first: the layer created first)."""
-    W, leaves = G.oracle_weights(fx, requires_grad)
-
-    def t(key):
-        v = torch.tensor(fx.w[key], requires_grad=requires_grad and key in fx.g)
-        leaves[key] = v
-        return v
-    senet = fx.layer_names("SENETLayer")[0]
-    W["senet"] = (t(senet + "/W_1"), t(senet + "/W_2"))
-    W["bilinear"] = [[t(k) for k in fx.w if k.startswith(name + "/bilinear_weight")]
-                     for name in sorted(fx.layer_names("BilinearInteraction"), key=_creation_order)]
-    W.setdefault("dnn_kernels", [])
-    W.setdefault("dnn_biases", [])
-    return W, leaves
-
-
-def oracle_forward(fx, W):
-    import fibinet_oracle as FO
-    from deepctr_b200 import feature_column as FC
-    lin, dnn = G.columns(fx, "linear", FC), G.columns(fx, "dnn", FC)
-    return FO.fibinet(fx.inputs(), lin, dnn, W, bilinear_type=fx.kwargs.get("bilinear_type", "interaction"),
-                      task=fx.task)
-
-
-def build(fx):
-    from deepctr_b200 import engine as E
-    from deepctr_b200 import models as M
-    args, kw = builder_args(fx)
-    E.clear_session()
-    return getattr(M, fx.builder)(*args, **kw)
+LAYER_CASES = G.layer_cases("fibinet")
+T = C.model_tests("fibinet")
+test_oracle_matches_reference_model = T.oracle
+test_builder_creates_the_reference_weight_set = T.weight_set
+test_builder_graph_is_the_reference_graph = T.graph
+test_reference_default_arguments_are_the_same = T.defaults
 
 
 def test_fixture_sets():
-    assert len(LAYER_CASES) == 12 and len(MODEL_CASES) == 5
-    assert set(Fixture(n).builder for n in MODEL_CASES) == {"FiBiNET"}
-    assert {Fixture(n).kwargs["bilinear_type"] for n in MODEL_CASES} == {"all", "each", "interaction"}
+    C.check_fixture_set(G.FAMILIES["fibinet"])
+    fam = G.FAMILIES["fibinet"]
+    assert len(LAYER_CASES) == 12
+    assert {fam.fixture(n).kwargs["bilinear_type"] for n in fam.cases} == {"all", "each", "interaction"}
 
 
 @pytest.mark.parametrize("name", LAYER_CASES)
 def test_oracle_matches_reference_layer(name):
     import fibinet_oracle as FO
-    meta, d = load_layer(name)
+    meta, d = G.load_layer("fibinet", name)
     x = torch.tensor(d["x"], requires_grad=True)
-    ws = [torch.tensor(d["w_" + k], requires_grad=True) for k in layer_weight_names(d)]
+    ws = [torch.tensor(d["w_" + k], requires_grad=True) for k in G.layer_weight_names(d)]
     if meta["layer"] == "SENETLayer":
         out = FO.senet(x, *ws)
     else:
@@ -116,62 +43,8 @@ def test_oracle_matches_reference_layer(name):
     np.testing.assert_allclose(out.detach().numpy(), d["out"], rtol=1e-5, atol=1e-6)
     (out * torch.as_tensor(d["dout"])).sum().backward()
     np.testing.assert_allclose(x.grad.numpy(), d["gx"], rtol=1e-4, atol=1e-6)
-    for k, v in zip(layer_weight_names(d), ws):
+    for k, v in zip(G.layer_weight_names(d), ws):
         np.testing.assert_allclose(v.grad.numpy(), d["g_" + k], rtol=1e-4, atol=1e-6, err_msg=k)
-
-
-@pytest.mark.parametrize("name", MODEL_CASES)
-def test_oracle_matches_reference_model(name):
-    fx = Fixture(name)
-    W, leaves = oracle_weights(fx, requires_grad=True)
-    logit, pred = oracle_forward(fx, W)
-    np.testing.assert_allclose(logit.detach().numpy().reshape(-1, 1), fx.logit, rtol=1e-4, atol=1e-5)
-    np.testing.assert_allclose(pred.detach().numpy().reshape(-1, 1), fx.out, rtol=1e-4, atol=1e-6)
-    loss = G.loss_of(fx, pred)
-    assert abs(float(loss.detach()) - fx.loss) <= 1e-5 * max(1.0, abs(fx.loss))
-    loss.backward()
-    assert set(k for k in fx.g if not G._ignored(k)) <= set(leaves)
-    for key, want in fx.g.items():
-        if G._ignored(key):
-            assert not np.any(want), key
-            continue
-        leaf = leaves[key]
-        got = leaf.grad.numpy() if leaf.grad is not None else np.zeros_like(want)
-        np.testing.assert_allclose(got, want, rtol=1e-4, atol=1e-4 * float(np.abs(want).max()) + 1e-7, err_msg=key)
-
-
-@pytest.mark.parametrize("name", MODEL_CASES)
-def test_builder_creates_the_reference_weight_set(name):
-    fx = Fixture(name)
-    model = build(fx)
-    wm = G.weight_map(fx, model)
-    assert len(wm) == len([k for k in fx.w if not G._ignored(k)])
-    assert [w.name for w in model.weights if not G._ignored(w.name)] == \
-        [k for k in fx.w if not G._ignored(k)], "weight order"
-    for key, w in wm.items():
-        assert w.trainable == (key in fx.g), key
-
-
-@pytest.mark.parametrize("name", MODEL_CASES)
-def test_builder_graph_is_the_reference_graph(name):
-    with open(BUILDERS_JSON) as f:
-        want = json.load(f)["signatures"][name]
-    got = signature(build(Fixture(name)))
-    assert want["inputs"] == got["inputs"]
-    assert want["weights"] == got["weights"]
-    assert want["slots"] == got["slots"] and want["fast"] == got["fast"]
-    assert sorted(want["layers"]) == sorted(got["layers"])
-
-
-def test_reference_default_arguments_are_the_same():
-    from deepctr_b200 import models as M
-    with open(BUILDERS_JSON) as f:
-        ref = json.load(f)["defaults"]
-    assert sorted(ref) == ["FiBiNET"]
-    mine = inspect.signature(M.FiBiNET)
-    assert [k for k, _ in ref["FiBiNET"]] == list(mine.parameters)
-    for k, d in ref["FiBiNET"]:
-        assert d == repr(mine.parameters[k].default), k
 
 
 @pytest.mark.parametrize("nfields,dim", [(65, 4), (3, 65)])

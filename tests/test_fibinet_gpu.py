@@ -4,9 +4,9 @@
   64 and E = 4 / 5 / 32 / 64, the input a window of a wider buffer, the output a strided window of a wider buffer,
   and batches that are not a multiple of a CTA's samples; both backwards are bit-identical from run to run;
 * layer fixtures of the reference's own SENETLayer / BilinearInteraction (tests/golden/fibinet/);
-* model fixtures (tests/golden/models_fibinet/): logits and one SGD step in both GEMM precisions;
-* a graph-replayed training step equals an eager one; the DNN-input placement gives the results of the unplaced
-  graph, and with it no copy wider than the dense tail touches the DNN input;
+* with the DNN-input placement no copy wider than the dense tail touches the DNN input ;
+* model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions, placed and unplaced;
+  a graph-replayed training step equals an eager one; the placement gives the results of the unplaced graph;
 * the C2 shape (26 fields, E = 32, B = 65536, 13 dense features: a [65536, 20816] DNN input and a K = 20813 GEMM):
   the logits of the first and last 512 samples against the CPU oracle.
 """
@@ -16,10 +16,23 @@ import numpy as np
 import pytest
 import torch
 
+import b2_helpers as H
 import golden_models as G
-import test_fibinet_goldens as FG
+import model_golden_checks as C
+from model_golden_checks import placement  # noqa: F401  (the placed / unplaced parameter)
 
 pytestmark = pytest.mark.gpu
+
+T = C.gpu_model_tests("fibinet")
+test_model_forward_matches_reference = T.forward
+test_model_sgd_step_matches_reference_gradients = T.sgd_step
+test_graph_replayed_step_equals_eager = C.graph_replay_test([
+    pytest.param("FiBiNET", dict(bilinear_type="interaction", dnn_hidden_units=(32, 16)), id="interaction"),
+    pytest.param("FiBiNET", dict(bilinear_type="each", dnn_hidden_units=(32,)), id="each"),
+    pytest.param("FiBiNET", dict(bilinear_type="all", dnn_hidden_units=()), id="all")])
+test_placement_gives_the_unplaced_results = C.placement_test([
+    pytest.param("FiBiNET", dict(bilinear_type="interaction", dnn_hidden_units=(32, 16)), 1e-6, 1e-7, id="interaction"),
+    pytest.param("FiBiNET", dict(bilinear_type="all", dnn_hidden_units=()), 1e-6, 1e-7, id="no_dnn")])
 TYPES = ("all", "each", "interaction")
 
 
@@ -40,12 +53,6 @@ def _ref_bilinear(x, t, W):
 def _ref_senet(x, W1, W2):
     a2 = torch.relu(torch.relu(x.mean(-1) @ W1) @ W2)
     return x * a2.unsqueeze(2)
-
-
-def _close(got, want, what, tol=2e-5):
-    scale = max(float(want.abs().max()), 1e-30)
-    err = float((got.double() - want).abs().max()) / scale
-    assert err < tol, "%s: max error %.3e relative to max |value|" % (what, err)
 
 
 def _check_bilinear(cuda, B, F, E, t, seed, tail=13):
@@ -73,9 +80,9 @@ def _check_bilinear(cuda, B, F, E, t, seed, tail=13):
     ref = _ref_bilinear(x64, t, W64)
     g64 = g[:, col0:col0 + P * pitch].reshape(B, P, pitch)[:, :, :E].double()
     (ref * g64).sum().backward()
-    _close(got, ref.detach(), "out")
-    _close(dx.reshape(B, F, E), x64.grad, "dx")
-    _close(dW, W64.grad, "dW")
+    H.close(got, ref.detach(), "out")
+    H.close(dx.reshape(B, F, E), x64.grad, "dx")
+    H.close(dW, W64.grad, "dW")
     return (gv, ld, pitch, xw, ldx, W, dx, dW)
 
 
@@ -109,10 +116,10 @@ def _check_senet(cuda, B, F, E, R, seed):
     W164, W264 = W1.double().requires_grad_(True), W2.double().requires_grad_(True)
     ref = _ref_senet(x64, W164, W264)
     (ref * g.double().reshape(B, F, E)).sum().backward()
-    _close(v.reshape(B, F, E), ref.detach(), "V")
-    _close(dx.reshape(B, F, E), x64.grad, "dx")
-    _close(dW1, W164.grad, "dW1", 1e-4)
-    _close(dW2, W264.grad, "dW2", 1e-4)
+    H.close(v.reshape(B, F, E), ref.detach(), "V")
+    H.close(dx.reshape(B, F, E), x64.grad, "dx")
+    H.close(dW1, W164.grad, "dW1", 1e-4)
+    H.close(dW2, W264.grad, "dW2", 1e-4)
     return (g, xw, ldx, W1, W2, saved, dx, dW1, dW2)
 
 
@@ -141,13 +148,13 @@ def test_kernels_reject_unsupported_shapes(cuda):
         K.senet_fwd(x, 65 * 4, 65, 4, torch.zeros((65, 2), device=cuda), torch.zeros((2, 65), device=cuda), 4)
 
 
-@pytest.mark.parametrize("name", FG.LAYER_CASES)
+@pytest.mark.parametrize("name", G.layer_cases("fibinet"))
 def test_layer_fixture(cuda, name):
     from deepctr_b200 import kernels as K
-    meta, d = FG.load_layer(name)
+    meta, d = G.load_layer("fibinet", name)
     x = torch.tensor(d["x"], device=cuda)
     B, F, Ed = x.shape
-    ws = [torch.tensor(d["w_" + k], device=cuda) for k in FG.layer_weight_names(d)]
+    ws = [torch.tensor(d["w_" + k], device=cuda) for k in G.layer_weight_names(d)]
     dout = torch.tensor(d["dout"], device=cuda).reshape(B, -1).contiguous()
     tol = dict(rtol=1e-4, atol=1e-5)
     if meta["layer"] == "SENETLayer":
@@ -163,104 +170,8 @@ def test_layer_fixture(cuda, name):
         grads = list(dW)
     np.testing.assert_allclose(out.reshape(d["out"].shape).cpu().numpy(), d["out"], **tol)
     np.testing.assert_allclose(dx.reshape(B, F, Ed).cpu().numpy(), d["gx"], **tol)
-    for k, gk in zip(FG.layer_weight_names(d), grads):
+    for k, gk in zip(G.layer_weight_names(d), grads):
         np.testing.assert_allclose(gk.cpu().numpy(), d["g_" + k], err_msg=k, **tol)
-
-
-# ---- model level ----------------------------------------------------------------------------------
-@pytest.fixture(params=[True, False], ids=["placed", "unplaced"])
-def placement(request):
-    from deepctr_b200 import inputs as I
-    I.DNN_INPUT_PLACEMENT = request.param
-    yield request.param
-    I.DNN_INPUT_PLACEMENT = True
-
-
-def _model(fx):
-    model = FG.build(fx)
-    return model, G.assign_weights(fx, model)
-
-
-@pytest.mark.usefixtures("gemm_precision", "placement")
-@pytest.mark.parametrize("name", FG.MODEL_CASES)
-def test_model_forward_matches_reference(cuda, name):
-    from test_model_goldens_gpu import _logits, _tol
-    fx = FG.Fixture(name)
-    model, _ = _model(fx)
-    x = fx.inputs()
-    np.testing.assert_allclose(_logits(model, x), fx.logit, rtol=1e-4, atol=_tol(fx.logit))
-    np.testing.assert_allclose(model.predict(x, batch_size=len(fx.y)), fx.out, rtol=1e-4, atol=_tol(fx.out))
-
-
-@pytest.mark.usefixtures("gemm_precision", "placement")
-@pytest.mark.parametrize("name", FG.MODEL_CASES)
-def test_model_sgd_step_matches_reference_gradients(cuda, name):
-    from deepctr_b200.engine import SGD
-    fx = FG.Fixture(name)
-    model, wm = _model(fx)
-    lr = 0.5
-    model.compile(SGD(lr), "binary_crossentropy", embedding_update="dense")
-    loss = model.train_on_batch(fx.inputs(), fx.y)
-    assert abs(loss - fx.loss) <= 2e-4 * max(1.0, abs(fx.loss)), (loss, fx.loss)
-    for key, w in wm.items():
-        if key not in fx.g:
-            continue
-        want = fx.g[key]
-        got = (fx.w[key] - w.value()) / lr
-        np.testing.assert_allclose(got, want, rtol=2e-3, atol=3e-4 * float(np.abs(want).max()) + 2e-6, err_msg=key)
-
-
-def _criteo_model(rng, n_dense, n=512, dim=8, **kw):
-    from deepctr_b200 import engine as E, models as M
-    from deepctr_b200 import feature_column as FC
-    cols = [FC.SparseFeat("C%d" % i, 50 + i, dim) for i in range(10)]
-    cols += [FC.DenseFeat("I%d" % i, 1) for i in range(n_dense)]
-    E.clear_session()
-    model = M.FiBiNET(cols, cols, l2_reg_linear=0, l2_reg_embedding=0, seed=3, **kw)
-    x = {"C%d" % i: rng.randint(0, 50 + i, size=n).astype(np.int32) for i in range(10)}
-    x.update({"I%d" % i: rng.rand(n).astype(np.float32) for i in range(n_dense)})
-    y = (rng.rand(n) < 0.3).astype(np.float32)
-    return model, x, y
-
-
-def _train(placed, graph, kw, steps=6, init=None):
-    from deepctr_b200 import inputs as I
-    from deepctr_b200.engine import SGD
-    I.DNN_INPUT_PLACEMENT = placed
-    try:
-        model, x, y = _criteo_model(np.random.RandomState(4), 3, **kw)
-    finally:
-        I.DNN_INPUT_PLACEMENT = True
-    assert bool(model.planner.dnn_places) == placed
-    if init is None:            # Keras leaves the final Dense kernel unseeded: start every run from the same weights
-        init = [w.value() for w in model.weights]
-    else:
-        model.set_weights(init)
-    model.compile(SGD(0.05), "binary_crossentropy", embedding_update="sparse", step_graph=graph)
-    losses = [model.train_on_batch(x, y) for _ in range(steps)]
-    return losses, {w.name: w.value() for w in model.weights}, model.replayed_launches, init
-
-
-@pytest.mark.parametrize("kw", [dict(bilinear_type="interaction", dnn_hidden_units=(32, 16)),
-                                dict(bilinear_type="each", dnn_hidden_units=(32,)),
-                                dict(bilinear_type="all", dnn_hidden_units=())], ids=["interaction", "each", "all"])
-def test_graph_replayed_step_equals_eager(cuda, kw):
-    l_graph, w_graph, replayed, init = _train(True, "auto", kw)
-    l_eager, w_eager, _, _ = _train(True, "off", kw, init=init)
-    assert replayed > 0, "the training step was never replayed as a CUDA graph"
-    np.testing.assert_allclose(l_graph, l_eager, rtol=1e-5, atol=1e-6)
-    for k, v in w_eager.items():
-        np.testing.assert_allclose(w_graph[k], v, rtol=1e-4, atol=1e-6 + 1e-4 * float(np.abs(v).max()), err_msg=k)
-
-
-@pytest.mark.parametrize("kw", [dict(bilinear_type="interaction", dnn_hidden_units=(32, 16)),
-                                dict(bilinear_type="all", dnn_hidden_units=())], ids=["interaction", "no_dnn"])
-def test_placement_gives_the_unplaced_results(cuda, kw):
-    l_p, w_p, _, init = _train(True, "off", kw)
-    l_u, w_u, _, _ = _train(False, "off", kw, init=init)
-    np.testing.assert_allclose(l_p, l_u, rtol=1e-6, atol=0)
-    for k, v in w_u.items():
-        np.testing.assert_allclose(w_p[k], v, rtol=1e-6, atol=1e-7 * float(np.abs(v).max()), err_msg=k)
 
 
 def test_placed_step_copies_only_the_dense_tail(cuda, monkeypatch):
@@ -288,7 +199,7 @@ def test_placed_step_copies_only_the_dense_tail(cuda, monkeypatch):
     for placed in (True, False):
         I.DNN_INPUT_PLACEMENT = placed
         try:
-            model, x, y = _criteo_model(np.random.RandomState(5), 3, dnn_hidden_units=(16,))
+            model, x, y = H.criteo_model("FiBiNET", np.random.RandomState(5), dnn_hidden_units=(16,))
         finally:
             I.DNN_INPUT_PLACEMENT = True
         model.compile(SGD(0.05), "binary_crossentropy", embedding_update="sparse", step_graph="off")
@@ -317,7 +228,6 @@ def test_c2_shape_tail_rows_match_the_oracle(cuda):
     from deepctr_b200 import engine as E, models as M
     from deepctr_b200 import feature_column as FC
     from deepctr_b200.layers import DNN, SENETLayer
-    from test_model_goldens_gpu import _logits, _tol
     B, F, Ed, nd, V = 65536, 26, 32, 13, 1 << 20
     cols = [FC.SparseFeat("C%d" % i, V, Ed) for i in range(F)] + [FC.DenseFeat("I%d" % i, 1) for i in range(nd)]
     E.clear_session()
@@ -333,7 +243,7 @@ def test_c2_shape_tail_rows_match_the_oracle(cuda):
     rng = np.random.RandomState(0)
     x = {"C%d" % i: rng.randint(0, V, size=B).astype(np.int32) for i in range(F)}
     x.update({"I%d" % i: rng.rand(B).astype(np.float32) for i in range(nd)})
-    full = _logits(model, x)
+    full = H.logits(model, x)
     assert np.isfinite(full).all()
 
     rows = np.r_[0:512, B - 512:B]
@@ -362,4 +272,4 @@ def test_c2_shape_tail_rows_match_the_oracle(cuda):
     with torch.no_grad():
         want, _ = FO.fibinet(xs, cols, cols, W, bilinear_type="interaction")
     want = want.numpy().reshape(-1, 1)
-    np.testing.assert_allclose(full[rows], want, rtol=1e-4, atol=_tol(want))
+    np.testing.assert_allclose(full[rows], want, rtol=1e-4, atol=H.logit_tol(want))

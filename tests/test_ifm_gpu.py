@@ -6,27 +6,27 @@
   are not a multiple of a CTA's samples;
 * the C2 shape (B = 65536, F = 26, E = 32): x a window of the [B, 848] gather buffer;
 * fm_weighted with m == 1 equals b2ctr_fm_fwd / _bwd bit for bit; the backwards are bit-identical from run to run;
-* model fixtures (tests/golden/models_ifm/): logits and one SGD step in both GEMM precisions;
-* a graph-replayed IFM / DIFM step equals an eager one; the IFM step runs fm_weighted and materialises no [B, F, E]
-  product; a refine product consumed by Flatten -> Dense as well as FM is materialised and has the right gradients;
-  the reference test's dnn_dropout=0.5 configurations train with a finite loss.
+* the IFM step runs fm_weighted and materialises no [B, F, E] product; a refine product consumed by Flatten -> Dense
+  as well as FM is materialised and has the right gradients; the reference test's dnn_dropout=0.5 configurations
+  train with a finite loss.
+Model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions; a graph-replayed IFM /
+DIFM step equals an eager one.
 """
 import numpy as np
 import pytest
 import torch
 
-import golden_models as G
-import test_ifm_goldens as IG
+import b2_helpers as H
+import model_golden_checks as C
 
 pytestmark = pytest.mark.gpu
 
-
-def _close(got, want, what, tol=5e-5, floor=0.0):
-    """Max error relative to max |want|, or to ``floor`` when that is larger: the magnitude of the terms whose
-    difference the kernel forms (FM with one field, or a saturated softmax, is a cancellation to about 0)."""
-    scale = max(float(want.abs().max()), float(floor), 1e-30)
-    err = float((got.double() - want).abs().max()) / scale
-    assert err < tol, "%s: max error %.3e relative to max |value|" % (what, err)
+T = C.gpu_model_tests("ifm")
+test_model_forward_matches_reference = T.forward
+test_model_sgd_step_matches_reference_gradients = T.sgd_step
+test_graph_replayed_step_equals_eager = C.graph_replay_test([
+    pytest.param("IFM", dict(dnn_hidden_units=(32, 16)), id="ifm"),
+    pytest.param("DIFM", dict(dnn_hidden_units=(32,), att_head_num=2), id="difm")])
 
 
 def _operands(cuda, B, F, E, seed, ldx=None, x0=2):
@@ -69,9 +69,9 @@ def _check_fm(cuda, B, F, E, seed, ldx=None, x0=2, chunk=8192):
             sq = float((y * y).sum((1, 2)).max())
             fdx = float((ga[:, None, None] * m64.abs().unsqueeze(-1) * y.sum(1, keepdim=True)).max())
             fdm = float((ga[:, None] * (x64.abs() * y.sum(1, keepdim=True)).sum(2)).max())
-        _close(out[sl], ref.detach(), "fm_weighted out", floor=sq)
-        _close((dxw[sl] - d0[sl, 4:4 + F * E]).reshape(-1, F, E), x64.grad, "fm_weighted dx", 1e-4, floor=fdx)
-        _close(dm[sl], m64.grad, "fm_weighted dm", 1e-4, floor=fdm)
+        H.close(out[sl], ref.detach(), "fm_weighted out", 5e-5, floor=sq)
+        H.close((dxw[sl] - d0[sl, 4:4 + F * E]).reshape(-1, F, E), x64.grad, "fm_weighted dx", 1e-4, floor=fdx)
+        H.close(dm[sl], m64.grad, "fm_weighted dm", 1e-4, floor=fdm)
     return xw, ldx, m, g
 
 
@@ -83,18 +83,18 @@ def _check_scale(cuda, B, F, E, seed):
     assert bool((yb[:, :3] == 7.0).all()) and bool((yb[:, 3 + F * E:] == 7.0).all())
     x64, m64 = xw.double().reshape(B, F, E).requires_grad_(True), m.double().requires_grad_(True)
     ref = x64 * m64.unsqueeze(-1)
-    _close(y.reshape(B, F, E), ref.detach(), "field_scale y", 1e-7)
+    H.close(y.reshape(B, F, E), ref.detach(), "field_scale y", 1e-7)
     gb = torch.tensor(rng.normal(0, 1.0, size=(B, F * E + 5)).astype(np.float32), device=cuda)
     g = gb[:, 5:]
     dbuf = torch.tensor(rng.normal(0, 1.0, size=(B, F * E + 2)).astype(np.float32), device=cuda)
     d0 = dbuf.clone()
     _, dm = K.field_scale_bwd(g, xw, ldx, m, F, E, B, dx=dbuf[:, 1:1 + F * E], accumulate=True)
     (ref * g.double().reshape(B, F, E)).sum().backward()
-    _close((dbuf[:, 1:1 + F * E] - d0[:, 1:1 + F * E]).reshape(B, F, E), x64.grad, "field_scale dx")
+    H.close((dbuf[:, 1:1 + F * E] - d0[:, 1:1 + F * E]).reshape(B, F, E), x64.grad, "field_scale dx", 5e-5)
     assert torch.equal(dbuf[:, 0], d0[:, 0]) and torch.equal(dbuf[:, -1], d0[:, -1])
-    _close(dm, m64.grad, "field_scale dm", 1e-5)
+    H.close(dm, m64.grad, "field_scale dm", 1e-5)
     dx2, dm2 = K.field_scale_bwd(g, xw, ldx, m, F, E, B)
-    _close(dx2.reshape(B, F, E), x64.grad, "field_scale dx (overwrite)", 1e-7)
+    H.close(dx2.reshape(B, F, E), x64.grad, "field_scale dx (overwrite)", 1e-7)
     _, dm3 = K.field_scale_bwd(g, xw, ldx, m, F, E, B, want_dx=False)
     assert torch.equal(dm2, dm) and torch.equal(dm3, dm)
 
@@ -127,12 +127,12 @@ def test_softmax_rows_matches_float64(cuda, C, scale):
     y = K.softmax_rows_fwd(x, scale)
     x64 = x.double().requires_grad_(True)
     ref = scale * torch.softmax(x64, dim=1)
-    _close(y, ref.detach(), "softmax y", 1e-6)
+    H.close(y, ref.detach(), "softmax y", 1e-6)
     gb = torch.tensor(rng.normal(0, 1.0, size=(B, C + 3)).astype(np.float32), device=cuda)
     g = gb[:, 3:]
     dx = K.softmax_rows_bwd(y, g, scale)
     (ref * g.double()).sum().backward()
-    _close(dx, x64.grad, "softmax dx", 1e-5, floor=float((ref.detach().abs() * g.double().abs()).max()))
+    H.close(dx, x64.grad, "softmax dx", 1e-5, floor=float((ref.detach().abs() * g.double().abs()).max()))
 
 
 def test_kernels_at_c2_shape(cuda):
@@ -170,77 +170,6 @@ def test_backwards_are_deterministic(cuda):
     assert torch.equal(K.softmax_rows_bwd(y, gy, 26.0), K.softmax_rows_bwd(y, gy, 26.0))
 
 
-# ---- model level ----------------------------------------------------------------------------------
-def _model(fx):
-    model = IG.build(fx)
-    return model, G.assign_weights(fx, model)
-
-
-@pytest.mark.usefixtures("gemm_precision")
-@pytest.mark.parametrize("name", IG.MODEL_CASES)
-def test_model_forward_matches_reference(cuda, name):
-    from test_model_goldens_gpu import _logits, _tol
-    fx = IG.Fixture(name)
-    model, _ = _model(fx)
-    x = fx.inputs()
-    np.testing.assert_allclose(_logits(model, x), fx.logit, rtol=1e-4, atol=_tol(fx.logit))
-    np.testing.assert_allclose(model.predict(x, batch_size=len(fx.y)), fx.out, rtol=1e-4, atol=_tol(fx.out))
-
-
-@pytest.mark.usefixtures("gemm_precision")
-@pytest.mark.parametrize("name", IG.MODEL_CASES)
-def test_model_sgd_step_matches_reference_gradients(cuda, name):
-    from deepctr_b200.engine import SGD
-    fx = IG.Fixture(name)
-    model, wm = _model(fx)
-    lr = 0.5
-    model.compile(SGD(lr), "mse" if fx.task == "regression" else "binary_crossentropy", embedding_update="dense")
-    loss = model.train_on_batch(fx.inputs(), fx.y)
-    assert abs(loss - fx.loss) <= 2e-4 * max(1.0, abs(fx.loss)), (loss, fx.loss)
-    for key, w in wm.items():
-        if key not in fx.g:
-            continue
-        want = fx.g[key]
-        got = (fx.w[key] - w.value()) / lr
-        np.testing.assert_allclose(got, want, rtol=2e-3, atol=3e-4 * float(np.abs(want).max()) + 2e-6, err_msg=key)
-
-
-def _criteo(rng, n=512, dim=8):
-    from deepctr_b200 import feature_column as FC
-    cols = [FC.SparseFeat("C%d" % i, 50 + i, dim) for i in range(10)] + [FC.DenseFeat("I%d" % i, 1) for i in range(3)]
-    x = {"C%d" % i: rng.randint(0, 50 + i, size=n).astype(np.int32) for i in range(10)}
-    x.update({"I%d" % i: rng.rand(n).astype(np.float32) for i in range(3)})
-    y = (rng.rand(n) < 0.3).astype(np.float32)
-    return cols, x, y
-
-
-def _train(builder, graph, kw, steps=6, init=None):
-    from deepctr_b200 import engine as E, models as M
-    from deepctr_b200.engine import SGD
-    cols, x, y = _criteo(np.random.RandomState(4))
-    E.clear_session()
-    model = getattr(M, builder)(cols, cols, l2_reg_linear=0, l2_reg_embedding=0, seed=3, **kw)
-    if init is None:            # Keras leaves the Dense kernels unseeded: start every run from the same weights
-        init = [w.value() for w in model.weights]
-    else:
-        model.set_weights(init)
-    model.compile(SGD(0.05), "binary_crossentropy", embedding_update="sparse", step_graph=graph)
-    losses = [model.train_on_batch(x, y) for _ in range(steps)]
-    return losses, {w.name: w.value() for w in model.weights}, model.replayed_launches, init
-
-
-@pytest.mark.parametrize("builder,kw", [("IFM", dict(dnn_hidden_units=(32, 16))),
-                                        ("DIFM", dict(dnn_hidden_units=(32,), att_head_num=2))],
-                         ids=["ifm", "difm"])
-def test_graph_replayed_step_equals_eager(cuda, builder, kw):
-    l_graph, w_graph, replayed, init = _train(builder, "auto", kw)
-    l_eager, w_eager, _, _ = _train(builder, "off", kw, init=init)
-    assert replayed > 0, "the training step was never replayed as a CUDA graph"
-    np.testing.assert_allclose(l_graph, l_eager, rtol=1e-5, atol=1e-6)
-    for k, v in w_eager.items():
-        np.testing.assert_allclose(w_graph[k], v, rtol=1e-4, atol=1e-6 + 1e-4 * float(np.abs(v).max()), err_msg=k)
-
-
 def test_ifm_step_runs_fm_weighted_and_writes_no_refined_block(cuda, monkeypatch):
     """The refined FM input m ⊙ x reaches FM as its factors: the step launches fm_weighted forward and backward, and
     the only materialised field scale is the dim-1 one of the linear lookups."""
@@ -253,7 +182,7 @@ def test_ifm_step_runs_fm_weighted_and_writes_no_refined_block(cuda, monkeypatch
             calls.append((_name, a[4] if _name == "field_scale_fwd" else None))
             return _real(*a, **kw)
         monkeypatch.setattr(K, name, spy)
-    _train("IFM", "off", dict(dnn_hidden_units=(16,)), steps=2)
+    H.train("IFM", "off", dict(dnn_hidden_units=(16,)), steps=2)
     names = [c[0] for c in calls]
     assert names.count("fm_weighted_fwd") == 2 and names.count("fm_weighted_bwd") == 2, names
     assert "fm_fwd" not in names
@@ -271,7 +200,7 @@ def test_refine_product_feeding_other_layers_is_materialised(cuda):
     from deepctr_b200.layers.utils import add_func, concat_func
     from oracle import ops as O
     rng = np.random.RandomState(9)
-    cols, x, y = _criteo(rng, n=256)
+    cols, x, y = H.criteo_like(rng, 256, n_sparse=10)
     cols = cols[:10]
     E.clear_session()
     features = build_input_features(cols)
@@ -311,7 +240,7 @@ def test_reference_test_configurations_train_with_dropout(cuda):
     from deepctr_b200.engine import SGD
     for builder in ("IFM", "DIFM"):
         for hidden in ((4,), (4, 4)):
-            cols, x, y = _criteo(np.random.RandomState(6))
+            cols, x, y = H.criteo_like(np.random.RandomState(6), 512, n_sparse=10)
             E.clear_session()
             model = getattr(M, builder)(cols, cols, dnn_hidden_units=hidden, dnn_dropout=0.5, l2_reg_linear=0,
                                         l2_reg_embedding=0)

@@ -1,58 +1,20 @@
-"""CPU: model-level pinning.
+"""CPU: model-level pinning of the five original builders (DeepFM, xDeepFM, DCN, AutoInt, DIN).
 
 The fixtures under tests/golden/models/ were produced by the REFERENCE's own composition code
-(/root/reference/deepctr/{feature_column,inputs}.py + the five builders, unmodified) under the
-torch-backed TF shim (tests/golden/generate_models.py).  Here:
-
-1. oracle/models.py (the CPU restatement the GPU parity tests lean on) reproduces their logits,
-   predictions, loss and every weight gradient;
-2. the deepctr_b200 builders create exactly the reference's weight set (names + shapes) for the same
-   feature columns - the precondition for loading reference weights by name.
+(deepctr/{feature_column,inputs}.py + the five builders, unmodified) under the torch-backed TF shim
+(tests/golden/generate_models.py).  The checks are model_golden_checks' (shared by every fixture family):
+oracle/models.py reproduces their logits, predictions, loss and every weight gradient, and the deepctr_b200
+builders create exactly the reference's weight set (names, shapes, trainable flags, order).  The builder graphs and
+keyword defaults are checked in tests/test_reference_builders_dropin.py.
 """
 import numpy as np
-import pytest
-import torch
 
-import golden_models as G
-from deepctr_b200 import feature_column as FC
+import model_golden_checks as C
 
-
-def test_fixture_set_covers_the_five_builders():
-    builders = set(G.Fixture(n).builder for n in G.CASES)
-    assert builders == {"DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN"}
-    assert len(G.CASES) >= 17
-
-
-@pytest.mark.parametrize("name", G.CASES)
-def test_oracle_matches_reference_model(name):
-    fx = G.Fixture(name)
-    W, leaves = G.oracle_weights(fx, requires_grad=True)
-    logit, pred = G.oracle_forward(fx, W, FC)
-    scale = float(np.abs(fx.logit).max())
-    np.testing.assert_allclose(logit.detach().numpy().reshape(-1, 1), fx.logit, rtol=1e-4, atol=1e-5 * max(scale, 1.0))
-    np.testing.assert_allclose(pred.detach().numpy().reshape(-1, 1), fx.out, rtol=1e-4, atol=1e-6)
-    loss = G.loss_of(fx, pred)
-    assert abs(float(loss.detach()) - fx.loss) <= 1e-5 * max(1.0, abs(fx.loss))
-    loss.backward()
-    for key, want in fx.g.items():
-        if G._ignored(key):
-            assert not np.any(want), key           # the reference's discarded lookup pass gets no gradient
-            continue
-        leaf = leaves[key]
-        got = leaf.grad.numpy() if leaf.grad is not None else np.zeros_like(want)
-        tol = 1e-4 * float(np.abs(want).max()) + 1e-7
-        np.testing.assert_allclose(got, want, rtol=1e-4, atol=tol, err_msg=key)
-
-
-@pytest.mark.parametrize("name", G.CASES)
-def test_builders_create_the_reference_weight_set(name):
-    fx = G.Fixture(name)
-    model = G.build_model(fx)
-    wm = G.weight_map(fx, model)           # raises on any name / shape difference
-    assert len(wm) == len([k for k in fx.w if not G._ignored(k)])
-    # trainable flags: everything the reference differentiates is trainable here and vice versa
-    for key, w in wm.items():
-        assert w.trainable == (key in fx.g), key
+T = C.model_tests("models")
+test_fixture_set_covers_the_five_builders = T.fixture_set
+test_oracle_matches_reference_model = T.oracle
+test_builders_create_the_reference_weight_set = T.weight_set
 
 
 def test_hash_tf_documentation_example():

@@ -1,64 +1,14 @@
-"""GPU: the CUDA models against MODEL-level golden vectors produced by the reference's own unmodified
-feature_column.py / inputs.py / builders (tests/golden/models/*.npz, tests/golden/generate_models.py):
-the reference's weights loaded by name, the same inputs, then
+"""GPU: the CUDA models of the five original builders against the MODEL-level golden vectors produced by the
+reference's own unmodified feature_column.py / inputs.py / builders (tests/golden/models/*.npz,
+tests/golden/generate_models.py), with model_golden_checks' forward and one-SGD-step checks (shared by every
+fixture family): the reference's weights loaded by name, the same inputs, then
 
 * logits and predictions within 1e-4 relative (north_star), in both GEMM precisions;
 * one SGD step: the loss and every weight's update  -lr * dL/dw  against the gradient torch autograd
   took THROUGH the reference's graph (tables included: dense Keras semantics).
 """
-import numpy as np
-import pytest
+import model_golden_checks as C
 
-import golden_models as G
-
-pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("gemm_precision")]
-
-
-def _logits(model, x):
-    """pre-activation logits of the compiled graph (what PredictionLayer receives)."""
-    from deepctr_b200 import engine as E
-    model._materialize()
-    feed = model._feed(x)
-    logit_t, head = model._head()
-    vals = model._run(feed, False, upto=head)
-    return E.contiguous(vals[id(logit_t)]).reshape(-1, 1).cpu().numpy()
-
-
-def _tol(want):
-    from deepctr_b200 import ops, _lib as L
-    scale = max(float(np.abs(want).max()), 1e-3)
-    return (1e-4 if ops.GEMM_PRECISION == L.GEMM_BF16X3 else 2e-5) * scale
-
-
-@pytest.mark.parametrize("name", G.CASES)
-def test_model_forward_matches_reference(cuda, name):
-    fx = G.Fixture(name)
-    model = G.build_model(fx)
-    G.assign_weights(fx, model)
-    x = fx.inputs()
-    if not (fx.training and "dice" in name):       # predict() runs Dice on its moving statistics
-        got = _logits(model, x)
-        np.testing.assert_allclose(got, fx.logit, rtol=1e-4, atol=_tol(fx.logit))
-        pred = model.predict(x, batch_size=len(fx.y))
-        np.testing.assert_allclose(pred, fx.out, rtol=1e-4, atol=_tol(fx.out))
-
-
-@pytest.mark.parametrize("name", G.CASES)
-def test_model_sgd_step_matches_reference_gradients(cuda, name):
-    from deepctr_b200.engine import SGD
-    fx = G.Fixture(name)
-    if "dice" in name and not fx.training:
-        pytest.skip("fixture differentiates Dice in inference mode; a training step uses batch statistics")
-    model = G.build_model(fx)
-    wm = G.assign_weights(fx, model)
-    lr = 0.5
-    model.compile(SGD(lr), "binary_crossentropy" if fx.task == "binary" else "mse", embedding_update="dense")
-    loss = model.train_on_batch(fx.inputs(), fx.y)
-    assert abs(loss - fx.loss) <= 2e-4 * max(1.0, abs(fx.loss)), (loss, fx.loss)
-    for key, w in wm.items():
-        if key not in fx.g:
-            continue
-        want = fx.g[key]
-        got = (fx.w[key] - w.value()) / lr
-        gmax = float(np.abs(want).max())
-        np.testing.assert_allclose(got, want, rtol=2e-3, atol=3e-4 * gmax + 2e-6, err_msg=key)
+T = C.gpu_model_tests("models")
+test_model_forward_matches_reference = T.forward
+test_model_sgd_step_matches_reference_gradients = T.sgd_step

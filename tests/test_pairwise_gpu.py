@@ -4,18 +4,27 @@
 * b2ctr_afm_fwd / _bwd and b2ctr_bi_interaction_fwd / _bwd against a float64 torch restatement over F = 2 / 26 / 64,
   E = 4 / 32, A = 1 / 8, an input that is a window of a wider buffer (ldx > F*E) and batches that are not a multiple
   of the CTA's samples; the AFM backward is bit-identical from run to run;
-* model fixtures (tests/golden/models_pairwise/): logits and one SGD step in both GEMM precisions;
-* a graph-replayed training step equals an eager one; 'sparse' embedding updates train AFM;
+* 'sparse' embedding updates train AFM ;
+* model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions; a graph-replayed
+  training step equals an eager one;
 * the C2 shape (26 fields, E = 32, A = 8, B = 65536).
 """
 import numpy as np
 import pytest
 import torch
 
+import b2_helpers as H
 import golden_models as G
-import test_pairwise_goldens as PG
+import model_golden_checks as C
 
 pytestmark = pytest.mark.gpu
+
+T = C.gpu_model_tests("pairwise")
+test_model_forward_matches_reference = T.forward
+test_model_sgd_step_matches_reference_gradients = T.sgd_step
+test_graph_replayed_step_equals_eager = C.graph_replay_test([("NFM", dict(dnn_hidden_units=(32, 16))),
+                                                          ("AFM", dict(n_dense=0, attention_factor=8)),
+                                                          ("AFM", dict(n_dense=0, use_attention=False))])
 
 
 def _ref_afm(x, W, b, h):
@@ -44,11 +53,11 @@ def _afm_weights(cuda, E, A, rng):
     return W, b, h
 
 
-@pytest.mark.parametrize("name", PG.LAYER_CASES)
+@pytest.mark.parametrize("name", G.layer_cases("pairwise"))
 def test_layer_fixture(cuda, name):
     from deepctr_b200 import engine as E, kernels as K
     from deepctr_b200.layers import AFMLayer, BiInteractionPooling
-    meta, d = PG.load_layer(name)
+    meta, d = G.load_layer("pairwise", name)
     x = torch.tensor(d["x"], device=cuda)
     B, F, Ed = x.shape
     E.clear_session()
@@ -90,18 +99,13 @@ def _check_afm(cuda, B, F, E, A, tail, seed):
     W64, b64, h64 = (t.double().requires_grad_(True) for t in (W, b, h))
     ref = _ref_afm(x64, W64, b64, h64)
     (ref * g.double()).sum().backward()
-
-    def close(got, want, what, floor=0.0):
-        scale = max(float(want.abs().max()), floor)
-        err = float((got.double() - want).abs().max()) / scale
-        assert err < 2e-5, "%s: max error %.3e relative to max |value|" % (what, err)
-    close(att, ref.detach(), "att")
-    close(dx.reshape(B, F, E), x64.grad, "dx")
+    H.close(att, ref.detach(), "att")
+    H.close(dx.reshape(B, F, E), x64.grad, "dx")
     # floor: with F = 2 the softmax is exactly 1, ds = 0 and the weight gradients vanish in float64, while fp32
     # keeps the rounding of <g, prod> - <g, att> (two summation orders of the same sum)
-    close(dW, W64.grad, "dW", 1e-3 * B)
-    close(db, b64.grad, "dbias", 1e-3 * B)
-    close(dh, h64.grad, "dh", 1e-3 * B)
+    H.close(dW, W64.grad, "dW", floor=1e-3 * B)
+    H.close(db, b64.grad, "dbias", floor=1e-3 * B)
+    H.close(dh, h64.grad, "dh", floor=1e-3 * B)
     # state: max and sum of the softmax of the scores
     assert torch.isfinite(state).all() and bool((state[:, 1] >= 1.0 - 1e-6).all())
     assert torch.equal(buf[:, F * E:], tail_before)     # the dense tail behind the window is never written
@@ -154,83 +158,12 @@ def test_afm_kernel_rejects_unsupported_shapes(cuda):
         K.afm_fwd(x, 65 * 4, 65, 4, W, b, h, 4)
 
 
-# ---- model level ----------------------------------------------------------------------------------
-def _model(fx):
-    model = PG.build(fx)
-    return model, G.assign_weights(fx, model)
-
-
-@pytest.mark.usefixtures("gemm_precision")
-@pytest.mark.parametrize("name", PG.MODEL_CASES)
-def test_model_forward_matches_reference(cuda, name):
-    from test_model_goldens_gpu import _logits, _tol
-    fx = PG.Fixture(name)
-    model, _ = _model(fx)
-    x = fx.inputs()
-    np.testing.assert_allclose(_logits(model, x), fx.logit, rtol=1e-4, atol=_tol(fx.logit))
-    np.testing.assert_allclose(model.predict(x, batch_size=len(fx.y)), fx.out, rtol=1e-4, atol=_tol(fx.out))
-
-
-@pytest.mark.usefixtures("gemm_precision")
-@pytest.mark.parametrize("name", PG.MODEL_CASES)
-def test_model_sgd_step_matches_reference_gradients(cuda, name):
-    from deepctr_b200.engine import SGD
-    fx = PG.Fixture(name)
-    model, wm = _model(fx)
-    lr = 0.5
-    model.compile(SGD(lr), "binary_crossentropy", embedding_update="dense")
-    loss = model.train_on_batch(fx.inputs(), fx.y)
-    assert abs(loss - fx.loss) <= 2e-4 * max(1.0, abs(fx.loss)), (loss, fx.loss)
-    for key, w in wm.items():
-        if key not in fx.g:
-            continue
-        want = fx.g[key]
-        got = (fx.w[key] - w.value()) / lr
-        np.testing.assert_allclose(got, want, rtol=2e-3, atol=3e-4 * float(np.abs(want).max()) + 2e-6, err_msg=key)
-
-
-def _criteo_model(builder, rng, n_dense, dim=8, **kw):
-    from deepctr_b200 import engine as E, models as M
-    from deepctr_b200 import feature_column as FC
-    cols = [FC.SparseFeat("C%d" % i, 50 + i, dim) for i in range(10)]
-    cols += [FC.DenseFeat("I%d" % i, 1) for i in range(n_dense)]
-    E.clear_session()
-    model = getattr(M, builder)(cols, cols, l2_reg_linear=0, l2_reg_embedding=0, seed=3, **kw)
-    n = 512
-    x = {"C%d" % i: rng.randint(0, 50 + i, size=n).astype(np.int32) for i in range(10)}
-    x.update({"I%d" % i: rng.rand(n).astype(np.float32) for i in range(n_dense)})
-    y = (rng.rand(n) < 0.3).astype(np.float32)
-    return model, x, y
-
-
-@pytest.mark.parametrize("builder,kw", [("NFM", dict(dnn_hidden_units=(32, 16))),
-                                        ("AFM", dict(attention_factor=8)),
-                                        ("AFM", dict(use_attention=False))])
-def test_graph_replayed_step_equals_eager(cuda, builder, kw):
-    from deepctr_b200.engine import SGD
-    runs, init = [], None
-    for graph in ("auto", "off"):
-        model, x, y = _criteo_model(builder, np.random.RandomState(4), 3 if builder == "NFM" else 0, **kw)
-        if init is None:         # Keras leaves the final Dense kernel unseeded: start both runs from the same weights
-            init = [w.value() for w in model.weights]
-        else:
-            model.set_weights(init)
-        model.compile(SGD(0.05), "binary_crossentropy", embedding_update="sparse", step_graph=graph)
-        losses = [model.train_on_batch(x, y) for _ in range(6)]
-        runs.append((losses, {w.name: w.value() for w in model.weights}, model.replayed_launches))
-    (l_graph, w_graph, replayed), (l_eager, w_eager, _) = runs
-    assert replayed > 0, "the training step was never replayed as a CUDA graph"
-    np.testing.assert_allclose(l_graph, l_eager, rtol=1e-5, atol=1e-6)
-    for k, v in w_eager.items():
-        np.testing.assert_allclose(w_graph[k], v, rtol=1e-4, atol=1e-6 + 1e-4 * float(np.abs(v).max()), err_msg=k)
-
-
 def test_afm_sparse_update_trains(cuda):
     """AFM's dx feeds the fused scatter-update: with l2 = 0, 'sparse' SGD equals 'dense' SGD."""
     from deepctr_b200.engine import SGD
     res, init = [], None
     for mode in ("sparse", "dense"):
-        model, x, y = _criteo_model("AFM", np.random.RandomState(9), 0, attention_factor=4, l2_reg_att=0)
+        model, x, y = H.criteo_model("AFM", np.random.RandomState(9), n_dense=0, attention_factor=4, l2_reg_att=0)
         if init is None:
             init = [w.value() for w in model.weights]
         else:

@@ -7,28 +7,39 @@
 * the C2 shape (B = 65536, F = 26, E = 32): the input a window of the [B, 848] gather buffer, the scores at column
   845 of a wider buffer;
 * layer fixtures of the reference's own InnerProductLayer / OutterProductLayer (tests/golden/pnn/);
-* model fixtures (tests/golden/models_pnn/): logits and one SGD step in both GEMM precisions, with the products
-  placed in the gather buffer and unplaced;
-* a graph-replayed training step equals an eager one; placed and unplaced PNN agree to rounding; the placed step
-  copies no product-sized block; the reference test's dnn_dropout=0.5 configuration trains with a finite loss.
+* the placed step copies no product-sized block; the reference test's dnn_dropout=0.5 configuration trains with a
+  finite loss;
+* model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions, placed and unplaced;
+  a graph-replayed training step equals an eager one; the placement gives the results of the unplaced graph.
 """
 import numpy as np
 import pytest
 import torch
 
+import b2_helpers as H
 import golden_models as G
+import model_golden_checks as C
+from model_golden_checks import placement  # noqa: F401  (the placed / unplaced parameter)
 import pnn_oracle as PO
-import test_pnn_goldens as PG
 
 pytestmark = pytest.mark.gpu
 
+T = C.gpu_model_tests("pnn")
+test_model_forward_matches_reference = T.forward
+test_model_sgd_step_matches_reference_gradients = T.sgd_step
+test_graph_replayed_step_equals_eager = C.graph_replay_test([
+    pytest.param("PNN", dict(dnn_hidden_units=(32, 16)), id="ipnn"),
+    pytest.param("PNN", dict(dnn_hidden_units=(32, 16), use_inner=False, use_outter=True), id="opnn_mat"),
+    pytest.param("PNN", dict(dnn_hidden_units=(32,), use_outter=True, kernel_type="vec"), id="both_vec"),
+    pytest.param("PNN", dict(dnn_hidden_units=(32,), use_inner=False, use_outter=True, kernel_type="num"),
+                 id="opnn_num")])
+test_placement_gives_the_unplaced_results = C.placement_test([
+    pytest.param("PNN", dict(dnn_hidden_units=(32, 16)), 1e-5, 1e-6, id="ipnn"),
+    pytest.param("PNN", dict(dnn_hidden_units=(32,), use_inner=False, use_outter=True), 1e-5, 1e-6, id="opnn_mat"),
+    pytest.param("PNN", dict(dnn_hidden_units=(32,), use_outter=True, kernel_type="vec"), 1e-5, 1e-6, id="both_vec"),
+    pytest.param("PNN", dict(dnn_hidden_units=(32,), use_outter=True, kernel_type="num"), 1e-5, 1e-6, id="both_num")])
+
 MODES = ["inner", "elementwise", "vec", "num", "mat"]
-
-
-def _close(got, want, what, tol=2e-5):
-    scale = max(float(want.abs().max()), 1e-30)
-    err = float((got.double() - want).abs().max()) / scale
-    assert err < tol, "%s: max error %.3e relative to max |value|" % (what, err)
 
 
 def _kernel(rng, mode, F, E, cuda):
@@ -83,10 +94,10 @@ def _check(cuda, mode, B, F, E, seed, ldx=None, col0=3, ld=None, chunk=4096):
         x64 = xw[sl].double().reshape(-1, F, E).requires_grad_(True)
         ref = _ref(x64, mode, K64)
         (ref * g[sl, col0:col0 + ncols].double()).sum().backward()
-        _close(out[sl, col0:col0 + ncols], ref.detach(), "%s out" % mode)
-        _close(dx[sl].reshape(-1, F, E), x64.grad, "%s dx" % mode)
+        H.close(out[sl, col0:col0 + ncols], ref.detach(), "%s out" % mode)
+        H.close(dx[sl].reshape(-1, F, E), x64.grad, "%s dx" % mode)
     if K64 is not None:
-        _close(dK, K64.grad, "%s dK" % mode, 1e-4)
+        H.close(dK, K64.grad, "%s dK" % mode, 1e-4)
     else:
         assert dK is None
     return (g, ld, col0, xw, ldx, Kw, dx, dK)
@@ -137,12 +148,12 @@ def test_kernels_reject_unsupported_shapes(cuda):
                         col0=3)
 
 
-@pytest.mark.parametrize("name", PG.LAYER_CASES)
+@pytest.mark.parametrize("name", G.layer_cases("pnn"))
 def test_layer_fixture(cuda, name):
     """The layers themselves, called on the F [B,1,E] slices, against the reference's outputs and gradients."""
     from deepctr_b200 import engine as E
     from deepctr_b200 import layers as Lyr
-    meta, d = PG.load_layer(name)
+    meta, d = G.load_layer("pnn", name)
     E.clear_session()
     F = d["x"].shape[1]
     vars_in = [E.to_var(np.ascontiguousarray(d["x"][:, f:f + 1])) for f in range(F)]
@@ -165,117 +176,16 @@ def test_layer_fixture(cuda, name):
         np.testing.assert_allclose(layer.kernel.grad.cpu().numpy(), d["g_kernel"], **tol)
 
 
-# ---- model level ----------------------------------------------------------------------------------
-@pytest.fixture(params=[True, False], ids=["placed", "unplaced"])
-def placement(request):
-    from deepctr_b200 import inputs as I
-    I.DNN_INPUT_PLACEMENT = request.param
-    yield request.param
-    I.DNN_INPUT_PLACEMENT = True
-
-
-def _model(fx):
-    model = PG.build(fx)
-    return model, G.assign_weights(fx, model)
-
-
-@pytest.mark.usefixtures("gemm_precision", "placement")
-@pytest.mark.parametrize("name", PG.MODEL_CASES)
-def test_model_forward_matches_reference(cuda, name):
-    from test_model_goldens_gpu import _logits, _tol
-    fx = PG.Fixture(name)
-    model, _ = _model(fx)
-    x = fx.inputs()
-    np.testing.assert_allclose(_logits(model, x), fx.logit, rtol=1e-4, atol=_tol(fx.logit))
-    np.testing.assert_allclose(model.predict(x, batch_size=len(fx.y)), fx.out, rtol=1e-4, atol=_tol(fx.out))
-
-
-@pytest.mark.usefixtures("gemm_precision", "placement")
-@pytest.mark.parametrize("name", PG.MODEL_CASES)
-def test_model_sgd_step_matches_reference_gradients(cuda, name):
-    from deepctr_b200.engine import SGD
-    fx = PG.Fixture(name)
-    model, wm = _model(fx)
-    lr = 0.5
-    model.compile(SGD(lr), "mse" if fx.task == "regression" else "binary_crossentropy", embedding_update="dense")
-    loss = model.train_on_batch(fx.inputs(), fx.y)
-    assert abs(loss - fx.loss) <= 2e-4 * max(1.0, abs(fx.loss)), (loss, fx.loss)
-    for key, w in wm.items():
-        if key not in fx.g:
-            continue
-        want = fx.g[key]
-        got = (fx.w[key] - w.value()) / lr
-        np.testing.assert_allclose(got, want, rtol=2e-3, atol=3e-4 * float(np.abs(want).max()) + 2e-6, err_msg=key)
-
-
-def _criteo_model(rng, n=512, dim=8, **kw):
-    from deepctr_b200 import engine as E, models as M
-    from deepctr_b200 import feature_column as FC
-    cols = [FC.SparseFeat("C%d" % i, 50 + i, dim) for i in range(10)] + [FC.DenseFeat("I%d" % i, 1) for i in range(3)]
-    E.clear_session()
-    model = M.PNN(cols, l2_reg_embedding=0, seed=3, **kw)
-    x = {"C%d" % i: rng.randint(0, 50 + i, size=n).astype(np.int32) for i in range(10)}
-    x.update({"I%d" % i: rng.rand(n).astype(np.float32) for i in range(3)})
-    y = (rng.rand(n) < 0.3).astype(np.float32)
-    return model, x, y
-
-
-def _train(graph, kw, steps=6, init=None, placed=True):
-    from deepctr_b200 import inputs as I
-    from deepctr_b200.engine import SGD
-    I.DNN_INPUT_PLACEMENT = placed
-    try:
-        model, x, y = _criteo_model(np.random.RandomState(4), **kw)
-    finally:
-        I.DNN_INPUT_PLACEMENT = True
-    assert bool(model.planner.pnn_places) == (placed and (kw.get("use_inner", True) or kw.get("use_outter", False)))
-    if init is None:            # Keras leaves the final Dense kernel unseeded: start every run from the same weights
-        init = [w.value() for w in model.weights]
-    else:
-        model.set_weights(init)
-    model.compile(SGD(0.05), "binary_crossentropy", embedding_update="sparse", step_graph=graph)
-    losses = [model.train_on_batch(x, y) for _ in range(steps)]
-    return losses, {w.name: w.value() for w in model.weights}, model.replayed_launches, init
-
-
-@pytest.mark.parametrize("kw", [dict(dnn_hidden_units=(32, 16)),
-                                dict(dnn_hidden_units=(32, 16), use_inner=False, use_outter=True),
-                                dict(dnn_hidden_units=(32,), use_outter=True, kernel_type="vec"),
-                                dict(dnn_hidden_units=(32,), use_inner=False, use_outter=True, kernel_type="num")],
-                         ids=["ipnn", "opnn_mat", "both_vec", "opnn_num"])
-def test_graph_replayed_step_equals_eager(cuda, kw):
-    l_graph, w_graph, replayed, init = _train("auto", kw)
-    l_eager, w_eager, _, _ = _train("off", kw, init=init)
-    assert replayed > 0, "the training step was never replayed as a CUDA graph"
-    np.testing.assert_allclose(l_graph, l_eager, rtol=1e-5, atol=1e-6)
-    for k, v in w_eager.items():
-        np.testing.assert_allclose(w_graph[k], v, rtol=1e-4, atol=1e-6 + 1e-4 * float(np.abs(v).max()), err_msg=k)
-
-
 def test_reference_test_configuration_trains_with_dropout(cuda):
     """The reference's tests/models/PNN_test.py configuration: dnn_hidden_units=[4, 4], dnn_dropout=0.5, each of the
     use_inner / use_outter combinations; a few steps of training give finite losses."""
     from deepctr_b200.engine import SGD
     for use_inner, use_outter in ((True, True), (True, False), (False, True), (False, False)):
-        model, x, y = _criteo_model(np.random.RandomState(6), dnn_hidden_units=[4, 4], dnn_dropout=0.5,
-                                    use_inner=use_inner, use_outter=use_outter)
+        model, x, y = H.criteo_model("PNN", np.random.RandomState(6), dnn_hidden_units=[4, 4], dnn_dropout=0.5,
+                                     use_inner=use_inner, use_outter=use_outter)
         model.compile(SGD(0.05), "binary_crossentropy", embedding_update="sparse")
         losses = [model.train_on_batch(x, y) for _ in range(3)]
         assert np.isfinite(losses).all(), (use_inner, use_outter, losses)
-
-
-@pytest.mark.parametrize("kw", [dict(dnn_hidden_units=(32, 16)),
-                                dict(dnn_hidden_units=(32,), use_inner=False, use_outter=True),
-                                dict(dnn_hidden_units=(32,), use_outter=True, kernel_type="vec"),
-                                dict(dnn_hidden_units=(32,), use_outter=True, kernel_type="num")],
-                         ids=["ipnn", "opnn_mat", "both_vec", "both_num"])
-def test_placement_gives_the_unplaced_results(cuda, kw):
-    # the same arithmetic on differently laid out operands: six steps agree to rounding
-    l_p, w_p, _, init = _train("off", kw)
-    l_u, w_u, _, _ = _train("off", kw, init=init, placed=False)
-    np.testing.assert_allclose(l_p, l_u, rtol=1e-6, atol=0)
-    for k, v in w_u.items():
-        np.testing.assert_allclose(w_p[k], v, rtol=1e-5, atol=1e-6 * float(np.abs(v).max()), err_msg=k)
 
 
 def test_placed_step_copies_no_product_block(cuda, monkeypatch):
@@ -299,7 +209,7 @@ def test_placed_step_copies_no_product_block(cuda, monkeypatch):
     for placed in (True, False):
         I.DNN_INPUT_PLACEMENT = placed
         try:
-            model, x, y = _criteo_model(np.random.RandomState(5), dnn_hidden_units=(16,))
+            model, x, y = H.criteo_model("PNN", np.random.RandomState(5), dnn_hidden_units=(16,))
         finally:
             I.DNN_INPUT_PLACEMENT = True
         assert bool(model.planner.pnn_places) == placed
