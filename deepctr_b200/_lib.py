@@ -102,6 +102,9 @@ SIGNATURES = {
     "b2ctr_embed_gather_uniform_fwd": (_i32, [C.POINTER(UniformGather), _i64, _vp]),
     "b2ctr_embed_scatter_uniform_bwd": (_i32, [C.POINTER(UniformGather), _vp, _vp, _vp, _f32, _f32,
                                                _i64, _vp]),
+    "b2ctr_embed_gather_uniform_fwd_ex": (_i32, [C.POINTER(UniformGather), _vp, _vp, _i64, _i64, _vp]),
+    "b2ctr_embed_scatter_uniform_bwd_ex": (_i32, [C.POINTER(UniformGather), _vp, _vp, _vp, _vp, _f32, _f32,
+                                                  _i64, _vp]),
     "b2ctr_embed_oob_count": (_i32, [C.POINTER(C.c_int64), _i32, _vp]),
     "b2ctr_embed_update_sorted_workspace_bytes": (_sz, [_i32, _i32, _i64]),
     "b2ctr_embed_update_sorted": (_i32, [C.POINTER(UniformGather), _vp, _vp, _vp, _i32, _f32, _f32, _f32,

@@ -1,6 +1,7 @@
 // common.cuh — shared helpers for libb2ctr (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <atomic>
@@ -55,6 +56,9 @@ static inline int64_t planes_cols_pad(int64_t cols) { return cols <= 64 ? 64 : (
 
 // ---- device helpers -------------------------------------------------------------------------
 #ifdef __CUDACC__
+__device__ __forceinline__ uint32_t pack_bf16(__nv_bfloat16 lo, __nv_bfloat16 hi) {
+  return (uint32_t)__bfloat16_as_ushort(lo) | ((uint32_t)__bfloat16_as_ushort(hi) << 16);
+}
 
 __device__ __forceinline__ float4 ldg_stream_f4(const float* p) {
   // read-once data (embedding rows, activations): do not allocate in L1

@@ -7,7 +7,9 @@
 // HBM-bound integer/byte work: no tensor cores.  Design rules (DESIGN.md §3):
 //   * one launch for all tables; descriptors travel by value in the kernel parameter block;
 //   * 128-bit row accesses, rows never staged through L1 (ld.global.nc.L1::no_allocate);
-//   * every lane keeps up to 8 independent 16 B loads in flight (Little's law at 6.5 TB/s);
+//   * every lane keeps several independent 16 B loads in flight.  Little's law on an H100 SXM: 3.35 TB/s x ~0.8 us
+//     of loaded HBM latency is ~2.7 MB in flight, i.e. ~20 KB per SM = ~1300 16 B loads; 32 warps x 32 lanes x
+//     4-7 loads per lane covers it;
 //   * row updates are REDG.E.ADD.F32x4 (the add executes in the L2 slice, no read by the SM);
 //   * grids are whole multiples of the 132 SMs.
 #include "common.cuh"
@@ -415,7 +417,27 @@ struct UniParams {
   float* const* peer_lin;
   int32_t world;
   int32_t wshift;
+  // FM sum vectors S[b, 0:dim] (gather: written, scatter: read instead of re-summing x), or NULL
+  float* fm_sum;
+  // gather only: bf16 hi/lo planes (b2ctr_split_planes layout) of x[:, 0:xp_cols], row pitch xp_pitch, or NULL
+  __nv_bfloat16* xp_hi;
+  __nv_bfloat16* xp_lo;
+  int64_t xp_pitch;
+  int64_t xp_rows_pad;
 };
+
+// hi = bf16_rn(v), lo = bf16_rn(v - hi): the values b2ctr_split_planes writes
+__device__ __forceinline__ void store_planes4(const UniParams& p, int64_t off, float4 v) {
+  const __nv_bfloat16 h0 = __float2bfloat16_rn(v.x), h1 = __float2bfloat16_rn(v.y);
+  const __nv_bfloat16 h2 = __float2bfloat16_rn(v.z), h3 = __float2bfloat16_rn(v.w);
+  uint2 h, l;
+  h.x = pack_bf16(h0, h1);
+  h.y = pack_bf16(h2, h3);
+  l.x = pack_bf16(__float2bfloat16_rn(v.x - __bfloat162float(h0)), __float2bfloat16_rn(v.y - __bfloat162float(h1)));
+  l.y = pack_bf16(__float2bfloat16_rn(v.z - __bfloat162float(h2)), __float2bfloat16_rn(v.w - __bfloat162float(h3)));
+  *reinterpret_cast<uint2*>(p.xp_hi + off) = h;
+  *reinterpret_cast<uint2*>(p.xp_lo + off) = l;
+}
 
 // peer (NVLink) accesses: no read-only / L2-policy qualifiers - the line lives in the owner's L2
 __device__ __forceinline__ float4 ld_peer_f4(const float* p) {
@@ -451,9 +473,12 @@ __device__ __forceinline__ int64_t uni_id(const UniParams& p, int f, int64_t b) 
 // LPR = lanes per row (= dim/4); RPI = rows per warp iteration; each lane keeps U 16-byte loads in flight.
 // Latency hiding (ncu, profiles/r1_embed_before.txt: 40 % DRAM, 35 % warps active): the id -> row -> store
 // chain is broken by prefetching the NEXT sample's ids before the current rows are requested, and the
-// register budget is capped at 64 (4 CTAs = 32 warps per SM).
-template <int LPR, bool SHARD>
-__global__ void __launch_bounds__(256, SHARD ? 3 : 4)
+// register budget is capped at 64 (4 CTAs = 32 warps per SM).  EXTRA: the instantiation that may also store S
+// (p.fm_sum) and X's bf16 planes (p.xp_hi); those stores need 80 registers, so it runs 3 CTAs = 24 warps per SM,
+// which still keep 24 x 32 x 7 x 16 B = 86 KB of row loads in flight per SM, four times the ~20 KB the H100's HBM
+// needs (see the top of this file), and it is launched as one wave of 132 x 3 CTAs.
+template <int LPR, bool SHARD, bool EXTRA>
+__global__ void __launch_bounds__(256, (SHARD || EXTRA) ? 3 : 4)
     gather_uniform_fwd_kernel(const __grid_constant__ UniParams p, int64_t batch) {
   constexpr int RPI = 32 / LPR;
   constexpr int U = 7;   // 7 x RPI(4) = 28 >= 26 Criteo fields in one pass at dim 32
@@ -505,6 +530,7 @@ __global__ void __launch_bounds__(256, SHARD ? 3 : 4)
         const int f = f0 + u * RPI + slot;
         if (f < F) {
           stg_stream_f4_pol(xrow + (int64_t)f * dim + chunk * 4, v[u], pol_stream);
+          if (EXTRA && p.xp_hi) store_planes4(p, b * p.xp_pitch + (int64_t)f * dim + chunk * 4, v[u]);
           if ((p.fm_mask >> f) & 1ull) {
             s.x += v[u].x; s.y += v[u].y; s.z += v[u].z; s.w += v[u].w;
             q += v[u].x * v[u].x + v[u].y * v[u].y + v[u].z * v[u].z + v[u].w * v[u].w;
@@ -521,6 +547,8 @@ __global__ void __launch_bounds__(256, SHARD ? 3 : 4)
         s.z += __shfl_xor_sync(0xffffffffu, s.z, o);
         s.w += __shfl_xor_sync(0xffffffffu, s.w, o);
       }
+      // S as the scatter needs it: ascending f per lane slot, then the xor tree above
+      if (EXTRA && p.fm_sum != nullptr && slot == 0) *reinterpret_cast<float4*>(p.fm_sum + b * dim + chunk * 4) = s;
       float sq = slot == 0 ? (s.x * s.x + s.y * s.y + s.z * s.z + s.w * s.w) : 0.f;
       sq = warp_sum(sq);
       q = warp_sum(q);
@@ -548,13 +576,32 @@ __global__ void __launch_bounds__(256, SHARD ? 3 : 4)
       const int j = (int)(c - c0);
       xrow[c] = j < p.ndense ? p.dense[b * p.dense_ld + j] : 0.f;
     }
+    if (EXTRA && p.xp_hi) {      // plane columns behind the embeddings: the dense features, then zeros up to the pitch
+      for (int64_t c = c0 + lane; c < p.xp_pitch; c += 32) {
+        const int j = (int)(c - c0);
+        const float v = j < p.ndense ? p.dense[b * p.dense_ld + j] : 0.f;
+        const __nv_bfloat16 h = __float2bfloat16_rn(v);
+        p.xp_hi[b * p.xp_pitch + c] = h;
+        p.xp_lo[b * p.xp_pitch + c] = __float2bfloat16_rn(v - __bfloat162float(h));
+      }
+    }
     id0 = nid0;
     id1 = nid1;
+  }
+  if (EXTRA && p.xp_hi) {        // plane rows [batch, rows_pad) are zero
+    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+    for (int64_t r = b; r < p.xp_rows_pad; r += nwarps)
+      for (int64_t c = lane * 8; c < p.xp_pitch; c += 256) {
+        *reinterpret_cast<uint4*>(p.xp_hi + r * p.xp_pitch + c) = z;
+        *reinterpret_cast<uint4*>(p.xp_lo + r * p.xp_pitch + c) = z;
+      }
   }
 }
 
 // Backward: 4 dx + 4 x loads in flight per lane, reds issued as soon as a chunk's gradient is formed
-// (fire-and-forget), ids re-broadcast by shuffle instead of being kept in registers -> 64 registers.
+// (fire-and-forget), ids re-broadcast by shuffle instead of being kept in registers.  With the gather's S
+// (p.fm_sum) the first red of a sample waits only for its own dx and x rows, not for a pass over all F rows; X is
+// still read once, for the x of the Jacobian.
 template <int LPR, bool SHARD>
 __global__ void __launch_bounds__(256, SHARD ? 2 : 3)
     scatter_uniform_bwd_kernel(const __grid_constant__ UniParams p, const float* __restrict__ dx,
@@ -583,7 +630,10 @@ __global__ void __launch_bounds__(256, SHARD ? 2 : 3)
     const float* dxrow = dx ? dx + b * p.ldx : nullptr;
     const float gfm = dfm ? dfm[b] : 0.f;
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (dfm) {
+    if (dfm && p.fm_sum) {
+      s = *reinterpret_cast<const float4*>(p.fm_sum + b * dim + chunk * 4);   // the gather's S
+    } else if (dfm) {
+      // no stored S: sum the FM rows of x in the gather's order (ascending f per lane slot, then the xor tree)
       for (int f0 = 0; f0 < F; f0 += U * RPI) {
         float4 v[U];
 #pragma unroll
@@ -614,7 +664,8 @@ __global__ void __launch_bounds__(256, SHARD ? 2 : 3)
         if (f < F) {
           const int64_t off = (int64_t)f * dim + chunk * 4;
           if (dxrow) g[u] = ldg_stream_f4_pol(dxrow + off, pol_stream);
-          if (dfm && ((p.fm_mask >> f) & 1ull)) xv[u] = *reinterpret_cast<const float4*>(xrow + off);  // L1 hit
+          // x for the Jacobian: an L1 hit after the pre-pass, else (stored S) the one read of the row
+          if (dfm && ((p.fm_mask >> f) & 1ull)) xv[u] = *reinterpret_cast<const float4*>(xrow + off);
         }
       }
 #pragma unroll
@@ -815,7 +866,22 @@ static b2ctr_status_t fill_uni(const b2ctr_uniform_gather_t* g, UniParams* p) {
   p->idx_dtype = g->feats[0].idx_dtype;
   p->has_lin = g->world > 1 ? (g->peer_lin_tables != nullptr) : (g->lin_tables != nullptr);
   p->store_grads = (g->flags & B2CTR_UNIFORM_STORE_GRADS) ? 1 : 0;
+  p->fm_sum = nullptr;
+  p->xp_hi = p->xp_lo = nullptr;
+  p->xp_pitch = p->xp_rows_pad = 0;
   return B2CTR_OK;
+}
+
+template <bool SHARD, bool EXTRA>
+static void launch_gather(const UniParams& p, int64_t batch, int grid, cudaStream_t st) {
+  switch (p.dim / 4) {
+    case 1: gather_uniform_fwd_kernel<1, SHARD, EXTRA><<<grid, 256, 0, st>>>(p, batch); break;
+    case 2: gather_uniform_fwd_kernel<2, SHARD, EXTRA><<<grid, 256, 0, st>>>(p, batch); break;
+    case 4: gather_uniform_fwd_kernel<4, SHARD, EXTRA><<<grid, 256, 0, st>>>(p, batch); break;
+    case 8: gather_uniform_fwd_kernel<8, SHARD, EXTRA><<<grid, 256, 0, st>>>(p, batch); break;
+    case 16: gather_uniform_fwd_kernel<16, SHARD, EXTRA><<<grid, 256, 0, st>>>(p, batch); break;
+    default: gather_uniform_fwd_kernel<32, SHARD, EXTRA><<<grid, 256, 0, st>>>(p, batch); break;
+  }
 }
 
 }  // namespace b2ctr
@@ -877,13 +943,36 @@ b2ctr_status_t b2ctr_embed_scatter_add(const b2ctr_feature_t* feats, int32_t nfe
 
 b2ctr_status_t b2ctr_embed_gather_uniform_fwd(const b2ctr_uniform_gather_t* g, int64_t batch,
                                               void* stream) {
+  return b2ctr_embed_gather_uniform_fwd_ex(g, nullptr, nullptr, 0, batch, stream);
+}
+
+b2ctr_status_t b2ctr_embed_gather_uniform_fwd_ex(const b2ctr_uniform_gather_t* g, float* fm_sum, void* x_planes,
+                                                 int64_t x_planes_cols, int64_t batch, void* stream) {
   UniParams p;
   b2ctr_status_t s = fill_uni(g, &p);
   if (s != B2CTR_OK) return s;
+  B2_REQUIRE(!fm_sum || (g->fm && aligned16(fm_sum)), "uniform gather: fm_sum needs fm and 16-byte alignment");
+  p.fm_sum = fm_sum;
+  if (x_planes) {
+    B2_REQUIRE(x_planes_cols >= (int64_t)g->nfeat * p.dim + g->ndense && x_planes_cols <= p.x_cols,
+               "uniform gather: x_planes_cols must be in [F*dim + ndense, x_cols]");
+    B2_REQUIRE(aligned16(x_planes), "uniform gather: x_planes must be 16-byte aligned");
+    p.xp_pitch = planes_cols_pad(x_planes_cols);
+    p.xp_rows_pad = planes_rows_pad(batch);
+    p.xp_hi = (__nv_bfloat16*)x_planes;
+    p.xp_lo = p.xp_hi + p.xp_rows_pad * p.xp_pitch;
+  }
   if (batch <= 0) return B2CTR_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int grid = grid_for(batch, 8, 8);
-  B2_DISPATCH_LPR(gather_uniform_fwd_kernel, p.dim, p, batch);
+  if (p.fm_sum || p.xp_hi) {      // one wave of the 3-CTA instantiation
+    const int grid = grid_for(batch, 8, 3);
+    if (p.world > 1) launch_gather<true, true>(p, batch, grid, st);
+    else launch_gather<false, true>(p, batch, grid, st);
+  } else {
+    const int grid = grid_for(batch, 8, 8);
+    if (p.world > 1) launch_gather<true, false>(p, batch, grid, st);
+    else launch_gather<false, false>(p, batch, grid, st);
+  }
   B2_CHECK_LAUNCH("b2ctr_embed_gather_uniform_fwd");
   return B2CTR_OK;
 }
@@ -891,10 +980,18 @@ b2ctr_status_t b2ctr_embed_gather_uniform_fwd(const b2ctr_uniform_gather_t* g, i
 b2ctr_status_t b2ctr_embed_scatter_uniform_bwd(const b2ctr_uniform_gather_t* g, const float* dx,
                                                const float* dfm, const float* dlinear, float scale,
                                                float lin_scale, int64_t batch, void* stream) {
+  return b2ctr_embed_scatter_uniform_bwd_ex(g, dx, dfm, nullptr, dlinear, scale, lin_scale, batch, stream);
+}
+
+b2ctr_status_t b2ctr_embed_scatter_uniform_bwd_ex(const b2ctr_uniform_gather_t* g, const float* dx,
+                                                  const float* dfm, const float* fm_sum, const float* dlinear,
+                                                  float scale, float lin_scale, int64_t batch, void* stream) {
   UniParams p;
   b2ctr_status_t s = fill_uni(g, &p);
   if (s != B2CTR_OK) return s;
   B2_REQUIRE(!dx || aligned16(dx), "uniform scatter: dx must be 16-byte aligned");
+  B2_REQUIRE(!fm_sum || aligned16(fm_sum), "uniform scatter: fm_sum must be 16-byte aligned");
+  p.fm_sum = const_cast<float*>(fm_sum);
   if (batch <= 0) return B2CTR_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = grid_for(batch, 8, 8);

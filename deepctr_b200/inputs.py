@@ -260,6 +260,7 @@ class EmbeddingPlanner(object):
         self.fm_hint = None        # (col0, ncols) of the main buffer an FM layer consumed
         self.lin_hint = False      # the linear buffer is only ever row-summed
         self.tail_hint = None      # (dense col0, ncols) appended behind the main buffer
+        self.planes_hint = None    # ncols of the leading main-buffer window ops.dense split into bf16 planes
         self.fm_result = None
         self.lin_result = None
         self._plans = {}
@@ -518,6 +519,7 @@ class EmbeddingPlanner(object):
         self.results = {}
         self.fm_result = self.lin_result = None
         self.tail_done = None
+        self.planes_result = None
         if not self.slots:
             return
         some = feed[self.slots[0].input_name].data
@@ -594,6 +596,12 @@ class EmbeddingPlanner(object):
                              else self.fast_n * fast_slots[0].dim)
             if peer is not None:
                 plan.set_peers(self.dist.world, peer[0].table, peer[1].table if peer[1] is not None else None)
+            from . import ops
+            kd = self.main_width + (self.tail_done[1] if self.tail_done is not None else 0)
+            if (self.planes_hint == kd and only_fast and not self.pnn_cols and batch >= 128
+                    and ops.GEMM_PRECISION == L.GEMM_BF16X3):
+                # the first Dense reads x[:, :kd] as its GEMM operand: the gather writes its bf16 planes too
+                self.planes_result = (kd, plan.set_planes(kd))
             K.embed_gather_uniform_fwd(plan, batch)
             if fm is not None:
                 self.fm_result = (self.fm_hint, E.Var(fm.reshape(batch, 1)))
@@ -687,7 +695,7 @@ class EmbeddingPlanner(object):
                 bplan.g.flags = L.UNIFORM_STORE_GRADS
                 K.embed_scatter_uniform_bwd(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
                                             None if dlin is None else dlin.reshape(-1).contiguous(),
-                                            1.0, 1.0, batch)
+                                            1.0, 1.0, batch, fm_sum=plan.fm_sum)
                 lr = opt["optimizer"].lr if opt and opt.get("optimizer") else 0.0
                 sc = -lr / self.dist.world
                 self.exchange.push(st, tabs, ltabs, dimf, grows, glin, sc, sc)
@@ -707,7 +715,7 @@ class EmbeddingPlanner(object):
                 bplan.set_peers(self.dist.world, emb.table, lin.table if (lin is not None and lin_fused) else None)
                 K.embed_scatter_uniform_bwd(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
                                             None if dlin is None else dlin.reshape(-1).contiguous(),
-                                            sc, sc, batch)
+                                            sc, sc, batch, fm_sum=plan.fm_sum)
             elif dx is not None or dfm is not None or dlin is not None:
                 tgts = [self._target(s.emb.embeddings, opt) for s in fast_slots]
                 feats = [self._feature(s, feed, main.data, self.main_ld, table=tgt)
@@ -733,7 +741,7 @@ class EmbeddingPlanner(object):
                     return self._backward_generic(feed, bufs, generic, opt, batch)
                 K.embed_scatter_uniform_bwd(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
                                             None if dlin is None else dlin.reshape(-1).contiguous(),
-                                            scale, lin_scale, batch)
+                                            scale, lin_scale, batch, fm_sum=plan.fm_sum)
         self._backward_generic(feed, bufs, generic, opt, batch)
 
     @staticmethod
@@ -786,6 +794,19 @@ class EmbeddingPlanner(object):
             return self.fm_result[1]
         if self.fast:
             self.fm_hint = key      # fused from the next step on
+        return None
+
+    def lookup_planes(self, x, t2):
+        """ops.dense in BF16X3: the bf16 planes of ``x`` (2-D view ``t2``) if this step's gather wrote them, i.e. if
+        ``x`` is the leading window of the main buffer that the planner learned on an earlier step."""
+        base = x.base
+        if (x.col0 != 0 or x.ncols == -1 or base.data is None or base.ncols != self.main_width
+                or t2.data_ptr() != base.data.data_ptr() or t2.stride(0) != base.data.stride(0)):
+            return None
+        if self.planes_result is not None and self.planes_result[0] == t2.shape[1]:
+            return self.planes_result[1]
+        if self.fast:
+            self.planes_hint = t2.shape[1]      # written by the gather from the next step on
         return None
 
     def lookup_rowsum(self, x):

@@ -128,6 +128,18 @@ class UniformPlan(object):
         self.g.ndense = dense.shape[1] if dense is not None else 0
         self.g.fm_mask[0] = fm_mask & 0xFFFFFFFFFFFFFFFF
         self.g.fm_mask[1] = 0
+        # with the FM fused: the gather also stores S [B, dim], which the scatter then reads instead of re-summing x
+        self.fm_sum = (torch.empty((x.shape[0], feats[0].dim), dtype=torch.float32, device=x.device)
+                       if fm is not None else None)
+        self.x_rows, self.x_device = x.shape[0], x.device
+        self.x_planes, self.x_planes_cols = None, 0
+
+    def set_planes(self, cols):
+        """Have the gather also write the bf16 operand planes (split_planes layout) of x[:, :cols]; returns them."""
+        nbytes = L.lib().b2ctr_planes_bytes(self.x_rows, cols)
+        self.x_planes = torch.empty((nbytes,), dtype=torch.uint8, device=self.x_device)
+        self.x_planes_cols = cols
+        return self.x_planes
 
     def set_peers(self, world, peer_tables, peer_lin_tables):
         """Row-sharded tables addressed through peer mappings (parallel.PeerTables.table device arrays)."""
@@ -138,13 +150,15 @@ class UniformPlan(object):
 
 
 def embed_gather_uniform_fwd(plan, batch):
-    L.check(L.lib().b2ctr_embed_gather_uniform_fwd(C.byref(plan.g), batch, stream()),
+    L.check(L.lib().b2ctr_embed_gather_uniform_fwd_ex(C.byref(plan.g), ptr(plan.fm_sum), ptr(plan.x_planes),
+                                                      plan.x_planes_cols, batch, stream()),
             "embed_gather_uniform_fwd")
 
 
-def embed_scatter_uniform_bwd(plan, dx, dfm, dlinear, scale, lin_scale, batch):
-    L.check(L.lib().b2ctr_embed_scatter_uniform_bwd(C.byref(plan.g), ptr(dx), ptr(dfm), ptr(dlinear),
-                                                    scale, lin_scale, batch, stream()),
+def embed_scatter_uniform_bwd(plan, dx, dfm, dlinear, scale, lin_scale, batch, fm_sum=None):
+    """``fm_sum``: the S [B, dim] a gather of the same x stored (UniformPlan.fm_sum), or None: the scatter sums x."""
+    L.check(L.lib().b2ctr_embed_scatter_uniform_bwd_ex(C.byref(plan.g), ptr(dx), ptr(dfm), ptr(fm_sum),
+                                                       ptr(dlinear), scale, lin_scale, batch, stream()),
             "embed_scatter_uniform_bwd")
 
 

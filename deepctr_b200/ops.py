@@ -63,6 +63,11 @@ def _as2d(x):
 def _planes_of(var, t2):
     """bf16 hi/lo planes of a Var's 2-D view, split once per step and shared by every GEMM that reads it
     (forward of each consumer + the wgrad GEMMs)."""
+    base = var.base
+    if base is not None and hasattr(base.owner, "lookup_planes"):
+        planes = base.owner.lookup_planes(var, t2)     # the fused embedding gather wrote them
+        if planes is not None:
+            return planes
     key = (t2.data_ptr(), tuple(t2.shape), t2.stride(0))
     if var.planes is None or var.planes[0] != key:
         var.planes = (key, K.split_planes(t2))

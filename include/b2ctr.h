@@ -154,6 +154,16 @@ typedef struct b2ctr_uniform_gather {
 
 B2CTR_API b2ctr_status_t b2ctr_embed_gather_uniform_fwd(const b2ctr_uniform_gather_t* g,
                                                        int64_t batch, void* stream);
+/* The same gather, also writing (each optional, NULL = off):
+ *   fm_sum   [batch, dim] fp32: S_b = sum over the fm_mask fields of x[b, f*dim:(f+1)*dim], the vector fm[b] is
+ *            formed from (needs fm).  Handing it to b2ctr_embed_scatter_uniform_bwd_ex saves the scatter its own
+ *            pass over x; it is summed in the order that scatter would use, so the update is the same bit for bit.
+ *   x_planes b2ctr_planes_bytes(batch, x_planes_cols) bytes: the bf16 hi/lo planes of x[:, 0:x_planes_cols] in
+ *            b2ctr_split_planes' layout and values (pad columns and pad rows zero), for a first GEMM that reads that
+ *            window; F*dim + ndense <= x_planes_cols <= x_cols. */
+B2CTR_API b2ctr_status_t b2ctr_embed_gather_uniform_fwd_ex(const b2ctr_uniform_gather_t* g, float* fm_sum,
+                                                          void* x_planes, int64_t x_planes_cols, int64_t batch,
+                                                          void* stream);
 
 /* Backward of the above fused with the row update:
  *   g_row(b,f) = dx[b, f*dim:(f+1)*dim] + dfm[b] * (S_b - x[b, f*dim:...])   (FM Jacobian, App. A.6)
@@ -165,6 +175,13 @@ B2CTR_API b2ctr_status_t b2ctr_embed_scatter_uniform_bwd(const b2ctr_uniform_gat
                                                         const float* dlinear, float scale,
                                                         float lin_scale, int64_t batch,
                                                         void* stream);
+/* The same update with S_b read from fm_sum (written by b2ctr_embed_gather_uniform_fwd_ex) instead of summed
+ * from x; fm_sum NULL = the call above. */
+B2CTR_API b2ctr_status_t b2ctr_embed_scatter_uniform_bwd_ex(const b2ctr_uniform_gather_t* g,
+                                                           const float* dx, const float* dfm,
+                                                           const float* fm_sum, const float* dlinear,
+                                                           float scale, float lin_scale, int64_t batch,
+                                                           void* stream);
 
 /* Ids outside [0, vocab) (b2ctr_feature_t.vocab = the FULL vocabulary_size, also for row-sharded tables):
  * every gather kernel returns a ZERO row for them and every update kernel skips them - no out-of-bounds
