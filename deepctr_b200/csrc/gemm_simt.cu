@@ -182,9 +182,12 @@ __global__ void __launch_bounds__(256) skinny_n_kernel(const GemmArgs g, int lpr
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   if (vec && g.k <= (int64_t)lpr * 4) {
     // one 16-byte load per lane covers its share of a row: four row groups per iteration, their loads issued
-    // back to back (the one-group loop below keeps a single load in flight per lane: 0.7 TB/s on [409600, 40])
+    // back to back (the one-group loop below keeps a single load in flight per lane: 0.7 TB/s on [409600, 40]).
+    // The last group may reach past k into the row's padding: those columns are replaced by zero rather than
+    // multiplied by a zero weight, so that a NaN or Inf in the padding cannot reach the output.
     const int64_t k = (int64_t)li * 4;
     const bool kin = k < g.k;
+    const bool in1 = k + 1 < g.k, in2 = k + 2 < g.k, in3 = k + 3 < g.k;
     float b[N][4];
 #pragma unroll
     for (int n = 0; n < N; ++n)
@@ -198,6 +201,9 @@ __global__ void __launch_bounds__(256) skinny_n_kernel(const GemmArgs g, int lpr
       for (int u = 0; u < 4; ++u) {
         const int64_t r = r0 + u * rows_per_warp + sub;
         a[u] = (r < g.m && kin) ? __ldg(reinterpret_cast<const float4*>(g.a + r * g.sam + k)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        a[u].y = in1 ? a[u].y : 0.f;
+        a[u].z = in2 ? a[u].z : 0.f;
+        a[u].w = in3 ? a[u].w : 0.f;
       }
 #pragma unroll
       for (int u = 0; u < 4; ++u) {

@@ -258,7 +258,10 @@ def bias_act_bwd(dy, y, act, want_dz=True, want_dbias=True, m=None, n=None, want
     if m is None:
         m, n = dy.shape[0], dy.shape[1]
     ld = dy.stride(0)
-    dz = torch.empty_like(dy) if want_dz else None
+    # one row pitch for dy, y and dz: a strided dy (a window of a wider buffer) gets a dz window with the same pitch
+    if y is not None and y.dim() == 2 and y.stride(0) != ld:
+        raise ValueError("bias_act_bwd: dy and y must have the same row pitch (%d != %d)" % (ld, y.stride(0)))
+    dz = torch.empty((m, ld), dtype=torch.float32, device=dy.device)[:, :n] if want_dz else None
     dbias = torch.empty((n,), dtype=torch.float32, device=dy.device) if want_dbias else None
     nbytes = L.lib().b2ctr_bias_act_bwd_workspace_bytes(m, n) if want_dbias else 0
     ws = workspace(nbytes, dy.device)

@@ -8,7 +8,7 @@ from . import _lib as L
 from . import kernels as K
 from . import engine as E
 
-# precision mode used by every dense GEMM (DNN / attention MLP / projections); see DESIGN.md section 4.2.
+# precision mode used by every dense GEMM (DNN / attention MLP / projections); see DESIGN.md section 5.
 # Default: split-bf16 on the wgmma tensor cores (three bf16 MMAs per product, fp32 accumulation; relative
 # error ~2^-16, inside the 1e-4 logit tolerance of the parity tests); 'fp32' selects the exact FFMA GEMM.
 GEMM_PRECISION = L.GEMM_BF16X3

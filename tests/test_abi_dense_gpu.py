@@ -237,7 +237,8 @@ def test_optimizers(cuda):
 @pytest.mark.parametrize("ta,tb", [(False, False), (False, True), (True, False), (True, True)])
 @pytest.mark.parametrize("variant", [3, 4])
 def test_gemm_bf16x3_tensor_core(cuda, m, n, k, ta, tb, variant):
-    """wgmma split-bf16 GEMM: error bound ~2^-16 relative to sum |a||b| (DESIGN.md section 4.2).
+    """wgmma split-bf16 GEMM: a = hi_a + lo_a and b = hi_b + lo_b in bf16, and the product drops only lo_a lo_b, at most
+    2^-16 |a||b| per term (DESIGN.md section 5); 2^-15 sum |a||b| also covers the fp32 accumulation at these k.
     Variants: 3 = non-persistent reference kernel, 4 = persistent warp-specialised kernel."""
     K, L = _kern()
     rng = np.random.RandomState(m + 3 * n + k)
