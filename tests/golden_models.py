@@ -1,6 +1,7 @@
 """Shared loader for the MODEL-level golden fixtures (tests/golden/models*/*.npz, produced by the
 reference's own feature_column.py / inputs.py / builders under the TF shim: see
-tests/golden/generate_*.py), the table of fixture families, and the mappings a test needs:
+tests/golden/generate_*.py), the table of fixture families, the table of LAYER-level fixture sets
+(``LAYER_SETS``, tests/golden/*.npz and tests/golden/<set>/*.npz), and the mappings a test needs:
 
 * ``oracle_weights``  fixture weight keys -> the dict oracle/models.py takes;
 * ``assign_weights``  fixture weight keys -> the weights of a deepctr_b200 model built from the same columns.
@@ -18,6 +19,8 @@ import re
 
 import numpy as np
 import torch
+
+import b2_helpers as H
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 MODELS = os.path.join(GOLDEN, "models")
@@ -444,17 +447,177 @@ FAMILIES = {
 }
 
 
-# ---- layer fixtures (tests/golden/<family>/*.npz) -----------------------------------------------------
-def layer_cases(subdir):
-    return _cases(os.path.join(GOLDEN, subdir))
+# ---- layer fixtures (tests/golden/*.npz, tests/golden/<set>/*.npz) -------------------------------------
+# Key convention: ``w_<weight>`` / ``g_<weight>`` (the weight's path inside the layer), the inputs ``x`` [B,F,E],
+# ``x_<i>`` or ``in_<i>`` with their gradients ``gx`` / ``gx_<i>``, ``out`` and, where there are gradients, the
+# ``dout`` they were taken for.
+def allclose(rtol, atol):
+    """elementwise: |got - want| <= atol + rtol |want|."""
+    def check(got, want, what):
+        np.testing.assert_allclose(got, want, rtol=rtol, atol=atol, err_msg=what)
+    return check
 
 
-def load_layer(subdir, name):
-    """(meta, {key: array}) of a layer fixture; the keys keep the npz's order."""
-    d = np.load(os.path.join(GOLDEN, subdir, name + ".npz"))
-    return json.loads(str(d["meta"])), {k: d[k] for k in d.files if k != "meta"}
+def max_rel(tol):
+    """normwise: max |got - want| < tol x max |want| (b2_helpers.close)."""
+    def check(got, want, what):
+        H.close(got, want, what, tol)
+    return check
 
 
-def layer_weight_names(d):
-    """weight names of a layer fixture, in the layer's order (the npz keeps insertion order)."""
-    return [k[2:] for k in d if k.startswith("w_")]
+def _root_out(got, want, what):
+    """1e-4 relative; under the split-bf16 GEMMs the atol is normwise, 1e-4 x max |want| (see test_layers_gpu)."""
+    from deepctr_b200 import ops, _lib as L
+    atol = 2e-6
+    if ops.GEMM_PRECISION == L.GEMM_BF16X3 and want.size:
+        atol = max(atol, 1e-4 * float(np.abs(want).max()))
+    np.testing.assert_allclose(got, want, rtol=1e-4, atol=atol, err_msg=what)
+
+
+def numbered(d, prefix):
+    """``prefix``0, ``prefix``1, ... as far as the fixture has them."""
+    return ["%s%d" % (prefix, i) for i in range(len([k for k in d if k.startswith(prefix)]))]
+
+
+def _one_or_list(vs):
+    return vs[0] if len(vs) == 1 else vs
+
+
+# layers called on a list of F [B,1,E] tensors; the others of the x-format sets take the [B,F,E] tensor
+_LIST_LAYERS = ("AFMLayer", "SENETLayer", "BilinearInteraction", "InnerProductLayer", "OutterProductLayer")
+
+
+def _x_args(meta, d, device):
+    """``x`` [B,F,E] as a model hands it to the layer, a [B, F*E] buffer read in place: F [B,1,E] windows of it
+    (which ops.concat joins back without a copy) or one [B,F,E] window.  The buffer collects ``gx``."""
+    from deepctr_b200 import engine as E, ops
+    b, f, e = d["x"].shape
+    buf = E.Var(torch.tensor(d["x"].reshape(b, f * e), device=device), requires_grad=True)
+    if meta["layer"] in _LIST_LAYERS:
+        return [ops._window(buf, i * e, e, (b, 1, e)) for i in range(f)], {"x": buf}
+    return ops._window(buf, 0, f * e, (b, f, e)), {"x": buf}
+
+
+def _x_i_args(meta, d, device):
+    """BST's ``x_<i>``; masked fixtures carry each input's mask as ``mask_<i>`` [B,T], a prefix of valid steps."""
+    from deepctr_b200 import engine as E
+    vs = []
+    for i, k in enumerate(numbered(d, "x_")):
+        a = d[k]
+        v = E.Var(torch.tensor(a, device=device), requires_grad=a.dtype == np.float32)
+        if meta["masked"]:
+            lengths = d["mask_%d" % i].sum(1).astype(np.int32)
+            v.mask = E.KMask(lengths=torch.tensor(lengths, device=device), maxlen=a.shape[1])
+        vs.append(v)
+    return _one_or_list(vs), dict(zip(numbered(d, "x_"), vs))
+
+
+def _in_args(meta, d, device):
+    """``in_<i>``; a Keras mask in meta['extra']['mask'] (one per input, or one for the first) becomes the
+    ``id != 0`` mask of its input."""
+    from deepctr_b200 import engine as E
+    vs = [E.to_var(d[k]) for k in numbered(d, "in_")]
+    mask = meta["extra"].get("mask")
+    if mask is not None:
+        ms = mask if (isinstance(mask, list) and (mask[0] is None or isinstance(mask[0][0], list))) else [mask]
+        for v, m in zip(vs, ms):
+            if m is not None:
+                v.mask = E.KMask(ids=[torch.as_tensor(np.asarray(m, dtype=np.int32)).to(v.data.device)])
+    return _one_or_list(vs), {}
+
+
+def _pairwise_layer(meta, xs, W, d):
+    import pairwise_oracle as PO
+    if meta["layer"] == "AFMLayer":
+        return PO.afm(xs[0], **W)
+    return PO.bi_interaction(xs[0])
+
+
+def _fibinet_layer(meta, xs, W, d):
+    import fibinet_oracle as FO
+    if meta["layer"] == "SENETLayer":
+        return FO.senet(xs[0], *W.values())
+    return FO.bilinear(xs[0], meta["kwargs"]["bilinear_type"], list(W.values()))
+
+
+def _fefm_layer(meta, xs, W, d):
+    import fefm_oracle as FO
+    if meta["layer"] == "FwFMLayer":
+        return FO.fwfm(xs[0], W["field_pair_strengths"])
+    return FO.fefm(xs[0], list(W.values()))
+
+
+def _pnn_layer(meta, xs, W, d):
+    import pnn_oracle as PO
+    kw = meta["kwargs"]
+    if meta["layer"] == "InnerProductLayer":
+        return PO.inner(xs[0], kw.get("reduce_sum", True))
+    return PO.outer(xs[0], W["kernel"], kw["kernel_type"])
+
+
+def _bst_layer(meta, xs, W, d):
+    import bst_oracle as BO
+    kw = meta["kwargs"]
+    cls = meta["layer"]
+    if cls == "LayerNormalization":
+        return BO.layer_norm(xs[0], W["gamma"], W["beta"])
+    if cls == "PositionEncoding":
+        return BO.position_encoding(xs[0], W["lookup_table"], kw.get("scale", True))
+    T = xs[0].shape[1]
+    if meta["masked"]:
+        qv, kv = torch.as_tensor(d["mask_0"]), torch.as_tensor(d["mask_1"])
+    else:
+        ar = torch.arange(T)[None, :]
+        qv, kv = ar < torch.as_tensor(xs[2]).long(), ar < torch.as_tensor(xs[3]).long()
+    return BO.transformer(xs[0], xs[1], qv, kv, W, **kw)
+
+
+class LayerSet(object):
+    """One directory of layer fixtures: the reference's layer, built from meta's ``layer`` and ``kwargs``, run on the
+    fixture's inputs and weights.
+
+    * ``n_cases`` and ``layers`` are what the set holds;
+    * ``args(meta, d, device)``: the layer's call argument and {input key: the Var its gradient lands in};
+    * ``oracle(meta, xs, W, d)``: the CPU restatement (``xs`` the inputs ``x`` or ``x_<i>``, ``W`` {weight: tensor});
+      the root set has none, test_oracle_pinning.py pins it layer by layer;
+    * ``cpu`` / ``gpu``: (output check, gradient check), each ``check(got, want, what)``;
+    * ``renames``: reference weight path -> path inside this package's layer.
+    """
+
+    def __init__(self, subdir, n_cases, layers, args, gpu, oracle=None, cpu=None, renames=(), skip=()):
+        self.dir = os.path.join(GOLDEN, subdir)
+        self.cases = [n for n in _cases(self.dir) if n not in skip]
+        self.n_cases, self.layers, self.args = n_cases, layers, args
+        self.oracle, self.cpu, self.gpu, self.renames = oracle, cpu, gpu, renames
+
+    def load(self, name):
+        """(meta, {key: array}); the keys keep the npz's order, the weights the layer's."""
+        d = np.load(os.path.join(self.dir, name + ".npz"))
+        return json.loads(str(d["meta"])), {k: d[k] for k in d.files if k != "meta"}
+
+    def weight_name(self, key):
+        for a, b in self.renames:
+            key = key.replace(a, b)
+        return key
+
+
+_FAMILY_CPU = (allclose(1e-5, 1e-6), allclose(1e-4, 1e-6))
+_FAMILY_GPU = allclose(1e-4, 1e-5)
+
+LAYER_SETS = {
+    "root": LayerSet("", 35, ("AttentionSequencePoolingLayer", "CIN", "CrossNet", "DNN", "Dice", "FM",
+                              "InteractingLayer", "Linear", "LocalActivationUnit", "PredictionLayer",
+                              "SequencePoolingLayer", "WeightedSequenceLayer"),
+                     _in_args, gpu=(_root_out, None), skip=("hash_vocab_kat",),
+                     renames=(("local_att/", "local_activation_unit/"), ("activation_layers", "act"))),
+    "pairwise": LayerSet("pairwise", 6, ("AFMLayer", "BiInteractionPooling"), _x_args, oracle=_pairwise_layer,
+                         cpu=_FAMILY_CPU, gpu=(allclose(1e-5, 1e-5), _FAMILY_GPU)),
+    "fibinet": LayerSet("fibinet", 12, ("SENETLayer", "BilinearInteraction"), _x_args, oracle=_fibinet_layer,
+                        cpu=_FAMILY_CPU, gpu=(_FAMILY_GPU, _FAMILY_GPU)),
+    "fefm": LayerSet("fefm", 6, ("FwFMLayer", "FEFMLayer"), _x_args, oracle=_fefm_layer,
+                     cpu=_FAMILY_CPU, gpu=(_FAMILY_GPU, _FAMILY_GPU)),
+    "pnn": LayerSet("pnn", 15, ("InnerProductLayer", "OutterProductLayer"), _x_args, oracle=_pnn_layer,
+                    cpu=_FAMILY_CPU, gpu=(_FAMILY_GPU, _FAMILY_GPU)),
+    "bst": LayerSet("bst", 7, ("Transformer", "PositionEncoding", "LayerNormalization"), _x_i_args,
+                    oracle=_bst_layer, cpu=(max_rel(1e-5), max_rel(1e-4)), gpu=(max_rel(2e-4), max_rel(2e-4))),
+}

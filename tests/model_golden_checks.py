@@ -1,25 +1,33 @@
-"""The model-golden checks, written once for every fixture family of golden_models.FAMILIES.
+"""The golden checks, written once: the model-level ones for every fixture family of golden_models.FAMILIES, the
+layer-level ones for every fixture set of golden_models.LAYER_SETS.
 
-Each family's test modules bind them under their own test names, so adding a family needs only its record in
-FAMILIES, its oracle functions and these bindings:
+Each family's test modules bind them under their own test names, so adding a family or a layer set needs only its
+record, its oracle functions and these bindings:
 
     T = model_golden_checks.model_tests("pairwise")          # CPU
     test_oracle_matches_reference_model = T.oracle
     T = model_golden_checks.gpu_model_tests("pairwise")      # GPU, both GEMM precisions
     test_model_forward_matches_reference = T.forward
+    test_oracle_matches_reference_layer = model_golden_checks.layer_tests("pairwise").oracle
+    test_layer_fixture = model_golden_checks.gpu_layer_test("pairwise")
 
 Every call makes new function objects, so the marks of one module never reach another.
 
-CPU, per fixture:
+Layer fixtures (the reference's layer run on given inputs and weights, with the gradients for a seeded ``dout``):
+on the CPU the set's restatement reproduces the output and every input and weight gradient (a gradient that is 0
+comes out exactly 0); on the GPU, in both GEMM precisions, the deepctr_b200 layer built from the fixture's arguments,
+with exactly the fixture's weight set loaded by name, reproduces the output and, run on a tape, every gradient.
+
+Model fixtures, CPU, per fixture:
 1. the family's restatement (oracle/models.py, tests/*_oracle.py) reproduces the logits, predictions, loss and
    every weight gradient;
 2. the deepctr_b200 builders create exactly the reference's weight set (names, shapes, trainable flags, order) -
    the precondition for loading reference weights by name;
 3. they build the graph the reference's builder SOURCE FILES build on this package (tests/golden/
    reference_builders*.json: inputs, layers, weights, planner slots) and have the reference's keyword defaults.
-GPU, per fixture, in both GEMM precisions (and with and without the DNN-input placement where the family has it):
-the reference's weights loaded by name reproduce the logits and predictions (1e-4 relative), and one SGD step's
-loss and weight updates  -lr * dL/dw  match the gradient torch autograd took THROUGH the reference's graph.
+Model fixtures, GPU, per fixture, in both GEMM precisions (and with and without the DNN-input placement where the
+family has it): the reference's weights loaded by name reproduce the logits and predictions (1e-4 relative), and one
+SGD step's loss and weight updates  -lr * dL/dw  match the gradient torch autograd took THROUGH the reference's graph.
 On synthetic Criteo-like data (b2_helpers.train): a graph-replayed training step equals an eager one, and the
 DNN-input placement gives the unplaced results.
 """
@@ -28,6 +36,7 @@ import types
 
 import numpy as np
 import pytest
+import torch
 
 import b2_helpers as H
 import golden_models as G
@@ -199,6 +208,103 @@ def gpu_model_tests(family):
             pytest.skip("fixture differentiates Dice in inference mode; a training step uses batch statistics")
         check_sgd_step(fam, name)
     return types.SimpleNamespace(forward=forward, sgd_step=sgd_step)
+
+
+# ---- layer fixtures -----------------------------------------------------------------------------------
+def check_layer_set(ls):
+    assert len(ls.cases) == ls.n_cases
+    assert {ls.load(n)[0]["layer"] for n in ls.cases} == set(ls.layers)
+
+
+def _gradient_keys(d):
+    return [k for k in d if k.startswith(("gx", "g_"))]
+
+
+def check_layer_oracle(ls, name):
+    meta, d = ls.load(name)
+    keys = ["x"] if "x" in d else G.numbered(d, "x_")
+    xs = {k: torch.tensor(d[k], requires_grad=d[k].dtype == np.float32) for k in keys}
+    W = {k[2:]: torch.tensor(d[k], requires_grad=True) for k in d if k.startswith("w_")}
+    out = ls.oracle(meta, list(xs.values()), W, d)
+    out_close, grad_close = ls.cpu
+    out_close(out.detach().numpy(), d["out"], "out")
+    (out * torch.as_tensor(d["dout"])).sum().backward()
+    leaves = {"g" + k: t for k, t in xs.items()}
+    leaves.update(("g_" + k, t) for k, t in W.items())
+    for key in _gradient_keys(d):
+        want = d[key]
+        got = leaves[key].grad.numpy() if leaves[key].grad is not None else np.zeros_like(want)
+        if np.any(want):
+            grad_close(got, want, key)
+        else:
+            np.testing.assert_array_equal(got, 0, err_msg=key)
+
+
+def check_layer_gpu(ls, name, device):
+    from deepctr_b200 import engine as E
+    from deepctr_b200 import layers as LY
+    meta, d = ls.load(name)
+    kwargs = dict(meta["kwargs"])
+    for k in ("layer_size", "att_hidden_units", "hidden_units"):
+        if k in kwargs:
+            kwargs[k] = tuple(kwargs[k])
+    E.clear_session()
+    layer = getattr(LY, meta["layer"])(**kwargs)
+    arg, inputs = ls.args(meta, d, device)
+    layer._maybe_build(E._shape_of(arg))
+    mine = {w.name.split("/", 1)[1]: w for w in layer.weights}
+    ref = {ls.weight_name(k[2:]): k[2:] for k in d if k.startswith("w_")}
+    assert sorted(mine) == sorted(ref), (sorted(mine), sorted(ref))
+    for n, w in mine.items():
+        w.set_value(d["w_" + ref[n]])
+    tape = E.Tape()
+    with E.recording(tape):
+        y = layer._invoke(arg, bool(meta.get("extra", {}).get("training", False)))
+    # a list output (SENETLayer's F [B,1,E] windows) is compared and seeded field by field
+    ys, part = (y, lambda a, i: a[:, i:i + 1]) if isinstance(y, list) else ([y], lambda a, i: a)
+    out_close, grad_close = ls.gpu
+    for i, yi in enumerate(ys):
+        want = part(d["out"], i)
+        out_close(E.contiguous(yi).cpu().numpy().reshape(want.shape), want, "out")
+    if "dout" not in d:             # the root set holds outputs only
+        return
+    for i, yi in enumerate(ys):
+        yi.requires_grad = True
+        E.add_grad(yi, torch.tensor(part(d["dout"], i), device=device).reshape(yi.shape))
+    tape.backward()
+    leaves = {"g" + k: v for k, v in inputs.items()}
+    leaves.update(("g_" + ref[n], w) for n, w in mine.items())
+    for key in _gradient_keys(d):
+        want = d[key]
+        g = leaves[key].grad
+        got = g.cpu().numpy().reshape(want.shape) if g is not None else np.zeros_like(want)
+        grad_close(got, want, key)
+
+
+def layer_tests(layer_set):
+    """The CPU tests of one layer-fixture set: oracle (parametrised by fixture name) and fixture_set."""
+    ls = G.LAYER_SETS[layer_set]
+
+    @pytest.mark.parametrize("name", ls.cases)
+    def oracle(name):
+        check_layer_oracle(ls, name)
+
+    def fixture_set():
+        check_layer_set(ls)
+    return types.SimpleNamespace(oracle=oracle, fixture_set=fixture_set)
+
+
+def gpu_layer_test(layer_set):
+    """The GPU test of one layer-fixture set, parametrised by fixture name and GEMM precision: the layer reproduces
+    the output and, where the fixture has them, the input and weight gradients."""
+    ls = G.LAYER_SETS[layer_set]
+
+    @pytest.mark.gpu
+    @pytest.mark.usefixtures("gemm_precision")
+    @pytest.mark.parametrize("name", ls.cases)
+    def layer(cuda, name):
+        check_layer_gpu(ls, name, cuda)
+    return layer
 
 
 def graph_replay_test(cases):

@@ -12,39 +12,28 @@ import itertools
 
 import numpy as np
 import pytest
-import torch
 
 import golden_models as G
 import model_golden_checks as C
 
-LAYER_CASES = G.layer_cases("fefm")
 T = C.model_tests("fefm")
 test_oracle_matches_reference_model = T.oracle
 test_builder_creates_the_reference_weight_set = T.weight_set
 test_builder_graph_is_the_reference_graph = T.graph
 test_reference_default_arguments_are_the_same = T.defaults
+L = C.layer_tests("fefm")
+test_oracle_matches_reference_layer = L.oracle
 
 
 def test_fixture_sets():
     C.check_fixture_set(G.FAMILIES["fefm"])
-    assert len(LAYER_CASES) == 6
-
-
-@pytest.mark.parametrize("name", LAYER_CASES)
-def test_oracle_matches_reference_layer(name):
-    import fefm_oracle as FO
-    meta, d = G.load_layer("fefm", name)
-    x = torch.tensor(d["x"], requires_grad=True)
-    ws = [torch.tensor(d["w_" + k], requires_grad=True) for k in G.layer_weight_names(d)]
-    out = FO.fwfm(x, ws[0]) if meta["layer"] == "FwFMLayer" else FO.fefm(x, ws)
-    np.testing.assert_allclose(out.detach().numpy(), d["out"], rtol=1e-5, atol=1e-6)
-    (out * torch.as_tensor(d["dout"])).sum().backward()
-    np.testing.assert_allclose(x.grad.numpy(), d["gx"], rtol=1e-4, atol=1e-6)
-    for k, v in zip(G.layer_weight_names(d), ws):
-        np.testing.assert_allclose(v.grad.numpy(), d["g_" + k], rtol=1e-4, atol=1e-6, err_msg=k)
-    if meta["layer"] == "FwFMLayer":
-        g = d["g_field_pair_strengths"]
-        assert not np.any(np.tril(g)), "the strengths' gradient is 0 on and below the diagonal"
+    L.fixture_set()
+    ls = G.LAYER_SETS["fefm"]
+    for name in ls.cases:
+        meta, d = ls.load(name)
+        if meta["layer"] == "FwFMLayer":
+            g = d["g_field_pair_strengths"]
+            assert not np.any(np.tril(g)), "the strengths' gradient is 0 on and below the diagonal"
 
 
 def test_unreachable_branches_hold_no_weights():

@@ -5,7 +5,8 @@
   batches that are not a multiple of a CTA's samples; both backwards are bit-identical from run to run;
 * the C2 shape (B = 65536, F = 26, E = 32): the input a window of the [B, 848] gather buffer, and FEFM's scores
   written behind its 845 embedding and dense columns in a [B, 1172] buffer;
-* layer fixtures of the reference's own FwFMLayer / FEFMLayer (tests/golden/fefm/);
+* layer fixtures of the reference's own FwFMLayer / FEFMLayer (tests/golden/fefm/, with
+  model_golden_checks): through the layers, outputs and gradients in both GEMM precisions;
 * with the placement, the step copies no score block ;
 * model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions, placed and unplaced;
   a graph-replayed training step equals an eager one; the placement gives the results of the unplaced graph;
@@ -16,12 +17,12 @@ import pytest
 import torch
 
 import b2_helpers as H
-import golden_models as G
 import model_golden_checks as C
 from model_golden_checks import placement  # noqa: F401  (the placed / unplaced parameter)
 
 pytestmark = pytest.mark.gpu
 
+test_layer_fixture = C.gpu_layer_test("fefm")
 T = C.gpu_model_tests("fefm")
 test_model_forward_matches_reference = T.forward
 test_model_sgd_step_matches_reference_gradients = T.sgd_step
@@ -147,30 +148,6 @@ def test_kernels_reject_unsupported_shapes(cuda):
     with pytest.raises(ValueError, match="does not fit"):
         K.fefm_fwd(x, 65 * 65, 4, 4, torch.zeros((6, 4, 4), device=cuda), 4, out=torch.zeros((4, 8), device=cuda),
                    col0=3)
-
-
-@pytest.mark.parametrize("name", G.layer_cases("fefm"))
-def test_layer_fixture(cuda, name):
-    from deepctr_b200 import kernels as K
-    meta, d = G.load_layer("fefm", name)
-    x = torch.tensor(d["x"], device=cuda)
-    B, F, Ed = x.shape
-    ws = [torch.tensor(d["w_" + k], device=cuda) for k in G.layer_weight_names(d)]
-    dout = torch.tensor(d["dout"], device=cuda).reshape(B, -1).contiguous()
-    tol = dict(rtol=1e-4, atol=1e-5)
-    if meta["layer"] == "FwFMLayer":
-        out = K.fwfm_fwd(x.reshape(B, -1), F * Ed, F, Ed, ws[0], B)
-        dx, dR = K.fwfm_bwd(dout, 1, x.reshape(B, -1), F * Ed, F, Ed, ws[0], B)
-        grads = [dR]
-    else:
-        S = K.fefm_sym(torch.stack(ws))
-        out = K.fefm_fwd(x.reshape(B, -1), F * Ed, F, Ed, S, B)
-        dx, dW = K.fefm_bwd(dout, dout.stride(0), 0, x.reshape(B, -1), F * Ed, F, Ed, S, B)
-        grads = list(dW)
-    np.testing.assert_allclose(out.reshape(d["out"].shape).cpu().numpy(), d["out"], **tol)
-    np.testing.assert_allclose(dx.reshape(B, F, Ed).cpu().numpy(), d["gx"], **tol)
-    for k, gk in zip(G.layer_weight_names(d), grads):
-        np.testing.assert_allclose(gk.cpu().numpy(), d["g_" + k], err_msg=k, **tol)
 
 
 def test_c2_shape_deepfefm_tail_rows_match_the_oracle(cuda):

@@ -8,43 +8,25 @@ builder code produced (tests/golden/generate_fibinet.py):
 3. the DNN-input placement is planned for FiBiNET's graph, and only there.
 """
 
-import numpy as np
 import pytest
-import torch
 
 import golden_models as G
 import model_golden_checks as C
 
-LAYER_CASES = G.layer_cases("fibinet")
 T = C.model_tests("fibinet")
 test_oracle_matches_reference_model = T.oracle
 test_builder_creates_the_reference_weight_set = T.weight_set
 test_builder_graph_is_the_reference_graph = T.graph
 test_reference_default_arguments_are_the_same = T.defaults
+L = C.layer_tests("fibinet")
+test_oracle_matches_reference_layer = L.oracle
 
 
 def test_fixture_sets():
     C.check_fixture_set(G.FAMILIES["fibinet"])
+    L.fixture_set()
     fam = G.FAMILIES["fibinet"]
-    assert len(LAYER_CASES) == 12
     assert {fam.fixture(n).kwargs["bilinear_type"] for n in fam.cases} == {"all", "each", "interaction"}
-
-
-@pytest.mark.parametrize("name", LAYER_CASES)
-def test_oracle_matches_reference_layer(name):
-    import fibinet_oracle as FO
-    meta, d = G.load_layer("fibinet", name)
-    x = torch.tensor(d["x"], requires_grad=True)
-    ws = [torch.tensor(d["w_" + k], requires_grad=True) for k in G.layer_weight_names(d)]
-    if meta["layer"] == "SENETLayer":
-        out = FO.senet(x, *ws)
-    else:
-        out = FO.bilinear(x, meta["kwargs"]["bilinear_type"], ws)
-    np.testing.assert_allclose(out.detach().numpy(), d["out"], rtol=1e-5, atol=1e-6)
-    (out * torch.as_tensor(d["dout"])).sum().backward()
-    np.testing.assert_allclose(x.grad.numpy(), d["gx"], rtol=1e-4, atol=1e-6)
-    for k, v in zip(G.layer_weight_names(d), ws):
-        np.testing.assert_allclose(v.grad.numpy(), d["g_" + k], rtol=1e-4, atol=1e-6, err_msg=k)
 
 
 @pytest.mark.parametrize("nfields,dim", [(65, 4), (3, 65)])

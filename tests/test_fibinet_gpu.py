@@ -3,7 +3,8 @@
 * b2ctr_bilinear_fwd / _bwd for the three bilinear types and b2ctr_senet_fwd / _bwd against float64 over F = 2 / 26 /
   64 and E = 4 / 5 / 32 / 64, the input a window of a wider buffer, the output a strided window of a wider buffer,
   and batches that are not a multiple of a CTA's samples; both backwards are bit-identical from run to run;
-* layer fixtures of the reference's own SENETLayer / BilinearInteraction (tests/golden/fibinet/);
+* layer fixtures of the reference's own SENETLayer / BilinearInteraction (tests/golden/fibinet/, with
+  model_golden_checks): through the layers, outputs and gradients in both GEMM precisions;
 * with the DNN-input placement no copy wider than the dense tail touches the DNN input ;
 * model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions, placed and unplaced;
   a graph-replayed training step equals an eager one; the placement gives the results of the unplaced graph;
@@ -17,12 +18,12 @@ import pytest
 import torch
 
 import b2_helpers as H
-import golden_models as G
 import model_golden_checks as C
 from model_golden_checks import placement  # noqa: F401  (the placed / unplaced parameter)
 
 pytestmark = pytest.mark.gpu
 
+test_layer_fixture = C.gpu_layer_test("fibinet")
 T = C.gpu_model_tests("fibinet")
 test_model_forward_matches_reference = T.forward
 test_model_sgd_step_matches_reference_gradients = T.sgd_step
@@ -146,32 +147,6 @@ def test_kernels_reject_unsupported_shapes(cuda):
         K.bilinear_fwd(x, 65 * 4, 3, 65, "all", torch.zeros((1, 65, 65), device=cuda), 4)
     with pytest.raises(ValueError, match="field count"):
         K.senet_fwd(x, 65 * 4, 65, 4, torch.zeros((65, 2), device=cuda), torch.zeros((2, 65), device=cuda), 4)
-
-
-@pytest.mark.parametrize("name", G.layer_cases("fibinet"))
-def test_layer_fixture(cuda, name):
-    from deepctr_b200 import kernels as K
-    meta, d = G.load_layer("fibinet", name)
-    x = torch.tensor(d["x"], device=cuda)
-    B, F, Ed = x.shape
-    ws = [torch.tensor(d["w_" + k], device=cuda) for k in G.layer_weight_names(d)]
-    dout = torch.tensor(d["dout"], device=cuda).reshape(B, -1).contiguous()
-    tol = dict(rtol=1e-4, atol=1e-5)
-    if meta["layer"] == "SENETLayer":
-        v, saved = K.senet_fwd(x.reshape(B, -1), F * Ed, F, Ed, ws[0], ws[1], B)
-        dx, dW1, dW2 = K.senet_bwd(dout, x.reshape(B, -1), F * Ed, F, Ed, ws[0], ws[1], saved, B)
-        grads = [dW1, dW2]
-        out = v
-    else:
-        t = meta["kwargs"]["bilinear_type"]
-        W = torch.stack(ws)
-        out = K.bilinear_fwd(x.reshape(B, -1), F * Ed, F, Ed, t, W, B)
-        dx, dW = K.bilinear_bwd(dout, dout.stride(0), 0, Ed, x.reshape(B, -1), F * Ed, F, Ed, t, W, B)
-        grads = list(dW)
-    np.testing.assert_allclose(out.reshape(d["out"].shape).cpu().numpy(), d["out"], **tol)
-    np.testing.assert_allclose(dx.reshape(B, F, Ed).cpu().numpy(), d["gx"], **tol)
-    for k, gk in zip(G.layer_weight_names(d), grads):
-        np.testing.assert_allclose(gk.cpu().numpy(), d["g_" + k], err_msg=k, **tol)
 
 
 def test_placed_step_copies_only_the_dense_tail(cuda, monkeypatch):

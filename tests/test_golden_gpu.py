@@ -1,73 +1,22 @@
 """GPU: the CUDA layers against the golden vectors produced by the REFERENCE's own layer code
 (tests/golden/*.npz, see tests/golden/generate.py) - same constructor arguments, same inputs, the
-reference's weights loaded by name.  fp32 tolerance 1e-4 relative (north_star)."""
-import glob
-import json
+reference's weights loaded by name (model_golden_checks' layer check).  fp32 tolerance 1e-4 relative (north_star).
+CPU: the set holds the fixtures and layers its record in golden_models.LAYER_SETS names."""
 import os
 
 import numpy as np
 import pytest
-import torch
 
-pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("gemm_precision")]
+import model_golden_checks as C
+
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-ALL = sorted(os.path.basename(p)[:-4] for p in glob.glob(os.path.join(GOLD, "*.npz")) if "hash_vocab" not in p)
 
-# reference weight path -> path inside this package's layer tree
-_RENAMES = [("local_att/", "local_activation_unit/"), ("activation_layers", "act"), ("bn/moving_mean", "bn/moving_mean"),
-            ("bn/moving_variance", "bn/moving_variance")]
+test_layer_matches_reference_output = C.gpu_layer_test("root")
+test_fixture_set = C.layer_tests("root").fixture_set
 
 
-def _norm(name):
-    for a, b in _RENAMES:
-        name = name.replace(a, b)
-    return name
-
-
-def _load(name):
-    d = np.load(os.path.join(GOLD, name + ".npz"))
-    meta = json.loads(str(d["meta"]))
-    ins = [d["in_%d" % i] for i in range(len([k for k in d.files if k.startswith("in_")]))]
-    w = {_norm(k[2:]): d[k] for k in d.files if k.startswith("w_")}
-    return meta, ins, w, d["out"]
-
-
-@pytest.mark.parametrize("name", ALL)
-def test_layer_matches_reference_output(cuda, name):
-    from deepctr_b200 import engine as E
-    from deepctr_b200 import layers as LY
-    meta, ins, w, want = _load(name)
-    kwargs = dict(meta["kwargs"])
-    for k in ("layer_size", "att_hidden_units", "hidden_units"):
-        if k in kwargs:
-            kwargs[k] = tuple(kwargs[k])
-    layer = getattr(LY, meta["layer"])(**kwargs)
-    vars_in = [E.to_var(a) for a in ins]
-    extra = meta["extra"]
-    mask = extra.get("mask")
-    if mask is not None:
-        # Keras masks arrive on the input tensors: rebuild them as KMask terms (valid = id != 0)
-        ms = mask if (isinstance(mask, list) and (mask[0] is None or isinstance(mask[0][0], list))) else [mask]
-        for v, m in zip(vars_in, ms):
-            if m is not None:
-                ids = torch.as_tensor(np.asarray(m, dtype=np.int32)).to(v.data.device)
-                v.mask = E.KMask(ids=[ids])
-    arg = vars_in[0] if len(vars_in) == 1 else vars_in
-    layer._maybe_build(E._shape_of(arg))
-    mine = {wt.name.split("/", 1)[1]: wt for wt in layer.weights}
-    for k, v in w.items():
-        key = k if k in mine else [n for n in mine if n.endswith(k)][0]
-        mine[key].set_value(v.reshape(mine[key].shape))
-    out = layer._invoke(arg, bool(extra.get("training", False)))
-    got = E.contiguous(out).cpu().numpy()
-    assert got.size == want.size
-    from deepctr_b200 import ops, _lib as L
-    atol = 2e-6
-    if ops.GEMM_PRECISION == L.GEMM_BF16X3 and want.size:     # normwise for the split-bf16 GEMMs (see test_layers_gpu)
-        atol = max(atol, 1e-4 * float(np.abs(want).max()))
-    np.testing.assert_allclose(got.reshape(want.shape), want, rtol=1e-4, atol=atol)
-
-
+@pytest.mark.gpu
+@pytest.mark.usefixtures("gemm_precision")
 def test_hash_known_answer_vector(cuda, tmp_path):
     """tests/layers/utils_test.py:20-22 through this package's Hash layer."""
     from deepctr_b200.layers import Hash

@@ -6,43 +6,23 @@ layer and builder code produced (tests/golden/generate_pairwise.py):
 2. the documented shape limits of the fused AFM kernels and AFM's DenseFeat refusal raise ValueError.
 """
 
-import numpy as np
 import pytest
-import torch
 
 import golden_models as G
 import model_golden_checks as C
 
-LAYER_CASES = G.layer_cases("pairwise")
 T = C.model_tests("pairwise")
 test_oracle_matches_reference_model = T.oracle
 test_builders_create_the_reference_weight_set = T.weight_set
 test_builder_graph_is_the_reference_graph = T.graph
 test_reference_default_arguments_are_the_same = T.defaults
+L = C.layer_tests("pairwise")
+test_oracle_matches_reference_layer = L.oracle
 
 
 def test_fixture_sets():
     C.check_fixture_set(G.FAMILIES["pairwise"])
-    assert len(LAYER_CASES) >= 6
-
-
-@pytest.mark.parametrize("name", LAYER_CASES)
-def test_oracle_matches_reference_layer(name):
-    import pairwise_oracle as PO
-    meta, d = G.load_layer("pairwise", name)
-    x = torch.tensor(d["x"], requires_grad=True)
-    if meta["layer"] == "AFMLayer":
-        ws = {k: torch.tensor(d["w_" + k], requires_grad=True)
-              for k in ("attention_W", "attention_b", "projection_h", "projection_p")}
-        out = PO.afm(x, **ws)
-    else:
-        ws = {}
-        out = PO.bi_interaction(x)
-    np.testing.assert_allclose(out.detach().numpy(), d["out"], rtol=1e-5, atol=1e-6)
-    (out * torch.as_tensor(d["dout"])).sum().backward()
-    np.testing.assert_allclose(x.grad.numpy(), d["gx"], rtol=1e-4, atol=1e-6)
-    for k, v in ws.items():
-        np.testing.assert_allclose(v.grad.numpy(), d["g_" + k], rtol=1e-4, atol=1e-6, err_msg=k)
+    L.fixture_set()
 
 
 def test_afm_rejects_dense_features():

@@ -1,6 +1,7 @@
 """GPU: the Bi-Interaction and fused AFM kernels, the layers and the NFM / AFM builders.
 
-* layer fixtures of the reference's own AFMLayer / BiInteractionPooling (tests/golden/pairwise/);
+* layer fixtures of the reference's own AFMLayer / BiInteractionPooling (tests/golden/pairwise/, with
+  model_golden_checks): through the layers, outputs and gradients in both GEMM precisions;
 * b2ctr_afm_fwd / _bwd and b2ctr_bi_interaction_fwd / _bwd against a float64 torch restatement over F = 2 / 26 / 64,
   E = 4 / 32, A = 1 / 8, an input that is a window of a wider buffer (ldx > F*E) and batches that are not a multiple
   of the CTA's samples; the AFM backward is bit-identical from run to run;
@@ -14,11 +15,11 @@ import pytest
 import torch
 
 import b2_helpers as H
-import golden_models as G
 import model_golden_checks as C
 
 pytestmark = pytest.mark.gpu
 
+test_layer_fixture = C.gpu_layer_test("pairwise")
 T = C.gpu_model_tests("pairwise")
 test_model_forward_matches_reference = T.forward
 test_model_sgd_step_matches_reference_gradients = T.sgd_step
@@ -51,39 +52,6 @@ def _afm_weights(cuda, E, A, rng):
     b = torch.tensor(rng.normal(0, 0.1, size=(A,)).astype(np.float32), device=cuda)
     h = torch.tensor(rng.normal(0, 1.0, size=(A,)).astype(np.float32), device=cuda)
     return W, b, h
-
-
-@pytest.mark.parametrize("name", G.layer_cases("pairwise"))
-def test_layer_fixture(cuda, name):
-    from deepctr_b200 import engine as E, kernels as K
-    from deepctr_b200.layers import AFMLayer, BiInteractionPooling
-    meta, d = G.load_layer("pairwise", name)
-    x = torch.tensor(d["x"], device=cuda)
-    B, F, Ed = x.shape
-    E.clear_session()
-    if meta["layer"] == "BiInteractionPooling":
-        out = BiInteractionPooling()(x).data
-        np.testing.assert_allclose(out.cpu().numpy(), d["out"], rtol=1e-5, atol=1e-5)
-        gx = K.bi_interaction_bwd(x.reshape(B, -1), F * Ed, F, Ed, torch.tensor(d["dout"], device=cuda).reshape(B, Ed), B)
-        np.testing.assert_allclose(gx.reshape(B, F, Ed).cpu().numpy(), d["gx"], rtol=1e-4, atol=1e-5)
-        return
-    layer = AFMLayer(**meta["kwargs"])
-    layer.build([(None, 1, Ed)] * F)
-    layer.set_weights([d["w_" + k] for k in ("attention_W", "attention_b", "projection_h", "projection_p")])
-    out = layer([x[:, f:f + 1, :] for f in range(F)]).data
-    np.testing.assert_allclose(out.cpu().numpy(), d["out"], rtol=1e-4, atol=1e-5)
-    W, b, h, p = (torch.tensor(d["w_" + k], device=cuda) for k in
-                  ("attention_W", "attention_b", "projection_h", "projection_p"))
-    att, state = K.afm_fwd(x.reshape(B, -1), F * Ed, F, Ed, W, b, h.reshape(-1), B)
-    dout = torch.tensor(d["dout"], device=cuda)                     # [B,1]
-    g = (dout @ p.T).contiguous()                                   # d att
-    dx, dW, db, dh = K.afm_bwd(g, x.reshape(B, -1), F * Ed, F, Ed, W, b, h.reshape(-1), state, att, B)
-    tol = dict(rtol=1e-4, atol=1e-5)
-    np.testing.assert_allclose(dx.reshape(B, F, Ed).cpu().numpy(), d["gx"], **tol)
-    np.testing.assert_allclose(dW.cpu().numpy(), d["g_attention_W"], **tol)
-    np.testing.assert_allclose(db.cpu().numpy(), d["g_attention_b"], **tol)
-    np.testing.assert_allclose(dh.cpu().numpy().reshape(-1, 1), d["g_projection_h"], **tol)
-    np.testing.assert_allclose((att.T @ dout).cpu().numpy(), d["g_projection_p"], **tol)
 
 
 def _check_afm(cuda, B, F, E, A, tail, seed):

@@ -8,46 +8,23 @@ builder code produced (tests/golden/generate_pnn.py):
 4. the placement of PNN's products in the DNN input is planned for PNN's graph, and only there.
 """
 
-import numpy as np
 import pytest
-import torch
 
 import golden_models as G
 import model_golden_checks as C
 
-LAYER_CASES = G.layer_cases("pnn")
 T = C.model_tests("pnn")
 test_oracle_matches_reference_model = T.oracle
 test_builder_creates_the_reference_weight_set = T.weight_set
 test_builder_graph_is_the_reference_graph = T.graph
 test_reference_default_arguments_are_the_same = T.defaults
+L = C.layer_tests("pnn")
+test_oracle_matches_reference_layer = L.oracle
 
 
 def test_fixture_sets():
     C.check_fixture_set(G.FAMILIES["pnn"])
-    assert len(LAYER_CASES) == 15
-    assert {G.load_layer("pnn", n)[0]["layer"] for n in LAYER_CASES} == {"InnerProductLayer", "OutterProductLayer"}
-
-
-def oracle_layer(meta, x, kernel):
-    import pnn_oracle as PO
-    kw = meta["kwargs"]
-    if meta["layer"] == "InnerProductLayer":
-        return PO.inner(x, kw.get("reduce_sum", True))
-    return PO.outer(x, kernel, kw["kernel_type"])
-
-
-@pytest.mark.parametrize("name", LAYER_CASES)
-def test_oracle_matches_reference_layer(name):
-    meta, d = G.load_layer("pnn", name)
-    x = torch.tensor(d["x"], requires_grad=True)
-    k = torch.tensor(d["w_kernel"], requires_grad=True) if "w_kernel" in d else None
-    out = oracle_layer(meta, x, k)
-    np.testing.assert_allclose(out.detach().numpy(), d["out"], rtol=1e-5, atol=1e-6)
-    (out * torch.as_tensor(d["dout"])).sum().backward()
-    np.testing.assert_allclose(x.grad.numpy(), d["gx"], rtol=1e-4, atol=1e-6)
-    if k is not None:
-        np.testing.assert_allclose(k.grad.numpy(), d["g_kernel"], rtol=1e-4, atol=1e-6)
+    L.fixture_set()
 
 
 def test_off_path_products_hold_no_weights():

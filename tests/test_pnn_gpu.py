@@ -6,7 +6,8 @@
   bit-identical from run to run; unsupported shapes are rejected;
 * the C2 shape (B = 65536, F = 26, E = 32): the input a window of the [B, 848] gather buffer, the scores at column
   845 of a wider buffer;
-* layer fixtures of the reference's own InnerProductLayer / OutterProductLayer (tests/golden/pnn/);
+* layer fixtures of the reference's own InnerProductLayer / OutterProductLayer (tests/golden/pnn/, with
+  model_golden_checks): through the layers, outputs and gradients in both GEMM precisions;
 * the placed step copies no product-sized block; the reference test's dnn_dropout=0.5 configuration trains with a
   finite loss;
 * model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions, placed and unplaced;
@@ -17,13 +18,13 @@ import pytest
 import torch
 
 import b2_helpers as H
-import golden_models as G
 import model_golden_checks as C
 from model_golden_checks import placement  # noqa: F401  (the placed / unplaced parameter)
 import pnn_oracle as PO
 
 pytestmark = pytest.mark.gpu
 
+test_layer_fixture = C.gpu_layer_test("pnn")
 T = C.gpu_model_tests("pnn")
 test_model_forward_matches_reference = T.forward
 test_model_sgd_step_matches_reference_gradients = T.sgd_step
@@ -146,34 +147,6 @@ def test_kernels_reject_unsupported_shapes(cuda):
     with pytest.raises(ValueError, match="does not fit"):
         K.pnn_outer_fwd(x, 65 * 65, 4, 4, torch.zeros((4, 6, 4), device=cuda), 4, out=torch.zeros((4, 8), device=cuda),
                         col0=3)
-
-
-@pytest.mark.parametrize("name", G.layer_cases("pnn"))
-def test_layer_fixture(cuda, name):
-    """The layers themselves, called on the F [B,1,E] slices, against the reference's outputs and gradients."""
-    from deepctr_b200 import engine as E
-    from deepctr_b200 import layers as Lyr
-    meta, d = G.load_layer("pnn", name)
-    E.clear_session()
-    F = d["x"].shape[1]
-    vars_in = [E.to_var(np.ascontiguousarray(d["x"][:, f:f + 1])) for f in range(F)]
-    for v in vars_in:
-        v.requires_grad = True
-    layer = getattr(Lyr, meta["layer"])(**meta["kwargs"])
-    layer._maybe_build(E._shape_of(vars_in))
-    if "w_kernel" in d:
-        layer.kernel.set_value(d["w_kernel"])
-    tape = E.Tape()
-    with E.recording(tape):
-        y = layer._invoke(vars_in, False)
-    tol = dict(rtol=1e-4, atol=1e-5)
-    np.testing.assert_allclose(E.contiguous(y).cpu().numpy().reshape(d["out"].shape), d["out"], **tol)
-    E.add_grad(y, torch.tensor(d["dout"], device=cuda).reshape(y.data.shape))
-    tape.backward()
-    gx = np.concatenate([v.grad.cpu().numpy().reshape(-1, 1, d["x"].shape[2]) for v in vars_in], axis=1)
-    np.testing.assert_allclose(gx, d["gx"], **tol)
-    if "w_kernel" in d:
-        np.testing.assert_allclose(layer.kernel.grad.cpu().numpy(), d["g_kernel"], **tol)
 
 
 def test_reference_test_configuration_trains_with_dropout(cuda):
