@@ -51,6 +51,13 @@ class UniformGather(C.Structure):
                 ("peer_tables", C.c_void_p), ("peer_lin_tables", C.c_void_p)]
 
 
+class FfmField(C.Structure):
+    """b2ctr_ffm_field_t"""
+    _fields_ = [("idx", C.c_void_p), ("pooled", C.c_void_p), ("grad", C.c_void_p), ("idx_stride", C.c_int64),
+                ("vocab", C.c_int64), ("pooled_ld", C.c_int64), ("grad_ld", C.c_int64), ("idx_dtype", C.c_int32),
+                ("hash_mode", C.c_int32)]
+
+
 class Gemm(C.Structure):
     """b2ctr_gemm_t"""
     _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("c", C.c_void_p), ("bias", C.c_void_p),
@@ -196,6 +203,8 @@ SIGNATURES = {
     "b2ctr_pnn_outer_fwd": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _vp]),
     "b2ctr_pnn_outer_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
     "b2ctr_pnn_outer_bwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _sz, _vp]),
+    "b2ctr_ffm_product_fwd": (_i32, [C.POINTER(FfmField), _i32, _vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp]),
+    "b2ctr_ffm_product_bwd": (_i32, [C.POINTER(FfmField), _i32, _vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp]),
     "b2ctr_din_att_input_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),
     "b2ctr_din_att_input_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _vp]),
     "b2ctr_din_pool_fwd": (_i32, [_vp, _vp, _i64, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),

@@ -884,6 +884,155 @@ static void launch_gather(const UniParams& p, int64_t batch, int grid, cudaStrea
   }
 }
 
+
+// ============================================================================================
+// Field-aware pairwise products (ONN / NFFM, deepctr/models/onn.py:79-97): field a has one table per partner
+// field b; pair p = (i, j), i < j, in itertools.combinations order, is  e_{i,(j)} * e_{j,(i)}.  One warp per
+// sample: the lanes resolve (and hash) the F ids once into shared memory, then walk the P pairs, each lane reading
+// its pair's two rows straight from their tables.  The [B, F(F-1), E] lookups are never written.
+// A pre-pooled field (a VarLenSparseFeat bag) is read from `pooled`, which the generic gather filled.
+// ============================================================================================
+constexpr int kFfmMaxF = 64;
+constexpr int kFfmWarps = 8;
+
+struct FfmParams {
+  b2ctr_ffm_field_t f[kFfmMaxF];
+  float* const* tables;          // device [F*F]: field a's table for partner b at a*F + b
+  float* out;                    // fwd: products; bwd: NULL
+  const float* g;                // bwd: gradient of the products, fwd: NULL
+  int64_t ld;                    // pitch of out / g
+  unsigned long long* oob;
+  int32_t F, E, reduce_sum, col;
+};
+
+template <int VEC>
+__device__ __forceinline__ typename VecT<VEC>::T vmul(typename VecT<VEC>::T a, typename VecT<VEC>::T b);
+template <>
+__device__ __forceinline__ float4 vmul<4>(float4 a, float4 b) {
+  return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w);
+}
+template <>
+__device__ __forceinline__ float vmul<1>(float a, float b) { return a * b; }
+__device__ __forceinline__ float vsum(float4 a) { return (a.x + a.y) + (a.z + a.w); }
+__device__ __forceinline__ float vsum(float a) { return a; }
+__device__ __forceinline__ float4 vbcast(float s, float4*) { return make_float4(s, s, s, s); }
+__device__ __forceinline__ float vbcast(float s, float*) { return s; }
+
+// field a's operand for partner c in sample b: a table row, a pooled row, or NULL (out-of-range id: a zero row)
+__device__ __forceinline__ const float* ffm_row(const FfmParams& p, const int64_t* ids, int a, int c, int64_t b) {
+  const b2ctr_ffm_field_t& fa = p.f[a];
+  const int s = c - (c > a);
+  if (fa.idx == nullptr) return fa.pooled + b * fa.pooled_ld + (int64_t)s * p.E;
+  const int64_t id = ids[a];
+  if (id < 0) return nullptr;
+  return p.tables[a * p.F + c] + id * p.E;
+}
+
+// the row index of a single-valued field in sample b (hashed if the field hashes), -1 when out of range
+__device__ __forceinline__ int64_t ffm_resolve_id(const b2ctr_ffm_field_t& f, int64_t b, unsigned long long* oob) {
+  int64_t id = load_idx(f.idx, b * f.idx_stride, f.idx_dtype);
+  if (f.hash_mode != B2CTR_HASH_NONE) id = farm::hash_bucket(id, f.vocab, f.hash_mode == B2CTR_HASH_FARM_MASK_ZERO);
+  if (id_in_range(id, f.vocab)) return id;
+  note_oob(oob);
+  return -1;
+}
+
+// (min 4 blocks per SM: without that bound the 64-bit hash modulo makes ptxas spill around its call)
+template <int VEC, bool BWD>
+__global__ void __launch_bounds__(kFfmWarps * 32, 4) ffm_product_kernel(const __grid_constant__ FfmParams p,
+                                                                     int64_t batch) {
+  using V = typename VecT<VEC>::T;
+  __shared__ uint16_t s_pair[kFfmMaxF * (kFfmMaxF - 1) / 2];
+  __shared__ int64_t s_id[kFfmWarps][kFfmMaxF];
+  const int F = p.F, E = p.E, P = F * (F - 1) / 2, nv = E / VEC;
+  for (int i = 0, q = 0; i < F - 1; q += F - 1 - i, ++i)
+    for (int k = threadIdx.x; k < F - 1 - i; k += blockDim.x) s_pair[q + k] = (uint16_t)((i << 8) | (i + 1 + k));
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int64_t* ids = s_id[warp];
+  for (int64_t b = (int64_t)blockIdx.x * kFfmWarps + warp; b < batch; b += (int64_t)gridDim.x * kFfmWarps) {
+    for (int a = lane; a < F; a += 32)
+      if (p.f[a].idx != nullptr) ids[a] = ffm_resolve_id(p.f[a], b, BWD ? nullptr : p.oob);
+    __syncwarp();
+    for (int q = lane; q < P; q += 32) {
+      const int i = s_pair[q] >> 8, j = s_pair[q] & 0xff;
+      const float* ri = ffm_row(p, ids, i, j, b);
+      const float* rj = ffm_row(p, ids, j, i, b);
+      if (!BWD) {
+        float* o = p.out + b * p.ld + p.col;
+        float acc = 0.f;
+        for (int c = 0; c < nv; ++c) {
+          const V x = ri ? vload(ri + c * VEC, (V*)nullptr) : vzero<VEC>();
+          const V y = rj ? vload(rj + c * VEC, (V*)nullptr) : vzero<VEC>();
+          const V z = vmul<VEC>(x, y);
+          if (p.reduce_sum) acc += vsum(z);
+          else *reinterpret_cast<V*>(o + (int64_t)q * E + c * VEC) = z;
+        }
+        if (p.reduce_sum) o[q] = acc;
+      } else {
+        // d e_{i,(j)} = g_p * e_{j,(i)},  d e_{j,(i)} = g_p * e_{i,(j)}: one writer per element, no atomics
+        const float* gr = p.g + b * p.ld + p.col;
+        const b2ctr_ffm_field_t& fi = p.f[i];
+        const b2ctr_ffm_field_t& fj = p.f[j];
+        float* di = fi.grad + b * fi.grad_ld + (int64_t)(j - 1) * E;
+        float* dj = fj.grad + b * fj.grad_ld + (int64_t)i * E;
+        const float gs = p.reduce_sum ? gr[q] : 0.f;
+        for (int c = 0; c < nv; ++c) {
+          const V x = ri ? vload(ri + c * VEC, (V*)nullptr) : vzero<VEC>();
+          const V y = rj ? vload(rj + c * VEC, (V*)nullptr) : vzero<VEC>();
+          const V gv = p.reduce_sum ? vbcast(gs, (V*)nullptr)
+                                    : *reinterpret_cast<const V*>(gr + (int64_t)q * E + c * VEC);
+          *reinterpret_cast<V*>(di + c * VEC) = vmul<VEC>(gv, y);
+          *reinterpret_cast<V*>(dj + c * VEC) = vmul<VEC>(gv, x);
+        }
+      }
+    }
+    __syncwarp();
+  }
+}
+
+static b2ctr_status_t ffm_params(const b2ctr_ffm_field_t* fields, int32_t nfield, float* const* tables, int32_t dim,
+                                 int32_t reduce_sum, int64_t ld, int32_t col, int64_t batch, bool bwd, FfmParams* p,
+                                 bool* vec4) {
+  B2_REQUIRE(nfield >= 2 && nfield <= kFfmMaxF, "ffm_product: the field count must be in [2, %d] (got %d)",
+             kFfmMaxF, nfield);
+  B2_REQUIRE(dim >= 1 && dim <= 64, "ffm_product: dim must be in [1, 64] (got %d)", dim);
+  B2_REQUIRE(fields && tables && batch >= 0 && col >= 0, "ffm_product: NULL pointer or negative batch / column");
+  B2_REQUIRE(reduce_sum == 0 || reduce_sum == 1, "ffm_product: reduce_sum must be 0 or 1");
+  const int64_t P = (int64_t)nfield * (nfield - 1) / 2;
+  B2_REQUIRE(ld >= col + P * (reduce_sum ? 1 : dim), "ffm_product: row pitch %lld too small for %lld products",
+             (long long)ld, (long long)P);
+  bool v4 = dim % 4 == 0 && ld % 4 == 0 && col % 4 == 0 && aligned16(tables);
+  for (int a = 0; a < nfield; ++a) {
+    const b2ctr_ffm_field_t& f = fields[a];
+    B2_REQUIRE((f.idx != nullptr) != (f.pooled != nullptr), "ffm_product: field %d needs exactly one of ids and "
+               "a pooled operand", a);
+    if (f.idx) {
+      B2_REQUIRE(f.idx_dtype == B2CTR_IDX_I32 || f.idx_dtype == B2CTR_IDX_I64, "ffm_product: field %d bad idx dtype", a);
+      B2_REQUIRE(f.hash_mode >= B2CTR_HASH_NONE && f.hash_mode <= B2CTR_HASH_FARM_MASK_ZERO && f.vocab >= 1,
+                 "ffm_product: field %d bad hash mode or vocabulary", a);
+    } else {
+      B2_REQUIRE(f.pooled_ld >= (int64_t)(nfield - 1) * dim, "ffm_product: field %d pooled pitch too small", a);
+      v4 = v4 && f.pooled_ld % 4 == 0 && aligned16(f.pooled);
+    }
+    if (bwd) {
+      B2_REQUIRE(f.grad && f.grad_ld >= (int64_t)(nfield - 1) * dim, "ffm_product: field %d needs a gradient "
+                 "buffer of pitch >= (F-1)*dim", a);
+      v4 = v4 && f.grad_ld % 4 == 0 && aligned16(f.grad);
+    }
+    p->f[a] = f;
+  }
+  p->tables = tables;
+  p->ld = ld;
+  p->oob = oob_counter();
+  p->F = nfield;
+  p->E = dim;
+  p->reduce_sum = reduce_sum;
+  p->col = col;
+  *vec4 = v4;
+  return B2CTR_OK;
+}
+
 }  // namespace b2ctr
 
 using namespace b2ctr;
@@ -1019,6 +1168,44 @@ b2ctr_status_t b2ctr_init_normal(float* dst, int64_t n, float mean, float std, u
   init_normal_kernel<<<grid_for((n + 3) / 4, 256, 8), 256, 0, (cudaStream_t)stream>>>(dst, n, mean,
                                                                                      std, seed);
   B2_CHECK_LAUNCH("b2ctr_init_normal");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_ffm_product_fwd(const b2ctr_ffm_field_t* fields, int32_t nfield, float* const* tables,
+                                     int32_t dim, int32_t reduce_sum, float* out, int64_t out_ld, int32_t out_col,
+                                     int64_t batch, void* stream) {
+  FfmParams p;
+  bool v4;
+  b2ctr_status_t s = ffm_params(fields, nfield, tables, dim, reduce_sum, out_ld, out_col, batch, false, &p, &v4);
+  if (s != B2CTR_OK) return s;
+  B2_REQUIRE(out, "ffm_product_fwd: NULL out");
+  p.out = out;
+  p.g = nullptr;
+  v4 = v4 && aligned16(out);
+  if (batch == 0) return B2CTR_OK;
+  const int grid = grid_for(batch, kFfmWarps, 8);
+  if (v4) ffm_product_kernel<4, false><<<grid, kFfmWarps * 32, 0, (cudaStream_t)stream>>>(p, batch);
+  else ffm_product_kernel<1, false><<<grid, kFfmWarps * 32, 0, (cudaStream_t)stream>>>(p, batch);
+  B2_CHECK_LAUNCH("b2ctr_ffm_product_fwd");
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_ffm_product_bwd(const b2ctr_ffm_field_t* fields, int32_t nfield, float* const* tables,
+                                     int32_t dim, int32_t reduce_sum, const float* g, int64_t g_ld, int32_t g_col,
+                                     int64_t batch, void* stream) {
+  FfmParams p;
+  bool v4;
+  b2ctr_status_t s = ffm_params(fields, nfield, tables, dim, reduce_sum, g_ld, g_col, batch, true, &p, &v4);
+  if (s != B2CTR_OK) return s;
+  B2_REQUIRE(g, "ffm_product_bwd: NULL gradient");
+  p.out = nullptr;
+  p.g = g;
+  v4 = v4 && aligned16(g);
+  if (batch == 0) return B2CTR_OK;
+  const int grid = grid_for(batch, kFfmWarps, 8);
+  if (v4) ffm_product_kernel<4, true><<<grid, kFfmWarps * 32, 0, (cudaStream_t)stream>>>(p, batch);
+  else ffm_product_kernel<1, true><<<grid, kFfmWarps * 32, 0, (cudaStream_t)stream>>>(p, batch);
+  B2_CHECK_LAUNCH("b2ctr_ffm_product_bwd");
   return B2CTR_OK;
 }
 

@@ -815,6 +815,39 @@ class Add(Layer):
         return tuple(best)
 
 
+class Multiply(Layer):
+    """tf.keras.layers.Multiply: the elementwise product of same-shaped inputs.  ONN's products (onn.py:94) are
+    served by the planner's field-aware kernel; a product the planner did not claim runs here on b2ctr_ewise."""
+
+    def compute_output_shape(self, input_shape):
+        shapes = [tuple(s) for s in input_shape]
+        if len(shapes) < 2:
+            raise ValueError("A merge layer should be called on a list of at least 2 inputs. Got %d inputs."
+                             % len(shapes))
+        for s in shapes[1:]:
+            if tuple(s[1:]) != tuple(shapes[0][1:]):
+                raise ValueError("Multiply: operands of shapes %s and %s differ (embedding dimensions %s and %s)"
+                                 % (shapes[0], s, shapes[0][-1], s[-1]))
+        return shapes[0]
+
+    def call(self, inputs, **kwargs):
+        return ops.multiply(list(inputs))
+
+
+def multiply(inputs, **kwargs):
+    """The functional interface to Multiply (tf.keras.layers.multiply)."""
+    return Multiply(**kwargs)(inputs)
+
+
+class _ShapeProbe(object):
+    """What Lambda.compute_output_shape hands its function to learn the output shape without running it: the
+    backend functions (``deepctr_b200.backend``) map a probe to a probe of their result's shape."""
+
+    def __init__(self, shape, summed_from=None):
+        self.shape = tuple(shape)
+        self.summed_from = summed_from      # (probe, axis) when this is backend.sum's result on ``probe``
+
+
 class Lambda(Layer):
     """tf.keras.layers.Lambda.  ``function`` receives / returns Vars; only ``ops`` functions make
     sense inside (DenseFeat.transform_fn, deepctr/inputs.py:170)."""
@@ -823,6 +856,7 @@ class Lambda(Layer):
         Layer.__init__(self, **kwargs)
         self.function = function
         self._out_shape = output_shape
+        self.reduces_last_axis = False
 
     def call(self, inputs, **kwargs):
         return self.function(inputs)
@@ -832,6 +866,17 @@ class Lambda(Layer):
         of an elementwise lambda such as ``x[0] * expand_dims(x[1], -1)``), so that the Lambda has one output."""
         if self._out_shape is not None:
             return self._out_shape
+        if not isinstance(input_shape, list):
+            x = _ShapeProbe(input_shape)
+            try:
+                probe = self.function(x)
+            except Exception:
+                probe = None
+            if isinstance(probe, _ShapeProbe):       # e.g. ONN's Lambda(lambda x: K.sum(x, axis=-1))
+                # the planner serves a sum over the last axis of the input from its own product kernel
+                self.reduces_last_axis = (probe.summed_from is not None and probe.summed_from[0] is x
+                                          and probe.summed_from[1] == len(x.shape) - 1)
+                return probe.shape
         if isinstance(input_shape, list) and input_shape and isinstance(input_shape[0], (list, tuple)):
             return tuple(max(input_shape, key=len))
         return input_shape

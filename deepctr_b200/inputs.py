@@ -17,6 +17,7 @@ Concatenations of those windows are then zero-copy views, and the backward pass 
 scatter (+ SGD update) launch.
 """
 from collections import defaultdict, OrderedDict
+import itertools
 from itertools import chain
 
 import ctypes as C
@@ -274,8 +275,13 @@ class EmbeddingPlanner(object):
         def as_input(t):
             return t.name if (isinstance(t.node.layer, E.InputLayer) and t.name in input_names) else None
 
+        # ONN's field-aware lookups and their products: one kernel pair of their own, never slots of the gather
+        self.ffm = _plan_field_aware(model, consumers, out_ids, as_input)
+        claimed = self.ffm.claimed if self.ffm is not None else ()
         for node in model._order:
             if not isinstance(node.layer, Embedding) or not isinstance(node.inputs, E.KTensor):
+                continue
+            if id(node) in claimed:
                 continue
             src, hcfg, virt = node.inputs, None, []
             if isinstance(src.node.layer, Hash) and isinstance(src.node.inputs, E.KTensor):
@@ -376,12 +382,16 @@ class EmbeddingPlanner(object):
 
     def configure(self, optimizer, mode):
         self.optimizer, self.mode = optimizer, mode
-        total = sum(w.numel() for w in self.tables())
+        total = sum(w.numel() for w in self.tables()) + (self.ffm.numel() if self.ffm is not None else 0)
         sparse = mode in ("sparse", "sparse_deterministic") or (mode == "auto" and total > (1 << 22))
         # 'sparse_deterministic': sort + ordered segmented reduce instead of fp32 atomics (bit-identical from run
         # to run); it is also the path of row-state optimizers, i.e. Keras' lazy sparse Adagrad.  Keras' Adam
         # decays m and v of EVERY row each step (SURVEY.md App. C): it has no faithful row-wise form.
         self.sorted_update = bool(sparse and (mode == "sparse_deterministic" or optimizer.name == "adagrad"))
+        if self.sorted_update and self.ffm is not None:
+            raise ValueError("the deterministic / Adagrad row-wise update does not cover ONN's field-aware tables "
+                             "(%s ..., %d tables): use embedding_update='dense', or 'sparse' with the 'sgd' optimizer"
+                             % (self.ffm.tables[0][1].name, self.ffm.n_tables()))
         if sparse and optimizer.name not in ("sgd", "adagrad"):
             raise ValueError("row-wise (sparse) embedding updates support 'sgd' and 'adagrad'; %r keeps dense state "
                              "for every row of every table - use embedding_update='dense' (O(vocabulary) per step)"
@@ -520,6 +530,8 @@ class EmbeddingPlanner(object):
         self.fm_result = self.lin_result = None
         self.tail_done = None
         self.planes_result = None
+        if self.ffm is not None:
+            self.ffm.forward(feed, self.results, training and E.current_tape() is not None)
         if not self.slots:
             return
         some = feed[self.slots[0].input_name].data
@@ -1112,6 +1124,250 @@ def _plan_dnn_input(model, consumers, out_ids):
         for k, l in enumerate(layers):
             places[id(l)] = (pl, k)
     return places
+
+
+class FieldAwarePlan(object):
+    """ONN's field-aware products (deepctr/models/onn.py:79-97) served by one b2ctr_ffm_product_fwd launch: the
+    output of pair p's ``multiply`` (or of the ``K.sum`` Lambda behind it) is the column window [p*E, (p+1)*E) (or
+    [p, p+1)) of one [B, P*E] (or [B, P]) buffer, so concat_func + Flatten of the P outputs is a zero-copy view of
+    it.  The backward is one tape node on that buffer: b2ctr_ffm_product_bwd writes every lookup's gradient row
+    into a [B, F(F-1)*E] scratch at the tables' pre-step values, then b2ctr_embed_scatter_add applies the scratch,
+    one single-valued or pooled feature per lookup, to the tables (fused SGD) or their dense gradients.
+
+    A VarLenSparseFeat field is pooled per partner by the generic gather into a [B, (F-1)*E] operand that the
+    product kernel reads; its gradient rows go back through the same scatter's pooling Jacobian.
+
+    ``fields[a]``: (input name, maxlen, pool, hash mode, vocabulary); ``tables[a*F + b]``: (a, b) -> Embedding layer
+    (None on the diagonal); ``pair_nodes[p]``: the node whose output pair p's window is; ``virtual``: every other
+    node the plan replaces."""
+
+    def __init__(self, fields, tables, E_, reduce_sum, pair_nodes, virtual, claimed):
+        self.fields, self.E, self.reduce_sum = fields, E_, reduce_sum
+        self.F = len(fields)
+        self.table_of = tables
+        self.tables = [(k, t) for k, t in enumerate(tables) if t is not None]
+        self.pair_nodes, self.virtual, self.claimed = pair_nodes, virtual, claimed
+        self.P = self.F * (self.F - 1) // 2
+        self.width = self.P * (1 if reduce_sum else E_)
+        self.ld = (self.width + 3) // 4 * 4
+        self._ptrs, self._dev_ptrs = None, None
+
+    def n_tables(self):
+        return len(self.tables)
+
+    def numel(self):
+        return sum(t.embeddings.numel() for _, t in self.tables)
+
+    def _slot(self, a, b):
+        return b - (b > a)
+
+    def _table_array(self, dev):
+        """The device array [F*F] of table pointers, kept at one address (a captured step reads it) and rewritten
+        in place only when a table moved."""
+        ptrs = tuple(t.embeddings.materialize().data_ptr() if t is not None else 0 for t in self.table_of)
+        if ptrs != self._ptrs:
+            host = torch.tensor(ptrs, dtype=torch.int64)
+            if self._dev_ptrs is None:
+                self._dev_ptrs = host.to(dev)
+            else:
+                self._dev_ptrs.copy_(host)
+            self._ptrs = ptrs
+        return self._dev_ptrs
+
+    def _bag_features(self, a, feed, buf, tables=None, scale_of=None):
+        """The generic-gather features of pooled field a: one bag per partner, at its slot of ``buf``."""
+        name, maxlen, pool, hash_mode, vocab = self.fields[a]
+        ids = feed[name].data
+        out = []
+        for b in range(self.F):
+            if b == a:
+                continue
+            emb = self.table_of[a * self.F + b].embeddings
+            tab = emb.materialize() if tables is None or tables[a * self.F + b] is None else tables[a * self.F + b]
+            col = self._slot(a, b) * self.E if tables is None else (a * (self.F - 1) + self._slot(a, b)) * self.E
+            out.append(K.make_feature(tab, ids, buf, out_col=col, out_ld=buf.stride(0), maxlen=maxlen, pool=pool,
+                                      mask_mode=L.MASK_ZERO_ID, hash_mode=hash_mode, vocab=vocab,
+                                      src_table=emb.data if (tables is not None and pool == L.POOL_MAX) else None))
+        return out
+
+    def forward(self, feed, results, grad):
+        F, E_ = self.F, self.E
+        some = feed[self.fields[0][0]].data
+        b, dev = some.shape[0], some.device
+        ptrs = self._table_array(dev)
+        pooled, kfields = {}, []
+        bags = []
+        for a, (name, maxlen, pool, hash_mode, vocab) in enumerate(self.fields):
+            if pool == L.POOL_NONE:
+                kfields.append(K.ffm_field(idx=feed[name].data.reshape(b, -1), vocab=vocab, hash_mode=hash_mode))
+            else:
+                pooled[a] = torch.empty((b, (F - 1) * E_), dtype=torch.float32, device=dev)
+                bags.extend(self._bag_features(a, feed, pooled[a]))
+                kfields.append(K.ffm_field(pooled=pooled[a]))
+        for c in range(0, len(bags), L.MAX_FEATURES):
+            K.embed_gather_fwd(bags[c:c + L.MAX_FEATURES], b)
+        buf = E.Var(torch.empty((b, self.ld), dtype=torch.float32, device=dev), ncols=self.width, owner=self,
+                    name="__ffm_products__")
+        K.ffm_product_fwd(kfields, ptrs, E_, self.reduce_sum, buf.data, 0, b)
+        trainable = any(t.embeddings.trainable for _, t in self.tables)
+        buf.requires_grad = grad and trainable
+        w = 1 if self.reduce_sum else E_
+        for p, node in enumerate(self.pair_nodes):
+            results[id(node)] = ops_window(buf, p * w, w, (b, 1) if self.reduce_sum else (b, 1, E_))
+        for node in self.virtual:
+            results[id(node)] = VIRTUAL
+        if buf.requires_grad:
+            E.current_tape().record([buf], lambda grads: self._backward(feed, buf, pooled, b))
+
+    def _backward(self, feed, buf, pooled, b):
+        g = buf.grad
+        if g is None:
+            return
+        F, E_ = self.F, self.E
+        opt = E.current_opt()
+        ptrs = self._table_array(g.device)
+        scratch = torch.empty((b, F * (F - 1) * E_), dtype=torch.float32, device=g.device)
+        kfields = []
+        for a, (name, maxlen, pool, hash_mode, vocab) in enumerate(self.fields):
+            gv = scratch[:, a * (F - 1) * E_:]
+            if pool == L.POOL_NONE:
+                kfields.append(K.ffm_field(idx=feed[name].data.reshape(b, -1), vocab=vocab, hash_mode=hash_mode,
+                                           grad=gv))
+            else:
+                kfields.append(K.ffm_field(pooled=pooled[a], grad=gv))
+        K.ffm_product_bwd(kfields, ptrs, E_, self.reduce_sum, g, 0, b)
+        # every lookup's row of the scratch, applied to its table: one feature each, grouped by update scale
+        targets = [None] * (F * F)
+        for k, t in self.tables:
+            if t.embeddings.trainable:
+                targets[k] = _grad_target(t.embeddings, opt)
+        groups = defaultdict(list)
+        for a, (name, maxlen, pool, hash_mode, vocab) in enumerate(self.fields):
+            tabs = [tg[0] if tg is not None else None for tg in targets]
+            if pool == L.POOL_NONE:
+                ids = feed[name].data.reshape(b, -1)
+                for c in range(F):
+                    if c == a or targets[a * F + c] is None:
+                        continue
+                    f = K.make_feature(tabs[a * F + c], ids, scratch, out_col=(a * (F - 1) + self._slot(a, c)) * E_,
+                                       out_ld=scratch.stride(0), hash_mode=hash_mode, vocab=vocab)
+                    groups[targets[a * F + c][1]].append(f)
+            else:
+                keep = [c for c in range(F) if c != a]
+                for c, f in zip(keep, self._bag_features(a, feed, scratch, tables=tabs)):
+                    if targets[a * F + c] is not None:
+                        groups[targets[a * F + c][1]].append(f)
+        for sc, feats in sorted(groups.items()):
+            for c in range(0, len(feats), L.MAX_FEATURES):
+                K.embed_scatter_add(feats[c:c + L.MAX_FEATURES], b, sc)
+
+
+def ops_window(base, col0, ncols, shape):
+    from . import ops
+    return ops._window(base, col0, ncols, shape)
+
+
+MAX_FFM_FIELDS, MAX_FFM_DIM = 64, 64       # b2ctr_ffm_product_fwd's limits
+
+
+def _plan_field_aware(model, consumers, out_ids, as_input):
+    """The FieldAwarePlan of ONN's graph (deepctr/models/onn.py:79-97), or None.  Per pair (i, j) of
+    itertools.combinations order: multiply([lookup_i, lookup_j]), optionally followed by Lambda(K.sum(., axis=-1)),
+    where a lookup is NoMask(Embedding(ids)) for a single-valued field or SequencePoolingLayer(combiner,
+    supports_masking=True)(Embedding(mask_zero=True)(ids)) for a varlen one, its ids a model input, optionally
+    through Hash(vocabulary_size).  Every intermediate has exactly one consumer and every layer one call.  The pairs
+    must name F fields and cover all F(F-1)/2 pairs in order, with one table per (field, partner); anything else
+    plans nothing and each layer runs as itself."""
+    from .layers.sequence import SequencePoolingLayer
+    from .layers.utils import Hash, NoMask
+    calls = defaultdict(int)
+    for node in model._order:
+        calls[id(node.layer)] += 1
+
+    def only_use(t):
+        return len(consumers[id(t)]) == 1 and id(t) not in out_ids
+
+    def lookup(t):
+        if not only_use(t) or calls[id(t.node.layer)] != 1 or not isinstance(t.node.inputs, E.KTensor):
+            return None
+        outer = t.node
+        if isinstance(outer.layer, NoMask):
+            pool = L.POOL_NONE
+        elif isinstance(outer.layer, SequencePoolingLayer) and outer.layer.supports_masking:
+            pool = L.POOL_BY_NAME[outer.layer.mode]
+        else:
+            return None
+        e = outer.inputs
+        emb = e.node.layer
+        if (not only_use(e) or not isinstance(emb, Embedding) or calls[id(emb)] != 1
+                or not isinstance(e.node.inputs, E.KTensor) or emb.mask_zero != (pool != L.POOL_NONE)):
+            return None
+        virt = [outer, e.node]
+        src, hash_mode = e.node.inputs, L.HASH_NONE
+        if isinstance(src.node.layer, Hash):
+            h = src.node.layer
+            if (not only_use(src) or h.mask_zero or h.vocabulary_path or calls[id(h)] != 1
+                    or not isinstance(src.node.inputs, E.KTensor)):
+                return None
+            virt.append(src.node)
+            src, hash_mode = src.node.inputs, L.HASH_FARM
+            if src.dtype in ("string", str):
+                return None
+        name = as_input(src)
+        if name is None:
+            return None
+        maxlen = int(np.prod(src.shape[1:])) if len(src.shape) > 1 else 1
+        if (pool == L.POOL_NONE) != (maxlen == 1):
+            return None
+        return (name, maxlen, pool, hash_mode, emb.input_dim), emb, virt
+
+    pairs = []
+    for node in model._order:
+        if not isinstance(node.layer, E.Multiply) or calls[id(node.layer)] != 1:
+            continue
+        ins = E._flatten(node.inputs)
+        sides = [lookup(t) for t in ins] if len(ins) == 2 else [None]
+        if any(sd is None for sd in sides):
+            continue
+        out, served, virt, reduce_sum = node.outputs[0], node, [node], False
+        if only_use(out):
+            nxt = consumers[id(out)][0]
+            if isinstance(nxt.layer, E.Lambda) and getattr(nxt.layer, "reduces_last_axis", False):
+                served, reduce_sum = nxt, True
+            else:
+                virt = []
+        else:
+            virt = []
+        pairs.append((sides, served, virt if reduce_sum else [], reduce_sum))
+    if not pairs:
+        return None
+    fields, index = [], {}
+    for sides, _, _, _ in pairs:
+        for fd, _, _ in sides:
+            if fd[0] not in index:
+                index[fd[0]] = len(fields)
+                fields.append(fd)
+    F = len(fields)
+    combos = list(itertools.combinations(range(F), 2))
+    if not 2 <= F <= MAX_FFM_FIELDS or len(pairs) != len(combos) or len(set(r for *_, r in pairs)) != 1:
+        return None
+    tables, pair_nodes, virtual, claimed = [None] * (F * F), [], [], set()
+    E_ = None
+    for (i, j), (sides, served, virt, _) in zip(combos, pairs):
+        (fi, ei, vi), (fj, ej, vj) = sides
+        if index[fi[0]] != i or index[fj[0]] != j or fi != fields[i] or fj != fields[j]:
+            return None
+        if E_ is None:
+            E_ = ei.output_dim
+        if ei.output_dim != E_ or ej.output_dim != E_ or not 1 <= E_ <= MAX_FFM_DIM:
+            return None
+        tables[i * F + j], tables[j * F + i] = ei, ej
+        pair_nodes.append(served)
+        virtual.extend(vi + vj + virt)
+        claimed.update(id(n) for n in vi + vj if isinstance(n.layer, Embedding))
+    if len(set(id(t) for t in tables if t is not None)) != F * (F - 1):
+        return None
+    return FieldAwarePlan(fields, tables, E_, pairs[0][3], pair_nodes, virtual, claimed)
 
 
 # ================================================================================================

@@ -545,8 +545,39 @@ def profile_summary():
     return out
 
 
+# ---- field-aware pairwise products (ONN) ---------------------------------------------------------------
+def ffm_field(idx=None, vocab=1, hash_mode=L.HASH_NONE, pooled=None, grad=None):
+    """One b2ctr_ffm_field_t: a single-valued field's ids [B] (or a strided column), or a pooled operand [B, ld]
+    holding its F-1 per-partner rows; ``grad`` [B, ld] receives the backward's per-partner gradient rows."""
+    _require_cuda(idx, pooled, grad)
+    f = L.FfmField()
+    if idx is not None:
+        f.idx, f.idx_stride, f.idx_dtype = idx.data_ptr(), idx.stride(0), idx_dtype(idx)
+        f.vocab, f.hash_mode = int(vocab), hash_mode
+    if pooled is not None:
+        f.pooled, f.pooled_ld = pooled.data_ptr(), pooled.stride(0)
+    if grad is not None:
+        f.grad, f.grad_ld = grad.data_ptr(), grad.stride(0)
+    return f
+
+
+def ffm_product_fwd(fields, tables, dim, reduce_sum, out, out_col, batch):
+    """prod_p = e_{i,(j)} * e_{j,(i)} for every pair into ``out`` [B, ld] from column ``out_col``; ``tables`` the
+    device int64 array [F*F] of table pointers."""
+    arr = (L.FfmField * len(fields))(*fields)
+    _lib_call("ffm_product_fwd", arr, len(fields), ptr(tables), dim, int(reduce_sum), ptr(out), out.stride(0),
+              out_col, batch, stream())
+
+
+def ffm_product_bwd(fields, tables, dim, reduce_sum, g, g_col, batch):
+    """Per-lookup gradient rows into each field's ``grad`` buffer, read at the tables' current values."""
+    arr = (L.FfmField * len(fields))(*fields)
+    _lib_call("ffm_product_bwd", arr, len(fields), ptr(tables), dim, int(reduce_sum), ptr(g), g.stride(0), g_col,
+              batch, stream())
+
+
 for _n in ("embed_update_sorted", "split_planes", "embed_gather_fwd", "embed_scatter_add", "embed_gather_uniform_fwd", "embed_scatter_uniform_bwd",
-           "hash64", "gemm", "bias_act_bwd", "act_fwd", "add_n", "axpy", "fill", "copy2d", "rowsum", "fm_fwd",
+           "ffm_product_fwd", "ffm_product_bwd", "hash64", "gemm", "bias_act_bwd", "act_fwd", "add_n", "axpy", "fill", "copy2d", "rowsum", "fm_fwd",
            "fm_bwd", "predict_loss", "sgd_step", "sgd_step_multi", "adam_step", "adagrad_step", "mask_nonzero_and",
            "mask_from_len"):
     globals()[_n] = _timed(globals()[_n])

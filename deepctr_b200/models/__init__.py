@@ -11,6 +11,7 @@ from .deepfefm import DeepFEFM
 from .pnn import PNN
 from .ifm import IFM
 from .difm import DIFM
+from .onn import ONN
 
 __all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM", "PNN",
-           "IFM", "DIFM"]
+           "IFM", "DIFM", "ONN"]

@@ -1458,7 +1458,34 @@ def reduce(x, kind, axis, keep_dims):
     if kind == "sum" and (axis in (-1, x.data.dim() - 1)) and x.data.dim() == 2:
         r = rowsum(x)
         return r if keep_dims else reshape(r, (x.shape[0],))
+    shape = tuple(x.data.shape)
+    if (kind == "sum" and x.data.dim() > 2 and axis in (-1, x.data.dim() - 1)
+            and all(d == 1 for d in shape[1:-1])):
+        # [B, 1.., E] over the last axis (ONN's K.sum(product, axis=-1), onn.py:96): the row sum of [B, E]
+        r = rowsum(x)
+        return reshape(r, shape[:-1] + ((1,) if keep_dims else ()))
     raise NotImplementedError("reduce_%s over axis %r of a %d-D tensor" % (kind, axis, x.data.dim()))
+
+
+def multiply(xs):
+    """Keras Multiply of same-shaped operands on b2ctr_ewise; d a_k = g * prod of the others."""
+    if len(xs) != 2:
+        return multiply([multiply(xs[:-1]), xs[-1]])
+    a, b = xs
+    if tuple(a.shape) != tuple(b.shape):
+        raise ValueError("multiply: operands of shapes %s and %s differ" % (tuple(a.shape), tuple(b.shape)))
+    at, bt = E.contiguous(a), E.contiguous(b)
+    res = E.Var(K.ewise(0, at, bt))
+
+    def bwd(grads):
+        g = grads[0].reshape(at.shape).contiguous()
+        if a.requires_grad:
+            E.add_grad(a, K.ewise(0, g, bt))
+        if b.requires_grad:
+            E.add_grad(b, K.ewise(0, g, at))
+
+    E.record([res], [a, b], bwd)
+    return res
 
 
 def div(x, y):

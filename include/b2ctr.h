@@ -71,7 +71,8 @@ enum { B2CTR_IDX_I32 = 0, B2CTR_IDX_I64 = 1 };
 enum { B2CTR_POOL_NONE = 0, /* emit the [T,dim] sequence, no pooling (DIN keys)      */
        B2CTR_POOL_SUM = 1, B2CTR_POOL_MEAN = 2, B2CTR_POOL_MAX = 3 };
 enum { B2CTR_MASK_NONE = 0,   /* every position valid                                  */
-       B2CTR_MASK_ZERO_ID = 1,/* Keras mask_zero: position valid iff raw id != 0       */
+       B2CTR_MASK_ZERO_ID = 1,/* Keras mask_zero: position valid iff id != 0, tested on the id AFTER hashing
+                                 (the raw id only under B2CTR_HASH_FARM_MASK_ZERO, which keeps 0 as 0) */
        B2CTR_MASK_LENGTH = 2  /* tf.sequence_mask: position t valid iff t < len[b]     */ };
 enum { B2CTR_HASH_NONE = 0,
        B2CTR_HASH_FARM = 1,          /* Fingerprint64(decimal(id)) % num_buckets                 */
@@ -190,6 +191,42 @@ B2CTR_API b2ctr_status_t b2ctr_embed_scatter_uniform_bwd_ex(const b2ctr_uniform_
  * counter; this call reads (and optionally resets) it, synchronising `stream` - the host mirror raises
  * ValueError like TF-CPU when it is non-zero. */
 B2CTR_API b2ctr_status_t b2ctr_embed_oob_count(int64_t* count, int32_t reset, void* stream);
+
+/* Field-aware pairwise products (ONN / NFFM, deepctr/models/onn.py): field a owns one [vocab_a, dim] table per
+ * partner field b != a.  Pair p = (i, j), i < j, in itertools.combinations order, is
+ *   prod_p = e_{i,(j)} * e_{j,(i)}          e_{a,(b)} = field a's row in its table for partner b
+ * written to out[b*out_ld + out_col + p*dim + e] (reduce_sum = 0) or its sum over e to out[b*out_ld + out_col + p]
+ * (reduce_sum = 1).  One launch forms all P = F(F-1)/2 products from the tables; the F(F-1) looked-up rows are
+ * never written.  A hashed field is hashed once per sample.  An id outside [0, vocab) reads a zero row and is
+ * counted as for every other gather (b2ctr_embed_oob_count).
+ *   tables: DEVICE array [F*F] of device pointers, field a's table for partner b at a*F + b (the diagonal is
+ *           unused); it can stay at one address for the life of a model, so a captured step keeps it.
+ * A field is either single-valued (idx != NULL) or a pre-pooled operand (pooled != NULL: a VarLenSparseFeat bag
+ * pooled per partner by b2ctr_embed_gather_fwd).  Partner b of field a has slot s = b - (b > a) in `pooled` and
+ * `grad`, whose rows hold F-1 operands of dim floats.  2 <= F <= 64, 1 <= dim <= 64. */
+typedef struct b2ctr_ffm_field {
+  const void* idx;       /* single-valued: the id of sample b at idx[b*idx_stride]; NULL for a pooled field       */
+  const float* pooled;   /* pooled: the operand for partner slot s at pooled[b*pooled_ld + s*dim]; else NULL     */
+  float* grad;           /* bwd: d(operand) of partner slot s goes to grad[b*grad_ld + s*dim] (written, no add)  */
+  int64_t idx_stride;
+  int64_t vocab;         /* rows of each of the field's tables; also num_buckets for hashing                     */
+  int64_t pooled_ld;
+  int64_t grad_ld;
+  int32_t idx_dtype;     /* B2CTR_IDX_*                                                                          */
+  int32_t hash_mode;     /* B2CTR_HASH_*                                                                         */
+} b2ctr_ffm_field_t;
+
+B2CTR_API b2ctr_status_t b2ctr_ffm_product_fwd(const b2ctr_ffm_field_t* fields, int32_t nfield,
+                                               float* const* tables, int32_t dim, int32_t reduce_sum, float* out,
+                                               int64_t out_ld, int32_t out_col, int64_t batch, void* stream);
+/* Gradient rows of every lookup at the tables' current (pre-step) values, given g = d(out) in the layout of the
+ * forward's out:  d e_{i,(j)} = g_p * e_{j,(i)},  d e_{j,(i)} = g_p * e_{i,(j)}  (g_p broadcast over e when
+ * reduce_sum).  Each element has one writer: the result is the same bit for bit from run to run.  The tables are
+ * only read; the caller applies the rows with b2ctr_embed_scatter_add, one single-valued (or pooled) feature per
+ * lookup, which also skips out-of-range ids. */
+B2CTR_API b2ctr_status_t b2ctr_ffm_product_bwd(const b2ctr_ffm_field_t* fields, int32_t nfield,
+                                               float* const* tables, int32_t dim, int32_t reduce_sum, const float* g,
+                                               int64_t g_ld, int32_t g_col, int64_t batch, void* stream);
 
 /* DETERMINISTIC fused update of the Criteo-shaped fast path (same descriptor and gradients as
  * b2ctr_embed_scatter_uniform_bwd; tables whole, world <= 1): the lookups are sorted by (table, id), the
