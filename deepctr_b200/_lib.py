@@ -96,6 +96,20 @@ class Mha(C.Structure):
                 ("dk", C.c_void_p), ("lddk", C.c_int64), ("dv", C.c_void_p), ("lddv", C.c_int64)]
 
 
+class Regulate(C.Structure):
+    """b2ctr_regulate_t"""
+    _fields_ = [("mode", C.c_int32), ("nfield", C.c_int32), ("dim", C.c_int32), ("dx_accumulate", C.c_int32),
+                ("batch", C.c_int64), ("x", C.c_void_p), ("ldx", C.c_int64), ("h", C.c_void_p), ("ldh", C.c_int64),
+                ("ax", C.c_void_p), ("ldax", C.c_int64), ("ah", C.c_void_p), ("ldah", C.c_int64),
+                ("g0", C.c_void_p), ("g1", C.c_void_p), ("inv_tau0", C.c_float), ("inv_tau1", C.c_float),
+                ("u", C.c_void_p), ("ldu", C.c_int64), ("ucol", C.c_int64),
+                ("y0", C.c_void_p), ("ldy0", C.c_int64), ("y0col", C.c_int64),
+                ("y1", C.c_void_p), ("ldy1", C.c_int64), ("y1col", C.c_int64),
+                ("dx", C.c_void_p), ("lddx", C.c_int64), ("dh", C.c_void_p), ("lddh", C.c_int64),
+                ("dax", C.c_void_p), ("lddax", C.c_int64), ("dah", C.c_void_p), ("lddah", C.c_int64),
+                ("dg0", C.c_void_p), ("dg1", C.c_void_p)]
+
+
 _vp, _i32, _i64, _f32, _sz, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t, C.c_uint64
 
 # name -> (restype, argtypes).  Must list every symbol of include/b2ctr.h (tests check this).
@@ -203,6 +217,9 @@ SIGNATURES = {
     "b2ctr_pnn_outer_fwd": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp, _i64, _i64, _i64, _vp]),
     "b2ctr_pnn_outer_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
     "b2ctr_pnn_outer_bwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i32, _i32, _vp, _vp, _i64, _vp, _i64, _vp, _sz, _vp]),
+    "b2ctr_regulate_fwd": (_i32, [C.POINTER(Regulate), _vp]),
+    "b2ctr_regulate_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
+    "b2ctr_regulate_bwd": (_i32, [C.POINTER(Regulate), _vp, _sz, _vp]),
     "b2ctr_ffm_product_fwd": (_i32, [C.POINTER(FfmField), _i32, _vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp]),
     "b2ctr_ffm_product_bwd": (_i32, [C.POINTER(FfmField), _i32, _vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp]),
     "b2ctr_din_att_input_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),

@@ -1744,6 +1744,229 @@ static inline int pn_dk_chunks(int nent, int64_t batch) {
   return (int)std::max<int64_t>(1, std::min(want, ceil_div(batch, 64)));
 }
 
+// ------------------------------------------------------------------------------------------------
+// EDCN's BridgeModule + RegulationModule (deepctr/layers/interaction.py:1556-1565, core.py:307-315), the math of
+// b2ctr_regulate_fwd / _bwd in include/b2ctr.h.  V = 4: every thread owns 4 consecutive columns of one field
+// (dim % 4 == 0, 16-byte aligned windows); V = 1 the scalar path.
+// * regulate_fwd_kernel: grid-stride over (sample, column group); the gates come from shared memory.
+// * regulate_bwd_kernel: CTA (batch chunk, column tile of whole fields); R row lanes of G column groups each
+//   (R * G <= 256).  A thread walks its chunk's rows in ascending order, writes dx / dh / dax / dah for its columns
+//   (one owner per element) and keeps sum_b v * dy_k in registers; the CTA then adds its row lanes and each field's
+//   columns in a fixed order into the per-(field, chunk) partial.  ordered_sum_kernel adds the chunks in order and
+//   regulate_dg_kernel applies the softmax Jacobian.  Bit-identical from run to run.
+// ------------------------------------------------------------------------------------------------
+constexpr int kRegMaxF = 1024;
+constexpr int kRegMaxE = 256;
+constexpr int kRegThreads = 256;
+
+// gates[f] = softmax_f(g[f] * it) by one warp; lanes stride over f and reduce with a fixed xor tree, so every CTA,
+// the backward and the final step form bit-identical gates
+__device__ __forceinline__ void reg_gates(const float* __restrict__ g, float it, int F, float* gates, int lane) {
+  float m = -INFINITY;
+  for (int f = lane; f < F; f += 32) m = fmaxf(m, g[f] * it);
+  for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  float s = 0.f;
+  for (int f = lane; f < F; f += 32) s += expf(g[f] * it - m);
+  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  for (int f = lane; f < F; f += 32) gates[f] = expf(g[f] * it - m) / s;
+}
+
+__device__ __forceinline__ void reg_stage_gates(const b2ctr_regulate_t& a, float* sg) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 0 && a.y0) reg_gates(a.g0, a.inv_tau0, a.nfield, sg, lane);
+  if (warp == 1 && a.y1) reg_gates(a.g1, a.inv_tau1, a.nfield, sg + kRegMaxF, lane);
+  __syncthreads();
+}
+
+template <int V>
+__device__ __forceinline__ void reg_ld(const float* p, float (&r)[V]) {
+  if constexpr (V == 4) {
+    const float4 t = *reinterpret_cast<const float4*>(p);
+    r[0] = t.x, r[1] = t.y, r[2] = t.z, r[3] = t.w;
+  } else {
+    r[0] = *p;
+  }
+}
+
+template <int V>
+__device__ __forceinline__ void reg_st(float* p, const float (&r)[V]) {
+  if constexpr (V == 4)
+    *reinterpret_cast<float4*>(p) = make_float4(r[0], r[1], r[2], r[3]);
+  else
+    *p = r[0];
+}
+
+// the operands of sample b at column c, and v
+template <int V, int kMode>
+__device__ __forceinline__ void reg_operands(const b2ctr_regulate_t& a, int64_t b, int c, float (&x)[V], float (&h)[V],
+                                             float (&ax)[V], float (&ah)[V], float (&v)[V]) {
+  reg_ld<V>(a.x + b * a.ldx + c, x);
+  if (kMode != B2CTR_REGULATE_COPY) reg_ld<V>(a.h + b * a.ldh + c, h);
+  if (kMode == B2CTR_REGULATE_ATTENTION) {
+    reg_ld<V>(a.ax + b * a.ldax + c, ax);
+    reg_ld<V>(a.ah + b * a.ldah + c, ah);
+  }
+#pragma unroll
+  for (int q = 0; q < V; ++q) {
+    if (kMode == B2CTR_REGULATE_COPY) v[q] = x[q];
+    else if (kMode == B2CTR_REGULATE_ADD) v[q] = x[q] + h[q];
+    else if (kMode == B2CTR_REGULATE_HADAMARD) v[q] = x[q] * h[q];
+    else v[q] = fmaf(ax[q], x[q], ah[q] * h[q]);
+  }
+}
+
+template <int V, int kMode>
+__global__ void __launch_bounds__(kRegThreads) regulate_fwd_kernel(const b2ctr_regulate_t a) {
+  __shared__ float sg[2 * kRegMaxF];
+  reg_stage_gates(a, sg);
+  const int E = a.dim, G = a.nfield * E / V;
+  const int64_t total = a.batch * G;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t b = i / G;
+    const int c = (int)(i - b * G) * V, f = c / E;
+    float x[V], h[V], ax[V], ah[V], v[V], y[V];
+    reg_operands<V, kMode>(a, b, c, x, h, ax, ah, v);
+    if (a.u) reg_st<V>(a.u + b * a.ldu + a.ucol + c, v);
+    if (a.y0) {
+      const float gt = sg[f];
+#pragma unroll
+      for (int q = 0; q < V; ++q) y[q] = v[q] * gt;
+      reg_st<V>(a.y0 + b * a.ldy0 + a.y0col + c, y);
+    }
+    if (a.y1) {
+      const float gt = sg[kRegMaxF + f];
+#pragma unroll
+      for (int q = 0; q < V; ++q) y[q] = v[q] * gt;
+      reg_st<V>(a.y1 + b * a.ldy1 + a.y1col + c, y);
+    }
+  }
+}
+
+template <int V, int kMode>
+__global__ void __launch_bounds__(kRegThreads, 4)
+    regulate_bwd_kernel(const b2ctr_regulate_t a, int W, int R, int nchunk, float* partial) {
+  __shared__ float sg[2 * kRegMaxF];
+  __shared__ float scol[2 * kRegThreads * V];
+  reg_stage_gates(a, sg);
+  const int F = a.nfield, E = a.dim, d = F * E, G = W / V;
+  const int r = threadIdx.x / G, j = threadIdx.x - r * G, c0 = blockIdx.y * W, c = c0 + j * V;
+  const bool active = r < R && c < d;
+  const int64_t per = (a.batch + nchunk - 1) / nchunk, lo = (int64_t)blockIdx.x * per, hi = min(a.batch, lo + per);
+  float acc0[V], acc1[V];
+#pragma unroll
+  for (int q = 0; q < V; ++q) acc0[q] = acc1[q] = 0.f;
+  if (active) {
+    const int f = c / E;
+    const float gt0 = a.y0 ? sg[f] : 0.f, gt1 = a.y1 ? sg[kRegMaxF + f] : 0.f;
+    for (int64_t b = lo + r; b < hi; b += R) {
+      float x[V], h[V], ax[V], ah[V], v[V], dv[V], t[V];
+      reg_operands<V, kMode>(a, b, c, x, h, ax, ah, v);
+      if (a.u) {
+        reg_ld<V>(a.u + b * a.ldu + a.ucol + c, dv);
+      } else {
+#pragma unroll
+        for (int q = 0; q < V; ++q) dv[q] = 0.f;
+      }
+      if (a.y0) {
+        reg_ld<V>(a.y0 + b * a.ldy0 + a.y0col + c, t);
+#pragma unroll
+        for (int q = 0; q < V; ++q) dv[q] = fmaf(gt0, t[q], dv[q]), acc0[q] = fmaf(v[q], t[q], acc0[q]);
+      }
+      if (a.y1) {
+        reg_ld<V>(a.y1 + b * a.ldy1 + a.y1col + c, t);
+#pragma unroll
+        for (int q = 0; q < V; ++q) dv[q] = fmaf(gt1, t[q], dv[q]), acc1[q] = fmaf(v[q], t[q], acc1[q]);
+      }
+      if (a.dx) {
+        float* p = a.dx + b * a.lddx + c;
+#pragma unroll
+        for (int q = 0; q < V; ++q)
+          t[q] = kMode == B2CTR_REGULATE_HADAMARD ? dv[q] * h[q] : kMode == B2CTR_REGULATE_ATTENTION ? dv[q] * ax[q] : dv[q];
+        if (a.dx_accumulate) {
+          float o[V];
+          reg_ld<V>(p, o);
+#pragma unroll
+          for (int q = 0; q < V; ++q) t[q] += o[q];
+        }
+        reg_st<V>(p, t);
+      }
+      if (kMode != B2CTR_REGULATE_COPY && a.dh) {
+#pragma unroll
+        for (int q = 0; q < V; ++q)
+          t[q] = kMode == B2CTR_REGULATE_HADAMARD ? dv[q] * x[q]
+                 : kMode == B2CTR_REGULATE_ATTENTION ? dv[q] * ah[q] : dv[q];
+        reg_st<V>(a.dh + b * a.lddh + c, t);
+      }
+      if (kMode == B2CTR_REGULATE_ATTENTION && a.dax) {
+#pragma unroll
+        for (int q = 0; q < V; ++q) t[q] = dv[q] * x[q];
+        reg_st<V>(a.dax + b * a.lddax + c, t);
+      }
+      if (kMode == B2CTR_REGULATE_ATTENTION && a.dah) {
+#pragma unroll
+        for (int q = 0; q < V; ++q) t[q] = dv[q] * h[q];
+        reg_st<V>(a.dah + b * a.lddah + c, t);
+      }
+    }
+  }
+  if (!partial) return;
+  float* s0 = scol;
+  float* s1 = scol + kRegThreads * V;
+  if (active) {
+#pragma unroll
+    for (int q = 0; q < V; ++q) s0[r * W + j * V + q] = acc0[q], s1[r * W + j * V + q] = acc1[q];
+  }
+  __syncthreads();
+  // the tile holds whole fields: c0 and min(W, d - c0) are multiples of E
+  const int nf = min(W, d - c0) / E;
+  for (int k = threadIdx.x; k < 2 * nf; k += blockDim.x) {
+    const int gate = k / nf, fl = k - gate * nf;
+    const float* s = gate ? s1 : s0;
+    float sum = 0.f;
+    for (int rr = 0; rr < R; ++rr)
+      for (int e = 0; e < E; ++e) sum += s[rr * W + fl * E + e];
+    partial[(int64_t)blockIdx.x * 2 * F + gate * F + c0 / E + fl] = sum;
+  }
+}
+
+// dg_k = inv_tau_k * gate_k * (s_k - <gate_k, s_k>), one warp per gate; s [2, F] the chunk-summed partials
+__global__ void regulate_dg_kernel(const b2ctr_regulate_t a, const float* __restrict__ s) {
+  __shared__ float sg[2 * kRegMaxF];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, F = a.nfield;
+  float* dg = warp ? a.dg1 : a.dg0;
+  if (!dg) return;
+  const float* g = warp ? a.g1 : a.g0;
+  const float it = warp ? a.inv_tau1 : a.inv_tau0;
+  float* gates = sg + warp * kRegMaxF;
+  const float* sk = s + warp * F;
+  reg_gates(g, it, F, gates, lane);
+  __syncwarp();
+  float dot = 0.f;
+  for (int f = lane; f < F; f += 32) dot = fmaf(gates[f], sk[f], dot);
+  for (int o = 16; o; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+  for (int f = lane; f < F; f += 32) dg[f] = it * gates[f] * (sk[f] - dot);
+}
+
+// backward geometry: column tiles of whole fields (W columns, G = W / V groups), R = 256 / G row lanes, and batch
+// chunks of at least 128 samples, about 8 CTAs per SM in all
+static inline int reg_tile(int E, int V) { return (kRegThreads * V / E) * E; }
+static inline int reg_chunks(int64_t batch) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(batch, 128), (int64_t)kNumSMs * 8));
+}
+
+template <class Op>
+cudaError_t reg_dispatch(int mode, bool vec, Op op) {
+  auto m = [&](auto v) -> cudaError_t {
+    switch (mode) {
+      case B2CTR_REGULATE_COPY: return op(v, std::integral_constant<int, B2CTR_REGULATE_COPY>());
+      case B2CTR_REGULATE_ADD: return op(v, std::integral_constant<int, B2CTR_REGULATE_ADD>());
+      case B2CTR_REGULATE_HADAMARD: return op(v, std::integral_constant<int, B2CTR_REGULATE_HADAMARD>());
+      default: return op(v, std::integral_constant<int, B2CTR_REGULATE_ATTENTION>());
+    }
+  };
+  return vec ? m(std::integral_constant<int, 4>()) : m(std::integral_constant<int, 1>());
+}
+
 }  // namespace b2ctr
 
 using namespace b2ctr;
@@ -2363,6 +2586,99 @@ b2ctr_status_t b2ctr_pnn_outer_bwd(const float* g, int64_t ldg, int64_t gcol0, c
     pnn_mat_dk_reduce_kernel<<<grid_for(count, 256, 8), 256, 0, ST>>>((const float*)workspace, P, dim, nchunk, dK,
                                                                       count);
     B2_CHECK_LAUNCH("b2ctr_pnn_outer_bwd(reduce)");
+  }
+  return B2CTR_OK;
+}
+
+static bool reg_aligned(const float* p, int64_t ld, int64_t col) {
+  return !p || (((uintptr_t)(p + col) & 15) == 0 && ld % 4 == 0);
+}
+
+// the checks the forward and the backward share: mode, limits, operands and the windows of u / y0 / y1
+static b2ctr_status_t reg_check(const b2ctr_regulate_t* a, const char* what) {
+  B2_REQUIRE(a, "%s: NULL descriptor", what);
+  B2_REQUIRE(a->mode >= B2CTR_REGULATE_COPY && a->mode <= B2CTR_REGULATE_ATTENTION, "%s: unknown mode %d", what,
+             a->mode);
+  B2_REQUIRE(a->nfield >= 1 && a->nfield <= kRegMaxF && a->dim >= 1 && a->dim <= kRegMaxE,
+             "%s: needs 1 <= field count <= %d and 1 <= embedding_size <= %d (got %d, %d)", what, kRegMaxF, kRegMaxE,
+             a->nfield, a->dim);
+  const int64_t d = (int64_t)a->nfield * a->dim;
+  B2_REQUIRE(a->batch >= 0, "%s: negative batch", what);
+  B2_REQUIRE(a->x && a->ldx >= d, "%s: x is NULL or its pitch is below %lld", what, (long long)d);
+  B2_REQUIRE(a->mode == B2CTR_REGULATE_COPY || (a->h && a->ldh >= d), "%s: h is NULL or its pitch is too small",
+             what);
+  B2_REQUIRE(a->mode != B2CTR_REGULATE_ATTENTION || (a->ax && a->ah && a->ldax >= d && a->ldah >= d),
+             "%s: attention weights NULL or their pitch too small", what);
+  B2_REQUIRE((!a->y0 || a->g0) && (!a->y1 || a->g1), "%s: a gated output without its gate weight", what);
+  B2_REQUIRE((!a->u || (a->ucol >= 0 && a->ldu >= a->ucol + d)) && (!a->y0 || (a->y0col >= 0 && a->ldy0 >= a->y0col + d)) &&
+                 (!a->y1 || (a->y1col >= 0 && a->ldy1 >= a->y1col + d)),
+             "%s: an output window does not fit its row", what);
+  return B2CTR_OK;
+}
+
+static bool reg_vec(const b2ctr_regulate_t* a) {
+  return a->dim % 4 == 0 && reg_aligned(a->x, a->ldx, 0) && reg_aligned(a->h, a->ldh, 0) &&
+         reg_aligned(a->ax, a->ldax, 0) && reg_aligned(a->ah, a->ldah, 0) && reg_aligned(a->u, a->ldu, a->ucol) &&
+         reg_aligned(a->y0, a->ldy0, a->y0col) && reg_aligned(a->y1, a->ldy1, a->y1col) &&
+         reg_aligned(a->dx, a->lddx, 0) && reg_aligned(a->dh, a->lddh, 0) && reg_aligned(a->dax, a->lddax, 0) &&
+         reg_aligned(a->dah, a->lddah, 0);
+}
+
+b2ctr_status_t b2ctr_regulate_fwd(const b2ctr_regulate_t* a, void* stream) {
+  const b2ctr_status_t st = reg_check(a, "regulate_fwd");
+  if (st != B2CTR_OK) return st;
+  B2_REQUIRE(a->u || a->y0 || a->y1, "regulate_fwd: no output");
+  if (a->batch == 0) return B2CTR_OK;
+  const int64_t d = (int64_t)a->nfield * a->dim;
+  const bool vec = reg_vec(a);
+  reg_dispatch(a->mode, vec, [&](auto v, auto m) {
+    constexpr int V = decltype(v)::value, kMode = decltype(m)::value;
+    regulate_fwd_kernel<V, kMode><<<grid_for(a->batch * d / V, kRegThreads, 8), kRegThreads, 0, ST>>>(*a);
+    return cudaSuccess;
+  });
+  B2_CHECK_LAUNCH("b2ctr_regulate_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_regulate_bwd_workspace_bytes(int32_t nfield, int32_t dim, int64_t batch) {
+  if (nfield < 1 || dim < 1 || batch <= 0) return 0;
+  return (size_t)(reg_chunks(batch) + 1) * 2 * (size_t)nfield * sizeof(float);
+}
+
+b2ctr_status_t b2ctr_regulate_bwd(const b2ctr_regulate_t* a, void* workspace, size_t workspace_bytes, void* stream) {
+  const b2ctr_status_t st = reg_check(a, "regulate_bwd");
+  if (st != B2CTR_OK) return st;
+  const bool want_dg = a->dg0 || a->dg1;
+  B2_REQUIRE(a->dx || a->dh || a->dax || a->dah || want_dg, "regulate_bwd: nothing to compute");
+  B2_REQUIRE((!a->dg0 || a->y0) && (!a->dg1 || a->y1), "regulate_bwd: a gate gradient without its incoming gradient");
+  const int64_t d = (int64_t)a->nfield * a->dim;
+  B2_REQUIRE((!a->dx || a->lddx >= d) && (!a->dh || a->lddh >= d) && (!a->dax || a->lddax >= d) &&
+                 (!a->dah || a->lddah >= d),
+             "regulate_bwd: a gradient pitch is below %lld", (long long)d);
+  if (a->batch == 0) return B2CTR_OK;
+  const size_t need = want_dg ? b2ctr_regulate_bwd_workspace_bytes(a->nfield, a->dim, a->batch) : 0;
+  if (want_dg && (!workspace || workspace_bytes < need)) {
+    set_error("regulate_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  const bool vec = reg_vec(a);
+  const int V = vec ? 4 : 1, W = reg_tile(a->dim, V), R = kRegThreads / (W / V), nchunk = reg_chunks(a->batch);
+  const int ntile = (int)ceil_div(d, W);
+  float* partial = want_dg ? (float*)workspace : nullptr;
+  const b2ctr_regulate_t k = *a;
+  reg_dispatch(a->mode, vec, [&](auto v, auto m) {
+    constexpr int VV = decltype(v)::value, kMode = decltype(m)::value;
+    regulate_bwd_kernel<VV, kMode><<<dim3(nchunk, ntile), kRegThreads, 0, ST>>>(k, W, R, nchunk, partial);
+    return cudaSuccess;
+  });
+  B2_CHECK_LAUNCH("b2ctr_regulate_bwd");
+  if (want_dg) {
+    float* sums = partial + (int64_t)nchunk * 2 * a->nfield;
+    ordered_sum_kernel<<<grid_for(2 * a->nfield, 256, 8), 256, 0, ST>>>(partial, 2 * a->nfield, nchunk,
+                                                                         2 * a->nfield, sums);
+    B2_CHECK_LAUNCH("b2ctr_regulate_bwd(reduce)");
+    regulate_dg_kernel<<<1, 64, 0, ST>>>(k, sums);
+    B2_CHECK_LAUNCH("b2ctr_regulate_bwd(gates)");
   }
   return B2CTR_OK;
 }

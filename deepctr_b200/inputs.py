@@ -366,6 +366,8 @@ class EmbeddingPlanner(object):
         self.lin_ld = max(1, (self.lin_width + 3) // 4 * 4)
         self.fast = self._fast_eligible()
         self.dnn_places = _plan_dnn_input(model, consumers, out_ids)
+        # EDCN's RegulationModule pairs and the bridges in front of them: one b2ctr_regulate launch each
+        self.regulate_plan = _plan_regulate(model, consumers, out_ids)
         # IFM / DIFM scale the linear lookups by per-sample field weights before Linear sums them: their rows are
         # needed, so they are never fused into the gather's row-sum (lin_hint)
         from .layers.utils import RefineWeight
@@ -870,6 +872,33 @@ class EmbeddingPlanner(object):
         P = f * (f - 1) // 2
         return ops._window(base, self.main_width + rel, P, (b, P))
 
+    def regulated(self, layer, x):
+        """RegulationModule ``layer`` on ``x``: when the planner pairs it with a second module reading the same tensor,
+        one launch writes both gated outputs; the partner's becomes that node's result.  Else None."""
+        from . import ops
+        p = self.regulate_plan.pairs.get(id(layer))
+        if p is None:
+            return None
+        partner, node = p
+        _, (y0, y1) = ops.regulate("copy", x, gates=[(layer.g, layer.tau), (partner.g, partner.tau)], want_u=False)
+        self.results[id(node)] = y1
+        return y0
+
+    def bridged(self, layer, mode, operands):
+        """BridgeModule ``layer`` whose output reaches only Reshape -> two RegulationModules: one launch writes the two
+        gated outputs as those modules' results, the bridge output and its reshape are never written (VIRTUAL).
+        Else None."""
+        from . import ops
+        plan = self.regulate_plan.bridges.get(id(layer))
+        if plan is None:
+            return None
+        reshape, regs = plan
+        _, ys = ops.regulate(mode, *operands, gates=[(l.g, l.tau) for l, _ in regs], want_u=False)
+        self.results[id(reshape)] = VIRTUAL
+        for (_, node), y in zip(regs, ys):
+            self.results[id(node)] = y
+        return VIRTUAL
+
     def append_dense(self, emb_flat, dense_flat):
         """combined_dnn_input: place the dense features behind the embeddings (and PNN's placed products) in the
         main buffer so the DNN input is a zero-copy window.  Returns the window or None."""
@@ -1124,6 +1153,59 @@ def _plan_dnn_input(model, consumers, out_ids):
         for k, l in enumerate(layers):
             places[id(l)] = (pl, k)
     return places
+
+
+class RegulatePlan(object):
+    """EDCN's information sharing (deepctr/models/edcn.py:66-85) with fewer passes over [B, F*E]:
+
+    * ``pairs`` {id(RegulationModule): (partner module, partner node)}: two RegulationModules reading one tensor (the
+      embeddings' concat_func, a window of the gather buffer read in place, or the Reshape of a 'concatenation'
+      bridge's Dense) are one 'copy' launch with both gates;
+    * ``bridges`` {id(BridgeModule): (Reshape node, [(module, node)] * 2)}: a non-concatenation BridgeModule whose
+      output reaches only Reshape([F, E]), which feeds only two RegulationModules, is one launch in the bridge's
+      mode that writes the two gated outputs; bridge_out and its reshape are never written.
+
+    Decided once from the model's graph; anything else runs layer by layer on the same kernel."""
+
+    def __init__(self, pairs, bridges):
+        self.pairs, self.bridges = pairs, bridges
+
+
+def _plan_regulate(model, consumers, out_ids):
+    from .layers.core import RegulationModule
+    from .layers.interaction import BridgeModule
+    calls = defaultdict(int)
+    for node in model._order:
+        calls[id(node.layer)] += 1
+
+    def regulators(t):
+        """The two RegulationModule nodes that are all of ``t``'s consumers, or None."""
+        cs = consumers[id(t)]
+        if id(t) in out_ids or len(cs) != 2 or len(t.shape) != 3 or cs[0].layer is cs[1].layer:
+            return None
+        if all(isinstance(c.layer, RegulationModule) and calls[id(c.layer)] == 1 for c in cs):
+            return cs
+        return None
+
+    pairs, bridges, claimed = {}, {}, set()
+    for node in model._order:
+        layer = node.layer
+        if not isinstance(layer, BridgeModule) or layer.bridge_type == "concatenation" or calls[id(layer)] != 1:
+            continue
+        out = node.outputs[0]
+        cs = consumers[id(out)]
+        if id(out) in out_ids or len(cs) != 1 or not isinstance(cs[0].layer, E.Reshape):
+            continue
+        regs = regulators(cs[0].outputs[0])
+        if regs is not None:
+            bridges[id(layer)] = (cs[0], [(c.layer, c) for c in regs])
+            claimed.add(id(cs[0].outputs[0]))
+    for node in model._order:
+        for t in node.outputs:
+            regs = regulators(t) if id(t) not in claimed else None
+            if regs is not None:
+                pairs[id(regs[0].layer)] = (regs[1].layer, regs[1])
+    return RegulatePlan(pairs, bridges)
 
 
 class FieldAwarePlan(object):

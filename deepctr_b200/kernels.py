@@ -932,6 +932,87 @@ def pnn_outer_bwd(g, ldg, gcol0, x, ldx, nfield, dim, Kw, batch, want_dx=True, w
     return dx, dK
 
 
+REGULATE_MODES = {"copy": 0, "add": 1, "hadamard": 2, "attention": 3}   # b2ctr.h B2CTR_REGULATE_*
+# limits of b2ctr_regulate_fwd / _bwd (include/b2ctr.h)
+REGULATE_MAX_FIELDS, REGULATE_MAX_DIM = 1024, 256
+
+
+def _2d(t):
+    return (t.data_ptr(), t.stride(0)) if t is not None else (None, 0)
+
+
+def _regulate_desc(mode, nfield, dim, batch, x, h, ax, ah, gates):
+    """The operands of b2ctr_regulate_t: x / h / ax / ah 2-D [B, >= nfield*dim] views read in place (row pitch =
+    stride(0)), ``gates`` [(g [nfield], inv_tau) or None] * 2."""
+    _require_cuda(x, h, ax, ah)
+    a = L.Regulate()
+    a.mode, a.nfield, a.dim, a.batch = REGULATE_MODES[mode], nfield, dim, batch
+    a.x, a.ldx = _2d(x)
+    a.h, a.ldh = _2d(h)
+    a.ax, a.ldax = _2d(ax)
+    a.ah, a.ldah = _2d(ah)
+    (g0, g1) = (list(gates) + [None, None])[:2]
+    if g0 is not None:
+        a.g0, a.inv_tau0 = g0[0].data_ptr(), float(g0[1])
+    if g1 is not None:
+        a.g1, a.inv_tau1 = g1[0].data_ptr(), float(g1[1])
+    return a
+
+
+def _window_of(a, name, out):
+    """out = (tensor [B, ld], col0) or None -> the (ptr, ld, col) fields ``name`` of the descriptor."""
+    if out is None:
+        return
+    t, col = out
+    _require_cuda(t)
+    setattr(a, name, t.data_ptr())
+    setattr(a, "ld" + name, t.stride(0))
+    setattr(a, name + "col", col)
+
+
+def regulate_fwd(mode, nfield, dim, batch, x, h=None, ax=None, ah=None, gates=(), u=None, y0=None, y1=None):
+    """EDCN's bridge + gates in one pass (b2ctr_regulate_fwd): ``u`` / ``y0`` / ``y1`` are (buffer [B, ld], col0)
+    windows to write v, v * gate0, v * gate1 into (None: not written)."""
+    a = _regulate_desc(mode, nfield, dim, batch, x, h, ax, ah, gates)
+    _window_of(a, "u", u)
+    _window_of(a, "y0", y0)
+    _window_of(a, "y1", y1)
+    L.check(L.lib().b2ctr_regulate_fwd(C.byref(a), stream()), "regulate_fwd")
+
+
+def regulate_bwd(mode, nfield, dim, batch, x, h=None, ax=None, ah=None, gates=(), du=None, dy0=None, dy1=None,
+                 want_dx=True, dx=None, dx_accumulate=False, want_dh=False, want_dax=False, want_dah=False,
+                 want_dg=(False, False)):
+    """-> (dx, dh, dax, dah, dg0, dg1) from the incoming gradients ``du`` / ``dy0`` / ``dy1`` ((buffer, col0) windows
+    or None).  ``dx``: a 2-D view to write (or, with ``dx_accumulate``, add) x's gradient into; default a new
+    [B, nfield*dim] tensor when ``want_dx``.  dh / dax / dah are new
+    [B, nfield*dim] tensors when asked for, dg_k new [nfield] tensors."""
+    a = _regulate_desc(mode, nfield, dim, batch, x, h, ax, ah, gates)
+    _window_of(a, "u", du)
+    _window_of(a, "y0", dy0)
+    _window_of(a, "y1", dy1)
+    dev, d = x.device, nfield * dim
+    if not want_dx:
+        dx = None
+    elif dx is None:
+        dx = torch.empty((batch, d), dtype=torch.float32, device=dev)
+    _require_cuda(dx)
+    dh, dax, dah = (torch.empty((batch, d), dtype=torch.float32, device=dev) if w else None
+                    for w in (want_dh, want_dax, want_dah))
+    dg = [torch.empty((nfield,), dtype=torch.float32, device=dev) if w else None for w in want_dg]
+    a.dx, a.lddx = _2d(dx)
+    a.dx_accumulate = int(bool(dx_accumulate))
+    a.dh, a.lddh = _2d(dh)
+    a.dax, a.lddax = _2d(dax)
+    a.dah, a.lddah = _2d(dah)
+    a.dg0 = dg[0].data_ptr() if dg[0] is not None else None
+    a.dg1 = dg[1].data_ptr() if dg[1] is not None else None
+    nbytes = L.lib().b2ctr_regulate_bwd_workspace_bytes(nfield, dim, batch) if any(w for w in want_dg) else 0
+    ws = workspace(nbytes, dev)
+    L.check(L.lib().b2ctr_regulate_bwd(C.byref(a), ptr(ws), nbytes, stream()), "regulate_bwd")
+    return dx, dh, dax, dah, dg[0], dg[1]
+
+
 def din_att_input_fwd(q, ldq, keys, ldk, batch, T, E):
     out = torch.empty((batch, T, 4 * E), dtype=torch.float32, device=q.device)
     _lib_call("din_att_input_fwd", ptr(q), ldq, ptr(keys), ldk, ptr(out), batch, T, E, stream())
@@ -1169,5 +1250,5 @@ for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filte
     globals()[_n] = _timed(globals()[_n])
 
 
-for _n in ("mha_fwd", "mha_bwd", "layernorm_fwd", "layernorm_bwd"):
+for _n in ("mha_fwd", "mha_bwd", "layernorm_fwd", "layernorm_bwd", "regulate_fwd", "regulate_bwd"):
     globals()[_n] = _timed(globals()[_n])

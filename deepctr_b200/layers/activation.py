@@ -11,15 +11,19 @@ def fusable_activation(name):
 
 
 class Activation(Layer):
-    """tf.keras.layers.Activation for the string activations the reference uses."""
+    """tf.keras.layers.Activation for the string activations the reference uses.  'softmax' (the output activation of
+    BridgeModule's attention DNNs) normalises the last axis of a 2-D tensor on b2ctr_softmax_rows; it cannot ride in
+    a GEMM epilogue."""
 
     def __init__(self, activation, **kwargs):
         Layer.__init__(self, **kwargs)
-        if not fusable_activation(activation):
+        if not fusable_activation(activation) and activation != "softmax":
             raise ValueError("unsupported activation %r (relu, sigmoid, tanh, linear, dice)" % (activation,))
         self.activation = activation
 
     def call(self, inputs, **kwargs):
+        if self.activation == "softmax":
+            return ops.softmax(inputs)
         return ops.activation(inputs, self.activation)
 
     def get_config(self):

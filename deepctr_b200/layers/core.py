@@ -1,9 +1,9 @@
 """Host mirror of deepctr/layers/core.py: DNN (:123-223), PredictionLayer (:226-267),
-LocalActivationUnit (:28-120)."""
+LocalActivationUnit (:28-120), RegulationModule (:270-321)."""
 from .. import _lib as L
 from .. import engine as E
 from .. import ops
-from ..engine import Layer, Zeros, glorot_normal, l2
+from ..engine import Layer, Ones, Zeros, glorot_normal, l2
 from .activation import activation_layer, fusable_activation
 
 
@@ -184,3 +184,41 @@ class LocalActivationUnit(Layer):
                   'seed': self.seed}
         base = Layer.get_config(self)
         return dict(list(base.items()) + list(config.items()))
+
+
+class RegulationModule(Layer):
+    """EDCN's field-wise gate, deepctr/layers/core.py:270-321: [B, F, E] -> [B, F*E],
+    y = x * softmax_f(g * (1 / tau)) with the weight g [1, F, 1].  As in the reference, ``self.tau`` holds 1 / tau and
+    ``get_config`` returns it.  On its own the layer is one b2ctr_regulate launch in 'copy' mode; in EDCN the planner
+    (inputs.RegulatePlan) serves two modules reading one tensor, and the bridge in front of them, with one launch."""
+
+    def __init__(self, tau=1.0, **kwargs):
+        if tau == 0:
+            raise ValueError("RegulationModule tau can not be zero.")
+        self.tau = 1.0 / tau
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        self.field_size = int(input_shape[1])
+        self.embedding_size = int(input_shape[2])
+        self.g = self.add_weight(shape=(1, self.field_size, 1), initializer=Ones(), name=self.name + '_field_weight')
+        self.built = True
+
+    def call(self, inputs, **kwargs):
+        if inputs.data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs.data.dim()))
+        planner = getattr(self, "_planner", None)
+        served = planner.regulated(self, inputs) if planner is not None else None
+        if served is not None:
+            return served
+        _, (y,) = ops.regulate("copy", inputs, gates=[(self.g, self.tau)], want_u=False)
+        return y
+
+    def compute_output_shape(self, input_shape):
+        return (None, self.field_size * self.embedding_size)
+
+    def get_config(self):
+        config = {'tau': self.tau}
+        base = Layer.get_config(self)
+        base.update(config)
+        return base

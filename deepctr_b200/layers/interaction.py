@@ -1,7 +1,7 @@
 """Host mirror of deepctr/layers/interaction.py for the operators on the hot path:
 AFMLayer (:39-160), BiInteractionPooling (:163-206), FM (:563-607), CrossNet (:344-435), CIN (:209-341),
 InteractingLayer (:697-790), SENETLayer (:1067-1139), BilinearInteraction (:1142-1221), FwFMLayer (:1350-1425),
-FEFMLayer (:1428-1499), InnerProductLayer (:610-695), OutterProductLayer (:793-931).
+FEFMLayer (:1428-1499), InnerProductLayer (:610-695), OutterProductLayer (:793-931), BridgeModule (:1502-1570).
 Same constructor arguments, weight names, shape checks and error messages as the reference."""
 import itertools
 
@@ -645,3 +645,71 @@ class OutterProductLayer(Layer):
         base_config = Layer.get_config(self)
         base_config.update(config)
         return base_config
+
+
+BRIDGE_TYPES = ("pointwise_addition", "hadamard_product", "concatenation", "attention_pooling")
+# b2ctr_regulate mode of each bridge type it serves; 'concatenation' is Concatenate + Dense on the GEMM
+_BRIDGE_MODES = {"pointwise_addition": "add", "hadamard_product": "hadamard", "attention_pooling": "attention"}
+
+
+class BridgeModule(Layer):
+    """EDCN's bridge between the cross and deep stacks, deepctr/layers/interaction.py:1502-1570.  Called on
+    [x, h], two [B, d] tensors: x + h ('pointwise_addition'), x * h ('hadamard_product'), Dense(d, activation)
+    of concat([x, h]) ('concatenation') or a_x * x + a_h * h with a_x = DNN([d, d], activation,
+    output_activation='softmax')(x) and a_h likewise of h ('attention_pooling').  The nested Dense / DNNs are created
+    in build() and take Keras' automatic names.  Except for 'concatenation' the bridge is one b2ctr_regulate launch;
+    when its output only feeds two RegulationModules through a Reshape, the planner (inputs.RegulatePlan) makes that
+    launch write the two gated outputs instead, and the bridge output itself is never written.
+
+    Deviation: an unknown ``bridge_type`` raises ValueError here; the reference's call returns None and fails later
+    inside TensorFlow."""
+
+    def __init__(self, bridge_type='hadamard_product', activation='relu', **kwargs):
+        if bridge_type not in BRIDGE_TYPES:
+            raise ValueError("BridgeModule bridge_type %r is not one of %s" % (bridge_type, ", ".join(BRIDGE_TYPES)))
+        self.bridge_type = bridge_type
+        self.activation = activation
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        if not isinstance(input_shape, list) or len(input_shape) < 2:
+            raise ValueError('A `BridgeModule` layer should be called '
+                             'on a list of 2 inputs')
+        self.dnn_dim = int(input_shape[0][-1])
+        from .core import DNN
+        if self.bridge_type == "concatenation":
+            self.dense = self._track(E.Dense(self.dnn_dim, self.activation, name=self.name + "/dense"))
+            self.dense._maybe_build((None, 2 * self.dnn_dim))
+        elif self.bridge_type == "attention_pooling":
+            self.dense_x = self._track(DNN([self.dnn_dim, self.dnn_dim], self.activation, output_activation='softmax',
+                                           name=self.name + "/dense_x"))
+            self.dense_h = self._track(DNN([self.dnn_dim, self.dnn_dim], self.activation, output_activation='softmax',
+                                           name=self.name + "/dense_h"))
+            self.dense_x._maybe_build(tuple(input_shape[0]))
+            self.dense_h._maybe_build(tuple(input_shape[1]))
+        self.built = True
+
+    def call(self, inputs, training=None, **kwargs):
+        x, h = inputs
+        if self.bridge_type == "concatenation":
+            return self.dense.call(ops.concat([x, h], axis=-1))
+        ax = ah = None
+        if self.bridge_type == "attention_pooling":
+            ax = self.dense_x.call(x, training=training)
+            ah = self.dense_h.call(h, training=training)
+        mode = _BRIDGE_MODES[self.bridge_type]
+        planner = getattr(self, "_planner", None)
+        served = planner.bridged(self, mode, (x, h, ax, ah)) if planner is not None else None
+        if served is not None:
+            return served
+        u, _ = ops.regulate(mode, x, h, ax, ah)
+        return u
+
+    def compute_output_shape(self, input_shape):
+        return (None, int(input_shape[0][-1]))
+
+    def get_config(self):
+        base = Layer.get_config(self).copy()
+        config = {'bridge_type': self.bridge_type, 'activation': self.activation}
+        config.update(base)
+        return config

@@ -12,6 +12,7 @@ from .pnn import PNN
 from .ifm import IFM
 from .difm import DIFM
 from .onn import ONN
+from .edcn import EDCN
 
 __all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM", "PNN",
-           "IFM", "DIFM", "ONN"]
+           "IFM", "DIFM", "ONN", "EDCN"]

@@ -876,6 +876,77 @@ def cross_matrix(x0, xl, w, bias):
     return res
 
 
+def _row_fields(d):
+    """(fields, dim) splitting a row of d values for b2ctr_regulate when no gate gives it fields: the largest dim
+    within the kernel's limits, a multiple of 4 where one divides d (its 16-byte path).  Without gates the split
+    does not change the result."""
+    fits = [e for e in range(min(d, K.REGULATE_MAX_DIM), 0, -1) if d % e == 0 and d // e <= K.REGULATE_MAX_FIELDS]
+    if not fits:
+        raise ValueError("a bridge over %d columns exceeds the regulate kernel's %d x %d limit"
+                         % (d, K.REGULATE_MAX_FIELDS, K.REGULATE_MAX_DIM))
+    e = next((e for e in fits if e % 4 == 0), fits[0])
+    return d // e, e
+
+
+def regulate(mode, x, h=None, ax=None, ah=None, gates=(), want_u=True):
+    """EDCN's BridgeModule and RegulationModules in one launch (b2ctr_regulate_fwd): v = x ('copy'), x + h ('add'),
+    x * h ('hadamard') or ax * x + ah * h ('attention') over [B, d] rows read in place, then u = v (when ``want_u``)
+    and y_k = v * softmax_f(g_k * inv_tau_k) per field for each gate (g_k the RegulationModule weight [1, F, 1],
+    inv_tau_k its stored 1 / tau).  Returns (u or None, [y_k]), each [B, d].  The backward recomputes v, writes dx
+    straight into the gather buffer's gradient when x is a window of it, and reduces the gate gradients in a fixed
+    order (b2ctr_regulate_bwd)."""
+    b = x.shape[0]
+    ops_ = [x, h, ax, ah]
+    t2 = [_rows2d(v)[0] if v is not None else None for v in ops_]
+    d = t2[0].shape[1]
+    for v in t2[1:]:
+        if v is not None and v.shape[1] != d:
+            raise ValueError("regulate: operands of %d and %d columns" % (d, v.shape[1]))
+    if gates:
+        f = int(gates[0][0].shape[1])
+        if d % f:
+            raise ValueError("regulate: %d columns are not %d fields" % (d, f))
+        e = d // f
+    else:
+        f, e = _row_fields(d)
+    if not (1 <= f <= K.REGULATE_MAX_FIELDS and 1 <= e <= K.REGULATE_MAX_DIM):
+        raise ValueError("RegulationModule supports 1 to %d fields and embedding_size 1 to %d (got %d fields, "
+                         "embedding_size %d)" % (K.REGULATE_MAX_FIELDS, K.REGULATE_MAX_DIM, f, e))
+    kg = [(_wdata(g).reshape(-1), it) for g, it in gates]
+    outs = [_empty((b, d), t2[0]) for _ in range(int(bool(want_u)) + len(gates))]
+    u = outs[0] if want_u else None
+    ys = outs[1:] if want_u else outs
+    K.regulate_fwd(mode, f, e, b, t2[0], t2[1], t2[2], t2[3], kg, u=(u, 0) if u is not None else None,
+                   y0=(ys[0], 0) if len(ys) > 0 else None, y1=(ys[1], 0) if len(ys) > 1 else None)
+    res = [E.Var(o) for o in outs]
+
+    def bwd(grads):
+        gs = [_pair_grad([g], b) if g is not None else None for g in grads]
+        gu = gs[0] if want_u else None
+        gy = (gs[1:] if want_u else gs) + [None, None]
+        want_dg = [gy[k] is not None and gates[k][0].requires_grad for k in range(len(gates))] + [False, False]
+        want = [v is not None and v.requires_grad for v in ops_]
+        if not (any(want) or any(want_dg)):
+            return
+        dxw, acc = _grad_window(x, d) if x.requires_grad else (None, False)
+        win = lambda g: (g, 0) if g is not None else None   # noqa: E731
+        dx, dh, dax, dah, dg0, dg1 = K.regulate_bwd(
+            mode, f, e, b, t2[0], t2[1], t2[2], t2[3], kg, du=win(gu), dy0=win(gy[0]), dy1=win(gy[1]),
+            want_dx=want[0], dx=dxw, dx_accumulate=acc, want_dh=want[1], want_dax=want[2], want_dah=want[3],
+            want_dg=want_dg[:2])
+        if x.requires_grad and dxw is None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        for v, g in ((h, dh), (ax, dax), (ah, dah)):
+            if g is not None:
+                E.add_grad(v, g.reshape(v.data.shape))
+        for (w, _), g in zip(gates, (dg0, dg1)):
+            if g is not None:
+                E.add_grad(w, g.reshape(w.shape))
+
+    E.record(res, [v for v in ops_ if v is not None] + [g for g, _ in gates], bwd)
+    return (res[0] if want_u else None), (res[1:] if want_u else res)
+
+
 CIN_CHUNK_BYTES = 24 << 20      # outer-product chunk kept well inside the 50 MB L2
 
 

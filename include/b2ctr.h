@@ -671,6 +671,49 @@ B2CTR_API b2ctr_status_t b2ctr_pnn_outer_bwd(const float* g, int64_t ldg, int64_
                                             float* dK, int64_t batch, void* workspace, size_t workspace_bytes,
                                             void* stream);
 
+/* EDCN's BridgeModule (deepctr/layers/interaction.py:1502-1570) and RegulationModule (deepctr/layers/core.py:270-321)
+ * in one pass over [B, nfield*dim].  Per element (b, f, e), from operands read in place through their own pitch:
+ *   B2CTR_REGULATE_COPY       v = x                       (a RegulationModule on its own)
+ *   B2CTR_REGULATE_ADD        v = x + h                   (bridge_type 'pointwise_addition')
+ *   B2CTR_REGULATE_HADAMARD   v = x * h                   ('hadamard_product')
+ *   B2CTR_REGULATE_ATTENTION  v = ax * x + ah * h         ('attention_pooling', ax / ah the two softmax DNNs)
+ * and writes, each into the column window [col, col + nfield*dim) of a wider buffer and only where its pointer is
+ * set: the bridge output u = v, and the gated outputs y_k = v * gate_k[f], gate_k = softmax_f(g_k * inv_tau_k)
+ * (g_k the module's [1, nfield, 1] weight, inv_tau_k the reference's stored 1 / tau).  Every CTA forms the gates in
+ * shared memory.  16-byte loads and stores when dim % 4 == 0 and every pointer and pitch allows, else a scalar path.
+ * Backward (the same descriptor; u / y0 / y1 now address the incoming gradients du / dy0 / dy1, NULL = zero):
+ * v is recomputed from the operands, dv = du + sum_k gate_k * dy_k, then by mode dx = dv (COPY, ADD) or dv * h
+ * (HADAMARD) or dv * ax (ATTENTION), dh = dv (ADD) or dv * x (HADAMARD) or dv * ah, dax = dv * x, dah = dv * h.
+ * dx is added to (dx_accumulate) or overwritten; dh / dax / dah are overwritten; any of them may be NULL.  dg_k
+ * [nfield] = inv_tau_k * gate_k * (s_k - <gate_k, s_k>) with s_k[f] = sum_{b,e} v * dy_k: per-(field, batch
+ * chunk) partials in the workspace, summed in chunk order, then the softmax Jacobian on the device.  Every element
+ * has one owner, no float atomics: bit-identical from run to run.
+ * Limits: 1 <= nfield <= 1024 (both gates in shared memory), 1 <= dim <= 256 (a field inside one backward column
+ * tile), hence nfield*dim <= 262144; anything else is INVALID_ARG. */
+enum { B2CTR_REGULATE_COPY = 0, B2CTR_REGULATE_ADD = 1, B2CTR_REGULATE_HADAMARD = 2, B2CTR_REGULATE_ATTENTION = 3 };
+typedef struct b2ctr_regulate {
+  int32_t mode, nfield, dim, dx_accumulate;
+  int64_t batch;
+  const float* x; int64_t ldx;
+  const float* h; int64_t ldh;                   /* ADD, HADAMARD, ATTENTION */
+  const float* ax; int64_t ldax;                 /* ATTENTION */
+  const float* ah; int64_t ldah;                 /* ATTENTION */
+  const float* g0; const float* g1;              /* [nfield] gate logits (a gate whose y is NULL is unused) */
+  float inv_tau0, inv_tau1;
+  float* u; int64_t ldu, ucol;                   /* forward outputs / backward incoming gradients */
+  float* y0; int64_t ldy0, y0col;
+  float* y1; int64_t ldy1, y1col;
+  float* dx; int64_t lddx;                       /* backward outputs */
+  float* dh; int64_t lddh;
+  float* dax; int64_t lddax;
+  float* dah; int64_t lddah;
+  float* dg0; float* dg1;                        /* [nfield] */
+} b2ctr_regulate_t;
+B2CTR_API b2ctr_status_t b2ctr_regulate_fwd(const b2ctr_regulate_t* a, void* stream);
+B2CTR_API size_t b2ctr_regulate_bwd_workspace_bytes(int32_t nfield, int32_t dim, int64_t batch);
+B2CTR_API b2ctr_status_t b2ctr_regulate_bwd(const b2ctr_regulate_t* a, void* workspace, size_t workspace_bytes,
+                                           void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* 6. Sequence operators (DIN, pooling, Dice / BatchNormalization, dropout)                     */
 /* ------------------------------------------------------------------------------------------ */
