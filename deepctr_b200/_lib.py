@@ -110,6 +110,27 @@ class Regulate(C.Structure):
                 ("dg0", C.c_void_p), ("dg1", C.c_void_p)]
 
 
+
+CONV_STACK_MAX_STAGES = 8          # b2ctr.h B2CTR_CONV_STACK_MAX_STAGES
+CONV_STAGE_CONV, CONV_STAGE_KMAX = 0, 1
+
+
+class ConvStage(C.Structure):
+    """b2ctr_conv_stage_t"""
+    _fields_ = [("kind", C.c_int32), ("width", C.c_int32), ("filters", C.c_int32), ("act", C.c_int32),
+                ("k", C.c_int32), ("reserved", C.c_int32), ("kernel", C.c_void_p), ("bias", C.c_void_p),
+                ("dkernel", C.c_void_p), ("dbias", C.c_void_p)]
+
+
+class ConvStack(C.Structure):
+    """b2ctr_conv_stack_t"""
+    _fields_ = [("struct_size", C.c_int32), ("nstage", C.c_int32), ("rows", C.c_int32), ("dim", C.c_int32),
+                ("channels", C.c_int32), ("dx_accumulate", C.c_int32), ("batch", C.c_int64),
+                ("x", C.c_void_p), ("ldx", C.c_int64), ("xcol", C.c_int64),
+                ("out", C.c_void_p), ("ldout", C.c_int64), ("outcol", C.c_int64),
+                ("dx", C.c_void_p), ("lddx", C.c_int64), ("dxcol", C.c_int64),
+                ("stage", ConvStage * CONV_STACK_MAX_STAGES)]
+
 _vp, _i32, _i64, _f32, _sz, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t, C.c_uint64
 
 # name -> (restype, argtypes).  Must list every symbol of include/b2ctr.h (tests check this).
@@ -220,6 +241,9 @@ SIGNATURES = {
     "b2ctr_regulate_fwd": (_i32, [C.POINTER(Regulate), _vp]),
     "b2ctr_regulate_bwd_workspace_bytes": (_sz, [_i32, _i32, _i64]),
     "b2ctr_regulate_bwd": (_i32, [C.POINTER(Regulate), _vp, _sz, _vp]),
+    "b2ctr_conv_stack_fwd": (_i32, [C.POINTER(ConvStack), _vp]),
+    "b2ctr_conv_stack_bwd_workspace_bytes": (_sz, [C.POINTER(ConvStack)]),
+    "b2ctr_conv_stack_bwd": (_i32, [C.POINTER(ConvStack), _vp, _sz, _vp]),
     "b2ctr_ffm_product_fwd": (_i32, [C.POINTER(FfmField), _i32, _vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp]),
     "b2ctr_ffm_product_bwd": (_i32, [C.POINTER(FfmField), _i32, _vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp]),
     "b2ctr_din_att_input_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),

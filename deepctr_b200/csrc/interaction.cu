@@ -1967,6 +1967,231 @@ cudaError_t reg_dispatch(int mode, bool vec, Op op) {
   return vec ? m(std::integral_constant<int, 4>()) : m(std::integral_constant<int, 1>());
 }
 
+// ------------------------------------------------------------------------------------------------
+// CCPM's convolution stack (b2ctr_conv_stack_fwd / _bwd in include/b2ctr.h).  A CTA serves kConvCols = 32 columns
+// (sample, e); each column gets kConvG threads, one per channel slot (G = the most channels of any map), so a thread
+// (g, col) owns the channels c = g, g + G, ... of its column in every stage.  The maps live in shared memory,
+// interleaved [element][column] so the 32 columns of a warp hit 32 banks.  Forward: two maps ping-pong.  Backward:
+// every map is kept (k-max stages also keep their selected rows), then the gradient goes back through two more maps;
+// the weight gradients of a tile are summed by one owner thread per weight over the tile's columns in column order
+// and added to the CTA's running sum, which goes to the workspace as the CTA's partial.
+// ------------------------------------------------------------------------------------------------
+constexpr int kConvCols = 32;
+constexpr size_t kConvSmemCap = 224 * 1024;
+
+struct ConvStagePlan {
+  int kind, width, pad, act, k;
+  int rows_in, cin, rows_out, cout;
+  int in_off, out_off, idx_off;  // map offsets (elements of one column; backward layout)
+  int w_off, nw;                 // weights in shared memory: kernel [width, cin, cout] then bias [cout]
+};
+struct ConvPlan {
+  int nstage, G, nw;           // channel slots per column, total weight floats
+  int map_floats, max_map;     // backward: all maps of a column; the largest map
+  int ga_off, gb_off;          // backward gradient maps
+  int rows_out, cout;          // last map
+  ConvStagePlan s[B2CTR_CONV_STACK_MAX_STAGES];
+};
+
+__device__ __forceinline__ float& cs_at(float* sm, int off, int i, int col) { return sm[(off + i) * kConvCols + col]; }
+
+// forward of stage p from map `in` to map `out` (and the selected rows to `idx` when k-max and idx_off >= 0)
+__device__ __forceinline__ void conv_stage_fwd(const ConvStagePlan& p, const float* sw, float* sm, int in, int out,
+                                               int idx, int g, int G, int col) {
+  if (p.kind == B2CTR_CONV_STAGE_CONV) {
+    const float* K = sw + p.w_off;
+    const float* bias = K + p.width * p.cin * p.cout;
+    for (int co = g; co < p.cout; co += G) {
+      for (int r = 0; r < p.rows_out; ++r) {
+        float acc = bias[co];
+        for (int t = 0; t < p.width; ++t) {
+          const int rr = r + t - p.pad;
+          if (rr < 0 || rr >= p.rows_in) continue;
+          const float* kt = K + t * p.cin * p.cout + co;
+          for (int ci = 0; ci < p.cin; ++ci) acc = fmaf(cs_at(sm, in, rr * p.cin + ci, col), kt[ci * p.cout], acc);
+        }
+        cs_at(sm, out, r * p.cout + co, col) = act_apply(acc, p.act);
+      }
+    }
+  } else {
+    const int C = p.cin;
+    for (int c = g; c < C; c += G) {
+      // the j-th pick is the largest value ordered after the (j-1)-th in (value descending, row ascending)
+      float pv = 0.f;
+      int pi = -1;
+      for (int j = 0; j < p.k; ++j) {
+        float bv = 0.f;
+        int bi = -1;
+        for (int r = 0; r < p.rows_in; ++r) {
+          const float v = cs_at(sm, in, r * C + c, col);
+          const bool after = pi < 0 || v < pv || (v == pv && r > pi);
+          if (after && (bi < 0 || v > bv)) { bv = v; bi = r; }
+        }
+        pv = bv;
+        pi = bi;
+        cs_at(sm, out, j * C + c, col) = bi < 0 ? __int_as_float(0x7fc00000) : bv;   // only NaN rows left
+        if (idx >= 0) cs_at(sm, idx, j * C + c, col) = __int_as_float(bi);
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ void conv_stage_weights(const b2ctr_conv_stack_t& a, const ConvPlan& P, float* sw) {
+  for (int s = 0; s < P.nstage; ++s) {
+    const ConvStagePlan& p = P.s[s];
+    if (p.kind != B2CTR_CONV_STAGE_CONV) continue;
+    const int nk = p.width * p.cin * p.cout;
+    for (int i = threadIdx.x; i < p.nw; i += blockDim.x)
+      sw[p.w_off + i] = i < nk ? a.stage[s].kernel[i] : (a.stage[s].bias ? a.stage[s].bias[i - nk] : 0.f);
+  }
+}
+
+// the input map of a column into map 0
+__device__ __forceinline__ void conv_load_input(const b2ctr_conv_stack_t& a, float* sm, int off, int64_t b, int e,
+                                                bool valid, int g, int G, int col) {
+  const int C = a.channels;
+  const float* xp = a.x + b * a.ldx + a.xcol;
+  for (int c = g; c < C; c += G)
+    for (int r = 0; r < a.rows; ++r)
+      cs_at(sm, off, r * C + c, col) = valid ? xp[((int64_t)r * a.dim + e) * C + c] : 0.f;
+}
+
+__global__ void conv_stack_fwd_kernel(const b2ctr_conv_stack_t a, const __grid_constant__ ConvPlan P) {
+  extern __shared__ float smem[];
+  float* sw = smem;
+  float* sm = smem + P.nw;
+  const int G = P.G, col = threadIdx.x % kConvCols, g = threadIdx.x / kConvCols;
+  const int64_t ncol = a.batch * a.dim, cg = (int64_t)blockIdx.x * kConvCols + col;
+  const bool valid = cg < ncol;
+  const int64_t b = valid ? cg / a.dim : 0;
+  const int e = valid ? (int)(cg % a.dim) : 0;
+  conv_stage_weights(a, P, sw);
+  int cur = 0, nxt = P.max_map;
+  conv_load_input(a, sm, cur, b, e, valid, g, G, col);
+  __syncthreads();
+  for (int s = 0; s < P.nstage; ++s) {
+    conv_stage_fwd(P.s[s], sw, sm, cur, nxt, -1, g, G, col);
+    __syncthreads();
+    const int t = cur;
+    cur = nxt;
+    nxt = t;
+  }
+  if (!valid) return;
+  float* op = a.out + b * a.ldout + a.outcol;
+  for (int c = g; c < P.cout; c += G)
+    for (int r = 0; r < P.rows_out; ++r) op[((int64_t)r * a.dim + e) * P.cout + c] = cs_at(sm, cur, r * P.cout + c, col);
+}
+
+__global__ void conv_stack_bwd_kernel(const b2ctr_conv_stack_t a, const __grid_constant__ ConvPlan P,
+                                      float* __restrict__ partial) {
+  extern __shared__ float smem[];
+  float* sw = smem;
+  float* sacc = smem + P.nw;
+  float* sm = smem + 2 * P.nw;
+  const int G = P.G, col = threadIdx.x % kConvCols, g = threadIdx.x / kConvCols;
+  const int64_t ncol = a.batch * a.dim;
+  conv_stage_weights(a, P, sw);
+  for (int i = threadIdx.x; i < P.nw; i += blockDim.x) sacc[i] = 0.f;
+  for (int64_t tile = blockIdx.x; tile * kConvCols < ncol; tile += gridDim.x) {
+    const int64_t cg = tile * kConvCols + col;
+    const bool valid = cg < ncol;
+    const int nvalid = (int)min((int64_t)kConvCols, ncol - tile * kConvCols);
+    const int64_t b = valid ? cg / a.dim : 0;
+    const int e = valid ? (int)(cg % a.dim) : 0;
+    __syncthreads();  // the previous tile's maps are no longer read
+    conv_load_input(a, sm, 0, b, e, valid, g, G, col);
+    __syncthreads();
+    for (int s = 0; s < P.nstage; ++s) {
+      const ConvStagePlan& p = P.s[s];
+      conv_stage_fwd(p, sw, sm, p.in_off, p.out_off, p.idx_off, g, G, col);
+      __syncthreads();
+    }
+    // incoming gradient of the last map
+    int gcur = P.ga_off, gnxt = P.gb_off;
+    if (valid) {
+      const float* dp = a.out + b * a.ldout + a.outcol;
+      for (int c = g; c < P.cout; c += G)
+        for (int r = 0; r < P.rows_out; ++r)
+          cs_at(sm, gcur, r * P.cout + c, col) = dp[((int64_t)r * a.dim + e) * P.cout + c];
+    } else {
+      for (int c = g; c < P.cout; c += G)
+        for (int r = 0; r < P.rows_out; ++r) cs_at(sm, gcur, r * P.cout + c, col) = 0.f;
+    }
+    __syncthreads();
+    for (int s = P.nstage - 1; s >= 0; --s) {
+      const ConvStagePlan& p = P.s[s];
+      if (p.kind == B2CTR_CONV_STAGE_KMAX) {
+        const int C = p.cin;
+        for (int c = g; c < C; c += G) {
+          for (int r = 0; r < p.rows_in; ++r) cs_at(sm, gnxt, r * C + c, col) = 0.f;
+          for (int j = 0; j < p.k; ++j) {
+            const int r = __float_as_int(cs_at(sm, p.idx_off, j * C + c, col));
+            if (r >= 0) cs_at(sm, gnxt, r * C + c, col) = cs_at(sm, gcur, j * C + c, col);
+          }
+        }
+        __syncthreads();
+      } else {
+        // dz = dy * act'(y), in place
+        for (int co = g; co < p.cout; co += G)
+          for (int r = 0; r < p.rows_out; ++r)
+            cs_at(sm, gcur, r * p.cout + co, col) *= act_grad_from_out(cs_at(sm, p.out_off, r * p.cout + co, col), p.act);
+        __syncthreads();
+        const float* K = sw + p.w_off;
+        if (s > 0 || a.dx) {
+          for (int ci = g; ci < p.cin; ci += G) {
+            for (int r = 0; r < p.rows_in; ++r) {
+              float acc = 0.f;
+              for (int t = 0; t < p.width; ++t) {
+                const int ro = r - t + p.pad;
+                if (ro < 0 || ro >= p.rows_out) continue;
+                const float* kt = K + (t * p.cin + ci) * p.cout;
+                for (int co = 0; co < p.cout; ++co) acc = fmaf(cs_at(sm, gcur, ro * p.cout + co, col), kt[co], acc);
+              }
+              cs_at(sm, gnxt, r * p.cin + ci, col) = acc;
+            }
+          }
+        }
+        // weight gradients of this tile: one owner per weight, columns in order
+        const int nk = p.width * p.cin * p.cout;
+        for (int w = threadIdx.x; w < p.nw; w += blockDim.x) {
+          float acc = 0.f;
+          if (w < nk) {
+            const int co = w % p.cout, ci = (w / p.cout) % p.cin, t = w / (p.cout * p.cin);
+            for (int c = 0; c < nvalid; ++c)
+              for (int r = 0; r < p.rows_out; ++r) {
+                const int rr = r + t - p.pad;
+                if (rr < 0 || rr >= p.rows_in) continue;
+                acc = fmaf(cs_at(sm, p.in_off, rr * p.cin + ci, c), cs_at(sm, gcur, r * p.cout + co, c), acc);
+              }
+          } else {
+            const int co = w - nk;
+            for (int c = 0; c < nvalid; ++c)
+              for (int r = 0; r < p.rows_out; ++r) acc += cs_at(sm, gcur, r * p.cout + co, c);
+          }
+          sacc[p.w_off + w] += acc;
+        }
+        __syncthreads();
+      }
+      const int t = gcur;
+      gcur = gnxt;
+      gnxt = t;
+    }
+    if (valid && a.dx) {
+      const int C = a.channels;
+      float* dp = a.dx + b * a.lddx + a.dxcol;
+      for (int c = g; c < C; c += G)
+        for (int r = 0; r < a.rows; ++r) {
+          const int64_t o = ((int64_t)r * a.dim + e) * C + c;
+          const float v = cs_at(sm, gcur, r * C + c, col);
+          dp[o] = a.dx_accumulate ? dp[o] + v : v;
+        }
+    }
+  }
+  __syncthreads();
+  if (partial)
+    for (int i = threadIdx.x; i < P.nw; i += blockDim.x) partial[(int64_t)blockIdx.x * P.nw + i] = sacc[i];
+}
+
 }  // namespace b2ctr
 
 using namespace b2ctr;
@@ -2679,6 +2904,157 @@ b2ctr_status_t b2ctr_regulate_bwd(const b2ctr_regulate_t* a, void* workspace, si
     B2_CHECK_LAUNCH("b2ctr_regulate_bwd(reduce)");
     regulate_dg_kernel<<<1, 64, 0, ST>>>(k, sums);
     B2_CHECK_LAUNCH("b2ctr_regulate_bwd(gates)");
+  }
+  return B2CTR_OK;
+}
+
+// ---- CCPM's convolution stack ---------------------------------------------------------------------
+static b2ctr_status_t conv_plan(const b2ctr_conv_stack_t* a, const char* what, ConvPlan* P) {
+  B2_REQUIRE(a, "%s: NULL descriptor", what);
+  B2_REQUIRE(a->struct_size == (int32_t)sizeof(b2ctr_conv_stack_t), "%s: struct_size %d, expected %d", what,
+             a->struct_size, (int)sizeof(b2ctr_conv_stack_t));
+  B2_REQUIRE(a->nstage >= 1 && a->nstage <= B2CTR_CONV_STACK_MAX_STAGES, "%s: needs 1 to %d stages (got %d)", what,
+             B2CTR_CONV_STACK_MAX_STAGES, a->nstage);
+  B2_REQUIRE(a->rows >= 1 && a->rows <= 64, "%s: needs 1 <= rows <= 64 (got %d)", what, a->rows);
+  B2_REQUIRE(a->dim >= 1 && a->channels >= 1 && a->channels <= 16, "%s: needs dim >= 1 and 1 <= channels <= 16", what);
+  B2_REQUIRE(a->batch >= 0, "%s: negative batch", what);
+  const int64_t in_w = (int64_t)a->rows * a->dim * a->channels;
+  B2_REQUIRE(a->x && a->xcol >= 0 && a->ldx >= a->xcol + in_w, "%s: x is NULL or its window does not fit its row", what);
+  *P = ConvPlan{};
+  P->nstage = a->nstage;
+  int rows = a->rows, C = a->channels, off = rows * C, G = C, maxmap = rows * C, nw = 0;
+  for (int s = 0; s < a->nstage; ++s) {
+    const b2ctr_conv_stage_t& st = a->stage[s];
+    ConvStagePlan& p = P->s[s];
+    p.kind = st.kind;
+    p.rows_in = rows;
+    p.cin = C;
+    p.in_off = s == 0 ? 0 : P->s[s - 1].out_off;
+    p.idx_off = -1;
+    if (st.kind == B2CTR_CONV_STAGE_CONV) {
+      B2_REQUIRE(st.width >= 1 && st.width <= 32 && st.filters >= 1 && st.filters <= 16,
+                 "%s: stage %d needs 1 <= width <= 32 and 1 <= filters <= 16 (got %d, %d)", what, s, st.width,
+                 st.filters);
+      B2_REQUIRE(st.act >= B2CTR_ACT_NONE && st.act <= B2CTR_ACT_TANH, "%s: stage %d: unknown activation %d", what, s,
+                 st.act);
+      B2_REQUIRE(st.kernel, "%s: stage %d: NULL kernel", what, s);
+      p.width = st.width;
+      p.pad = (st.width - 1) / 2;
+      p.act = st.act;
+      p.rows_out = rows;
+      p.cout = st.filters;
+      p.w_off = nw;
+      p.nw = st.width * C * st.filters + st.filters;
+      nw += p.nw;
+      p.out_off = off;
+      off += rows * st.filters;
+      C = st.filters;
+    } else {
+      B2_REQUIRE(st.kind == B2CTR_CONV_STAGE_KMAX, "%s: stage %d: unknown kind %d", what, s, st.kind);
+      B2_REQUIRE(st.k >= 1 && st.k <= rows, "%s: stage %d needs 1 <= k <= %d rows (got %d)", what, s, rows, st.k);
+      p.k = st.k;
+      p.rows_out = st.k;
+      p.cout = C;
+      p.out_off = off;
+      p.idx_off = off + st.k * C;
+      off += 2 * st.k * C;
+      rows = st.k;
+    }
+    G = std::max(G, C);
+    maxmap = std::max(maxmap, rows * C);
+  }
+  P->G = G;
+  P->nw = nw;
+  P->max_map = maxmap;
+  P->ga_off = off;
+  P->gb_off = off + maxmap;
+  P->map_floats = off + 2 * maxmap;
+  P->rows_out = rows;
+  P->cout = C;
+  const size_t smem = (2 * (size_t)nw + (size_t)kConvCols * P->map_floats) * sizeof(float);
+  B2_REQUIRE(smem <= kConvSmemCap, "%s: the backward needs %zu bytes of shared memory, above the %zu limit", what, smem,
+             kConvSmemCap);
+  const int64_t out_w = (int64_t)rows * a->dim * C;
+  B2_REQUIRE(a->out && a->outcol >= 0 && a->ldout >= a->outcol + out_w,
+             "%s: out is NULL or its window does not fit its row", what);
+  return B2CTR_OK;
+}
+
+static size_t conv_fwd_smem(const ConvPlan& P) { return ((size_t)P.nw + (size_t)kConvCols * 2 * P.max_map) * sizeof(float); }
+static size_t conv_bwd_smem(const ConvPlan& P) { return (2 * (size_t)P.nw + (size_t)kConvCols * P.map_floats) * sizeof(float); }
+static int conv_bwd_blocks(const b2ctr_conv_stack_t* a, const ConvPlan& P) {
+  const int per_sm = std::max(1, (int)((228 * 1024) / (conv_bwd_smem(P) + 1024)));
+  return grid_for(a->batch * a->dim, kConvCols, std::min(per_sm, 2048 / (kConvCols * P.G)));
+}
+
+b2ctr_status_t b2ctr_conv_stack_fwd(const b2ctr_conv_stack_t* a, void* stream) {
+  ConvPlan P;
+  const b2ctr_status_t st = conv_plan(a, "conv_stack_fwd", &P);
+  if (st != B2CTR_OK) return st;
+  if (a->batch == 0) return B2CTR_OK;
+  const size_t smem = conv_fwd_smem(P);
+  if (cudaFuncSetAttribute(conv_stack_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+    set_error("conv_stack_fwd: cannot reserve %zu bytes of shared memory", smem);
+    return B2CTR_ERR_CUDA;
+  }
+  const int64_t nblk = ceil_div(a->batch * a->dim, kConvCols);
+  conv_stack_fwd_kernel<<<(unsigned)nblk, kConvCols * P.G, smem, ST>>>(*a, P);
+  B2_CHECK_LAUNCH("b2ctr_conv_stack_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_conv_stack_bwd_workspace_bytes(const b2ctr_conv_stack_t* a) {
+  ConvPlan P;
+  if (conv_plan(a, "conv_stack_bwd_workspace_bytes", &P) != B2CTR_OK || a->batch <= 0) return 0;
+  return (size_t)conv_bwd_blocks(a, P) * P.nw * sizeof(float);
+}
+
+b2ctr_status_t b2ctr_conv_stack_bwd(const b2ctr_conv_stack_t* a, void* workspace, size_t workspace_bytes, void* stream) {
+  ConvPlan P;
+  const b2ctr_status_t st = conv_plan(a, "conv_stack_bwd", &P);
+  if (st != B2CTR_OK) return st;
+  const int64_t in_w = (int64_t)a->rows * a->dim * a->channels;
+  B2_REQUIRE(!a->dx || (a->dxcol >= 0 && a->lddx >= a->dxcol + in_w), "conv_stack_bwd: the dx window does not fit its row");
+  bool want_dw = false;
+  for (int s = 0; s < a->nstage; ++s)
+    if (a->stage[s].kind == B2CTR_CONV_STAGE_CONV) want_dw = want_dw || a->stage[s].dkernel || a->stage[s].dbias;
+  B2_REQUIRE(a->dx || want_dw, "conv_stack_bwd: nothing to compute");
+  if (a->batch == 0) {
+    // no column: the weight gradients are zero
+    for (int s = 0; s < a->nstage; ++s) {
+      const ConvStagePlan& p = P.s[s];
+      if (p.kind != B2CTR_CONV_STAGE_CONV) continue;
+      if (a->stage[s].dkernel) cudaMemsetAsync(a->stage[s].dkernel, 0, sizeof(float) * (p.nw - p.cout), ST);
+      if (a->stage[s].dbias) cudaMemsetAsync(a->stage[s].dbias, 0, sizeof(float) * p.cout, ST);
+    }
+    return B2CTR_OK;
+  }
+  const int nblk = conv_bwd_blocks(a, P);
+  const size_t need = want_dw ? (size_t)nblk * P.nw * sizeof(float) : 0;
+  if (want_dw && (!workspace || workspace_bytes < need)) {
+    set_error("conv_stack_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  const size_t smem = conv_bwd_smem(P);
+  if (cudaFuncSetAttribute(conv_stack_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+    set_error("conv_stack_bwd: cannot reserve %zu bytes of shared memory", smem);
+    return B2CTR_ERR_CUDA;
+  }
+  float* partial = want_dw ? (float*)workspace : nullptr;
+  conv_stack_bwd_kernel<<<nblk, kConvCols * P.G, smem, ST>>>(*a, P, partial);
+  B2_CHECK_LAUNCH("b2ctr_conv_stack_bwd");
+  for (int s = 0; s < a->nstage && want_dw; ++s) {
+    const ConvStagePlan& p = P.s[s];
+    if (p.kind != B2CTR_CONV_STAGE_CONV) continue;
+    const int nk = p.nw - p.cout;
+    if (a->stage[s].dkernel) {
+      ordered_sum_kernel<<<grid_for(nk, 256, 8), 256, 0, ST>>>(partial + p.w_off, P.nw, nblk, nk, a->stage[s].dkernel);
+      B2_CHECK_LAUNCH("b2ctr_conv_stack_bwd(dkernel)");
+    }
+    if (a->stage[s].dbias) {
+      ordered_sum_kernel<<<1, 32, 0, ST>>>(partial + p.w_off + nk, P.nw, nblk, p.cout, a->stage[s].dbias);
+      B2_CHECK_LAUNCH("b2ctr_conv_stack_bwd(dbias)");
+    }
   }
   return B2CTR_OK;
 }

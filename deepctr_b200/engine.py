@@ -733,6 +733,81 @@ class Dense(Layer):
         return c
 
 
+
+def _pair(v, what):
+    if isinstance(v, int):
+        return (v, v)
+    v = tuple(int(i) for i in v)
+    if len(v) != 2:
+        raise ValueError("%s must be an int or a pair, got %r" % (what, v))
+    return v
+
+
+class Conv2D(Layer):
+    """tf.keras.layers.Conv2D as CCPM uses it (deepctr/models/ccpm.py:65-66): a kernel (width, 1) over [B, rows, E, C]
+    channels_last, strides (1, 1), padding 'same', an activation of the package's set and a bias.  Each embedding
+    coordinate is an independent 1-D signal over the rows; the layer is one stage of b2ctr_conv_stack, and in CCPM
+    the planner (inputs.ConvStackPlan) runs every Conv2D and KMaxPooling of the stack in one launch.  Weights
+    ``kernel`` [width, 1, C, filters] (glorot_uniform) and ``bias`` [filters] (zeros), as Keras names them.  Any
+    other configuration raises NotImplementedError naming the argument."""
+
+    def __init__(self, filters, kernel_size, strides=(1, 1), padding='valid', data_format=None, dilation_rate=(1, 1),
+                 activation=None, use_bias=True, kernel_initializer=None, bias_initializer=None,
+                 kernel_regularizer=None, bias_regularizer=None, **kwargs):
+        from .layers.activation import fusable_activation
+        ks = _pair(kernel_size, "kernel_size")
+        if ks[1] != 1:
+            raise NotImplementedError("Conv2D kernel_size %r: only (width, 1) kernels are supported" % (kernel_size,))
+        if _pair(strides, "strides") != (1, 1):
+            raise NotImplementedError("Conv2D strides %r: only (1, 1) is supported" % (strides,))
+        if str(padding).lower() != "same":
+            raise NotImplementedError("Conv2D padding %r: only 'same' is supported" % (padding,))
+        if data_format not in (None, "channels_last"):
+            raise NotImplementedError("Conv2D data_format %r: only 'channels_last' is supported" % (data_format,))
+        if _pair(dilation_rate, "dilation_rate") != (1, 1):
+            raise NotImplementedError("Conv2D dilation_rate %r: only (1, 1) is supported" % (dilation_rate,))
+        if activation not in (None, "linear") and (not fusable_activation(activation) or activation == "dice"):
+            raise NotImplementedError("Conv2D activation %r: only None, linear, relu, sigmoid and tanh are supported"
+                                      % (activation,))
+        if kernel_regularizer is not None or bias_regularizer is not None:
+            raise NotImplementedError("Conv2D kernel_regularizer / bias_regularizer are not supported")
+        Layer.__init__(self, **kwargs)
+        self.filters, self.kernel_size, self.activation, self.use_bias = int(filters), ks, activation, use_bias
+        self.kernel_initializer = kernel_initializer or GlorotUniform()
+        self.bias_initializer = bias_initializer or Zeros()
+
+    def build(self, input_shape):
+        if len(input_shape) != 4:
+            raise ValueError("Conv2D expects a 4-D input [batch, rows, embedding, channels], got %s"
+                             % (tuple(input_shape),))
+        rows, channels = int(input_shape[1]), int(input_shape[3])
+        K.conv_stack_check(rows, channels, [("conv", self.kernel_size[0], self.filters)])
+        self.kernel = self.add_weight("kernel", (self.kernel_size[0], 1, channels, self.filters),
+                                      self.kernel_initializer)
+        self.bias = self.add_weight("bias", (self.filters,), self.bias_initializer) if self.use_bias else None
+        self.built = True
+
+    def stage(self):
+        """This layer as a b2ctr_conv_stack stage (ops.conv_stack)."""
+        return ("conv", self.kernel_size[0], self.filters, self.activation, self.kernel, self.bias)
+
+    def call(self, inputs, **kwargs):
+        planner = getattr(self, "_planner", None)
+        served = planner.conv_stacked(self, inputs) if planner is not None else None
+        if served is not None:
+            return served
+        b, rows, dim, channels = inputs.data.shape
+        return ops.conv_stack(inputs, [self.stage()], rows, dim, channels, (b, rows, dim, self.filters))
+
+    def compute_output_shape(self, input_shape):
+        return tuple(input_shape[:3]) + (self.filters,)
+
+    def get_config(self):
+        c = Layer.get_config(self)
+        c.update(filters=self.filters, kernel_size=self.kernel_size, strides=(1, 1), padding="same",
+                 activation=self.activation, use_bias=self.use_bias)
+        return c
+
 class Flatten(Layer):
     def call(self, inputs, **kwargs):
         return ops.flatten(inputs)

@@ -368,6 +368,8 @@ class EmbeddingPlanner(object):
         self.dnn_places = _plan_dnn_input(model, consumers, out_ids)
         # EDCN's RegulationModule pairs and the bridges in front of them: one b2ctr_regulate launch each
         self.regulate_plan = _plan_regulate(model, consumers, out_ids)
+        # CCPM's Lambda(expand_dims) -> [Conv2D -> KMaxPooling(axis=1)] x l -> Flatten: one b2ctr_conv_stack launch
+        self.conv_plan = _plan_conv_stack(model, consumers, out_ids)
         # IFM / DIFM scale the linear lookups by per-sample field weights before Linear sums them: their rows are
         # needed, so they are never fused into the gather's row-sum (lin_hint)
         from .layers.utils import RefineWeight
@@ -899,6 +901,23 @@ class EmbeddingPlanner(object):
             self.results[id(node)] = y
         return VIRTUAL
 
+    def conv_stacked(self, layer, x):
+        """The first Conv2D of a chain the planner claimed (ConvStackPlan): one launch runs every Conv2D and
+        KMaxPooling of the chain on ``x`` and becomes the last KMaxPooling's result; the maps between are never
+        written (VIRTUAL).  Else None."""
+        from . import ops
+        chain = self.conv_plan.chains.get(id(layer))
+        if chain is None:
+            return None
+        b, rows, dim, channels = x.data.shape
+        last = chain[-1]
+        res = ops.conv_stack(x, [n.layer.stage() for n in chain], rows, dim, channels,
+                             (b,) + tuple(last.outputs[0].shape[1:]))
+        for n in chain[1:-1]:
+            self.results[id(n)] = VIRTUAL
+        self.results[id(last)] = res
+        return VIRTUAL
+
     def append_dense(self, emb_flat, dense_flat):
         """combined_dnn_input: place the dense features behind the embeddings (and PNN's placed products) in the
         main buffer so the DNN input is a zero-copy window.  Returns the window or None."""
@@ -1206,6 +1225,60 @@ def _plan_regulate(model, consumers, out_ids):
             if regs is not None:
                 pairs[id(regs[0].layer)] = (regs[1].layer, regs[1])
     return RegulatePlan(pairs, bridges)
+
+
+class ConvStackPlan(object):
+    """CCPM's convolution stack (deepctr/models/ccpm.py:58-70) served by one b2ctr_conv_stack launch: the chain
+    concat_func(embeddings) -> Lambda(expand_dims(x, 3)) -> [Conv2D -> KMaxPooling(axis=1)] x l -> Flatten, every
+    intermediate with this one consumer, runs when its first Conv2D is called.  The input is read in place (a
+    window of the gather buffer), the per-layer maps are never written, and Flatten of the result is a view.
+
+    ``chains`` {id(first Conv2D layer): [Conv2D node, KMaxPooling node, ...]}.  Decided once from the model's graph;
+    any other graph, or a stack beyond the kernel's limits, runs layer by layer on the same kernel."""
+
+    def __init__(self, chains):
+        self.chains = chains
+
+
+def _plan_conv_stack(model, consumers, out_ids):
+    from . import kernels as K
+    from .layers.sequence import KMaxPooling
+    calls = defaultdict(int)
+    for node in model._order:
+        calls[id(node.layer)] += 1
+
+    def only(t, cls):
+        """The single consumer node of ``t`` when it is a ``cls`` called once, else None."""
+        cs = consumers[id(t)]
+        if id(t) in out_ids or len(cs) != 1 or not isinstance(cs[0].layer, cls) or calls[id(cs[0].layer)] != 1:
+            return None
+        return cs[0]
+
+    chains = {}
+    for node in model._order:
+        if not isinstance(node.layer, E.Lambda) or not isinstance(node.inputs, E.KTensor):
+            continue
+        src, out = node.inputs, node.outputs[0]
+        if len(src.shape) != 3 or tuple(out.shape) != tuple(src.shape) + (1,):
+            continue
+        chain, t = [], out
+        while True:
+            conv = only(t, E.Conv2D)
+            if conv is None:
+                break
+            pool = only(conv.outputs[0], KMaxPooling)
+            if pool is None or pool.layer.axis != 1:
+                break
+            chain += [conv, pool]
+            t = pool.outputs[0]
+        if not chain or only(t, E.Flatten) is None:
+            continue
+        try:
+            K.conv_stack_check(int(src.shape[1]), 1, [n.layer.stage()[:3] for n in chain])
+        except ValueError:
+            continue
+        chains[id(chain[0].layer)] = chain
+    return ConvStackPlan(chains)
 
 
 class FieldAwarePlan(object):

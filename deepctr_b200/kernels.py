@@ -1013,6 +1013,103 @@ def regulate_bwd(mode, nfield, dim, batch, x, h=None, ax=None, ah=None, gates=()
     return dx, dh, dax, dah, dg[0], dg[1]
 
 
+
+# limits of b2ctr_conv_stack_fwd / _bwd (include/b2ctr.h)
+CONV_MAX_ROWS, CONV_MAX_CHANNELS, CONV_MAX_WIDTH, CONV_SMEM_BYTES = 64, 16, 32, 224 * 1024
+
+
+def conv_stack_check(rows, channels, stages):
+    """Raise ValueError naming the limit of b2ctr_conv_stack that ``stages`` on a [rows, channels] column breaks.
+    ``stages``: ("conv", width, filters) or ("kmax", k) tuples (extra entries ignored).  Returns the last map's
+    (rows, channels)."""
+    if not 1 <= len(stages) <= L.CONV_STACK_MAX_STAGES:
+        raise ValueError("the convolution stack supports 1 to %d stages (got %d)"
+                         % (L.CONV_STACK_MAX_STAGES, len(stages)))
+    if not 1 <= rows <= CONV_MAX_ROWS:
+        raise ValueError("the convolution stack supports 1 to %d rows (CONV_MAX_ROWS), got %d" % (CONV_MAX_ROWS, rows))
+    if not 1 <= channels <= CONV_MAX_CHANNELS:
+        raise ValueError("the convolution stack supports 1 to %d channels (CONV_MAX_CHANNELS), got %d"
+                         % (CONV_MAX_CHANNELS, channels))
+    maps = [rows * channels]
+    nw = 0
+    for st in stages:
+        if st[0] == "conv":
+            width, filters = st[1], st[2]
+            if not 1 <= width <= CONV_MAX_WIDTH:
+                raise ValueError("Conv2D supports kernel widths 1 to %d (CONV_MAX_WIDTH), got %d"
+                                 % (CONV_MAX_WIDTH, width))
+            if not 1 <= filters <= CONV_MAX_CHANNELS:
+                raise ValueError("Conv2D supports 1 to %d filters (CONV_MAX_CHANNELS), got %d"
+                                 % (CONV_MAX_CHANNELS, filters))
+            nw += width * channels * filters + filters
+            channels = filters
+            maps.append(rows * channels)
+        else:
+            if not 1 <= st[1] <= rows:
+                raise ValueError("k must be in 1 ~ %d,now k is %d" % (rows, st[1]))
+            rows = st[1]
+            maps += [rows * channels, rows * channels]
+    smem = 4 * (2 * nw + 32 * (sum(maps) + 2 * max(maps)))
+    if smem > CONV_SMEM_BYTES:
+        raise ValueError("the convolution stack needs %d bytes of shared memory per 32 columns, above its %d-byte "
+                         "limit (CONV_SMEM_BYTES): fewer rows or channels" % (smem, CONV_SMEM_BYTES))
+    return rows, channels
+
+
+def _conv_desc(stages, x, rows, dim, channels, batch, out):
+    """b2ctr_conv_stack_t over x (2-D [B, >= rows*dim*channels] view read in place, pitch stride(0)) and out (the
+    forward output or the backward's incoming gradient, the same kind of view).  ``stages``: ("conv", width,
+    filters, act, kernel, bias or None) or ("kmax", k)."""
+    _require_cuda(x, out)
+    a = L.ConvStack()
+    a.struct_size = C.sizeof(L.ConvStack)
+    a.nstage, a.rows, a.dim, a.channels, a.batch = len(stages), rows, dim, channels, batch
+    a.x, a.ldx = x.data_ptr(), x.stride(0)
+    a.out, a.ldout = out.data_ptr(), out.stride(0)
+    for i, st in enumerate(stages):
+        d = a.stage[i]
+        if st[0] == "conv":
+            _, width, filters, act, kernel, bias = st
+            _require_cuda(kernel, bias)
+            d.kind, d.width, d.filters, d.act = L.CONV_STAGE_CONV, width, filters, L.ACT_BY_NAME[act]
+            d.kernel = kernel.data_ptr()
+            d.bias = bias.data_ptr() if bias is not None else None
+        else:
+            d.kind, d.k = L.CONV_STAGE_KMAX, st[1]
+    return a
+
+
+def conv_stack_fwd(stages, x, rows, dim, channels, batch, out):
+    """CCPM's conv / k-max stack per (sample, e) column in one launch (b2ctr_conv_stack_fwd): x [B, rows, dim,
+    channels] read in place, the last map written in Flatten order into ``out`` (a 2-D view)."""
+    a = _conv_desc(stages, x, rows, dim, channels, batch, out)
+    L.check(L.lib().b2ctr_conv_stack_fwd(C.byref(a), stream()), "conv_stack_fwd")
+    return out
+
+
+def conv_stack_bwd(stages, x, rows, dim, channels, batch, dout, dx=None, dx_accumulate=False, want_dw=()):
+    """Recompute the stack and take its gradient (b2ctr_conv_stack_bwd): ``dx`` a 2-D view to write (or add) x's
+    gradient into, or None; ``want_dw`` per conv stage whether its (dkernel, dbias) are wanted.  Returns the list of
+    (dkernel, dbias) per stage (None for k-max stages or when not wanted)."""
+    a = _conv_desc(stages, x, rows, dim, channels, batch, dout)
+    if dx is not None:
+        _require_cuda(dx)
+        a.dx, a.lddx, a.dx_accumulate = dx.data_ptr(), dx.stride(0), int(bool(dx_accumulate))
+    dws = []
+    for i, st in enumerate(stages):
+        if st[0] == "conv" and (want_dw[i] if i < len(want_dw) else False):
+            dk = torch.empty(tuple(st[4].shape), dtype=torch.float32, device=x.device)
+            db = torch.empty((st[2],), dtype=torch.float32, device=x.device) if st[5] is not None else None
+            a.stage[i].dkernel = dk.data_ptr()
+            a.stage[i].dbias = db.data_ptr() if db is not None else None
+            dws.append((dk, db))
+        else:
+            dws.append(None)
+    nbytes = L.lib().b2ctr_conv_stack_bwd_workspace_bytes(C.byref(a)) if any(d is not None for d in dws) else 0
+    ws = workspace(nbytes, x.device)
+    L.check(L.lib().b2ctr_conv_stack_bwd(C.byref(a), ptr(ws), nbytes, stream()), "conv_stack_bwd")
+    return dws
+
 def din_att_input_fwd(q, ldq, keys, ldk, batch, T, E):
     out = torch.empty((batch, T, 4 * E), dtype=torch.float32, device=q.device)
     _lib_call("din_att_input_fwd", ptr(q), ldq, ptr(keys), ldk, ptr(out), batch, T, E, stream())
@@ -1250,5 +1347,6 @@ for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filte
     globals()[_n] = _timed(globals()[_n])
 
 
-for _n in ("mha_fwd", "mha_bwd", "layernorm_fwd", "layernorm_bwd", "regulate_fwd", "regulate_bwd"):
+for _n in ("mha_fwd", "mha_bwd", "layernorm_fwd", "layernorm_bwd", "regulate_fwd", "regulate_bwd",
+           "conv_stack_fwd", "conv_stack_bwd"):
     globals()[_n] = _timed(globals()[_n])

@@ -1,6 +1,6 @@
 """Host mirror of deepctr/layers/sequence.py for the hot path: SequencePoolingLayer (:41-120),
-WeightedSequenceLayer (:123-197), AttentionSequencePoolingLayer (:200-315), Transformer (:431-651) and
-PositionEncoding (:654-703).
+WeightedSequenceLayer (:123-197), AttentionSequencePoolingLayer (:200-315), Transformer (:431-651),
+PositionEncoding (:654-703) and KMaxPooling (:818-874).
 
 When these layers hang directly off an embedding lookup of a model input (the shape
 ``get_varlen_pooling_list`` produces) the EmbeddingPlanner folds them into the fused gather and their
@@ -8,6 +8,7 @@ When these layers hang directly off an embedding lookup of a model input (the sh
 import numpy as np
 
 from .. import engine as E
+from .. import kernels as K
 from .. import ops
 from ..engine import Layer, Constant, TruncatedNormal, glorot_uniform
 from .core import LocalActivationUnit
@@ -331,3 +332,52 @@ class PositionEncoding(Layer):
                   'scale': self.scale}
         base = Layer.get_config(self)
         return dict(list(base.items()) + list(config.items()))
+
+
+class KMaxPooling(Layer):
+    """The k largest values along ``axis`` in descending order (tf.nn.top_k(sorted=True): equal values keep the
+    lower index first), deepctr/layers/sequence.py:818-874.  An n-D input is viewed as [outer, n, inner] with n the
+    pooled axis; the layer is one k-max stage of b2ctr_conv_stack over its inner columns, and in CCPM the planner
+    (inputs.ConvStackPlan) runs it inside the launch of the whole convolution stack.  The gradient goes to the
+    selected elements only.
+
+    Deviation: ``axis == len(input_shape)`` passes the reference's check and then fails inside tf.transpose; here it
+    raises ValueError when the layer is built."""
+
+    def __init__(self, k=1, axis=-1, **kwargs):
+        self.k = k
+        self.axis = axis
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        if self.axis < 1 or self.axis > len(input_shape):
+            raise ValueError("axis must be 1~%d,now is %d" % (len(input_shape), self.axis))
+        if self.axis == len(input_shape):
+            raise ValueError("axis must be 1~%d,now is %d: axis %d is past the last axis of a %d-D input"
+                             % (len(input_shape) - 1, self.axis, self.axis, len(input_shape)))
+        if self.k < 1 or self.k > input_shape[self.axis]:
+            raise ValueError("k must be in 1 ~ %d,now k is %d" % (input_shape[self.axis], self.k))
+        self.dims = len(input_shape)
+        K.conv_stack_check(int(input_shape[self.axis]), 1, [("kmax", self.k)])
+        self.built = True
+
+    def stage(self):
+        return ("kmax", self.k)
+
+    def call(self, inputs, **kwargs):
+        shape = tuple(inputs.data.shape)
+        n = shape[self.axis]
+        inner = int(np.prod(shape[self.axis + 1:])) if self.axis + 1 < len(shape) else 1
+        out_shape = shape[:self.axis] + (self.k,) + shape[self.axis + 1:]
+        return ops.conv_stack(inputs, [self.stage()], n, inner, 1, out_shape)
+
+    def compute_output_shape(self, input_shape):
+        output_shape = list(input_shape)
+        output_shape[self.axis] = self.k
+        return tuple(output_shape)
+
+    def get_config(self):
+        config = {'k': self.k, 'axis': self.axis}
+        base = Layer.get_config(self)
+        base.update(config)
+        return base

@@ -13,6 +13,7 @@ from .ifm import IFM
 from .difm import DIFM
 from .onn import ONN
 from .edcn import EDCN
+from .ccpm import CCPM
 
 __all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM", "PNN",
-           "IFM", "DIFM", "ONN", "EDCN"]
+           "IFM", "DIFM", "ONN", "EDCN", "CCPM"]

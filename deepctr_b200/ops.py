@@ -947,6 +947,52 @@ def regulate(mode, x, h=None, ax=None, ah=None, gates=(), want_u=True):
     return (res[0] if want_u else None), (res[1:] if want_u else res)
 
 
+
+def conv_stack(x, stages, rows, dim, channels, out_shape):
+    """CCPM's Conv2D / KMaxPooling stages (deepctr/models/ccpm.py:58-70) on x viewed as [n, rows, dim, channels]
+    (n = the elements of x over rows * dim * channels), one b2ctr_conv_stack launch for all of them: every
+    (n, dim) column runs the whole stack on chip and only the last map is written, as a new [n, k * dim * C] tensor
+    reshaped to ``out_shape``.  ``stages``: ("conv", width, filters, activation, kernel Weight, bias Weight or None)
+    or ("kmax", k).  x is read in place when it is a window of a wider buffer (the gather buffer); the backward
+    recomputes the stack, adds dx to that buffer's gradient and sums the weight gradients in a fixed order."""
+    w_in = rows * dim * channels
+    src, _ = _rows2d(x) if x.data.dim() >= 2 else (None, 0)
+    if src is None or src.shape[1] != w_in:
+        src = E.contiguous(x).reshape(-1, w_in)
+    n = src.shape[0]
+    kst = [st if st[0] != "conv" else st[:4] + (_wdata(st[4]), _wdata(st[5]) if st[5] is not None else None)
+           for st in stages]
+    k_out, c_out = K.conv_stack_check(rows, channels, stages)
+    w_out = k_out * dim * c_out
+    y = _empty((n, w_out), src)
+    K.conv_stack_fwd(kst, src, rows, dim, channels, n, y)
+    res = E.Var(y.reshape(out_shape))
+    weights = [w for st in stages if st[0] == "conv" for w in st[4:] if w is not None]
+
+    def bwd(grads):
+        want_dw = [st[0] == "conv" and (st[4].requires_grad or (st[5] is not None and st[5].requires_grad))
+                   for st in stages]
+        if not (x.requires_grad or any(want_dw)):
+            return
+        g = grads[0].reshape(n, w_out)
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dxw, acc = (None, False)
+        if x.requires_grad:
+            dxw, acc = _grad_window(x, w_in) if src.shape[0] == x.data.shape[0] else (None, False)
+        dx = dxw if dxw is not None else (_empty((n, w_in), g) if x.requires_grad else None)
+        dws = K.conv_stack_bwd(kst, src, rows, dim, channels, n, g, dx=dx, dx_accumulate=acc, want_dw=want_dw)
+        if x.requires_grad and dxw is None:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        for st, d in zip(stages, dws):
+            if d is not None:
+                E.add_grad(st[4], d[0])
+                if d[1] is not None:
+                    E.add_grad(st[5], d[1])
+
+    E.record([res], [x] + weights, bwd)
+    return res
+
 CIN_CHUNK_BYTES = 24 << 20      # outer-product chunk kept well inside the 50 MB L2
 
 

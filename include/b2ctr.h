@@ -714,6 +714,51 @@ B2CTR_API size_t b2ctr_regulate_bwd_workspace_bytes(int32_t nfield, int32_t dim,
 B2CTR_API b2ctr_status_t b2ctr_regulate_bwd(const b2ctr_regulate_t* a, void* workspace, size_t workspace_bytes,
                                            void* stream);
 
+/* CCPM's convolution stack (deepctr/models/ccpm.py:58-70) over a [B, rows, dim, channels] view, run per column.
+ * Every stage keeps the embedding coordinate e apart, so each (sample, e) column is an independent 1-D signal over
+ * the rows carrying C channels; the whole stack runs on chip per column and only the last map is written.  Stages:
+ *   B2CTR_CONV_STAGE_CONV  Keras Conv2D with kernel (width, 1), strides (1, 1), padding 'same', channels_last:
+ *                          out[r, co] = act(bias[co] + sum_{t, ci} in[r + t - pb, ci] * kernel[t, ci, co]), a
+ *                          cross-correlation; rows outside [0, rows) read zero; pb = (width - 1) / 2 rows of padding
+ *                          before and width - 1 - pb after (TF's 'same'; width may exceed rows).  kernel is Keras'
+ *                          [width, 1, C_in, filters] as [width, C_in, filters]; bias [filters] or NULL.
+ *   B2CTR_CONV_STAGE_KMAX  KMaxPooling(k) along the rows (deepctr/layers/sequence.py:818-874): per channel the k
+ *                          largest values in descending order, equal values lower row first (tf.nn.top_k, sorted).
+ * Element (r, e, c) of the input is x[b * ldx + xcol + (r * dim + e) * channels + c]; the last map [k, dim, C] is
+ * written in Keras' Flatten order, (r * dim + e) * C + c from column outcol of a [B, ldout] buffer.
+ * Backward (the same descriptor; `out` now addresses the incoming gradient): the forward is recomputed per column,
+ * the gradient goes back through each k-max (to the selected rows only), activation and conv; dx is written (or
+ * added, dx_accumulate) in x's layout from column dxcol of a [B, lddx] buffer (NULL: not wanted).  The weight
+ * gradients dkernel / dbias (overwritten; NULL: not wanted) go through per-CTA partials in the workspace, each CTA
+ * adding its columns in a fixed order, then summed in CTA order: no float atomics, bit-identical from run to run.
+ * Nothing but the output is written by the forward, so the backward needs no saved state.
+ * Limits: 1 <= nstage <= B2CTR_CONV_STACK_MAX_STAGES, 1 <= rows <= 64, 1 <= channels, filters <= 16,
+ * 1 <= width <= 32, 1 <= k <= the rows it pools; and the backward's shared memory fits in 224 KB: 4 bytes times
+ * 2 * W + 32 * (M + 2 * G), with W the conv weights and biases of all stages (kept with their gradient sums), M the
+ * floats of every map of one column (the input, each conv output, each k-max output twice: values and rows) and G
+ * the largest map (the gradient ping-pong).  Anything else is INVALID_ARG. */
+enum { B2CTR_CONV_STAGE_CONV = 0, B2CTR_CONV_STAGE_KMAX = 1 };
+#define B2CTR_CONV_STACK_MAX_STAGES 8
+typedef struct b2ctr_conv_stage {
+  int32_t kind, width, filters, act, k, reserved;  /* width / filters / act: CONV; k: KMAX */
+  const float* kernel;                             /* [width, C_in, filters] */
+  const float* bias;                               /* [filters] or NULL */
+  float* dkernel; float* dbias;                    /* backward outputs or NULL */
+} b2ctr_conv_stage_t;
+typedef struct b2ctr_conv_stack {
+  int32_t struct_size;                             /* sizeof(b2ctr_conv_stack_t) */
+  int32_t nstage, rows, dim, channels, dx_accumulate;
+  int64_t batch;
+  const float* x; int64_t ldx, xcol;
+  float* out; int64_t ldout, outcol;               /* forward output / backward incoming gradient */
+  float* dx; int64_t lddx, dxcol;                  /* backward */
+  b2ctr_conv_stage_t stage[B2CTR_CONV_STACK_MAX_STAGES];
+} b2ctr_conv_stack_t;
+B2CTR_API b2ctr_status_t b2ctr_conv_stack_fwd(const b2ctr_conv_stack_t* a, void* stream);
+B2CTR_API size_t b2ctr_conv_stack_bwd_workspace_bytes(const b2ctr_conv_stack_t* a);
+B2CTR_API b2ctr_status_t b2ctr_conv_stack_bwd(const b2ctr_conv_stack_t* a, void* workspace, size_t workspace_bytes,
+                                             void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* 6. Sequence operators (DIN, pooling, Dice / BatchNormalization, dropout)                     */
 /* ------------------------------------------------------------------------------------------ */
