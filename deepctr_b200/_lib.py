@@ -131,6 +131,22 @@ class ConvStack(C.Structure):
                 ("dx", C.c_void_p), ("lddx", C.c_int64), ("dxcol", C.c_int64),
                 ("stage", ConvStage * CONV_STACK_MAX_STAGES)]
 
+FWBI_MAX_FIELDS, FWBI_MAX_GROUPS = 256, 8   # b2ctr.h B2CTR_FWBI_MAX_FIELDS / _GROUPS
+
+
+class FieldWiseBi(C.Structure):
+    """b2ctr_field_wise_bi_t"""
+    _fields_ = [("struct_size", C.c_int32), ("nfield", C.c_int32), ("ngroup", C.c_int32), ("dim", C.c_int32),
+                ("dx_accumulate", C.c_int32), ("reserved", C.c_int32), ("batch", C.c_int64),
+                ("x", C.c_void_p), ("ldx", C.c_int64),
+                ("col", C.c_int64 * FWBI_MAX_FIELDS), ("group", C.c_int32 * FWBI_MAX_FIELDS),
+                ("kernel_mf", C.c_void_p), ("kernel_fm", C.c_void_p), ("bias_mf", C.c_void_p), ("bias_fm", C.c_void_p),
+                ("out", C.c_void_p), ("ldout", C.c_int64), ("outcol", C.c_int64),
+                ("dx", C.c_void_p), ("lddx", C.c_int64),
+                ("dkernel_mf", C.c_void_p), ("dkernel_fm", C.c_void_p), ("dbias_mf", C.c_void_p),
+                ("dbias_fm", C.c_void_p)]
+
+
 _vp, _i32, _i64, _f32, _sz, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t, C.c_uint64
 
 # name -> (restype, argtypes).  Must list every symbol of include/b2ctr.h (tests check this).
@@ -244,6 +260,9 @@ SIGNATURES = {
     "b2ctr_conv_stack_fwd": (_i32, [C.POINTER(ConvStack), _vp]),
     "b2ctr_conv_stack_bwd_workspace_bytes": (_sz, [C.POINTER(ConvStack)]),
     "b2ctr_conv_stack_bwd": (_i32, [C.POINTER(ConvStack), _vp, _sz, _vp]),
+    "b2ctr_field_wise_bi_fwd": (_i32, [C.POINTER(FieldWiseBi), _vp]),
+    "b2ctr_field_wise_bi_bwd_workspace_bytes": (_sz, [C.POINTER(FieldWiseBi)]),
+    "b2ctr_field_wise_bi_bwd": (_i32, [C.POINTER(FieldWiseBi), _vp, _sz, _vp]),
     "b2ctr_ffm_product_fwd": (_i32, [C.POINTER(FfmField), _i32, _vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp]),
     "b2ctr_ffm_product_bwd": (_i32, [C.POINTER(FfmField), _i32, _vp, _i32, _i32, _vp, _i64, _i32, _i64, _vp]),
     "b2ctr_din_att_input_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),

@@ -2192,6 +2192,196 @@ __global__ void conv_stack_bwd_kernel(const b2ctr_conv_stack_t a, const __grid_c
     for (int i = threadIdx.x; i < P.nw; i += blockDim.x) partial[(int64_t)blockIdx.x * P.nw + i] = sacc[i];
 }
 
+// ------------------------------------------------------------------------------------------------
+// FLEN's FieldWiseBiInteraction (b2ctr_field_wise_bi_fwd / _bwd in include/b2ctr.h).  A CTA is R row lanes of
+// Gc = dim / V column groups; thread (r, j) owns the V columns [j * V, j * V + V) of every row it visits, so each
+// thread forms S_g and S_g^2 - Q_g of its columns in registers from the members of every group, read in place
+// through the per-field columns (sorted by group on the host).  Arrays over groups are indexed by compile-time
+// g < kFwbiMaxG only (unrolled, guarded by the runtime G), so they stay in registers.
+// * fwbi_fwd_kernel: row blocks of R rows, grid-stride; writes only h.
+// * fwbi_bwd_kernel: CTA = one batch chunk walked in ascending row order; dx has one owner per element; the
+//   weight-gradient sums stay in registers, then the CTA adds its threads (and row lanes, for the biases) in a
+//   fixed order into its partial.  ordered_sum_kernel adds the partials in CTA order: bit-identical from run to run.
+// ------------------------------------------------------------------------------------------------
+constexpr int kFwbiMaxG = B2CTR_FWBI_MAX_GROUPS;
+constexpr int kFwbiMaxP = kFwbiMaxG * (kFwbiMaxG - 1) / 2;
+constexpr int kFwbiMaxE = 256;
+constexpr int kFwbiThreads = 256;
+
+struct FwbiArgs {
+  int F, G, E, dx_accumulate;
+  int64_t batch;
+  const float* x; int64_t ldx;
+  const float* kmf; const float* kfm; const float* bmf; const float* bfm;
+  float* out; int64_t ldout, outcol;
+  float* dx; int64_t lddx;
+  int start[kFwbiMaxG + 1];                  // the members of group g are cols[start[g] .. start[g + 1])
+  int cols[B2CTR_FWBI_MAX_FIELDS];
+};
+
+// index of pair (g, h), g < h, in itertools.combinations(range(G), 2) order
+__device__ __forceinline__ int fwbi_pair(int g, int h, int G) { return g * (2 * G - g - 1) / 2 + h - g - 1; }
+
+__device__ __forceinline__ void fwbi_stage_weights(const FwbiArgs& a, float* skmf, float* skfm) {
+  const int P = a.G * (a.G - 1) / 2;
+  for (int i = threadIdx.x; i < P; i += blockDim.x) skmf[i] = a.kmf[i];
+  for (int i = threadIdx.x; i < a.G; i += blockDim.x) skfm[i] = a.kfm[i];
+  __syncthreads();
+}
+
+// S[g] = sum of the members of group g and, through fm(g, v, S_g^2 - Q_g), the FM term of each group, for the V
+// columns at xr
+template <int V, class Fm>
+__device__ __forceinline__ void fwbi_sums(const FwbiArgs& a, const float* xr, float (&S)[kFwbiMaxG][V], Fm fm) {
+#pragma unroll
+  for (int g = 0; g < kFwbiMaxG; ++g) {
+    float s[V], q[V];
+#pragma unroll
+    for (int v = 0; v < V; ++v) s[v] = q[v] = 0.f;
+    if (g < a.G) {
+      for (int i = a.start[g]; i < a.start[g + 1]; ++i) {
+        float t[V];
+        reg_ld<V>(xr + a.cols[i], t);
+#pragma unroll
+        for (int v = 0; v < V; ++v) s[v] += t[v], q[v] = fmaf(t[v], t[v], q[v]);
+      }
+#pragma unroll
+      for (int v = 0; v < V; ++v) fm(g, v, fmaf(s[v], s[v], -q[v]));
+    }
+#pragma unroll
+    for (int v = 0; v < V; ++v) S[g][v] = s[v];
+  }
+}
+
+template <int V>
+__global__ void __launch_bounds__(kFwbiThreads, 2) fwbi_fwd_kernel(const __grid_constant__ FwbiArgs a) {
+  __shared__ float skmf[kFwbiMaxP], skfm[kFwbiMaxG];
+  fwbi_stage_weights(a, skmf, skfm);
+  const int Gc = a.E / V, R = kFwbiThreads / Gc, r = threadIdx.x / Gc, c = (threadIdx.x - r * Gc) * V;
+  if (r >= R) return;
+  float bm[V], bf[V];
+#pragma unroll
+  for (int v = 0; v < V; ++v) bm[v] = a.bmf ? a.bmf[c + v] : 0.f, bf[v] = a.bfm ? a.bfm[c + v] : 0.f;
+  for (int64_t b = (int64_t)blockIdx.x * R + r; b < a.batch; b += (int64_t)gridDim.x * R) {
+    float S[kFwbiMaxG][V], hmf[V], hfm[V];
+#pragma unroll
+    for (int v = 0; v < V; ++v) hmf[v] = hfm[v] = 0.f;
+    fwbi_sums<V>(a, a.x + b * a.ldx + c, S, [&](int g, int v, float d) { hfm[v] = fmaf(d, skfm[g], hfm[v]); });
+#pragma unroll
+    for (int g = 0; g < kFwbiMaxG; ++g) {
+#pragma unroll
+      for (int h = g + 1; h < kFwbiMaxG; ++h) {
+        if (h < a.G) {
+          const float k = skmf[fwbi_pair(g, h, a.G)];
+#pragma unroll
+          for (int v = 0; v < V; ++v) hmf[v] = fmaf(S[g][v] * S[h][v], k, hmf[v]);
+        }
+      }
+    }
+    float y[V];
+#pragma unroll
+    for (int v = 0; v < V; ++v) y[v] = (hmf[v] + bm[v]) + (hfm[v] + bf[v]);
+    reg_st<V>(a.out + b * a.ldout + a.outcol + c, y);
+  }
+}
+
+template <int V>
+__global__ void __launch_bounds__(kFwbiThreads, 2)
+    fwbi_bwd_kernel(const __grid_constant__ FwbiArgs a, int nchunk, float* partial, int pitch) {
+  __shared__ float skmf[kFwbiMaxP], skfm[kFwbiMaxG];
+  __shared__ float sred[(kFwbiMaxP + kFwbiMaxG) * kFwbiThreads];
+  __shared__ float sbias[kFwbiThreads * 4];
+  fwbi_stage_weights(a, skmf, skfm);
+  const int G = a.G, Gc = a.E / V, R = kFwbiThreads / Gc, r = threadIdx.x / Gc, c = (threadIdx.x - r * Gc) * V;
+  const bool active = r < R;
+  const int64_t per = (a.batch + nchunk - 1) / nchunk, lo = (int64_t)blockIdx.x * per, hi = min(a.batch, lo + per);
+  float amf[kFwbiMaxP], afm[kFwbiMaxG], adb[V];
+#pragma unroll
+  for (int k = 0; k < kFwbiMaxP; ++k) amf[k] = 0.f;
+#pragma unroll
+  for (int g = 0; g < kFwbiMaxG; ++g) afm[g] = 0.f;
+#pragma unroll
+  for (int v = 0; v < V; ++v) adb[v] = 0.f;
+  if (active) {
+    for (int64_t b = lo + r; b < hi; b += R) {
+      const float* xr = a.x + b * a.ldx + c;
+      float S[kFwbiMaxG][V], dh[V];
+      reg_ld<V>(a.out + b * a.ldout + a.outcol + c, dh);
+      fwbi_sums<V>(a, xr, S, [&](int g, int v, float d) { afm[g] = fmaf(dh[v], d, afm[g]); });
+#pragma unroll
+      for (int v = 0; v < V; ++v) adb[v] += dh[v];
+#pragma unroll
+      for (int g = 0, k = 0; g < kFwbiMaxG; ++g) {
+#pragma unroll
+        for (int h = g + 1; h < kFwbiMaxG; ++h, ++k) {
+#pragma unroll
+          for (int v = 0; v < V; ++v) amf[k] = fmaf(dh[v], S[g][v] * S[h][v], amf[k]);
+        }
+      }
+      if (!a.dx) continue;
+#pragma unroll
+      for (int g = 0; g < kFwbiMaxG; ++g) {
+        if (g >= G) break;
+        const float two_fm = 2.f * skfm[g];
+        float t[V];
+#pragma unroll
+        for (int v = 0; v < V; ++v) t[v] = two_fm * S[g][v];
+#pragma unroll
+        for (int h = 0; h < kFwbiMaxG; ++h) {
+          if (h != g && h < G) {
+            const float k = skmf[h < g ? fwbi_pair(h, g, G) : fwbi_pair(g, h, G)];
+#pragma unroll
+            for (int v = 0; v < V; ++v) t[v] = fmaf(k, S[h][v], t[v]);
+          }
+        }
+        for (int i = a.start[g]; i < a.start[g + 1]; ++i) {
+          float xv[V], d[V];
+          reg_ld<V>(xr + a.cols[i], xv);
+#pragma unroll
+          for (int v = 0; v < V; ++v) d[v] = dh[v] * (t[v] - two_fm * xv[v]);
+          float* p = a.dx + b * a.lddx + a.cols[i] + c;
+          if (a.dx_accumulate) {
+            float o[V];
+            reg_ld<V>(p, o);
+#pragma unroll
+            for (int v = 0; v < V; ++v) d[v] += o[v];
+          }
+          reg_st<V>(p, d);
+        }
+      }
+    }
+  }
+  if (!partial) return;
+  // the sums in combinations order, then the groups, then the columns: k-th entry of thread t at sred[k * 256 + t]
+  const int P = G * (G - 1) / 2;
+#pragma unroll
+  for (int g = 0, k = 0; g < kFwbiMaxG; ++g) {
+    if (g < G) sred[(P + g) * kFwbiThreads + threadIdx.x] = afm[g];
+#pragma unroll
+    for (int h = g + 1; h < kFwbiMaxG; ++h, ++k)
+      if (h < G) sred[fwbi_pair(g, h, G) * kFwbiThreads + threadIdx.x] = amf[k];
+  }
+  if (active) {
+#pragma unroll
+    for (int v = 0; v < V; ++v) sbias[r * a.E + c + v] = adb[v];
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < P + G + a.E; k += blockDim.x) {
+    float s = 0.f;
+    if (k < P + G) {
+      for (int t = 0; t < kFwbiThreads; ++t) s += sred[k * kFwbiThreads + t];
+    } else {
+      for (int rr = 0; rr < R; ++rr) s += sbias[rr * a.E + k - P - G];
+    }
+    partial[(int64_t)blockIdx.x * pitch + k] = s;
+  }
+}
+
+// backward batch chunks: at least 128 samples each, about 4 CTAs per SM in all
+static inline int fwbi_chunks(int64_t batch) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(batch, 128), (int64_t)kNumSMs * 4));
+}
+
 }  // namespace b2ctr
 
 using namespace b2ctr;
@@ -3055,6 +3245,125 @@ b2ctr_status_t b2ctr_conv_stack_bwd(const b2ctr_conv_stack_t* a, void* workspace
       ordered_sum_kernel<<<1, 32, 0, ST>>>(partial + p.w_off + nk, P.nw, nblk, p.cout, a->stage[s].dbias);
       B2_CHECK_LAUNCH("b2ctr_conv_stack_bwd(dbias)");
     }
+  }
+  return B2CTR_OK;
+}
+
+// ---- FLEN's FieldWiseBiInteraction ----------------------------------------------------------------
+static bool fwbi_aligned(const void* p, int64_t ld) { return !p || (((uintptr_t)p & 15) == 0 && ld % 4 == 0); }
+
+// the checks the forward and the backward share, and the kernels' arguments (the fields sorted by group)
+static b2ctr_status_t fwbi_args(const b2ctr_field_wise_bi_t* a, const char* what, FwbiArgs* k, bool* vec) {
+  B2_REQUIRE(a, "%s: NULL descriptor", what);
+  B2_REQUIRE(a->struct_size == (int32_t)sizeof(b2ctr_field_wise_bi_t), "%s: struct_size %d, expected %d", what,
+             a->struct_size, (int)sizeof(b2ctr_field_wise_bi_t));
+  B2_REQUIRE(a->ngroup >= 2 && a->ngroup <= kFwbiMaxG, "%s: needs 2 <= groups <= %d (got %d)", what, kFwbiMaxG,
+             a->ngroup);
+  B2_REQUIRE(a->nfield >= a->ngroup && a->nfield <= B2CTR_FWBI_MAX_FIELDS, "%s: needs groups <= fields <= %d (got %d)",
+             what, B2CTR_FWBI_MAX_FIELDS, a->nfield);
+  B2_REQUIRE(a->dim >= 1 && a->dim <= kFwbiMaxE, "%s: needs 1 <= embedding_size <= %d (got %d)", what, kFwbiMaxE,
+             a->dim);
+  B2_REQUIRE(a->batch >= 0, "%s: negative batch", what);
+  B2_REQUIRE(a->x && a->ldx >= a->dim && a->ldx < ((int64_t)1 << 31), "%s: x is NULL or its pitch is out of range",
+             what);
+  B2_REQUIRE(a->kernel_mf && a->kernel_fm, "%s: NULL kernel_mf / kernel_fm", what);
+  B2_REQUIRE(a->out && a->outcol >= 0 && a->ldout >= a->outcol + a->dim, "%s: out is NULL or its window does not fit",
+             what);
+  *k = FwbiArgs{};
+  int count[kFwbiMaxG + 1] = {0};
+  bool cols4 = true;
+  for (int f = 0; f < a->nfield; ++f) {
+    B2_REQUIRE(a->group[f] >= 0 && a->group[f] < a->ngroup, "%s: field %d: group %d outside [0, %d)", what, f,
+               a->group[f], a->ngroup);
+    B2_REQUIRE(a->col[f] >= 0 && a->col[f] + a->dim <= a->ldx, "%s: field %d: column %lld does not fit the row", what,
+               f, (long long)a->col[f]);
+    ++count[a->group[f] + 1];
+    cols4 = cols4 && a->col[f] % 4 == 0;
+  }
+  for (int g = 0; g < a->ngroup; ++g) {
+    B2_REQUIRE(count[g + 1] > 0, "%s: group %d has no field", what, g);
+    k->start[g + 1] = k->start[g] + count[g + 1];
+  }
+  int fill[kFwbiMaxG];
+  for (int g = 0; g < a->ngroup; ++g) fill[g] = k->start[g];
+  for (int f = 0; f < a->nfield; ++f) k->cols[fill[a->group[f]]++] = (int)a->col[f];
+  k->F = a->nfield, k->G = a->ngroup, k->E = a->dim, k->dx_accumulate = a->dx_accumulate != 0;
+  k->batch = a->batch;
+  k->x = a->x, k->ldx = a->ldx;
+  k->kmf = a->kernel_mf, k->kfm = a->kernel_fm, k->bmf = a->bias_mf, k->bfm = a->bias_fm;
+  k->out = a->out, k->ldout = a->ldout, k->outcol = a->outcol;
+  k->dx = a->dx, k->lddx = a->lddx;
+  *vec = a->dim % 4 == 0 && cols4 && fwbi_aligned(a->x, a->ldx) && fwbi_aligned(a->out + a->outcol, a->ldout) &&
+         fwbi_aligned(a->dx, a->lddx);
+  return B2CTR_OK;
+}
+
+static inline int fwbi_pitch(const b2ctr_field_wise_bi_t* a) {
+  return a->ngroup * (a->ngroup - 1) / 2 + a->ngroup + a->dim;
+}
+
+b2ctr_status_t b2ctr_field_wise_bi_fwd(const b2ctr_field_wise_bi_t* a, void* stream) {
+  FwbiArgs k;
+  bool vec;
+  const b2ctr_status_t st = fwbi_args(a, "field_wise_bi_fwd", &k, &vec);
+  if (st != B2CTR_OK) return st;
+  if (a->batch == 0) return B2CTR_OK;
+  const int V = vec ? 4 : 1, R = kFwbiThreads / (a->dim / V);
+  const int grid = grid_for(ceil_div(a->batch, R), 1, 8);
+  if (vec)
+    fwbi_fwd_kernel<4><<<grid, kFwbiThreads, 0, ST>>>(k);
+  else
+    fwbi_fwd_kernel<1><<<grid, kFwbiThreads, 0, ST>>>(k);
+  B2_CHECK_LAUNCH("b2ctr_field_wise_bi_fwd");
+  return B2CTR_OK;
+}
+
+size_t b2ctr_field_wise_bi_bwd_workspace_bytes(const b2ctr_field_wise_bi_t* a) {
+  FwbiArgs k;
+  bool vec;
+  if (fwbi_args(a, "field_wise_bi_bwd_workspace_bytes", &k, &vec) != B2CTR_OK || a->batch <= 0) return 0;
+  return (size_t)fwbi_chunks(a->batch) * fwbi_pitch(a) * sizeof(float);
+}
+
+b2ctr_status_t b2ctr_field_wise_bi_bwd(const b2ctr_field_wise_bi_t* a, void* workspace, size_t workspace_bytes,
+                                       void* stream) {
+  FwbiArgs k;
+  bool vec;
+  const b2ctr_status_t st = fwbi_args(a, "field_wise_bi_bwd", &k, &vec);
+  if (st != B2CTR_OK) return st;
+  if (a->dx)
+    for (int f = 0; f < a->nfield; ++f)
+      B2_REQUIRE(a->col[f] + a->dim <= a->lddx, "field_wise_bi_bwd: field %d does not fit a row of dx", f);
+  const int P = a->ngroup * (a->ngroup - 1) / 2;
+  const bool want_dw = a->dkernel_mf || a->dkernel_fm || a->dbias_mf || a->dbias_fm;
+  B2_REQUIRE(a->dx || want_dw, "field_wise_bi_bwd: nothing to compute");
+  if (a->batch == 0) {
+    // no sample: the weight gradients are zero
+    if (a->dkernel_mf) cudaMemsetAsync(a->dkernel_mf, 0, sizeof(float) * P, ST);
+    if (a->dkernel_fm) cudaMemsetAsync(a->dkernel_fm, 0, sizeof(float) * a->ngroup, ST);
+    if (a->dbias_mf) cudaMemsetAsync(a->dbias_mf, 0, sizeof(float) * a->dim, ST);
+    if (a->dbias_fm) cudaMemsetAsync(a->dbias_fm, 0, sizeof(float) * a->dim, ST);
+    return B2CTR_OK;
+  }
+  const int nchunk = fwbi_chunks(a->batch), pitch = fwbi_pitch(a);
+  const size_t need = want_dw ? (size_t)nchunk * pitch * sizeof(float) : 0;
+  if (want_dw && (!workspace || workspace_bytes < need)) {
+    set_error("field_wise_bi_bwd: needs %zu workspace bytes, got %zu", need, workspace_bytes);
+    return B2CTR_ERR_WORKSPACE;
+  }
+  float* partial = want_dw ? (float*)workspace : nullptr;
+  if (vec)
+    fwbi_bwd_kernel<4><<<nchunk, kFwbiThreads, 0, ST>>>(k, nchunk, partial, pitch);
+  else
+    fwbi_bwd_kernel<1><<<nchunk, kFwbiThreads, 0, ST>>>(k, nchunk, partial, pitch);
+  B2_CHECK_LAUNCH("b2ctr_field_wise_bi_bwd");
+  const struct { float* out; int off, count; } sums[4] = {
+      {a->dkernel_mf, 0, P}, {a->dkernel_fm, P, a->ngroup}, {a->dbias_mf, P + a->ngroup, a->dim},
+      {a->dbias_fm, P + a->ngroup, a->dim}};
+  for (const auto& s : sums) {
+    if (!s.out) continue;
+    ordered_sum_kernel<<<grid_for(s.count, 256, 8), 256, 0, ST>>>(partial + s.off, pitch, nchunk, s.count, s.out);
+    B2_CHECK_LAUNCH("b2ctr_field_wise_bi_bwd(reduce)");
   }
   return B2CTR_OK;
 }

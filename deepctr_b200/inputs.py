@@ -370,6 +370,8 @@ class EmbeddingPlanner(object):
         self.regulate_plan = _plan_regulate(model, consumers, out_ids)
         # CCPM's Lambda(expand_dims) -> [Conv2D -> KMaxPooling(axis=1)] x l -> Flatten: one b2ctr_conv_stack launch
         self.conv_plan = _plan_conv_stack(model, consumers, out_ids)
+        # FLEN's FieldWiseBiInteraction on concatenations of gather-buffer windows: one launch reading them in place
+        self.field_wise_plan = _plan_field_wise(model, consumers, out_ids, self.main)
         # IFM / DIFM scale the linear lookups by per-sample field weights before Linear sums them: their rows are
         # needed, so they are never fused into the gather's row-sum (lin_hint)
         from .layers.utils import RefineWeight
@@ -650,6 +652,8 @@ class EmbeddingPlanner(object):
             for vn in s.virtual_nodes:
                 if vn is not s.node:
                     self.results[id(vn)] = VIRTUAL
+        for node in self.field_wise_plan.virtual:      # never formed: a Var without data
+            self.results[id(node)] = E.Var(None, vshape=(batch,) + tuple(node.outputs[0].shape[1:]))
         if grad:
             outs = [b for b in bufs.values()]
             if self.fm_result is not None:
@@ -917,6 +921,14 @@ class EmbeddingPlanner(object):
             self.results[id(n)] = VIRTUAL
         self.results[id(last)] = res
         return VIRTUAL
+
+    def field_wise_groups(self, layer):
+        """FieldWiseBiInteraction ``layer`` the planner claimed (FieldWisePlan): its groups as lists of this step's
+        gather-buffer windows, to be read in place (the groups' concatenations are Vars without data).  Else None."""
+        groups = self.field_wise_plan.groups.get(id(layer))
+        if groups is None:
+            return None
+        return [[self.results[id(n)] for n in g] for g in groups]
 
     def append_dense(self, emb_flat, dense_flat):
         """combined_dnn_input: place the dense features behind the embeddings (and PNN's placed products) in the
@@ -1279,6 +1291,63 @@ def _plan_conv_stack(model, consumers, out_ids):
             continue
         chains[id(chain[0].layer)] = chain
     return ConvStackPlan(chains)
+
+
+class FieldWisePlan(object):
+    """FLEN's FieldWiseBiInteraction (deepctr/models/flen.py:69-70) served in place: a FieldWiseBiInteraction called
+    once, whose every input is concat_func(members, axis=1) (a Concat, or NoMask for a one-member group) of
+    embedding or pooled windows of the gather buffer, each concatenation used by that layer only, runs as one
+    b2ctr_field_wise_bi launch reading the members where the gather wrote them.  The concatenations are never
+    formed (their results are Vars without data), whether or not a group's members are adjacent.
+
+    ``groups`` {id(layer): [[member slot node, ...] per group]}, ``virtual`` the concatenation nodes.  Decided
+    once from the model's graph; any other graph runs the layer on its concrete inputs, on the same kernel."""
+
+    def __init__(self, groups, virtual):
+        self.groups = groups
+        self.virtual = virtual
+
+
+def _plan_field_wise(model, consumers, out_ids, main_slots):
+    from .layers.interaction import FieldWiseBiInteraction
+    from .layers.utils import Concat, NoMask
+    slot_out = {id(s.node.outputs[0]): s.node for s in main_slots}
+    calls = defaultdict(int)
+    for node in model._order:
+        calls[id(node.layer)] += 1
+    groups, virtual = {}, []
+    for node in model._order:
+        if not isinstance(node.layer, FieldWiseBiInteraction) or calls[id(node.layer)] != 1:
+            continue
+        if not isinstance(node.inputs, (list, tuple)) or len(node.inputs) < 2:
+            continue
+        plan, concats = [], []
+        for t in node.inputs:
+            src = t.node
+            if id(t) in out_ids or len(consumers[id(t)]) != 1:
+                break
+            if isinstance(src.layer, Concat) and src.layer.axis in (1, -2):
+                members = E._flatten(src.inputs)
+            elif isinstance(src.layer, NoMask) and isinstance(src.inputs, E.KTensor):
+                members = [src.inputs]
+            else:
+                break
+            if not all(id(m) in slot_out and len(m.shape) == 3 for m in members):
+                break
+            plan.append([slot_out[id(m)] for m in members])
+            concats.append(src)
+        else:
+            dims = set(int(n.outputs[0].shape[-1]) for g in plan for n in g)
+            nfield = sum(int(n.outputs[0].shape[1]) for g in plan for n in g)
+            try:
+                K.field_wise_bi_check(nfield, len(plan), dims.pop())
+            except ValueError:
+                continue
+            if dims:
+                continue
+            groups[id(node.layer)] = plan
+            virtual += concats
+    return FieldWisePlan(groups, virtual)
 
 
 class FieldAwarePlan(object):

@@ -1110,6 +1110,74 @@ def conv_stack_bwd(stages, x, rows, dim, channels, batch, dout, dx=None, dx_accu
     L.check(L.lib().b2ctr_conv_stack_bwd(C.byref(a), ptr(ws), nbytes, stream()), "conv_stack_bwd")
     return dws
 
+# limits of b2ctr_field_wise_bi_fwd / _bwd (include/b2ctr.h)
+FWBI_MAX_DIM = 256
+
+
+def field_wise_bi_check(nfield, ngroup, dim):
+    """Raise ValueError naming the limit of b2ctr_field_wise_bi that nfield fields in ngroup groups of dim
+    coordinates break."""
+    if not 2 <= ngroup <= L.FWBI_MAX_GROUPS:
+        raise ValueError("FieldWiseBiInteraction supports 2 to %d groups (FWBI_MAX_GROUPS), got %d"
+                         % (L.FWBI_MAX_GROUPS, ngroup))
+    if not ngroup <= nfield <= L.FWBI_MAX_FIELDS:
+        raise ValueError("FieldWiseBiInteraction supports at most %d fields in all (FWBI_MAX_FIELDS), got %d"
+                         % (L.FWBI_MAX_FIELDS, nfield))
+    if not 1 <= dim <= FWBI_MAX_DIM:
+        raise ValueError("FieldWiseBiInteraction supports embedding_size 1 to %d (FWBI_MAX_DIM), got %d"
+                         % (FWBI_MAX_DIM, dim))
+
+
+def _fwbi_desc(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm, bias_mf, bias_fm, out, outcol):
+    """b2ctr_field_wise_bi_t: field f is the [dim] row at column cols[f] of x (a 2-D [B, ld] view read in place,
+    pitch stride(0)) in group groups[f]; ``out`` a 2-D view whose columns [outcol, outcol + dim) are h (forward)
+    or dh (backward)."""
+    _require_cuda(x, kernel_mf, kernel_fm, bias_mf, bias_fm, out)
+    a = L.FieldWiseBi()
+    a.struct_size = C.sizeof(L.FieldWiseBi)
+    a.nfield, a.ngroup, a.dim, a.batch = len(cols), ngroup, dim, batch
+    if len(cols) > L.FWBI_MAX_FIELDS:
+        raise ValueError("FieldWiseBiInteraction supports at most %d fields in all (FWBI_MAX_FIELDS), got %d"
+                         % (L.FWBI_MAX_FIELDS, len(cols)))
+    for f, (c, g) in enumerate(zip(cols, groups)):
+        a.col[f], a.group[f] = c, g
+    a.x, a.ldx = x.data_ptr(), x.stride(0)
+    a.kernel_mf, a.kernel_fm = kernel_mf.data_ptr(), kernel_fm.data_ptr()
+    a.bias_mf = bias_mf.data_ptr() if bias_mf is not None else None
+    a.bias_fm = bias_fm.data_ptr() if bias_fm is not None else None
+    a.out, a.ldout, a.outcol = out.data_ptr(), out.stride(0), outcol
+    return a
+
+
+def field_wise_bi_fwd(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm, bias_mf, bias_fm, out, outcol=0):
+    """FLEN's FieldWiseBiInteraction in one launch (b2ctr_field_wise_bi_fwd): reads the fields in place and writes
+    only h into the columns [outcol, outcol + dim) of ``out``."""
+    a = _fwbi_desc(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm, bias_mf, bias_fm, out, outcol)
+    L.check(L.lib().b2ctr_field_wise_bi_fwd(C.byref(a), stream()), "field_wise_bi_fwd")
+    return out
+
+
+def field_wise_bi_bwd(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm, bias_mf, bias_fm, dout, doutcol=0,
+                      dx=None, dx_accumulate=False, want_dkernel=(False, False), want_dbias=(False, False)):
+    """Recompute the forward and take its gradient (b2ctr_field_wise_bi_bwd): ``dx`` a 2-D view whose columns
+    cols[f] take (or, with ``dx_accumulate``, add) field f's gradient, or None.  Returns (dkernel_mf [P, 1],
+    dkernel_fm [G, 1], dbias_mf [dim], dbias_fm [dim]), None where not wanted."""
+    a = _fwbi_desc(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm, bias_mf, bias_fm, dout, doutcol)
+    if dx is not None:
+        _require_cuda(dx)
+        a.dx, a.lddx, a.dx_accumulate = dx.data_ptr(), dx.stride(0), int(bool(dx_accumulate))
+    dev = x.device
+    shapes = ((ngroup * (ngroup - 1) // 2, 1), (ngroup, 1), (dim,), (dim,))
+    res = [torch.empty(sh, dtype=torch.float32, device=dev) if w else None
+           for sh, w in zip(shapes, tuple(want_dkernel) + tuple(want_dbias))]
+    a.dkernel_mf, a.dkernel_fm, a.dbias_mf, a.dbias_fm = [t.data_ptr() if t is not None else None for t in res]
+    nbytes = (L.lib().b2ctr_field_wise_bi_bwd_workspace_bytes(C.byref(a))
+              if any(t is not None for t in res) else 0)
+    ws = workspace(nbytes, dev)
+    L.check(L.lib().b2ctr_field_wise_bi_bwd(C.byref(a), ptr(ws), nbytes, stream()), "field_wise_bi_bwd")
+    return tuple(res)
+
+
 def din_att_input_fwd(q, ldq, keys, ldk, batch, T, E):
     out = torch.empty((batch, T, 4 * E), dtype=torch.float32, device=q.device)
     _lib_call("din_att_input_fwd", ptr(q), ldq, ptr(keys), ldk, ptr(out), batch, T, E, stream())
@@ -1348,5 +1416,5 @@ for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filte
 
 
 for _n in ("mha_fwd", "mha_bwd", "layernorm_fwd", "layernorm_bwd", "regulate_fwd", "regulate_bwd",
-           "conv_stack_fwd", "conv_stack_bwd"):
+           "conv_stack_fwd", "conv_stack_bwd", "field_wise_bi_fwd", "field_wise_bi_bwd"):
     globals()[_n] = _timed(globals()[_n])

@@ -3,7 +3,8 @@ from ..engine import Layer, Dense, Flatten, Reshape, Concatenate, Add, Lambda, I
 from .activation import Dice, Activation, activation_layer
 from .core import DNN, LocalActivationUnit, PredictionLayer, RegulationModule
 from .interaction import (AFMLayer, BiInteractionPooling, BilinearInteraction, FM, CrossNet, CIN, InteractingLayer,
-                          SENETLayer, FwFMLayer, FEFMLayer, InnerProductLayer, OutterProductLayer, BridgeModule)
+                          SENETLayer, FwFMLayer, FEFMLayer, InnerProductLayer, OutterProductLayer, BridgeModule,
+                          FieldWiseBiInteraction)
 from .normalization import BatchNormalization, Dropout, LayerNormalization
 from .sequence import (SequencePoolingLayer, WeightedSequenceLayer, AttentionSequencePoolingLayer, Transformer,
                        PositionEncoding, KMaxPooling)
@@ -22,4 +23,5 @@ custom_objects = {
     'Linear': Linear, 'Concat': Concat, 'NoMask': NoMask, '_Add': _Add,
     'Transformer': Transformer, 'PositionEncoding': PositionEncoding, 'LayerNormalization': LayerNormalization,
     'RegulationModule': RegulationModule, 'BridgeModule': BridgeModule, 'KMaxPooling': KMaxPooling,
+    'FieldWiseBiInteraction': FieldWiseBiInteraction,
 }

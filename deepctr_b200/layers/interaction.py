@@ -1,15 +1,17 @@
 """Host mirror of deepctr/layers/interaction.py for the operators on the hot path:
 AFMLayer (:39-160), BiInteractionPooling (:163-206), FM (:563-607), CrossNet (:344-435), CIN (:209-341),
 InteractingLayer (:697-790), SENETLayer (:1067-1139), BilinearInteraction (:1142-1221), FwFMLayer (:1350-1425),
-FEFMLayer (:1428-1499), InnerProductLayer (:610-695), OutterProductLayer (:793-931), BridgeModule (:1502-1570).
+FEFMLayer (:1428-1499), InnerProductLayer (:610-695), OutterProductLayer (:793-931), BridgeModule (:1502-1570),
+FieldWiseBiInteraction (:1224-1348).
 Same constructor arguments, weight names, shape checks and error messages as the reference."""
 import itertools
 
 import torch
 
 from .. import engine as E
+from .. import kernels as K
 from .. import ops
-from ..engine import Layer, Lambda, Zeros, glorot_normal, glorot_uniform, TruncatedNormal, l2
+from ..engine import Layer, Lambda, Zeros, Ones, Constant, glorot_normal, glorot_uniform, TruncatedNormal, l2
 from .normalization import Dropout
 
 # shapes the fused AFM kernels serve (include/b2ctr.h, b2ctr_afm_fwd)
@@ -713,3 +715,55 @@ class BridgeModule(Layer):
         config = {'bridge_type': self.bridge_type, 'activation': self.activation}
         config.update(base)
         return config
+
+
+class FieldWiseBiInteraction(Layer):
+    """FLEN's Field-Wise Bi-Interaction, deepctr/layers/interaction.py:1224-1348.  Called on a list of G >= 2
+    [B, F_g, E] tensors (the field groups); output [B, E] =
+      sum_{g<h} kernel_mf[p] * S_g * S_h + bias_mf + sum_g kernel_fm[g] * (S_g^2 - Q_g) + bias_fm
+    with S_g / Q_g the sum / sum of squares of group g's fields.  One b2ctr_field_wise_bi launch: the groups are read
+    wherever they are when they are windows of one buffer, else copied once into one [B, F, E] buffer.  In FLEN
+    the planner (inputs.FieldWisePlan) hands it the group members, windows of the gather buffer, so the groups'
+    concatenations are never written."""
+
+    def __init__(self, use_bias=True, seed=1024, **kwargs):
+        self.use_bias = use_bias
+        self.seed = seed
+        Layer.__init__(self, **kwargs)
+
+    def build(self, input_shape):
+        if not isinstance(input_shape, list) or len(input_shape) < 2:
+            raise ValueError('A `Field-Wise Bi-Interaction` layer should be called '
+                             'on a list of at least 2 inputs')
+        self.num_fields = len(input_shape)
+        embedding_size = int(input_shape[0][-1])
+        nfield = sum(int(s[1]) for s in input_shape if len(s) == 3)
+        K.field_wise_bi_check(nfield, self.num_fields, embedding_size)
+        self.kernel_mf = self.add_weight(name='kernel_mf', shape=(int(self.num_fields * (self.num_fields - 1) / 2), 1),
+                                         initializer=Ones(), regularizer=None, trainable=True)
+        self.kernel_fm = self.add_weight(name='kernel_fm', shape=(self.num_fields, 1), initializer=Constant(value=0.5),
+                                         regularizer=None, trainable=True)
+        if self.use_bias:
+            self.bias_mf = self.add_weight(name='bias_mf', shape=(embedding_size,), initializer=Zeros())
+            self.bias_fm = self.add_weight(name='bias_fm', shape=(embedding_size,), initializer=Zeros())
+        self.built = True
+
+    def call(self, inputs, **kwargs):
+        bias = (self.bias_mf, self.bias_fm) if self.use_bias else (None, None)
+        planner = getattr(self, "_planner", None)
+        groups = planner.field_wise_groups(self) if planner is not None else None
+        if groups is None:
+            if inputs[0].data.dim() != 3:
+                raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions"
+                                 % (inputs[0].data.dim()))
+            groups = [[x] for x in inputs]
+        return ops.field_wise_bi(groups, self.kernel_mf, self.kernel_fm, *bias)
+
+    def compute_output_shape(self, input_shape):
+        return (None, input_shape[0][-1])
+
+    def get_config(self):
+        config = {'use_bias': self.use_bias, 'seed': self.seed}
+        base_config = Layer.get_config(self).copy()
+        base_config.update(config)
+        return base_config

@@ -14,6 +14,7 @@ from .difm import DIFM
 from .onn import ONN
 from .edcn import EDCN
 from .ccpm import CCPM
+from .flen import FLEN
 
 __all__ = ["DeepFM", "xDeepFM", "DCN", "AutoInt", "DIN", "NFM", "AFM", "FiBiNET", "BST", "FwFM", "DeepFEFM", "PNN",
-           "IFM", "DIFM", "ONN", "EDCN", "CCPM"]
+           "IFM", "DIFM", "ONN", "EDCN", "CCPM", "FLEN"]

@@ -993,6 +993,67 @@ def conv_stack(x, stages, rows, dim, channels, out_shape):
     E.record([res], [x] + weights, bwd)
     return res
 
+def field_wise_bi(groups, kernel_mf, kernel_fm, bias_mf=None, bias_fm=None):
+    """FLEN's FieldWiseBiInteraction (deepctr/layers/interaction.py:1283-1337) in one b2ctr_field_wise_bi launch.
+    ``groups``: G lists of [B, n, E] tensors, the members of each group (a group is the field axis concatenation of
+    its list).  When every member is a column window of one buffer (the gather buffer) the fields are read there in
+    place, whether or not a group's members are adjacent; otherwise the members are first copied into one
+    [B, F, E] buffer.  Returns h [B, E]; only h is written.  The backward recomputes the group sums, adds dx into
+    that buffer's gradient (or writes it into the copy's) and sums the weight gradients in a fixed order."""
+    members = [m for g in groups for m in g]
+    b, e = members[0].data.shape[0], members[0].data.shape[-1]
+    G = len(groups)
+    nf = [int(np.prod(m.data.shape[1:])) // e for m in members]
+    K.field_wise_bi_check(sum(nf), G, e)
+    gid = [k for k, g in enumerate(groups) for _ in g]
+    base = members[0].base
+    in_place = (base is not None and base.data is not None and base.data.dim() == 2
+                and all(m.base is base and m.ncols != -1 and m.data is not None for m in members))
+    if in_place:
+        x, src = None, base.data
+        cols = [m.col0 + i * e for m, n in zip(members, nf) for i in range(n)]
+    else:
+        x = concat(members, 1)
+        src = E.contiguous(x).reshape(b, -1)
+        cols = [i * e for i in range(sum(nf))]
+    fgroup = [k for k, n in zip(gid, nf) for _ in range(n)]
+    w = [_wdata(v) if v is not None else None for v in (kernel_mf, kernel_fm, bias_mf, bias_fm)]
+    h = _empty((b, e), src)
+    K.field_wise_bi_fwd(src, cols, fgroup, G, e, b, w[0], w[1], w[2], w[3], h)
+    res = E.Var(h)
+    weights = [v for v in (kernel_mf, kernel_fm, bias_mf, bias_fm) if v is not None]
+    xs = members if in_place else [x]
+
+    def bwd(grads):
+        want_dx = any(v.requires_grad for v in xs)
+        want_dk = (kernel_mf.requires_grad, kernel_fm.requires_grad)
+        want_db = tuple(v is not None and v.requires_grad for v in (bias_mf, bias_fm))
+        if not (want_dx or any(want_dk) or any(want_db)):
+            return
+        g = grads[0].reshape(b, e)
+        if not g.is_contiguous():
+            g = g.contiguous()
+        dx, acc = None, False
+        if want_dx and in_place:
+            if base.grad is None:
+                base.grad = torch.empty_like(base.data)
+                K.fill(base.grad, 0.0)
+                base.requires_grad = True
+            dx, acc = base.grad, True
+        elif want_dx:
+            dx = _empty((b, src.shape[1]), g)
+        dkm, dkf, dbm, dbf = K.field_wise_bi_bwd(src, cols, fgroup, G, e, b, w[0], w[1], w[2], w[3], g, dx=dx,
+                                                 dx_accumulate=acc, want_dkernel=want_dk, want_dbias=want_db)
+        if want_dx and not in_place:
+            E.add_grad(x, dx.reshape(x.data.shape))
+        for v, d in ((kernel_mf, dkm), (kernel_fm, dkf), (bias_mf, dbm), (bias_fm, dbf)):
+            if d is not None:
+                E.add_grad(v, d)
+
+    E.record([res], xs + weights, bwd)
+    return res
+
+
 CIN_CHUNK_BYTES = 24 << 20      # outer-product chunk kept well inside the 50 MB L2
 
 

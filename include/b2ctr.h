@@ -759,6 +759,44 @@ B2CTR_API size_t b2ctr_conv_stack_bwd_workspace_bytes(const b2ctr_conv_stack_t* 
 B2CTR_API b2ctr_status_t b2ctr_conv_stack_bwd(const b2ctr_conv_stack_t* a, void* workspace, size_t workspace_bytes,
                                              void* stream);
 
+/* FLEN's FieldWiseBiInteraction (deepctr/layers/interaction.py:1224-1348) over G groups of fields read in place.
+ * Field f (0 <= f < nfield) is the [dim] row at column col[f] of a [B, ldx] buffer and belongs to group
+ * group[f]; the members of a group need not be adjacent.  Per sample and coordinate e, with
+ * S_g = sum_{f in g} x_f and Q_g = sum_{f in g} x_f^2:
+ *   h[e] = sum_{p = (g < h)} kernel_mf[p] * S_g * S_h + bias_mf  +  sum_g kernel_fm[g] * (S_g^2 - Q_g) + bias_fm
+ * (pairs in itertools.combinations order, no 1/2 on the FM term, as in the reference).  S_g and Q_g live in
+ * registers; only h is written, into the column window [outcol, outcol + dim) of a [B, ldout] buffer.
+ * Backward (the same descriptor; `out` now addresses the incoming gradient dh): the forward is recomputed from x,
+ *   dx_f = dh * (sum_{h != g} kernel_mf[p(g, h)] * S_h + 2 * kernel_fm[g] * (S_g - x_f))
+ * written (or added, dx_accumulate) at column col[f] of a [B, lddx] buffer (NULL: not wanted), and
+ *   dkernel_mf[p] = sum_{b, e} dh * S_g * S_h,  dkernel_fm[g] = sum_{b, e} dh * (S_g^2 - Q_g),
+ *   dbias_mf = dbias_fm = sum_b dh,
+ * each overwritten (NULL: not wanted), through per-CTA partials in the workspace summed in CTA order: no float
+ * atomics, bit-identical from run to run.  The forward saves nothing.  bias_mf / bias_fm may be NULL (use_bias
+ * False).  16-byte loads and stores when dim % 4 == 0 and every column, pitch and pointer allows, else a scalar
+ * path.  Limits: 2 <= ngroup <= B2CTR_FWBI_MAX_GROUPS, every group non-empty, ngroup <= nfield <=
+ * B2CTR_FWBI_MAX_FIELDS, 1 <= dim <= 256, 0 <= col[f] and col[f] + dim <= ldx < 2^31; anything else is INVALID_ARG. */
+#define B2CTR_FWBI_MAX_FIELDS 256
+#define B2CTR_FWBI_MAX_GROUPS 8
+typedef struct b2ctr_field_wise_bi {
+  int32_t struct_size;                             /* sizeof(b2ctr_field_wise_bi_t) */
+  int32_t nfield, ngroup, dim, dx_accumulate, reserved;
+  int64_t batch;
+  const float* x; int64_t ldx;
+  int64_t col[B2CTR_FWBI_MAX_FIELDS];              /* column of field f in a row of x (and of dx) */
+  int32_t group[B2CTR_FWBI_MAX_FIELDS];            /* group of field f, 0 <= group < ngroup */
+  const float* kernel_mf;                          /* [ngroup * (ngroup - 1) / 2] */
+  const float* kernel_fm;                          /* [ngroup] */
+  const float* bias_mf; const float* bias_fm;      /* [dim] or NULL */
+  float* out; int64_t ldout, outcol;               /* forward output h / backward incoming gradient dh */
+  float* dx; int64_t lddx;                         /* backward */
+  float* dkernel_mf; float* dkernel_fm; float* dbias_mf; float* dbias_fm;
+} b2ctr_field_wise_bi_t;
+B2CTR_API b2ctr_status_t b2ctr_field_wise_bi_fwd(const b2ctr_field_wise_bi_t* a, void* stream);
+B2CTR_API size_t b2ctr_field_wise_bi_bwd_workspace_bytes(const b2ctr_field_wise_bi_t* a);
+B2CTR_API b2ctr_status_t b2ctr_field_wise_bi_bwd(const b2ctr_field_wise_bi_t* a, void* workspace,
+                                                size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* 6. Sequence operators (DIN, pooling, Dice / BatchNormalization, dropout)                     */
 /* ------------------------------------------------------------------------------------------ */
