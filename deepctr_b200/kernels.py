@@ -4,7 +4,9 @@ torch only provides device memory (``torch.empty``) and the current stream handl
 byte of arithmetic happens inside libb2ctr.so.  These functions are what the GPU parity tests
 call ("through the C-ABI") and what the engine (``engine.py``) builds its tape ops from.
 """
+import contextlib
 import ctypes as C
+import functools
 
 import torch
 
@@ -53,6 +55,66 @@ def idx_dtype(t):
     raise ValueError("ids must be int32 or int64, got %s" % t.dtype)
 
 
+# ---- optional per-kernel timing (bench.py): CUDA events around each launch on the launching stream --
+PROFILE = None
+PROFILE_TAG = None       # set by `profile_tag(...)`: the launch is recorded as "<tag>:<wrapper name>"
+
+
+@contextlib.contextmanager
+def profiled():
+    """Record the launches of a block into a fresh PROFILE dict, which is yielded; PROFILE is None again after."""
+    global PROFILE
+    PROFILE = {}
+    try:
+        yield PROFILE
+    finally:
+        PROFILE = None
+
+
+class profile_tag(object):
+    """Attribute the launches of a region (CIN layers, the DIN attention unit ...) to a named group."""
+
+    def __init__(self, tag):
+        self.tag = tag
+
+    def __enter__(self):
+        global PROFILE_TAG
+        self.prev, PROFILE_TAG = PROFILE_TAG, (self.tag if PROFILE_TAG is None else PROFILE_TAG)
+
+    def __exit__(self, *a):
+        global PROFILE_TAG
+        PROFILE_TAG = self.prev
+
+
+def _timed(fn):
+    """Decorate a wrapper that enqueues device work: while PROFILE is a dict, each call records one CUDA-event
+    pair around it under the wrapper's name."""
+    name = fn.__name__
+
+    @functools.wraps(fn)
+    def wrap(*a, **k):
+        prof = PROFILE
+        if prof is None:
+            return fn(*a, **k)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        r = fn(*a, **k)
+        e1.record()
+        prof.setdefault(name if PROFILE_TAG is None else "%s:%s" % (PROFILE_TAG, name), []).append((e0, e1))
+        return r
+
+    return wrap
+
+
+def profile_summary():
+    """{kernel wrapper name: (launch groups, total ms)} for everything recorded into PROFILE."""
+    torch.cuda.synchronize()
+    out = {}
+    for name, evs in (PROFILE or {}).items():
+        out[name] = (len(evs), float(sum(a.elapsed_time(b) for a, b in evs)))
+    return out
+
+
 # ---- embedding ------------------------------------------------------------------------------
 def make_feature(table, idx, out, out_col=0, out_ld=None, maxlen=1, pool=L.POOL_NONE,
                  mask_mode=L.MASK_NONE, length=None, weight=None, weight_mode=L.WEIGHT_NONE,
@@ -89,6 +151,7 @@ def _feat_array(feats):
     return arr
 
 
+@_timed
 def embed_gather_fwd(feats, batch):
     arr = _feat_array(feats)
     L.check(L.lib().b2ctr_embed_gather_fwd(arr, len(feats), batch, stream()), "embed_gather_fwd")
@@ -102,6 +165,7 @@ def embed_oob_count(reset=True):
     return int(n.value)
 
 
+@_timed
 def embed_scatter_add(feats, batch, scale):
     arr = _feat_array(feats)
     L.check(L.lib().b2ctr_embed_scatter_add(arr, len(feats), batch, scale, stream()),
@@ -149,12 +213,14 @@ class UniformPlan(object):
         self.g.peer_lin_tables = peer_lin_tables.data_ptr() if peer_lin_tables is not None else None
 
 
+@_timed
 def embed_gather_uniform_fwd(plan, batch):
     L.check(L.lib().b2ctr_embed_gather_uniform_fwd_ex(C.byref(plan.g), ptr(plan.fm_sum), ptr(plan.x_planes),
                                                       plan.x_planes_cols, batch, stream()),
             "embed_gather_uniform_fwd")
 
 
+@_timed
 def embed_scatter_uniform_bwd(plan, dx, dfm, dlinear, scale, lin_scale, batch, fm_sum=None):
     """``fm_sum``: the S [B, dim] a gather of the same x stored (UniformPlan.fm_sum), or None: the scatter sums x."""
     L.check(L.lib().b2ctr_embed_scatter_uniform_bwd_ex(C.byref(plan.g), ptr(dx), ptr(dfm), ptr(fm_sum),
@@ -162,6 +228,7 @@ def embed_scatter_uniform_bwd(plan, dx, dfm, dlinear, scale, lin_scale, batch, f
             "embed_scatter_uniform_bwd")
 
 
+@_timed
 def embed_update_sorted(plan, dx, dfm, dlinear, optimizer, lr, lin_lr, eps, acc_tables, lin_acc_tables, batch):
     """Deterministic fused update (sort by (table, id) + ordered segmented reduce, one write per row):
     optimizer 0 = SGD, 1 = Keras Adagrad (lazy / sparse apply) with per-element accumulators."""
@@ -177,6 +244,7 @@ def embed_update_sorted(plan, dx, dfm, dlinear, optimizer, lr, lin_lr, eps, acc_
             "embed_update_sorted")
 
 
+@_timed
 def hash64(ids, num_buckets, mask_zero):
     _require_cuda(ids)
     ids = ids.contiguous()
@@ -186,6 +254,7 @@ def hash64(ids, num_buckets, mask_zero):
     return out
 
 
+@_timed
 def init_normal(dst, mean, std, seed):
     _require_cuda(dst)
     L.check(L.lib().b2ctr_init_normal(ptr(dst), dst.numel(), mean, std, seed, stream()), "init_normal")
@@ -193,6 +262,7 @@ def init_normal(dst, mean, std, seed):
 
 
 # ---- GEMM -----------------------------------------------------------------------------------
+@_timed
 def gemm(a, b, c=None, bias=None, trans_a=False, trans_b=False, act=L.ACT_NONE, accumulate=False,
          precision=L.GEMM_FP32, split_k=1, alpha=1.0, m=None, n=None, k=None, variant=0, a_planes=None,
          b_planes=None):
@@ -235,6 +305,7 @@ def gemm(a, b, c=None, bias=None, trans_a=False, trans_b=False, act=L.ACT_NONE, 
     return c
 
 
+@_timed
 def split_planes(x2d):
     """bf16 hi/lo planes of a 2-D fp32 tensor (row stride may exceed the width) for BF16X3 GEMMs."""
     _require_cuda(x2d)
@@ -251,6 +322,7 @@ def planes_fusable(m, n):
     return m % 256 == 0 and (n == 64 or n % 128 == 0) and n % 4 == 0 and n // 4 <= 256 and 256 % (n // 4) == 0
 
 
+@_timed
 def bias_act_bwd(dy, y, act, want_dz=True, want_dbias=True, m=None, n=None, want_planes=False):
     """dz = dy * act'(y), dbias = colsum(dz); with want_planes also the bf16 operand planes of dz
     (returned as third value)."""
@@ -275,6 +347,7 @@ def bias_act_bwd(dy, y, act, want_dz=True, want_dbias=True, m=None, n=None, want
     return dz, dbias
 
 
+@_timed
 def act_fwd(x, act, out=None):
     _require_cuda(x)
     out = torch.empty_like(x) if out is None else out
@@ -282,6 +355,7 @@ def act_fwd(x, act, out=None):
     return out
 
 
+@_timed
 def add_n(ins, scales=None, out=None):
     _require_cuda(*ins)
     out = torch.empty_like(ins[0]) if out is None else out
@@ -291,18 +365,21 @@ def add_n(ins, scales=None, out=None):
     return out
 
 
+@_timed
 def axpy(x, y, alpha=1.0):
     _require_cuda(x, y)
     L.check(L.lib().b2ctr_axpy(ptr(x), ptr(y), alpha, x.numel(), stream()), "axpy")
     return y
 
 
+@_timed
 def fill(dst, value):
     _require_cuda(dst)
     L.check(L.lib().b2ctr_fill(ptr(dst), value, dst.numel(), stream()), "fill")
     return dst
 
 
+@_timed
 def mask_nonzero_and(ids, inout=None):
     """uint8 mask [B,T] of ids != 0, AND-ed into ``inout`` when given."""
     _require_cuda(ids, inout)
@@ -314,6 +391,7 @@ def mask_nonzero_and(ids, inout=None):
     return inout
 
 
+@_timed
 def mask_from_len(lengths, maxlen):
     _require_cuda(lengths)
     lengths = lengths.reshape(-1)
@@ -323,6 +401,7 @@ def mask_from_len(lengths, maxlen):
     return out
 
 
+@_timed
 def copy2d(src, ld_src, dst, ld_dst, rows, cols, accumulate=False, src_off=0, dst_off=0):
     _require_cuda(src, dst)
     sp = C.c_void_p(src.data_ptr() + 4 * src_off)
@@ -331,6 +410,7 @@ def copy2d(src, ld_src, dst, ld_dst, rows, cols, accumulate=False, src_off=0, ds
     return dst
 
 
+@_timed
 def pack_rows(src_flat, widths, batch, out=None):
     """[sum_i B*w_i] flat blocks -> row-major [B, sum w_i]."""
     _require_cuda(src_flat)
@@ -342,6 +422,7 @@ def pack_rows(src_flat, widths, batch, out=None):
     return out
 
 
+@_timed
 def rowsum(x, rows, cols, ld=None):
     _require_cuda(x)
     out = torch.empty((rows,), dtype=torch.float32, device=x.device)
@@ -350,6 +431,7 @@ def rowsum(x, rows, cols, ld=None):
     return out
 
 
+@_timed
 def fm_fwd(x, nfield, dim, ldx=None):
     _require_cuda(x)
     batch = x.shape[0]
@@ -359,6 +441,7 @@ def fm_fwd(x, nfield, dim, ldx=None):
     return out
 
 
+@_timed
 def fm_bwd(x, nfield, dim, dout, dx=None, accumulate=False, ldx=None):
     _require_cuda(x, dout)
     batch = x.shape[0]
@@ -371,6 +454,7 @@ def fm_bwd(x, nfield, dim, dout, dx=None, accumulate=False, ldx=None):
     return dx
 
 
+@_timed
 def fm_weighted_fwd(x, ldx, m, nfield, dim, batch):
     """FM of m ⊙ x: x a [B, nfield*dim] window (row pitch ldx), m [B, nfield] (row pitch m.stride(0)) -> [B]."""
     _require_cuda(x, m)
@@ -380,6 +464,7 @@ def fm_weighted_fwd(x, ldx, m, nfield, dim, batch):
     return out
 
 
+@_timed
 def fm_weighted_bwd(x, ldx, m, nfield, dim, dout, batch, dx=None, accumulate=False, want_dx=True, want_dm=True):
     """(dx [B, nfield*dim] or the given window, dm [B, nfield] | None).  ``dx`` given: written with its own row pitch,
     added to when ``accumulate``."""
@@ -394,6 +479,7 @@ def fm_weighted_bwd(x, ldx, m, nfield, dim, dout, batch, dx=None, accumulate=Fal
     return dx, dm
 
 
+@_timed
 def field_scale_fwd(x, ldx, m, nfield, dim, batch, out=None):
     """y[b, f*dim + e] = x[b, f*dim + e] * m[b, f] -> [B, nfield*dim] (or into ``out``, a 2-D window)."""
     _require_cuda(x, m, out)
@@ -404,6 +490,7 @@ def field_scale_fwd(x, ldx, m, nfield, dim, batch, out=None):
     return out
 
 
+@_timed
 def field_scale_bwd(dy, x, ldx, m, nfield, dim, batch, dx=None, accumulate=False, want_dx=True, want_dm=True):
     """(dx = dy * m [B, nfield*dim] or the given window, dm = sum_e dy x [B, nfield] | None)."""
     _require_cuda(dy, x, m, dx)
@@ -417,6 +504,7 @@ def field_scale_bwd(dy, x, ldx, m, nfield, dim, batch, dx=None, accumulate=False
     return dx, dm
 
 
+@_timed
 def softmax_rows_fwd(x, scale=1.0):
     """scale * softmax along the rows of a 2-D window x (row pitch x.stride(0)) -> a new [rows, cols] tensor."""
     _require_cuda(x)
@@ -427,6 +515,7 @@ def softmax_rows_fwd(x, scale=1.0):
     return y
 
 
+@_timed
 def softmax_rows_bwd(y, dy, scale=1.0):
     """dx = y * (dy - sum_j y_j dy_j / scale) for 2-D windows y, dy -> a new [rows, cols] tensor."""
     _require_cuda(y, dy)
@@ -438,6 +527,7 @@ def softmax_rows_bwd(y, dy, scale=1.0):
 
 
 # ---- head / loss / optimizers ---------------------------------------------------------------
+@_timed
 def predict_loss(logit, bias=None, labels=None, task=L.TASK_BINARY, want_grad=False):
     """Returns (pred[B], dlogit[B] | None, dbias[1] | None, loss_sum[1] | None)."""
     _require_cuda(logit, bias, labels)
@@ -455,11 +545,13 @@ def predict_loss(logit, bias=None, labels=None, task=L.TASK_BINARY, want_grad=Fa
     return pred, dlogit, dbias, loss_sum
 
 
+@_timed
 def sgd_step(w, g, lr, l2=0.0):
     _require_cuda(w, g)
     L.check(L.lib().b2ctr_sgd_step(ptr(w), ptr(g), lr, l2, w.numel(), stream()), "sgd_step")
 
 
+@_timed
 def sgd_step_multi(ws, gs, lr, l2s):
     """w -= lr * (g + 2 l2 w) for a list of tensors in one launch."""
     n = len(ws)
@@ -473,12 +565,14 @@ def sgd_step_multi(ws, gs, lr, l2s):
     L.check(L.lib().b2ctr_sgd_step_multi(wp, gp, nn, ll, n, lr, stream()), "sgd_step_multi")
 
 
+@_timed
 def adam_step(w, g, m, v, lr, step, beta1=0.9, beta2=0.999, eps=1e-7, l2=0.0):
     _require_cuda(w, g, m, v)
     L.check(L.lib().b2ctr_adam_step(ptr(w), ptr(g), ptr(m), ptr(v), lr, beta1, beta2, eps, l2, step,
                                     w.numel(), stream()), "adam_step")
 
 
+@_timed
 def adam_step_dev(w, g, m, v, lr, step_dev, beta1=0.9, beta2=0.999, eps=1e-7, l2=0.0):
     """Adam with the step count read from the device tensor `step_dev` (int64 [1]): graph-replayable."""
     _require_cuda(w, g, m, v, step_dev)
@@ -486,63 +580,17 @@ def adam_step_dev(w, g, m, v, lr, step_dev, beta1=0.9, beta2=0.999, eps=1e-7, l2
                                         w.numel(), stream()), "adam_step_dev")
 
 
+@_timed
 def counter_add(counter, delta=1):
     _require_cuda(counter)
     L.check(L.lib().b2ctr_counter_add(ptr(counter), delta, stream()), "counter_add")
 
 
+@_timed
 def adagrad_step(w, g, acc, lr, eps=1e-7, l2=0.0):
     _require_cuda(w, g, acc)
     L.check(L.lib().b2ctr_adagrad_step(ptr(w), ptr(g), ptr(acc), lr, eps, l2, w.numel(), stream()),
             "adagrad_step")
-
-
-# ---- optional per-kernel timing (bench.py): CUDA events around each launch on the launching stream --
-PROFILE = None
-PROFILE_TAG = None       # set by `profile_tag(...)`: the launch is recorded as "<tag>:<wrapper name>"
-
-
-class profile_tag(object):
-    """Attribute the launches of a region (CIN layers, the DIN attention unit ...) to a named group."""
-
-    def __init__(self, tag):
-        self.tag = tag
-
-    def __enter__(self):
-        global PROFILE_TAG
-        self.prev, PROFILE_TAG = PROFILE_TAG, (self.tag if PROFILE_TAG is None else PROFILE_TAG)
-
-    def __exit__(self, *a):
-        global PROFILE_TAG
-        PROFILE_TAG = self.prev
-
-
-def _timed(fn):
-    name = fn.__name__
-
-    def wrap(*a, **k):
-        prof = PROFILE
-        if prof is None:
-            return fn(*a, **k)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        r = fn(*a, **k)
-        e1.record()
-        prof.setdefault(name if PROFILE_TAG is None else "%s:%s" % (PROFILE_TAG, name), []).append((e0, e1))
-        return r
-
-    wrap.__name__ = name
-    wrap.__doc__ = fn.__doc__
-    return wrap
-
-
-def profile_summary():
-    """{kernel wrapper name: (launch groups, total ms)} for everything recorded into PROFILE."""
-    torch.cuda.synchronize()
-    out = {}
-    for name, evs in (PROFILE or {}).items():
-        out[name] = (len(evs), float(sum(a.elapsed_time(b) for a, b in evs)))
-    return out
 
 
 # ---- field-aware pairwise products (ONN) ---------------------------------------------------------------
@@ -561,6 +609,7 @@ def ffm_field(idx=None, vocab=1, hash_mode=L.HASH_NONE, pooled=None, grad=None):
     return f
 
 
+@_timed
 def ffm_product_fwd(fields, tables, dim, reduce_sum, out, out_col, batch):
     """prod_p = e_{i,(j)} * e_{j,(i)} for every pair into ``out`` [B, ld] from column ``out_col``; ``tables`` the
     device int64 array [F*F] of table pointers."""
@@ -569,6 +618,7 @@ def ffm_product_fwd(fields, tables, dim, reduce_sum, out, out_col, batch):
               out_col, batch, stream())
 
 
+@_timed
 def ffm_product_bwd(fields, tables, dim, reduce_sum, g, g_col, batch):
     """Per-lookup gradient rows into each field's ``grad`` buffer, read at the tables' current values."""
     arr = (L.FfmField * len(fields))(*fields)
@@ -576,18 +626,12 @@ def ffm_product_bwd(fields, tables, dim, reduce_sum, g, g_col, batch):
               batch, stream())
 
 
-for _n in ("embed_update_sorted", "split_planes", "embed_gather_fwd", "embed_scatter_add", "embed_gather_uniform_fwd", "embed_scatter_uniform_bwd",
-           "ffm_product_fwd", "ffm_product_bwd", "hash64", "gemm", "bias_act_bwd", "act_fwd", "add_n", "axpy", "fill", "copy2d", "rowsum", "fm_fwd",
-           "fm_bwd", "predict_loss", "sgd_step", "sgd_step_multi", "adam_step", "adagrad_step", "mask_nonzero_and",
-           "mask_from_len"):
-    globals()[_n] = _timed(globals()[_n])
-
-
 # ---- interaction / sequence operators ---------------------------------------------------------------
 def _lib_call(name, *args):
     L.check(getattr(L.lib(), "b2ctr_" + name)(*args), name)
 
 
+@_timed
 def ewise(op, a, b, c=None, out=None, accumulate=False):
     _require_cuda(a, b, c, out)
     out = torch.empty_like(a) if out is None else out
@@ -595,6 +639,7 @@ def ewise(op, a, b, c=None, out=None, accumulate=False):
     return out
 
 
+@_timed
 def cross_vector_fwd(x0, ld0, xl, ldl, w, bias, batch, dim):
     out = torch.empty((batch, dim), dtype=torch.float32, device=x0.device)
     s = torch.empty((batch,), dtype=torch.float32, device=x0.device)
@@ -603,6 +648,7 @@ def cross_vector_fwd(x0, ld0, xl, ldl, w, bias, batch, dim):
     return out, s
 
 
+@_timed
 def cross_vector_bwd(x0, ld0, w, dout, s, batch, dim):
     dx0 = torch.empty((batch, dim), dtype=torch.float32, device=x0.device)
     dxl = torch.empty((batch, dim), dtype=torch.float32, device=x0.device)
@@ -616,12 +662,14 @@ def _off(t, elems):
     return C.c_void_p(t.data_ptr() + 4 * elems)
 
 
+@_timed
 def cin_outer_fwd(x0, v0, xk, vk, z, b0, nb, m, h, d):
     """v0 / vk = (sb, si, sd) element strides; b0 = first sample of the chunk."""
     _lib_call("cin_outer_fwd", _off(x0, b0 * v0[0]), v0[0], v0[1], v0[2], _off(xk, b0 * vk[0]), vk[0], vk[1],
               vk[2], ptr(z), nb, m, h, d, stream())
 
 
+@_timed
 def cin_outer_bwd(dz, x0, v0, xk, vk, dx0, g0, acc0, dxk, gk, acck, b0, nb, m, h, d, hp=0):
     _lib_call("cin_outer_bwd", ptr(dz), _off(x0, b0 * v0[0]), v0[0], v0[1], v0[2], _off(xk, b0 * vk[0]), vk[0],
               vk[1], vk[2], _off(dx0, b0 * g0[0]) if dx0 is not None else C.c_void_p(0), g0[0], g0[1], g0[2],
@@ -629,6 +677,7 @@ def cin_outer_bwd(dz, x0, v0, xk, vk, dx0, g0, acc0, dxk, gk, acck, b0, nb, m, h
               int(acck), nb, m, h, d, hp, stream())
 
 
+@_timed
 def cin_t0(x0, v0, nb, m, d, ld0):
     """T0[(b,d), i] = X0(b,i,d), zero-padded to ld0 columns: the per-row factors of the generated outer product."""
     t0 = torch.empty((nb * d, ld0), dtype=torch.float32, device=x0.device)
@@ -636,6 +685,7 @@ def cin_t0(x0, v0, nb, m, d, ld0):
     return t0
 
 
+@_timed
 def cin_filter_planes(w2d, m, h, hp):
     """bf16 hi/lo planes of the filter in the padded layout W'[i*hp + j, n] (w2d: [m*h, n])."""
     n = w2d.shape[1]
@@ -644,6 +694,7 @@ def cin_filter_planes(w2d, m, h, hp):
     return planes
 
 
+@_timed
 def cin_gemm(mode, t0, xk, ldk, rows, m, h, hp, n, planes, bias=None, act=L.ACT_NONE, split_k=1, out=None):
     """mode 0: Y[rows, n] = act(Z W' + bias) with planes = cin_filter_planes; mode 1: dW'[m*hp, n] = Z^T dY with
     planes = split_planes(dY).  Z[r, i*hp+j] = t0[r,i] * xk[r,j] is generated inside the GEMM producer."""
@@ -663,6 +714,7 @@ def cin_gemm(mode, t0, xk, ldk, rows, m, h, hp, n, planes, bias=None, act=L.ACT_
     return out
 
 
+@_timed
 def att_gemm(mode, q2d, ldq, keys2d, key_batch_stride, batch, T, E, n, planes, bias=None, act=L.ACT_NONE, split_k=1):
     """First LocalActivationUnit layer with its [q, k, q-k, q*k] input generated inside the GEMM producer.
     mode 0: [B*T, n] = act(A W + bias) (planes of W [4E, n]); mode 1: [4E, n] = A^T dY (planes of dY [B*T, n])."""
@@ -680,6 +732,7 @@ def att_gemm(mode, q2d, ldq, keys2d, key_batch_stride, batch, T, E, n, planes, b
     return out
 
 
+@_timed
 def cin_fold(t0, xk, ldk, rows, m, h, hp, n, w_planes, dy_planes, dt0, dxk, ldx):
     """dZ = dY W'^T folded onto the factors inside the GEMM epilogue: dt0 [rows, ld0] and dxk [rows, ldx] are
     accumulated (zero them first; layer 0: dxk is dt0)."""
@@ -690,10 +743,12 @@ def cin_fold(t0, xk, ldk, rows, m, h, hp, n, w_planes, dy_planes, dt0, dxk, ldx)
     L.check(L.lib().b2ctr_cin_fold(C.byref(g), ptr(dt0), ptr(dxk), ldx, stream()), "cin_fold")
 
 
+@_timed
 def cin_t0_bwd(dt0, ld0, dx, gx, accumulate, nb, m, d):
     _lib_call("cin_t0_bwd", ptr(dt0), ld0, ptr(dx), gx[0], gx[1], gx[2], int(accumulate), nb, m, d, stream())
 
 
+@_timed
 def cin_unpad_rows(src, m, h, hp):
     n = src.shape[1]
     dst = torch.empty((m * h, n), dtype=torch.float32, device=src.device)
@@ -701,15 +756,18 @@ def cin_unpad_rows(src, m, h, hp):
     return dst
 
 
+@_timed
 def cin_sum_d(y, ldy, col0, ncols, d, out, ldo, out_col, b0, nb):
     _lib_call("cin_sum_d", ptr(y), ldy, col0, ncols, d, _off(out, b0 * ldo), ldo, out_col, nb, stream())
 
 
+@_timed
 def cin_expand_grad(dout, ldo, out_col, col0, ncols, dh, ldh, hcols, dy, nfilt, d, b0, nb):
     _lib_call("cin_expand_grad", _off(dout, b0 * ldo), ldo, out_col, col0, ncols, ptr(dh), ldh, hcols, ptr(dy),
               nfilt, d, nb, stream())
 
 
+@_timed
 def interacting_fwd(q, k, v, res, batch, F, H, D, scaling):
     out = torch.empty_like(q)
     _lib_call("interacting_fwd", ptr(q), ptr(k), ptr(v), ptr(res), ptr(out), batch, F, H, D, int(scaling),
@@ -717,6 +775,7 @@ def interacting_fwd(q, k, v, res, batch, F, H, D, scaling):
     return out
 
 
+@_timed
 def interacting_bwd(q, k, v, out, dout, want_res, batch, F, H, D, scaling):
     dq, dk, dv = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
     dres = torch.empty_like(q) if want_res else None
@@ -725,6 +784,7 @@ def interacting_bwd(q, k, v, out, dout, want_res, batch, F, H, D, scaling):
     return dq, dk, dv, dres
 
 
+@_timed
 def bi_interaction_fwd(x, ldx, nfield, dim, batch):
     """[B, nfield*dim] window (pitch ldx) -> [B, dim]:  0.5 * ((sum_f x)^2 - sum_f x^2)."""
     _require_cuda(x)
@@ -733,6 +793,7 @@ def bi_interaction_fwd(x, ldx, nfield, dim, batch):
     return out
 
 
+@_timed
 def bi_interaction_bwd(x, ldx, nfield, dim, g, batch):
     _require_cuda(x, g)
     dx = torch.empty((batch, nfield * dim), dtype=torch.float32, device=x.device)
@@ -741,6 +802,7 @@ def bi_interaction_bwd(x, ldx, nfield, dim, g, batch):
     return dx
 
 
+@_timed
 def afm_fwd(x, ldx, nfield, dim, W, bias, h, batch):
     """AFM attention pooling -> (att [B, dim], softmax state [B, 2])."""
     _require_cuda(x, W, bias, h)
@@ -752,6 +814,7 @@ def afm_fwd(x, ldx, nfield, dim, W, bias, h, batch):
     return att, state
 
 
+@_timed
 def afm_bwd(g, x, ldx, nfield, dim, W, bias, h, state, att, batch):
     """-> (dx [B, nfield*dim], dW [dim, factor], dbias [factor], dh [factor])."""
     _require_cuda(g, x, W, bias, h, state, att)
@@ -769,6 +832,7 @@ def afm_bwd(g, x, ldx, nfield, dim, W, bias, h, state, att, batch):
     return dx, dW, db, dh
 
 
+@_timed
 def senet_fwd(x, ldx, nfield, dim, W1, W2, batch):
     """SENETLayer on a [B, nfield*dim] window (pitch ldx) -> (V [B, nfield*dim], saved (A1, A2) [B, R + nfield])."""
     _require_cuda(x, W1, W2)
@@ -780,6 +844,7 @@ def senet_fwd(x, ldx, nfield, dim, W1, W2, batch):
     return v, saved
 
 
+@_timed
 def senet_bwd(g, x, ldx, nfield, dim, W1, W2, saved, batch):
     """-> (dx [B, nfield*dim], dW1 [nfield, R], dW2 [R, nfield])."""
     _require_cuda(g, x, W1, W2, saved)
@@ -798,6 +863,7 @@ def senet_bwd(g, x, ldx, nfield, dim, W1, W2, saved, batch):
 BILINEAR_TYPES = {"all": 0, "each": 1, "interaction": 2}
 
 
+@_timed
 def bilinear_fwd(x, ldx, nfield, dim, btype, W, batch, out=None, col0=0, pitch=None):
     """BilinearInteraction on a [B, nfield*dim] window (pitch ldx) with the stacked weights W [nW, dim, dim].
     Pair p goes to columns [col0 + p*pitch, +dim) of ``out`` [B, ld] (default: a new [B, P*dim])."""
@@ -811,6 +877,7 @@ def bilinear_fwd(x, ldx, nfield, dim, btype, W, batch, out=None, col0=0, pitch=N
     return out
 
 
+@_timed
 def bilinear_bwd(g, ldg, gcol0, gpitch, x, ldx, nfield, dim, btype, W, batch, want_dx=True, want_dw=True):
     """g: the data pointer of the gradient buffer addressed like the forward's output -> (dx [B, nfield*dim], dW)."""
     _require_cuda(g, x, W)
@@ -824,6 +891,7 @@ def bilinear_bwd(g, ldg, gcol0, gpitch, x, ldx, nfield, dim, btype, W, batch, wa
     return dx, dW
 
 
+@_timed
 def fwfm_fwd(x, ldx, nfield, dim, r, batch):
     """FwFMLayer on a [B, nfield*dim] window (pitch ldx) with the strengths r [nfield, nfield] -> [B, 1]."""
     _require_cuda(x, r)
@@ -832,6 +900,7 @@ def fwfm_fwd(x, ldx, nfield, dim, r, batch):
     return out
 
 
+@_timed
 def fwfm_bwd(g, ldg, x, ldx, nfield, dim, r, batch, want_dx=True, want_dr=True):
     """-> (dx [B, nfield*dim] or None, dR [nfield, nfield] or None)."""
     _require_cuda(g, x, r)
@@ -845,6 +914,7 @@ def fwfm_bwd(g, ldg, x, ldx, nfield, dim, r, batch, want_dx=True, want_dr=True):
     return dx, dR
 
 
+@_timed
 def fefm_sym(W):
     """S_p = W_p + W_p^T for the stacked weights W [P, dim, dim]."""
     _require_cuda(W)
@@ -853,6 +923,7 @@ def fefm_sym(W):
     return S
 
 
+@_timed
 def fefm_fwd(x, ldx, nfield, dim, S, batch, out=None, col0=0):
     """FEFMLayer on a [B, nfield*dim] window (pitch ldx) with S from fefm_sym: pair p's score goes to column
     col0 + p of ``out`` [B, ld] (default: a new [B, P])."""
@@ -863,6 +934,7 @@ def fefm_fwd(x, ldx, nfield, dim, S, batch, out=None, col0=0):
     return out
 
 
+@_timed
 def fefm_bwd(g, ldg, gcol0, x, ldx, nfield, dim, S, batch, want_dx=True, want_dw=True):
     """g: the data pointer of the gradient buffer addressed like the forward's output -> (dx [B, nfield*dim] or
     None, dW [P, dim, dim] or None)."""
@@ -880,6 +952,7 @@ def fefm_bwd(g, ldg, gcol0, x, ldx, nfield, dim, S, batch, want_dx=True, want_dw
 PNN_MODES = {"inner": 0, "elementwise": 1, "vec": 2, "num": 3}   # b2ctr.h B2CTR_PNN_*
 
 
+@_timed
 def pnn_inner_fwd(x, ldx, nfield, dim, mode, Kw, batch, out=None, col0=0):
     """InnerProductLayer / OutterProductLayer('vec' | 'num') on a [B, nfield*dim] window (pitch ldx); ``mode`` a
     PNN_MODES key, ``Kw`` the kernel (None for 'inner' / 'elementwise').  The pair scores (P*dim products for
@@ -893,6 +966,7 @@ def pnn_inner_fwd(x, ldx, nfield, dim, mode, Kw, batch, out=None, col0=0):
     return out
 
 
+@_timed
 def pnn_inner_bwd(g, ldg, gcol0, x, ldx, nfield, dim, mode, Kw, batch, want_dx=True, want_dk=True):
     """g: the data pointer of the gradient buffer addressed like the forward's output -> (dx [B, nfield*dim] or
     None, dK shaped like Kw or None)."""
@@ -909,6 +983,7 @@ def pnn_inner_bwd(g, ldg, gcol0, x, ldx, nfield, dim, mode, Kw, batch, want_dx=T
     return dx, dK
 
 
+@_timed
 def pnn_outer_fwd(x, ldx, nfield, dim, Kw, batch, out=None, col0=0):
     """OutterProductLayer('mat') with the kernel Kw [dim, P, dim] read in place: pair p's score goes to column
     col0 + p of ``out`` [B, ld] (default: a new [B, P])."""
@@ -919,6 +994,7 @@ def pnn_outer_fwd(x, ldx, nfield, dim, Kw, batch, out=None, col0=0):
     return out
 
 
+@_timed
 def pnn_outer_bwd(g, ldg, gcol0, x, ldx, nfield, dim, Kw, batch, want_dx=True, want_dk=True):
     """-> (dx [B, nfield*dim] or None, dK [dim, P, dim] or None)."""
     _require_cuda(g, x, Kw)
@@ -970,6 +1046,7 @@ def _window_of(a, name, out):
     setattr(a, name + "col", col)
 
 
+@_timed
 def regulate_fwd(mode, nfield, dim, batch, x, h=None, ax=None, ah=None, gates=(), u=None, y0=None, y1=None):
     """EDCN's bridge + gates in one pass (b2ctr_regulate_fwd): ``u`` / ``y0`` / ``y1`` are (buffer [B, ld], col0)
     windows to write v, v * gate0, v * gate1 into (None: not written)."""
@@ -980,6 +1057,7 @@ def regulate_fwd(mode, nfield, dim, batch, x, h=None, ax=None, ah=None, gates=()
     L.check(L.lib().b2ctr_regulate_fwd(C.byref(a), stream()), "regulate_fwd")
 
 
+@_timed
 def regulate_bwd(mode, nfield, dim, batch, x, h=None, ax=None, ah=None, gates=(), du=None, dy0=None, dy1=None,
                  want_dx=True, dx=None, dx_accumulate=False, want_dh=False, want_dax=False, want_dah=False,
                  want_dg=(False, False)):
@@ -1079,6 +1157,7 @@ def _conv_desc(stages, x, rows, dim, channels, batch, out):
     return a
 
 
+@_timed
 def conv_stack_fwd(stages, x, rows, dim, channels, batch, out):
     """CCPM's conv / k-max stack per (sample, e) column in one launch (b2ctr_conv_stack_fwd): x [B, rows, dim,
     channels] read in place, the last map written in Flatten order into ``out`` (a 2-D view)."""
@@ -1087,6 +1166,7 @@ def conv_stack_fwd(stages, x, rows, dim, channels, batch, out):
     return out
 
 
+@_timed
 def conv_stack_bwd(stages, x, rows, dim, channels, batch, dout, dx=None, dx_accumulate=False, want_dw=()):
     """Recompute the stack and take its gradient (b2ctr_conv_stack_bwd): ``dx`` a 2-D view to write (or add) x's
     gradient into, or None; ``want_dw`` per conv stage whether its (dkernel, dbias) are wanted.  Returns the list of
@@ -1149,6 +1229,7 @@ def _fwbi_desc(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm, bias_m
     return a
 
 
+@_timed
 def field_wise_bi_fwd(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm, bias_mf, bias_fm, out, outcol=0):
     """FLEN's FieldWiseBiInteraction in one launch (b2ctr_field_wise_bi_fwd): reads the fields in place and writes
     only h into the columns [outcol, outcol + dim) of ``out``."""
@@ -1157,6 +1238,7 @@ def field_wise_bi_fwd(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm,
     return out
 
 
+@_timed
 def field_wise_bi_bwd(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm, bias_mf, bias_fm, dout, doutcol=0,
                       dx=None, dx_accumulate=False, want_dkernel=(False, False), want_dbias=(False, False)):
     """Recompute the forward and take its gradient (b2ctr_field_wise_bi_bwd): ``dx`` a 2-D view whose columns
@@ -1178,12 +1260,14 @@ def field_wise_bi_bwd(x, cols, groups, ngroup, dim, batch, kernel_mf, kernel_fm,
     return tuple(res)
 
 
+@_timed
 def din_att_input_fwd(q, ldq, keys, ldk, batch, T, E):
     out = torch.empty((batch, T, 4 * E), dtype=torch.float32, device=q.device)
     _lib_call("din_att_input_fwd", ptr(q), ldq, ptr(keys), ldk, ptr(out), batch, T, E, stream())
     return out
 
 
+@_timed
 def din_att_input_bwd(q, ldq, keys, ldk, g, batch, T, E):
     dq = torch.empty((batch, 1, E), dtype=torch.float32, device=q.device)
     dk = torch.empty((batch, T, E), dtype=torch.float32, device=q.device)
@@ -1191,6 +1275,7 @@ def din_att_input_bwd(q, ldq, keys, ldk, g, batch, T, E):
     return dq, dk
 
 
+@_timed
 def din_pool_fwd(score, keys, ldk, mask, batch, T, E, weight_norm, return_score):
     w = torch.empty((batch, T), dtype=torch.float32, device=score.device)
     out = torch.empty((batch, 1, T if return_score else E), dtype=torch.float32, device=score.device)
@@ -1199,6 +1284,7 @@ def din_pool_fwd(score, keys, ldk, mask, batch, T, E, weight_norm, return_score)
     return out, w
 
 
+@_timed
 def din_pool_bwd(w, keys, ldk, mask, dout, batch, T, E, weight_norm, return_score, want_dkeys=True):
     dscore = torch.empty((batch, T, 1), dtype=torch.float32, device=w.device)
     dkeys = torch.empty((batch, T, E), dtype=torch.float32, device=w.device) if (want_dkeys and not return_score) \
@@ -1208,30 +1294,35 @@ def din_pool_bwd(w, keys, ldk, mask, dout, batch, T, E, weight_norm, return_scor
     return dscore, dkeys
 
 
+@_timed
 def seqpool_fwd(x, mask, length, batch, T, E, mode):
     out = torch.empty((batch, 1, E), dtype=torch.float32, device=x.device)
     _lib_call("seqpool_fwd", ptr(x), ptr(mask), ptr(length), ptr(out), batch, T, E, mode, stream())
     return out
 
 
+@_timed
 def seqpool_bwd(x, mask, length, dout, batch, T, E, mode):
     dx = torch.empty((batch, T, E), dtype=torch.float32, device=x.device)
     _lib_call("seqpool_bwd", ptr(x), ptr(mask), ptr(length), ptr(dout), ptr(dx), batch, T, E, mode, stream())
     return dx
 
 
+@_timed
 def seqweight(w, mask, length, batch, T, normalize):
     wt = torch.empty((batch, T), dtype=torch.float32, device=w.device)
     _lib_call("seqweight", ptr(w), ptr(mask), ptr(length), ptr(wt), batch, T, int(normalize), stream())
     return wt
 
 
+@_timed
 def seqscale(x, wt, rows, E):
     out = torch.empty_like(x)
     _lib_call("seqscale", ptr(x), ptr(wt), ptr(out), rows, E, stream())
     return out
 
 
+@_timed
 def colstats(x, ld, m, n):
     stats = torch.empty((2, n), dtype=torch.float32, device=x.device)
     nbytes = L.lib().b2ctr_colstats_workspace_bytes(m, n)
@@ -1240,16 +1331,19 @@ def colstats(x, ld, m, n):
     return stats
 
 
+@_timed
 def moving_update(moving, batch_stat, momentum):
     _lib_call("moving_update", ptr(moving), ptr(batch_stat), momentum, moving.numel(), stream())
 
 
+@_timed
 def bn_apply(x, mean, var, gamma, beta, m, n, eps):
     y = torch.empty_like(x)
     _lib_call("bn_apply", ptr(x), ptr(mean), ptr(var), ptr(gamma), ptr(beta), ptr(y), m, n, eps, stream())
     return y
 
 
+@_timed
 def bn_bwd(x, mean, var, gamma, dy, m, n, eps, training):
     dx = torch.empty_like(x)
     dgamma = torch.empty((n,), dtype=torch.float32, device=x.device)
@@ -1261,12 +1355,14 @@ def bn_bwd(x, mean, var, gamma, dy, m, n, eps, training):
     return dx, dgamma, dbeta
 
 
+@_timed
 def dice_fwd(x, mean, var, alpha, m, n, eps):
     y = torch.empty_like(x)
     _lib_call("dice_fwd", ptr(x), ptr(mean), ptr(var), ptr(alpha), ptr(y), m, n, eps, stream())
     return y
 
 
+@_timed
 def dice_bwd(x, mean, var, alpha, dy, m, n, eps, training):
     dx = torch.empty_like(x)
     dalpha = torch.empty((n,), dtype=torch.float32, device=x.device)
@@ -1277,6 +1373,7 @@ def dice_bwd(x, mean, var, alpha, dy, m, n, eps, training):
     return dx, dalpha
 
 
+@_timed
 def dropout(x, rate, seed):
     y = torch.empty_like(x)
     _lib_call("dropout", ptr(x), ptr(y), x.numel(), rate, seed & 0xFFFFFFFFFFFFFFFF, stream())
@@ -1296,6 +1393,7 @@ def _mha_desc(q, ldq, k, ldk, v, ldv, batch, T, heads, d, scale, blinding, rate,
     return a
 
 
+@_timed
 def mha_fwd(q, ldq, k, ldk, v, ldv, batch, T, heads, d, scale, blinding=False, rate=0.0, seed=0, res=None, ldr=0,
             qlen=None, klen=None, qmask=None, kmask=None):
     """Masked multi-head attention over rows b*T + t of q / k / v (row pitches ld*) -> (out [B*T, heads*d],
@@ -1311,6 +1409,7 @@ def mha_fwd(q, ldq, k, ldk, v, ldv, batch, T, heads, d, scale, blinding=False, r
     return out, stats
 
 
+@_timed
 def mha_bwd(dout, lddo, q, ldq, k, ldk, v, ldv, stats, batch, T, heads, d, scale, blinding=False, rate=0.0, seed=0,
             qlen=None, klen=None, qmask=None, kmask=None):
     """-> (dq, dk, dv), each [B*T, heads*d]."""
@@ -1325,6 +1424,7 @@ def mha_bwd(dout, lddo, q, ldq, k, ldk, v, ldv, stats, batch, T, heads, d, scale
     return dq, dk, dv
 
 
+@_timed
 def layernorm_fwd(a, lda, b, ldb, gamma, beta, rows, n, eps):
     """LayerNormalization of a (+ b) over rows of n columns -> (y [rows, n], stats (mean, rstd) [rows, 2])."""
     _require_cuda(a, b, gamma, beta)
@@ -1335,6 +1435,7 @@ def layernorm_fwd(a, lda, b, ldb, gamma, beta, rows, n, eps):
     return y, stats
 
 
+@_timed
 def layernorm_bwd(a, lda, b, ldb, gamma, stats, dy, rows, n, want_dgamma=True, want_dbeta=True):
     """-> (dx [rows, n], dgamma [n] | None, dbeta [n] | None)."""
     _require_cuda(a, b, gamma, stats, dy)
@@ -1349,18 +1450,8 @@ def layernorm_bwd(a, lda, b, ldb, gamma, stats, dy, rows, n, want_dgamma=True, w
     return dx, dgamma, dbeta
 
 
-for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
-           "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
-           "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
-           "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "fwfm_fwd", "fwfm_bwd", "fefm_sym",
-           "fefm_fwd", "fefm_bwd", "pnn_inner_fwd", "pnn_inner_bwd", "pnn_outer_fwd", "pnn_outer_bwd",
-           "din_att_input_fwd", "din_att_input_bwd",
-           "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
-           "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
-    globals()[_n] = _timed(globals()[_n])
-
-
 # ---- row-sharded embedding exchange (device side) ----------------------------------------------------
+@_timed
 def shard_bucketize(feats, batch, world):
     """-> (counts int32 [world], slot int64 [B*F]) for the lookups described by feats[f].idx."""
     dev = torch.device("cuda", torch.cuda.current_device())
@@ -1372,6 +1463,7 @@ def shard_bucketize(feats, batch, world):
     return counts, slot
 
 
+@_timed
 def shard_fill(feats, batch, world, counts, slot):
     dev = counts.device
     n = batch * len(feats)
@@ -1386,6 +1478,7 @@ def _ptr_array(tensors):
     return (C.c_void_p * len(tensors))(*[t.data_ptr() if t is not None else None for t in tensors])
 
 
+@_timed
 def shard_gather_rows(tables, lin_tables, dim, keys, n):
     dev = keys.device
     rows = torch.empty((max(n, 1), dim), dtype=torch.float32, device=dev)
@@ -1395,26 +1488,7 @@ def shard_gather_rows(tables, lin_tables, dim, keys, n):
     return rows, lin
 
 
+@_timed
 def shard_scatter_rows(tables, lin_tables, dim, keys, n, grows, glin, scale, lin_scale):
     _lib_call("shard_scatter_rows", _ptr_array(tables), _ptr_array(lin_tables) if lin_tables is not None else None,
               len(tables), dim, ptr(keys), n, ptr(grows), ptr(glin), scale, lin_scale, stream())
-
-
-for _n in ("shard_bucketize", "shard_fill", "shard_gather_rows", "shard_scatter_rows"):
-    globals()[_n] = _timed(globals()[_n])
-
-
-for _n in ("ewise", "cross_vector_fwd", "cross_vector_bwd", "cin_t0", "cin_filter_planes", "cin_gemm", "cin_fold", "cin_t0_bwd", "cin_unpad_rows", "att_gemm",
-           "cin_outer_fwd", "cin_outer_bwd", "cin_sum_d",
-           "cin_expand_grad", "interacting_fwd", "interacting_bwd", "bi_interaction_fwd", "bi_interaction_bwd", "afm_fwd",
-           "afm_bwd", "senet_fwd", "senet_bwd", "bilinear_fwd", "bilinear_bwd", "fwfm_fwd", "fwfm_bwd", "fefm_sym",
-           "fefm_fwd", "fefm_bwd", "pnn_inner_fwd", "pnn_inner_bwd", "pnn_outer_fwd", "pnn_outer_bwd",
-           "din_att_input_fwd", "din_att_input_bwd",
-           "din_pool_fwd", "din_pool_bwd", "seqpool_fwd", "seqpool_bwd", "seqweight", "seqscale", "colstats",
-           "moving_update", "bn_apply", "bn_bwd", "dice_fwd", "dice_bwd", "dropout"):
-    globals()[_n] = _timed(globals()[_n])
-
-
-for _n in ("mha_fwd", "mha_bwd", "layernorm_fwd", "layernorm_bwd", "regulate_fwd", "regulate_bwd",
-           "conv_stack_fwd", "conv_stack_bwd", "field_wise_bi_fwd", "field_wise_bi_bwd"):
-    globals()[_n] = _timed(globals()[_n])

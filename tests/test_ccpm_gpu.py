@@ -284,15 +284,12 @@ def test_one_launch_forward_and_backward(cuda):
     model, x, y = _ccpm_model(conv_kernel_width=(4, 3, 2), conv_filters=(3, 2, 2))
     model.compile(SGD(0.01), "binary_crossentropy", step_graph="off")
     model.predict(x, batch_size=512)
-    K.PROFILE = {}
-    try:
+    with K.profiled() as prof:
         model.predict(x, batch_size=512)
-        fwd = {k: len(v) for k, v in K.PROFILE.items()}
-        K.PROFILE = {}
+    fwd = {k: len(v) for k, v in prof.items()}
+    with K.profiled() as prof:
         model.train_on_batch(x, y)
-        step = {k: len(v) for k, v in K.PROFILE.items()}
-    finally:
-        K.PROFILE = None
+    step = {k: len(v) for k, v in prof.items()}
     assert fwd.get("conv_stack_fwd") == 1 and "conv_stack_bwd" not in fwd, fwd
     assert "copy2d" not in fwd and "ewise" not in fwd, fwd
     assert step.get("conv_stack_fwd") == 1 and step.get("conv_stack_bwd") == 1, step

@@ -181,12 +181,9 @@ def test_inner_bridge_outputs_are_not_materialised(cuda, bridge_type):
     from deepctr_b200 import kernels as K
     model, x = _edcn_model(bridge_type, 3)
     model.predict(x, batch_size=512)                   # warm up: weights, staging buffers
-    K.PROFILE = {}
-    try:
+    with K.profiled() as prof:
         model.predict(x, batch_size=512)
-        launched = {k: len(v) for k, v in K.PROFILE.items()}
-    finally:
-        K.PROFILE = None
+    launched = {k: len(v) for k, v in prof.items()}
     concat = bridge_type == "concatenation"
     assert launched.get("regulate_fwd", 0) == (3 if concat else 4), launched
     assert "ewise" not in launched, launched

@@ -162,15 +162,12 @@ def _launches(model, x, y):
     from deepctr_b200.engine import SGD
     model.compile(SGD(0.01), "binary_crossentropy", step_graph="off")
     model.predict(x, batch_size=512)
-    K.PROFILE = {}
-    try:
+    with K.profiled() as prof:
         model.predict(x, batch_size=512)
-        fwd = {k: len(v) for k, v in K.PROFILE.items()}
-        K.PROFILE = {}
+    fwd = {k: len(v) for k, v in prof.items()}
+    with K.profiled() as prof:
         model.train_on_batch(x, y)
-        step = {k: len(v) for k, v in K.PROFILE.items()}
-    finally:
-        K.PROFILE = None
+    step = {k: len(v) for k, v in prof.items()}
     return fwd, step
 
 

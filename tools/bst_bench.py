@@ -23,7 +23,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import bench  # noqa: E402
-from pairwise_bench import hardware, median_us, HBM_BYTES_PER_S  # noqa: E402
+from harness import HBM_BYTES_PER_S, hardware, kernel_ms, time_train_steps  # noqa: E402
 
 
 def step_time(builder, steps, warmup):
@@ -39,26 +39,11 @@ def step_time(builder, steps, warmup):
         model = bench.build_model(cfg)
     bench.seed_initializers(model)
     model.compile(SGD(bench.LR), "binary_crossentropy", embedding_update="sparse")
-    dev = torch.device("cuda", 0)
-    batches = [bench.device_inputs(cfg, x, y, dev) for x, y in bench.synth_batches(cfg, bench.N_BATCHES)]
-    i = 0
-    while i < warmup or (i < warmup + bench.N_BATCHES + 4 and model._graph_eligible()
-                         and len(model._step_graphs) < bench.N_BATCHES):
-        model.train_step(*batches[i % bench.N_BATCHES])
-        i += 1
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(steps):
-        model.train_step(*batches[(i + k) % bench.N_BATCHES])
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
-    res = {"what": "train_step", "model": builder, "batch": cfg["batch"], "steps": steps,
-           "graph_replayed": bool(model._step_graphs), "ms_per_step": ms, "samples_per_s": cfg["batch"] / ms * 1e3}
-    del model, batches
+    ms, replayed, _ = time_train_steps(model, cfg, steps, warmup)
+    del model
     torch.cuda.empty_cache()
-    return res
+    return {"what": "train_step", "model": builder, "batch": cfg["batch"], "steps": steps, "graph_replayed": replayed,
+            "ms_per_step": ms, "samples_per_s": cfg["batch"] / ms * 1e3}
 
 
 def kernels(reps, hw):
@@ -96,9 +81,10 @@ def kernels(reps, hw):
     ]
     res = []
     for name, fn, flops, nbytes in cases:
-        med, lo, hi = median_us(fn, reps)
+        ts = np.array(kernel_ms(fn, reps)) * 1e3
+        med = float(np.median(ts))
         r = {"what": "kernel", "kernel": name, "shape": "B=%d T=%d E=%d heads=%d" % (B, T, E, H),
-             "median_us": med, "min_us": lo, "max_us": hi, "bytes": nbytes,
+             "median_us": med, "min_us": float(ts.min()), "max_us": float(ts.max()), "bytes": nbytes,
              "hbm_bound_us": nbytes / HBM_BYTES_PER_S * 1e6}
         if flops is not None:
             r["flops"] = flops

@@ -18,15 +18,16 @@ import json
 import os
 import sys
 
+import numpy as np
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import bench  # noqa: E402
-from onn_bench import _median_ms  # noqa: E402
-from pairwise_bench import hardware  # noqa: E402
+from harness import HBM_BYTES_PER_S as HBM, hardware, kernel_ms, time_train_steps  # noqa: E402
 
-HBM, FFMA = 3.35e12, 67e12
+FFMA = 67e12
 CFG = dict(bench.CONFIGS["c2"], dim=32, n_dense=0,
            workload="CCPM synthetic Criteo: 26 fields x 1M ids, E=32, batch=65536, no dense, reference defaults")
 STACK = [("conv", 6, 4, "tanh"), ("kmax", 13), ("conv", 5, 4, "tanh"), ("kmax", 3)]
@@ -74,7 +75,7 @@ def kernels(reps):
             ("conv_stack_bwd", lambda: K.conv_stack_bwd(stages, x, F, E, 1, B, dy, dx=dx, dx_accumulate=True,
                                                         want_dw=[True, False, True, False]),
              B * 4 * (F * E + w_out + 2 * F * E), fma_b * B * E)):
-        ms = _median_ms(fn, reps)
+        ms = float(np.median(kernel_ms(fn, reps)))
         hb, fb = nbytes / HBM * 1e3, 2 * fma / FFMA * 1e3
         out.append({"what": "kernel", "kernel": name, "batch": B, "fields": F, "dim": E, "ms": ms, "bytes": nbytes,
                     "fma": fma, "hbm_bound_ms": hb, "ffma_bound_ms": fb, "x_bound": ms / max(hb, fb)})
@@ -92,28 +93,11 @@ def step(builder, steps, warmup):
     model = getattr(M, builder)(cols, cols, l2_reg_linear=0, l2_reg_embedding=0)
     bench.seed_initializers(model)
     model.compile(SGD(bench.LR), "binary_crossentropy", embedding_update="sparse")
-    dev = torch.device("cuda", 0)
-    batches = [bench.device_inputs(CFG, x, y, dev) for x, y in bench.synth_batches(CFG, bench.N_BATCHES)]
-    i = 0
-    while i < warmup or (i < warmup + bench.N_BATCHES + 4 and model._graph_eligible()
-                         and len(model._step_graphs) < bench.N_BATCHES):
-        model.train_step(*batches[i % bench.N_BATCHES])
-        i += 1
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(steps):
-        model.train_step(*batches[(i + k) % bench.N_BATCHES])
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
-    model._check_ids()
-    res = {"what": "train_step", "model": builder, "workload": CFG["workload"], "batch": CFG["batch"],
-           "steps": steps, "graph_replayed": bool(model._step_graphs), "ms_per_step": ms,
-           "samples_per_s": CFG["batch"] / ms * 1e3}
-    del model, batches
+    ms, replayed, _ = time_train_steps(model, CFG, steps, warmup)
+    del model
     torch.cuda.empty_cache()
-    return res
+    return {"what": "train_step", "model": builder, "workload": CFG["workload"], "batch": CFG["batch"],
+            "steps": steps, "graph_replayed": replayed, "ms_per_step": ms, "samples_per_s": CFG["batch"] / ms * 1e3}
 
 
 def main():

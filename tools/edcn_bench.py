@@ -13,6 +13,7 @@ Prints one JSON line per measurement:
 """
 import argparse
 import contextlib
+import functools
 import json
 import os
 import sys
@@ -24,10 +25,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import bench  # noqa: E402
-from onn_bench import _median_ms  # noqa: E402
-from pairwise_bench import hardware  # noqa: E402
+from harness import HBM_BYTES_PER_S as HBM, hardware, kernel_ms, time_train_steps  # noqa: E402
 
-HBM = 3.35e12
 CFG = dict(bench.CONFIGS["c2"], dim=16, n_dense=0,
            workload="EDCN synthetic Criteo: 26 fields x 1M ids, E=16, batch=65536, no dense, cross_num=2")
 BRIDGES = ("pointwise_addition", "hadamard_product", "concatenation", "attention_pooling")
@@ -48,16 +47,17 @@ def kernels(reps):
     out = []
     for mode, n_in in N_IN.items():
         x, h, ax, ah = [ops_[k] if k < n_in else None for k in range(4)]
-        ms = _median_ms(lambda: K.regulate_fwd(mode, F, E, B, x, h, ax, ah, gates, y0=(y0, 0), y1=(y1, 0)), reps)
+        fwd = functools.partial(K.regulate_fwd, mode, F, E, B, x, h, ax, ah, gates, y0=(y0, 0), y1=(y1, 0))
+        ms = float(np.median(kernel_ms(fwd, reps)))
         nbytes = B * d * 4 * (n_in + 2)
         out.append({"what": "kernel", "kernel": "regulate_fwd", "mode": mode, "outputs": "y0,y1", "batch": B,
                     "fields": F, "dim": E, "ms": ms, "bytes": nbytes, "hbm_bound_ms": nbytes / HBM * 1e3,
                     "x_hbm_bound": ms / (nbytes / HBM * 1e3)})
         acc = mode == "copy"             # layer 0 adds dx to the gather buffer's gradient
-        ms = _median_ms(lambda: K.regulate_bwd(mode, F, E, B, x, h, ax, ah, gates, dy0=(dy0, 0), dy1=(dy1, 0),
-                                               dx=dx if acc else None, dx_accumulate=acc, want_dh=h is not None,
-                                               want_dax=ax is not None, want_dah=ah is not None,
-                                               want_dg=(True, True)), reps)
+        bwd = functools.partial(K.regulate_bwd, mode, F, E, B, x, h, ax, ah, gates, dy0=(dy0, 0), dy1=(dy1, 0),
+                                dx=dx if acc else None, dx_accumulate=acc, want_dh=h is not None,
+                                want_dax=ax is not None, want_dah=ah is not None, want_dg=(True, True))
+        ms = float(np.median(kernel_ms(bwd, reps)))
         nbytes = B * d * 4 * (n_in + 2 + n_in + (1 if acc else 0))
         out.append({"what": "kernel", "kernel": "regulate_bwd", "mode": mode, "outputs": "y0,y1", "batch": B,
                     "fields": F, "dim": E, "ms": ms, "bytes": nbytes, "hbm_bound_ms": nbytes / HBM * 1e3,
@@ -77,28 +77,12 @@ def step(bridge_type, steps, warmup):
         model = M.EDCN(cols, cols, cross_num=2, bridge_type=bridge_type, l2_reg_linear=0, l2_reg_embedding=0)
     bench.seed_initializers(model)
     model.compile(SGD(bench.LR), "binary_crossentropy", embedding_update="sparse")
-    dev = torch.device("cuda", 0)
-    batches = [bench.device_inputs(CFG, x, y, dev) for x, y in bench.synth_batches(CFG, bench.N_BATCHES)]
-    i = 0
-    while i < warmup or (i < warmup + bench.N_BATCHES + 4 and model._graph_eligible()
-                         and len(model._step_graphs) < bench.N_BATCHES):
-        model.train_step(*batches[i % bench.N_BATCHES])
-        i += 1
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(steps):
-        model.train_step(*batches[(i + k) % bench.N_BATCHES])
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
-    model._check_ids()
-    res = {"what": "train_step", "model": "EDCN", "bridge_type": bridge_type, "workload": CFG["workload"],
-           "batch": CFG["batch"], "steps": steps, "graph_replayed": bool(model._step_graphs), "ms_per_step": ms,
-           "samples_per_s": CFG["batch"] / ms * 1e3}
-    del model, batches
+    ms, replayed, _ = time_train_steps(model, CFG, steps, warmup)
+    del model
     torch.cuda.empty_cache()
-    return res
+    return {"what": "train_step", "model": "EDCN", "bridge_type": bridge_type, "workload": CFG["workload"],
+            "batch": CFG["batch"], "steps": steps, "graph_replayed": replayed, "ms_per_step": ms,
+            "samples_per_s": CFG["batch"] / ms * 1e3}
 
 
 def main():

@@ -21,29 +21,13 @@ import json
 import os
 import sys
 
+import numpy as np
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from pairwise_bench import hardware  # noqa: E402
-
-HBM_BYTES_PER_S = 3.35e12
-
-
-def median_us(fn, reps):
-    import torch
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        e1.synchronize()
-        ts.append(e0.elapsed_time(e1) * 1e3)
-    ts.sort()
-    return ts[len(ts) // 2]
+from harness import HBM_BYTES_PER_S, hardware, kernel_ms  # noqa: E402
 
 
 def main():
@@ -117,7 +101,7 @@ def main():
         runs["scatter+S"] = lambda: K.embed_scatter_uniform_bwd(b_full, dx, dfm, dlin, -1e-3, -1e-3, B,
                                                                 fm_sum=p_full.fm_sum)
     print(json.dumps(dict(hardware(), shape=dict(F=F, V=V, E=E, ndense=ND, batch=B), tree=ROOT)), flush=True)
-    us = {k: median_us(fn, a.reps) for k, fn in runs.items()}
+    us = {k: float(np.median(kernel_ms(fn, a.reps))) * 1e3 for k, fn in runs.items()}
     ceil = {k: traffic[k] * B / (us[k] * 1e-6) for k in ("copy", "red")}
     for k, t in us.items():
         nbytes = traffic[k] * B

@@ -20,15 +20,15 @@ import json
 import os
 import sys
 
+import numpy as np
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import bench  # noqa: E402
-from onn_bench import _median_ms  # noqa: E402
-from pairwise_bench import hardware  # noqa: E402
+from harness import HBM_BYTES_PER_S as HBM, hardware, kernel_ms, launch_list, time_train_steps  # noqa: E402
 
-HBM = 3.35e12
 C2 = dict(bench.CONFIGS["c2"], dim=32)
 RUN_FLEN_GROUPS = ("context", "user", "context", "context", "context", "context", "item", "item", "item", "user",
                    "user", "user", "context", "user", "user", "user", "user", "user", "user", "user", "user")
@@ -65,8 +65,7 @@ def kernels(reps):
                                                               dx=dx, dx_accumulate=True, want_dkernel=(True, True),
                                                               want_dbias=(True, True)),
              B * 4 * (F * E + E + 2 * F * E))):
-        fn()
-        ms = _median_ms(fn, reps)
+        ms = float(np.median(kernel_ms(fn, reps)))
         hb = nbytes / HBM * 1e3
         out.append({"what": "kernel", "kernel": name, "batch": B, "fields": F, "groups": 3, "dim": E, "ms": ms,
                     "bytes": nbytes, "hbm_bound_ms": hb, "x_bound": ms / hb})
@@ -91,49 +90,22 @@ def step(name, steps, warmup):
     import torch
     cfg, groups = SHAPES[name]
     model = _model(cfg, groups)
-    dev = torch.device("cuda", 0)
-    batches = [bench.device_inputs(cfg, x, y, dev) for x, y in bench.synth_batches(cfg, bench.N_BATCHES)]
-    i = 0
-    while i < warmup or (i < warmup + bench.N_BATCHES + 4 and model._graph_eligible()
-                         and len(model._step_graphs) < bench.N_BATCHES):
-        model.train_step(*batches[i % bench.N_BATCHES])
-        i += 1
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(steps):
-        model.train_step(*batches[(i + k) % bench.N_BATCHES])
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
-    model._check_ids()
-    res = {"what": "train_step", "model": "FLEN", "shape": name, "workload": cfg["workload"], "batch": cfg["batch"],
-           "steps": steps, "graph_replayed": bool(model._step_graphs), "ms_per_step": ms,
-           "samples_per_s": cfg["batch"] / ms * 1e3}
-    del model, batches
-    torch.cuda.empty_cache()
-    return res
-
-
-def launch_list(name):
-    import torch
-    from deepctr_b200 import kernels as K
-    cfg, groups = SHAPES[name]
-    model = _model(cfg, groups, step_graph="off")
-    dev = torch.device("cuda", 0)
-    (x, y), = bench.synth_batches(cfg, 1)
-    batch = bench.device_inputs(cfg, x, y, dev)
-    model.train_step(*batch)
-    K.PROFILE = {}
-    try:
-        model.train_step(*batch)
-        prof = K.profile_summary()
-    finally:
-        K.PROFILE = None
+    ms, replayed, _ = time_train_steps(model, cfg, steps, warmup)
     del model
     torch.cuda.empty_cache()
-    return {"what": "launch_list", "shape": name, "step": {k: {"launches": n, "ms": round(ms, 4)}
-                                                           for k, (n, ms) in sorted(prof.items())}}
+    return {"what": "train_step", "model": "FLEN", "shape": name, "workload": cfg["workload"], "batch": cfg["batch"],
+            "steps": steps, "graph_replayed": replayed, "ms_per_step": ms, "samples_per_s": cfg["batch"] / ms * 1e3}
+
+
+def step_launches(name):
+    import torch
+    cfg, groups = SHAPES[name]
+    model = _model(cfg, groups, step_graph="off")
+    (x, y), = bench.synth_batches(cfg, 1)
+    launches = launch_list(model, bench.device_inputs(cfg, x, y, torch.device("cuda", 0)))
+    del model
+    torch.cuda.empty_cache()
+    return {"what": "launch_list", "shape": name, "step": launches}
 
 
 def main():
@@ -150,7 +122,7 @@ def main():
         print(json.dumps(r), flush=True)
     for name in SHAPES:
         print(json.dumps(step(name, a.steps, a.warmup)), flush=True)
-    print(json.dumps(launch_list("c2_interleaved")), flush=True)
+    print(json.dumps(step_launches("c2_interleaved")), flush=True)
 
 
 if __name__ == "__main__":

@@ -25,23 +25,9 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import bench  # noqa: E402
-from pairwise_bench import hardware  # noqa: E402
+from harness import HBM_BYTES_PER_S as HBM, hardware, kernel_ms, time_train_steps  # noqa: E402
 
-HBM = 3.35e12
 CFG = dict(bench.CONFIGS["c2"], dim=4, workload="ONN synthetic Criteo: 26 fields x 1M ids, E=4, batch=65536, 13 dense")
-
-
-def _median_ms(fn, reps):
-    import torch
-    ts = []
-    for _ in range(reps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ts.append(e0.elapsed_time(e1))
-    return float(np.median(ts))
 
 
 def kernels(reps):
@@ -64,7 +50,7 @@ def kernels(reps):
         w = P if reduce_sum else P * E
         o = torch.empty((B, (w + 3) // 4 * 4), device=dev)      # the planner's pitch: a multiple of 4 floats
         fields = [K.ffm_field(idx=i, vocab=V) for i in ids]
-        ms = _median_ms(lambda: K.ffm_product_fwd(fields, ptrs, E, reduce_sum, o, 0, B), reps)
+        ms = float(np.median(kernel_ms(lambda: K.ffm_product_fwd(fields, ptrs, E, reduce_sum, o, 0, B), reps)))
         alg = B * (F * idb + 2 * P * row + w * 4)
         sec = B * (F * idb + 2 * P * sector + w * 4)
         out.append({"what": "kernel", "kernel": "ffm_product_fwd", "mode": "reduce_sum" if reduce_sum else
@@ -74,7 +60,7 @@ def kernels(reps):
     g = torch.randn((B, P * E), device=dev)
     scratch = torch.empty((B, F * (F - 1) * E), device=dev)
     fields = [K.ffm_field(idx=i, vocab=V, grad=scratch[:, a * (F - 1) * E:]) for a, i in enumerate(ids)]
-    ms = _median_ms(lambda: K.ffm_product_bwd(fields, ptrs, E, False, g, 0, B), reps)
+    ms = float(np.median(kernel_ms(lambda: K.ffm_product_bwd(fields, ptrs, E, False, g, 0, B), reps)))
     alg = B * (F * idb + P * E * 4 + 2 * P * row + 2 * P * row)
     sec = B * (F * idb + P * E * 4 + 2 * P * sector + 2 * P * row)
     out.append({"what": "kernel", "kernel": "ffm_product_bwd", "mode": "elementwise", "batch": B, "fields": F,
@@ -92,7 +78,7 @@ def kernels(reps):
     def scatter():
         for c in range(0, len(feats), L.MAX_FEATURES):
             K.embed_scatter_add(feats[c:c + L.MAX_FEATURES], B, -1e-6)
-    ms = _median_ms(scatter, reps)
+    ms = float(np.median(kernel_ms(scatter, reps)))
     # reads the scratch and the ids, read-modify-writes 650 rows (each a 32 B sector) per sample
     alg = B * (2 * P * row + 2 * P * idb + 2 * 2 * P * row)
     out.append({"what": "kernel", "kernel": "embed_scatter_add (ONN scratch, fused SGD)", "batch": B,
@@ -104,7 +90,6 @@ def kernels(reps):
 
 
 def step(steps, warmup):
-    import torch
     from deepctr_b200 import engine as E, models as M
     from deepctr_b200.engine import SGD
     cols = bench.feature_columns(CFG)
@@ -112,25 +97,9 @@ def step(steps, warmup):
     model = M.ONN(cols, cols, dnn_hidden_units=(256, 128, 64), l2_reg_linear=0, l2_reg_embedding=0)
     bench.seed_initializers(model)
     model.compile(SGD(bench.LR), "binary_crossentropy", embedding_update="sparse")
-    dev = torch.device("cuda", 0)
-    batches = [bench.device_inputs(CFG, x, y, dev) for x, y in bench.synth_batches(CFG, bench.N_BATCHES)]
-    i = 0
-    while i < warmup or (i < warmup + bench.N_BATCHES + 4 and model._graph_eligible()
-                         and len(model._step_graphs) < bench.N_BATCHES):
-        model.train_step(*batches[i % bench.N_BATCHES])
-        i += 1
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(steps):
-        model.train_step(*batches[(i + k) % bench.N_BATCHES])
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
-    model._check_ids()
+    ms, replayed, _ = time_train_steps(model, CFG, steps, warmup)
     return {"what": "train_step", "model": "ONN", "workload": CFG["workload"], "batch": CFG["batch"],
-            "steps": steps, "graph_replayed": bool(model._step_graphs), "ms_per_step": ms,
-            "samples_per_s": CFG["batch"] / ms * 1e3}
+            "steps": steps, "graph_replayed": replayed, "ms_per_step": ms, "samples_per_s": CFG["batch"] / ms * 1e3}
 
 
 def main():

@@ -29,7 +29,6 @@ Prints one JSON line per measurement:
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -38,26 +37,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import bench  # noqa: E402
+from harness import HBM_BYTES_PER_S, hardware, kernel_ms, time_train_steps  # noqa: E402
 
-HBM_BYTES_PER_S = 3.35e12
 # --models PNN: the three product configurations timed
 PNN_STEPS = {"PNN-inner": dict(use_inner=True, use_outter=False),
              "PNN-outer-mat": dict(use_inner=False, use_outter=True, kernel_type="mat"),
              "PNN-inner-outer-mat": dict(use_inner=True, use_outter=True, kernel_type="mat")}
-
-
-def hardware():
-    import torch
-    out = {"card": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
-                            "-i", "0"], capture_output=True, text=True, timeout=30).stdout.strip().split(",")
-        out["power_limit_w"] = float(q[0])
-        out["max_sm_clock_mhz"] = float(q[1])
-    except Exception as e:      # the numbers are then reported as unknown, never guessed
-        out["power_limit_w"] = out["max_sm_clock_mhz"] = None
-        out["query_error"] = repr(e)
-    return out
 
 
 def step_time(builder, steps, warmup):
@@ -86,42 +71,11 @@ def step_time(builder, steps, warmup):
         model = M.AFM(cols, cols, attention_factor=8, l2_reg_linear=0, l2_reg_embedding=0, l2_reg_att=0)
     bench.seed_initializers(model)
     model.compile(SGD(bench.LR), "binary_crossentropy", embedding_update="sparse")
-    dev = torch.device("cuda", 0)
-    batches = [bench.device_inputs(cfg, x, y, dev) for x, y in bench.synth_batches(cfg, bench.N_BATCHES)]
-    i = 0
-    while i < warmup or (i < warmup + bench.N_BATCHES + 4 and model._graph_eligible()
-                         and len(model._step_graphs) < bench.N_BATCHES):
-        model.train_step(*batches[i % bench.N_BATCHES])
-        i += 1
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(steps):
-        loss = model.train_step(*batches[(i + k) % bench.N_BATCHES])
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / steps
-    res = {"what": "train_step", "model": builder, "batch": cfg["batch"], "steps": steps,
-           "graph_replayed": bool(model._step_graphs), "ms_per_step": ms,
-           "samples_per_s": cfg["batch"] / ms * 1e3, "loss": float(loss[0]) if isinstance(loss, tuple) else None}
-    del model, batches
+    ms, replayed, loss = time_train_steps(model, cfg, steps, warmup)
+    del model
     torch.cuda.empty_cache()
-    return res
-
-
-def median_us(fn, reps):
-    import torch
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ts.append(a.elapsed_time(b) * 1e3)
-    return float(np.median(ts)), float(np.min(ts)), float(np.max(ts))
+    return {"what": "train_step", "model": builder, "batch": cfg["batch"], "steps": steps, "graph_replayed": replayed,
+            "ms_per_step": ms, "samples_per_s": cfg["batch"] / ms * 1e3, "loss": loss}
 
 
 def kernels(reps, hw):
@@ -154,21 +108,15 @@ def kernels(reps, hw):
         ("bi_interaction_bwd", lambda: K.bi_interaction_bwd(xw, ld, F, E, gatt, B),
          B * F * E * 3, B * (2 * x_bytes + E * 4)),
     ]
-    out = []
-    for name, fn, flops, nbytes in cases:
-        med, lo, hi = median_us(fn, reps)
-        r = {"what": "kernel", "kernel": name, "shape": dict(B=B, F=F, E=E, A=A, ldx=ld), "reps": reps,
-             "median_us": med, "min_us": lo, "max_us": hi, "flops": flops, "bytes": nbytes,
-             "hbm_bound_us": nbytes / HBM_BYTES_PER_S * 1e6,
-             "ffma_bound_us": flops / ffma_peak * 1e6 if ffma_peak else None}
-        out.append(r)
-    return out
+    shape = dict(B=B, F=F, E=E, A=A, ldx=ld)
+    return [_report(name, shape, reps, fn, flops, nbytes, ffma_peak) for name, fn, flops, nbytes in cases]
 
 
 def _report(name, shape, reps, fn, flops, nbytes, ffma_peak):
-    med, lo, hi = median_us(fn, reps)
-    return {"what": "kernel", "kernel": name, "shape": shape, "reps": reps, "median_us": med, "min_us": lo,
-            "max_us": hi, "flops": flops, "bytes": nbytes, "hbm_bound_us": nbytes / HBM_BYTES_PER_S * 1e6,
+    ts = np.array(kernel_ms(fn, reps)) * 1e3
+    return {"what": "kernel", "kernel": name, "shape": shape, "reps": reps, "median_us": float(np.median(ts)),
+            "min_us": float(ts.min()), "max_us": float(ts.max()), "flops": flops, "bytes": nbytes,
+            "hbm_bound_us": nbytes / HBM_BYTES_PER_S * 1e6,
             "ffma_bound_us": flops / ffma_peak * 1e6 if ffma_peak else None}
 
 
