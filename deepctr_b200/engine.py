@@ -792,10 +792,6 @@ class Conv2D(Layer):
         return ("conv", self.kernel_size[0], self.filters, self.activation, self.kernel, self.bias)
 
     def call(self, inputs, **kwargs):
-        planner = getattr(self, "_planner", None)
-        served = planner.conv_stacked(self, inputs) if planner is not None else None
-        if served is not None:
-            return served
         b, rows, dim, channels = inputs.data.shape
         return ops.conv_stack(inputs, [self.stage()], rows, dim, channels, (b, rows, dim, self.filters))
 
@@ -1241,6 +1237,9 @@ class Model(object):
                 continue
             if node is upto:
                 break
+            launch = self.planner.launches.get(id(node))
+            if launch is not None:        # a fused chain's first node: one launch serves it and the later nodes
+                self.planner.results.update(launch(values, training))
             planned = self.planner.results.get(id(node))
             if planned is not None:       # served by the fused embedding launch (inputs.EmbeddingPlanner)
                 values[id(node.outputs[0])] = planned

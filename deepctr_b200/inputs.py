@@ -17,6 +17,7 @@ Concatenations of those windows are then zero-copy views, and the backward pass 
 scatter (+ SGD update) launch.
 """
 from collections import defaultdict, OrderedDict
+import functools
 import itertools
 from itertools import chain
 
@@ -249,6 +250,36 @@ class _Slot(object):
                  "mask_zero")
 
 
+class _Graph(object):
+    """The model graph as the planner passes query it: every tensor's consumer nodes, the model outputs and how many
+    times each layer is called."""
+
+    def __init__(self, model):
+        self.order = model._order
+        self.consumers = defaultdict(list)
+        self.calls = defaultdict(int)
+        for node in model._order:
+            self.calls[id(node.layer)] += 1
+            for t in E._flatten(node.inputs):
+                self.consumers[id(t)].append(node)
+        self.out_ids = set(id(t) for t in E._flatten(model.outputs))
+        self.input_names = set(t.name for t in model.inputs)
+
+    def only_use(self, t):
+        """The node of ``t``'s only use, when it has one and ``t`` is not a model output, else None."""
+        cs = self.consumers[id(t)]
+        return cs[0] if len(cs) == 1 and id(t) not in self.out_ids else None
+
+    def only(self, t, cls):
+        """The single consumer node of ``t`` when its layer is a ``cls`` called once, else None."""
+        c = self.only_use(t)
+        return c if c is not None and isinstance(c.layer, cls) and self.calls[id(c.layer)] == 1 else None
+
+    def input_name(self, t):
+        """The model input's name when ``t`` is one, else None."""
+        return t.name if (isinstance(t.node.layer, E.InputLayer) and t.name in self.input_names) else None
+
+
 class EmbeddingPlanner(object):
     def __init__(self, model):
         from .layers.utils import Hash
@@ -265,18 +296,9 @@ class EmbeddingPlanner(object):
         self.fm_result = None
         self.lin_result = None
         self._plans = {}
-        consumers = defaultdict(list)
-        for node in model._order:
-            for t in E._flatten(node.inputs):
-                consumers[id(t)].append(node)
-        out_ids = set(id(t) for t in E._flatten(model.outputs))
-        input_names = set(t.name for t in model.inputs)
-
-        def as_input(t):
-            return t.name if (isinstance(t.node.layer, E.InputLayer) and t.name in input_names) else None
-
+        g = _Graph(model)
         # ONN's field-aware lookups and their products: one kernel pair of their own, never slots of the gather
-        self.ffm = _plan_field_aware(model, consumers, out_ids, as_input)
+        self.ffm = _plan_field_aware(g)
         claimed = self.ffm.claimed if self.ffm is not None else ()
         for node in model._order:
             if not isinstance(node.layer, Embedding) or not isinstance(node.inputs, E.KTensor):
@@ -286,9 +308,9 @@ class EmbeddingPlanner(object):
             src, hcfg, virt = node.inputs, None, []
             if isinstance(src.node.layer, Hash) and isinstance(src.node.inputs, E.KTensor):
                 h = src.node.layer
-                if len(consumers[id(src)]) == 1 and id(src) not in out_ids:
+                if g.only_use(src):
                     hcfg, virt, src = h, [src.node], src.node.inputs
-            name = as_input(src)
+            name = g.input_name(src)
             if name is None:
                 continue
             if hcfg is not None and (hcfg.vocabulary_path or src.dtype in ("string", str)):
@@ -304,22 +326,20 @@ class EmbeddingPlanner(object):
             s.pool, s.mask_mode, s.len_name, s.weight_name, s.weight_mode = L.POOL_NONE, L.MASK_NONE, None, None, L.WEIGHT_NONE
             s.node, s.virtual_nodes = node, list(virt)
             out_t = node.outputs[0]
-            cons = consumers[id(out_t)]
+            c = g.only_use(out_t)
             # --- pooled-bag patterns of get_varlen_pooling_list (inputs.py:133-158) ----------------
-            if len(cons) == 1 and id(out_t) not in out_ids:
-                c = cons[0]
+            if c is not None:
                 wnode = None
                 if isinstance(c.layer, WeightedSequenceLayer) and E._flatten(c.inputs)[0] is out_t:
                     wins = E._flatten(c.inputs)
-                    wt = c.outputs[0]
-                    wc = consumers[id(wt)]
-                    if (len(wc) == 1 and id(wt) not in out_ids and isinstance(wc[0].layer, SequencePoolingLayer)
-                            and all(as_input(t) for t in wins[1:])):
-                        wnode, c = c, wc[0]
+                    pc = g.only_use(c.outputs[0])
+                    if (pc is not None and isinstance(pc.layer, SequencePoolingLayer)
+                            and all(g.input_name(t) for t in wins[1:])):
+                        wnode, c = c, pc
                 if isinstance(c.layer, SequencePoolingLayer):
                     pins = E._flatten(c.inputs)
                     first = wnode.outputs[0] if wnode is not None else out_t
-                    ok = pins[0] is first and all(as_input(t) for t in pins[1:])
+                    ok = pins[0] is first and all(g.input_name(t) for t in pins[1:])
                     pl = c.layer
                     if ok and pl.supports_masking and not s.mask_zero:
                         ok = False   # reference raises at run time: input must carry a mask
@@ -357,21 +377,26 @@ class EmbeddingPlanner(object):
             if t.dtype in ("float32", "float64", "float16") and len(t.shape) == 2:
                 self.tail_reserve += int(t.shape[1])
         # DeepFEFM's FEFM scores go behind the dense columns (fefm_place): P more columns in the row pitch
-        self.fefm_places = _plan_fefm_input(model, consumers, out_ids)
+        self.fefm_places = _plan_fefm_input(g)
         # PNN's inner / outer products go between the embeddings and the dense columns (pnn_place): P per product
         # more columns in the row pitch
-        self.pnn_places, self.pnn_cols = _plan_pnn_input(model, consumers, out_ids)
+        self.pnn_places, self.pnn_cols = _plan_pnn_input(g)
         self.main_ld = (self.main_width + self.tail_reserve + sum(self.fefm_places.values()) + self.pnn_cols
                         + 3) // 4 * 4
         self.lin_ld = max(1, (self.lin_width + 3) // 4 * 4)
         self.fast = self._fast_eligible()
-        self.dnn_places = _plan_dnn_input(model, consumers, out_ids)
+        self.dnn_places = _plan_dnn_input(g)
         # EDCN's RegulationModule pairs and the bridges in front of them: one b2ctr_regulate launch each
-        self.regulate_plan = _plan_regulate(model, consumers, out_ids)
+        self.regulate_plan = _plan_regulate(g)
         # CCPM's Lambda(expand_dims) -> [Conv2D -> KMaxPooling(axis=1)] x l -> Flatten: one b2ctr_conv_stack launch
-        self.conv_plan = _plan_conv_stack(model, consumers, out_ids)
+        self.conv_plan = _plan_conv_stack(g)
         # FLEN's FieldWiseBiInteraction on concatenations of gather-buffer windows: one launch reading them in place
-        self.field_wise_plan = _plan_field_wise(model, consumers, out_ids, self.main)
+        self.field_wise_plan = _plan_field_wise(g, self.main)
+        # {id(first node of a fused chain): (values, training) -> {id(node): result}}: Model._run makes the launch
+        # when it reaches that node, and the results serve it and the chain's later nodes
+        self.launches = {}
+        for plan in (self.regulate_plan, self.conv_plan, self.field_wise_plan):
+            self.launches.update(plan.launches())
         # IFM / DIFM scale the linear lookups by per-sample field weights before Linear sums them: their rows are
         # needed, so they are never fused into the gather's row-sum (lin_hint)
         from .layers.utils import RefineWeight
@@ -652,8 +677,8 @@ class EmbeddingPlanner(object):
             for vn in s.virtual_nodes:
                 if vn is not s.node:
                     self.results[id(vn)] = VIRTUAL
-        for node in self.field_wise_plan.virtual:      # never formed: a Var without data
-            self.results[id(node)] = E.Var(None, vshape=(batch,) + tuple(node.outputs[0].shape[1:]))
+        for node in self.field_wise_plan.virtual:      # folded into the FieldWiseBiInteraction launch
+            self.results[id(node)] = VIRTUAL
         if grad:
             outs = [b for b in bufs.values()]
             if self.fm_result is not None:
@@ -878,58 +903,6 @@ class EmbeddingPlanner(object):
         P = f * (f - 1) // 2
         return ops._window(base, self.main_width + rel, P, (b, P))
 
-    def regulated(self, layer, x):
-        """RegulationModule ``layer`` on ``x``: when the planner pairs it with a second module reading the same tensor,
-        one launch writes both gated outputs; the partner's becomes that node's result.  Else None."""
-        from . import ops
-        p = self.regulate_plan.pairs.get(id(layer))
-        if p is None:
-            return None
-        partner, node = p
-        _, (y0, y1) = ops.regulate("copy", x, gates=[(layer.g, layer.tau), (partner.g, partner.tau)], want_u=False)
-        self.results[id(node)] = y1
-        return y0
-
-    def bridged(self, layer, mode, operands):
-        """BridgeModule ``layer`` whose output reaches only Reshape -> two RegulationModules: one launch writes the two
-        gated outputs as those modules' results, the bridge output and its reshape are never written (VIRTUAL).
-        Else None."""
-        from . import ops
-        plan = self.regulate_plan.bridges.get(id(layer))
-        if plan is None:
-            return None
-        reshape, regs = plan
-        _, ys = ops.regulate(mode, *operands, gates=[(l.g, l.tau) for l, _ in regs], want_u=False)
-        self.results[id(reshape)] = VIRTUAL
-        for (_, node), y in zip(regs, ys):
-            self.results[id(node)] = y
-        return VIRTUAL
-
-    def conv_stacked(self, layer, x):
-        """The first Conv2D of a chain the planner claimed (ConvStackPlan): one launch runs every Conv2D and
-        KMaxPooling of the chain on ``x`` and becomes the last KMaxPooling's result; the maps between are never
-        written (VIRTUAL).  Else None."""
-        from . import ops
-        chain = self.conv_plan.chains.get(id(layer))
-        if chain is None:
-            return None
-        b, rows, dim, channels = x.data.shape
-        last = chain[-1]
-        res = ops.conv_stack(x, [n.layer.stage() for n in chain], rows, dim, channels,
-                             (b,) + tuple(last.outputs[0].shape[1:]))
-        for n in chain[1:-1]:
-            self.results[id(n)] = VIRTUAL
-        self.results[id(last)] = res
-        return VIRTUAL
-
-    def field_wise_groups(self, layer):
-        """FieldWiseBiInteraction ``layer`` the planner claimed (FieldWisePlan): its groups as lists of this step's
-        gather-buffer windows, to be read in place (the groups' concatenations are Vars without data).  Else None."""
-        groups = self.field_wise_plan.groups.get(id(layer))
-        if groups is None:
-            return None
-        return [[self.results[id(n)] for n in g] for g in groups]
-
     def append_dense(self, emb_flat, dense_flat):
         """combined_dnn_input: place the dense features behind the embeddings (and PNN's placed products) in the
         main buffer so the DNN input is a zero-copy window.  Returns the window or None."""
@@ -1042,7 +1015,7 @@ class DnnInputPlacement(object):
 DNN_INPUT_PLACEMENT = True
 
 
-def _plan_fefm_input(model, consumers, out_ids):
+def _plan_fefm_input(g):
     """{id(FEFMLayer): P} for DeepFEFM's DNN input concat([combined_dnn_input(...), NoMask(FEFM(x))], axis=1)
     (deepctr/models/deepfefm.py:64-78) when that concatenation reaches only the DNN: the planner then reserves the
     P score columns behind the dense tail of the main buffer (fefm_place).  Decided once from the model's graph;
@@ -1052,33 +1025,29 @@ def _plan_fefm_input(model, consumers, out_ids):
     from .layers.core import DNN
     from .layers.interaction import FEFMLayer
     from .layers.utils import Concat, NoMask, _CombinedDNNInput
-    calls = defaultdict(int)
-    for node in model._order:
-        calls[id(node.layer)] += 1
     places = {}
-    for node in model._order:
+    for node in g.order:
         if not isinstance(node.layer, Concat) or node.layer.axis not in (1, -1):
             continue
         srcs = E._flatten(node.inputs)
         if len(srcs) != 2 or len(srcs[0].shape) != 2 or len(srcs[1].shape) != 2:
             continue
         head, tail = srcs
-        if not isinstance(head.node.layer, (_CombinedDNNInput, E.Flatten)) or len(consumers[id(head)]) != 1:
+        if not isinstance(head.node.layer, (_CombinedDNNInput, E.Flatten)) or len(g.consumers[id(head)]) != 1:
             continue
         while isinstance(tail.node.layer, NoMask):                   # concat_func of the single FEFM output
             tail = E._flatten(tail.node.inputs)[0]
         fefm = tail.node.layer
-        if not isinstance(fefm, FEFMLayer) or calls[id(fefm)] != 1 or id(fefm) in places:
+        if not isinstance(fefm, FEFMLayer) or g.calls[id(fefm)] != 1 or id(fefm) in places:
             continue
-        out = node.outputs[0]
-        oc = consumers[id(out)]
-        if len(oc) != 1 or id(out) in out_ids or not isinstance(oc[0].layer, DNN):
+        c = g.only_use(node.outputs[0])
+        if c is None or not isinstance(c.layer, DNN):
             continue
         places[id(fefm)] = int(tail.shape[1])
     return places
 
 
-def _plan_pnn_input(model, consumers, out_ids):
+def _plan_pnn_input(g):
     """({id(product layer): column offset behind the embeddings}, total product columns) for PNN's DNN input
     concat([linear_signal, Flatten(InnerProductLayer(...)), OutterProductLayer(...)]) (deepctr/models/pnn.py:46-63,
     either product or both) when that concatenation reaches the first DNN layer only through combined_dnn_input:
@@ -1089,18 +1058,11 @@ def _plan_pnn_input(model, consumers, out_ids):
     from .layers.core import DNN
     from .layers.interaction import InnerProductLayer, OutterProductLayer
     from .layers.utils import Concat, NoMask, _CombinedDNNInput
-    calls = defaultdict(int)
-    for node in model._order:
-        calls[id(node.layer)] += 1
-
-    def only_use(t):
-        return len(consumers[id(t)]) == 1 and id(t) not in out_ids
-
-    for node in model._order:
+    for node in g.order:
         if not isinstance(node.layer, Concat) or node.layer.axis not in (1, -1):
             continue
         srcs = E._flatten(node.inputs)
-        if not 2 <= len(srcs) <= 3 or any(len(t.shape) != 2 or not only_use(t) for t in srcs):
+        if not 2 <= len(srcs) <= 3 or any(len(t.shape) != 2 or not g.only_use(t) for t in srcs):
             continue
         if not isinstance(srcs[0].node.layer, E.Reshape):
             continue
@@ -1110,11 +1072,11 @@ def _plan_pnn_input(model, consumers, out_ids):
             if isinstance(layer, E.Flatten):                          # Flatten(InnerProductLayer()(...))
                 inner = E._flatten(t.node.inputs)[0]
                 layer = inner.node.layer
-                if not (isinstance(layer, InnerProductLayer) and layer.reduce_sum and only_use(inner)):
+                if not (isinstance(layer, InnerProductLayer) and layer.reduce_sum and g.only_use(inner)):
                     break
             elif not isinstance(layer, OutterProductLayer):
                 break
-            if calls[id(layer)] != 1:
+            if g.calls[id(layer)] != 1:
                 break
             products.append((layer, int(t.shape[1])))
         if len(products) != len(srcs) - 1 or len(set(id(l) for l, _ in products)) != len(products):
@@ -1122,16 +1084,13 @@ def _plan_pnn_input(model, consumers, out_ids):
         # combined_dnn_input: NoMask + Flatten of the single deep input, then _CombinedDNNInput with the dense
         # features or the DNN directly
         flat = node.outputs[0]
-        while only_use(flat) and isinstance(consumers[id(flat)][0].layer, (NoMask, E.Flatten)):
-            flat = consumers[id(flat)][0].outputs[0]
-        if not only_use(flat):
-            continue
-        nxt = consumers[id(flat)][0]
-        if isinstance(nxt.layer, _CombinedDNNInput):
-            if E._flatten(nxt.inputs)[0] is not flat or not only_use(nxt.outputs[0]):
-                continue
-            nxt = consumers[id(nxt.outputs[0])][0]
-        if not isinstance(nxt.layer, DNN):
+        nxt = g.only_use(flat)
+        while nxt is not None and isinstance(nxt.layer, (NoMask, E.Flatten)):
+            flat = nxt.outputs[0]
+            nxt = g.only_use(flat)
+        if nxt is not None and isinstance(nxt.layer, _CombinedDNNInput):
+            nxt = g.only_use(nxt.outputs[0]) if E._flatten(nxt.inputs)[0] is flat else None
+        if nxt is None or not isinstance(nxt.layer, DNN):
             continue
         places, col = {}, 0
         for layer, w in products:
@@ -1141,43 +1100,39 @@ def _plan_pnn_input(model, consumers, out_ids):
     return {}, 0
 
 
-def _plan_dnn_input(model, consumers, out_ids):
+def _plan_dnn_input(g):
     """{id(BilinearInteraction layer): (DnnInputPlacement, index)}, decided once from the model's graph."""
     if not DNN_INPUT_PLACEMENT:
         return {}
     from .layers.core import DNN
     from .layers.interaction import BilinearInteraction
     from .layers.utils import Concat, NoMask, _CombinedDNNInput
-    calls = defaultdict(int)
-    for node in model._order:
-        calls[id(node.layer)] += 1
     places = {}
-    for node in model._order:
+    for node in g.order:
         if not isinstance(node.layer, Concat) or node.layer.axis not in (-1, 2):
             continue
         srcs = E._flatten(node.inputs)
         layers = [t.node.layer for t in srcs]
         if (len(srcs) < 2 or not all(isinstance(l, BilinearInteraction) for l in layers)
-                or len(set(id(l) for l in layers)) != len(layers) or any(calls[id(l)] != 1 for l in layers)
-                or any(len(consumers[id(t)]) != 1 or id(t) in out_ids for t in srcs)
+                or len(set(id(l) for l in layers)) != len(layers) or any(g.calls[id(l)] != 1 for l in layers)
+                or not all(g.only_use(t) for t in srcs)
                 or len(set(tuple(t.shape) for t in srcs)) != 1):
             continue
         # then only Flatten / NoMask (combined_dnn_input wraps the flattened concat in both) up to the DNN input
-        flat, fc = node.outputs[0], None
-        while True:
-            fc = consumers[id(flat)]
-            if len(fc) != 1 or id(flat) in out_ids or not isinstance(fc[0].layer, (E.Flatten, NoMask)):
-                break
-            flat = fc[0].outputs[0]
-        if flat is node.outputs[0] or len(fc) != 1 or id(flat) in out_ids or len(flat.shape) != 2:
+        flat = node.outputs[0]
+        nxt = g.only_use(flat)
+        while nxt is not None and isinstance(nxt.layer, (E.Flatten, NoMask)):
+            flat = nxt.outputs[0]
+            nxt = g.only_use(flat)
+        if flat is node.outputs[0] or nxt is None or len(flat.shape) != 2:
             continue
         ndense = 0
-        if isinstance(fc[0].layer, _CombinedDNNInput):
-            ins = E._flatten(fc[0].inputs)
+        if isinstance(nxt.layer, _CombinedDNNInput):
+            ins = E._flatten(nxt.inputs)
             if ins[0] is not flat:
                 continue
             ndense = int(np.prod(ins[1].shape[1:]))
-        elif not isinstance(fc[0].layer, DNN):
+        elif not isinstance(nxt.layer, DNN):
             continue
         _, P, Ed = srcs[0].shape
         pl = DnnInputPlacement(len(srcs), int(P), int(Ed), ndense)
@@ -1189,85 +1144,92 @@ def _plan_dnn_input(model, consumers, out_ids):
 class RegulatePlan(object):
     """EDCN's information sharing (deepctr/models/edcn.py:66-85) with fewer passes over [B, F*E]:
 
-    * ``pairs`` {id(RegulationModule): (partner module, partner node)}: two RegulationModules reading one tensor (the
+    * ``pairs`` {id(first node): (first node, second node)}: two RegulationModules reading one tensor (the
       embeddings' concat_func, a window of the gather buffer read in place, or the Reshape of a 'concatenation'
-      bridge's Dense) are one 'copy' launch with both gates;
-    * ``bridges`` {id(BridgeModule): (Reshape node, [(module, node)] * 2)}: a non-concatenation BridgeModule whose
-      output reaches only Reshape([F, E]), which feeds only two RegulationModules, is one launch in the bridge's
-      mode that writes the two gated outputs; bridge_out and its reshape are never written.
+      bridge's Dense) are one 'copy' launch with both gates, made where the first of them runs;
+    * ``bridges`` {id(BridgeModule node): (that node, Reshape node, [RegulationModule node] * 2)}: a
+      non-concatenation BridgeModule whose output reaches only Reshape([F, E]), which feeds only two
+      RegulationModules, is one launch in the bridge's mode that writes the two gated outputs; bridge_out and its
+      reshape are never written.
 
     Decided once from the model's graph; anything else runs layer by layer on the same kernel."""
 
     def __init__(self, pairs, bridges):
         self.pairs, self.bridges = pairs, bridges
 
+    def launches(self):
+        out = {k: functools.partial(_regulate_pair, *p) for k, p in self.pairs.items()}
+        out.update((k, functools.partial(_regulate_bridge, *b)) for k, b in self.bridges.items())
+        return out
 
-def _plan_regulate(model, consumers, out_ids):
+
+def _regulate_pair(first, second, values, training):
+    from . import ops
+    gates = [(n.layer.g, n.layer.tau) for n in (first, second)]
+    _, (y0, y1) = ops.regulate("copy", values[id(first.inputs)], gates=gates, want_u=False)
+    return {id(first): y0, id(second): y1}
+
+
+def _regulate_bridge(bridge, reshape, regs, values, training):
+    from . import ops
+    x, h = [values[id(t)] for t in bridge.inputs]
+    mode, operands = bridge.layer.operands(x, h, training)
+    _, (y0, y1) = ops.regulate(mode, *operands, gates=[(n.layer.g, n.layer.tau) for n in regs], want_u=False)
+    return {id(bridge): VIRTUAL, id(reshape): VIRTUAL, id(regs[0]): y0, id(regs[1]): y1}
+
+
+def _plan_regulate(g):
     from .layers.core import RegulationModule
     from .layers.interaction import BridgeModule
-    calls = defaultdict(int)
-    for node in model._order:
-        calls[id(node.layer)] += 1
-
-    def regulators(t):
-        """The two RegulationModule nodes that are all of ``t``'s consumers, or None."""
-        cs = consumers[id(t)]
-        if id(t) in out_ids or len(cs) != 2 or len(t.shape) != 3 or cs[0].layer is cs[1].layer:
-            return None
-        if all(isinstance(c.layer, RegulationModule) and calls[id(c.layer)] == 1 for c in cs):
-            return cs
-        return None
-
-    pairs, bridges, claimed = {}, {}, set()
-    for node in model._order:
-        layer = node.layer
-        if not isinstance(layer, BridgeModule) or layer.bridge_type == "concatenation" or calls[id(layer)] != 1:
-            continue
-        out = node.outputs[0]
-        cs = consumers[id(out)]
-        if id(out) in out_ids or len(cs) != 1 or not isinstance(cs[0].layer, E.Reshape):
-            continue
-        regs = regulators(cs[0].outputs[0])
-        if regs is not None:
-            bridges[id(layer)] = (cs[0], [(c.layer, c) for c in regs])
-            claimed.add(id(cs[0].outputs[0]))
-    for node in model._order:
+    gated = {}      # id(tensor): the two RegulationModule nodes that are all of its consumers
+    for node in g.order:
         for t in node.outputs:
-            regs = regulators(t) if id(t) not in claimed else None
-            if regs is not None:
-                pairs[id(regs[0].layer)] = (regs[1].layer, regs[1])
-    return RegulatePlan(pairs, bridges)
+            cs = g.consumers[id(t)]
+            if (id(t) not in g.out_ids and len(cs) == 2 and len(t.shape) == 3 and cs[0].layer is not cs[1].layer
+                    and all(isinstance(c.layer, RegulationModule) and g.calls[id(c.layer)] == 1 for c in cs)):
+                gated[id(t)] = cs
+    bridges = {}
+    for node in g.order:
+        layer = node.layer
+        if not isinstance(layer, BridgeModule) or layer.bridge_type == "concatenation" or g.calls[id(layer)] != 1:
+            continue
+        r = g.only_use(node.outputs[0])
+        if r is not None and isinstance(r.layer, E.Reshape) and id(r.outputs[0]) in gated:
+            bridges[id(node)] = (node, r, gated.pop(id(r.outputs[0])))
+    return RegulatePlan({id(cs[0]): tuple(cs) for cs in gated.values()}, bridges)
 
 
 class ConvStackPlan(object):
     """CCPM's convolution stack (deepctr/models/ccpm.py:58-70) served by one b2ctr_conv_stack launch: the chain
     concat_func(embeddings) -> Lambda(expand_dims(x, 3)) -> [Conv2D -> KMaxPooling(axis=1)] x l -> Flatten, every
-    intermediate with this one consumer, runs when its first Conv2D is called.  The input is read in place (a
-    window of the gather buffer), the per-layer maps are never written, and Flatten of the result is a view.
+    intermediate with this one consumer, runs where its first Conv2D would.  The input is read in place (a window
+    of the gather buffer), the per-layer maps are never written, and Flatten of the result is a view.
 
-    ``chains`` {id(first Conv2D layer): [Conv2D node, KMaxPooling node, ...]}.  Decided once from the model's graph;
+    ``chains`` {id(first Conv2D node): [Conv2D node, KMaxPooling node, ...]}.  Decided once from the model's graph;
     any other graph, or a stack beyond the kernel's limits, runs layer by layer on the same kernel."""
 
     def __init__(self, chains):
         self.chains = chains
 
+    def launches(self):
+        return {k: functools.partial(_conv_stack, chain) for k, chain in self.chains.items()}
 
-def _plan_conv_stack(model, consumers, out_ids):
+
+def _conv_stack(chain, values, training):
+    from . import ops
+    x = values[id(chain[0].inputs)]
+    b, rows, dim, channels = x.data.shape
+    out = {id(n): VIRTUAL for n in chain[:-1]}
+    out[id(chain[-1])] = ops.conv_stack(x, [n.layer.stage() for n in chain], rows, dim, channels,
+                                        (b,) + tuple(chain[-1].outputs[0].shape[1:]))
+    return out
+
+
+def _plan_conv_stack(g):
     from . import kernels as K
     from .layers.sequence import KMaxPooling
-    calls = defaultdict(int)
-    for node in model._order:
-        calls[id(node.layer)] += 1
-
-    def only(t, cls):
-        """The single consumer node of ``t`` when it is a ``cls`` called once, else None."""
-        cs = consumers[id(t)]
-        if id(t) in out_ids or len(cs) != 1 or not isinstance(cs[0].layer, cls) or calls[id(cs[0].layer)] != 1:
-            return None
-        return cs[0]
-
     chains = {}
-    for node in model._order:
+    for node in g.order:
         if not isinstance(node.layer, E.Lambda) or not isinstance(node.inputs, E.KTensor):
             continue
         src, out = node.inputs, node.outputs[0]
@@ -1275,21 +1237,21 @@ def _plan_conv_stack(model, consumers, out_ids):
             continue
         chain, t = [], out
         while True:
-            conv = only(t, E.Conv2D)
+            conv = g.only(t, E.Conv2D)
             if conv is None:
                 break
-            pool = only(conv.outputs[0], KMaxPooling)
+            pool = g.only(conv.outputs[0], KMaxPooling)
             if pool is None or pool.layer.axis != 1:
                 break
             chain += [conv, pool]
             t = pool.outputs[0]
-        if not chain or only(t, E.Flatten) is None:
+        if not chain or g.only(t, E.Flatten) is None:
             continue
         try:
             K.conv_stack_check(int(src.shape[1]), 1, [n.layer.stage()[:3] for n in chain])
         except ValueError:
             continue
-        chains[id(chain[0].layer)] = chain
+        chains[id(chain[0])] = chain
     return ConvStackPlan(chains)
 
 
@@ -1298,33 +1260,37 @@ class FieldWisePlan(object):
     once, whose every input is concat_func(members, axis=1) (a Concat, or NoMask for a one-member group) of
     embedding or pooled windows of the gather buffer, each concatenation used by that layer only, runs as one
     b2ctr_field_wise_bi launch reading the members where the gather wrote them.  The concatenations are never
-    formed (their results are Vars without data), whether or not a group's members are adjacent.
+    formed (VIRTUAL), whether or not a group's members are adjacent.
 
-    ``groups`` {id(layer): [[member slot node, ...] per group]}, ``virtual`` the concatenation nodes.  Decided
-    once from the model's graph; any other graph runs the layer on its concrete inputs, on the same kernel."""
+    ``heads`` the FieldWiseBiInteraction nodes, ``groups`` {id(head): [[member tensor, ...] per group]}, ``virtual``
+    the concatenation nodes.  Decided once from the model's graph; any other graph runs the layer on its concrete
+    inputs, on the same kernel."""
 
-    def __init__(self, groups, virtual):
-        self.groups = groups
-        self.virtual = virtual
+    def __init__(self, heads, groups, virtual):
+        self.heads, self.groups, self.virtual = heads, groups, virtual
+
+    def launches(self):
+        return {id(n): functools.partial(_field_wise, n, self.groups[id(n)]) for n in self.heads}
 
 
-def _plan_field_wise(model, consumers, out_ids, main_slots):
+def _field_wise(node, groups, values, training):
+    return {id(node): node.layer.interact([[values[id(m)] for m in members] for members in groups])}
+
+
+def _plan_field_wise(g, main_slots):
     from .layers.interaction import FieldWiseBiInteraction
     from .layers.utils import Concat, NoMask
-    slot_out = {id(s.node.outputs[0]): s.node for s in main_slots}
-    calls = defaultdict(int)
-    for node in model._order:
-        calls[id(node.layer)] += 1
-    groups, virtual = {}, []
-    for node in model._order:
-        if not isinstance(node.layer, FieldWiseBiInteraction) or calls[id(node.layer)] != 1:
+    slot_out = set(id(s.node.outputs[0]) for s in main_slots)
+    heads, groups, virtual = [], {}, []
+    for node in g.order:
+        if not isinstance(node.layer, FieldWiseBiInteraction) or g.calls[id(node.layer)] != 1:
             continue
         if not isinstance(node.inputs, (list, tuple)) or len(node.inputs) < 2:
             continue
         plan, concats = [], []
         for t in node.inputs:
             src = t.node
-            if id(t) in out_ids or len(consumers[id(t)]) != 1:
+            if not g.only_use(t):
                 break
             if isinstance(src.layer, Concat) and src.layer.axis in (1, -2):
                 members = E._flatten(src.inputs)
@@ -1334,20 +1300,21 @@ def _plan_field_wise(model, consumers, out_ids, main_slots):
                 break
             if not all(id(m) in slot_out and len(m.shape) == 3 for m in members):
                 break
-            plan.append([slot_out[id(m)] for m in members])
+            plan.append(members)
             concats.append(src)
         else:
-            dims = set(int(n.outputs[0].shape[-1]) for g in plan for n in g)
-            nfield = sum(int(n.outputs[0].shape[1]) for g in plan for n in g)
+            dims = set(int(m.shape[-1]) for members in plan for m in members)
+            nfield = sum(int(m.shape[1]) for members in plan for m in members)
             try:
                 K.field_wise_bi_check(nfield, len(plan), dims.pop())
             except ValueError:
                 continue
             if dims:
                 continue
-            groups[id(node.layer)] = plan
+            heads.append(node)
+            groups[id(node)] = plan
             virtual += concats
-    return FieldWisePlan(groups, virtual)
+    return FieldWisePlan(heads, groups, virtual)
 
 
 class FieldAwarePlan(object):
@@ -1494,7 +1461,7 @@ def ops_window(base, col0, ncols, shape):
 MAX_FFM_FIELDS, MAX_FFM_DIM = 64, 64       # b2ctr_ffm_product_fwd's limits
 
 
-def _plan_field_aware(model, consumers, out_ids, as_input):
+def _plan_field_aware(g):
     """The FieldAwarePlan of ONN's graph (deepctr/models/onn.py:79-97), or None.  Per pair (i, j) of
     itertools.combinations order: multiply([lookup_i, lookup_j]), optionally followed by Lambda(K.sum(., axis=-1)),
     where a lookup is NoMask(Embedding(ids)) for a single-valued field or SequencePoolingLayer(combiner,
@@ -1504,15 +1471,9 @@ def _plan_field_aware(model, consumers, out_ids, as_input):
     plans nothing and each layer runs as itself."""
     from .layers.sequence import SequencePoolingLayer
     from .layers.utils import Hash, NoMask
-    calls = defaultdict(int)
-    for node in model._order:
-        calls[id(node.layer)] += 1
-
-    def only_use(t):
-        return len(consumers[id(t)]) == 1 and id(t) not in out_ids
 
     def lookup(t):
-        if not only_use(t) or calls[id(t.node.layer)] != 1 or not isinstance(t.node.inputs, E.KTensor):
+        if not g.only_use(t) or g.calls[id(t.node.layer)] != 1 or not isinstance(t.node.inputs, E.KTensor):
             return None
         outer = t.node
         if isinstance(outer.layer, NoMask):
@@ -1523,21 +1484,21 @@ def _plan_field_aware(model, consumers, out_ids, as_input):
             return None
         e = outer.inputs
         emb = e.node.layer
-        if (not only_use(e) or not isinstance(emb, Embedding) or calls[id(emb)] != 1
+        if (not g.only_use(e) or not isinstance(emb, Embedding) or g.calls[id(emb)] != 1
                 or not isinstance(e.node.inputs, E.KTensor) or emb.mask_zero != (pool != L.POOL_NONE)):
             return None
         virt = [outer, e.node]
         src, hash_mode = e.node.inputs, L.HASH_NONE
         if isinstance(src.node.layer, Hash):
             h = src.node.layer
-            if (not only_use(src) or h.mask_zero or h.vocabulary_path or calls[id(h)] != 1
+            if (not g.only_use(src) or h.mask_zero or h.vocabulary_path or g.calls[id(h)] != 1
                     or not isinstance(src.node.inputs, E.KTensor)):
                 return None
             virt.append(src.node)
             src, hash_mode = src.node.inputs, L.HASH_FARM
             if src.dtype in ("string", str):
                 return None
-        name = as_input(src)
+        name = g.input_name(src)
         if name is None:
             return None
         maxlen = int(np.prod(src.shape[1:])) if len(src.shape) > 1 else 1
@@ -1546,23 +1507,18 @@ def _plan_field_aware(model, consumers, out_ids, as_input):
         return (name, maxlen, pool, hash_mode, emb.input_dim), emb, virt
 
     pairs = []
-    for node in model._order:
-        if not isinstance(node.layer, E.Multiply) or calls[id(node.layer)] != 1:
+    for node in g.order:
+        if not isinstance(node.layer, E.Multiply) or g.calls[id(node.layer)] != 1:
             continue
         ins = E._flatten(node.inputs)
         sides = [lookup(t) for t in ins] if len(ins) == 2 else [None]
         if any(sd is None for sd in sides):
             continue
-        out, served, virt, reduce_sum = node.outputs[0], node, [node], False
-        if only_use(out):
-            nxt = consumers[id(out)][0]
-            if isinstance(nxt.layer, E.Lambda) and getattr(nxt.layer, "reduces_last_axis", False):
-                served, reduce_sum = nxt, True
-            else:
-                virt = []
-        else:
-            virt = []
-        pairs.append((sides, served, virt if reduce_sum else [], reduce_sum))
+        served, reduce_sum = node, False
+        nxt = g.only_use(node.outputs[0])
+        if nxt is not None and isinstance(nxt.layer, E.Lambda) and getattr(nxt.layer, "reduces_last_axis", False):
+            served, reduce_sum = nxt, True
+        pairs.append((sides, served, [node] if reduce_sum else [], reduce_sum))
     if not pairs:
         return None
     fields, index = [], {}

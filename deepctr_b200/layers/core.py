@@ -207,10 +207,6 @@ class RegulationModule(Layer):
     def call(self, inputs, **kwargs):
         if inputs.data.dim() != 3:
             raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs.data.dim()))
-        planner = getattr(self, "_planner", None)
-        served = planner.regulated(self, inputs) if planner is not None else None
-        if served is not None:
-            return served
         _, (y,) = ops.regulate("copy", inputs, gates=[(self.g, self.tau)], want_u=False)
         return y
 

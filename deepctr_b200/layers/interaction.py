@@ -695,17 +695,18 @@ class BridgeModule(Layer):
         x, h = inputs
         if self.bridge_type == "concatenation":
             return self.dense.call(ops.concat([x, h], axis=-1))
+        mode, operands = self.operands(x, h, training)
+        u, _ = ops.regulate(mode, *operands)
+        return u
+
+    def operands(self, x, h, training=None):
+        """(b2ctr_regulate mode, (x, h, ax, ah)) of a non-concatenation bridge; 'attention_pooling' runs its two DNNs
+        here for ax and ah."""
         ax = ah = None
         if self.bridge_type == "attention_pooling":
             ax = self.dense_x.call(x, training=training)
             ah = self.dense_h.call(h, training=training)
-        mode = _BRIDGE_MODES[self.bridge_type]
-        planner = getattr(self, "_planner", None)
-        served = planner.bridged(self, mode, (x, h, ax, ah)) if planner is not None else None
-        if served is not None:
-            return served
-        u, _ = ops.regulate(mode, x, h, ax, ah)
-        return u
+        return _BRIDGE_MODES[self.bridge_type], (x, h, ax, ah)
 
     def compute_output_shape(self, input_shape):
         return (None, int(input_shape[0][-1]))
@@ -723,8 +724,8 @@ class FieldWiseBiInteraction(Layer):
       sum_{g<h} kernel_mf[p] * S_g * S_h + bias_mf + sum_g kernel_fm[g] * (S_g^2 - Q_g) + bias_fm
     with S_g / Q_g the sum / sum of squares of group g's fields.  One b2ctr_field_wise_bi launch: the groups are read
     wherever they are when they are windows of one buffer, else copied once into one [B, F, E] buffer.  In FLEN
-    the planner (inputs.FieldWisePlan) hands it the group members, windows of the gather buffer, so the groups'
-    concatenations are never written."""
+    the planner (inputs.FieldWisePlan) runs it on the group members (``interact``), windows of the gather buffer, so
+    the groups' concatenations are never written."""
 
     def __init__(self, use_bias=True, seed=1024, **kwargs):
         self.use_bias = use_bias
@@ -749,14 +750,13 @@ class FieldWiseBiInteraction(Layer):
         self.built = True
 
     def call(self, inputs, **kwargs):
+        if inputs[0].data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs[0].data.dim()))
+        return self.interact([[x] for x in inputs])
+
+    def interact(self, groups):
+        """The layer on G groups, each a list of [B, n, E] members whose field axis concatenation is the group."""
         bias = (self.bias_mf, self.bias_fm) if self.use_bias else (None, None)
-        planner = getattr(self, "_planner", None)
-        groups = planner.field_wise_groups(self) if planner is not None else None
-        if groups is None:
-            if inputs[0].data.dim() != 3:
-                raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions"
-                                 % (inputs[0].data.dim()))
-            groups = [[x] for x in inputs]
         return ops.field_wise_bi(groups, self.kernel_mf, self.kernel_fm, *bias)
 
     def compute_output_shape(self, input_shape):
