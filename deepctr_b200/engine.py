@@ -652,7 +652,7 @@ class Layer(object):
 
     def _invoke(self, vars_in, training, kwargs=None):
         if not self.takes_scaled_fields:
-            vars_in = _map_structure(lambda v: v.product() if isinstance(v, ops.ScaledFields) else v, vars_in)
+            vars_in = _concrete(vars_in)
         if self._call_args is None:
             try:
                 self._call_args = set(inspect.signature(self.call).parameters)
@@ -674,6 +674,11 @@ class Layer(object):
             has = any(m is not None for m in _flatten(masks))
             out.mask = self.compute_mask(vars_in, masks if has else None)
         return out
+
+
+def _concrete(vars_in):
+    """``vars_in`` with every ops.ScaledFields replaced by its product (computed once), as call() receives it."""
+    return _map_structure(lambda v: v.product() if isinstance(v, ops.ScaledFields) else v, vars_in)
 
 
 class InputLayer(Layer):
@@ -1238,14 +1243,14 @@ class Model(object):
             if node is upto:
                 break
             launch = self.planner.launches.get(id(node))
-            if launch is not None:        # a fused chain's first node: one launch serves it and the later nodes
+            if launch is not None:        # a planned node, or a fused chain's first node that serves the later nodes
                 self.planner.results.update(launch(values, training))
-            planned = self.planner.results.get(id(node))
-            if planned is not None:       # served by the fused embedding launch (inputs.EmbeddingPlanner)
+            # popped: what a step's launches made is held by that step's values and tape only
+            planned = self.planner.results.pop(id(node), None)
+            if planned is not None:       # served by the planner (inputs.EmbeddingPlanner), with the result's own mask
                 values[id(node.outputs[0])] = planned
                 continue
             ins = _map_structure(lambda t: values[id(t)], node.inputs)
-            node.layer._planner = self.planner
             out = node.layer._invoke(ins, training)
             outs = _flatten(out) if len(node.outputs) > 1 else [out]
             for t, v in zip(node.outputs, outs):

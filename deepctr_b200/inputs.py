@@ -376,27 +376,42 @@ class EmbeddingPlanner(object):
         for t in model.inputs:
             if t.dtype in ("float32", "float64", "float16") and len(t.shape) == 2:
                 self.tail_reserve += int(t.shape[1])
-        # DeepFEFM's FEFM scores go behind the dense columns (fefm_place): P more columns in the row pitch
+        # DeepFEFM's FEFM scores go behind the dense columns (_fefm_scores): P more columns in the row pitch
         self.fefm_places = _plan_fefm_input(g)
-        # PNN's inner / outer products go between the embeddings and the dense columns (pnn_place): P per product
+        # PNN's inner / outer products go between the embeddings and the dense columns (_pnn_products): P per product
         # more columns in the row pitch
         self.pnn_places, self.pnn_cols = _plan_pnn_input(g)
         self.main_ld = (self.main_width + self.tail_reserve + sum(self.fefm_places.values()) + self.pnn_cols
                         + 3) // 4 * 4
         self.lin_ld = max(1, (self.lin_width + 3) // 4 * 4)
         self.fast = self._fast_eligible()
-        self.dnn_places = _plan_dnn_input(g)
+        self.dnn_places, bilinear_concats = _plan_dnn_input(g)
         # EDCN's RegulationModule pairs and the bridges in front of them: one b2ctr_regulate launch each
         self.regulate_plan = _plan_regulate(g)
         # CCPM's Lambda(expand_dims) -> [Conv2D -> KMaxPooling(axis=1)] x l -> Flatten: one b2ctr_conv_stack launch
         self.conv_plan = _plan_conv_stack(g)
         # FLEN's FieldWiseBiInteraction on concatenations of gather-buffer windows: one launch reading them in place
         self.field_wise_plan = _plan_field_wise(g, self.main)
-        # {id(first node of a fused chain): (values, training) -> {id(node): result}}: Model._run makes the launch
-        # when it reaches that node, and the results serve it and the chain's later nodes
+        # {id(node): (values, training) -> {id(node): result}}: Model._run makes the launch when it reaches that node,
+        # and the results serve it and a fused chain's later nodes; {} lets the node's layer run
         self.launches = {}
         for plan in (self.regulate_plan, self.conv_plan, self.field_wise_plan):
             self.launches.update(plan.launches())
+        for concat, layout, nodes in bilinear_concats:
+            self.launches[id(concat)] = functools.partial(_bilinear_into_dnn_input, concat, layout, nodes)
+        # nodes whose output a launch at a later node folds away: FLEN's concatenations and FiBiNET's bilinear layers
+        self.virtual = self.field_wise_plan.virtual + [n for _, _, nodes in bilinear_concats for n in nodes]
+        from .layers.interaction import FM
+        from .layers.utils import Linear, _CombinedDNNInput
+        for node in g.order:
+            layer = node.layer
+            launch = (self._fm if isinstance(layer, FM) else
+                      self._linear if isinstance(layer, Linear) and layer.mode != 1 else
+                      self._combined_dnn_input if isinstance(layer, _CombinedDNNInput) else
+                      self._fefm_scores if id(layer) in self.fefm_places else
+                      self._pnn_products if id(layer) in self.pnn_places else None)
+            if launch is not None:
+                self.launches[id(node)] = functools.partial(launch, node)
         # IFM / DIFM scale the linear lookups by per-sample field weights before Linear sums them: their rows are
         # needed, so they are never fused into the gather's row-sum (lin_hint)
         from .layers.utils import RefineWeight
@@ -557,7 +572,7 @@ class EmbeddingPlanner(object):
 
     # ---- per-step execution ------------------------------------------------------------------------
     def begin_step(self, feed, training):
-        self.results = {}
+        self.results = {id(node): VIRTUAL for node in self.virtual}
         self.fm_result = self.lin_result = None
         self.tail_done = None
         self.planes_result = None
@@ -677,8 +692,6 @@ class EmbeddingPlanner(object):
             for vn in s.virtual_nodes:
                 if vn is not s.node:
                     self.results[id(vn)] = VIRTUAL
-        for node in self.field_wise_plan.virtual:      # folded into the FieldWiseBiInteraction launch
-            self.results[id(node)] = VIRTUAL
         if grad:
             outs = [b for b in bufs.values()]
             if self.fm_result is not None:
@@ -866,43 +879,6 @@ class EmbeddingPlanner(object):
             self.lin_hint = True
         return None
 
-    def dnn_input_place(self, layer):
-        """(DnnInputPlacement, index) when ``layer`` writes its output into the first DNN layer's input."""
-        return self.dnn_places.get(id(layer))
-
-    def fefm_place(self, layer, x):
-        """The [B, P] window of this step's main buffer, behind the dense columns, where the FEFMLayer ``layer``
-        writes its scores (ops.fefm ``out``), or None.  With the embeddings at [0, main_width) and
-        combined_dnn_input's dense columns behind them, DeepFEFM's concat([combined_dnn_input, scores]) is then the
-        zero-copy window [0, main_width + n_dense + P) of the buffer, the first Dense reads it in place and its data
-        gradient becomes the buffer's gradient, whose score columns the FEFM backward reads in place."""
-        from . import ops
-        P = self.fefm_places.get(id(layer))
-        base = x.base
-        if (P is None or base is None or base.owner is not self or base.data is None
-                or base.ncols != self.main_width or base.data.shape[1] != self.main_ld):
-            return None
-        b = base.data.shape[0]
-        return ops._window(base, self.main_width + self.tail_reserve, P, (b, P))
-
-    def pnn_place(self, layer, x):
-        """The [B, P] window of this step's main buffer where PNN's InnerProductLayer / OutterProductLayer ``layer``
-        writes its scores (ops.pnn_inner / ops.pnn_outer ``out``), or None.  ``x`` must be the embeddings' window
-        [0, main_width): the products then follow it in the order of PNN's concat([linear_signal, inner, outer]),
-        so that concatenation is a zero-copy window, combined_dnn_input copies only the dense columns behind it
-        (append_dense) and the first Dense reads the buffer in place.  Its data gradient becomes the buffer's
-        gradient, whose product columns the product backwards read in place."""
-        from . import ops
-        rel = self.pnn_places.get(id(layer))
-        base = x.base
-        if (rel is None or base is None or base.owner is not self or base.data is None or x.ncols == -1
-                or x.col0 != 0 or x.ncols != self.main_width or base.ncols != self.main_width
-                or base.data.shape[1] != self.main_ld):
-            return None
-        b, f, _ = x.data.shape
-        P = f * (f - 1) // 2
-        return ops._window(base, self.main_width + rel, P, (b, P))
-
     def append_dense(self, emb_flat, dense_flat):
         """combined_dnn_input: place the dense features behind the embeddings (and PNN's placed products) in the
         main buffer so the DNN input is a zero-copy window.  Returns the window or None."""
@@ -941,58 +917,74 @@ class EmbeddingPlanner(object):
                 self.tail_hint = (dense_flat.col0, nd)
         return ops._window(base, 0, self.main_width + nd, (b, self.main_width + nd))
 
+    # ---- launches of single nodes (self.launches) ----------------------------------------------------
+    def _fm(self, node, values, training):
+        """FM: the gather's in-kernel FM; IFM / DIFM's ops.ScaledFields input runs the field-weighted FM instead."""
+        from . import ops
+        x = values[id(node.inputs)]
+        fused = None if isinstance(x, ops.ScaledFields) else self.lookup_fm(x)
+        return {} if fused is None else {id(node): fused}
+
+    def _linear(self, node, values, training):
+        """Linear in mode 0 or 2: the gather's in-kernel row-sum of the linear lookups, plus the bias or dense part."""
+        inputs = E._map_structure(lambda t: values[id(t)], node.inputs)
+        fused = self.lookup_rowsum(inputs if node.layer.mode == 0 else inputs[0])
+        return {} if fused is None else {id(node): node.layer.combine(fused, inputs)}
+
+    def _combined_dnn_input(self, node, values, training):
+        win = self.append_dense(*[values[id(t)] for t in node.inputs])
+        return {} if win is None else {id(node): win}
+
+    def _fefm_scores(self, node, values, training):
+        """DeepFEFM's FEFMLayer writes its [B, P] scores into this step's main buffer, behind the dense columns:
+        DeepFEFM's concat([combined_dnn_input, scores]) is then the zero-copy window [0, main_width + n_dense + P),
+        the first Dense reads it in place and the FEFM backward reads the score columns of its data gradient."""
+        from . import ops
+        x = values[id(node.inputs)]
+        base = x.base
+        if (base is None or base.owner is not self or base.data is None
+                or base.ncols != self.main_width or base.data.shape[1] != self.main_ld):
+            return {}
+        P = self.fefm_places[id(node.layer)]
+        out = ops._window(base, self.main_width + self.tail_reserve, P, (base.data.shape[0], P))
+        return {id(node): node.layer.scores(x, out=out)}
+
+    def _pnn_products(self, node, values, training):
+        """PNN's InnerProductLayer / OutterProductLayer writes its [B, P] products into this step's main buffer when
+        its operand is the embeddings' window [0, main_width), in the order of PNN's concat([linear_signal, inner,
+        outer]): that concatenation is then a zero-copy window, combined_dnn_input copies only the dense columns
+        behind it and the product backwards read the product columns of the first Dense's data gradient.  Any other
+        operand gets the layer's own output, since forming it may have copied."""
+        from . import ops
+        from .layers.interaction import _product_operand
+        x = _product_operand(E._concrete([values[id(t)] for t in node.inputs]))
+        base, out = x.base, None
+        if (base is not None and base.owner is self and base.data is not None and x.ncols != -1 and x.col0 == 0
+                and x.ncols == self.main_width and base.ncols == self.main_width
+                and base.data.shape[1] == self.main_ld):
+            b, f, _ = x.data.shape
+            P = f * (f - 1) // 2
+            out = ops._window(base, self.main_width + self.pnn_places[id(node.layer)], P, (b, P))
+        return {id(node): node.layer.products(x, out=out)}
+
 
 class DnnInputPlacement(object):
-    """n BilinearInteraction layers whose [B,P,E] outputs reach the DNN only as Flatten(Concat(outputs, -1))
-    (FiBiNET, deepctr/models/fibinet.py:58), possibly followed by combined_dnn_input's dense columns.  The layers
-    write their pairs straight into one [B, ld] buffer, ld = round_up(n*P*E + n_dense, 4): pair p of layer k at
-    columns p*n*E + k*E, which is exactly the layout of the concatenation.  The Concat is then a zero-copy window,
-    combined_dnn_input copies only the dense columns behind it, and the first Dense reads the buffer in place; its
-    data gradient is adopted as the buffer's gradient and each layer's backward reads its strided part."""
+    """Layout of n BilinearInteraction layers whose [B,P,E] outputs reach the DNN only as Flatten(Concat(outputs, -1))
+    (FiBiNET, deepctr/models/fibinet.py:58), possibly followed by combined_dnn_input's dense columns.  Where the Concat
+    runs, the layers write their pairs into one [B, ld] buffer, ld = round_up(n*P*E + n_dense, 4): pair p of layer k
+    at columns p*n*E + k*E, the layout of the concatenation (_bilinear_into_dnn_input).  The Concat is then a zero-copy
+    window, combined_dnn_input copies only the dense columns behind it, and the first Dense reads the buffer in place;
+    its data gradient is adopted as the buffer's gradient and each layer's backward reads its strided part."""
 
     def __init__(self, n, P, E, ndense):
         self.n, self.P, self.E, self.ndense = n, P, E, ndense
         self.width = n * P * E
         self.ld = (self.width + ndense + 3) // 4 * 4
-        self.buf = None                 # this step's buffer Var, dropped once the backward has consumed it
-        self.outs = [None] * n
 
-    def _release(self):
-        """Forget this step's buffer (5.46 GB at C2), so that it is freed with the step's last reference and never
-        coexists with the next step's."""
-        self.buf = None
-        self.outs = [None] * self.n
-
-    def out_view(self, k, b, device):
-        """Where layer k writes its [B,P,E] output this step (a new buffer when a step starts)."""
-        if self.buf is None or self.outs[k] is not None or self.buf.data.shape[0] != b:
-            self._release()
-            t = torch.empty((b, self.ld), dtype=torch.float32, device=device)
-            self.buf = E.Var(t, ncols=self.width, owner=self, name="__dnn_input__")
-            self.outs = [None] * self.n
-        t = self.buf.data
-        return t.as_strided((b, self.P, self.E), (self.ld, self.n * self.E, 1), t.storage_offset() + k * self.E)
-
-    def placed(self, k, var):
-        var.owner = self
-        self.outs[k] = var
-
-    def placed_concat(self, xs, axis):
-        """ops.concat of the n placed outputs along the last axis: the window [0, n*P*E) of the buffer."""
-        from . import ops
-        if (self.buf is None or axis not in (-1, 2) or len(xs) != self.n
-                or any(a is not b for a, b in zip(xs, self.outs))):
-            return None
-        base, b, n, E_ = self.buf, self.buf.data.shape[0], self.n, self.E
-
-        def bwd(grads):
-            g = grads[0]
-            for k, v in enumerate(xs):
-                E.add_grad(v, g.as_strided((b, self.P, E_), (g.stride(0), n * E_, 1), g.storage_offset() + k * E_))
-            self._release()             # only the tape still holds the buffer; it goes when the backward ends
-
-        E.record([base], xs, bwd)
-        return ops._window(base, 0, self.width, (b, self.P, n * E_))
+    def buffer(self, b, device):
+        """A new [b, ld] buffer Var for one step (5.46 GB at C2: only that step's values and tape hold it)."""
+        t = torch.empty((b, self.ld), dtype=torch.float32, device=device)
+        return E.Var(t, ncols=self.width, owner=self, name="__dnn_input__")
 
     def append_dense(self, emb_flat, dense_flat):
         from . import ops
@@ -1018,7 +1010,7 @@ DNN_INPUT_PLACEMENT = True
 def _plan_fefm_input(g):
     """{id(FEFMLayer): P} for DeepFEFM's DNN input concat([combined_dnn_input(...), NoMask(FEFM(x))], axis=1)
     (deepctr/models/deepfefm.py:64-78) when that concatenation reaches only the DNN: the planner then reserves the
-    P score columns behind the dense tail of the main buffer (fefm_place).  Decided once from the model's graph;
+    P score columns behind the dense tail of the main buffer (_fefm_scores).  Decided once from the model's graph;
     every other graph plans nothing and keeps its row pitch."""
     if not DNN_INPUT_PLACEMENT:
         return {}
@@ -1052,7 +1044,7 @@ def _plan_pnn_input(g):
     concat([linear_signal, Flatten(InnerProductLayer(...)), OutterProductLayer(...)]) (deepctr/models/pnn.py:46-63,
     either product or both) when that concatenation reaches the first DNN layer only through combined_dnn_input:
     the planner then reserves the product columns between the embeddings and the dense columns of the main buffer
-    (pnn_place).  Decided once from the model's graph; every other graph plans nothing and keeps its row pitch."""
+    (_pnn_products).  Decided once from the model's graph; every other graph plans nothing and keeps its row pitch."""
     if not DNN_INPUT_PLACEMENT:
         return {}, 0
     from .layers.core import DNN
@@ -1101,13 +1093,14 @@ def _plan_pnn_input(g):
 
 
 def _plan_dnn_input(g):
-    """{id(BilinearInteraction layer): (DnnInputPlacement, index)}, decided once from the model's graph."""
+    """({id(BilinearInteraction layer): (DnnInputPlacement, index)}, [(Concat node, DnnInputPlacement,
+    [BilinearInteraction node] * n)]), decided once from the model's graph."""
     if not DNN_INPUT_PLACEMENT:
-        return {}
+        return {}, []
     from .layers.core import DNN
     from .layers.interaction import BilinearInteraction
     from .layers.utils import Concat, NoMask, _CombinedDNNInput
-    places = {}
+    places, concats = {}, []
     for node in g.order:
         if not isinstance(node.layer, Concat) or node.layer.axis not in (-1, 2):
             continue
@@ -1138,7 +1131,29 @@ def _plan_dnn_input(g):
         pl = DnnInputPlacement(len(srcs), int(P), int(Ed), ndense)
         for k, l in enumerate(layers):
             places[id(l)] = (pl, k)
-    return places
+        concats.append((node, pl, [t.node for t in srcs]))
+    return places, concats
+
+
+def _bilinear_into_dnn_input(concat, layout, nodes, values, training):
+    """The Concat of FiBiNET's bilinear outputs: every BilinearInteraction ``nodes[k]`` writes its pairs into the
+    strided part k of one new [B, ld] buffer, and the Concat is the window [0, n*P*E) of it."""
+    from . import ops
+    inputs = [E._concrete([values[id(t)] for t in n.inputs]) for n in nodes]
+    x0 = inputs[0][0].data
+    b, n, P, E_ = x0.shape[0], layout.n, layout.P, layout.E
+    base = layout.buffer(b, x0.device)
+    t = base.data
+    outs = [node.layer.pairs(x, out=t.as_strided((b, P, E_), (layout.ld, n * E_, 1), t.storage_offset() + k * E_))
+            for k, (node, x) in enumerate(zip(nodes, inputs))]
+
+    def bwd(grads):
+        g = grads[0]
+        for k, v in enumerate(outs):
+            E.add_grad(v, g.as_strided((b, P, E_), (g.stride(0), n * E_, 1), g.storage_offset() + k * E_))
+
+    E.record([base], outs, bwd)
+    return {id(concat): ops._window(base, 0, layout.width, (b, P, n * E_))}
 
 
 class RegulatePlan(object):

@@ -144,11 +144,6 @@ class FM(Layer):
     def call(self, inputs, **kwargs):
         if len(inputs.shape) != 3:
             raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (len(inputs.shape)))
-        planner = getattr(self, "_planner", None)
-        if planner is not None and not isinstance(inputs, ops.ScaledFields):
-            fused = planner.lookup_fm(inputs)
-            if fused is not None:
-                return fused
         return ops.fm(inputs)
 
     def compute_output_shape(self, input_shape):
@@ -382,7 +377,8 @@ class BilinearInteraction(Layer):
     tensors; output [B, P, E] with row p = (i < j) equal to (v_i W) * v_j, W one weight ('all'), one per first field
     ('each') or one per pair ('interaction').  The weights keep the reference's names and order but their data are
     views of one stacked [nW, E, E] buffer, which is what b2ctr_bilinear_fwd / _bwd take.  When the model's graph
-    lets it (inputs.DnnInputPlacement), the pairs are written straight into the first DNN layer's input."""
+    lets it (inputs.DnnInputPlacement), the pairs are written straight into the first DNN layer's input where the
+    Concat of the layers' outputs runs (inputs._bilinear_into_dnn_input)."""
 
     def __init__(self, bilinear_type="interaction", seed=1024, **kwargs):
         self.bilinear_type = bilinear_type
@@ -414,21 +410,17 @@ class BilinearInteraction(Layer):
         self.built = True
 
     def call(self, inputs, **kwargs):
+        return self.pairs(inputs)
+
+    def pairs(self, inputs, out=None):
+        """The [B, P, E] pairs of the list ``inputs``, written into the strided [B, P, E] view ``out`` if given."""
         if inputs[0].data.dim() != 3:
             raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs[0].data.dim()))
         if self.bilinear_type not in ("all", "each", "interaction"):
             raise NotImplementedError
         x = ops.concat(inputs, axis=1)
         ws, st = _weights_stacked(self, [self.W] if self.bilinear_type == "all" else self.W_list)
-        planner = getattr(self, "_planner", None)
-        place = planner.dnn_input_place(self) if planner is not None else None
-        if place is None:
-            return ops.bilinear_interaction(x, ws, st, self.bilinear_type)
-        pl, k = place
-        b, f, e = x.data.shape
-        out = ops.bilinear_interaction(x, ws, st, self.bilinear_type, out=pl.out_view(k, b, x.data.device))
-        pl.placed(k, out)
-        return out
+        return ops.bilinear_interaction(x, ws, st, self.bilinear_type, out=out)
 
     def compute_output_shape(self, input_shape):
         filed_size = len(input_shape)
@@ -491,7 +483,7 @@ class FEFMLayer(Layer):
     column p = (i < j) equal to x_i (W_p + W_p^T) x_j^T.  The P weights field_embeddings{i}-{j} keep the reference's
     names and order but their data are views of one stacked [P, E, E] buffer, which is what b2ctr_fefm_sym / _fwd /
     _bwd take.  In DeepFEFM the scores are written straight into the first DNN layer's input
-    (inputs.EmbeddingPlanner.fefm_place)."""
+    (inputs.EmbeddingPlanner._fefm_scores)."""
 
     def __init__(self, regularizer, **kwargs):
         self.regularizer = regularizer
@@ -519,12 +511,14 @@ class FEFMLayer(Layer):
         self.built = True
 
     def call(self, inputs, **kwargs):
-        if inputs.data.dim() != 3:
-            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs.data.dim()))
+        return self.scores(inputs)
+
+    def scores(self, x, out=None):
+        """The [B, P] scores of ``x``, written into the [B, P] column window ``out`` of a wider buffer if given."""
+        if x.data.dim() != 3:
+            raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (x.data.dim()))
         ws, st = _weights_stacked(self, list(self.field_embeddings.values()))
-        planner = getattr(self, "_planner", None)
-        out = planner.fefm_place(self, inputs) if planner is not None else None
-        return ops.fefm(inputs, ws, st, out=out)
+        return ops.fefm(x, ws, st, out=out)
 
     def compute_output_shape(self, input_shape):
         # the reference divides with `/` (a float); the graph here needs the integer column count
@@ -559,11 +553,6 @@ def _check_product_inputs(name, input_shape):
     return num_inputs, embed_size
 
 
-def _product_place(layer, x):
-    planner = getattr(layer, "_planner", None)
-    return planner.pnn_place(layer, x) if planner is not None else None
-
-
 def _product_operand(inputs):
     if inputs[0].data.dim() != 3:
         raise ValueError("Unexpected inputs dimensions %d, expect to be 3 dimensions" % (inputs[0].data.dim()))
@@ -576,7 +565,7 @@ class InnerProductLayer(Layer):
     [B, P, 1] with row p = (i < j) equal to <v_i, v_j> (reduce_sum=True), or [B, P, E] with v_i * v_j
     (b2ctr_pnn_inner_fwd: the gather buffer is read in place and no per-pair [B, E] product is written for the
     inner products).  In PNN the products are written straight into the first DNN layer's input
-    (inputs.EmbeddingPlanner.pnn_place)."""
+    (inputs.EmbeddingPlanner._pnn_products)."""
 
     def __init__(self, reduce_sum=True, **kwargs):
         self.reduce_sum = reduce_sum
@@ -587,10 +576,13 @@ class InnerProductLayer(Layer):
         self.built = True
 
     def call(self, inputs, **kwargs):
-        x = _product_operand(inputs)
+        return self.products(_product_operand(inputs))
+
+    def products(self, x, out=None):
+        """The products of the [B, F, E] operand ``x``; the inner products into the [B, P] window ``out`` if given."""
         if not self.reduce_sum:
             return ops.pnn_inner(x, "elementwise")
-        return ops.pnn_inner(x, "inner", out=_product_place(self, x))
+        return ops.pnn_inner(x, "inner", out=out)
 
     def compute_output_shape(self, input_shape):
         num_inputs = len(input_shape)
@@ -632,8 +624,10 @@ class OutterProductLayer(Layer):
         self.built = True
 
     def call(self, inputs, **kwargs):
-        x = _product_operand(inputs)
-        out = _product_place(self, x)
+        return self.products(_product_operand(inputs))
+
+    def products(self, x, out=None):
+        """The [B, P] products of the [B, F, E] operand ``x``, written into the [B, P] window ``out`` if given."""
         if self.kernel_type == 'mat':
             return ops.pnn_outer(x, self.kernel, out=out)
         return ops.pnn_inner(x, self.kernel_type, self.kernel, out=out)

@@ -199,23 +199,19 @@ class Linear(Layer):
                                           initializer=glorot_normal(self.seed), regularizer=l2(self.l2_reg))
         self.built = True
 
-    def _sparse_sum(self, sparse_input):
-        planner = getattr(self, "_planner", None)
-        fused = planner.lookup_rowsum(sparse_input) if planner is not None else None
-        return fused if fused is not None else ops.rowsum(sparse_input)
-
     def call(self, inputs, **kwargs):
+        if self.mode == 1:
+            return ops.dense(ops.flatten(inputs), self.kernel, self.bias if self.use_bias else None)
+        return self.combine(ops.rowsum(inputs if self.mode == 0 else inputs[0]), inputs)
+
+    def combine(self, sparse_sum, inputs):
+        """Modes 0 and 2: the output from ``sparse_sum`` [B, 1], the row-sum of the sparse input (computed here, or
+        by the fused gather: inputs.EmbeddingPlanner._linear), plus the bias (mode 0) or the dense part (mode 2)."""
         bias = self.bias if self.use_bias else None
         if self.mode == 0:
-            out = self._sparse_sum(inputs)
-            if bias is not None:
-                out = ops.add_bias(out, bias)
-            return out
-        if self.mode == 1:
-            return ops.dense(ops.flatten(inputs), self.kernel, bias)
-        sparse_input, dense_input = inputs
-        fc = ops.dense(ops.flatten(dense_input), self.kernel, bias)
-        return ops.add_n([self._sparse_sum(sparse_input), fc])
+            return sparse_sum if bias is None else ops.add_bias(sparse_sum, bias)
+        fc = ops.dense(ops.flatten(inputs[1]), self.kernel, bias)
+        return ops.add_n([sparse_sum, fc])
 
     def compute_output_shape(self, input_shape):
         return (None, 1)
@@ -362,16 +358,10 @@ def add_func(inputs):
 class _CombinedDNNInput(Layer):
     """Flatten(concat(embeddings)) || Flatten(concat(dense)) as ONE op: when the embeddings are the
     planner's main buffer the dense features are appended behind them in place and the result is a
-    zero-copy window (the K-padded GEMM operand)."""
+    zero-copy window (the K-padded GEMM operand; inputs.EmbeddingPlanner._combined_dnn_input)."""
 
     def call(self, inputs, **kwargs):
-        sparse_part, dense_part = inputs
-        planner = getattr(self, "_planner", None)
-        if planner is not None:
-            win = planner.append_dense(sparse_part, dense_part)
-            if win is not None:
-                return win
-        return ops.concat([sparse_part, dense_part], -1)
+        return ops.concat(inputs, -1)
 
     def compute_output_shape(self, input_shape):
         return (input_shape[0][0], input_shape[0][1] + input_shape[1][1])

@@ -1,6 +1,6 @@
 """FiBiNET (Huang et al. 2019) - drop-in for the reference builder deepctr/models/fibinet.py:19-66.
 logit = first-order term + DNN tower over [Bilinear(SENET(embeddings)) || Bilinear(embeddings) || dense features].
-Both bilinear layers write their pairs straight into the first DNN layer's input (inputs.DnnInputPlacement)."""
+Both bilinear layers write their pairs into the DNN input where their Concat runs (inputs._bilinear_into_dnn_input)."""
 from ..engine import Dense, Flatten
 from ..layers.core import DNN
 from ..layers.interaction import BilinearInteraction, SENETLayer

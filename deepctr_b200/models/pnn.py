@@ -4,8 +4,8 @@ DNN input = [embeddings F*E || inner products P || outer products P || dense fea
 As in the reference, InnerProductLayer and OutterProductLayer are both created and called whatever the switches say;
 a product that is not on the output path holds no weight in the model and launches nothing.  When the concatenation
 reaches the first DNN layer only through combined_dnn_input, the products are written straight into the gather buffer
-between the embeddings and the dense columns (inputs.EmbeddingPlanner.pnn_place), so the DNN input is a zero-copy
-window of it."""
+between the embeddings and the dense columns (inputs.EmbeddingPlanner._pnn_products), so the DNN input is a
+zero-copy window of it."""
 from ..engine import Dense, Flatten, Model, Reshape
 from ..feature_column import build_input_features, input_from_feature_columns
 from ..layers.core import DNN, PredictionLayer

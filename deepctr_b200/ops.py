@@ -208,11 +208,6 @@ def concat(xs, axis=-1):
     xs = list(xs)
     if len(xs) == 1:
         return xs[0]
-    placed = getattr(xs[0].owner, "placed_concat", None)
-    if placed is not None:             # outputs written side by side into one buffer (inputs.DnnInputPlacement)
-        res = placed(xs, axis)
-        if res is not None:
-            return res
     shapes = [tuple(v.shape) for v in xs]
     ax, flat_ok = _flat_concat_ok(shapes, axis)
     out_shape = list(shapes[0])
@@ -655,7 +650,7 @@ def fefm(x, weights, stack, out=None):
     x is read in place; no per-pair [B,E] product is written.
 
     ``out``: a [B,P] column window (``_window``) of a wider buffer Var to write the scores into (DeepFEFM's DNN
-    input behind the gather buffer's dense columns, inputs.EmbeddingPlanner.fefm_place); it is returned.  Every
+    input behind the gather buffer's dense columns, inputs.EmbeddingPlanner._fefm_scores); it is returned.  Every
     consumer's gradient then lands in that buffer's gradient, so the backward is keyed on the buffer: it reads the
     score columns of its gradient in place and leaves the gradient to the buffer's own backward (the gather's
     scatter), which runs after it.  Default: a new [B,P] tensor."""
@@ -703,7 +698,7 @@ def pnn_inner(x, mode, kernel=None, out=None):
     :912-919, with ``kernel`` [P,E] / [P,1]).  x is read in place.
 
     ``out``: a [B,P] column window (``_window``) of a wider buffer Var to write the scores into (PNN's DNN input,
-    inputs.EmbeddingPlanner.pnn_place); the result is then a window of that buffer.  Every consumer's gradient
+    inputs.EmbeddingPlanner._pnn_products); the result is then a window of that buffer.  Every consumer's gradient
     lands in that buffer's gradient, so the backward is keyed on the buffer: it reads the score columns of its
     gradient in place and leaves the gradient to the buffer's own backward (the gather's scatter), as ops.fefm."""
     b, f, e = x.data.shape

@@ -5,7 +5,8 @@
   and batches that are not a multiple of a CTA's samples; both backwards are bit-identical from run to run;
 * layer fixtures of the reference's own SENETLayer / BilinearInteraction (tests/golden/fibinet/, with
   model_golden_checks): through the layers, outputs and gradients in both GEMM precisions;
-* with the DNN-input placement no copy wider than the dense tail touches the DNN input ;
+* with the DNN-input placement no copy wider than the dense tail touches the DNN input; a bilinear layer called eagerly
+  after training is not placed;
 * model fixtures (with model_golden_checks): logits and one SGD step in both GEMM precisions, placed and unplaced;
   a graph-replayed training step equals an eager one; the placement gives the results of the unplaced graph;
 * the C2 shape (26 fields, E = 32, B = 65536, 13 dense features: a [65536, 20816] DNN input and a K = 20813 GEMM):
@@ -149,27 +150,27 @@ def test_kernels_reject_unsupported_shapes(cuda):
         K.senet_fwd(x, 65 * 4, 65, 4, torch.zeros((65, 2), device=cuda), torch.zeros((2, 65), device=cuda), 4)
 
 
-def test_placed_step_copies_only_the_dense_tail(cuda, monkeypatch):
+def test_placed_step_buffer_takes_only_the_dense_tail_copy(cuda, monkeypatch):
     """With the placement, the only copy kernel that reads or writes the DNN input is the dense tail's (3 columns);
     without it, the bilinear outputs are copied by the Concat and again by combined_dnn_input."""
     from deepctr_b200 import kernels as K
     from deepctr_b200.engine import SGD
     from deepctr_b200 import inputs as I
     events = []                # ("buf", lo, hi) when a step's DNN-input buffer is made, ("copy", src, dst, cols)
-    real_copy, real_view = K.copy2d, I.DnnInputPlacement.out_view
+    real_copy, real_buffer = K.copy2d, I.DnnInputPlacement.buffer
 
     def copy_spy(src, ld_src, dst, ld_dst, rows, cols, accumulate=False, src_off=0, dst_off=0):
         events.append(("copy", src.data_ptr() + 4 * src_off, dst.data_ptr() + 4 * dst_off, int(cols)))
         return real_copy(src, ld_src, dst, ld_dst, rows, cols, accumulate=accumulate, src_off=src_off,
                          dst_off=dst_off)
 
-    def view_spy(self, k, b, device):
-        v = real_view(self, k, b, device)
-        st = v.untyped_storage()
+    def buffer_spy(self, b, device):
+        v = real_buffer(self, b, device)
+        st = v.data.untyped_storage()
         events.append(("buf", st.data_ptr(), st.data_ptr() + st.nbytes()))
         return v
     monkeypatch.setattr(K, "copy2d", copy_spy)
-    monkeypatch.setattr(I.DnnInputPlacement, "out_view", view_spy)
+    monkeypatch.setattr(I.DnnInputPlacement, "buffer", buffer_spy)
     widths = {}
     for placed in (True, False):
         I.DNN_INPUT_PLACEMENT = placed
@@ -192,6 +193,26 @@ def test_placed_step_copies_only_the_dense_tail(cuda, monkeypatch):
     P, E_ = 45, 8
     assert widths[True] == [3], widths[True]
     assert max(widths[False]) >= 2 * P * E_, widths[False]
+
+
+def test_eager_bilinear_call_after_training_is_unplaced(cuda):
+    """A BilinearInteraction of a trained FiBiNET called eagerly returns its own contiguous [B,P,E] output, equal to
+    the same call before the model ever ran: the DNN-input placement belongs to the model's steps only."""
+    from deepctr_b200.engine import SGD
+    from deepctr_b200.layers import BilinearInteraction
+    model, x, y = H.criteo_model("FiBiNET", np.random.RandomState(6), dnn_hidden_units=(16,))
+    layer = next(l for l in model.layers if isinstance(l, BilinearInteraction))
+    assert id(layer) in model.planner.dnn_places
+    model._materialize()
+    gen = torch.Generator(device=cuda).manual_seed(2)
+    inputs = [torch.randn((64, 1, 8), device=cuda, generator=gen) for _ in range(10)]
+    before = layer(inputs).data.clone()
+    model.compile(SGD(0.0), "binary_crossentropy", embedding_update="sparse", step_graph="off")
+    model.train_on_batch(x, y)
+    out = layer(inputs)
+    assert out.owner is None and out.base is None
+    assert tuple(out.data.shape) == (64, 45, 8) and out.data.is_contiguous()
+    assert torch.equal(out.data, before)
 
 
 def test_c2_shape_tail_rows_match_the_oracle(cuda):
