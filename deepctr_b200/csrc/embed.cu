@@ -1002,6 +1002,8 @@ static b2ctr_status_t ffm_params(const b2ctr_ffm_field_t* fields, int32_t nfield
   const int64_t P = (int64_t)nfield * (nfield - 1) / 2;
   B2_REQUIRE(ld >= col + P * (reduce_sum ? 1 : dim), "ffm_product: row pitch %lld too small for %lld products",
              (long long)ld, (long long)P);
+  // the table pointers live in device memory and cannot be checked here: b2ctr.h makes 16-byte aligned tables
+  // a precondition when dim % 4 == 0 (FieldAwarePlan checks its host copy of them)
   bool v4 = dim % 4 == 0 && ld % 4 == 0 && col % 4 == 0 && aligned16(tables);
   for (int a = 0; a < nfield; ++a) {
     const b2ctr_ffm_field_t& f = fields[a];

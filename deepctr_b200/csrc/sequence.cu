@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(256)
 // ------------------------------------------------------------------------------------------------
 // Standalone SequencePoolingLayer / WeightedSequenceLayer on an arbitrary [B,T,E] tensor
 // (same arithmetic order as the fused gather: ascending t, fp32, no fma contraction)
-// mode: 1 sum, 2 mean, 3 max.  valid(b,t) = mask ? mask[b,t] : t < len[b];  L = len[b] or popcount(mask)
+// mode: 1 sum, 2 mean, 3 max.  valid(b,t) = mask ? mask[b,t] != 0 : t < len[b];  L = len[b] or the valid count
 // ------------------------------------------------------------------------------------------------
 __global__ void seqpool_fwd_kernel(const float* __restrict__ x, const uint8_t* __restrict__ mask,
                                    const int32_t* __restrict__ len, float* out, int64_t batch, int T, int E,
@@ -137,7 +137,7 @@ __global__ void seqpool_fwd_kernel(const float* __restrict__ x, const uint8_t* _
     const int64_t b = i / E;
     const int e = (int)(i - b * E);
     float L = 0.f;
-    if (mask) { int c = 0; for (int t = 0; t < T; ++t) c += mask[b * T + t]; L = (float)c; }
+    if (mask) { int c = 0; for (int t = 0; t < T; ++t) c += mask[b * T + t] != 0; L = (float)c; }
     else L = (float)len[b];
     float acc = 0.f;
     for (int t = 0; t < T; ++t) {
@@ -163,7 +163,7 @@ __global__ void seqpool_bwd_kernel(const float* __restrict__ x, const uint8_t* _
     const int64_t b = i / E;
     const int e = (int)(i - b * E);
     float L = 0.f;
-    if (mask) { int c = 0; for (int t = 0; t < T; ++t) c += mask[b * T + t]; L = (float)c; }
+    if (mask) { int c = 0; for (int t = 0; t < T; ++t) c += mask[b * T + t] != 0; L = (float)c; }
     else L = (float)len[b];
     float g = dout[i];
     if (mode == 2) g = g / (L + 1e-8f);

@@ -1372,6 +1372,12 @@ class FieldAwarePlan(object):
         in place only when a table moved."""
         ptrs = tuple(t.embeddings.materialize().data_ptr() if t is not None else 0 for t in self.table_of)
         if ptrs != self._ptrs:
+            # b2ctr_ffm_product_* read the tables with float4 loads when E % 4 == 0 and cannot see these pointers
+            bad = [k for k, p in enumerate(ptrs) if p % 16] if self.E % 4 == 0 else []
+            if bad:
+                raise ValueError("field-aware tables must be 16-byte aligned when the embedding dim (%d) is a "
+                                 "multiple of 4: table %d (field %d, partner %d) is at 0x%x"
+                                 % (self.E, bad[0], bad[0] // self.F, bad[0] % self.F, ptrs[bad[0]]))
             host = torch.tensor(ptrs, dtype=torch.int64)
             if self._dev_ptrs is None:
                 self._dev_ptrs = host.to(dev)

@@ -201,6 +201,8 @@ B2CTR_API b2ctr_status_t b2ctr_embed_oob_count(int64_t* count, int32_t reset, vo
  * counted as for every other gather (b2ctr_embed_oob_count).
  *   tables: DEVICE array [F*F] of device pointers, field a's table for partner b at a*F + b (the diagonal is
  *           unused); it can stay at one address for the life of a model, so a captured step keeps it.
+ *           When dim % 4 == 0, every table must be 16-byte aligned: the kernel takes its float4 path from the
+ *           other operands' alignment and cannot see the pointers inside this device array.
  * A field is either single-valued (idx != NULL) or a pre-pooled operand (pooled != NULL: a VarLenSparseFeat bag
  * pooled per partner by b2ctr_embed_gather_fwd).  Partner b of field a has slot s = b - (b > a) in `pooled` and
  * `grad`, whose rows hold F-1 operands of dim floats.  2 <= F <= 64, 1 <= dim <= 64. */
@@ -818,7 +820,8 @@ B2CTR_API b2ctr_status_t b2ctr_din_pool_bwd(const float* w, const float* keys, i
                                            float* dkeys, int64_t batch, int32_t T, int32_t E,
                                            int32_t weight_norm, int32_t return_score, void* stream);
 /* SequencePoolingLayer on a materialised [B,T,E] tensor (deepctr/layers/sequence.py:76-106);
- * mode = B2CTR_POOL_SUM/MEAN/MAX; validity from mask (uint8 [B,T]) or len ([B]).               */
+ * mode = B2CTR_POOL_SUM/MEAN/MAX; validity from mask (uint8 [B,T], any non-zero byte is a valid
+ * position, and mean divides by the number of valid positions) or len ([B]).                   */
 B2CTR_API b2ctr_status_t b2ctr_seqpool_fwd(const float* x, const uint8_t* mask, const int32_t* len,
                                           float* out, int64_t batch, int32_t T, int32_t E,
                                           int32_t mode, void* stream);
