@@ -157,6 +157,7 @@ SIGNATURES = {
     "b2ctr_reset_launch_count": (None, []),
     "b2ctr_embed_gather_fwd": (_i32, [C.POINTER(Feature), _i32, _i64, _vp]),
     "b2ctr_embed_scatter_add": (_i32, [C.POINTER(Feature), _i32, _i64, _f32, _vp]),
+    "b2ctr_embed_max_pool_shares": (_i32, [C.POINTER(Feature), _i32, _i64, _vp, _i64, _vp]),
     "b2ctr_embed_gather_uniform_fwd": (_i32, [C.POINTER(UniformGather), _i64, _vp]),
     "b2ctr_embed_scatter_uniform_bwd": (_i32, [C.POINTER(UniformGather), _vp, _vp, _vp, _f32, _f32,
                                                _i64, _vp]),

@@ -303,6 +303,51 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// Max pooling's backward for the VEC columns at e of sample b, at the forward rows `src` (which nothing may write
+// during the launch): TF's max gradient splits g evenly among the positions that attain the max.  Pass 0 finds the
+// max and its count per column, pass 1 calls emit(t, id, ok, hit[VEC], share[VEC]) for every position t, with
+// share[i] = g[i] / cnt[i] * w_t valid where hit[i] (the position attains the max of column i).
+template <int VEC, class Emit>
+__device__ __forceinline__ void max_pool_bwd(const b2ctr_feature_t& ft, const float* src, const SeqInfo& si,
+                                             int64_t b, int len, int e, const float* gv, Emit emit) {
+  using V = typename VecT<VEC>::T;
+  const int dim = ft.dim, T = ft.maxlen;
+  const int64_t ibase = b * ft.idx_stride;
+  float mx[VEC];
+  int cnt[VEC];
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) { mx[i] = -INFINITY; cnt[i] = 0; }
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int t = 0; t < T; ++t) {
+      const int64_t id = lookup_id(ft, ibase + t);
+      const bool valid = pos_valid(ft, t, id, len);
+      const bool ok = id_in_range(id, ft.vocab);
+      V xv = ok ? vload(src + id * dim + e, (V*)nullptr) : vzero<VEC>();
+      const float w = pos_weight(ft, si, b, t, valid);
+      if (ft.weight_mode != B2CTR_WEIGHT_NONE) xv = vmuls(xv, w);
+      if (!valid) xv = vsubs(xv, 1e9f);
+      float xs[VEC];
+      *reinterpret_cast<V*>(xs) = xv;
+      if (pass == 0) {
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) {
+          if (xs[i] > mx[i]) { mx[i] = xs[i]; cnt[i] = 1; }
+          else if (xs[i] == mx[i]) cnt[i]++;
+        }
+      } else {
+        bool hit[VEC];
+        float share[VEC];
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) {
+          hit[i] = xs[i] == mx[i];
+          share[i] = gv[i] / (float)cnt[i] * w;
+        }
+        emit(t, id, ok, hit, share);
+      }
+    }
+  }
+}
+
 template <int G, int VEC>
 __global__ void __launch_bounds__(256)
     embed_scatter_generic_kernel(const __grid_constant__ FeatBlock fb, int64_t batch, float scale) {
@@ -340,39 +385,16 @@ __global__ void __launch_bounds__(256)
       V g = vmuls(vload(gout + e, (V*)nullptr), scale);
       if (ft.pool == B2CTR_POOL_MEAN) g = vdivs(g, __fadd_rn(si.L, 1e-8f));
       if (ft.pool == B2CTR_POOL_MAX) {
-        // TF's max gradient: split evenly among the positions that attain the max
-        float gv[VEC], mx[VEC];
-        int cnt[VEC];
-        {
-          float tmp[VEC];
-          *reinterpret_cast<V*>(tmp) = g;
+        // the arg-max is re-found at src_table, which the host requires to be a buffer other than `table`
+        float gv[VEC];
+        *reinterpret_cast<V*>(gv) = g;
+        float* tab = ft.table;
+        max_pool_bwd<VEC>(ft, ft.src_table, si, b, len, e, gv,
+                          [&](int, int64_t id, bool ok, const bool* hit, const float* share) {
 #pragma unroll
-          for (int i = 0; i < VEC; ++i) { gv[i] = tmp[i]; mx[i] = -INFINITY; cnt[i] = 0; }
-        }
-        for (int pass = 0; pass < 2; ++pass) {
-          for (int t = 0; t < T; ++t) {
-            const int64_t id = lookup_id(ft, ibase + t);
-            const bool valid = pos_valid(ft, t, id, len);
-            const bool ok = id_in_range(id, ft.vocab);
-            V xv = ok ? vload((ft.src_table ? ft.src_table : ft.table) + id * dim + e, (V*)nullptr) : vzero<VEC>();
-            const float w = pos_weight(ft, si, b, t, valid);
-            if (ft.weight_mode != B2CTR_WEIGHT_NONE) xv = vmuls(xv, w);
-            if (!valid) xv = vsubs(xv, 1e9f);
-            float xs[VEC];
-            *reinterpret_cast<V*>(xs) = xv;
-            if (pass == 0) {
-#pragma unroll
-              for (int i = 0; i < VEC; ++i) {
-                if (xs[i] > mx[i]) { mx[i] = xs[i]; cnt[i] = 1; }
-                else if (xs[i] == mx[i]) cnt[i]++;
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < VEC; ++i)
-                if (xs[i] == mx[i] && ok) red_add_f1(ft.table + id * dim + e + i, gv[i] / (float)cnt[i] * w);
-            }
-          }
-        }
+                            for (int i = 0; i < VEC; ++i)
+                              if (hit[i] && ok) red_add_f1(tab + id * dim + e + i, share[i]);
+                          });
         continue;
       }
       for (int t = 0; t < T; ++t) {
@@ -383,6 +405,48 @@ __global__ void __launch_bounds__(256)
         if (ft.weight_mode != B2CTR_WEIGHT_NONE) gt = vmuls(gt, pos_weight(ft, si, b, t, true));
         vred(ft.table + id * dim + e, gt);
       }
+    }
+  }
+}
+
+// Max pooling's backward written out per position instead of applied: a fused update (`table` updated in place)
+// cannot re-find the arg-max at rows it is writing.  Feature f's [T, dim] block of sample b starts at
+// shares + b * ld + col[f]; every element of it is written.
+struct ShareBlock {
+  FeatBlock fb;
+  float* shares;
+  int64_t ld;
+  int64_t col[kFeatChunk];
+};
+
+template <int G, int VEC>
+__global__ void __launch_bounds__(256)
+    embed_max_shares_kernel(const __grid_constant__ ShareBlock sb, int64_t batch) {
+  using V = typename VecT<VEC>::T;
+  constexpr int kGroups = 256 / G;
+  const FeatBlock& fb = sb.fb;
+  const int lane = threadIdx.x % G;
+  const int64_t ntasks = batch * fb.nfeat;
+  for (int64_t task = (int64_t)blockIdx.x * kGroups + threadIdx.x / G; task < ntasks;
+       task += (int64_t)gridDim.x * kGroups) {
+    const int64_t b = task / fb.nfeat;
+    const int k = (int)(task - b * fb.nfeat);
+    const b2ctr_feature_t& ft = fb.f[k];
+    const int dim = ft.dim;
+    const float* gout = ft.out + b * ft.out_ld + ft.out_col;
+    float* dst = sb.shares + b * sb.ld + sb.col[k];
+    const int len = ft.mask_mode == B2CTR_MASK_LENGTH ? ft.len[b * lstride(ft)] : 0;
+    const SeqInfo si = seq_info(ft, b);
+    for (int e = lane * VEC; e < dim; e += G * VEC) {
+      float gv[VEC];
+      *reinterpret_cast<V*>(gv) = vload(gout + e, (V*)nullptr);
+      max_pool_bwd<VEC>(ft, ft.table, si, b, len, e, gv,
+                        [&](int t, int64_t, bool ok, const bool* hit, const float* share) {
+                          float s[VEC];
+#pragma unroll
+                          for (int i = 0; i < VEC; ++i) s[i] = hit[i] && ok ? share[i] : 0.f;
+                          vstore(dst + (int64_t)t * dim + e, *reinterpret_cast<V*>(s));
+                        });
     }
   }
 }
@@ -779,7 +843,8 @@ static b2ctr_status_t validate_feats(const b2ctr_feature_t* feats, int32_t nfeat
     B2_REQUIRE(f.hash_mode >= 0 && f.hash_mode <= 2, "embed: feature %d bad hash_mode", i);
     B2_REQUIRE(f.hash_mode != B2CTR_HASH_FARM_MASK_ZERO || f.vocab >= 2,
                "embed: feature %d: mask_zero hashing needs >= 2 buckets", i);
-    if (f.dim % 4 || f.out_col % 4 || f.out_ld % 4 || !aligned16(f.table) || !aligned16(f.out))
+    if (f.dim % 4 || f.out_col % 4 || f.out_ld % 4 || !aligned16(f.table) || !aligned16(f.out) ||
+        !aligned16(f.src_table))
       *vec4 = false;
   }
   for (int i = 0; i < nfeat; ++i) {
@@ -1066,6 +1131,10 @@ b2ctr_status_t b2ctr_embed_scatter_add(const b2ctr_feature_t* feats, int32_t nfe
   int lanes;
   b2ctr_status_t s = validate_feats(feats, nfeat, batch, &vec4, &lanes);
   if (s != B2CTR_OK) return s;
+  for (int i = 0; i < nfeat; ++i)
+    B2_REQUIRE(feats[i].pool != B2CTR_POOL_MAX || (feats[i].src_table && feats[i].src_table != feats[i].table),
+               "embed_scatter_add: max-pooled feature %d needs its forward rows in a src_table other than the table "
+               "it updates (b2ctr_embed_max_pool_shares serves updates in place)", i);
   if (batch == 0) return B2CTR_OK;
   cudaStream_t st = (cudaStream_t)stream;
   for (int base = 0; base < nfeat; base += kFeatChunk) {
@@ -1075,6 +1144,41 @@ b2ctr_status_t b2ctr_embed_scatter_add(const b2ctr_feature_t* feats, int32_t nfe
     for (int i = 0; i < fb.nfeat; ++i) fb.f[i] = feats[base + i];
     B2_DISPATCH_G(embed_scatter_generic_kernel, lanes, vec4, fb, batch, scale);
     B2_CHECK_LAUNCH("b2ctr_embed_scatter_add");
+  }
+  return B2CTR_OK;
+}
+
+b2ctr_status_t b2ctr_embed_max_pool_shares(const b2ctr_feature_t* feats, int32_t nfeat, int64_t batch,
+                                           float* shares, int64_t shares_ld, void* stream) {
+  bool vec4;
+  int lanes;
+  b2ctr_status_t s = validate_feats(feats, nfeat, batch, &vec4, &lanes);
+  if (s != B2CTR_OK) return s;
+  int64_t cols = 0;
+  for (int i = 0; i < nfeat; ++i) {
+    B2_REQUIRE(feats[i].pool == B2CTR_POOL_MAX, "embed_max_pool_shares: feature %d is not max-pooled", i);
+    cols += (int64_t)feats[i].maxlen * feats[i].dim;
+  }
+  B2_REQUIRE(shares && shares_ld >= cols, "embed_max_pool_shares: NULL shares or shares_ld < %lld columns",
+             (long long)cols);
+  if (shares_ld % 4 || !aligned16(shares)) vec4 = false;
+  if (batch == 0) return B2CTR_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t col = 0;
+  for (int base = 0; base < nfeat; base += kFeatChunk) {
+    ShareBlock sb;
+    FeatBlock& fb = sb.fb;
+    fb.oob = nullptr;            // the forward pass already counted them
+    fb.nfeat = nfeat - base < kFeatChunk ? nfeat - base : kFeatChunk;
+    for (int i = 0; i < fb.nfeat; ++i) {
+      fb.f[i] = feats[base + i];
+      sb.col[i] = col;
+      col += (int64_t)fb.f[i].maxlen * fb.f[i].dim;
+    }
+    sb.shares = shares;
+    sb.ld = shares_ld;
+    B2_DISPATCH_G(embed_max_shares_kernel, lanes, vec4, sb, batch);
+    B2_CHECK_LAUNCH("b2ctr_embed_max_pool_shares");
   }
   return B2CTR_OK;
 }

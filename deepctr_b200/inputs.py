@@ -729,6 +729,8 @@ class EmbeddingPlanner(object):
 
     def _backward(self, feed, bufs, plan, fast_slots, generic, lin_fused, batch):
         opt = E.current_opt()
+        # before any table of this step is updated (a fast-path feature may share a max-pooled bag's table)
+        shares = self._max_pool_shares(feed, bufs, generic, batch)
         if fast_slots:
             main = bufs["main"]
             dx = main.grad
@@ -796,11 +798,11 @@ class EmbeddingPlanner(object):
                     K.embed_update_sorted(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
                                           None if dlin is None else dlin.reshape(-1).contiguous(),
                                           1 if adagrad else 0, o.lr, o.lr, 1e-7, acc, lacc, batch)
-                    return self._backward_generic(feed, bufs, generic, opt, batch)
+                    return self._backward_generic(feed, bufs, generic, opt, batch, shares)
                 K.embed_scatter_uniform_bwd(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
                                             None if dlin is None else dlin.reshape(-1).contiguous(),
                                             scale, lin_scale, batch, fm_sum=plan.fm_sum)
-        self._backward_generic(feed, bufs, generic, opt, batch)
+        self._backward_generic(feed, bufs, generic, opt, batch, shares)
 
     @staticmethod
     def _adagrad_state(w):
@@ -810,7 +812,28 @@ class EmbeddingPlanner(object):
             K.fill(acc, 0.1)               # Keras initial_accumulator_value
         return acc
 
-    def _backward_generic(self, feed, bufs, generic, opt, batch):
+    def _max_pool_shares(self, feed, bufs, generic, batch):
+        """Max-pooled bags whose table the fused SGD updates in place cannot re-find their arg-max in the scatter
+        that writes those rows: b2ctr_embed_max_pool_shares writes every position's share of the gradient at the
+        forward rows, and the scatter applies the shares as plain [B, T] lookups.  Returns (shares, {id(slot):
+        first column}), or None when no bag needs it."""
+        sel = []
+        for s in generic:
+            w = s.emb.embeddings
+            buf = bufs[id(s)] if s.buf == "seq" else bufs[s.buf]
+            if s.pool == L.POOL_MAX and w.trainable and w.sparse_grad and buf.grad is not None:
+                sel.append((s, buf.grad))
+        if not sel:
+            return None
+        cols, width = {}, 0
+        for s, _ in sel:
+            cols[id(s)] = width
+            width += s.maxlen * s.dim
+        shares = torch.empty((batch, (width + 3) // 4 * 4), dtype=torch.float32, device=sel[0][1].device)
+        K.embed_max_pool_shares([self._feature(s, feed, g, g.stride(0)) for s, g in sel], batch, shares)
+        return shares, cols
+
+    def _backward_generic(self, feed, bufs, generic, opt, batch, shares=None):
         feats, scales = [], []
         flat = {}            # (rows, scale) -> features of plain sequences re-described as B*T single lookups
         for s in generic:
@@ -820,8 +843,15 @@ class EmbeddingPlanner(object):
             if buf.grad is None:
                 continue
             tgt, scale = _grad_target(s.emb.embeddings, opt)
-            src = s.emb.embeddings.data if s.pool == L.POOL_MAX else None
             ids = feed[s.input_name].data
+            if shares is not None and id(s) in shares[1]:
+                shard = s.emb.embeddings.opt_state.get("shard")
+                feats.append(K.make_feature(tgt, ids, shares[0], out_col=shares[1][id(s)], out_ld=shares[0].stride(0),
+                                            maxlen=s.maxlen, hash_mode=s.hash[0],
+                                            vocab=shard[2] if shard else s.emb.input_dim))
+                scales.append(scale)
+                continue
+            src = s.emb.embeddings.data if s.pool == L.POOL_MAX else None
             g = buf.grad
             if (s.buf == "seq" and s.maxlen > 1 and s.hash[0] == L.HASH_NONE and ids.dim() == 2 and ids.is_contiguous()
                     and g.is_contiguous() and g.shape[1] == s.maxlen * s.dim):
@@ -1454,6 +1484,7 @@ class FieldAwarePlan(object):
             if t.embeddings.trainable:
                 targets[k] = _grad_target(t.embeddings, opt)
         groups = defaultdict(list)
+        inplace = []          # max-pooled bags updated in place: (field, partner, bag feature)
         for a, (name, maxlen, pool, hash_mode, vocab) in enumerate(self.fields):
             tabs = [tg[0] if tg is not None else None for tg in targets]
             if pool == L.POOL_NONE:
@@ -1467,8 +1498,25 @@ class FieldAwarePlan(object):
             else:
                 keep = [c for c in range(F) if c != a]
                 for c, f in zip(keep, self._bag_features(a, feed, scratch, tables=tabs)):
-                    if targets[a * F + c] is not None:
+                    if targets[a * F + c] is None:
+                        continue
+                    if pool == L.POOL_MAX and self.table_of[a * F + c].embeddings.sparse_grad:
+                        inplace.append((a, c, f))
+                    else:
                         groups[targets[a * F + c][1]].append(f)
+        if inplace:
+            # the bag features read their forward rows from `table` (the live table): shares first, then plain
+            # lookups of them (b2ctr_embed_scatter_add refuses a max-pooled feature that updates its own rows)
+            width = sum(self.fields[a][1] * E_ for a, _, _ in inplace)
+            shares = torch.empty((b, (width + 3) // 4 * 4), dtype=torch.float32, device=g.device)
+            K.embed_max_pool_shares([f for _, _, f in inplace], b, shares)
+            col = 0
+            for a, c, _ in inplace:
+                name, maxlen, pool, hash_mode, vocab = self.fields[a]
+                f = K.make_feature(targets[a * F + c][0], feed[name].data, shares, out_col=col,
+                                   out_ld=shares.stride(0), maxlen=maxlen, hash_mode=hash_mode, vocab=vocab)
+                groups[targets[a * F + c][1]].append(f)
+                col += maxlen * E_
         for sc, feats in sorted(groups.items()):
             for c in range(0, len(feats), L.MAX_FEATURES):
                 K.embed_scatter_add(feats[c:c + L.MAX_FEATURES], b, sc)

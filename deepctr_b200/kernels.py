@@ -172,6 +172,16 @@ def embed_scatter_add(feats, batch, scale):
             "embed_scatter_add")
 
 
+@_timed
+def embed_max_pool_shares(feats, batch, shares):
+    """Max pooling's backward per position: feature f's [T*dim] block of ``shares`` (a [batch, >= sum T*dim] view)
+    starts at the sum of the preceding features' T*dim; see b2ctr_embed_max_pool_shares."""
+    _require_cuda(shares)
+    arr = _feat_array(feats)
+    L.check(L.lib().b2ctr_embed_max_pool_shares(arr, len(feats), batch, ptr(shares), shares.stride(0), stream()),
+            "embed_max_pool_shares")
+
+
 class UniformPlan(object):
     """Host-side descriptor for the Criteo-shaped fast path; keeps ctypes arrays alive."""
 

@@ -118,6 +118,17 @@ B2CTR_API b2ctr_status_t b2ctr_embed_gather_fwd(const b2ctr_feature_t* feats, in
  * Duplicate ids are combined with fp32 atomics (vector red.global.add.v4.f32).            */
 B2CTR_API b2ctr_status_t b2ctr_embed_scatter_add(const b2ctr_feature_t* feats, int32_t nfeat,
                                                 int64_t batch, float scale, void* stream);
+/* Max pooling re-finds its arg-max at the forward rows, so a POOL_MAX feature of the scatter above needs them in a
+ * src_table other than `table` (B2CTR_ERR_INVALID_ARG otherwise, before any launch).  An update in place goes
+ * through this call instead: it reads the forward rows from `table` (and writes no table), and writes every
+ * position's share of the gradient `out`
+ *   shares[b*shares_ld + c_f + t*dim + e] = out[b, e] / cnt * w_t   where position t attains the max of column e
+ *                                           0                        elsewhere (and for out-of-range ids)
+ * (cnt = number of positions attaining it, w_t the position weight or 1), c_f = sum over g < f of
+ * maxlen_g * dim_g.  Feature f's block is then one B2CTR_POOL_NONE feature of b2ctr_embed_scatter_add (same ids and
+ * hashing, out = shares, out_col = c_f), which skips the all-zero rows.  Every feature must be POOL_MAX. */
+B2CTR_API b2ctr_status_t b2ctr_embed_max_pool_shares(const b2ctr_feature_t* feats, int32_t nfeat, int64_t batch,
+                                                    float* shares, int64_t shares_ld, void* stream);
 
 /* Criteo-shaped fast path (all features single-valued, same dim, dim % 4 == 0, dim <= 128):
  * one warp per sample gathers F rows with 128-bit loads into x[b, f*dim : (f+1)*dim], copies

@@ -368,7 +368,7 @@ def test_hash64_matches_oracle(cuda):
         assert np.array_equal(got, want)
         got32 = K.hash64(torch.tensor(ids, dtype=torch.int32, device=cuda), nb, mz).cpu().numpy()
         assert np.array_equal(got32, want)
-    big = np.array([2 ** 62 + 12345, -2 ** 63, 2 ** 63 - 1, 10 ** 18], dtype=np.int64)  # 17..20 chars
+    big = np.array([2 ** 62 + 12345, -2 ** 63, 2 ** 63 - 1, 10 ** 18], dtype=np.int64)  # 19 and 20 chars
     got = K.hash64(torch.tensor(big, device=cuda), 10 ** 6, False).cpu().numpy()
     assert np.array_equal(got, O.hash_layer(big, 10 ** 6, False))
 
