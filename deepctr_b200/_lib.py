@@ -22,7 +22,6 @@ WEIGHT_NONE, WEIGHT_RAW, WEIGHT_SOFTMAX = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_SIGMOID, ACT_TANH = 0, 1, 2, 3
 GEMM_FP32, GEMM_BF16X3 = 0, 1
 TASK_BINARY, TASK_REGRESSION = 0, 1
-MAX_FEATURES = 128
 UNIFORM_STORE_GRADS = 1
 
 ACT_BY_NAME = {None: ACT_NONE, "linear": ACT_NONE, "relu": ACT_RELU, "sigmoid": ACT_SIGMOID,

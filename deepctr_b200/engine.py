@@ -1076,6 +1076,7 @@ class Model(object):
         from .inputs import EmbeddingPlanner
         self.planner = EmbeddingPlanner(self)
         self._feeder = None
+        self.dist = None           # the process group's DistContext when compiled for multi-GPU training
 
     # ---- graph -----------------------------------------------------------------------------
     def _toposort(self):
@@ -1217,12 +1218,11 @@ class Model(object):
         the CUDA-IPC mappings of the other ranks' table shards.  Call before dist.destroy_process_group()."""
         self._step_graphs = {}
         self._graph_pool = None
-        planner = getattr(self, "planner", None)
-        if planner is not None and getattr(planner, "peers", None) is not None:
-            for pt in planner.peers[:2]:
+        if self.planner.peers is not None:
+            for pt in self.planner.peers[:2]:
                 if pt is not None:
                     pt.close()
-            planner.peers = None
+            self.planner.peers = None
         gc.collect()
         if torch.cuda.is_available():
             torch.cuda.synchronize()
@@ -1345,8 +1345,7 @@ class Model(object):
         from . import ops
         if self.step_graph in (False, None, "off") or K.PROFILE is not None:
             return False
-        if getattr(self, "dist", None) is not None and getattr(self.planner, "sharded", False) \
-                and not getattr(self.planner, "peer_mode", False):
+        if self.dist is not None and self.planner.sharded and not self.planner.peer_mode:
             return False                       # NCCL all-to-all transport: split sizes are read on the host
         return ops.UNCAPTURABLE == self._uncapturable0
 
@@ -1420,7 +1419,7 @@ class Model(object):
             tape.ctx["optimizer"] = self.optimizer
             tape.backward()
             dense = [w for w in self.trainable_weights if not w.sparse_grad]
-            if getattr(self, "dist", None) is not None:
+            if self.dist is not None:
                 from . import parallel
                 parallel.reduce_dense_grads(
                     self.dist, dense,

@@ -77,9 +77,7 @@ class Embedding(Layer):
 
         def bwd(grads):
             g = grads[0].reshape(b, t * self.output_dim).contiguous()
-            tgt, scale = _grad_target(w, E.current_opt())
-            fb = K.make_feature(tgt, ids2, g, maxlen=t)
-            K.embed_scatter_add([fb], b, scale)
+            _generic_update([K.make_feature(table, ids2, g, maxlen=t)], [w], b, E.current_opt())()
 
         E.record([res], [w], bwd)
         return res
@@ -99,6 +97,52 @@ def _grad_target(w, opt_ctx):
         w.grad = torch.empty_like(w.data)
         K.fill(w.grad, 0.0)
     return w.grad, 1.0
+
+
+def _generic_update(feats, weights, batch, opt):
+    """Apply the gradients of generic lookups to their trainable tables, each at its ``_grad_target``.  ``feats`` are
+    the lookups' gather-shaped features with ``out`` at their gradient rows, ``weights`` their tables' Weights.
+
+    Step one runs here: a max-pooled bag whose table is updated in place cannot re-find its arg-max in the scatter
+    that writes those rows, so b2ctr_embed_max_pool_shares writes every position's share of the gradient at the
+    forward rows, and the bag is applied as plain lookups of the shares.  It must run before any table these
+    features read is updated this step.  Returns step two, the scatter: one b2ctr_embed_scatter_add per distinct
+    scale, then the plain [B, T] sequences re-described as B*T single lookups (one sub-warp per ROW instead of one per
+    sample walking its T rows in sequence: 8192 tasks x 50 dependent updates at C4)."""
+    inplace = [(f, w) for f, w in zip(feats, weights) if f.pool == L.POOL_MAX and w.trainable and w.sparse_grad]
+    shares = None
+    if inplace:
+        width = sum(f.maxlen * f.dim for f, _ in inplace)
+        shares = torch.empty((batch, (width + 3) // 4 * 4), dtype=torch.float32, device=inplace[0][1].data.device)
+        K.embed_max_pool_shares([f for f, _ in inplace], batch, shares)
+
+    def scatter():
+        groups, flat, col = defaultdict(list), defaultdict(list), 0
+        for f, w in zip(feats, weights):
+            if not w.trainable:
+                continue
+            tgt, scale = _grad_target(w, opt)
+            u = L.Feature.from_buffer_copy(f)      # shard vocabulary, hash mode and id stride carry over
+            u.table = tgt.data_ptr()
+            if f.pool == L.POOL_MAX and w.sparse_grad:
+                u.out, u.out_col, u.out_ld = shares.data_ptr(), col, shares.stride(0)
+                u.pool, u.mask_mode, u.weight_mode = L.POOL_NONE, L.MASK_NONE, L.WEIGHT_NONE
+                u.len, u.weight = None, None
+                col += f.maxlen * f.dim
+            elif f.pool == L.POOL_MAX:
+                u.src_table = w.data.data_ptr()
+            elif (f.pool == L.POOL_NONE and f.maxlen > 1 and f.hash_mode == L.HASH_NONE and f.idx_stride == f.maxlen
+                  and f.out_col == 0 and f.out_ld == f.maxlen * f.dim):
+                u.maxlen, u.idx_stride, u.out_ld = 1, 1, f.dim
+                flat[(batch * f.maxlen, scale)].append(u)
+                continue
+            groups[scale].append(u)
+        for sc in sorted(groups):
+            K.embed_scatter_add(groups[sc], batch, sc)
+        for (rows, sc), fs in flat.items():
+            K.embed_scatter_add(fs, rows, sc)
+
+    return scatter
 
 
 # ================================================================================================
@@ -295,6 +339,12 @@ class EmbeddingPlanner(object):
         self.planes_hint = None    # ncols of the leading main-buffer window ops.dense split into bf16 planes
         self.fm_result = None
         self.lin_result = None
+        self.tail_done = None      # (dense col0, ncols) the gather wrote behind the main buffer this step
+        self.planes_result = None  # (ncols, planes) of the bf16 planes the gather wrote this step
+        self.sorted_update = False
+        # multi-GPU (set_dist): the process group, whether the fast-path tables are row-sharded, and over which
+        # transport; `peers` are the NVLink mappings of the other ranks' shards, `route` a step's all-to-all exchange
+        self.dist, self.sharded, self.peer_mode, self.peers, self.route = None, False, False, None, None
         self._plans = {}
         g = _Graph(model)
         # ONN's field-aware lookups and their products: one kernel pair of their own, never slots of the gather
@@ -384,7 +434,9 @@ class EmbeddingPlanner(object):
         self.main_ld = (self.main_width + self.tail_reserve + sum(self.fefm_places.values()) + self.pnn_cols
                         + 3) // 4 * 4
         self.lin_ld = max(1, (self.lin_width + 3) // 4 * 4)
-        self.fast = self._fast_eligible()
+        self.fast_n = self._fast_n()
+        self.fast = self.fast_n >= 1
+        self.lin_matches_fast = self._lin_matches_fast()
         self.dnn_places, bilinear_concats = _plan_dnn_input(g)
         # EDCN's RegulationModule pairs and the bridges in front of them: one b2ctr_regulate launch each
         self.regulate_plan = _plan_regulate(g)
@@ -395,12 +447,15 @@ class EmbeddingPlanner(object):
         # {id(node): (values, training) -> {id(node): result}}: Model._run makes the launch when it reaches that node,
         # and the results serve it and a fused chain's later nodes; {} lets the node's layer run
         self.launches = {}
-        for plan in (self.regulate_plan, self.conv_plan, self.field_wise_plan):
-            self.launches.update(plan.launches())
+        for plan in (self.regulate_plan, self.conv_plan, self.field_wise_plan, self.ffm):
+            if plan is not None:
+                self.launches.update(plan.launches())
         for concat, layout, nodes in bilinear_concats:
             self.launches[id(concat)] = functools.partial(_bilinear_into_dnn_input, concat, layout, nodes)
-        # nodes whose output a launch at a later node folds away: FLEN's concatenations and FiBiNET's bilinear layers
-        self.virtual = self.field_wise_plan.virtual + [n for _, _, nodes in bilinear_concats for n in nodes]
+        # nodes whose output a launch at a later node folds away: FLEN's concatenations, FiBiNET's bilinear layers
+        # and ONN's field-aware lookups and products
+        self.virtual = (self.field_wise_plan.virtual + [n for _, _, nodes in bilinear_concats for n in nodes]
+                        + (self.ffm.virtual if self.ffm is not None else []))
         from .layers.interaction import FM
         from .layers.utils import Linear, _CombinedDNNInput
         for node in g.order:
@@ -483,7 +538,7 @@ class EmbeddingPlanner(object):
         self.sharded = False
         if ctx.world == 1:
             return
-        lin_ok = self.fast and self._lin_matches_fast() and not self.lin_refined
+        lin_ok = self.lin_matches_fast and not self.lin_refined
         shardable = self.fast and (lin_ok or not self.lin)
         will_shard = set()
         if shardable:
@@ -540,25 +595,25 @@ class EmbeddingPlanner(object):
             self.peers = (emb, lin, token)
         return self.peers
 
-    def _fast_eligible(self):
+    def _fast_n(self):
+        """The number of fast-path features: the leading run of plain single-valued features of `main` (the rest goes
+        through the generic kernel), or 0."""
         m = self.main
         if not m or len(m) > 64:
-            return False
+            return 0
         d = m[0].dim
         if d not in (4, 8, 16, 32, 64, 128):
-            return False
-        # the leading run of plain single-valued features (rest of `main` goes through the generic kernel)
+            return 0
         n = 0
         for s in m:
             if s.dim == d and s.maxlen == 1 and s.pool == L.POOL_NONE and s.hash[0] == L.HASH_NONE:
                 n += 1
             else:
                 break
-        self.fast_n = n
-        return n >= 1
+        return n
 
     def _all_fast_single(self):
-        return len(self.main) == self.fast_n and not self.seq and (not self.lin or self._lin_matches_fast())
+        return len(self.main) == self.fast_n and not self.seq and (not self.lin or self.lin_matches_fast)
 
     def _lin_matches_fast(self):
         """linear (dim-1) lookups mirror the fast features one-to-one -> summed inside the kernel."""
@@ -576,8 +631,6 @@ class EmbeddingPlanner(object):
         self.fm_result = self.lin_result = None
         self.tail_done = None
         self.planes_result = None
-        if self.ffm is not None:
-            self.ffm.forward(feed, self.results, training and E.current_tape() is not None)
         if not self.slots:
             return
         some = feed[self.slots[0].input_name].data
@@ -587,7 +640,7 @@ class EmbeddingPlanner(object):
         if self.main:
             bufs["main"] = E.Var(torch.empty((batch, self.main_ld), dtype=torch.float32, device=dev),
                                  ncols=self.main_width, owner=self)
-        lin_fused = self.fast and self.lin_hint and self._lin_matches_fast()
+        lin_fused = self.lin_hint and self.lin_matches_fast
         if self.lin and not lin_fused:
             bufs["lin"] = E.Var(torch.empty((batch, self.lin_ld), dtype=torch.float32, device=dev),
                                 ncols=self.lin_width, owner=self)
@@ -608,12 +661,12 @@ class EmbeddingPlanner(object):
             x = bufs["main"].data
             self.route = None
             peer = None
-            if getattr(self, "sharded", False) and getattr(self, "peer_mode", False):
+            if self.sharded and self.peer_mode:
                 # row-sharded tables addressed in place over NVLink peer mappings: same launch as one GPU
-                peer = self._peer_tables(fast_slots, self.fast and self.lin_hint and self._lin_matches_fast())
+                peer = self._peer_tables(fast_slots, lin_fused)
                 feats = [self._feature(s, feed, x, self.main_ld) for s in fast_slots]
                 lin_tabs = None
-            elif getattr(self, "sharded", False):
+            elif self.sharded:
                 # ids -> owners (all-to-all), rows -> back (all-to-all); the returned row buffer then plays
                 # the role of the table and `pos` the role of the ids for the ordinary fused gather
                 id_feats = [self._feature(s, feed, x, self.main_ld) for s in fast_slots]
@@ -704,7 +757,7 @@ class EmbeddingPlanner(object):
             tape.record(outs, lambda grads: self._backward(feed, bufs, plan, fast_slots, generic, lin_fused,
                                                            batch))
 
-    def _feature(self, s, feed, out, out_ld, table=None, src_table=None):
+    def _feature(self, s, feed, out, out_ld, table=None):
         ids = feed[s.input_name].data
         length = feed[s.len_name].data if s.len_name else None
         weight = feed[s.weight_name].data if s.weight_name else None
@@ -715,7 +768,7 @@ class EmbeddingPlanner(object):
         return K.make_feature(tab, ids, out, out_col=s.col if s.buf != "seq" else 0, out_ld=out_ld,
                               maxlen=s.maxlen, pool=s.pool, mask_mode=s.mask_mode, length=length,
                               weight=weight, weight_mode=s.weight_mode, hash_mode=s.hash[0],
-                              src_table=src_table, vocab=shard[2] if shard else s.emb.input_dim)
+                              vocab=shard[2] if shard else s.emb.input_dim)
 
     @staticmethod
     def _target(w, opt):
@@ -729,14 +782,22 @@ class EmbeddingPlanner(object):
 
     def _backward(self, feed, bufs, plan, fast_slots, generic, lin_fused, batch):
         opt = E.current_opt()
+        feats, weights = [], []
+        for s in generic:
+            g = (bufs[id(s)] if s.buf == "seq" else bufs[s.buf]).grad
+            if g is not None:
+                feats.append(self._feature(s, feed, g, g.stride(0)))
+                weights.append(s.emb.embeddings)
         # before any table of this step is updated (a fast-path feature may share a max-pooled bag's table)
-        shares = self._max_pool_shares(feed, bufs, generic, batch)
+        scatter_generic = _generic_update(feats, weights, batch, opt)
         if fast_slots:
             main = bufs["main"]
             dx = main.grad
             dfm = self.fm_result[1].grad if self.fm_result is not None else None
             dlin = self.lin_result.grad if self.lin_result is not None else None
-            if (dx is not None or dfm is not None or dlin is not None) and getattr(self, "route", None) is not None:
+            dfm = None if dfm is None else dfm.reshape(-1).contiguous()
+            dlin = None if dlin is None else dlin.reshape(-1).contiguous()
+            if (dx is not None or dfm is not None or dlin is not None) and self.route is not None:
                 # sharded: gradient rows are formed in request order, return to their owners over NVLink
                 # and are applied there by the fused SGD scatter (scale = -lr / world: global-batch mean)
                 st, tabs, ltabs, dimf = self.route
@@ -753,9 +814,7 @@ class EmbeddingPlanner(object):
                                       None, None, plan.g.fm_mask[0])
                 bplan.g.x_cols = plan.g.x_cols
                 bplan.g.flags = L.UNIFORM_STORE_GRADS
-                K.embed_scatter_uniform_bwd(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
-                                            None if dlin is None else dlin.reshape(-1).contiguous(),
-                                            1.0, 1.0, batch, fm_sum=plan.fm_sum)
+                K.embed_scatter_uniform_bwd(bplan, dx, dfm, dlin, 1.0, 1.0, batch, fm_sum=plan.fm_sum)
                 lr = opt["optimizer"].lr if opt and opt.get("optimizer") else 0.0
                 sc = -lr / self.dist.world
                 self.exchange.push(st, tabs, ltabs, dimf, grows, glin, sc, sc)
@@ -773,9 +832,7 @@ class EmbeddingPlanner(object):
                 bplan = K.UniformPlan(feats, None, None, main.data, None, None, plan.g.fm_mask[0])
                 bplan.g.x_cols = plan.g.x_cols
                 bplan.set_peers(self.dist.world, emb.table, lin.table if (lin is not None and lin_fused) else None)
-                K.embed_scatter_uniform_bwd(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
-                                            None if dlin is None else dlin.reshape(-1).contiguous(),
-                                            sc, sc, batch, fm_sum=plan.fm_sum)
+                K.embed_scatter_uniform_bwd(bplan, dx, dfm, dlin, sc, sc, batch, fm_sum=plan.fm_sum)
             elif dx is not None or dfm is not None or dlin is not None:
                 tgts = [self._target(s.emb.embeddings, opt) for s in fast_slots]
                 feats = [self._feature(s, feed, main.data, self.main_ld, table=tgt)
@@ -788,21 +845,18 @@ class EmbeddingPlanner(object):
                     lin_scale = max(abs(sc) for _, sc in lt) * (-1.0 if any(sc < 0 for _, sc in lt) else 1.0)
                 bplan = K.UniformPlan(feats, lin_tabs, None, main.data, None, None, plan.g.fm_mask[0])
                 bplan.g.x_cols = plan.g.x_cols
-                if getattr(self, "sorted_update", False) and all(sc < 0 for _, sc in tgts):
+                if self.sorted_update and all(sc < 0 for _, sc in tgts):
                     o = opt["optimizer"]
                     adagrad = o.name == "adagrad"
                     acc = lacc = None
                     if adagrad:
                         acc = [self._adagrad_state(s.emb.embeddings) for s in fast_slots]
                         lacc = [self._adagrad_state(s.emb.embeddings).reshape(-1) for s in self.lin] if lin_fused else None
-                    K.embed_update_sorted(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
-                                          None if dlin is None else dlin.reshape(-1).contiguous(),
-                                          1 if adagrad else 0, o.lr, o.lr, 1e-7, acc, lacc, batch)
-                    return self._backward_generic(feed, bufs, generic, opt, batch, shares)
-                K.embed_scatter_uniform_bwd(bplan, dx, None if dfm is None else dfm.reshape(-1).contiguous(),
-                                            None if dlin is None else dlin.reshape(-1).contiguous(),
-                                            scale, lin_scale, batch, fm_sum=plan.fm_sum)
-        self._backward_generic(feed, bufs, generic, opt, batch, shares)
+                    K.embed_update_sorted(bplan, dx, dfm, dlin, 1 if adagrad else 0, o.lr, o.lr, 1e-7, acc, lacc,
+                                          batch)
+                else:
+                    K.embed_scatter_uniform_bwd(bplan, dx, dfm, dlin, scale, lin_scale, batch, fm_sum=plan.fm_sum)
+        scatter_generic()
 
     @staticmethod
     def _adagrad_state(w):
@@ -812,70 +866,15 @@ class EmbeddingPlanner(object):
             K.fill(acc, 0.1)               # Keras initial_accumulator_value
         return acc
 
-    def _max_pool_shares(self, feed, bufs, generic, batch):
-        """Max-pooled bags whose table the fused SGD updates in place cannot re-find their arg-max in the scatter
-        that writes those rows: b2ctr_embed_max_pool_shares writes every position's share of the gradient at the
-        forward rows, and the scatter applies the shares as plain [B, T] lookups.  Returns (shares, {id(slot):
-        first column}), or None when no bag needs it."""
-        sel = []
-        for s in generic:
-            w = s.emb.embeddings
-            buf = bufs[id(s)] if s.buf == "seq" else bufs[s.buf]
-            if s.pool == L.POOL_MAX and w.trainable and w.sparse_grad and buf.grad is not None:
-                sel.append((s, buf.grad))
-        if not sel:
-            return None
-        cols, width = {}, 0
-        for s, _ in sel:
-            cols[id(s)] = width
-            width += s.maxlen * s.dim
-        shares = torch.empty((batch, (width + 3) // 4 * 4), dtype=torch.float32, device=sel[0][1].device)
-        K.embed_max_pool_shares([self._feature(s, feed, g, g.stride(0)) for s, g in sel], batch, shares)
-        return shares, cols
-
-    def _backward_generic(self, feed, bufs, generic, opt, batch, shares=None):
-        feats, scales = [], []
-        flat = {}            # (rows, scale) -> features of plain sequences re-described as B*T single lookups
-        for s in generic:
-            if not s.emb.embeddings.trainable:
-                continue
-            buf = bufs[id(s)] if s.buf == "seq" else bufs[s.buf]
-            if buf.grad is None:
-                continue
-            tgt, scale = _grad_target(s.emb.embeddings, opt)
-            ids = feed[s.input_name].data
-            if shares is not None and id(s) in shares[1]:
-                shard = s.emb.embeddings.opt_state.get("shard")
-                feats.append(K.make_feature(tgt, ids, shares[0], out_col=shares[1][id(s)], out_ld=shares[0].stride(0),
-                                            maxlen=s.maxlen, hash_mode=s.hash[0],
-                                            vocab=shard[2] if shard else s.emb.input_dim))
-                scales.append(scale)
-                continue
-            src = s.emb.embeddings.data if s.pool == L.POOL_MAX else None
-            g = buf.grad
-            if (s.buf == "seq" and s.maxlen > 1 and s.hash[0] == L.HASH_NONE and ids.dim() == 2 and ids.is_contiguous()
-                    and g.is_contiguous() and g.shape[1] == s.maxlen * s.dim):
-                # a [B, T] behaviour sequence scattered as B*T independent rows: one sub-warp per ROW instead of
-                # one per sample walking its T rows in sequence (8192 tasks x 50 dependent updates at C4)
-                shard = s.emb.embeddings.opt_state.get("shard")
-                f = K.make_feature(tgt, ids.reshape(-1), g.reshape(-1, s.dim), maxlen=1,
-                                   vocab=shard[2] if shard else s.emb.input_dim)
-                flat.setdefault((batch * s.maxlen, scale), []).append(f)
-                continue
-            feats.append(self._feature(s, feed, g, g.stride(0), table=tgt, src_table=src))
-            scales.append(scale)
-        # one launch per distinct scale (normally exactly one)
-        for sc in sorted(set(scales)):
-            K.embed_scatter_add([f for f, s_ in zip(feats, scales) if s_ == sc], batch, sc)
-        for (rows, sc), fs in flat.items():
-            K.embed_scatter_add(fs, rows, sc)
-
     # ---- fusion hooks used by layers ---------------------------------------------------------------
+    def _is_main(self, base):
+        """Whether ``base`` is this step's main gather buffer."""
+        return (base is not None and base.owner is self and base.data is not None and base.ncols == self.main_width
+                and base.data.shape[1] == self.main_ld)
+
     def lookup_fm(self, x):
         """FM layer: return the in-kernel FM if this step computed it for exactly this window."""
-        if x.base is None or x.base.owner is not self or x.ncols == -1:
-            return None
-        if x.base.ncols != self.main_width or x.base.data is None or x.base.data.shape[1] != self.main_ld:
+        if x.ncols == -1 or not self._is_main(x.base):
             return None
         key = (x.col0, x.ncols)
         if self.fm_result is not None and self.fm_result[0] == key:
@@ -904,8 +903,8 @@ class EmbeddingPlanner(object):
             if x.col0 == 0 and x.ncols == self.lin_width and self.lin_result is not None:
                 return self.lin_result
             raise L.B2ctrError("the linear-term lookups were fused into a row-sum but a layer asked for the rows")
-        if (self.fast and x.base.ncols == self.lin_width and x.col0 == 0 and x.ncols == self.lin_width
-                and x.base.data.shape[1] == self.lin_ld and self._lin_matches_fast()):
+        if (self.lin_matches_fast and x.base.ncols == self.lin_width and x.col0 == 0 and x.ncols == self.lin_width
+                and x.base.data.shape[1] == self.lin_ld):
             self.lin_hint = True
         return None
 
@@ -915,9 +914,7 @@ class EmbeddingPlanner(object):
         from . import ops
         if emb_flat.base is not None and isinstance(emb_flat.base.owner, DnnInputPlacement):
             return emb_flat.base.owner.append_dense(emb_flat, dense_flat)
-        if (emb_flat.base is None or emb_flat.base.owner is not self or emb_flat.ncols == -1
-                or emb_flat.base.ncols != self.main_width or emb_flat.base.data is None
-                or emb_flat.base.data.shape[1] != self.main_ld):
+        if emb_flat.ncols == -1 or not self._is_main(emb_flat.base):
             return None
         width = self.main_width + self.pnn_cols if self.pnn_cols else self.main_width
         if emb_flat.col0 != 0 or emb_flat.ncols != width:
@@ -972,8 +969,7 @@ class EmbeddingPlanner(object):
         from . import ops
         x = values[id(node.inputs)]
         base = x.base
-        if (base is None or base.owner is not self or base.data is None
-                or base.ncols != self.main_width or base.data.shape[1] != self.main_ld):
+        if not self._is_main(base):
             return {}
         P = self.fefm_places[id(node.layer)]
         out = ops._window(base, self.main_width + self.tail_reserve, P, (base.data.shape[0], P))
@@ -989,9 +985,7 @@ class EmbeddingPlanner(object):
         from .layers.interaction import _product_operand
         x = _product_operand(E._concrete([values[id(t)] for t in node.inputs]))
         base, out = x.base, None
-        if (base is not None and base.owner is self and base.data is not None and x.ncols != -1 and x.col0 == 0
-                and x.ncols == self.main_width and base.ncols == self.main_width
-                and base.data.shape[1] == self.main_ld):
+        if self._is_main(base) and x.ncols != -1 and x.col0 == 0 and x.ncols == self.main_width:
             b, f, _ = x.data.shape
             P = f * (f - 1) // 2
             out = ops._window(base, self.main_width + self.pnn_places[id(node.layer)], P, (b, P))
@@ -1366,19 +1360,21 @@ class FieldAwarePlan(object):
     """ONN's field-aware products (deepctr/models/onn.py:79-97) served by one b2ctr_ffm_product_fwd launch: the
     output of pair p's ``multiply`` (or of the ``K.sum`` Lambda behind it) is the column window [p*E, (p+1)*E) (or
     [p, p+1)) of one [B, P*E] (or [B, P]) buffer, so concat_func + Flatten of the P outputs is a zero-copy view of
-    it.  The backward is one tape node on that buffer: b2ctr_ffm_product_bwd writes every lookup's gradient row
-    into a [B, F(F-1)*E] scratch at the tables' pre-step values, then b2ctr_embed_scatter_add applies the scratch,
-    one single-valued or pooled feature per lookup, to the tables (fused SGD) or their dense gradients.
+    it.  The launch runs where the graph executor reaches the first pair node.  The backward is one tape node on
+    that buffer: b2ctr_ffm_product_bwd writes every lookup's gradient row into a [B, F(F-1)*E] scratch at the
+    tables' pre-step values, then the generic update (_generic_update) applies the scratch, one single-valued or
+    pooled feature per lookup, to the tables (fused SGD) or their dense gradients.
 
     A VarLenSparseFeat field is pooled per partner by the generic gather into a [B, (F-1)*E] operand that the
     product kernel reads; its gradient rows go back through the same scatter's pooling Jacobian.
 
     ``fields[a]``: (input name, maxlen, pool, hash mode, vocabulary); ``tables[a*F + b]``: (a, b) -> Embedding layer
     (None on the diagonal); ``pair_nodes[p]``: the node whose output pair p's window is; ``virtual``: every other
-    node the plan replaces."""
+    node the plan replaces; ``inputs[a]``: the model input field a's ids come from (only the launch reads them, so a
+    plan built just to check its tables may leave them out)."""
 
-    def __init__(self, fields, tables, E_, reduce_sum, pair_nodes, virtual, claimed):
-        self.fields, self.E, self.reduce_sum = fields, E_, reduce_sum
+    def __init__(self, fields, tables, E_, reduce_sum, pair_nodes, virtual, claimed, inputs=()):
+        self.fields, self.inputs, self.E, self.reduce_sum = fields, inputs, E_, reduce_sum
         self.F = len(fields)
         self.table_of = tables
         self.tables = [(k, t) for k, t in enumerate(tables) if t is not None]
@@ -1416,110 +1412,64 @@ class FieldAwarePlan(object):
             self._ptrs = ptrs
         return self._dev_ptrs
 
-    def _bag_features(self, a, feed, buf, tables=None, scale_of=None):
-        """The generic-gather features of pooled field a: one bag per partner, at its slot of ``buf``."""
-        name, maxlen, pool, hash_mode, vocab = self.fields[a]
-        ids = feed[name].data
-        out = []
-        for b in range(self.F):
-            if b == a:
-                continue
-            emb = self.table_of[a * self.F + b].embeddings
-            tab = emb.materialize() if tables is None or tables[a * self.F + b] is None else tables[a * self.F + b]
-            col = self._slot(a, b) * self.E if tables is None else (a * (self.F - 1) + self._slot(a, b)) * self.E
-            out.append(K.make_feature(tab, ids, buf, out_col=col, out_ld=buf.stride(0), maxlen=maxlen, pool=pool,
-                                      mask_mode=L.MASK_ZERO_ID, hash_mode=hash_mode, vocab=vocab,
-                                      src_table=emb.data if (tables is not None and pool == L.POOL_MAX) else None))
-        return out
+    def _lookup_features(self, a, ids, buf):
+        """The generic features of field a's lookups, one per partner at its slot of ``buf``."""
+        _, maxlen, pool, hash_mode, vocab = self.fields[a]
+        return [K.make_feature(self.table_of[a * self.F + c].embeddings.materialize(), ids, buf,
+                               out_col=self._slot(a, c) * self.E, out_ld=buf.stride(0), maxlen=maxlen, pool=pool,
+                               mask_mode=L.MASK_NONE if pool == L.POOL_NONE else L.MASK_ZERO_ID,
+                               hash_mode=hash_mode, vocab=vocab)
+                for c in range(self.F) if c != a]
 
-    def forward(self, feed, results, grad):
+    def launches(self):
+        return {id(self.pair_nodes[0]): self._launch}
+
+    def _launch(self, values, training):
         F, E_ = self.F, self.E
-        some = feed[self.fields[0][0]].data
-        b, dev = some.shape[0], some.device
+        ids = [values[id(t)].data for t in self.inputs]
+        b, dev = ids[0].shape[0], ids[0].device
         ptrs = self._table_array(dev)
         pooled, kfields = {}, []
         bags = []
         for a, (name, maxlen, pool, hash_mode, vocab) in enumerate(self.fields):
             if pool == L.POOL_NONE:
-                kfields.append(K.ffm_field(idx=feed[name].data.reshape(b, -1), vocab=vocab, hash_mode=hash_mode))
+                kfields.append(K.ffm_field(idx=ids[a].reshape(b, -1), vocab=vocab, hash_mode=hash_mode))
             else:
                 pooled[a] = torch.empty((b, (F - 1) * E_), dtype=torch.float32, device=dev)
-                bags.extend(self._bag_features(a, feed, pooled[a]))
+                bags.extend(self._lookup_features(a, ids[a], pooled[a]))
                 kfields.append(K.ffm_field(pooled=pooled[a]))
-        for c in range(0, len(bags), L.MAX_FEATURES):
-            K.embed_gather_fwd(bags[c:c + L.MAX_FEATURES], b)
+        if bags:
+            K.embed_gather_fwd(bags, b)
         buf = E.Var(torch.empty((b, self.ld), dtype=torch.float32, device=dev), ncols=self.width, owner=self,
                     name="__ffm_products__")
         K.ffm_product_fwd(kfields, ptrs, E_, self.reduce_sum, buf.data, 0, b)
         trainable = any(t.embeddings.trainable for _, t in self.tables)
-        buf.requires_grad = grad and trainable
+        buf.requires_grad = training and E.current_tape() is not None and trainable
         w = 1 if self.reduce_sum else E_
-        for p, node in enumerate(self.pair_nodes):
-            results[id(node)] = ops_window(buf, p * w, w, (b, 1) if self.reduce_sum else (b, 1, E_))
-        for node in self.virtual:
-            results[id(node)] = VIRTUAL
+        out = {id(node): ops_window(buf, p * w, w, (b, 1) if self.reduce_sum else (b, 1, E_))
+               for p, node in enumerate(self.pair_nodes)}
         if buf.requires_grad:
-            E.current_tape().record([buf], lambda grads: self._backward(feed, buf, pooled, b))
+            E.current_tape().record([buf], lambda grads: self._backward(ids, buf, pooled, b))
+        return out
 
-    def _backward(self, feed, buf, pooled, b):
+    def _backward(self, ids, buf, pooled, b):
         g = buf.grad
         if g is None:
             return
         F, E_ = self.F, self.E
-        opt = E.current_opt()
         ptrs = self._table_array(g.device)
         scratch = torch.empty((b, F * (F - 1) * E_), dtype=torch.float32, device=g.device)
-        kfields = []
+        kfields, feats = [], []
         for a, (name, maxlen, pool, hash_mode, vocab) in enumerate(self.fields):
             gv = scratch[:, a * (F - 1) * E_:]
             if pool == L.POOL_NONE:
-                kfields.append(K.ffm_field(idx=feed[name].data.reshape(b, -1), vocab=vocab, hash_mode=hash_mode,
-                                           grad=gv))
+                kfields.append(K.ffm_field(idx=ids[a].reshape(b, -1), vocab=vocab, hash_mode=hash_mode, grad=gv))
             else:
                 kfields.append(K.ffm_field(pooled=pooled[a], grad=gv))
+            feats += self._lookup_features(a, ids[a], gv)
         K.ffm_product_bwd(kfields, ptrs, E_, self.reduce_sum, g, 0, b)
-        # every lookup's row of the scratch, applied to its table: one feature each, grouped by update scale
-        targets = [None] * (F * F)
-        for k, t in self.tables:
-            if t.embeddings.trainable:
-                targets[k] = _grad_target(t.embeddings, opt)
-        groups = defaultdict(list)
-        inplace = []          # max-pooled bags updated in place: (field, partner, bag feature)
-        for a, (name, maxlen, pool, hash_mode, vocab) in enumerate(self.fields):
-            tabs = [tg[0] if tg is not None else None for tg in targets]
-            if pool == L.POOL_NONE:
-                ids = feed[name].data.reshape(b, -1)
-                for c in range(F):
-                    if c == a or targets[a * F + c] is None:
-                        continue
-                    f = K.make_feature(tabs[a * F + c], ids, scratch, out_col=(a * (F - 1) + self._slot(a, c)) * E_,
-                                       out_ld=scratch.stride(0), hash_mode=hash_mode, vocab=vocab)
-                    groups[targets[a * F + c][1]].append(f)
-            else:
-                keep = [c for c in range(F) if c != a]
-                for c, f in zip(keep, self._bag_features(a, feed, scratch, tables=tabs)):
-                    if targets[a * F + c] is None:
-                        continue
-                    if pool == L.POOL_MAX and self.table_of[a * F + c].embeddings.sparse_grad:
-                        inplace.append((a, c, f))
-                    else:
-                        groups[targets[a * F + c][1]].append(f)
-        if inplace:
-            # the bag features read their forward rows from `table` (the live table): shares first, then plain
-            # lookups of them (b2ctr_embed_scatter_add refuses a max-pooled feature that updates its own rows)
-            width = sum(self.fields[a][1] * E_ for a, _, _ in inplace)
-            shares = torch.empty((b, (width + 3) // 4 * 4), dtype=torch.float32, device=g.device)
-            K.embed_max_pool_shares([f for _, _, f in inplace], b, shares)
-            col = 0
-            for a, c, _ in inplace:
-                name, maxlen, pool, hash_mode, vocab = self.fields[a]
-                f = K.make_feature(targets[a * F + c][0], feed[name].data, shares, out_col=col,
-                                   out_ld=shares.stride(0), maxlen=maxlen, hash_mode=hash_mode, vocab=vocab)
-                groups[targets[a * F + c][1]].append(f)
-                col += maxlen * E_
-        for sc, feats in sorted(groups.items()):
-            for c in range(0, len(feats), L.MAX_FEATURES):
-                K.embed_scatter_add(feats[c:c + L.MAX_FEATURES], b, sc)
+        weights = [self.table_of[a * F + c].embeddings for a in range(F) for c in range(F) if c != a]
+        _generic_update(feats, weights, b, E.current_opt())()
 
 
 def ops_window(base, col0, ncols, shape):
@@ -1540,6 +1490,8 @@ def _plan_field_aware(g):
     plans nothing and each layer runs as itself."""
     from .layers.sequence import SequencePoolingLayer
     from .layers.utils import Hash, NoMask
+
+    inputs = {}          # input name -> the model input
 
     def lookup(t):
         if not g.only_use(t) or g.calls[id(t.node.layer)] != 1 or not isinstance(t.node.inputs, E.KTensor):
@@ -1573,6 +1525,7 @@ def _plan_field_aware(g):
         maxlen = int(np.prod(src.shape[1:])) if len(src.shape) > 1 else 1
         if (pool == L.POOL_NONE) != (maxlen == 1):
             return None
+        inputs[name] = src
         return (name, maxlen, pool, hash_mode, emb.input_dim), emb, virt
 
     pairs = []
@@ -1616,7 +1569,8 @@ def _plan_field_aware(g):
         claimed.update(id(n) for n in vi + vj if isinstance(n.layer, Embedding))
     if len(set(id(t) for t in tables if t is not None)) != F * (F - 1):
         return None
-    return FieldAwarePlan(fields, tables, E_, pairs[0][3], pair_nodes, virtual, claimed)
+    return FieldAwarePlan(fields, tables, E_, pairs[0][3], pair_nodes, virtual, claimed,
+                          [inputs[fd[0]] for fd in fields])
 
 
 # ================================================================================================
@@ -1657,6 +1611,7 @@ class Feeder(object):
         self._pinned = {}
         self._carrays = {}
         self._plan = None
+        self.slot = -1             # the staging-ring slot of the batch fed last (-1: none yet)
         self._views = {}
         self._copied_ev = {}
         self._consumed_ev = {}
@@ -1682,7 +1637,7 @@ class Feeder(object):
     #   consumed[slot] - recorded by the model on the compute stream after the step that read the device side;
     #                    the staging stream waits on it before the next H2D into that slot
     def _next_slot(self):
-        self.slot = (getattr(self, "slot", -1) + 1) % self._RING
+        self.slot = (self.slot + 1) % self._RING
         ev = self._copied_ev.get(self.slot)
         if ev is not None:
             ev.synchronize()
@@ -1751,7 +1706,7 @@ class Feeder(object):
     # only have their array pointers collected (~2 us per input) before the native pack + the H2D copies: the
     # per-step Python cost of the input pipeline must stay well under the ~1.2 ms training step it feeds.
     def _feed_fast(self, xd):
-        plan = getattr(self, "_plan", None)
+        plan = self._plan
         if plan is None:
             return None
         b = -1
@@ -1768,7 +1723,7 @@ class Feeder(object):
                     return None
                 col.append(a.__array_interface__["data"][0])
             ptrs[key] = col
-        slot = (getattr(self, "slot", -1) + 1) % self._RING
+        slot = (self.slot + 1) % self._RING
         for key, np_dt, items, names in plan:          # every view of the slot this batch will land in must exist
             if (slot, key, b, names) not in self._views:
                 return None
@@ -1943,7 +1898,7 @@ class Feeder(object):
         if isinstance(y, torch.Tensor) and y.is_cuda:
             return y.reshape(-1).float()
         a = np.asarray(y, dtype=np.float32).reshape(-1)
-        if not hasattr(self, "slot"):
+        if self.slot < 0:
             self._next_slot()
         stage, dbuf = self._stage("labels", (a.shape[0],), torch.float32)
         stage.numpy()[:] = a

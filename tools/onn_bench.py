@@ -32,7 +32,7 @@ CFG = dict(bench.CONFIGS["c2"], dim=4, workload="ONN synthetic Criteo: 26 fields
 
 def kernels(reps):
     import torch
-    from deepctr_b200 import kernels as K, _lib as L
+    from deepctr_b200 import kernels as K
     B, F, E, V = CFG["batch"], CFG["n_sparse"], CFG["dim"], CFG["vocab"]
     P = F * (F - 1) // 2
     dev = torch.device("cuda", 0)
@@ -75,10 +75,7 @@ def kernels(reps):
                 feats.append(K.make_feature(tables[a * F + b], ids[a], scratch, out_col=(a * (F - 1) + s) * E,
                                             out_ld=scratch.stride(0), vocab=V))
 
-    def scatter():
-        for c in range(0, len(feats), L.MAX_FEATURES):
-            K.embed_scatter_add(feats[c:c + L.MAX_FEATURES], B, -1e-6)
-    ms = float(np.median(kernel_ms(scatter, reps)))
+    ms = float(np.median(kernel_ms(lambda: K.embed_scatter_add(feats, B, -1e-6), reps)))
     # reads the scratch and the ids, read-modify-writes 650 rows (each a 32 B sector) per sample
     alg = B * (2 * P * row + 2 * P * idb + 2 * 2 * P * row)
     out.append({"what": "kernel", "kernel": "embed_scatter_add (ONN scratch, fused SGD)", "batch": B,
