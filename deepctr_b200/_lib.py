@@ -175,6 +175,12 @@ SIGNATURES = {
     "b2ctr_gemm": (_i32, [C.POINTER(Gemm), _vp, _sz, _vp]),
     "b2ctr_planes_bytes": (_sz, [_i64, _i64]),
     "b2ctr_split_planes": (_i32, [_vp, _i64, _i64, _i64, _vp, _vp]),
+    "b2ctr_mlp_relu_supported": (_i32, [C.POINTER(_i32), _i32]),
+    "b2ctr_mlp_relu_fwd": (_i32, [_vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _vp, C.POINTER(_i32), _i32,
+                                  _i64, _vp]),
+    "b2ctr_mlp_relu_bwd_workspace_bytes": (_sz, [C.POINTER(_i32), _i32]),
+    "b2ctr_mlp_relu_bwd": (_i32, [_vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp),
+                                  C.POINTER(_i32), _i32, _i64, _vp, _sz, _vp]),
     "b2ctr_bias_act_bwd_workspace_bytes": (_sz, [_i64, _i64]),
     "b2ctr_bias_act_bwd": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _sz, _vp]),
     "b2ctr_bias_act_bwd_planes": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _sz, _vp]),

@@ -357,6 +357,50 @@ def bias_act_bwd(dy, y, act, want_dz=True, want_dbias=True, m=None, n=None, want
     return dz, dbias
 
 
+# ---- fused relu tower (hidden layers 1..L-1 of a DNN) -----------------------------------------
+def _widths(widths):
+    return (C.c_int32 * len(widths))(*widths), len(widths)
+
+
+def _ptrs(ts):
+    return (C.c_void_p * len(ts))(*[t.data_ptr() if t is not None else None for t in ts])
+
+
+def _planes(rows, cols, device):
+    return torch.empty((L.lib().b2ctr_planes_bytes(rows, cols),), dtype=torch.uint8, device=device)
+
+
+@_timed
+def mlp_relu_fwd(y0, ws, bs):
+    """y_i = relu(y_{i-1} W_i + b_i) for the layers after y0 [B, n0] (b2ctr_mlp_relu_fwd).  Returns the planes of
+    y_0 .. y_{L-2} and y_{L-1}."""
+    _require_cuda(y0, *ws, *bs)
+    widths = [y0.shape[1]] + [w.shape[1] for w in ws]
+    m = y0.shape[0]
+    planes = [_planes(m, n, y0.device) for n in widths[:-1]]
+    y = torch.empty((m, widths[-1]), dtype=torch.float32, device=y0.device)
+    L.check(L.lib().b2ctr_mlp_relu_fwd(ptr(y0.contiguous()), _ptrs(ws), _ptrs(bs), _ptrs(planes), ptr(y),
+                                       *_widths(widths), m, stream()), "mlp_relu_fwd")
+    return planes, y
+
+
+@_timed
+def mlp_relu_bwd(dy, y, y0, planes, ws):
+    """The backward of mlp_relu_fwd from dy = d y_{L-1} (b2ctr_mlp_relu_bwd): the planes of dz_0 .. dz_{L-1} and
+    the bias gradients db_0 .. db_{L-1}."""
+    _require_cuda(dy, y, y0, *ws)
+    widths = [y0.shape[1]] + [w.shape[1] for w in ws]
+    m = y0.shape[0]
+    dzp = [_planes(m, n, y0.device) for n in widths]
+    db = [torch.empty((n,), dtype=torch.float32, device=y0.device) for n in widths]
+    wid = _widths(widths)
+    nbytes = L.lib().b2ctr_mlp_relu_bwd_workspace_bytes(*wid)
+    wsp = workspace(nbytes, y0.device)
+    L.check(L.lib().b2ctr_mlp_relu_bwd(ptr(dy.contiguous()), ptr(y), ptr(y0), _ptrs(planes), _ptrs(ws), _ptrs(dzp),
+                                       _ptrs(db), *wid, m, ptr(wsp), nbytes, stream()), "mlp_relu_bwd")
+    return dzp, db
+
+
 @_timed
 def act_fwd(x, act, out=None):
     _require_cuda(x)

@@ -61,6 +61,11 @@ class DNN(Layer):
         """``first(kernel, bias, activation)``: an alternative implementation of layer 0's  act(x W + b)  for a
         caller that never materialises x (the DIN attention unit generates it inside the GEMM)."""
         deep_input = inputs
+        if (first is None and not self.use_bn and not (self.dropout_rate and training)
+                and all(a == 'relu' for a in self.act_names)
+                and ops.mlp_fusable(inputs, [int(u) for u in self.hidden_units])):
+            # the whole relu tower as one tape node: layer 0's GEMM, then fused kernels for the layers after it
+            return ops.mlp(inputs, self.kernels, self.bias)
         for i in range(len(self.hidden_units)):
             act_layer = self.activation_layers[i]
             dense = first if (i == 0 and first is not None) else \

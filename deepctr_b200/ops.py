@@ -1,6 +1,8 @@
 """Differentiable ops on ``engine.Var``: each launches libb2ctr kernels for the forward and pushes a
 closure on the active tape that launches the backward kernels.  No torch arithmetic anywhere.
 """
+import ctypes
+
 import numpy as np
 import torch
 
@@ -74,22 +76,63 @@ def _planes_of(var, t2):
     return var.planes[1]
 
 
+class _Layer(object):
+    """What the backward of one act(x @ w + b) GEMM layer needs: the operands, their planes and the precision."""
+    __slots__ = ("x2", "m", "kdim", "n", "wd", "prec", "reuse", "xp", "wp")
+
+
+def _dense_fwd(x, w, b, act):
+    """act(x @ w + b) over the last axis of x as one GEMM, bias and activation in its epilogue; returns (y [m, n],
+    the _Layer its backward reads)."""
+    st = _Layer()
+    st.x2, _ = _as2d(x)
+    st.m, st.kdim = st.x2.shape
+    st.n = w.shape[1]
+    st.wd = w.materialize() if isinstance(w, E.Weight) else w.data
+    bd = (b.materialize() if isinstance(b, E.Weight) else b.data) if b is not None else None
+    # BF16X3: operands are split into bf16 planes once and the planes are reused by forward/dgrad/wgrad
+    # skinny layers (the final [*, 1] projection) are GEMVs: exact-fp32 FFMA path, no tensor-core staging
+    st.prec = GEMM_PRECISION if min(st.n, st.kdim) >= 16 else L.GEMM_FP32
+    st.reuse = st.prec == L.GEMM_BF16X3 and st.m >= 128
+    st.xp = _planes_of(x, st.x2) if st.reuse else None
+    st.wp = K.split_planes(st.wd) if st.reuse else None
+    y = K.gemm(st.x2, st.wd, bias=bd, act=act, precision=st.prec, m=st.m, n=st.n, k=st.kdim, a_planes=st.xp,
+               b_planes=st.wp)
+    return y, st
+
+
+def _dense_grads(x, w, st, dz, dzp):
+    """dx = dz w^T and dw = x^T dz of a _dense_fwd layer, added to x's and w's gradients.  dz may be None when its
+    planes dzp are given."""
+    m, kdim, n, prec = st.m, st.kdim, st.n, st.prec
+    if x.requires_grad:
+        base = x.base
+        if (base is not None and x.col0 == 0 and x.ncols != -1 and base.data.dim() == 2
+                and base.data.shape[0] == m and x.ncols == kdim):
+            # x is the leading window of a K-padded buffer: write dx with the same ld so that
+            # the buffer's gradient is adopted without a copy
+            ld = base.data.stride(0)
+            buf = _empty((m, ld), base.data)
+            dxw = buf[:, :kdim]
+            K.gemm(dz, st.wd, c=dxw, trans_b=True, precision=prec, m=m, n=kdim, k=n, a_planes=dzp,
+                   b_planes=st.wp)
+            E.add_grad(x, dxw)
+        else:
+            dx = K.gemm(dz, st.wd, trans_b=True, precision=prec, m=m, n=kdim, k=n, a_planes=dzp,
+                        b_planes=st.wp)
+            E.add_grad(x, dx.reshape(x.data.shape))
+    if w.requires_grad:
+        dw = K.gemm(st.x2, dz, trans_a=True, precision=prec, split_k=_split_k(kdim, n, m),
+                    m=kdim, n=n, k=m, a_planes=st.xp, b_planes=dzp)
+        E.add_grad(w, dw)
+
+
 def dense(x, w, b=None, activation=None):
     """y = act(x @ w + b) over the last axis (tf.tensordot(x, w, axes=(-1, 0)) + bias_add)."""
     act = L.ACT_BY_NAME.get(activation, None)
     fused_act = act if act is not None else L.ACT_NONE
-    x2, _ = _as2d(x)
-    m, kdim = x2.shape
-    n = w.shape[1]
-    wd = w.materialize() if isinstance(w, E.Weight) else w.data
-    bd = (b.materialize() if isinstance(b, E.Weight) else b.data) if b is not None else None
-    # BF16X3: operands are split into bf16 planes once and the planes are reused by forward/dgrad/wgrad
-    # skinny layers (the final [*, 1] projection) are GEMVs: exact-fp32 FFMA path, no tensor-core staging
-    prec = GEMM_PRECISION if min(n, kdim) >= 16 else L.GEMM_FP32
-    reuse = prec == L.GEMM_BF16X3 and m >= 128
-    xp = _planes_of(x, x2) if reuse else None
-    wp = K.split_planes(wd) if reuse else None
-    y = K.gemm(x2, wd, bias=bd, act=fused_act, precision=prec, m=m, n=n, k=kdim, a_planes=xp, b_planes=wp)
+    y, st = _dense_fwd(x, w, b, fused_act)
+    m, n = st.m, st.n
     out = E.Var(y.reshape(tuple(x.data.shape[:-1]) + (n,)))
     if act is None and activation is not None:
         raise ValueError("activation %r cannot be fused into dense(); apply it as a layer" % activation)
@@ -99,7 +142,7 @@ def dense(x, w, b=None, activation=None):
         if not dy.is_contiguous():
             dy = dy.contiguous()
         need_db = b is not None and b.requires_grad
-        need_planes = reuse and (x.requires_grad or w.requires_grad)
+        need_planes = st.reuse and (x.requires_grad or w.requires_grad)
         dzp = None
         if fused_act != L.ACT_NONE or need_db:
             if need_planes and fused_act != L.ACT_NONE and dy.stride(0) % 4 == 0 and K.planes_fusable(m, n):
@@ -113,30 +156,48 @@ def dense(x, w, b=None, activation=None):
             dz, db = dy, None
         if need_planes and dzp is None:
             dzp = K.split_planes(dz)
-        if x.requires_grad:
-            base = x.base
-            if (base is not None and x.col0 == 0 and x.ncols != -1 and base.data.dim() == 2
-                    and base.data.shape[0] == m and x.ncols == kdim):
-                # x is the leading window of a K-padded buffer: write dx with the same ld so that
-                # the buffer's gradient is adopted without a copy
-                ld = base.data.stride(0)
-                buf = _empty((m, ld), dy)
-                dxw = buf[:, :kdim]
-                K.gemm(dz, wd, c=dxw, trans_b=True, precision=prec, m=m, n=kdim, k=n, a_planes=dzp,
-                       b_planes=wp)
-                E.add_grad(x, dxw)
-            else:
-                dx = K.gemm(dz, wd, trans_b=True, precision=prec, m=m, n=kdim, k=n, a_planes=dzp,
-                            b_planes=wp)
-                E.add_grad(x, dx.reshape(x.data.shape))
-        if w.requires_grad:
-            dw = K.gemm(x2, dz, trans_a=True, precision=prec, split_k=_split_k(kdim, n, m),
-                        m=kdim, n=n, k=m, a_planes=xp, b_planes=dzp)
-            E.add_grad(w, dw)
+        _dense_grads(x, w, st, dz, dzp)
         if need_db:
             E.add_grad(b, db)
 
     E.record([out], [x, w, b], bwd)
+    return out
+
+
+def mlp_fusable(x, widths):
+    """ops.mlp runs this relu tower: split-bf16 GEMMs, layer 0 on operand planes (at least 128 rows, both of its
+    dimensions at least 16) and fused kernels for the widths after it."""
+    m = int(np.prod(x.data.shape[:-1]))
+    return (GEMM_PRECISION == L.GEMM_BF16X3 and len(widths) >= 2 and m >= 128 and x.data.shape[-1] >= 16
+            and widths[0] >= 16 and L.lib().b2ctr_mlp_relu_supported((ctypes.c_int32 * len(widths))(*widths),
+                                                                     len(widths)) == 1)
+
+
+def mlp(x, kernels, biases):
+    """A relu DNN tower, y_i = relu(y_{i-1} W_i + b_i), as one tape node (mlp_fusable must hold): layer 0 is
+    dense()'s GEMM, the layers after it one fused forward kernel; the backward runs one fused kernel for every
+    layer's bias and activation gradient, then the split-K weight-gradient GEMMs on the planes it wrote and
+    layer 0's dgrad."""
+    y0, st = _dense_fwd(x, kernels[0], biases[0], L.ACT_RELU)
+    ws = [w.materialize() if isinstance(w, E.Weight) else w.data for w in kernels[1:]]
+    bs = [b.materialize() if isinstance(b, E.Weight) else b.data for b in biases[1:]]
+    planes, y = K.mlp_relu_fwd(y0, ws, bs)
+    out = E.Var(y.reshape(tuple(x.data.shape[:-1]) + (y.shape[1],)))
+
+    def bwd(grads):
+        dzp, db = K.mlp_relu_bwd(grads[0].reshape(y.shape), y, y0, planes, ws)
+        _dense_grads(x, kernels[0], st, None, dzp[0])
+        m = st.m
+        for i in range(1, len(kernels)):
+            if kernels[i].requires_grad:
+                kdim, n = ws[i - 1].shape
+                dw = K.gemm(None, None, trans_a=True, precision=L.GEMM_BF16X3, split_k=_split_k(kdim, n, m),
+                            m=kdim, n=n, k=m, a_planes=planes[i - 1], b_planes=dzp[i])
+                E.add_grad(kernels[i], dw)
+        for bias, g in zip(biases, db):
+            E.add_grad(bias, g)
+
+    E.record([out], [x] + list(kernels) + list(biases), bwd)
     return out
 
 

@@ -309,6 +309,26 @@ B2CTR_API size_t b2ctr_gemm_workspace_bytes(const b2ctr_gemm_t* g);
 B2CTR_API b2ctr_status_t b2ctr_gemm(const b2ctr_gemm_t* g, void* workspace, size_t workspace_bytes,
                                    void* stream);
 
+/* A relu DNN tower's hidden layers after the first, fused.  widths[0..nlayers-1] are the widths of hidden layers
+ * 0..L-1 (L = nlayers); y_i = relu(y_{i-1} W_i + b_i) for i = 1..L-1 in split-bf16 (hi*hi + hi*lo + lo*hi, fp32
+ * accumulation), W_i = w[i-1] [widths[i-1], widths[i]] row-major, b_i = b[i-1].  All activations and gradients are
+ * contiguous [batch, width] fp32.  b2ctr_mlp_relu_supported says whether a tower is supported (1) or not (0); the
+ * other calls return B2CTR_ERR_INVALID_ARG for an unsupported one.
+ * Forward: reads y0, writes planes[i] = b2ctr_split_planes of y_i for i = 0..L-2 (b2ctr_planes_bytes(batch,
+ * widths[i]) bytes each) and y_last = y_{L-1}.
+ * Backward: dy_last is the gradient of y_last; dz_{L-1} = dy_last * [y_last > 0], dz_{i-1} = (dz_i W_i^T) * [y_{i-1} > 0]
+ * (y_0's mask from y0, the inner layers' from the forward's planes).  Writes dz_planes[i] = b2ctr_split_planes of dz_i
+ * and dbias[i] = column sums of dz_i (per-CTA partials reduced in a fixed order: deterministic), i = 0..L-1. */
+B2CTR_API int32_t b2ctr_mlp_relu_supported(const int32_t* widths, int32_t nlayers);
+B2CTR_API b2ctr_status_t b2ctr_mlp_relu_fwd(const float* y0, const float* const* w, const float* const* b,
+                                           void* const* planes, float* y_last, const int32_t* widths,
+                                           int32_t nlayers, int64_t batch, void* stream);
+B2CTR_API size_t b2ctr_mlp_relu_bwd_workspace_bytes(const int32_t* widths, int32_t nlayers);
+B2CTR_API b2ctr_status_t b2ctr_mlp_relu_bwd(const float* dy_last, const float* y_last, const float* y0,
+                                           void* const* planes, const float* const* w, void* const* dz_planes,
+                                           float* const* dbias, const int32_t* widths, int32_t nlayers,
+                                           int64_t batch, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* 3. Elementwise / reductions                                                                 */
 /* ------------------------------------------------------------------------------------------ */
